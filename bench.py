@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- clouds/s of the PointNet++ (SSG) point-set-abstraction forward on B200.
+"""bench.py -- clouds/s of the PointNet++ (SSG) point-set-abstraction forward on H100.
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One "step" = one inference forward of pointnet2_cls_ssg (FPS -> fused ball-query/group/MLP/max-pool x2 ->
 group-all MLP -> FC head, BN in moving-average mode) over one batch of B=32 synthetic clouds of N=2048 points
@@ -47,7 +47,7 @@ def _peaks():
         with open(p) as f:
             d = json.load(f)
         return dict(hbm=d["hbm_gbs"], tf=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf=1590.0, tf_sus=1400.0, src="fallback")
+    return dict(hbm=3350.0, tf=989.0, tf_sus=989.0, src="H100 SXM data sheet (dense BF16, 700 W)")
 
 
 class ClockSampler:
@@ -271,7 +271,7 @@ def run_sweep(dev, peaks):
 
 
 def run_ref_gpu(dev, x, l1_xyz, l2_xyz, l1_pts_shape_c=128):
-    """R-GPU contender (SURVEY 8d): the reference's own CUDA kernels, compiled unmodified for sm_100a by oracle/Makefile into
+    """R-GPU contender (SURVEY 8d): the reference's own CUDA kernels, compiled unmodified for sm_90a by oracle/Makefile into
     oracle/_ref/libref_tfops.so, timed on the same tensors in the same run.  Reported baseline only (like cpu_baseline)."""
     import ctypes as C
 
@@ -330,14 +330,18 @@ def main():
     ap.add_argument("--warmup", type=int, default=8)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
-    ap.add_argument("--streams", type=int, default=6, help="batches kept in flight (1 = strictly one step at a time; measured 4: 93.9 k, 6: 95.8 k, 8: 95.4 k clouds/s)")
+    ap.add_argument("--streams", type=int, default=6, help="batches kept in flight (1 = strictly one step at a time)")
     ap.add_argument("--no-extra", action="store_true", help="skip the BGA / DGCNN / single-op / sweep measurements")
     ap.add_argument("--no-train", action="store_true", help="skip the training-step measurement")
     ap.add_argument("--train-steps", type=int, default=20)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the logits of the last timed step to DIR/logits.npy (float32)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs writes the outputs of the CUDA path; --impl reference times the CPU arm only")
         return run_reference(args)
 
     import numpy as np
@@ -360,7 +364,7 @@ def main():
     solo = world == 1  # the side measurements (per-kernel times, other models, sweep, CPU arm) run on the single-GPU line only
 
     params = pointnet2_cls_ssg.init_params(seed=1, device=dev, randomize_bn=True)
-    # input pool larger than L2 (126 MB): 192 distinct batches x 786 KB = 151 MB, rotated every step
+    # input pool larger than L2 (50 MB on the H100): 192 distinct batches x 786 KB = 151 MB, rotated every step
     POOL = 192
     base = make_clouds("ball", B, N, seed=rank_seed(1001, rank))
     rng = np.random.default_rng(rank)
@@ -382,12 +386,13 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
+    last_slot = {}
+
     def timed(engine, host, steps, warmup):
         def step_fn(i):
             if host:
-                engine.submit(pool_host[i % POOL], to_host=True)    # pinned host batch in, logits back to pinned host memory
-            else:
-                engine.submit(pool_dev[i % POOL])                   # device-resident batch (rotating pool > L2)
+                return engine.submit(pool_host[i % POOL], to_host=True)    # pinned host batch in, logits back to pinned host memory
+            return engine.submit(pool_dev[i % POOL])                       # device-resident batch (rotating pool > L2)
         for i in range(warmup):
             step_fn(i)
         barrier()
@@ -396,7 +401,7 @@ def main():
         e0.record(main)
         engine.fence_begin(e0)
         for i in range(steps):
-            step_fn(warmup + i)
+            last_slot[engine] = step_fn(warmup + i)
         engine.fence_end(main)
         e1.record(main)
         barrier()
@@ -407,6 +412,11 @@ def main():
     if rank == 0:
         sampler.start()
     ms_res = timed(engine, False, args.steps, args.warmup)
+    if args.dump_outputs and rank == 0:
+        # logits of the last timed step (its input is pool batch (warmup + steps - 1) % POOL: the same for the same arguments)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        logits = engine.result(last_slot[engine]).float().cpu().numpy()
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), logits.astype(np.float32))
     ms_e2e = timed(engine, True, args.steps, args.warmup)
     clocks = sampler.stop() if rank == 0 else None
     ms_res_1 = None
@@ -605,7 +615,7 @@ def main():
             v["gbs"] = v["alg_bytes"] / (v["us"] * 1e-6) / 1e9
             v["hbm_frac"] = v["gbs"] / peaks["hbm"]
             if ref_gpu and k in ref_gpu:
-                v["ref_gpu_us"] = ref_gpu[k]          # the reference's own kernel (sm_100a build) on the same tensors
+                v["ref_gpu_us"] = ref_gpu[k]          # the reference's own kernel (sm_90a build) on the same tensors
         for k in ("sa1_mlp", "sa2_mlp", "sa3_mlp"):
             kern[k] = {"us": stages[k], "tflops_fp32": SA_FLOPS[k[:3]] / (stages[k] * 1e-6) / 1e12}
         if ref_gpu:

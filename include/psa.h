@@ -1,5 +1,5 @@
 /*
- * psa.h -- C ABI of libpsa.so: the B200-native (sm_100a) point-set-abstraction hot path.
+ * psa.h -- C ABI of libpsa.so: the H100-native (sm_90a) point-set-abstraction hot path.
  *
  * This is the drop-in boundary.  The reference (hkust-vgd/scanobjectnn) reaches its native code through
  * plain C++ "Launcher" functions called from TensorFlow OpKernel::Compute (raw device pointers + int
@@ -42,7 +42,7 @@ typedef void* psa_stream_t; /* cudaStream_t */
 /* library identity / diagnostics */
 PSA_API int psa_version(void);                 /* MAJOR*10000 + MINOR*100 + PATCH */
 PSA_API const char* psa_last_error(void);      /* thread-local, valid until the next failing call on this thread */
-PSA_API int psa_sm_arch(void);                 /* 100: the only architecture compiled in (sm_100a) */
+PSA_API int psa_sm_arch(void);                 /* 90: the only architecture compiled in (sm_90a) */
 
 /* ---------------------------------------------------------------------------------------------
  * sampling/  (tf_sampling.cpp, tf_sampling_g.cu)
@@ -245,8 +245,8 @@ PSA_API int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, const 
                                    float* out, void* workspace, size_t workspace_bytes, psa_stream_t stream);
 
 /* Arithmetic of the grouped MLP.  Whenever the shapes allow -- set-abstraction levels with widths 64/128 (last width 64 or a
- * multiple of 128) and nsample 32/64/128 on tc_sa_dual_kernel, dense layers with N = 64 or a multiple of 128 on tc_dense2 /
- * tc_dense3 -- the layers after the first run on the tcgen05 tensor cores with fp32 accumulation in tensor memory; other shapes
+ * multiple of 128) and nsample 32/64/128 on tc_sa_kernel, dense layers with N = 64 or a multiple of 128 on tc_dense_kernel
+ * -- the layers after the first run on the Hopper tensor cores (wgmma) with fp32 accumulation; other shapes
  * run on the fp32-FMA kernels.  The fp32 operands are split into exactly representable 16-bit pieces:
  *   0 (default): two fp16 pieces per operand (22 mantissa bits), three MMAs per product  a1w2 + a2w1 + a1w1  -- the same error
  *      against fp64 as an fp32 FMA chain (1e-5 contract of the tests).  fp16 covers |v| < 65504: every kernel tracks the pieces

@@ -1,6 +1,6 @@
 """ctypes/numpy face of the CPU checker (oracle/liboracle.so) and of the compiled reference
 (oracle/_ref/libref_cpu.so = the reference's own CPU code, oracle/_ref/libref_tfops.so = the reference's
-own CUDA kernels for sm_100a).
+own CUDA kernels for sm_90a).
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__.smoke() and bench.py's cpu_baseline /
 ``--impl reference`` leg.  Nothing under scanobjectnn_b200/ may import this module.

@@ -10,7 +10,7 @@
  * so the ONLY fused multiply-adds are the fmaf() calls written below).
  *
  * Floating-point contract (verified from `cuobjdump -sass` of the reference .cu files compiled by
- * nvcc 12.9 for sm_100a, see DESIGN.md "Arithmetic pinned from SASS"):
+ * nvcc 12.9; the same contraction for sm_90a, see DESIGN.md "Arithmetic pinned from SASS"):
  *   GPU ops (FPS, ball query):  d2 = fma(dz,dz, fma(dx,dx, dy*dy))   -- FMUL(dy), FFMA(dx), FFMA(dz)
  *   CPU ops (three_nn, the test/ harness ball query): plain x86-64 g++ -O2, no FMA contraction:
  *                               d2 = (dx*dx + dy*dy) + dz*dz, each op rounded to float.

@@ -212,13 +212,13 @@ __device__ __forceinline__ BqGrid bq_stage_and_build(const BqSmem& s, int n, flo
     return g;
 }
 
-// squared distances of two dataset points to one query on the packed f32x2 pipe: per element the reference's
+// squared distances of two dataset points to one query, as float pairs: per element the reference's
 // FMUL(dy*dy), FFMA(dx,dx), FFMA(dz,dz) (x_k - q instead of q - x_k: identical squares)
 __device__ __forceinline__ float2 bq_dist2_pair(float2 x, float2 y, float2 z, float2 nqx, float2 nqy, float2 nqz) {
-    const float2 dx = __fadd2_rn(x, nqx), dy = __fadd2_rn(y, nqy), dz = __fadd2_rn(z, nqz);
-    float2 t = __fmul2_rn(dy, dy);
-    t = __ffma2_rn(dx, dx, t);
-    t = __ffma2_rn(dz, dz, t);
+    const float2 dx = fadd2_rn(x, nqx), dy = fadd2_rn(y, nqy), dz = fadd2_rn(z, nqz);
+    float2 t = fmul2_rn(dy, dy);
+    t = ffma2_rn(dx, dx, t);
+    t = ffma2_rn(dz, dz, t);
     return t;
 }
 

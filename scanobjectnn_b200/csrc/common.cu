@@ -15,5 +15,5 @@ void set_error(const char* fmt, ...) {
 extern "C" {
 int psa_version(void) { return 100; /* 0.1.0 */ }
 const char* psa_last_error(void) { return psa::g_err; }
-int psa_sm_arch(void) { return 100; }
+int psa_sm_arch(void) { return 90; }
 }

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libpsa.so (sm_100a only).
+// common.cuh -- shared helpers for libpsa.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,13 +6,13 @@
 
 #include "../../include/psa.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libpsa is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "libpsa is written for sm_90a (H100) only"
 #endif
 
 namespace psa {
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM
 
 void set_error(const char* fmt, ...);
 
@@ -82,6 +82,11 @@ __device__ __forceinline__ void stage_floats(float* __restrict__ dst, const floa
     }
     for (; i < count; i += THREADS) dst[i] = __ldg(src + i);
 }
+
+// Two-lane float arithmetic, each lane rounded on its own (identical results to two scalar __f*_rn calls).
+__device__ __forceinline__ float2 fadd2_rn(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2_rn(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 __device__ __forceinline__ unsigned lanemask_lt() {
     unsigned m;

@@ -1,4 +1,4 @@
-// graph.cu -- DGCNN graph functions for sm_100a: pairwise_distance, knn (top-k), the fused kNN graph that never
+// graph.cu -- DGCNN graph functions for sm_90a: pairwise_distance, knn (top-k), the fused kNN graph that never
 // materialises the (B,N,N) matrix, and get_edge_feature.
 //
 // Reference: dgcnn/utils/tf_util.py:638-706 -- tf.matmul + reduce_sum + transpose (a (B,N,N) fp32 matrix, 512 MiB at

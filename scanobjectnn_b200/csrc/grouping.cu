@@ -1,4 +1,4 @@
-// grouping.cu -- ball query, group_point (+grad), SelectionSort / knn_point for sm_100a.
+// grouping.cu -- ball query, group_point (+grad), SelectionSort / knn_point for sm_90a.
 //
 // Replaces pointnet2/tf_ops/grouping/tf_grouping_g.cu of the reference (one CTA per cloud, one thread per
 // query walking all n points from global memory).  The ball query itself lives in ball_query.cuh (spatial grid +
@@ -303,7 +303,7 @@ extern "C" int psa_query_ball_point(int b, int n, int m, float radius, int nsamp
     PSA_SUPPORTED(smem <= 200 * 1024, "query_ball_point: n=%d exceeds the shared-memory resident limit", n);
     bool none = false;
     float thr = ball_query_threshold(radius, &none);
-    // enough CTAs for ~2 waves of 148 SMs, at least two warp-batches of queries per CTA
+    // enough CTAs for ~2 waves of the SMs, at least two warp-batches of queries per CTA
     int chunks = (2 * kNumSMs + b - 1) / b;
     int q_per_cta = (m + chunks - 1) / chunks;
     // a CTA answers a multiple of 64 queries (8 warps x 8 queries per lane-per-slab step)

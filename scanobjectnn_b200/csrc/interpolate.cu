@@ -1,4 +1,4 @@
-// interpolate.cu -- three_nn / three_interpolate (+grad) and the fused FP-module interpolation for sm_100a.
+// interpolate.cu -- three_nn / three_interpolate (+grad) and the fused FP-module interpolation for sm_90a.
 //
 // The reference implements these only on the CPU (pointnet2/tf_ops/3d_interpolation/tf_interpolate.cpp:60-153,
 // single thread, DEVICE_CPU registration :187,222,262), so every PointNet++-BGA step bounces device->host->device

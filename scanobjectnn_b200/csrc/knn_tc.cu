@@ -1,14 +1,14 @@
 // knn_tc.cu -- DGCNN's kNN graph (pairwise_distance + top_k, dgcnn/utils/tf_util.py:638-671) with the X.X^T contraction on
-// the tcgen05 tensor cores and an EXACT refine, so the neighbour indices stay bit-identical to the canonical fp32 evaluation
+// the Hopper tensor cores (wgmma) and an EXACT refine, so the neighbour indices stay bit-identical to the canonical fp32 evaluation
 // (oracle/psa_oracle.c orc_dgcnn_knn: dot as an fma chain over the channels, adj = (|p|^2 + (-2 dot)) + |q|^2, k smallest,
 // lower index first on ties).
 //
 //   prep      a translation vector per cloud (knn_centre_kernel); every point row minus that vector is split once into bf16 pieces
 //             and laid out as [128 rows][64 k] K-major SWIZZLE_128B blocks (the weight-image layout of tc_mlp.cu), + the
 //             canonical |x|^2 and the centred |x - mu|^2 per row;
-//   main      CTA = 128 query rows of one cloud (TMEM lane = query row).  The query block is the A operand, candidate blocks
-//             stream through a two-stage ring (cp.async.bulk) as the B operand, D[128 x 128] = G tile in TMEM, two D slots.
-//             Four threads share a row, each reads ITS 32 columns of every tile with one tcgen05.ld -- no cross-lane traffic:
+//   main      CTA = 128 query rows of one cloud.  The query block is the A operand, candidate blocks stream through a two-stage
+//             ring (cp.async.bulk, one loader warp) as the B operand; four warpgroups each compute one 64 x 64 quarter of the
+//             G tile with wgmma and consume it straight from their accumulator registers (two rows x 16 columns per thread):
 //     pass 1  one bf16 MMA term (4 MMAs per tile): coarse distances (error <= E1) -> per-row histogram over logarithmic bins
 //             (float exponent + 4 mantissa bits) in shared memory -> tau = upper edge of the bin that holds the k-th smallest;
 //     pass 2  six MMA terms (bf16x3, error <= E2): every candidate with d < tau + E1 + E2 -- a superset of the true top-k -- is
@@ -37,7 +37,7 @@ namespace psa {
 using namespace tc;
 
 constexpr int kKtRowT = 4;                        // threads per query row (each owns 128 / kKtRowT columns of every tile)
-constexpr int kKtThreads = 128 * kKtRowT + 32;    // row warps + 1 issuer warp
+constexpr int kKtThreads = 128 * kKtRowT + 32;    // row warps (four warpgroups) + 1 loader warp
 constexpr uint32_t kKtPiece = 128u * 128u;        // one bf16 piece of a [128 rows][64 k] block: 16 KB
 constexpr uint32_t kKtBlock = 3u * kKtPiece;      // 48 KB
 constexpr int kKtBins = 256;
@@ -149,8 +149,7 @@ __device__ __forceinline__ float knn_canonical(const float* __restrict__ xp, con
 
 __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_constant__ KnnTcArgs a) {
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_qfull, s_full[2], s_dfull[2], s_dfree[2];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_qfull, s_full[2], s_dfree[2];
     __shared__ float s_wmax[kKtThreads / 32], s_wmaxo[kKtThreads / 32];
     __shared__ float s_T[128];
     __shared__ int s_cnt[128], s_namb[128];
@@ -170,10 +169,9 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
     const float* sqc = a.sqc + (size_t)cloud * npad;      // centred norms: what the tensor-core distances are assembled from
     const float* sqo = a.sq + (size_t)cloud * npad;       // original norms: the canonical formula and its rounding bound
 
-    if (warp_u == 4 * kKtRowT) tmem_alloc(&s_tmem, 256);
     if (tid == 0) {
         mbar_init(&s_qfull, 1);
-        for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_dfull[i], 1); mbar_init(&s_dfree[i], 4 * kKtRowT); }
+        for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_dfree[i], 4 * kKtRowT); }
         fence_mbar_init();
     }
     // candidate norms -> shared memory; the cloud's largest finite-or-not norm over the real points
@@ -189,10 +187,7 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) { mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o)); mxo = fmaxf(mxo, __shfl_xor_sync(0xffffffffu, mxo, o)); }
     if (lane == 0) { s_wmax[warp_u] = mx; s_wmaxo[warp_u] = mxo; }
-    fence_before_thread_sync();
     __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = warp_uniform(s_tmem);
     // pass 1 could look at a subset of the tiles (the k-th smallest of a SUBSET is still an upper bound of the k-th smallest of the
     // cloud): measured, every second tile halves the histogram work but doubles the lists -- 1-3 % of the rows of a feature cloud then
     // overflow kKtCap and the exhaustive kernel costs more than was saved (716 -> 1218 us at C = 64).  So: every tile.
@@ -202,61 +197,28 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
 
     constexpr uint32_t kTermPieces = PSA_KNN_TERMS == 6 ? 3u : 2u;
     if (warp_u == 4 * kKtRowT) {
-        // ================= issuer / loader warp =================
+        // ================= loader warp =================
         auto load = [&](int j) {
             const int s = j & 1, t = j < NT1 ? kStride1 * j : j - NT1;
             const uint32_t bytes = j < NT1 ? kKtPiece : (kTermPieces * kKtPiece);   // pass 1 needs the leading piece only
-            if (lane == 0) {
-                mbar_expect_tx(&s_full[s], bytes);
-                for (uint32_t o = 0; o < bytes; o += 16384u) bulk_g2s(cstage + (uint32_t)s * kKtBlock + o, img + (size_t)t * kKtBlock + o, 16384u, &s_full[s]);
-            }
+            mbar_expect_tx(&s_full[s], bytes);
+            for (uint32_t o = 0; o < bytes; o += 16384u) bulk_g2s(cstage + (uint32_t)s * kKtBlock + o, img + (size_t)t * kKtBlock + o, 16384u, &s_full[s]);
         };
         if (lane == 0) {
             mbar_expect_tx(&s_qfull, kKtBlock);
             for (uint32_t o = 0; o < kKtBlock; o += 16384u) bulk_g2s(qblk + o, img + (size_t)blockIdx.x * kKtBlock + o, 16384u, &s_qfull);
-        }
-        load(0);
-        if (J > 1) load(1);
-        mbar_wait(&s_qfull, 0);
-        const uint32_t idesc = make_idesc(kFmtBF16, 128, 128);
-        constexpr int kTerms = PSA_KNN_TERMS;                // 6: bf16x3 (all products down to 2^-24); 3: bf16x2 (2^-16)
-#if PSA_KNN_TERMS == 6
-        constexpr uint32_t qp[6] = {0, 1, 2, 0, 1, 0};       // query piece / candidate piece of the terms, small products first
-        constexpr uint32_t cp[6] = {2, 1, 0, 1, 0, 0};
-#else
-        constexpr uint32_t qp[3] = {0, 1, 0};
-        constexpr uint32_t cp[3] = {1, 0, 0};
-#endif
-        const int ks = (a.c + 15) / 16;                      // k-steps of 16 channels that hold data (the image is zero beyond c)
-        const SmemDescBase qa = smem_desc_base(warp_uniform(smem_u32(qblk)));
-        for (int j = 0; j < J; ++j) {
-            const int s = j & 1;
-            const uint32_t par = (uint32_t)((j >> 1) & 1);
-            mbar_wait(&s_full[s], par);
-            if (j >= 2) mbar_wait(&s_dfree[s], (uint32_t)(((j - 2) >> 1) & 1));      // rows finished reading this D slot
-            __syncwarp();
-            fence_after_thread_sync();
-            const uint32_t d = tmem_base + (uint32_t)s * 128u;
-            const SmemDescBase cb = smem_desc_base(warp_uniform(smem_u32(cstage) + (uint32_t)s * kKtBlock));
-            if (j < NT1) {
-                for (int s4 = 0; s4 < ks; ++s4) mma_bf16_ss(d, smem_desc_at(qa, s4 * 32), smem_desc_at(cb, s4 * 32), idesc, s4 ? 1u : 0u);
-            } else {
-#pragma unroll
-                for (int t6 = 0; t6 < kTerms; ++t6)
-                    for (int s4 = 0; s4 < ks; ++s4)
-                        mma_bf16_ss(d, smem_desc_at(qa, qp[t6] * kKtPiece + s4 * 32), smem_desc_at(cb, cp[t6] * kKtPiece + s4 * 32), idesc, (t6 | s4) ? 1u : 0u);
-            }
-            mma_commit(&s_dfull[s]);
-            if (j + 2 < J) {
-                mbar_wait(&s_dfull[s], par);             // this stage's operands are consumed: refill it two jobs ahead
+            load(0);
+            if (J > 1) load(1);
+            for (int j = 0; j + 2 < J; ++j) {
+                mbar_wait(&s_dfree[j & 1], (uint32_t)((j >> 1) & 1));     // every warpgroup's MMAs of job j are done: refill two jobs ahead
                 load(j + 2);
             }
         }
     } else {
         // ================= row threads: kKtRowT threads per query row =================
-        // thread (r, h): row r = tid & 127, part h = tid >> 7 owns columns [CW h, CW h + CW) of every candidate tile, CW = 128 / kKtRowT
-        // (warps w, w + 4, w + 8, .. read the same TMEM lanes).  Histogram counters and the candidate list of a row are shared by its two threads
-        // through shared-memory atomics; twice the warps hide twice the latency of the serial per-row work.
+        // In the two passes every thread consumes its own wgmma fragment (two rows x 16 columns of a 64 x 64 quarter of the tile); in the
+        // per-row work after them, thread (r, h) = (tid & 127, tid >> 7) is one of the kKtRowT threads of query row r.  Histogram counters
+        // and the candidate list of a row are shared by all threads that touch the row through shared-memory atomics.
         const int r = tid & 127, h = tid >> 7;
         const int q = blockIdx.x * 128 + r;
         const bool valid = q < n;
@@ -272,51 +234,81 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
         const float E2 = (PSA_KNN_TERMS == 6 ? 1e-4f : 1.5e-4f) * sgeo + 8e-6f * sqrtf(sqqo * sqmaxo) + 2e-6f * (sqqo + sqmaxo);
         const float dmax = 2.0f * (sqq + sqmax);
         const int keymax = (int)(__float_as_uint(fmaxf(dmax, 1e-30f)) >> 19) + 1;
-        constexpr int CW = 128 / kKtRowT;
-        static_assert(CW == 32, "one 32-column tcgen05.ld per thread and tile");
-        auto load_base = [&](float (&base)[32], int t) {
-            const float4* sc4 = reinterpret_cast<const float4*>(s_sq + t * 128 + h * CW);
-#pragma unroll
-            for (int l = 0; l < 8; ++l) {
-                const float4 v = sc4[l];
-                base[4 * l] = sqq + v.x; base[4 * l + 1] = sqq + v.y; base[4 * l + 2] = sqq + v.z; base[4 * l + 3] = sqq + v.w;
-            }
-        };
         constexpr int kRowThreads = 128 * kKtRowT;
-        const uint32_t taddr = tmem_base + ((uint32_t)((warp_u & 3) * 32) << 16) + (uint32_t)(h * CW);
-        for (int b = tid; b < kKtBins * 64; b += kRowThreads) hist[b] = 0u;
-        if (h == 0) { s_cnt[r] = 0; s_namb[r] = 0; }
-        asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");
-        const unsigned hinc = r < 64 ? 1u : 65536u;
-        unsigned* hcol = hist + (r & 63);
-        // ---- pass 1: coarse distances -> histogram ----
-        // (A running cut -- skipping the atomics of candidates farther than the bins that already hold k -- was measured slower:
-        //  987 vs 716 us at C = 64; the predicated atomics and the periodic histogram scans cost more than the atomics they save.)
-        for (int t1 = 0; t1 < NT1; ++t1) {
-            const int s = t1 & 1, t = kStride1 * t1;
-            float base[32];                                      // |q|^2 + |c|^2 of this thread's 32 columns, fetched while the MMAs run
-            load_base(base, t);
-            mbar_wait(&s_dfull[s], (uint32_t)((t1 >> 1) & 1));
-            fence_after_thread_sync();
-            {
-                uint32_t d[32];
-                tmem_ld32(taddr + (uint32_t)s * 128u, d);
-                tmem_ld_wait();
+        static_assert(kKtRowT == 4, "four warpgroups, one 64 x 64 quarter of every tile each");
+        // G tile of job j: warpgroup h computes rows 64 (h & 1) .., columns 64 (h >> 1) ..; this thread holds rows fr[0], fr[1] and
+        // columns 64 (h >> 1) + 8 i + 2 t + e of d[4 i + 2 u + e] (u = row), see tc_common.cuh
+        const int g = lane >> 2, tq = lane & 3;
+        const int fr[2] = {(h & 1) * 64 + (warp_u & 3) * 16 + g, (h & 1) * 64 + (warp_u & 3) * 16 + g + 8};
+        const int fc0 = (h >> 1) * 64 + 2 * tq;
+        float fsq[2];
+        int fkeymax[2];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float dist = fmaf(-2.0f, __uint_as_float(d[i]), base[i]);
-                    const int key = __float_as_int(dist) >> 19;      // arithmetic shift: zero / negative distances land in the last (nearest) bin
-                    const int bin = min(max(keymax - key, 0), kKtBins - 1);
-                    atomicAdd(hcol + bin * 64, hinc);            // fire-and-forget: no dependent chain through shared memory
-                }
+        for (int u = 0; u < 2; ++u) {
+            const int fq = blockIdx.x * 128 + fr[u];
+            fsq[u] = s_sq[fq < n ? fq : 0];
+            fkeymax[u] = (int)(__float_as_uint(fmaxf(2.0f * (fsq[u] + sqmax), 1e-30f)) >> 19) + 1;
+        }
+#if PSA_KNN_TERMS == 6
+        constexpr uint32_t qp[6] = {0, 1, 2, 0, 1, 0};       // query piece / candidate piece of the terms, small products first
+        constexpr uint32_t cp[6] = {2, 1, 0, 1, 0, 0};
+#else
+        constexpr uint32_t qp[3] = {0, 1, 0};
+        constexpr uint32_t cp[3] = {1, 0, 0};
+#endif
+        // all four k-steps of the 64-channel block, whatever c is: the image is zero beyond c, so the extra products are exact zeros,
+        // and a fixed count keeps the wgmma sequence straight-line (a runtime trip count makes ptxas serialise it)
+        constexpr int ks = 4;
+        const uint32_t qa = smem_u32(qblk) + (uint32_t)(h & 1) * 8192u;
+        // the MMAs of job j into d (waits for the stage; tells the loader when the stage may be refilled)
+        auto gram = [&](int j, bool fine, float (&d)[32]) {
+            const int s = j & 1;
+            mbar_wait(&s_full[s], (uint32_t)((j >> 1) & 1));
+            const uint32_t cb = smem_u32(cstage) + (uint32_t)s * kKtBlock + (uint32_t)(h >> 1) * 8192u;
+            wg_fence();
+            if (!fine) {
+#pragma unroll
+                for (int s4 = 0; s4 < ks; ++s4) wg_mma_ss_bf16(d, wg_desc(qa + s4 * 32), wg_desc(cb + s4 * 32), s4 ? 1u : 0u);
+            } else {
+#pragma unroll
+                for (int t6 = 0; t6 < PSA_KNN_TERMS; ++t6)
+#pragma unroll
+                    for (int s4 = 0; s4 < ks; ++s4)
+                        wg_mma_ss_bf16(d, wg_desc(qa + qp[t6] * kKtPiece + s4 * 32), wg_desc(cb + cp[t6] * kKtPiece + s4 * 32), (t6 | s4) ? 1u : 0u);
             }
-            fence_before_thread_sync();
+            wg_commit();
+            wg_wait_all();
+            wg_fence_acc(d);
             __syncwarp();
             if (lane == 0) mbar_arrive1(&s_dfree[s]);
+        };
+        for (int b = tid; b < kKtBins * 64; b += kRowThreads) hist[b] = 0u;
+        if (h == 0) { s_cnt[r] = 0; s_namb[r] = 0; }
+        mbar_wait(&s_qfull, 0);
+        asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");
+        // ---- pass 1: coarse distances -> histogram ----
+        // (A running cut -- skipping the atomics of candidates farther than the bins that already hold k -- costs more in predicated
+        //  atomics and periodic histogram scans than the atomics it saves.)
+        for (int t1 = 0; t1 < NT1; ++t1) {
+            const int t = kStride1 * t1;
+            float d[32];
+            gram(t1, false, d);
+#pragma unroll
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float dist = fmaf(-2.0f, d[4 * i + 2 * u + e], fsq[u] + s_sq[t * 128 + fc0 + 8 * i + e]);
+                        const int key = __float_as_int(dist) >> 19;      // arithmetic shift: zero / negative distances land in the last (nearest) bin
+                        const int bin = min(max(fkeymax[u] - key, 0), kKtBins - 1);
+                        atomicAdd(hist + (fr[u] & 63) + bin * 64, fr[u] < 64 ? 1u : 65536u);     // fire-and-forget
+                    }
         }
-        asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");           // both halves of every row are in the histogram
+        asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");           // every row's histogram is complete
         // ---- threshold: upper edge of the bin that holds the k-th smallest coarse distance, widened by the error bounds ----
         if (h == 0) {
+            const unsigned* hcol = hist + (r & 63);
             int cum = 0, b = kKtBins - 1;
             for (; b >= 0; --b) { const unsigned w = hcol[b * 64]; cum += (int)(r < 64 ? (w & 0xffffu) : (w >> 16)); if (cum >= a.k) break; }
             const float tau = b < 0 ? __int_as_float(0x7f800000) : __uint_as_float((uint32_t)(keymax - b + 1) << 19);
@@ -326,33 +318,27 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
         }
         // every row is done with its histogram before anybody's candidate list / distances overwrite the scratch area
         asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");
-        const float T = s_T[r];
+        const float fT[2] = {s_T[fr[0]], s_T[fr[1]]};
         // ---- pass 2: fine distances -> the row's candidate list (slots handed out by a shared-memory counter) ----
         for (int t = 0; t < NT; ++t) {
-            const int j = NT1 + t, s = j & 1;
-            float base[32];
-            load_base(base, t);
-            mbar_wait(&s_dfull[s], (uint32_t)((j >> 1) & 1));
-            fence_after_thread_sync();
-            {
-                uint32_t d[32];
-                tmem_ld32(taddr + (uint32_t)s * 128u, d);
-                tmem_ld_wait();
+            float d[32];
+            gram(NT1 + t, true, d);
 #pragma unroll
-                for (int i = 0; i < 32; ++i) {
-                    const float dist = fmaf(-2.0f, __uint_as_float(d[i]), base[i]);
-                    if (dist < T) {
-                        const int slot = atomicAdd(&s_cnt[r], 1);
-                        if (slot < kKtCap) {
-                            lidx[slot * 128 + r] = (unsigned short)(t * 128 + h * CW + i);
-                            ladj[slot * 128 + r] = dist;
+            for (int i = 0; i < 8; ++i)
+#pragma unroll
+                for (int u = 0; u < 2; ++u)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = fc0 + 8 * i + e;
+                        const float dist = fmaf(-2.0f, d[4 * i + 2 * u + e], fsq[u] + s_sq[t * 128 + col]);
+                        if (dist < fT[u]) {
+                            const int slot = atomicAdd(&s_cnt[fr[u]], 1);
+                            if (slot < kKtCap) {
+                                lidx[slot * 128 + fr[u]] = (unsigned short)(t * 128 + col);
+                                ladj[slot * 128 + fr[u]] = dist;
+                            }
                         }
                     }
-                }
-            }
-            fence_before_thread_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive1(&s_dfree[s]);
         }
         asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");
         const int cnt = s_cnt[r];
@@ -447,9 +433,6 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
             if (rank < a.k) out[rank] = ie;
         }
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    if (warp_u == 4 * kKtRowT) tmem_dealloc(tmem_base, 256);
 }
 
 // ---- exhaustive rows (worklist): one warp per row, canonical distances of all n candidates in shared memory, then k rounds of

@@ -1,5 +1,5 @@
 // mlp.cu -- grouped per-point shared MLP with the neighbourhood gather fused in front and the channel-wise
-// max-pool fused behind it (fp32 FMA path, sm_100a).
+// max-pool fused behind it (fp32 FMA path, sm_90a).
 //
 // Reference: pointnet_sa_module (pointnet2/utils/pointnet_util.py:87-154) = group_point + tile/sub + concat,
 // then three tf_util.conv2d 1x1 (+bias+BN+ReLU, pointnet2/utils/tf_util.py:120-185) and tf.reduce_max -- each a

@@ -52,7 +52,7 @@ sa_conv1_prebn_kernel(const __grid_constant__ F1Args a) {
     const BqGrid g = bq_stage_and_build<PPT>(s, n, a.radius, a.want_grid != 0);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int sub = lane & 7, rsub = lane >> 3;
-    // packed f32x2 registers: pair p of vector i covers channels 32*i + 4*sub + 2*p, +1
+    // float pairs: pair p of vector i covers channels 32*i + 4*sub + 2*p, +1
     constexpr int NPK = 2 * NV;
     float2 wx[NPK], wy[NPK], wz[NPK], bs[NPK], ssum[NPK], ssq[NPK];
 #pragma unroll
@@ -96,15 +96,15 @@ sa_conv1_prebn_kernel(const __grid_constant__ F1Args a) {
                     float2 s0 = bs[2 * i], s1 = bs[2 * i + 1];
                     if (urow) {
                         const float4 u = __ldg(reinterpret_cast<const float4*>(urow + 32 * i));
-                        s0 = __fadd2_rn(s0, make_float2(u.x, u.y)); s1 = __fadd2_rn(s1, make_float2(u.z, u.w));
+                        s0 = fadd2_rn(s0, make_float2(u.x, u.y)); s1 = fadd2_rn(s1, make_float2(u.z, u.w));
                     }
-                    // FFMA2: two channels per instruction
-                    const float2 v0 = __ffma2_rn(dz, wz[2 * i], __ffma2_rn(dy, wy[2 * i], __ffma2_rn(dx, wx[2 * i], s0)));
-                    const float2 v1 = __ffma2_rn(dz, wz[2 * i + 1], __ffma2_rn(dy, wy[2 * i + 1], __ffma2_rn(dx, wx[2 * i + 1], s1)));
+                    // two channels per float pair
+                    const float2 v0 = ffma2_rn(dz, wz[2 * i], ffma2_rn(dy, wy[2 * i], ffma2_rn(dx, wx[2 * i], s0)));
+                    const float2 v1 = ffma2_rn(dz, wz[2 * i + 1], ffma2_rn(dy, wy[2 * i + 1], ffma2_rn(dx, wx[2 * i + 1], s1)));
                     __stcs(reinterpret_cast<float4*>(orow + 32 * i), make_float4(v0.x, v0.y, v1.x, v1.y));   // streaming store
                     if (STATS) {
-                        ssum[2 * i] = __fadd2_rn(ssum[2 * i], v0); ssum[2 * i + 1] = __fadd2_rn(ssum[2 * i + 1], v1);
-                        ssq[2 * i] = __ffma2_rn(v0, v0, ssq[2 * i]); ssq[2 * i + 1] = __ffma2_rn(v1, v1, ssq[2 * i + 1]);
+                        ssum[2 * i] = fadd2_rn(ssum[2 * i], v0); ssum[2 * i + 1] = fadd2_rn(ssum[2 * i + 1], v1);
+                        ssq[2 * i] = ffma2_rn(v0, v0, ssq[2 * i]); ssq[2 * i + 1] = ffma2_rn(v1, v1, ssq[2 * i + 1]);
                     }
                 }
             }
@@ -147,14 +147,14 @@ sa_conv1_prebn_kernel(const __grid_constant__ F1Args a) {
 //   * three warpgroups = three pipeline stages (registers re-partitioned with setmaxnreg: 128 / 56 / 56):
 //       SEARCH   warps 0-3.  No spatial grid: at these sizes (n <= 4096, ~60 queries per CTA) an exhaustive test out of
 //                REGISTERS is cheaper than building one.  A search thread keeps PPTP CONSECUTIVE points of the cloud in
-//                registers as packed f32x2 pairs and tests them against every query of a batch with the reference's
+//                registers as float pairs and tests them against every query of a batch with the reference's
 //                arithmetic (NaN counts as inside); the SIGN of (thr - d) is shifted straight into the lane's hit mask, and
 //                because the lane's points are consecutive that mask IS bits [PPTP*tid, +PPTP) of the query's bitmap -- no
 //                ballots, no atomics, no compaction;
 //       EXTRACT  warps 4-7.  LPQ = 16 lanes per query read the nsample lowest set bits out in index order (popcount prefix
 //                sums: the reference's "first nsample in index order", padded with the first hit), write idx / pts_cnt to
 //                global memory and the centred rows (dx,dy,dz,j) of the batch into the rows ring;
-//       CONV     warps 8-11.  Per step 4 rows x C1 channels -- one LDS.128 for the row's (dx,dy,dz,j), 6 FFMA2 per 4 channels
+//       CONV     warps 8-11.  Per step 4 rows x C1 channels -- one LDS.128 for the row's (dx,dy,dz,j), 12 FFMA per 4 channels
 //                with the weights resident in registers, 128-byte streaming stores, BN statistics in registers.
 //     Levels WITH input features (HAS_U) run two stages instead: warps 0-3 search and extract, warps 4-11 convolve (the
 //     512-byte U-row gathers of the conv stage are what needs the warps there);
@@ -228,13 +228,17 @@ __device__ __forceinline__ long long clock_after_smem(const volatile int* w) {
 #define F1CLK() clock_after_smem(reinterpret_cast<const volatile int*>(centres))
 #endif
 
-// packed f32x2 arithmetic on 64-bit registers (aligned pairs by construction: the compiler never has to shuffle halves)
+// float pairs in 64-bit registers, each half rounded on its own (sm_90 has no packed f32x2 instructions: two scalar ops each)
 typedef unsigned long long u64;
 __device__ __forceinline__ u64 f2_pack(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ u64 f2_add(u64 a, u64 b) { u64 r; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 f2_sub(u64 a, u64 b) { u64 r; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 f2_mul(u64 a, u64 b) { u64 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ u64 f2_fma(u64 a, u64 b, u64 c) { u64 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r; }
+__device__ __forceinline__ float2 f2_split(u64 v) { float lo, hi; asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); return make_float2(lo, hi); }
+__device__ __forceinline__ u64 f2_add(u64 a, u64 b) { const float2 x = f2_split(a), y = f2_split(b); return f2_pack(__fadd_rn(x.x, y.x), __fadd_rn(x.y, y.y)); }
+__device__ __forceinline__ u64 f2_sub(u64 a, u64 b) { const float2 x = f2_split(a), y = f2_split(b); return f2_pack(__fsub_rn(x.x, y.x), __fsub_rn(x.y, y.y)); }
+__device__ __forceinline__ u64 f2_mul(u64 a, u64 b) { const float2 x = f2_split(a), y = f2_split(b); return f2_pack(__fmul_rn(x.x, y.x), __fmul_rn(x.y, y.y)); }
+__device__ __forceinline__ u64 f2_fma(u64 a, u64 b, u64 c) {
+    const float2 x = f2_split(a), y = f2_split(b), z = f2_split(c);
+    return f2_pack(__fmaf_rn(x.x, y.x, z.x), __fmaf_rn(x.y, y.y, z.y));
+}
 __device__ __forceinline__ void f2_unpack_bits(u64 v, unsigned& lo, unsigned& hi) { asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v)); }
 
 template <int NV, bool HAS_U, int PPTP>
@@ -418,8 +422,8 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
 #endif
                 if (warp == 0 && lane < nqb) centres[bslot * QB + lane] = make_float4(cqx, cqy, cqz, 0.f);
                 if (!TWO && tid == 0) s_hdrB[slot] = make_int4((int)(gq0 - q_begin), nqb, (gq0 + nqb == seg_end && seg_end < q_end) ? 1 : 0, 0);
-                // ---- exhaustive test on the packed f32x2 pipe: per point pair 3 FADD2 + FMUL2 + 2 FFMA2 (the reference's
-                //      distance) + one FADD2 s = thr - d + two funnel shifts that push the SIGN of s into the lane's mask.
+                // ---- exhaustive test on float pairs: per point 3 FADD + FMUL + 2 FFMA (the reference's
+                //      distance) + one FADD s = thr - d + funnel shifts that push the SIGN of s into the lane's mask.
                 //      sign(s) = 1 <=> d > thr; d == thr gives +0 and a NaN distance the canonical (positive) NaN, i.e. both
                 //      count as inside exactly like !(d > thr) (tf_grouping_g.cu:20-21: max(sqrtf(NaN),1e-20f) < r holds) ----
                 if (!a.none) {
@@ -578,14 +582,14 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                 float2 s0 = ba, s1 = bb;
                 if (HAS_U) {
                     const float4 uu = __ldg(reinterpret_cast<const float4*>(ucloud + (unsigned)__float_as_int(d.w) * (unsigned)C1c));
-                    s0 = __fadd2_rn(s0, make_float2(uu.x, uu.y)); s1 = __fadd2_rn(s1, make_float2(uu.z, uu.w));
+                    s0 = fadd2_rn(s0, make_float2(uu.x, uu.y)); s1 = fadd2_rn(s1, make_float2(uu.z, uu.w));
                 }
                 const float2 dx = make_float2(d.x, d.x), dy = make_float2(d.y, d.y), dz = make_float2(d.z, d.z);
-                const float2 v0 = __ffma2_rn(dz, wza, __ffma2_rn(dy, wya, __ffma2_rn(dx, wxa, s0)));
-                const float2 v1 = __ffma2_rn(dz, wzb, __ffma2_rn(dy, wyb, __ffma2_rn(dx, wxb, s1)));
+                const float2 v0 = ffma2_rn(dz, wza, ffma2_rn(dy, wya, ffma2_rn(dx, wxa, s0)));
+                const float2 v1 = ffma2_rn(dz, wzb, ffma2_rn(dy, wyb, ffma2_rn(dx, wxb, s1)));
                 __stcs(reinterpret_cast<float4*>(dst), make_float4(v0.x, v0.y, v1.x, v1.y));
-                ssum[0] = __fadd2_rn(ssum[0], v0); ssum[1] = __fadd2_rn(ssum[1], v1);
-                ssq[0] = __ffma2_rn(v0, v0, ssq[0]); ssq[1] = __ffma2_rn(v1, v1, ssq[1]);
+                ssum[0] = fadd2_rn(ssum[0], v0); ssum[1] = fadd2_rn(ssum[1], v1);
+                ssq[0] = ffma2_rn(v0, v0, ssq[0]); ssq[1] = ffma2_rn(v1, v1, ssq[1]);
             };
             if ((nrows & (4 * RPI - 1)) == 0) {
                 const float4* sp = sd + cw * 4 * RPI + lr;
@@ -854,13 +858,13 @@ sa_conv1_sync_kernel(const __grid_constant__ F1SArgs a) {
                         float2 s0 = ba, s1 = bb;
                         if (HAS_U) {
                             const float4 uu = __ldg(reinterpret_cast<const float4*>(ucloud + (unsigned)__float_as_int(d.w) * (unsigned)C1));
-                            s0 = __fadd2_rn(s0, make_float2(uu.x, uu.y)); s1 = __fadd2_rn(s1, make_float2(uu.z, uu.w));
+                            s0 = fadd2_rn(s0, make_float2(uu.x, uu.y)); s1 = fadd2_rn(s1, make_float2(uu.z, uu.w));
                         }
-                        const float2 v0 = __ffma2_rn(dz, wza, __ffma2_rn(dy, wya, __ffma2_rn(dx, wxa, s0)));
-                        const float2 v1 = __ffma2_rn(dz, wzb, __ffma2_rn(dy, wyb, __ffma2_rn(dx, wxb, s1)));
+                        const float2 v0 = ffma2_rn(dz, wza, ffma2_rn(dy, wya, ffma2_rn(dx, wxa, s0)));
+                        const float2 v1 = ffma2_rn(dz, wzb, ffma2_rn(dy, wyb, ffma2_rn(dx, wxb, s1)));
                         __stcs(reinterpret_cast<float4*>(outl + (unsigned)r * (unsigned)C1), make_float4(v0.x, v0.y, v1.x, v1.y));
-                        ssum[0] = __fadd2_rn(ssum[0], v0); ssum[1] = __fadd2_rn(ssum[1], v1);
-                        ssq[0] = __ffma2_rn(v0, v0, ssq[0]); ssq[1] = __ffma2_rn(v1, v1, ssq[1]);
+                        ssum[0] = fadd2_rn(ssum[0], v0); ssum[1] = fadd2_rn(ssum[1], v1);
+                        ssq[0] = ffma2_rn(v0, v0, ssq[0]); ssq[1] = ffma2_rn(v1, v1, ssq[1]);
                     }
                 }
             }

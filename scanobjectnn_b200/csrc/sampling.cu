@@ -1,11 +1,11 @@
-// sampling.cu -- farthest point sampling + gather_point (+grad) for sm_100a.
+// sampling.cu -- farthest point sampling + gather_point (+grad) for sm_90a.
 //
 // Replaces pointnet2/tf_ops/sampling/tf_sampling_g.cu:105-192 of the reference.  Results are index-exact with the
 // reference kernel, including its tie-break (minimum over (k mod 512, k) among equal maxima), which is carried as an
 // explicit 32-bit key so the thread <-> point mapping is free.  One CTA per cloud with as FEW warps as the registers
 // allow (4 warps up to N=2048: the round time is dominated by the cross-warp arg-max, not by arithmetic); coordinates
-// and running min-distances live in registers (no global `temp` round trip), distances use the packed f32x2 pipe
-// (FADD2/FMUL2/FFMA2, same IEEE operations and order as the reference's contraction), the block arg-max is
+// and running min-distances live in registers (no global `temp` round trip), distances are computed on float pairs
+// (same IEEE operations and order as the reference's contraction), the block arg-max is
 // REDUX.MAX + REDUX.MIN per warp and one shared-memory hop (1 __syncthreads per round instead of the reference's 10),
 // and the gather of the sampled coordinates is fused.
 #include <limits.h>
@@ -63,11 +63,11 @@ fps_kernel(int n, int m, const float* __restrict__ xyz, int* __restrict__ idx_ou
         unsigned bkey = 0xffffffffu;
 #pragma unroll
         for (int q = 0; q < NP; ++q) {
-            // FMUL2 dy*dy ; FFMA2 dx,dx ; FFMA2 dz,dz : per element the reference's contraction, two points per instruction
-            const float2 dx = __fadd2_rn(px[q], nx), dy = __fadd2_rn(py[q], ny), dz = __fadd2_rn(pz[q], nz);
-            float2 d = __fmul2_rn(dy, dy);
-            d = __ffma2_rn(dx, dx, d);
-            d = __ffma2_rn(dz, dz, d);
+            // FMUL dy*dy ; FFMA dx,dx ; FFMA dz,dz : per element the reference's contraction, two points per float pair
+            const float2 dx = fadd2_rn(px[q], nx), dy = fadd2_rn(py[q], ny), dz = fadd2_rn(pz[q], nz);
+            float2 d = fmul2_rn(dy, dy);
+            d = ffma2_rn(dx, dx, d);
+            d = ffma2_rn(dz, dz, d);
             td[q].x = fminf(d.x, td[q].x);                         // NaN d leaves td unchanged, as CUDA min() does
             td[q].y = fminf(d.y, td[q].y);
             if (td[q].x > best) { best = td[q].x; bkey = key[2 * q]; }

@@ -1,13 +1,14 @@
-// tc_common.cuh -- hand-written tcgen05 / TMEM / mbarrier wrappers for sm_100a (inline PTX, no CUTLASS).
+// tc_common.cuh -- hand-written wgmma / TMA bulk copy / mbarrier wrappers for sm_90a (inline PTX, no CUTLASS).
 //
-// Conventions used by the kernels in tc_mlp.cu:
-//   * accumulators D and the A operand live in TMEM (128 lanes x 512 32-bit columns per SM); row r of a 128-row tile
-//     is TMEM lane r, warp w of the CTA's four "row" warps owns lanes 32w..32w+31;
+// Conventions used by the kernels in tc_mlp.cu and knn_tc.cu:
+//   * one WARPGROUP (4 warps, 128 threads) computes a 64-row tile: D[64 x 64] (+)= A[64 x 16] . B[16 x 64] per
+//     wgmma.mma_async m64n64k16, fp32 accumulators in registers.  Warp w of the group holds rows 16w..16w+15; lane
+//     (g = lane / 4, t = lane % 4) holds, of every 8-column block j, d[4j], d[4j+1] = row g, columns 8j+2t, 8j+2t+1 and
+//     d[4j+2], d[4j+3] = the same columns of row g+8.  The A operand from registers has the matching layout (a0: row g,
+//     k 2t..2t+1; a1: row g+8; a2, a3: k + 8), so the D of one layer becomes the A of the next without leaving registers;
 //   * the B operand (weights, [N][K] "K-major") lives in shared memory in the canonical 128-byte-swizzle layout:
 //     8-row x 128-byte atoms, 16-byte chunk index XOR (row % 8), atoms of consecutive 8-row groups 1024 B apart (SBO),
-//     consecutive 128-byte K blocks N*128 B apart;
-//   * one warp runs the issue code converged, its elected lane issues tcgen05.mma and commits to an mbarrier (see MMA
-//     ISSUE CONVENTION below); everybody else waits on the barrier's parity.
+//     consecutive 128-byte K blocks N*128 B apart.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -18,19 +19,7 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// ---- TMEM allocation (one full warp executes these) ----
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-__device__ __forceinline__ void fence_before_thread_sync() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void fence_after_thread_sync() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
-// generic-proxy shared-memory writes -> visible to the async proxy (tcgen05.mma reads B through descriptors)
+// generic-proxy shared-memory writes -> visible to the async proxy (wgmma reads operands through descriptors)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
 
 // ---- mbarrier ----
@@ -49,27 +38,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "=r"(done)
             : "r"(addr), "r"(parity)
             : "memory");
-#if defined(PSA_MBAR_SLEEP_NS) && PSA_MBAR_SLEEP_NS > 0
-        if (!done) __nanosleep(PSA_MBAR_SLEEP_NS);      // A/B builds (tools/build_variant.py): back off instead of re-polling at once
-#endif
     } while (!done);
 }
-// MMA ISSUE CONVENTION.  tcgen05.mma takes its operands from UNIFORM registers.  Issued from `if (tid == 0)` the
-// compiler cannot prove uniformity and wraps every MMA in an ELECT / R2UR.BROADCAST loop (~17 instructions, ~110 cycles
-// per MMA measured -- slower than the 32 / 64 cycles the tensor pipe needs for an N = 64 / 128 instruction,
-// tools/microbench/mma_rate.cu).  So: the WHOLE issuer warp runs the issue code converged, with operands derived from
-// warp-uniform values (kernel parameters, loop counters, `warp_uniform(...)`), and elect.sync picks the lane that
-// executes the instruction.  The elected lane is the same every time (lowest active), so tcgen05.commit tracks its MMAs.
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
-
-// all previously issued tcgen05.mma of the elected lane arrive on `bar` when they complete (converged warp)
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}\n" ::"r"(smem_u32(bar))
-        : "memory");
-}
 
 // ---- bulk async copy global -> shared (TMA engine, 1-D, no tensor map), completion on an mbarrier ----
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -83,97 +54,53 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
 }
 
 // ---- descriptors ----
-// Shared-memory matrix descriptor, K-major, SWIZZLE_128B (cute::UMMA::SmemDescriptor bit layout):
+// wgmma shared-memory matrix descriptor, K-major, SWIZZLE_128B:
 //   [0,14) start address >> 4 | [16,30) leading byte offset >> 4 (unused for swizzled K-major; 1) |
-//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups) | [46,48) version = 1 | [61,64) layout type = 2
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
+//   [32,46) stride byte offset >> 4 (1024 B between 8-row groups) | [62,64) layout type = 1 (128-byte swizzle)
+// Moving the tile by `off` bytes (a multiple of 16 inside the 256 KB window, e.g. 32 B per 16-element K step) is one add on the
+// start-address field.
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr) {
     const uint32_t lo = ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
-    const uint32_t hi = (1024u >> 4) | (1u << 14) | (2u << 29);
+    const uint32_t hi = (1024u >> 4) | (1u << 30);
     return ((uint64_t)hi << 32) | lo;
 }
-// The same descriptor as base + byte offset: the start-address field is (address >> 4), so moving the tile by `off`
-// bytes (a multiple of 16, same 256 KB window) is one add on the low word -- per-MMA descriptor math stays uniform.
-struct SmemDescBase { uint32_t lo, hi; };
-__device__ __forceinline__ SmemDescBase smem_desc_base(uint32_t smem_addr) {
-    SmemDescBase b;
-    b.lo = ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
-    b.hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-    return b;
-}
-__device__ __forceinline__ uint64_t smem_desc_at(SmemDescBase b, uint32_t off) { return ((uint64_t)b.hi << 32) | (uint64_t)(b.lo + (off >> 4)); }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = f32, A/B format (2 = tf32, 1 = bf16), both K-major,
-// N >> 3 at [17,23), M >> 4 at [24,29).
-__device__ __forceinline__ uint32_t make_idesc(uint32_t ab_format, uint32_t M, uint32_t N) {
-    return (1u << 4) | (ab_format << 7) | (ab_format << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1, kFmtTF32 = 2;     // kind::f16 takes F16 or BF16 operands; kind::tf32 takes TF32
+constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1;
 
-// D[tmem] (+)= A[tmem] * B[smem desc]; accumulate = 0 overwrites D.  Call from a CONVERGED warp (see above).
-__device__ __forceinline__ void mma_tf32_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void mma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// ---- wgmma (whole warpgroup, converged) ----
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+// accumulators are written asynchronously: after wg_wait_all, pin every read of them behind the wait
+__device__ __forceinline__ void wg_fence_acc(float (&d)[32]) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc] (both operands from shared memory).  Converged warp, as above.
-__device__ __forceinline__ void mma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// D[64 x 64] (+)= A[64 x 16] (registers, NP = 2: fp16, NP = 3: bf16) . B[16 x 64] (shared memory); accumulate = 0 overwrites D
+template <int NP>
+__device__ __forceinline__ void wg_mma_rs(float (&d)[32], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t bdesc, uint32_t accumulate) {
+    if constexpr (NP == 2) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(accumulate));
+    } else {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+            : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(bdesc), "r"(accumulate));
+    }
 }
-
-// ---- TMEM <-> registers: each lane moves its own row (TMEM lane = 32*(warp%4) + laneid) ----
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// D[64 x 64] (+)= A[64 x 16] . B[16 x 64], both bf16 from shared memory (K-major SWIZZLE_128B descriptors)
+__device__ __forceinline__ void wg_mma_ss_bf16(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};\n" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-        "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-        "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};\n" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;\n" ::: "memory"); }
 
 // ---- operand quantisation (done by us, so the tensor core only ever sees exactly representable values) ----
 __device__ __forceinline__ float tf32_trunc(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }

@@ -1,35 +1,30 @@
-// tc_mlp.cu -- the grouped shared MLP of a set-abstraction level and the dense layers on the 5th-gen tensor cores
-// (tcgen05 + TMEM), hand-written PTX wrappers in tc_common.cuh.
+// tc_mlp.cu -- the grouped shared MLP of a set-abstraction level and the dense layers on the Hopper tensor cores
+// (wgmma, A from registers, B from shared memory), hand-written PTX wrappers in tc_common.cuh.
 //
 // What the reference does (pointnet2/utils/pointnet_util.py:113-127): group_point -> (B,m,K,3+C) tensor -> three
 // cuDNN 1x1 convs over B*m*K rows -> reduce_max.  What the kernels here do per 128-row tile (128/K neighbourhoods):
 //
 //   layer 1   is never a GEMM over grouped rows.  (x_j - c) . Wx + f_j . Wf  =  U[j] + (x_j - c) . Wx   with
 //             U = points . W1[3:,:] computed ONCE per source point (K-fold fewer rows, a dense-layer launch); each
-//             row-thread gathers its U row (512 B), adds the 3-term xyz part in FMAs, applies the folded BN affine + ReLU
-//             and writes the result straight into TENSOR MEMORY as the A operand of layer 2 -- the (B,m,K,C) tensors of
-//             the reference never exist, not even in shared memory.
-//   layers 2+ tcgen05.mma, A from TMEM (lane = row), B = weights in shared memory in the canonical K-major SWIZZLE_128B
-//             layout, dropped there by cp.async.bulk from pre-arranged images; D in TMEM.  Between layers the row warps
-//             pull D with tcgen05.ld, apply affine + ReLU and push the next A operand with tcgen05.st.
-//   max-pool  the last epilogue reduces each neighbourhood's rows with a transposing warp butterfly and writes
-//             (B,m,C_out) coalesced.  64-wide levels ending in a 128-wide layer (DB = 3, SA1) run the LAST layer transposed
-//             instead: H^T written to shared memory by the previous epilogue, D^T[channel][row] -- lane = channel, so the
-//             max-pool is an in-thread reduction, the affine a per-thread scalar and the stores coalesced row segments.
+//             thread gathers its part of the U rows, adds the 3-term xyz part in FMAs, applies the folded BN affine + ReLU
+//             and keeps the result in registers as the A operand of layer 2 -- the (B,m,K,C) tensors of the reference
+//             never exist, not even in shared memory.
+//   layers 2+ wgmma, A from registers, B = weights in shared memory in the canonical K-major SWIZZLE_128B layout, dropped
+//             there by cp.async.bulk from pre-arranged images; D in registers, whose layout is that of the next A operand.
+//   max-pool  the last epilogue reduces each neighbourhood's rows in-thread, across the warp with shuffles and across warps in
+//             shared memory, and writes (B,m,C_out) coalesced.
 //
-// Kernels (all templated on NP, the pieces per operand -- Split<NP> in tc_common.cuh):
-//   tc_sa_dual_kernel<DB,NP>  SA level, two row groups per CTA, per-group streamed last layer, tensor-pipe token, one or two D
-//                             slots (DB = 0/1/2), DB = 3 = transposed last layer; optional centre weights = multi-layer EdgeConv over 3-D points
-//   tc_dense3_kernel<NP>      dense layer, transposed (lane = channel), both operands from shared memory; also the
-//                             training-mode forward (previous batch norm applied on load, statistics in the epilogue)
-//   tc_dense2_kernel<NT,NP>   dense layer, A from TMEM, warp-specialised pipeline (N = 64 or K > 512)
+// Kernels (both templated on NP, the pieces per operand -- Split<NP> in tc_common.cuh):
+//   tc_sa_kernel<NP,..>       SA level (specialised on its shape); optional centre weights = multi-layer EdgeConv over 3-D points
+//   tc_dense_kernel<NP,NC>    dense layer, 64 NC output channels per CTA; also the training-mode forward (previous batch norm
+//                             applied on load, column statistics in the epilogue)
 // fp32 parity: operands are quantised by this code, so the tensor core only ever sees exactly representable values; fp32
-// accumulation in TMEM truncates, hence small terms first and K cut into <= 128-wide pieces (tests hold 1e-5 vs fp64).
+// accumulation in the tensor core truncates, hence small terms first and K cut into <= 128-wide pieces (tests hold 1e-5 vs fp64).
 //   NP = 2 (inference default): two fp16 pieces, three MMAs per product; every kernel tracks the leading pieces it stores and raises
 //           a device-side flag when a value leaves the fp16 range -- the launchers then rerun the op on the NP = 3 instantiation
 //           (enqueued unconditionally, a no-op unless the flag is set: `run_if`);
 //   NP = 3 (psa_set_mlp_mode(2), the guarded rerun, the training forward): three bf16 pieces, six MMAs per product.
-// Levels the dual kernel cannot hold run on the fp32-FMA fused kernel of mlp.cu.
+// Levels the SA kernel cannot hold run on the fp32-FMA fused kernel of mlp.cu.
 #include <float.h>
 #include <stdlib.h>
 
@@ -47,13 +42,13 @@ constexpr int kMaxTcLayers = 2;
 
 // ------------------------------------------------------------------------------------------------------------------
 // Weight images.  A tensor layer W (K x N, row-major, fp32) is pre-arranged once per weight set (tc_prep_weights_kernel) into
-// blocks that can be dropped into shared memory by a single cp.async.bulk and fed to tcgen05.mma unchanged:
+// blocks that can be dropped into shared memory by a single cp.async.bulk and fed to wgmma unchanged:
 //   block (nt, kc) covers output channels [nt*Nt, nt*Nt+Nt) x input channels [kc*64, kc*64+64): NP 16-bit pieces
 //   (every piece exactly representable), each [Nt][64] K-major SWIZZLE_128B, Nt*128 B per piece; blocks stored in (nt major,
 //   kc minor) order.  2 NP bytes per weight.
 // ------------------------------------------------------------------------------------------------------------------
 // np = pieces per weight: 3 (bf16x3, 6 bytes per weight) or 2 (fp16x2, 4 bytes); see Split<NP> in tc_common.cuh
-__host__ __device__ inline uint32_t tc_block_bytes(int Nt, int np) { return (uint32_t)Nt * 128u * (uint32_t)np; }
+__host__ __device__ constexpr uint32_t tc_block_bytes(int Nt, int np) { return (uint32_t)Nt * 128u * (uint32_t)np; }
 __host__ __device__ inline size_t tc_image_bytes(int K, int N, int np) { return (size_t)K * N * 2u * (size_t)np; }     // independent of the tile width
 // an image allocation = the blocks + a 256-byte trailer whose first word is set when a weight left the fp16 range (np = 2)
 __host__ __device__ inline size_t tc_image_alloc_bytes(int K, int N, int np) { return ((tc_image_bytes(K, N, np) + 255) & ~(size_t)255) + 256; }
@@ -80,56 +75,43 @@ struct TcArgs {
     const float* t[kMaxTcLayers];
     int relu[kMaxTcLayers];
     int Kd[kMaxTcLayers], Ntot[kMaxTcLayers];
-    int stream_last;       // 1: the last layer's weights do not fit next to the others -> one 128-channel tile at a time
-    int ntcap;             // 64 (narrow configuration) or 128 (wide)
-    int dual;              // 1: tc_sa_dual_kernel (two row groups per CTA, 64-wide output tiles)
+    int stream_last;       // 1: the last layer's weights do not fit next to the others -> one 64-channel chunk at a time
     unsigned int* tile_counter;   // zeroed before the launch: tiles are handed out dynamically (CTAs that start late or
                                   // share their SM with another stream's kernels simply take fewer)
     int np;                       // operand pieces: 2 (fp16x2) or 3 (bf16x3)
-    int tmode;                    // 1: the last layer runs TRANSPOSED (tc_sa_dual_kernel<3, 2>, see dual_dcol): lane = channel
     unsigned int* ovf;            // np = 2: set to 1 when an activation or weight left the fp16 range (the result is then invalid)
     const unsigned int* run_if;   // non-null: the launch is a no-op unless *run_if != 0 (the np = 3 rerun of a flagged launch)
     const unsigned int* wflag[kMaxTcLayers];   // np = 2: trailer word of each weight image
 };
 
-// transposing butterfly: v[q] = column q of this lane's row; afterwards v[0] on lane l = max over the warp's 32 rows of column l
-__device__ __forceinline__ float warp_colmax_32x32(float (&v)[32], int lane) {
+// ------------------------------------------------------------------------------------------------------------------
+// Fragment helpers of the warpgroup kernels (layout in tc_common.cuh).  A 128-row tile is two warpgroups; warp w of the
+// CTA holds tile rows 16w + g and 16w + g + 8 (g = lane / 4, t = lane % 4).
+// ------------------------------------------------------------------------------------------------------------------
+// split the pair (x0, x1) of consecutive k into NP pieces and store piece i as register r of K step s of A
+template <int NP, int S>
+__device__ __forceinline__ void put_a(uint32_t (&A)[NP][S][4], int s, int r, float x0, float x1, uint32_t& ovf) {
+    uint32_t p[NP];
+    split_pair<NP>(x0, x1, p, ovf);
 #pragma unroll
-    for (int half = 16; half >= 1; half >>= 1) {
-        const bool up = (lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const float send = up ? v[i] : v[i + half];
-            const float keep = up ? v[i + half] : v[i];
-            const float recv = __shfl_xor_sync(0xffffffffu, send, half);
-            v[i] = fmaxf(keep, recv);
-        }
-    }
-    return v[0];
+    for (int i = 0; i < NP; ++i) A[i][s][r] = p[i];
 }
 
-#ifdef PSA_TC_TIMING
-// debug build only (tools/tc_timing.py): cycles thread 0 of every CTA spends in each phase of the tensor-core kernels
-__device__ unsigned long long g_tc_timing[8];
-#define TC_STAMP(i) do { if (tid == 0) { const long long now_ = clock64(); tacc[i] += (unsigned long long)(now_ - tprev); tprev = now_; } } while (0)
-#else
-#define TC_STAMP(i) do { } while (0)
-#endif
+// max over the 16 rows of a warp of columns (8j + 2t, 8j + 2t + 1): in-thread over rows g / g + 8, then across g
+__device__ __forceinline__ float warp_rowmax16(float lo, float hi) {
+    float m = fmaxf(lo, hi);
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 4));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
+    m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
+    return m;
+}
+__device__ __forceinline__ float warp_rowsum16(float v) {
+    v += __shfl_xor_sync(0xffffffffu, v, 4);
+    v += __shfl_xor_sync(0xffffffffu, v, 8);
+    v += __shfl_xor_sync(0xffffffffu, v, 16);
+    return v;
+}
 
-// ------------------------------------------------------------------------------------------------------------------
-// tc_sa_dual_kernel -- levels with 128-wide layers (PointNet++ SA2: 131 -> 128 -> 128 -> 256 over 64-point neighbourhoods).
-//
-// One tile at a time per CTA serialises "row work" (gather, BN/ReLU, operand split, max-pool: ~56 % of a tile) and the MMAs
-// (~44 %); two CTAs per SM would hide one behind the other, but a 128-wide level does not fit twice (TMEM columns, 96 KB of
-// weights).  This kernel gets the overlap inside ONE CTA:
-//   * two independent ROW GROUPS of 8 warps, each with its own 128-row tile, its own 256 TMEM columns, its own MMA
-//     issuer (thread 0 of the group), mbarriers, named barrier and tile claims; while one group gathers / pools, the
-//     other group's MMAs run;
-//   * the weights of the inner layer are resident ONCE and shared by both groups; a last layer that does not fit is
-//     streamed per group, one 64-channel tile (48 KB) at a time, L2 -> shared memory during the previous epilogue;
-//   * operands are split into NP 16-bit pieces each (Split<NP>): the A operand of a K = 128 layer is 64 NP TMEM columns, so that
-//     A + a 64-column D (two of them with NP = 2) fit in a group's 256; weights are 2 NP bytes per element.
-// ------------------------------------------------------------------------------------------------------------------
 constexpr int kImageBf16x3 = 0x100;      // flags in psa_mlp.image_nt / psa_mlp_image_plan: image holds three bf16 pieces ..
 constexpr int kImageF16x2 = 0x200;       // .. or two fp16 pieces
 constexpr int kImageFlags = kImageBf16x3 | kImageF16x2;
@@ -155,661 +137,280 @@ __global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float
     if (NP == 2 && f16x2_overflowed(ovf)) atomicOr(trailer, 1u);
 }
 
-struct TcDual {
-    static constexpr int kThreads = 512, kGroupThreads = 256, kGroupCols = 256, kNt = 64;
-    static constexpr uint32_t D = 0, A1 = 64, A2 = 128, A3 = 192;
-};
+// ------------------------------------------------------------------------------------------------------------------
+// tc_sa_kernel -- one set-abstraction level (e.g. PointNet++ SA2: 131 -> 128 -> 128 -> 256 over 64-point neighbourhoods).
+//   CTA = 256 threads = two warpgroups = one 128-row tile (128 / K neighbourhoods) at a time, tiles claimed dynamically
+//   (persistent CTAs; a CTA that starts late or shares its SM with another stream simply takes fewer).
+//   * layer 1 on the FMA pipe: each thread evaluates U[j] + (x_j - c) . Wx (+ c . Wc), the folded affine and ReLU for the
+//     rows and channels of ITS A fragment and splits the result into NP pieces -- straight into registers;
+//   * inner tensor layers: wgmma with A from registers, B = weight image in shared memory; the D fragment goes through
+//     affine + ReLU + split and is the next layer's A fragment (same register layout), nothing is staged;
+//   * last layer in 64-channel chunks: wgmma, affine + ReLU, max over each neighbourhood's rows (in-thread, shuffles across
+//     the warp, shared memory across warps), coalesced (B,m,C_out) stores.
+//   Weights of every layer are resident in shared memory (one TMA bulk load per CTA); a last layer that does not fit next to
+//   the others is streamed one 64-channel chunk at a time through a two-slot ring, one chunk ahead.
+// ------------------------------------------------------------------------------------------------------------------
+constexpr int kSaNt = 64;                        // tile width of the SA weight images
+constexpr int kSaThreads = 256;
+constexpr uint32_t kSmemBudget = 220u * 1024u;   // dynamic shared memory (incl. 1 KB alignment) next to the static arrays
 
-__device__ __forceinline__ void group_bar(int g) { asm volatile("bar.sync %0, 256;\n" ::"r"(g + 1) : "memory"); }
-
-// split 32 activations into NP pieces and store them as 16 columns each at a1, a1 + ps, .. (h is clobbered)
-template <int NP>
-__device__ __forceinline__ void store_a_at(uint32_t a1, float (&h)[32], uint32_t ps, uint32_t& ovf) {
-    uint32_t p[16];
-    if constexpr (NP == 3) {
-        (void)ovf;
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_bf16x2(h[2 * q], h[2 * q + 1]);
-            h[2 * q] -= __uint_as_float(p[q] << 16);
-            h[2 * q + 1] -= __uint_as_float(p[q] & 0xffff0000u);
-        }
-        tmem_st16(a1, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_bf16x2(h[2 * q], h[2 * q + 1]);
-            h[2 * q] -= __uint_as_float(p[q] << 16);
-            h[2 * q + 1] -= __uint_as_float(p[q] & 0xffff0000u);
-        }
-        tmem_st16(a1 + ps, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) p[q] = pack_bf16x2(h[2 * q], h[2 * q + 1]);
-        tmem_st16(a1 + 2 * ps, p);
-    } else {
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_f16x2(h[2 * q], h[2 * q + 1]);
-            track_f16x2(ovf, p[q]);
-            const float2 f = unpack_f16x2(p[q]);
-            h[2 * q] -= f.x;
-            h[2 * q + 1] -= f.y;
-        }
-        tmem_st16(a1, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) p[q] = pack_f16x2(h[2 * q], h[2 * q + 1]);
-        tmem_st16(a1 + ps, p);
-    }
-}
-
-// the same for activations held as 16 float2 (the dual kernel's row work runs on the packed FFMA2 / FADD2 pipe: two channels per
-// instruction); the fp16 residual h - f32(a1) is one FFMA2 with (-1, -1)
-template <int NP>
-__device__ __forceinline__ void store_a2_at(uint32_t a1, float2 (&h)[16], uint32_t ps, uint32_t& ovf) {
-    uint32_t p[16];
-    if constexpr (NP == 3) {
-        (void)ovf;
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_bf16x2(h[q].x, h[q].y);
-            h[q].x -= __uint_as_float(p[q] << 16);
-            h[q].y -= __uint_as_float(p[q] & 0xffff0000u);
-        }
-        tmem_st16(a1, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_bf16x2(h[q].x, h[q].y);
-            h[q].x -= __uint_as_float(p[q] << 16);
-            h[q].y -= __uint_as_float(p[q] & 0xffff0000u);
-        }
-        tmem_st16(a1 + ps, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) p[q] = pack_bf16x2(h[q].x, h[q].y);
-        tmem_st16(a1 + 2 * ps, p);
-    } else {
-        const float2 neg1 = make_float2(-1.f, -1.f);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) {
-            p[q] = pack_f16x2(h[q].x, h[q].y);
-            track_f16x2(ovf, p[q]);
-            h[q] = __ffma2_rn(unpack_f16x2(p[q]), neg1, h[q]);       // exact: a product with -1, then one rounding of the difference
-        }
-        tmem_st16(a1, p);
-#pragma unroll
-        for (int q = 0; q < 16; ++q) p[q] = pack_f16x2(h[q].x, h[q].y);
-        tmem_st16(a1 + ps, p);
-    }
-}
-
-// tmode: 32 activations of row `row` (input channels [k0, k0 + 32)) split into NP pieces and written as the B operand of the transposed
-// last layer: [128 rows][64 k] K-major SWIZZLE_128B per piece (16 KB), four 16-byte chunks per piece (conflict-free per quarter warp)
-template <int NP>
-__device__ __forceinline__ void store_h_smem(uint8_t* hbase, int row, int k0, float2 (&h)[16], uint32_t& ovf) {
-    static_assert(NP == 2, "the transposed mode is instantiated for fp16x2 operands");
-    uint32_t p[16];
-    const float2 neg1 = make_float2(-1.f, -1.f);
-    const uint32_t rbase = (uint32_t)(row >> 3) * 1024u + (uint32_t)(row & 7) * 128u;
-#pragma unroll
-    for (int q = 0; q < 16; ++q) {
-        p[q] = pack_f16x2(h[q].x, h[q].y);
-        track_f16x2(ovf, p[q]);
-        h[q] = __ffma2_rn(unpack_f16x2(p[q]), neg1, h[q]);
-    }
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(hbase + rbase + ((((uint32_t)(k0 >> 3) + j) ^ (uint32_t)(row & 7)) << 4)) = make_uint4(p[4 * j], p[4 * j + 1], p[4 * j + 2], p[4 * j + 3]);
-#pragma unroll
-    for (int q = 0; q < 16; ++q) p[q] = pack_f16x2(h[q].x, h[q].y);
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<uint4*>(hbase + 16384u + rbase + ((((uint32_t)(k0 >> 3) + j) ^ (uint32_t)(row & 7)) << 4)) =
-            make_uint4(p[4 * j], p[4 * j + 1], p[4 * j + 2], p[4 * j + 3]);
-}
-
-// issuer warp (converged): D[128 x NT_] (+)= sum over the piece pairs of Split<NP>, KC blocks of 64 input channels.
-// a1_col: TMEM column of piece 1 of the A operand (pieces PS columns apart); d_col: accumulator (overwritten by the first MMA).
-template <int KC, int NT_, int PS, int NP>
-__device__ __forceinline__ void issue_tile_c(uint32_t tmem_base, uint32_t d_col, uint32_t a1_col, uint32_t blocks_addr) {
-    constexpr uint32_t bb = NT_ * 128u * NP, piece = NT_ * 128u;
-    const uint32_t tb = warp_uniform(tmem_base);
-    const uint32_t d = tb + d_col;
-    const uint32_t a1 = tb + a1_col;
-    const uint32_t idesc = make_idesc(Split<NP>::kFmt, 128, NT_);
-    const SmemDescBase b0 = smem_desc_base(warp_uniform(blocks_addr));
-#pragma unroll
-    for (int t = 0; t < Split<NP>::kTerms; ++t)
-#pragma unroll
-        for (int kc = 0; kc < KC; ++kc)
-#pragma unroll
-            for (int s4 = 0; s4 < 4; ++s4)
-                mma_bf16_ts(d, a1 + Split<NP>::a(t) * PS + kc * 32 + s4 * 8, smem_desc_at(b0, kc * bb + Split<NP>::w(t) * piece + s4 * 32), idesc,
-                            (t | kc | s4) ? 1u : 0u);
-}
-// TMEM columns of a row group (256), by D-buffering mode DB:
-//   0  one D slot:            D 0..63 | A pieces 64 columns apart from 64
-//   1  levels whose layers are all <= 64 wide: D slots 0 and 64 | A pieces 32 columns apart from 128
-//   2  two-piece operands (NP = 2) of 128-wide layers leave 192..255 free: D slots 0 and 192 | A pieces at 64 and 128
-//   3  64-wide levels whose last layer is 128 wide, NP = 2: inner layer as in mode 1 (D 0..63, A pieces from 128); the LAST layer runs
-//      transposed, D^T[128 channels][128 rows] at 0..127 = W^T (A operand, shared memory) x H^T (B operand, shared memory, written by
-//      the previous epilogue) -- lane = channel: the max-pool is an in-thread reduction, the affine a per-thread scalar, the output
-//      store a coalesced 128-byte row segment
-template <int DB> __device__ __forceinline__ constexpr uint32_t dual_dcol(int dslot) { return dslot == 0 ? 0u : (DB == 2 ? 192u : 64u); }
-template <int NP, int DB>
-__device__ __forceinline__ void issue_tile(uint32_t gbase, uint32_t blocks_addr, int KC, int dslot) {
-    if constexpr (DB == 1 || DB == 3) {
-        if (dslot == 0) issue_tile_c<1, TcDual::kNt, 32, NP>(gbase, 0, 128, blocks_addr);
-        else issue_tile_c<1, TcDual::kNt, 32, NP>(gbase, 64, 128, blocks_addr);
-    } else if constexpr (DB == 2) {
-        if (KC == 1) {
-            if (dslot == 0) issue_tile_c<1, TcDual::kNt, 64, NP>(gbase, 0, TcDual::A1, blocks_addr);
-            else issue_tile_c<1, TcDual::kNt, 64, NP>(gbase, 192, TcDual::A1, blocks_addr);
-        } else {
-            if (dslot == 0) issue_tile_c<2, TcDual::kNt, 64, NP>(gbase, 0, TcDual::A1, blocks_addr);
-            else issue_tile_c<2, TcDual::kNt, 64, NP>(gbase, 192, TcDual::A1, blocks_addr);
-        }
-    } else {
-        if (KC == 1) issue_tile_c<1, TcDual::kNt, 64, NP>(gbase, TcDual::D, TcDual::A1, blocks_addr);
-        else issue_tile_c<2, TcDual::kNt, 64, NP>(gbase, TcDual::D, TcDual::A1, blocks_addr);
-    }
-}
-
-struct TcDualLayout {
-    uint32_t hbuf[2];            // tmode: per group, the last layer's B operand [128 rows][64 k] K-major SWIZZLE_128B, np pieces of 16 KB
+struct TcSaLayout {
     uint32_t w[kMaxTcLayers];    // resident layers
-    uint32_t ring[2];            // per-group ring (one 64-channel tile of the streamed last layer)
+    uint32_t ring[2];            // streamed last layer: one 64-channel chunk per slot
     uint32_t ring_bytes;
     uint32_t vec, total;
 };
 
-__host__ __device__ inline TcDualLayout tc_dual_layout(const TcArgs& a) {
-    TcDualLayout L;
+__host__ __device__ inline TcSaLayout tc_sa_layout(const TcArgs& a) {
+    TcSaLayout L;
     uint32_t off = 0;
-    for (int l = 0; l < a.nl; ++l) {
+#pragma unroll
+    for (int l = 0; l < kMaxTcLayers; ++l) {      // constant indices: the layout stays in registers inside the kernel
         L.w[l] = off;
-        if (!(a.stream_last && l == a.nl - 1)) off += (uint32_t)tc_image_bytes(a.Kd[l], a.Ntot[l], a.np);
+        if (l < a.nl && !(a.stream_last && l == a.nl - 1)) off += (uint32_t)tc_image_bytes(a.Kd[l], a.Ntot[l], a.np);
     }
-    L.ring_bytes = a.stream_last ? (uint32_t)(a.Kd[a.nl - 1] / 64) * tc_block_bytes(TcDual::kNt, a.np) : 0u;
+    L.ring_bytes = a.stream_last ? (uint32_t)(a.Kd[a.nl - 1] / 64) * tc_block_bytes(kSaNt, a.np) : 0u;
     L.ring[0] = off; off += L.ring_bytes;
     L.ring[1] = off; off += L.ring_bytes;
-    L.hbuf[0] = off; if (a.tmode) off += (uint32_t)a.np * 16384u;
-    L.hbuf[1] = off; if (a.tmode) off += (uint32_t)a.np * 16384u;
     L.vec = off;
-    off += 8u * a.C1 * 4u;       // w1x (3 C1), s1, t1, w1c (3 C1)
-    for (int l = 0; l < a.nl; ++l) off += 2u * a.Ntot[l] * 4u;
+    off += 8u * a.C1 * 4u;       // w1x (3 C1), w1c (3 C1), s1, t1
+#pragma unroll
+    for (int l = 0; l < kMaxTcLayers; ++l) off += l < a.nl ? 2u * a.Ntot[l] * 4u : 0u;
     L.total = off;
     return L;
 }
 
-// D chunk (32 columns of this lane's row) -> relu?(d * scale + shift).  Rows past the end of the problem need no masking: a row of D
-// depends on the same row of A only, validity is per NEIGHBOURHOOD (K divides the tile), and outputs of neighbourhoods past the end are
-// never stored; their layer-1 inputs are zeros, so they carry finite values (no spurious range flag either).
-__device__ __forceinline__ void affine_chunk(const uint32_t (&d)[32], const float* __restrict__ sc_, const float* __restrict__ sh_, int relu,
-                                             float2 (&h)[16]) {
-    const float4* s4 = reinterpret_cast<const float4*>(sc_);
-    const float4* t4 = reinterpret_cast<const float4*>(sh_);
+// thread 0: use q of the streamed last layer's ring = 64-channel chunk q % ncl into slot q & 1
+__device__ __forceinline__ void sa_fill_ring(uint32_t q, const uint8_t* image, int ncl, const TcSaLayout& L, uint8_t* base, uint64_t* bars) {
+    uint64_t* bar = &bars[q & 1];
+    mbar_expect_tx(bar, L.ring_bytes);
+    const uint8_t* src = image + (size_t)(q % (uint32_t)ncl) * L.ring_bytes;
+    for (uint32_t o = 0; o < L.ring_bytes; o += 32768u) bulk_g2s(base + L.ring[q & 1] + o, src + o, min(32768u, L.ring_bytes - o), bar);
+}
+
+// D[64 x 64 NCH] (+)= A . W over KS steps of 16 input channels, all piece pairs of Split<NP>: straight-line wgmma (no predicated
+// issue, so ptxas keeps the whole sequence asynchronous).  Output chunk c reads the weight blocks at wb + c * cstride.
+template <int NP, int KS, int NCH>
+__device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[NP][8][4], uint32_t wb, uint32_t cstride) {
+    constexpr uint32_t bb = tc_block_bytes(kSaNt, NP), piece = kSaNt * 128u;
+    wg_fence();
 #pragma unroll
-    for (int q = 0; q < 8; ++q) {
-        const float4 sc = s4[q], sh = t4[q];
-        float2 v0 = __ffma2_rn(make_float2(__uint_as_float(d[4 * q + 0]), __uint_as_float(d[4 * q + 1])), make_float2(sc.x, sc.y), make_float2(sh.x, sh.y));
-        float2 v1 = __ffma2_rn(make_float2(__uint_as_float(d[4 * q + 2]), __uint_as_float(d[4 * q + 3])), make_float2(sc.z, sc.w), make_float2(sh.z, sh.w));
-        if (relu) { v0.x = fmaxf(v0.x, 0.f); v0.y = fmaxf(v0.y, 0.f); v1.x = fmaxf(v1.x, 0.f); v1.y = fmaxf(v1.y, 0.f); }
-        h[2 * q] = v0; h[2 * q + 1] = v1;
-    }
+    for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+#pragma unroll
+        for (int s = 0; s < KS; ++s)
+#pragma unroll
+            for (int c = 0; c < NCH; ++c)
+                wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
+                              wg_desc(wb + (uint32_t)c * cstride + (uint32_t)(s >> 2) * bb + Split<NP>::w(tt) * piece + (uint32_t)(s & 3) * 32u),
+                              (tt | s) ? 1u : 0u);
+    wg_commit();
+    wg_wait_all();
+#pragma unroll
+    for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
 }
 
-// DBUF (levels whose layers are all <= 64 wide, nothing streamed): the A operand is 3 x 32 columns (at 128..), which leaves
-// room for two D slots (0, 64) -- the last layer's tiles are issued in pairs and the second tile's MMAs run under the
-// first tile's pooled epilogue.
-// The two row groups of a CTA have identical phase lengths, so left alone they run in lock-step: both in row work
-// (fighting for issue slots), then both in their MMA batch (each at half the tensor rate).  A token makes the batches
-// run one after the other: the first group finishes at full rate and its row work then overlaps the second group's
-// MMAs -- the groups fall into anti-phase.  Released right after the batch is ISSUED (the pipe executes in order).
-// (branch-free at the source level -- predicated atomics + a shuffle -- so the issuer warp's control flow stays uniform)
-__device__ __forceinline__ void pipe_acquire(int* token, int lane) {
-    (void)lane;
-    uint32_t busy;
-    do {
-        uint32_t r;
-        asm volatile(
-            "{\n\t.reg .pred q;\n\t"
-            "elect.sync _|q, 0xffffffff;\n\t"
-            "mov.b32 %0, 1;\n\t"
-            "@q atom.shared.cas.b32 %0, [%1], 0, 1;\n\t}\n"
-            : "=r"(r)
-            : "r"(smem_u32(token))
-            : "memory");
-        busy = __shfl_sync(0xffffffffu, r, 0);
-    } while (busy != 0u);
-    __syncwarp();
-}
-__device__ __forceinline__ void pipe_release(int* token, int lane) {
-    (void)lane;
-    asm volatile(
-        "{\n\t.reg .pred q;\n\t.reg .b32 t;\n\t"
-        "elect.sync _|q, 0xffffffff;\n\t"
-        "@q atom.shared.exch.b32 t, [%0], 0;\n\t}\n" ::"r"(smem_u32(token))
-        : "memory");
-}
-
-template <int DB, int NP>
-__global__ void __launch_bounds__(TcDual::kThreads, 1)
-tc_sa_dual_kernel(const __grid_constant__ TcArgs a) {
-    constexpr bool DBUF = DB != 0;
+// Specialised on the level shape: C1 = width of layer 1 (64 | 128), NL = tensor layers (1 | 2), N0 = width of the inner tensor
+// layer when NL = 2 (64 | 128).  The last layer's width is a runtime multiple of 64.
+template <int NP, int C1, int NL, int N0>
+__global__ void __launch_bounds__(kSaThreads, 1)
+tc_sa_kernel(const __grid_constant__ TcArgs a) {
+    static_assert((C1 == 64 || C1 == 128) && (NL == 1 || (NL == 2 && (N0 == 64 || N0 == 128))), "unsupported level shape");
+    constexpr int last = NL - 1;
+    constexpr int KSL = (NL == 2 ? N0 : C1) / 16;            // K steps of the last layer
     if (a.run_if != nullptr && *a.run_if == 0u) return;      // np = 3 rerun of a launch that stayed inside the fp16 range: nothing to do
-    constexpr int kNt = TcDual::kNt;
+    constexpr uint32_t bb = tc_block_bytes(kSaNt, NP);
     uint32_t ovf = 0u;                                        // np = 2: packed |max| of every leading piece this thread stores
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_mbar[2];  // MMA completion, per group
-    __shared__ __align__(8) uint64_t s_mbar2[2]; // MMA completion of the second D slot (dbuf levels), per group
-    __shared__ __align__(8) uint64_t s_wbar[2];  // ring tile landed, per group
-    __shared__ __align__(8) uint64_t s_rbar;     // resident weights landed
-    __shared__ uint32_t s_tmem;
-    __shared__ float s_red[TcDual::kThreads / 32][32];
-    __shared__ unsigned int s_tile[2][2];
-    __shared__ __align__(16) float4 s_geo[2][128];   // per group: (dx, dy, dz, source row) of the NEXT tile's rows, prefetched
-    __shared__ int s_token;                          // tensor-pipe token: the two groups' MMA batches run one after the other
-    __shared__ int s_nonneg;                         // every scale of the last layer >= 0: pool first, affine + ReLU after
+    __shared__ __align__(8) uint64_t s_rbar;                 // resident weights landed
+    __shared__ __align__(8) uint64_t s_wbar[2];              // ring slot landed
+    __shared__ float s_red[8][64];
+    __shared__ unsigned int s_tile;
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int warp_u = (int)warp_uniform((uint32_t)warp);
-    const int g = warp_u >> 3, gtid = tid & 255;
-    const bool issuer = (warp_u & 7) == 0;    // first warp of each group: converged MMA issue (tc_common.cuh), ring refills
-    const int quarter = warp_u & 3, cs = (warp_u >> 2) & 1;
-    const int row = quarter * 32 + lane;
+    const int g = lane >> 2, t = lane & 3;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const TcDualLayout L = tc_dual_layout(a);
-    const int last = a.nl - 1;
+    const TcSaLayout L = tc_sa_layout(a);
 
-    if (warp == 0) tmem_alloc(&s_tmem, 512);
-    if (tid == 0) {
-        mbar_init(&s_mbar[0], 1); mbar_init(&s_mbar[1], 1); mbar_init(&s_mbar2[0], 1); mbar_init(&s_mbar2[1], 1); mbar_init(&s_wbar[0], 1); mbar_init(&s_wbar[1], 1); mbar_init(&s_rbar, 1);
-        fence_mbar_init();
-    }
     float* vec = reinterpret_cast<float*>(base + L.vec);
     float* w1x = vec;
-    float* s1 = vec + 3 * a.C1;
-    float* t1 = s1 + a.C1;
-    float* sl[kMaxTcLayers];
-    float* tl[kMaxTcLayers];
-    {
-        float* p = t1 + 4 * a.C1;
-        for (int l = 0; l < a.nl; ++l) { sl[l] = p; tl[l] = p + a.Ntot[l]; p += 2 * a.Ntot[l]; }
-    }
-    float* w1c = t1 + a.C1;
-    // the BN scale of layer 1 is folded into its xyz / centre weights (s (U + d.W) + t = (s U + t) + d.(s W)): one FFMA2 less per channel
-    // pair and, for levels without input features, no accumulator to clear
-    for (int i = tid; i < 3 * a.C1; i += TcDual::kThreads) {
-        const float sc = a.s1 ? __ldg(a.s1 + i % a.C1) : 1.f;
+    float* w1c = vec + 3 * C1;
+    float* s1 = vec + 6 * C1;
+    float* t1 = s1 + C1;
+    float* sl0 = t1 + C1;                                     // scale / shift of tensor layer 0 ..
+    float* tl0 = sl0 + a.Ntot[0];
+    float* slL = NL == 2 ? tl0 + a.Ntot[0] : sl0;             // .. and of the last one
+    float* tlL = slL + a.Ntot[last];
+    // the BN scale of layer 1 is folded into its xyz / centre weights: s (U + d.W) + t = (s U + t) + d.(s W)
+    for (int i = tid; i < 3 * C1; i += kSaThreads) {
+        const float sc = a.s1 ? __ldg(a.s1 + i % C1) : 1.f;
         w1x[i] = __ldg(a.w1x + i) * sc;
         w1c[i] = a.w1c ? __ldg(a.w1c + i) * sc : 0.f;
     }
-    for (int i = tid; i < a.C1; i += TcDual::kThreads) { s1[i] = a.s1 ? __ldg(a.s1 + i) : 1.f; t1[i] = __ldg(a.t1 + i); }
-    if (tid == 0) { s_nonneg = 1; s_token = 0; }
-    __syncthreads();
-    for (int l = 0; l < a.nl; ++l)
-        for (int i = tid; i < a.Ntot[l]; i += TcDual::kThreads) {
-            sl[l][i] = a.s[l] ? __ldg(a.s[l] + i) : 1.f;
-            tl[l][i] = __ldg(a.t[l] + i);
-            if (l == last && !(sl[l][i] >= 0.f)) s_nonneg = 0;
+    for (int i = tid; i < C1; i += kSaThreads) { s1[i] = a.s1 ? __ldg(a.s1 + i) : 1.f; t1[i] = __ldg(a.t1 + i); }
+#pragma unroll
+    for (int l = 0; l < NL; ++l)
+        for (int i = tid; i < a.Ntot[l]; i += kSaThreads) {
+            (l == 0 ? sl0 : slL)[i] = a.s[l] ? __ldg(a.s[l] + i) : 1.f;
+            (l == 0 ? tl0 : tlL)[i] = __ldg(a.t[l] + i);
         }
-    __syncthreads();
     if (tid == 0) {
-        uint32_t total = 0;
-        for (int l = 0; l < a.nl; ++l)
-            if (!(a.stream_last && l == last)) total += (uint32_t)tc_image_bytes(a.Kd[l], a.Ntot[l], NP);
-        if (total) {
-            mbar_expect_tx(&s_rbar, total);
-            for (int l = 0; l < a.nl; ++l) {
+        mbar_init(&s_rbar, 1); mbar_init(&s_wbar[0], 1); mbar_init(&s_wbar[1], 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    const int NCL = a.Ntot[last] / 64;                        // 64-channel chunks of the last layer
+    uint32_t resident = 0;
+#pragma unroll
+    for (int l = 0; l < NL; ++l)
+        if (!(a.stream_last && l == last)) resident += (uint32_t)tc_image_bytes(a.Kd[l], a.Ntot[l], NP);
+    if (tid == 0) {
+        if (resident) {
+            mbar_expect_tx(&s_rbar, resident);
+#pragma unroll
+            for (int l = 0; l < NL; ++l) {
                 if (a.stream_last && l == last) continue;
                 const uint32_t bytes = (uint32_t)tc_image_bytes(a.Kd[l], a.Ntot[l], NP);
                 for (uint32_t o = 0; o < bytes; o += 32768u) bulk_g2s(base + L.w[l] + o, a.image[l] + o, min(32768u, bytes - o), &s_rbar);
             }
-            mbar_wait(&s_rbar, 0);
         }
+        if (a.stream_last) { sa_fill_ring(0, a.image[last], NCL, L, base, s_wbar); sa_fill_ring(1, a.image[last], NCL, L, base, s_wbar); }
     }
-    // ring protocol: one fill outstanding or landed before every issue of the streamed layer
-    uint32_t wphase = 0;
-    if (issuer && a.stream_last && lane == 0) {
-        mbar_expect_tx(&s_wbar[g], L.ring_bytes);
-        for (uint32_t o = 0; o < L.ring_bytes; o += 32768u) bulk_g2s(base + L.ring[g] + o, a.image[last] + o, min(32768u, L.ring_bytes - o), &s_wbar[g]);
-    }
-    fence_before_thread_sync();
-    __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = warp_uniform(s_tmem) + (uint32_t)g * TcDual::kGroupCols;
-    const uint32_t row_taddr = tmem_base + ((uint32_t)(quarter * 32) << 16);
-    uint32_t phase = 0, phase2 = 0;
-    constexpr uint32_t a1_col = (DB == 1 || DB == 3) ? 128u : TcDual::A1, a_ps = (DB == 1 || DB == 3) ? 32u : 64u;
-    uint8_t* hbuf = base + L.hbuf[g];           // DB == 3: B operand of the transposed last layer
-    const bool pool_first = s_nonneg != 0;    // relu(s*d + t) is non-decreasing in d when s >= 0: max over rows commutes with it
-    bool have_geo = false;                    // s_geo[g] holds this tile's geometry (written during the previous tile)
+    uint32_t q_used = 0;                                      // ring uses consumed (fills issued: q_used + 2)
+    if (resident) mbar_wait(&s_rbar, 0);
 
-    const int G = 128 / a.K;
+    const int K = a.K, G = 128 / K;
     const long long ntiles = (a.groups + G - 1) / G;
-    if (gtid == 0) s_tile[g][0] = atomicAdd(a.tile_counter, 1u);
-    group_bar(g);
-    int tpar = 0;
-#ifdef PSA_TC_TIMING
-    unsigned long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long tprev = clock64();
-#endif
-    for (long long tile = warp_uniform(s_tile[g][0]); tile < ntiles; tile = warp_uniform(s_tile[g][tpar])) {
-#ifdef PSA_TC_TIMING
-        if (tid == 0) tacc[7] += 1;
-#endif
-        long long next_tile = 0;
-        if (gtid == 0) { const unsigned int t = atomicAdd(a.tile_counter, 1u); s_tile[g][tpar ^ 1] = t; next_tile = t; }
-        tpar ^= 1;
+    const int rl[2] = {warp * 16 + g, warp * 16 + g + 8};     // this thread's two tile rows
+    for (;;) {
+        if (tid == 0) s_tile = atomicAdd(a.tile_counter, 1u);
+        __syncthreads();
+        const long long tile = (long long)s_tile;
+        if (tile >= ntiles) break;
         const long long g0 = tile * G;
-        const long long gid = g0 + row / a.K;
-        const bool valid = gid < a.groups;
-        // ---- layer 1 on the FMA pipe, straight into the A operand ----
+
+        // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
+        uint32_t A[NP][8][4];
         {
-            float dx = 0.f, dy = 0.f, dz = 0.f;
-            float cx = 0.f, cy = 0.f, cz = 0.f;
-            const float* urow = nullptr;
-            if (a.w1c != nullptr && valid) {
-                const float* c = a.new_xyz + (size_t)gid * 3;
-                cx = __ldg(c); cy = __ldg(c + 1); cz = __ldg(c + 2);
+            float dx[2], dy[2], dz[2], cx[2], cy[2], cz[2];
+            const float* urow[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const long long gid = g0 + rl[i] / K;
+                dx[i] = dy[i] = dz[i] = cx[i] = cy[i] = cz[i] = 0.f;
+                urow[i] = nullptr;
+                if (gid < a.groups) {
+                    const long long bi = gid / a.m;
+                    const int j = __ldg(a.idx + gid * K + (rl[i] % K));
+                    const float* p = a.xyz + ((size_t)bi * a.n + j) * 3;
+                    const float* c = a.new_xyz + (size_t)gid * 3;
+                    cx[i] = __ldg(c); cy[i] = __ldg(c + 1); cz[i] = __ldg(c + 2);
+                    dx[i] = __ldg(p) - cx[i]; dy[i] = __ldg(p + 1) - cy[i]; dz[i] = __ldg(p + 2) - cz[i];
+                    if (a.uf) urow[i] = a.uf + ((size_t)bi * a.n + j) * C1;
+                }
             }
-            if (have_geo) {
-                const float4 gq = s_geo[g][row];
-                dx = gq.x; dy = gq.y; dz = gq.z;
-                if (a.uf && valid) urow = a.uf + (size_t)__float_as_int(gq.w) * a.C1;
-            } else if (valid) {
-                const long long bi = gid / a.m;
-                const int j = __ldg(a.idx + gid * a.K + (row % a.K));
-                const float* p = a.xyz + ((size_t)bi * a.n + j) * 3;
-                const float* c = a.new_xyz + (size_t)gid * 3;
-                dx = __ldg(p) - __ldg(c); dy = __ldg(p + 1) - __ldg(c + 1); dz = __ldg(p + 2) - __ldg(c + 2);
-                if (a.uf) urow = a.uf + ((size_t)bi * a.n + j) * a.C1;
-            }
-            const float2 dx2 = make_float2(dx, dx), dy2 = make_float2(dy, dy), dz2 = make_float2(dz, dz);
-            for (int ch = cs; ch < a.C1 / 32; ch += 2) {
-                float2 h[16];                         // 32 channels, two per register pair: the chain below runs on the FFMA2 pipe
-                const float4* s4 = reinterpret_cast<const float4*>(s1 + ch * 32);
-                const float4* t4 = reinterpret_cast<const float4*>(t1 + ch * 32);
-                if (urow) {
 #pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const float4 u = __ldg(reinterpret_cast<const float4*>(urow + ch * 32) + q);
-                        const float4 sc = s4[q], sh = t4[q];
-                        h[2 * q] = __ffma2_rn(make_float2(u.x, u.y), make_float2(sc.x, sc.y), make_float2(sh.x, sh.y));
-                        h[2 * q + 1] = __ffma2_rn(make_float2(u.z, u.w), make_float2(sc.z, sc.w), make_float2(sh.z, sh.w));
+            for (int s = 0; s < C1 / 16; ++s) {
+                {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int k = 16 * s + 8 * h + 2 * t;
+                        const float2 sc = *reinterpret_cast<const float2*>(s1 + k), sh = *reinterpret_cast<const float2*>(t1 + k);
+                        const float2 wx = *reinterpret_cast<const float2*>(w1x + k), wy = *reinterpret_cast<const float2*>(w1x + C1 + k),
+                                     wz = *reinterpret_cast<const float2*>(w1x + 2 * C1 + k);
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            float2 v = urow[i] ? ffma2_rn(__ldg(reinterpret_cast<const float2*>(urow[i] + k)), sc, sh) : sh;
+                            if (a.w1c != nullptr) {        // EdgeConv: the part of the first layer that acts on the centre x_i
+                                const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
+                                             cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
+                                v = ffma2_rn(make_float2(cz[i], cz[i]), cwz, ffma2_rn(make_float2(cy[i], cy[i]), cwy, ffma2_rn(make_float2(cx[i], cx[i]), cwx, v)));
+                            }
+                            v = ffma2_rn(make_float2(dz[i], dz[i]), wz, ffma2_rn(make_float2(dy[i], dy[i]), wy, ffma2_rn(make_float2(dx[i], dx[i]), wx, v)));
+                            if (a.relu1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+                            put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);     // rows past the end carry finite values, never stored
+                        }
                     }
-                } else {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const float4 sh = t4[q];
-                        h[2 * q] = make_float2(sh.x, sh.y); h[2 * q + 1] = make_float2(sh.z, sh.w);
-                    }
-                }
-                if (a.w1c != nullptr) {       // EdgeConv: the part of the first layer that acts on the centre x_i
-                    const float2 cx2 = make_float2(cx, cx), cy2 = make_float2(cy, cy), cz2 = make_float2(cz, cz);
-                    const float4* cx4 = reinterpret_cast<const float4*>(w1c + ch * 32);
-                    const float4* cy4 = reinterpret_cast<const float4*>(w1c + a.C1 + ch * 32);
-                    const float4* cz4 = reinterpret_cast<const float4*>(w1c + 2 * a.C1 + ch * 32);
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const float4 wx = cx4[q], wy = cy4[q], wz = cz4[q];
-                        h[2 * q] = __ffma2_rn(cz2, make_float2(wz.x, wz.y), __ffma2_rn(cy2, make_float2(wy.x, wy.y), __ffma2_rn(cx2, make_float2(wx.x, wx.y), h[2 * q])));
-                        h[2 * q + 1] = __ffma2_rn(cz2, make_float2(wz.z, wz.w),
-                                                  __ffma2_rn(cy2, make_float2(wy.z, wy.w), __ffma2_rn(cx2, make_float2(wx.z, wx.w), h[2 * q + 1])));
-                    }
-                }
-                const float4* wx4 = reinterpret_cast<const float4*>(w1x + ch * 32);
-                const float4* wy4 = reinterpret_cast<const float4*>(w1x + a.C1 + ch * 32);
-                const float4* wz4 = reinterpret_cast<const float4*>(w1x + 2 * a.C1 + ch * 32);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) {
-                    const float4 wx = wx4[q], wy = wy4[q], wz = wz4[q];
-                    float2 v0 = __ffma2_rn(dz2, make_float2(wz.x, wz.y), __ffma2_rn(dy2, make_float2(wy.x, wy.y), __ffma2_rn(dx2, make_float2(wx.x, wx.y), h[2 * q])));
-                    float2 v1 = __ffma2_rn(dz2, make_float2(wz.z, wz.w),
-                                           __ffma2_rn(dy2, make_float2(wy.z, wy.w), __ffma2_rn(dx2, make_float2(wx.z, wx.w), h[2 * q + 1])));
-                    if (a.relu1) { v0.x = fmaxf(v0.x, 0.f); v0.y = fmaxf(v0.y, 0.f); v1.x = fmaxf(v1.x, 0.f); v1.y = fmaxf(v1.y, 0.f); }
-                    h[2 * q] = v0; h[2 * q + 1] = v1;                    // rows past the end: see affine_chunk
-                }
-                if constexpr (DB == 3) {
-                    if (a.nl == 1) store_h_smem<NP>(hbuf, row, ch * 32, h, ovf);      // layer 1 feeds the transposed layer directly
-                    else store_a2_at<NP>(row_taddr + a1_col + ch * 16, h, a_ps, ovf);
-                } else {
-                    store_a2_at<NP>(row_taddr + a1_col + ch * 16, h, a_ps, ovf);
                 }
             }
         }
-        if constexpr (DB == 3) fence_proxy_async_smem();
-        tmem_st_wait();
-        fence_before_thread_sync();
-        group_bar(g);
-        TC_STAMP(0);
-        for (int l = 0; l < a.nl; ++l) {
-            const int NT = (int)warp_uniform((uint32_t)a.Ntot[l]) / kNt, KC = (int)warp_uniform((uint32_t)a.Kd[l]) / 64;
-            if (l != last) {
-                // inner layer, one or two 64-wide tiles: the next A operand may only be written once ALL MMAs of this
-                // layer are done reading the current one, so the first tile's activations wait in registers
-                float2 h0[16], h1[16];
-                for (int nt = 0; nt < NT; ++nt) {
-                    if (issuer) {
-                        pipe_acquire(&s_token, lane);
-                        fence_after_thread_sync();
-                        issue_tile<NP, DB>(tmem_base, smem_u32(base + L.w[l]) + (uint32_t)nt * KC * tc_block_bytes(kNt, NP), KC, 0);
-                        mma_commit(&s_mbar[g]);
-                        pipe_release(&s_token, lane);
+
+        if constexpr (NL == 2) {
+            // ---- inner layer (N0 wide): D fragments -> affine + ReLU -> A fragments of the last layer ----
+            constexpr int NCH = N0 / 64;
+            float d[NCH][32];
+            sa_mma<NP, C1 / 16, NCH>(d, A, smem_u32(base + L.w[0]), (uint32_t)(C1 / 64) * bb);
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int j = 2 * jj + h, col = c * 64 + 8 * j + 2 * t;
+                        const float sc0 = sl0[col], sc1 = sl0[col + 1], sh0 = tl0[col], sh1 = tl0[col + 1];
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            float v0 = fmaf(d[c][4 * j + 2 * i], sc0, sh0), v1 = fmaf(d[c][4 * j + 2 * i + 1], sc1, sh1);
+                            if (a.relu[0]) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+                            put_a<NP, 8>(A, c * 4 + jj, i + 2 * h, v0, v1, ovf);
+                        }
                     }
-                    TC_STAMP(1);
-                    mbar_wait(&s_mbar[g], phase);
-                    phase ^= 1u;
-                    fence_after_thread_sync();
-                    TC_STAMP(2);
-                    uint32_t d[32];
-                    tmem_ld32(row_taddr + TcDual::D + cs * 32, d);
-                    tmem_ld_wait();
-                    if (nt == 0) affine_chunk(d, sl[l] + cs * 32, tl[l] + cs * 32, a.relu[l], h0);
-                    else affine_chunk(d, sl[l] + kNt + cs * 32, tl[l] + kNt + cs * 32, a.relu[l], h1);
-                    if (nt + 1 < NT) { fence_before_thread_sync(); group_bar(g); }       // D drained before the next tile lands in it
                 }
-                if constexpr (DB == 3) {
-                    store_h_smem<NP>(hbuf, row, cs * 32, h0, ovf);                    // NT == 1: the inner layer of this mode is 64 wide
-                    fence_proxy_async_smem();
+            }
+        }
+        {
+            // ---- last layer, 64 output channels at a time, max-pooled over each neighbourhood ----
+            const int N = a.Ntot[last];
+            for (int nc = 0; nc < NCL; ++nc) {
+                uint32_t wb;
+                if (a.stream_last) {
+                    mbar_wait(&s_wbar[q_used & 1], (q_used >> 1) & 1u);
+                    wb = smem_u32(base + L.ring[q_used & 1]);
                 } else {
-                    store_a2_at<NP>(row_taddr + a1_col + cs * 16, h0, a_ps, ovf);
-                    if (NT == 2) store_a2_at<NP>(row_taddr + a1_col + (2 + cs) * 16, h1, a_ps, ovf);
+                    wb = smem_u32(base + L.w[last]) + (uint32_t)(nc * (KSL / 4)) * bb;
                 }
-                tmem_st_wait();
-                fence_before_thread_sync();
-                group_bar(g);
-                TC_STAMP(3);
-            } else if constexpr (DB == 3) {
-                // ---- last layer, transposed: D^T[128 ch][128 rows] = W^T . H^T, both operands from shared memory ----
-                if (issuer) {
-                    pipe_acquire(&s_token, lane);
-                    fence_after_thread_sync();
-                    const uint32_t idesc = make_idesc(Split<NP>::kFmt, 128, 128);
-                    const SmemDescBase wa = smem_desc_base(warp_uniform(smem_u32(base + L.w[l])));
-                    const SmemDescBase hb = smem_desc_base(warp_uniform(smem_u32(hbuf)));
-                    const uint32_t dT = warp_uniform(tmem_base);
+                float d[1][32];
+                sa_mma<NP, KSL, 1>(d, A, wb, 0u);
 #pragma unroll
-                    for (int t = 0; t < Split<NP>::kTerms; ++t)
+                for (int j = 0; j < 8; ++j) {
 #pragma unroll
-                        for (int s4 = 0; s4 < 4; ++s4)
-                            mma_bf16_ss(dT, smem_desc_at(wa, Split<NP>::w(t) * 16384u + s4 * 32), smem_desc_at(hb, Split<NP>::a(t) * 16384u + s4 * 32), idesc,
-                                        (t | s4) ? 1u : 0u);
-                    mma_commit(&s_mbar[g]);
-                    pipe_release(&s_token, lane);
-                }
-                TC_STAMP(4);
-                {
-                    // the next tile's index -> point -> offset chain (two dependent L2 round trips) runs under these MMAs
-                    const long long ntile = (long long)s_tile[g][tpar];
-                    have_geo = ntile < ntiles;
-                    if (have_geo && cs == 0) {
-                        const long long ngid = ntile * G + row / a.K;
-                        float4 gq = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (ngid < a.groups) {
-                            const long long bi = ngid / a.m;
-                            const int j = __ldg(a.idx + ngid * a.K + (row % a.K));
-                            const float* p = a.xyz + ((size_t)bi * a.n + j) * 3;
-                            const float* c = a.new_xyz + (size_t)ngid * 3;
-                            gq.x = __ldg(p) - __ldg(c); gq.y = __ldg(p + 1) - __ldg(c + 1); gq.z = __ldg(p + 2) - __ldg(c + 2);
-                            gq.w = __int_as_float((int)(bi * a.n + j));
-                        }
-                        s_geo[g][row] = gq;
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = nc * 64 + 8 * j + 2 * t + e;
+                        const float sc = slL[col], sh = tlL[col];
+                        float lo = fmaf(d[0][4 * j + e], sc, sh), hi = fmaf(d[0][4 * j + 2 + e], sc, sh);
+                        if (a.relu[last]) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
+                        const float m = warp_rowmax16(lo, hi);
+                        if (g == 0) s_red[warp][8 * j + 2 * t + e] = m;
                     }
                 }
-                mbar_wait(&s_mbar[g], phase);
-                phase ^= 1u;
-                fence_after_thread_sync();
-                TC_STAMP(5);
-                {
-                    // lane = channel (32 quarter + lane); this warp's half of the rows = columns [64 cs, 64 cs + 64): 64 / K neighbourhoods
-                    const int chn = quarter * 32 + lane;
-                    const float sc = sl[l][chn], sh = tl[l][chn];
-                    const int npg = 64 / a.K;                                        // K = 32: two neighbourhoods per half, K = 64: one
-                    for (int j = 0; j < npg; ++j) {
-                        float mx = -FLT_MAX;
-                        for (int c = 0; c < a.K / 32; ++c) {
-                            uint32_t d[32];
-                            tmem_ld32(row_taddr + (uint32_t)(cs * 64 + j * a.K + c * 32), d);
-                            tmem_ld_wait();
-                            if (pool_first) {
-#pragma unroll
-                                for (int q = 0; q < 32; ++q) mx = fmaxf(mx, __uint_as_float(d[q]));
-                            } else {
-#pragma unroll
-                                for (int q = 0; q < 32; ++q) {
-                                    float v = fmaf(__uint_as_float(d[q]), sc, sh);
-                                    if (a.relu[l]) v = fmaxf(v, 0.f);
-                                    mx = fmaxf(mx, v);
-                                }
-                            }
-                        }
-                        if (pool_first) {
-                            mx = fmaf(mx, sc, sh);
-                            if (a.relu[l]) mx = fmaxf(mx, 0.f);
-                        }
-                        const long long og = g0 + cs * npg + j;
-                        if (og < a.groups) a.out[(size_t)og * a.Ntot[l] + chn] = mx;      // 32 lanes = 128 contiguous bytes
-                    }
+                __syncthreads();                                  // every warp's maxima are in s_red; ring slot consumed
+                if (a.stream_last) {
+                    if (tid == 0) sa_fill_ring(q_used + 2, a.image[last], NCL, L, base, s_wbar);
+                    ++q_used;
                 }
-                fence_before_thread_sync();
-                group_bar(g);
-                TC_STAMP(6);
-            } else {
-                const bool streamed = a.stream_last != 0;
-                const int quarters_per_group = a.K / 32;        // 1, 2 or 4
-                const long long wg = g0 + (quarter * 32) / a.K; // this warp's neighbourhood
-                // pooled epilogue of output tile `nt` out of D slot `dslot`
-                auto pooled_epilogue = [&](int nt, int dslot) {
-                    uint32_t d[32];
-                    tmem_ld32(row_taddr + (dslot == 0 ? dual_dcol<DB>(0) : dual_dcol<DB>(1)) + cs * 32, d);
-                    tmem_ld_wait();
-                    float v[32];
-                    if (pool_first) {
-#pragma unroll
-                        for (int q = 0; q < 32; ++q) v[q] = __uint_as_float(d[q]);
-                    } else {
-                        float2 v2[16];
-                        affine_chunk(d, sl[l] + nt * kNt + cs * 32, tl[l] + nt * kNt + cs * 32, a.relu[l], v2);
-#pragma unroll
-                        for (int q = 0; q < 16; ++q) { v[2 * q] = v2[q].x; v[2 * q + 1] = v2[q].y; }
-                    }
-                    float mx = warp_colmax_32x32(v, lane);
-                    if (quarters_per_group > 1) {
-                        s_red[warp][lane] = mx;
-                        group_bar(g);
-                        if ((quarter % quarters_per_group) == 0)
-                            for (int o = 1; o < quarters_per_group; ++o) mx = fmaxf(mx, s_red[warp + o][lane]);
-                    }
-                    if (pool_first) {
-                        mx = fmaf(mx, sl[l][nt * kNt + cs * 32 + lane], tl[l][nt * kNt + cs * 32 + lane]);
-                        if (a.relu[l]) mx = fmaxf(mx, 0.f);
-                    }
-                    if ((quarter % quarters_per_group) == 0 && wg < a.groups)
-                        a.out[(size_t)wg * a.Ntot[l] + nt * kNt + cs * 32 + lane] = mx;
-                };
-                constexpr int kStep = DBUF ? 2 : 1;
-                for (int nt = 0; nt < NT; nt += kStep) {
-                    if (issuer) {
-                        if (streamed) { mbar_wait(&s_wbar[g], wphase); wphase ^= 1u; }
-                        pipe_acquire(&s_token, lane);   // (ends in __syncwarp: the issue below must be warp-uniform)
-                        fence_after_thread_sync();
-                        const uint32_t blocks = streamed ? smem_u32(base + L.ring[g]) : smem_u32(base + L.w[l]) + (uint32_t)nt * KC * tc_block_bytes(kNt, NP);
-                        issue_tile<NP, DB>(tmem_base, blocks, KC, 0);
-                        mma_commit(&s_mbar[g]);
-                        if (DBUF) {                 // the pair's second tile goes to the other D slot right away (NT is even)
-                            issue_tile<NP, DB>(tmem_base, blocks + (uint32_t)KC * tc_block_bytes(kNt, NP), KC, 1);
-                            mma_commit(&s_mbar2[g]);
-                        }
-                        pipe_release(&s_token, lane);
-                    }
-                    TC_STAMP(4);
-                    if (nt + kStep >= NT) {
-                        // the next tile's index -> point -> offset chain (two dependent L2 round trips) runs under these MMAs
-                        const long long ntile = (long long)s_tile[g][tpar];
-                        have_geo = ntile < ntiles;
-                        if (have_geo && cs == 0) {
-                            const long long ngid = ntile * G + row / a.K;
-                            float4 gq = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (ngid < a.groups) {
-                                const long long bi = ngid / a.m;
-                                const int j = __ldg(a.idx + ngid * a.K + (row % a.K));
-                                const float* p = a.xyz + ((size_t)bi * a.n + j) * 3;
-                                const float* c = a.new_xyz + (size_t)ngid * 3;
-                                gq.x = __ldg(p) - __ldg(c); gq.y = __ldg(p + 1) - __ldg(c + 1); gq.z = __ldg(p + 2) - __ldg(c + 2);
-                                gq.w = __int_as_float((int)(bi * a.n + j));
-                            }
-                            s_geo[g][row] = gq;       // read after this tile's closing group barriers
-                        }
-                    }
-                    mbar_wait(&s_mbar[g], phase);
-                    phase ^= 1u;
-                    fence_after_thread_sync();
-                    TC_STAMP(5);
-                    if (issuer && streamed) {
-                        // the ring is free again: fetch the next tile (wrapping to tile 0 for the group's next row tile)
-                        const bool more = (nt + 1 < NT) || (__shfl_sync(0xffffffffu, next_tile, 0) < ntiles);
-                        if (more && lane == 0) {
-                            const int rt = (nt + 1) % NT;
-                            mbar_expect_tx(&s_wbar[g], L.ring_bytes);
-                            for (uint32_t o = 0; o < L.ring_bytes; o += 32768u)
-                                bulk_g2s(base + L.ring[g] + o, a.image[l] + (size_t)rt * L.ring_bytes + o, min(32768u, L.ring_bytes - o), &s_wbar[g]);
-                        }
-                    }
-                    pooled_epilogue(nt, 0);
-                    if (DBUF) {
-                        if (quarters_per_group > 1) group_bar(g);       // s_red is reused by the second tile
-                        mbar_wait(&s_mbar2[g], phase2);
-                        phase2 ^= 1u;
-                        fence_after_thread_sync();
-                        pooled_epilogue(nt + 1, 1);
-                    }
-                    // D fully read (and s_red consumed) by every warp of the group before the next MMAs / maxima land
-                    fence_before_thread_sync();
-                    group_bar(g);
-                    TC_STAMP(6);
+                if (tid < G * 64) {
+                    const int grp = tid >> 6, cl = tid & 63, wpg = K / 16;
+                    float mx = s_red[grp * wpg][cl];
+                    for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[grp * wpg + w][cl]);
+                    const long long og = g0 + grp;
+                    if (og < a.groups) a.out[(size_t)og * N + nc * 64 + cl] = mx;
                 }
+                __syncthreads();                                  // s_red is reused by the next chunk
             }
         }
     }
-#ifdef PSA_TC_TIMING
-    if (tid == 0)
-        for (int i = 0; i < 8; ++i) atomicAdd(&g_tc_timing[i], tacc[i]);
-#endif
     if constexpr (NP == 2) {
         if (f16x2_overflowed(ovf)) atomicOr(a.ovf, 1u);
         if (tid == 0)
-            for (int l = 0; l < a.nl; ++l)
+            for (int l = 0; l < NL; ++l)
                 if (a.wflag[l] != nullptr && *a.wflag[l] != 0u) atomicOr(a.ovf, 1u);
     }
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(s_tmem, 512);
+    if (tid == 0 && a.stream_last)                                    // the two fills issued ahead must land before the CTA exits
+        for (uint32_t q = q_used; q < q_used + 2; ++q) mbar_wait(&s_wbar[q & 1], (q >> 1) & 1u);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Dense layer on the tensor cores: out = relu?((x . W) * scale + shift), optional max over runs of pool_k rows.
-// CTA = 128 rows x Nt output channels.  K is walked in segments of 128: per segment the row warps quantise their x
-// chunk into the TMEM A operand, one thread issues the three-term MMAs against the segment's weight blocks (bulk-copied
-// into a two-slot shared-memory ring one segment ahead), and the segment's D is added to fp32 register accumulators --
-// so the truncating TMEM accumulation never runs over more than 128 K, however long the dot product is.
+// Dense layer on the tensor cores: out = relu?((x . W [+ xyz3 . w3]) * scale + shift), optional max over runs of pool_k rows.
 // ------------------------------------------------------------------------------------------------------------------
 struct TcDenseArgs {
     long long rows;
@@ -823,7 +424,7 @@ struct TcDenseArgs {
     const float* xyz3;     // optional side input (rows, 3): out += xyz3 . w3 before scale/shift (the xyz rows of a
     const float* w3;       // (3, N)                          [xyz, features] . W product, kept off the K loop)
     float* out;
-    // training-mode forward (tc_dense3 only): the input is relu(x * in_scale + in_shift) per INPUT channel (the previous layer's
+    // training-mode forward: the input is relu(x * in_scale + in_shift) per INPUT channel (the previous layer's
     // batch norm, applied while the operand is staged) and per-tile column statistics of the stored values are written
     const float* in_scale = nullptr;   // (K) or null
     const float* in_shift = nullptr;
@@ -835,496 +436,188 @@ struct TcDenseArgs {
     const unsigned int* wflag = nullptr;
 };
 
-// ------------------------------------------------------------------------------------------------------------------
-// tc_dense2_kernel -- the dense layer as a software pipeline.
-//   CTA = 128 rows x Nt output channels (Nt = 128, or 64 for a 64-wide layer), 17 warps, one CTA per SM:
-//   * 16 ROW warps (quarter = w & 3 -> TMEM lanes, slot = w >> 2 -> 32-column chunk) quantise their chunk of the next
-//     K = 128 segment of x into NP pieces in one of TWO A-operand buffers in TMEM, while
-//   * the ISSUER warp (converged, tc_common.cuh) waits for that buffer, the segment's weight blocks (cp.async.bulk
-//     into a two-slot shared-memory ring, refilled as soon as the MMAs that read a slot have completed) and for D to
-//     be drained, then issues the segment's MMAs (three or six terms) and commits;
-//   * the row warps add each segment's D to fp32 register accumulators (the truncating TMEM accumulation never runs
-//     over more than 128 K), then run the epilogue (affine, ReLU, xyz side input, max-pool).
-//   A-preparation of segment s+1 overlaps the MMAs of segment s; all hand-offs are mbarriers, no CTA-wide barrier
-//   inside the K loop.   TMEM: D 128 | A[0] 192 | A[1] 192 columns.
-// ------------------------------------------------------------------------------------------------------------------
-struct TcDense2 {
-    static constexpr int kRowWarps = 16, kThreads = 17 * 32;
-    static constexpr uint32_t D = 0, A0 = 128, ABUF = 192;     // A buffer b at A0 + b * ABUF, pieces 64 columns apart
-};
+// CTA = 256 threads = two warpgroups = 128 rows x Nt = 64 NC output channels.  K is walked in 64-wide blocks: the block's x is
+// read straight into A fragments (the previous layer's batch norm + ReLU applied on the fly in training mode) while its weight
+// block lands through a four-slot TMA ring; each block's wgmma sum is added to fp32 register accumulators, so the tensor core's
+// accumulation never runs over more than 64 K however long the dot product is.  Epilogue in the fragment layout: xyz side input,
+// affine, ReLU, then either float2 stores (+ per-tile column statistics) or the max over pool_k rows.
+constexpr int kDenseThreads = 256, kDenseStages = 4;
 
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(nthreads) : "memory"); }
-
-template <int NT_, int NP>
-__global__ void __launch_bounds__(TcDense2::kThreads, 1)
-tc_dense2_kernel(const __grid_constant__ TcDenseArgs a) {
+template <int NP, int NC>
+__global__ void __launch_bounds__(kDenseThreads, 1)
+tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
     if (a.run_if != nullptr && *a.run_if == 0u) return;
+    constexpr int Nt = 64 * NC;
+    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u;
     uint32_t ovf = 0u;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_wfull[2];     // weight slot landed (tx)
-    __shared__ __align__(8) uint64_t s_afull[2];     // A buffer written by all 16 row warps
-    __shared__ __align__(8) uint64_t s_mma;          // segment's MMAs complete
-    __shared__ __align__(8) uint64_t s_dfree;        // D drained by all 16 row warps
-    __shared__ uint32_t s_tmem;
-    __shared__ float s_red[TcDense2::kRowWarps][32];
-    __shared__ __align__(16) float s_vec[5][NT_];    // scale, shift, three xyz rows of W for this CTA's output channels
-    const int tid = threadIdx.x, lane = tid & 31;
-    const int warp_u = (int)warp_uniform((uint32_t)(tid >> 5));
+    __shared__ __align__(8) uint64_t s_wfull[kDenseStages];
+    __shared__ float s_red[2][8][Nt];
+    __shared__ __align__(16) float s_vec[5][Nt];     // scale, shift, three xyz rows of W for this CTA's output channels
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int g = lane >> 2, t = lane & 3;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int KCtot = a.Kp / 64;
-    constexpr uint32_t bb = NT_ * 128u * NP, slot_bytes = 2u * bb;
+    const int KC = a.Kp / 64;
     const int nt = blockIdx.y;
-    for (int i = tid; i < NT_; i += TcDense2::kThreads) {
-        const int c = nt * NT_ + i;
+    const long long row0 = (long long)blockIdx.x * 128;
+    const uint8_t* img = a.image + (size_t)nt * KC * bb;
+    for (int i = tid; i < Nt; i += kDenseThreads) {
+        const int c = nt * Nt + i;
         s_vec[0][i] = a.scale ? __ldg(a.scale + c) : 1.f;
         s_vec[1][i] = a.shift ? __ldg(a.shift + c) : 0.f;
         s_vec[2][i] = a.xyz3 ? __ldg(a.w3 + c) : 0.f;
         s_vec[3][i] = a.xyz3 ? __ldg(a.w3 + a.N + c) : 0.f;
         s_vec[4][i] = a.xyz3 ? __ldg(a.w3 + 2 * a.N + c) : 0.f;
     }
-    const long long row0 = (long long)blockIdx.x * 128;
-    const int nseg = (KCtot + 1) / 2;
-    const uint8_t* img = a.image + (size_t)nt * KCtot * bb;
-
-    if (warp_u == 0) tmem_alloc(&s_tmem, 512);
     if (tid == 0) {
-        mbar_init(&s_wfull[0], 1); mbar_init(&s_wfull[1], 1);
-        mbar_init(&s_afull[0], TcDense2::kRowWarps); mbar_init(&s_afull[1], TcDense2::kRowWarps);
-        mbar_init(&s_mma, 1); mbar_init(&s_dfree, TcDense2::kRowWarps);
+        for (int i = 0; i < kDenseStages; ++i) mbar_init(&s_wfull[i], 1);
         fence_mbar_init();
     }
-    fence_before_thread_sync();
     __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = warp_uniform(s_tmem);
-#ifdef PSA_TC_TIMING
-    unsigned long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 1};
-    long long tprev = clock64();
-#endif
-
-    if (warp_u == TcDense2::kRowWarps) {
-        // ================= issuer warp =================
-        auto load_seg = [&](int sg) {       // one lane
-            const int kcs = min(2, KCtot - 2 * sg);
-            const uint32_t bytes = (uint32_t)kcs * bb;
-            uint64_t* bar = &s_wfull[sg & 1];
-            mbar_expect_tx(bar, bytes);
-            for (uint32_t o = 0; o < bytes; o += 32768u)
-                bulk_g2s(base + (sg & 1) * slot_bytes + o, img + (size_t)sg * slot_bytes + o, min(32768u, bytes - o), bar);
-        };
-        if (lane == 0) { load_seg(0); if (nseg > 1) load_seg(1); }
-        __syncwarp();
-        for (int sg = 0; sg < nseg; ++sg) {
-            const int b = sg & 1;
-            const uint32_t par = (uint32_t)((sg >> 1) & 1);
-            mbar_wait(&s_wfull[b], par);
-            mbar_wait(&s_afull[b], par);
-            if (sg > 0) {
-                mbar_wait(&s_dfree, (uint32_t)((sg - 1) & 1));        // D drained => MMAs of segment sg-1 completed too
-                if (lane == 0 && sg + 1 < nseg) load_seg(sg + 1);     // their weight slot is free again
-            }
-            __syncwarp();
-            fence_after_thread_sync();
-            const uint32_t blocks = smem_u32(base) + (uint32_t)b * slot_bytes;
-            const uint32_t a1 = TcDense2::A0 + (uint32_t)b * TcDense2::ABUF;
-            if (KCtot - 2 * sg >= 2) issue_tile_c<2, NT_, 64, NP>(tmem_base, TcDense2::D, a1, blocks);
-            else issue_tile_c<1, NT_, 64, NP>(tmem_base, TcDense2::D, a1, blocks);
-            mma_commit(&s_mma);
-        }
-    } else {
-        // ================= row warps =================
-        const int quarter = warp_u & 3, cs = warp_u >> 2;
-        const int row = quarter * 32 + lane;
-        const long long grow = row0 + row;
-        const bool valid = grow < a.rows;
-        const uint32_t row_taddr = tmem_base + ((uint32_t)(quarter * 32) << 16);
-        const bool vec_ok = ((a.K & 3) == 0) && ((reinterpret_cast<uintptr_t>(a.x) & 15) == 0);
-        const bool has_out_chunk = cs < NT_ / 32;
-        float acc[32];
-#pragma unroll
-        for (int q = 0; q < 32; ++q) acc[q] = 0.f;
-
-        // this warp's 32-wide chunk of segment sg of x, raw (loads only: issued early, consumed a segment later)
-        auto load_x = [&](int sg, float (&h)[32]) {
-            const int kcs = min(2, KCtot - 2 * sg);
-            if (cs < kcs * 2) {
-                const int k0 = sg * 128 + cs * 32;
-                const float* xr = a.x + (size_t)(valid ? grow : 0) * a.K + k0;
-                if (valid && vec_ok && k0 + 32 <= a.K) {
-#pragma unroll
-                    for (int q = 0; q < 8; ++q) {
-                        const float4 u = __ldg(reinterpret_cast<const float4*>(xr) + q);
-                        h[4 * q] = u.x; h[4 * q + 1] = u.y; h[4 * q + 2] = u.z; h[4 * q + 3] = u.w;
-                    }
-                } else {
-#pragma unroll
-                    for (int q = 0; q < 32; ++q) h[q] = (valid && k0 + q < a.K) ? __ldg(xr + q) : 0.f;
-                }
-            }
-        };
-        // split into NP pieces -> A buffer sg & 1, then tell the issuer
-        auto store_x = [&](int sg, float (&h)[32]) {
-            const int kcs = min(2, KCtot - 2 * sg);
-            if (cs < kcs * 2) {
-                store_a_at<NP>(row_taddr + TcDense2::A0 + (uint32_t)(sg & 1) * TcDense2::ABUF + cs * 16, h, 64, ovf);
-                tmem_st_wait();
-            }
-            fence_before_thread_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_afull[sg & 1]);
-        };
-
-        TC_STAMP(0);
-        float h[32];
-        load_x(0, h);
-        store_x(0, h);
-        if (nseg > 1) load_x(1, h);
-        TC_STAMP(1);
-        for (int sg = 0; sg < nseg; ++sg) {
-            if (sg + 1 < nseg) {
-                store_x(sg + 1, h);                   // buffer (sg+1)&1 was released by the MMAs of segment sg-1 (waited below)
-                if (sg + 2 < nseg) load_x(sg + 2, h); // in flight across this segment's MMA wait and drain
-            }
-            TC_STAMP(2);
-            mbar_wait(&s_mma, (uint32_t)(sg & 1));
-            fence_after_thread_sync();
-            TC_STAMP(3);
-            if (has_out_chunk) {
-                uint32_t d[32];
-                tmem_ld32(row_taddr + TcDense2::D + cs * 32, d);
-                tmem_ld_wait();
-#pragma unroll
-                for (int q = 0; q < 32; ++q) acc[q] += __uint_as_float(d[q]);
-            }
-            fence_before_thread_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_dfree);
-            TC_STAMP(4);
-        }
-        // ---- epilogue ----
-        const int col0 = nt * NT_ + cs * 32;
-        float v[32];
-        if (has_out_chunk) {
-            float sx3 = 0.f, sy3 = 0.f, sz3 = 0.f;
-            if (a.xyz3 != nullptr && valid) {
-                sx3 = __ldg(a.xyz3 + (size_t)grow * 3); sy3 = __ldg(a.xyz3 + (size_t)grow * 3 + 1); sz3 = __ldg(a.xyz3 + (size_t)grow * 3 + 2);
-            }
-            const float* vs = &s_vec[0][cs * 32];
-            if (a.xyz3 != nullptr) {
-#pragma unroll
-                for (int q = 0; q < 32; ++q)
-                    acc[q] = fmaf(sz3, vs[4 * NT_ + q], fmaf(sy3, vs[3 * NT_ + q], fmaf(sx3, vs[2 * NT_ + q], acc[q])));
-            }
-#pragma unroll
-            for (int q = 0; q < 32; ++q) {
-                float x = fmaf(acc[q], vs[q], vs[NT_ + q]);
-                if (a.relu) x = fmaxf(x, 0.f);
-                v[q] = x;
-            }
-        }
-        if (a.pool_k == 1) {
-            if (has_out_chunk && valid) {
-                float4* o = reinterpret_cast<float4*>(a.out + (size_t)grow * a.N + col0);
-#pragma unroll
-                for (int q = 0; q < 8; ++q) o[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            }
-        } else {
-            const bool big = a.pool_k > 128;                         // the whole 128-row tile lies inside one group
-            const int quarters_per_group = big ? 4 : a.pool_k / 32;
-            const long long wg = (row0 + quarter * 32) / a.pool_k;
-            float mx = -FLT_MAX;
-            if (has_out_chunk) {
-#pragma unroll
-                for (int q = 0; q < 32; ++q) v[q] = valid ? v[q] : -FLT_MAX;
-                mx = warp_colmax_32x32(v, lane);
-            }
-            if (quarters_per_group > 1) {
-                s_red[warp_u][lane] = mx;
-                named_bar_sync(1, TcDense2::kRowWarps * 32);
-                if ((quarter % quarters_per_group) == 0)
-                    for (int o = 1; o < quarters_per_group; ++o) mx = fmaxf(mx, s_red[warp_u + o][lane]);
-            }
-            if (has_out_chunk && (quarter % quarters_per_group) == 0 && row0 + quarter * 32 < a.rows) {
-                if (!big) {
-                    a.out[(size_t)wg * a.N + col0 + lane] = mx;
-                } else {
-                    int code = __float_as_int(mx);
-                    code = code >= 0 ? code : code ^ 0x7fffffff;
-                    atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + col0 + lane, code);
-                }
-            }
-        }
-    }
-    TC_STAMP(5);
-    if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
-    }
-    fence_before_thread_sync();
-    __syncthreads();
-    TC_STAMP(6);
-#ifdef PSA_TC_TIMING
+    auto load_block = [&](int kb) {       // thread 0
+        uint64_t* bar = &s_wfull[kb % kDenseStages];
+        mbar_expect_tx(bar, bb);
+        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (kb % kDenseStages) * bb + o, img + (size_t)kb * bb + o, min(16384u, bb - o), bar);
+    };
     if (tid == 0)
-        for (int i = 0; i < 8; ++i) atomicAdd(&g_tc_timing[i], tacc[i]);
-#endif
-    if (warp_u == 0) tmem_dealloc(tmem_base, 512);
-}
+        for (int kb = 0; kb < kDenseStages && kb < KC; ++kb) load_block(kb);
 
-// ------------------------------------------------------------------------------------------------------------------
-// tc_dense3_kernel -- the dense layer in TRANSPOSED form, both operands from shared memory:
-//      D^T[channel][row] = sum_k W^T[channel][k] . x^T[k][row]
-//   M = 128 output channels (TMEM lanes), N = 128 rows (TMEM columns), K walked in 64-wide blocks, two stages.
-//   * A operand = the weight image block exactly as tc_dense2 uses it as B ([128 ch][64 k] K-major SWIZZLE_128B, three
-//     bf16 pieces, 48 KB, one cp.async.bulk);
-//   * B operand = x quantised into the same layout by 16 prep warps: each warp reads 8 rows x 256 B fully COALESCED
-//     (lane = two consecutive k), splits into NP pieces and writes 4-byte words into the swizzled rows -- conflict-free.
-//     (tc_dense2's lane = row loads cost 4096 L1 wavefronts per K = 128 segment; here 256 per 64-K block.)
-//   * the issuer warp waits for a stage's two operands and issues its 24 MMAs; the commit frees the stage;
-//   * accumulation: K-block kb goes to accumulator kb & 3 (4 x 128 TMEM columns), so no accumulator takes more than 48
-//     truncating adds at K = 512 (the bound tc_dense2 keeps with its register sums); the epilogue adds the four;
-//   * epilogue with lane = CHANNEL: scale / shift / xyz-side weights are per-thread scalars, a max over rows is an
-//     in-thread reduction (no shuffles), and every global store is a coalesced 128-byte row segment.
-// ------------------------------------------------------------------------------------------------------------------
-struct TcDense3 {
-    static constexpr int kPrepWarps = 16, kThreads = 17 * 32;
-    static constexpr uint32_t kPiece = 128u * 128u;          // one 16-bit piece of a 128 x 64 block: 16 KB
-};
-
-// CP = channel tiles per CTA.  CP = 2 (fp16x2, N a multiple of 256): the x block of a K step is staged ONCE and multiplied with the
-// weight blocks of two 128-channel tiles (accumulators 0/1 and 2/3) -- the staging work per output halves and SA3's 512 -> 1024 layer
-// becomes a single wave of 128 CTAs instead of 1.7 waves of 256.
-template <int NP, int CP>
-__global__ void __launch_bounds__(TcDense3::kThreads, 1)
-tc_dense3_kernel(const __grid_constant__ TcDenseArgs a) {
-    if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr uint32_t kBlock = NP * TcDense3::kPiece;       // 48 KB (bf16x3) or 32 KB (fp16x2)
-    constexpr int kAcc = 4 / CP;                             // TMEM accumulators (128 columns each) per channel tile
-    uint32_t ovf = 0u;
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_wfull[2];     // weight block landed (tx)
-    __shared__ __align__(8) uint64_t s_xfull[2];     // x block written by the 16 prep warps
-    __shared__ __align__(8) uint64_t s_free[2];      // the MMAs that read a stage completed
-    __shared__ uint32_t s_tmem;
-    __shared__ float s_red[TcDense3::kPrepWarps][32];
-    __shared__ float s_xyz[128][3];
-    const int tid = threadIdx.x, lane = tid & 31;
-    const int warp_u = (int)warp_uniform((uint32_t)(tid >> 5));
-    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* wslot = base;                                   // 2 stages x CP weight blocks
-    uint8_t* xslot = base + 2 * CP * kBlock;                 // 2 stages x 1 x block
-    const int KB = a.Kp / 64;
-    const int nt = blockIdx.y * CP;                          // first channel tile of this CTA
-    const long long row0 = (long long)blockIdx.x * 128;
-    const uint8_t* img = a.image + (size_t)nt * KB * kBlock;
-
-    if (warp_u == 0) tmem_alloc(&s_tmem, 512);
-    if (tid == 0) {
-        mbar_init(&s_wfull[0], 1); mbar_init(&s_wfull[1], 1);
-        mbar_init(&s_xfull[0], TcDense3::kPrepWarps); mbar_init(&s_xfull[1], TcDense3::kPrepWarps);
-        mbar_init(&s_free[0], 1); mbar_init(&s_free[1], 1);
-        fence_mbar_init();
-    }
-    if (a.xyz3 != nullptr)
-        for (int i = tid; i < 128 * 3; i += TcDense3::kThreads) {
-            const long long r = row0 + i / 3;
-            s_xyz[i / 3][i % 3] = r < a.rows ? __ldg(a.xyz3 + (size_t)r * 3 + i % 3) : 0.f;
-        }
-    fence_before_thread_sync();
-    __syncthreads();
-    fence_after_thread_sync();
-    const uint32_t tmem_base = warp_uniform(s_tmem);
-#ifdef PSA_TC_TIMING
-    unsigned long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 1};
-    long long tprev = clock64();
-#endif
-
-    if (warp_u == TcDense3::kPrepWarps) {
-        // ================= issuer warp =================
-        const uint32_t idesc = make_idesc(Split<NP>::kFmt, 128, 128);
-        for (int kb = 0; kb < KB; ++kb) {
-            const int st = kb & 1;
-            const uint32_t par = (uint32_t)((kb >> 1) & 1);
-            mbar_wait(&s_wfull[st], par);
-            mbar_wait(&s_xfull[st], par);
-            __syncwarp();
-            fence_after_thread_sync();
-            const SmemDescBase xb = smem_desc_base(warp_uniform(smem_u32(xslot) + (uint32_t)st * kBlock));
-            const uint32_t first = kb < kAcc ? 0u : 1u;      // an accumulator's first block overwrites it
-#pragma unroll
-            for (int c = 0; c < CP; ++c) {
-                const uint32_t d = tmem_base + (uint32_t)(c * kAcc + (kb % kAcc)) * 128u;
-                const SmemDescBase wa = smem_desc_base(warp_uniform(smem_u32(wslot) + (uint32_t)(st * CP + c) * kBlock));
-#pragma unroll
-                for (int t = 0; t < Split<NP>::kTerms; ++t)
-#pragma unroll
-                    for (int s4 = 0; s4 < 4; ++s4)
-                        mma_bf16_ss(d, smem_desc_at(wa, Split<NP>::w(t) * TcDense3::kPiece + s4 * 32),
-                                    smem_desc_at(xb, Split<NP>::a(t) * TcDense3::kPiece + s4 * 32), idesc, (t | s4) ? 1u : first);
-            }
-            mma_commit(&s_free[st]);
-        }
-    } else {
-        // ================= prep warps: x block -> B operand; then the epilogue =================
-        const bool vec2 = ((a.K & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.x) & 7) == 0);
-        float2 v[8];
-        // this warp's 8 rows x 64 k of block kb, raw: issued a block ahead, before the stage is known to be free
-        auto load_x = [&](int kb) {
-            const int k = kb * 64 + 2 * lane;
-            float2 isc = make_float2(1.f, 1.f), ish = make_float2(0.f, 0.f);
+    const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
+    const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
+    const bool vec2 = ((a.K & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.x) & 7) == 0);
+    auto load_x2 = [&](int i, int k) {    // x[r_i][k], x[r_i][k + 1] (zero past the end), batch norm + ReLU of training mode
+        float2 x = make_float2(0.f, 0.f);
+        if (v[i]) {
+            const float* xr = a.x + (size_t)r[i] * a.K + k;
+            if (vec2 && k + 1 < a.K) x = __ldg(reinterpret_cast<const float2*>(xr));
+            else { if (k < a.K) x.x = __ldg(xr); if (k + 1 < a.K) x.y = __ldg(xr + 1); }
             if (a.in_scale != nullptr) {
-                if (k < a.K) { isc.x = __ldg(a.in_scale + k); ish.x = __ldg(a.in_shift + k); }
-                if (k + 1 < a.K) { isc.y = __ldg(a.in_scale + k + 1); ish.y = __ldg(a.in_shift + k + 1); }
+                if (k < a.K) { x.x = fmaf(x.x, __ldg(a.in_scale + k), __ldg(a.in_shift + k)); if (a.in_relu) x.x = fmaxf(x.x, 0.f); }
+                if (k + 1 < a.K) { x.y = fmaf(x.y, __ldg(a.in_scale + k + 1), __ldg(a.in_shift + k + 1)); if (a.in_relu) x.y = fmaxf(x.y, 0.f); }
             }
+        }
+        return x;
+    };
+
+    float acc[NC][32];
+    for (int kb = 0; kb < KC; ++kb) {
+        uint32_t A[NP][4][4];
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const long long r = row0 + warp_u * 8 + i;
-                v[i] = make_float2(0.f, 0.f);
-                if (r < a.rows) {
-                    const float* xr = a.x + (size_t)r * a.K + k;
-                    if (vec2 && k + 1 < a.K) v[i] = __ldg(reinterpret_cast<const float2*>(xr));
-                    else { if (k < a.K) v[i].x = __ldg(xr); if (k + 1 < a.K) v[i].y = __ldg(xr + 1); }
-                    if (a.in_scale != nullptr) {       // previous layer's batch norm (+ relu) on the fly; padded rows / channels stay 0
-                        if (k < a.K) { v[i].x = fmaf(v[i].x, isc.x, ish.x); if (a.in_relu) v[i].x = fmaxf(v[i].x, 0.f); }
-                        if (k + 1 < a.K) { v[i].y = fmaf(v[i].y, isc.y, ish.y); if (a.in_relu) v[i].y = fmaxf(v[i].y, 0.f); }
+        for (int s = 0; s < 4; ++s)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const float2 x = load_x2(i, kb * 64 + 16 * s + 8 * h + 2 * t);
+                    put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
+                }
+        mbar_wait(&s_wfull[kb % kDenseStages], (uint32_t)((kb / kDenseStages) & 1));
+        const uint32_t wb = smem_u32(base) + (uint32_t)(kb % kDenseStages) * bb;
+        float d[NC][32];
+        wg_fence();
+#pragma unroll
+        for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+#pragma unroll
+            for (int s = 0; s < 4; ++s)
+#pragma unroll
+                for (int c = 0; c < NC; ++c)
+                    wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
+                                  wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)c * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
+        wg_commit();
+        wg_wait_all();
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+            wg_fence_acc(d[c]);
+#pragma unroll
+            for (int q = 0; q < 32; ++q) acc[c][q] = kb ? acc[c][q] + d[c][q] : d[c][q];
+        }
+        __syncthreads();                                             // both warpgroups are done with this weight slot
+        if (tid == 0 && kb + kDenseStages < KC) load_block(kb + kDenseStages);
+    }
+
+    // ---- epilogue ----
+    float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+    if (a.xyz3 != nullptr)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+            if (v[i])
+#pragma unroll
+                for (int q = 0; q < 3; ++q) xs[i][q] = __ldg(a.xyz3 + (size_t)r[i] * 3 + q);
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int cl = c * 64 + 8 * j + 2 * t;
+            float y[2][2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    float x = acc[c][4 * j + 2 * i + e];
+                    if (a.xyz3 != nullptr) x = fmaf(xs[i][2], s_vec[4][cl + e], fmaf(xs[i][1], s_vec[3][cl + e], fmaf(xs[i][0], s_vec[2][cl + e], x)));
+                    x = fmaf(x, s_vec[0][cl + e], s_vec[1][cl + e]);
+                    if (a.relu) x = fmaxf(x, 0.f);
+                    y[i][e] = x;
+                }
+            if (a.pool_k == 1) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (v[i]) *reinterpret_cast<float2*>(a.out + (size_t)r[i] * a.N + nt * Nt + cl) = make_float2(y[i][0], y[i][1]);
+                if (a.stat_partial != nullptr) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float ssum = 0.f, ssq = 0.f;
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+                            if (v[i]) { ssum += y[i][e]; ssq = fmaf(y[i][e], y[i][e], ssq); }
+                        ssum = warp_rowsum16(ssum);
+                        ssq = warp_rowsum16(ssq);
+                        if (g == 0) { s_red[0][warp][cl + e] = ssum; s_red[1][warp][cl + e] = ssq; }
                     }
                 }
-            }
-        };
-        load_x(0);
-        TC_STAMP(0);
-        for (int kb = 0; kb < KB; ++kb) {
-            const int st = kb & 1;
-            if (kb >= 2) mbar_wait(&s_free[st], (uint32_t)(((kb - 2) >> 1) & 1));      // stage released by block kb-2's MMAs
-            TC_STAMP(1);
-            if (warp_u == 0 && lane == 0) {                                             // its weight slot is free too
-                mbar_expect_tx(&s_wfull[st], CP * kBlock);
-                for (int c = 0; c < CP; ++c)
-                    for (uint32_t o = 0; o < kBlock; o += 16384u)
-                        bulk_g2s(wslot + (uint32_t)(st * CP + c) * kBlock + o, img + ((size_t)c * KB + kb) * kBlock + o, 16384u, &s_wfull[st]);
-            }
-            uint8_t* xs = xslot + (uint32_t)st * kBlock;
+            } else {
 #pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const uint32_t rr = (uint32_t)(warp_u * 8 + i);
-                const uint32_t off = swz_off_bf16(rr, 2u * (uint32_t)lane, 128u);
-                uint32_t pc[NP];
-                split_pair<NP>(v[i].x, v[i].y, pc, ovf);
-#pragma unroll
-                for (int j = 0; j < NP; ++j) *reinterpret_cast<uint32_t*>(xs + (uint32_t)j * TcDense3::kPiece + off) = pc[j];
-            }
-            fence_proxy_async_smem();            // generic-proxy writes -> visible to the MMA's async-proxy reads
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_xfull[st]);
-            if (kb + 1 < KB) load_x(kb + 1);
-            TC_STAMP(2);
-        }
-        // all MMAs done: the last block's commit covers every earlier one (in-order completion)
-        mbar_wait(&s_free[(KB - 1) & 1], (uint32_t)(((KB - 1) >> 1) & 1));
-        fence_after_thread_sync();
-        TC_STAMP(3);
-
-        // ---- epilogue: lane = channel ----
-        const int quarter = warp_u & 3, slot = warp_u >> 2;          // channels 32*quarter.., rows 32*slot..
-        const long long rbase = row0 + slot * 32;
-#pragma unroll 1
-        for (int ct = 0; ct < CP; ++ct) {                             // the CTA's channel tiles, one after the other
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(ct * kAcc) * 128u + (uint32_t)slot * 32u;
-        const int ch = (nt + ct) * 128 + quarter * 32 + lane;
-        float acc[32];
-        {
-            uint32_t d[32];
-            tmem_ld32(taddr, d);
-            tmem_ld_wait();
-#pragma unroll
-            for (int q = 0; q < 32; ++q) acc[q] = __uint_as_float(d[q]);
-            const int nacc = KB < kAcc ? KB : kAcc;
-            for (int c = 1; c < nacc; ++c) {
-                tmem_ld32(taddr + (uint32_t)c * 128u, d);
-                tmem_ld_wait();
-#pragma unroll
-                for (int q = 0; q < 32; ++q) acc[q] += __uint_as_float(d[q]);
-            }
-        }
-        const float sc = a.scale ? __ldg(a.scale + ch) : 1.f;
-        const float sh = a.shift ? __ldg(a.shift + ch) : 0.f;
-        if (a.xyz3 != nullptr) {
-            const float w0 = __ldg(a.w3 + ch), w1 = __ldg(a.w3 + a.N + ch), w2 = __ldg(a.w3 + 2 * a.N + ch);
-#pragma unroll
-            for (int q = 0; q < 32; ++q) {
-                const float* xq = s_xyz[slot * 32 + q];
-                acc[q] = fmaf(xq[2], w2, fmaf(xq[1], w1, fmaf(xq[0], w0, acc[q])));
-            }
-        }
-#pragma unroll
-        for (int q = 0; q < 32; ++q) {
-            float x = fmaf(acc[q], sc, sh);
-            if (a.relu) x = fmaxf(x, 0.f);
-            acc[q] = x;
-        }
-        if (a.pool_k == 1) {
-#pragma unroll
-            for (int q = 0; q < 32; ++q)
-                if (rbase + q < a.rows) a.out[(size_t)(rbase + q) * a.N + ch] = acc[q];       // 32 lanes = 128 contiguous bytes
-            if (a.stat_partial != nullptr) {
-                // column statistics of the stored tile: lane = channel, so sum / sum of squares over this slot's 32 rows are
-                // in-thread; the four row slots of a channel quarter fold through shared memory in slot order (deterministic)
-                float ssum = 0.f, ssq = 0.f;
-#pragma unroll
-                for (int q = 0; q < 32; ++q)
-                    if (rbase + q < a.rows) { ssum += acc[q]; ssq = fmaf(acc[q], acc[q], ssq); }
-                __shared__ float s_st[2][TcDense3::kPrepWarps][32];
-                s_st[0][warp_u][lane] = ssum;
-                s_st[1][warp_u][lane] = ssq;
-                named_bar_sync(1, TcDense3::kPrepWarps * 32);
-                if (slot == 0) {
-                    float t0 = 0.f, t1 = 0.f;
-#pragma unroll
-                    for (int o = 0; o < 4; ++o) { t0 += s_st[0][quarter + 4 * o][lane]; t1 += s_st[1][quarter + 4 * o][lane]; }
-                    float* dst = a.stat_partial + (size_t)blockIdx.x * 2 * a.N;
-                    dst[ch] = t0;
-                    dst[a.N + ch] = t1;
-                }
-            }
-        } else {
-            float mx = -FLT_MAX;
-#pragma unroll
-            for (int q = 0; q < 32; ++q) mx = (rbase + q < a.rows) ? fmaxf(mx, acc[q]) : mx;
-            const bool big = a.pool_k > 128;
-            const int slots_per_group = big ? 4 : a.pool_k / 32;         // 1, 2 or 4 row slots per pooling group
-            if (slots_per_group > 1) {
-                s_red[warp_u][lane] = mx;
-                named_bar_sync(1, TcDense3::kPrepWarps * 32);
-                if ((slot % slots_per_group) == 0)
-                    for (int o = 1; o < slots_per_group; ++o) mx = fmaxf(mx, s_red[warp_u + 4 * o][lane]);
-            }
-            if ((slot % slots_per_group) == 0 && rbase < a.rows) {
-                const long long wg = rbase / a.pool_k;
-                if (!big) {
-                    a.out[(size_t)wg * a.N + ch] = mx;
-                } else {
-                    int code = __float_as_int(mx);
-                    code = code >= 0 ? code : code ^ 0x7fffffff;
-                    atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + ch, code);
+                for (int e = 0; e < 2; ++e) {
+                    const float m = warp_rowmax16(v[0] ? y[0][e] : -FLT_MAX, v[1] ? y[1][e] : -FLT_MAX);
+                    if (g == 0) s_red[0][warp][cl + e] = m;
                 }
             }
         }
-        if (CP > 1) named_bar_sync(1, TcDense3::kPrepWarps * 32);       // s_red / s_st are reused by the next channel tile
+    if (a.pool_k == 1) {
+        if (a.stat_partial != nullptr) {
+            // per-tile column statistics, the eight warps' 16-row partials folded in warp order (deterministic)
+            __syncthreads();
+            for (int cl = tid; cl < Nt; cl += kDenseThreads) {
+                float t0 = 0.f, t1 = 0.f;
+                for (int w = 0; w < 8; ++w) { t0 += s_red[0][w][cl]; t1 += s_red[1][w][cl]; }
+                float* dst = a.stat_partial + (size_t)blockIdx.x * 2 * a.N;
+                dst[nt * Nt + cl] = t0;
+                dst[a.N + nt * Nt + cl] = t1;
+            }
+        }
+    } else {
+        __syncthreads();
+        const bool big = a.pool_k > 128;                             // the whole 128-row tile lies inside one group
+        const int wpg = big ? 8 : a.pool_k / 16;                     // warps per pooling group
+        for (int e = tid; e < (8 / wpg) * Nt; e += kDenseThreads) {
+            const int grp = e / Nt, cl = e % Nt;
+            const long long rs = row0 + grp * wpg * 16;
+            if (rs >= a.rows) continue;
+            float mx = s_red[0][grp * wpg][cl];
+            for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[0][grp * wpg + w][cl]);
+            const long long wg = rs / a.pool_k;
+            if (!big) {
+                a.out[(size_t)wg * a.N + nt * Nt + cl] = mx;
+            } else {
+                int code = __float_as_int(mx);
+                code = code >= 0 ? code : code ^ 0x7fffffff;
+                atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + nt * Nt + cl, code);
+            }
         }
     }
-    TC_STAMP(4);
     if constexpr (NP == 2) {
         if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
     }
-    fence_before_thread_sync();
-    __syncthreads();
-    TC_STAMP(5);
-#ifdef PSA_TC_TIMING
-    if (tid == 0)
-        for (int i = 0; i < 8; ++i) atomicAdd(&g_tc_timing[i], tacc[i]);
-#endif
-    if (warp_u == 0) tmem_dealloc(tmem_base, 512);
 }
 
 bool tc_dense_eligible(long long rows, int K, int N, int pool_k) {
@@ -1369,34 +662,16 @@ static const unsigned int* image_trailer(const uint8_t* image, int Kp, int N, in
 // one launch of a dense layer with NP pieces; `image` holds the weights in that format
 template <int NP>
 static int launch_tc_dense_np(TcDenseArgs& a, int Nt, cudaStream_t st) {
-    dim3 grid2((unsigned)((a.rows + 127) / 128), a.N / Nt);
+    const dim3 grid((unsigned)((a.rows + 127) / 128), a.N / Nt);
     const bool big = a.pool_k > 128;
     if (big) { int rc0 = launch_fill_ord_neg_inf(a.rows / a.pool_k * a.N, a.out, st, a.run_if); if (rc0 != PSA_OK) return rc0; }
-    if (Nt == 128 && a.Kp <= 512) {
-        // transposed kernel, both operands from shared memory; two channel tiles per CTA where the operands are small enough (fp16x2)
-        // and the halved grid still covers half of the SMs.  (Pairing always: +0.6 % clouds/s with four batches in flight -- SM-time
-        // per output drops -- but SA3 alone 63 -> 76 us, so small grids keep one tile per CTA.)
-        const bool pair = NP == 2 && (a.N % 256) == 0 && a.stat_partial == nullptr && (long long)grid2.x * (a.N / 256) >= kNumSMs / 2;
-        if (pair) {
-            constexpr int CPn = NP == 2 ? 2 : 1;
-            const size_t smem3 = (2 * CPn + 2) * (size_t)NP * TcDense3::kPiece + 1024;
-            grid2.y = a.N / (128 * CPn);
-            PSA_CUDA(cudaFuncSetAttribute(tc_dense3_kernel<NP, CPn>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-            tc_dense3_kernel<NP, CPn><<<grid2, TcDense3::kThreads, smem3, st>>>(a);
-        } else {
-            const size_t smem3 = 4 * (size_t)NP * TcDense3::kPiece + 1024;
-            PSA_CUDA(cudaFuncSetAttribute(tc_dense3_kernel<NP, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-            tc_dense3_kernel<NP, 1><<<grid2, TcDense3::kThreads, smem3, st>>>(a);
-        }
+    const size_t smem = kDenseStages * (size_t)tc_block_bytes(Nt, NP) + 1024;
+    if (Nt == 128) {
+        PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        tc_dense_kernel<NP, 2><<<grid, kDenseThreads, smem, st>>>(a);
     } else {
-        const size_t smem2 = 4 * (size_t)tc_block_bytes(Nt, NP) + 1024;      // two slots of two 64-K blocks
-        if (Nt == 128) {
-            PSA_CUDA(cudaFuncSetAttribute(tc_dense2_kernel<128, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-            tc_dense2_kernel<128, NP><<<grid2, TcDense2::kThreads, smem2, st>>>(a);
-        } else {
-            PSA_CUDA(cudaFuncSetAttribute(tc_dense2_kernel<64, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-            tc_dense2_kernel<64, NP><<<grid2, TcDense2::kThreads, smem2, st>>>(a);
-        }
+        PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        tc_dense_kernel<NP, 1><<<grid, kDenseThreads, smem, st>>>(a);
     }
     int rc = check_launch("tc_dense_kernel");
     if (rc != PSA_OK) return rc;
@@ -1440,12 +715,12 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
     return launch_tc_dense_np<3>(a, Nt, st);
 }
 
-// Training-mode forward of one layer on tc_dense3: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
+// Training-mode forward of one layer on tc_dense_kernel: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
 // statistics.  The weights change every step, so the image is rebuilt into `image_ws` (tc_dense_image_bytes(K, N)) per call.
 // bf16x3 only: batch-statistics activations are not range-checked.
 bool tc_train_fwd_eligible(long long rows, int K, int N) {
-    // one CTA per 128-row tile with ~14 k cycles of fixed prologue / epilogue: pays off from two K blocks up (K = 64 layers over
-    // 500 k rows run faster on the fp32 FMA kernel: 268 vs 302 us measured at SA1's 64 -> 128 layer)
+    // one CTA per 128-row tile with a fixed prologue / epilogue: pays off from two K blocks up (K = 64 layers stay on the fp32
+    // FMA kernel)
     return rows >= 128 && K >= 128 && K <= 512 && N >= 128 && (N % 128) == 0;
 }
 int launch_tc_dense_train(long long rows, int K, int N, const float* x, const float* in_scale, const float* in_shift, int in_relu,
@@ -1465,13 +740,6 @@ int launch_tc_dense_train(long long rows, int K, int N, const float* x, const fl
 static const uint8_t* prebuilt_image(const psa_mlp* mlp, int l, int row0, int Nt) {
     if (mlp->image[l] != nullptr && mlp->image_nt[l] == Nt && mlp->image_row0[l] == row0) return reinterpret_cast<const uint8_t*>(mlp->image[l]);
     return nullptr;
-}
-
-// PSA_SA_TMODE=0 keeps the last layer of 64-wide levels in row form (A/B runs)
-static bool tmode_enabled() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("PSA_SA_TMODE"); v = (e && e[0] == '0') ? 0 : 1; }
-    return v != 0;
 }
 
 // Can this MLP / geometry run on the tensor-core kernel with `np` pieces per operand?  (otherwise the fp32-FMA fused kernel
@@ -1494,18 +762,11 @@ bool tc_sa_eligible(const psa_mlp* mlp, int c, int nsample, TcArgs* out, int np)
         if (!is_last && !(a.Ntot[l] == 64 || a.Ntot[l] == 128)) return false;       // D and the next A operand are one tile wide
         if (is_last && !(a.Ntot[l] == 64 || a.Ntot[l] % 128 == 0)) return false;
     }
-    // two row groups per CTA, 64-wide tiles; the last layer is streamed per group if it does not fit; a level that does not fit
-    // even then runs on the fp32-FMA fused kernel
-    a.dual = 1; a.ntcap = 64; a.stream_last = 0; a.tmode = 0;
-    if (tc_dual_layout(a).total + 1024 > 226u * 1024u) a.stream_last = 1;
-    if (tc_dual_layout(a).total + 1024 > 226u * 1024u) return false;
-    // transposed last layer (lane = channel): 64-wide levels ending in a 128-wide layer, fp16x2 operands, whole neighbourhoods per half tile
-    bool t = np == 2 && !a.stream_last && C1 == 64 && a.Ntot[a.nl - 1] == 128 && (nsample == 32 || nsample == 64) && tmode_enabled();
-    for (int l = 0; l < a.nl; ++l) t = t && a.Kd[l] == 64;
-    if (t) {
-        a.tmode = 1;
-        if (tc_dual_layout(a).total + 1024 > 226u * 1024u) a.tmode = 0;
-    }
+    // the last layer is streamed in 64-channel chunks if it does not fit next to the others; a level that does not fit even then
+    // runs on the fp32-FMA fused kernel
+    a.stream_last = 0;
+    if (tc_sa_layout(a).total + 1024 > kSmemBudget) a.stream_last = 1;
+    if (tc_sa_layout(a).total + 1024 > kSmemBudget) return false;
     *out = a;
     return true;
 }
@@ -1524,42 +785,30 @@ size_t tc_sa_workspace_bytes(const TcArgs& a, int b, int n, int c) {
     return bytes;
 }
 
-// tile width (with the image-format flag of the current split) of tensor layer l of a level: 64-wide blocks, except the last layer of
-// a transposed-mode level, which is the A operand of an M = 128 MMA (one [128 ch][64 k] block)
-static int tc_sa_image_nt(const TcArgs& a, int l) { return ((a.tmode && l == a.nl - 1) ? 128 : TcDual::kNt) | image_flag(g_tc_np); }
+// tile width (with the image-format flag of the current split) of the tensor layers of a level: 64-wide blocks
+static int tc_sa_image_nt() { return kSaNt | image_flag(g_tc_np); }
+
+template <int NP, int C1, int NL, int N0>
+static int launch_tc_sa_shape(const TcArgs& a, int ctas, size_t smem, cudaStream_t st) {
+    PSA_CUDA(cudaFuncSetAttribute(tc_sa_kernel<NP, C1, NL, N0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    tc_sa_kernel<NP, C1, NL, N0><<<ctas, kSaThreads, smem, st>>>(a);
+    return check_launch("tc_sa_kernel");
+}
 
 template <int NP>
 static int launch_tc_sa_np(TcArgs& a, cudaStream_t st) {
     const int G = 128 / a.K;
     const long long ntiles = (a.groups + G - 1) / G;
-    const size_t smem = (size_t)tc_dual_layout(a).total + 1024;
-    long long ctas = (ntiles + 1) / 2;
-    if (ctas > kNumSMs) ctas = kNumSMs;
+    const size_t smem = (size_t)tc_sa_layout(a).total + 1024;
+    int ctas = (int)(ntiles < kNumSMs ? ntiles : kNumSMs);
     if (ctas < 1) ctas = 1;
-    if (a.tmode) {
-        if constexpr (NP == 2) {
-            PSA_CUDA(cudaFuncSetAttribute(tc_sa_dual_kernel<3, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            tc_sa_dual_kernel<3, 2><<<(int)ctas, TcDual::kThreads, smem, st>>>(a);
-            return check_launch("tc_sa_dual_kernel");
-        }
-    }
-    const bool pairs = !a.stream_last && (a.Ntot[a.nl - 1] % 128) == 0;            // tile pairs: an even number of resident 64-wide tiles
-    bool narrow = a.C1 <= 64;
-    for (int l = 0; l < a.nl; ++l) narrow = narrow && a.Kd[l] <= 64;
-    if (pairs && narrow) {
-        PSA_CUDA(cudaFuncSetAttribute(tc_sa_dual_kernel<1, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tc_sa_dual_kernel<1, NP><<<(int)ctas, TcDual::kThreads, smem, st>>>(a);
-    } else if (pairs && NP == 2) {
-        PSA_CUDA(cudaFuncSetAttribute(tc_sa_dual_kernel<(NP == 2 ? 2 : 0), NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tc_sa_dual_kernel<(NP == 2 ? 2 : 0), NP><<<(int)ctas, TcDual::kThreads, smem, st>>>(a);
-    } else {
-        PSA_CUDA(cudaFuncSetAttribute(tc_sa_dual_kernel<0, NP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tc_sa_dual_kernel<0, NP><<<(int)ctas, TcDual::kThreads, smem, st>>>(a);
-    }
-    return check_launch("tc_sa_dual_kernel");
+    // shapes accepted by tc_sa_eligible: C1 in {64, 128}, one or two tensor layers, an inner layer 64 or 128 wide
+    if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas, smem, st);
+    if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas, smem, st);
+    return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 128, 2, 64>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 128, 2, 128>(a, ctas, smem, st);
 }
 
-// One set-abstraction level on the dual-group kernel (`a` = eligibility result for the current split): weight images, the U GEMM
+// One set-abstraction level on the SA kernel (`a` = eligibility result for the current split): weight images, the U GEMM
 // of the feature part of layer 1, the level, and -- fp16x2 -- its guarded bf16x3 rerun.  w1c: optional centre weights (EdgeConv).
 static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const float* xyz, const float* new_xyz, const float* points,
                      const int* idx, const psa_mlp* mlp, const float* w1c, float* out, void* workspace, cudaStream_t st) {
@@ -1601,7 +850,7 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     };
     fill(a);
     for (int l = 0; l < a.nl; ++l) {
-        const int nt_img = tc_sa_image_nt(a, l);
+        const int nt_img = tc_sa_image_nt();
         const uint8_t* pre = prebuilt_image(mlp, 1 + l, 0, nt_img);
         uint8_t* own = a.np == 2 ? img2[l] : img3[l];
         if (pre == nullptr) { rc = build_image(a.Kd[l], a.Kd[l], a.Ntot[l], nt_img, mlp->weight[1 + l], own, st); if (rc != PSA_OK) return rc; }
@@ -1618,13 +867,12 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     PSA_REQUIRE(tc_sa_eligible(mlp, c, nsample, &a3, 3), "sa_module: internal error (bf16x3 eligibility)");
     fill(a3);
     for (int l = 0; l < a3.nl; ++l) {
-        // a prebuilt fp16x2 image carries its bf16x3 twin behind it -- usable here if it has the 64-wide blocks of the row-form kernel
-        // (the last layer of a transposed-mode level does not: its twin is rebuilt, conditionally)
-        const uint8_t* pre = prebuilt_image(mlp, 1 + l, 0, TcDual::kNt | kImageF16x2);
+        // a prebuilt fp16x2 image carries its bf16x3 twin behind it
+        const uint8_t* pre = prebuilt_image(mlp, 1 + l, 0, kSaNt | kImageF16x2);
         if (pre != nullptr) {
             a3.image[l] = pre + tc_image_alloc_bytes(a3.Kd[l], a3.Ntot[l], 2);
         } else {
-            rc = build_image(a3.Kd[l], a3.Kd[l], a3.Ntot[l], TcDual::kNt | kImageBf16x3, mlp->weight[1 + l], img3[l], st, words + 2);
+            rc = build_image(a3.Kd[l], a3.Kd[l], a3.Ntot[l], kSaNt | kImageBf16x3, mlp->weight[1 + l], img3[l], st, words + 2);
             if (rc != PSA_OK) return rc;
             a3.image[l] = img3[l];
         }
@@ -1983,7 +1231,7 @@ extern "C" int psa_mlp_image_plan(int usage, long long rows, int pool_k, int c, 
     TcArgs a;
     if (!tc_sa_eligible(mlp, c, nsample, &a)) return PSA_OK;
     if (c > 0 && tc_dense_eligible(rows, c, a.C1, 1)) { nt[0] = tc_dense_nt(a.C1); row0[0] = 3; bytes[0] = tc_plan_image_bytes((c + 63) & ~63, a.C1); }
-    for (int l = 0; l < a.nl; ++l) { nt[1 + l] = tc_sa_image_nt(a, l); row0[1 + l] = 0; bytes[1 + l] = tc_plan_image_bytes(a.Kd[l], a.Ntot[l]); }
+    for (int l = 0; l < a.nl; ++l) { nt[1 + l] = tc_sa_image_nt(); row0[1 + l] = 0; bytes[1 + l] = tc_plan_image_bytes(a.Kd[l], a.Ntot[l]); }
     return PSA_OK;
 }
 

@@ -6,7 +6,7 @@
 //   ActIn   h_{l-1}[r][c] = relu(y_{l-1}[r][c] * scale[c] + shift[c]) (* dropout mask)      the forward input of layer l
 //   GradIn  dy_l[r][c]    = ca[c] * dz + cb[c] * y_l[r][c] + cc[c],  dz = dh * [relu active]  the batch-norm backward
 //           with dh either a dense tensor or the max-pool routing (dp[g][c] where argmax[g][c] == r mod K, else 0).
-// Three products per layer, all on this kernel (C = A * B, fp32 FMA on the packed FFMA2 pipe, 128x128 / 128x64 / 64x64
+// Three products per layer, all on this kernel (C = A * B, fp32 FMA on float pairs, 128x128 / 128x64 / 64x64
 // tiles, double-buffered shared memory, split over the contraction for the weight gradient):
 //   forward          y_l  = ActIn   * W            A contraction-contiguous, B column-contiguous
 //   input gradient   dh   = GradIn  * W^T          A contraction-contiguous, B contraction-contiguous
@@ -275,7 +275,7 @@ train_gemm_kernel(const FA fa, const FB fb, const GemmOut o, long long M, int N,
 #pragma unroll
                 for (int i = 0; i < TM; ++i)
 #pragma unroll
-                    for (int j = 0; j < TN / 2; ++j) acc[i][j] = __ffma2_rn(make_float2(a[i], a[i]), b[j], acc[i][j]);
+                    for (int j = 0; j < TN / 2; ++j) acc[i][j] = ffma2_rn(make_float2(a[i], a[i]), b[j], acc[i][j]);
             }
             if (more) {
                 stash(buf ^ 1);

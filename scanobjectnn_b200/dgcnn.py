@@ -1,4 +1,4 @@
-"""dgcnn/models/dgcnn.py and dgcnn_bga.py on the B200 kernels (inference, and training through autograd over the same kernels: is_training=True).
+"""dgcnn/models/dgcnn.py and dgcnn_bga.py on the libpsa kernels (inference, and training through autograd over the same kernels: is_training=True).
 
 Every `pairwise_distance -> knn -> get_edge_feature -> conv2d -> reduce_max` group of the reference
 (dgcnn.py:31-80) is two launches here: the fused kNN graph (no (B,N,N) matrix) and the fused EdgeConv

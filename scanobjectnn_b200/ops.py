@@ -604,7 +604,7 @@ def edgeconv_infer(x, nn_idx, mlp: MlpParams) -> torch.Tensor:
 
 
 def set_mlp_mode(mode: int) -> None:
-    """0 = tcgen05 tensor cores where the shapes allow, fp16x2 operands with the device-side range guard (default);
+    """0 = tensor cores (wgmma) where the shapes allow, fp16x2 operands with the device-side range guard (default);
     1 = always the fp32-FMA kernels; 2 = tensor cores with bf16x3 operands (include/psa.h)."""
     check(_lib.load().psa_set_mlp_mode(int(mode)), "set_mlp_mode")
 

@@ -1,4 +1,4 @@
-"""pointnet2/models/pointnet2_cls_bga.py on the B200 kernels: joint classification + background-mask segmentation.
+"""pointnet2/models/pointnet2_cls_bga.py on the libpsa kernels: joint classification + background-mask segmentation.
 get_model(point_cloud, is_training, bn_decay, num_class) -> (class_pred (B,num_class), seg_pred (B,N,2)), same
 layer hyper-parameters (pointnet2_cls_bga.py:30-66).  Inference (fused kernels, BN folded) and training (is_training=True:
 batch-statistics BN, autograd over the hand-written level / MLP / interpolation kernels)."""

@@ -1,4 +1,4 @@
-"""pointnet2/models/pointnet2_cls_ssg.py on the B200 kernels: get_model(point_cloud, is_training, bn_decay,
+"""pointnet2/models/pointnet2_cls_ssg.py on the libpsa kernels: get_model(point_cloud, is_training, bn_decay,
 num_class) -> (logits (B,num_class), end_points), same layer hyper-parameters (pointnet2_cls_ssg.py:35-45)."""
 from __future__ import annotations
 
@@ -48,7 +48,7 @@ def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *,
     end_points = {"l0_xyz": point_cloud}
     l0_xyz, l0_points = point_cloud, None
     # Sampling of BOTH levels up front: level 2's FPS needs level 1's centroids only, so it runs on a side stream while
-    # the main stream does level 1's ball query + MLP (the FPS kernels occupy one CTA per cloud: 32 of 148 SMs).
+    # the main stream does level 1's ball query + MLP (the FPS kernels occupy one CTA per cloud: 32 of 132 SMs).
     _, l1_new = ops.farthest_point_sample_and_gather(512, l0_xyz)
     main = torch.cuda.current_stream()
     side = _side_stream(point_cloud.device)

@@ -1,4 +1,4 @@
-"""PointNet++ layers on the B200 kernels: same names, argument order and return values as
+"""PointNet++ layers on the libpsa kernels: same names, argument order and return values as
 pointnet2/utils/pointnet_util.py (plus a keyword-only ``params`` variable store, torch being stateless about
 variable scopes).  Inference mode: batch norm uses the moving averages and is folded into the fused kernels."""
 from __future__ import annotations

@@ -1,4 +1,4 @@
-"""Training mode of the PointNet++ classifier (pointnet2_cls_ssg) on the B200 kernels: forward with batch-statistics
+"""Training mode of the PointNet++ classifier (pointnet2_cls_ssg) on the libpsa kernels: forward with batch-statistics
 batch norm through every layer, backward of the fused set-abstraction levels and the FC head, Adam, and the
 data-parallel gradient all-reduce.
 

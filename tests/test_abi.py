@@ -31,17 +31,17 @@ def test_library_builds_and_exports_header_symbols():
     for s in declared:
         assert hasattr(lib, s)
     assert set(_lib.SIGNATURES) | set(_lib.INFO_SYMBOLS) == set(declared)
-    assert lib.psa_version() >= 100 and lib.psa_sm_arch() == 100
+    assert lib.psa_version() >= 100 and lib.psa_sm_arch() == 90
 
 
-def test_library_is_sm100a_only_and_uses_tensor_cores():
+def test_library_is_sm90a_only_and_uses_tensor_cores():
     from scanobjectnn_b200.build import LIB, build_library
     build_library()
     elf = subprocess.run(["cuobjdump", "-lelf", LIB], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_(\d+a?)", elf))
-    assert archs == {"100a"}, archs
+    assert archs == {"90a"}, archs
     sass = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True).stdout
-    assert "UTCHMMA" in sass and "LDTM" in sass and "STTM" in sass     # tcgen05.mma / tcgen05.ld / tcgen05.st
+    assert "HGMMA" in sass and "UBLKCP" in sass     # wgmma.mma_async / cp.async.bulk
 
 
 def test_invalid_arguments_are_rejected_without_a_gpu():

@@ -1,4 +1,4 @@
-"""Golden vectors produced by the REFERENCE's own code (tests/golden/make_golden.py: its CUDA kernels run on a B200,
+"""Golden vectors produced by the REFERENCE's own code (tests/golden/make_golden.py: its CUDA kernels run on the GPU,
 its CPU ops run on x86-64).  CPU half: the oracle restatement must reproduce them bit for bit -- this is what pins
 the oracle.  GPU half (-m gpu): this repo's kernels must reproduce them too."""
 import os

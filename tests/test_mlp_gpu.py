@@ -25,8 +25,8 @@ def _store(seed=0):
 
 @pytest.fixture(params=["tensor", "fma", "tensor_bf16x3"])
 def mlp_mode(request):
-    """0 = auto (tcgen05 kernels where the shapes allow: fp16x2 operands + range guard), 1 = fp32 FMA kernels,
-    2 = tcgen05 kernels with bf16x3 operands (also what the range guard reruns on)"""
+    """0 = auto (tensor-core kernels where the shapes allow: fp16x2 operands + range guard), 1 = fp32 FMA kernels,
+    2 = tensor-core kernels with bf16x3 operands (also what the range guard reruns on)"""
     ops.set_mlp_mode({"tensor": 0, "fma": 1, "tensor_bf16x3": 2}[request.param])
     yield request.param
     ops.set_mlp_mode(0)
@@ -36,7 +36,7 @@ def mlp_mode(request):
                                                (300, 1, [131, 128, 40]), (640, 32, [64, 64]), (2 * 2048, 2048, [320, 1024]),
                                                (1280, 8, [6, 64, 128]),
                                                # dense tensor-core kernels, edge shapes: partial row tile + K tail; odd K (scalar x loads);
-                                               # pool 32 / 64 / 256 (atomicMax path); K > 512 and N = 64 (TMEM-A kernel); 8 K-blocks x 3 n-tiles
+                                               # pool 32 / 64 / 256 (atomicMax path); K > 512 and N = 64; 8 K-blocks x 3 n-tiles
                                                (1000, 1, [100, 128]), (1000, 1, [99, 256]), (1024, 32, [64, 128, 256]), (1024, 64, [128, 128]),
                                                (512, 256, [200, 128]), (384, 1, [576, 128]), (384, 1, [64, 64]), (130, 1, [512, 384])])
 def test_shared_mlp_matches_fp64(rows, pool_k, chans, mlp_mode):

@@ -1,5 +1,5 @@
-"""GPU parity: this repo's sm_100a kernels (through the C ABI via scanobjectnn_b200.ops) against
-(1) the CPU oracle and (2) the REFERENCE's own CUDA kernels compiled for sm_100a (oracle/_ref/libref_tfops.so).
+"""GPU parity: this repo's sm_90a kernels (through the C ABI via scanobjectnn_b200.ops) against
+(1) the CPU oracle and (2) the REFERENCE's own CUDA kernels compiled for sm_90a (oracle/_ref/libref_tfops.so).
 Index outputs must be bit-exact."""
 import numpy as np
 import pytest

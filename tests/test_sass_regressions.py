@@ -1,12 +1,7 @@
 """SASS-level regression checks on the built library (cuobjdump, no GPU needed).
 
-The tensor-core kernels depend on two code-generation properties that a harmless-looking source change can lose:
-  * tcgen05.mma must be issued on the UNIFORM datapath.  When the compiler cannot prove the issuer warp converged and the
-    operands warp-uniform, it wraps every UTCHMMA in ELECT / R2UR(.BROADCAST) sequences -- measured ~110 cycles per MMA
-    instead of the 32 / 64 the tensor pipe needs (DESIGN.md 3.3, tools/microbench/mma_rate.cu).  Guard: the kernel-wide R2UR count stays near one per UTCHMMA (the broken state is 4-5 per UTCHMMA; the
-    dual kernel has ~110 R2UR of fixed overhead for 72 (fp16x2) or 144 (bf16x3) UTCHMMA).
-  * the hot kernels really contain the Blackwell instructions they are written for (UTCHMMA, TMEM loads/stores, bulk
-    copies, mbarrier waits), i.e. nothing fell back to a generic path."""
+The hot kernels really contain the Hopper instructions they are written for (HGMMA = wgmma, bulk copies, mbarrier waits),
+i.e. nothing fell back to a generic path, and the index kernels keep their code shape."""
 import os
 import re
 import shutil
@@ -46,61 +41,48 @@ def _kernels(sass, pattern):
     return ks
 
 
-@pytest.mark.parametrize("pattern,fixed", [("tc_sa_dual_kernel", 90), ("tc_dense3_kernel", 20), ("tc_dense2_kernel", 8)])
-def test_mma_issue_stays_on_the_uniform_datapath(sass, pattern, fixed):
-    """R2UR count <= the kernel's fixed set-up moves + one per UTCHMMA.  (Healthy: dual 80-120 R2UR for 36-144 UTCHMMA, dense
-    16-18 for 12-72; broken: 4-5 R2UR per UTCHMMA on top.)  Both operand splits (fp16x2: half the MMAs) are instantiated."""
-    ks = _kernels(sass, pattern)
-    assert len(ks) >= 2, f"{pattern}: expected the fp16x2 and bf16x3 instantiations, got {list(ks)}"
-    for name, lines in ks.items():
-        mma, r2ur = _count(lines, "UTCHMMA"), _count(lines, r"R2UR(\.\w+)*")
-        assert mma >= 12, (name, mma)
-        assert r2ur <= fixed + mma, f"{name}: {r2ur} R2UR for {mma} UTCHMMA -- the MMA operands left the uniform datapath"
-
-
-def test_default_kernels_contain_the_blackwell_instructions(sass):
-    for pattern, needed in {"tc_sa_dual_kernel": ["UTCHMMA", "LDTM", "STTM", "UBLKCP", "SYNCS", "UTCBAR"],
-                            "tc_dense3_kernel": ["UTCHMMA", "LDTM", "UBLKCP", "SYNCS", "UTCBAR"],
-                            "tc_dense2_kernel": ["UTCHMMA", "LDTM", "STTM", "UBLKCP", "SYNCS", "UTCBAR"]}.items():
-        for name, lines in _kernels(sass, pattern).items():
+def test_default_kernels_contain_the_hopper_instructions(sass):
+    for pattern, needed in {"tc_sa_kernel": ["HGMMA", "UBLKCP", "SYNCS"],
+                            "tc_dense_kernel": ["HGMMA", "UBLKCP", "SYNCS"],
+                            "knn_tc_kernel": ["HGMMA", "UBLKCP", "SYNCS"]}.items():
+        ks = _kernels(sass, pattern)
+        for name, lines in ks.items():
             text = "\n".join(lines)
             for mn in needed:
                 assert re.search(r"\b" + mn, text), f"{name}: no {mn} in SASS"
+            assert _count(lines, r"HGMMA(\.\w+)*") >= 12, name
+    assert len(_kernels(sass, "tc_sa_kernel")) >= 2 and len(_kernels(sass, "tc_dense_kernel")) >= 2     # fp16x2 and bf16x3 instantiations
 
 
-def test_index_kernels_use_packed_f32x2_and_redux(sass):
+def test_index_kernels_use_redux(sass):
     fps = "\n".join(l for k, v in _kernels(sass, "fps_kernel").items() for l in v)
-    assert re.search(r"\bFFMA2\b|\bFMUL2\b|\bFADD2\b", fps), "FPS lost its packed f32x2 distance math"
     assert re.search(r"\bREDUX\b|\bCREDUX\b", fps), "FPS lost its warp REDUX arg-max"
 
 
 def test_streaming_f1_kernel_keeps_its_code_shape(sass):
-    """sa_conv1_stream_kernel (north_star's named kernel, DESIGN.md 3.5): the search runs on the packed f32x2 pipe with funnel shifts
-    collecting the sign masks (no per-word ballots: VOTE only in the extraction's bookkeeping), the warpgroups re-partition their
-    registers with setmaxnreg, the output leaves in 128-bit evict-first streaming stores, and the 128-register search stage does not
-    spill beyond a few words."""
+    """sa_conv1_stream_kernel (DESIGN.md 3.5): the search is unrolled over the thread's point pairs with funnel shifts collecting the
+    sign masks (no per-word ballots: VOTE only in the extraction's bookkeeping), the warpgroups re-partition their registers with
+    setmaxnreg, the output leaves in 128-bit evict-first streaming stores, and the 128-register search stage does not spill beyond a
+    few words."""
     ks = _kernels(sass, "sa_conv1_stream_kernel")
     assert len(ks) == 12, sorted(ks)                  # NV in {2, 4} x HAS_U x PPTP in {8, 16, 32}
     for name, lines in ks.items():
         text = "\n".join(lines)
         pptp = int(re.search(r"ELi(\d+)EEEv", name).group(1))
         pairs = pptp // 2                             # point pairs per thread = unrolled distance tests
-        assert _count(lines, "FMUL2") >= pairs and _count(lines, "FFMA2") >= 2 * pairs and _count(lines, "FADD2") >= 4 * pairs, name
+        assert _count(lines, "FMUL") >= 2 * pairs and _count(lines, "FFMA") >= 4 * pairs and _count(lines, "FADD") >= 8 * pairs, name
         assert _count(lines, r"SHF(\.\w+)*") >= 2 * pairs, f"{name}: the sign-mask funnel shifts are gone"
         assert _count(lines, r"VOTE(\.\w+)*") <= 8, f"{name}: ballots are back in the search"
         assert _count(lines, "USETMAXREG") >= 3, f"{name}: no setmaxnreg"
         assert re.search(r"STG\.E\.EF\.128", text), f"{name}: output no longer leaves in 128-bit evict-first stores"
-        assert _count(lines, r"STL(\.\w+)*") <= 16 and _count(lines, r"LDL(\.\w+)*") <= 16, f"{name}: register spills"
+        assert _count(lines, r"STL(\.\w+)*") <= 40 and _count(lines, r"LDL(\.\w+)*") <= 40, f"{name}: register spills"   # scalar f32 pairs on sm_90: more live registers
         assert not re.search(r"\bRED\b|\bATOMG\b.*\.F32", text), f"{name}: float atomics in the statistics"
 
 
-def test_transposed_sa_level_pools_in_thread(sass):
-    """tc_sa_dual_kernel<3,2> (64-wide levels, last layer transposed: DESIGN.md 3.3): with lane = channel the max over a neighbourhood
-    is an in-thread FMNMX3 chain -- the shuffle butterfly of the row-form kernels (45-78 SHFL) must not come back -- and the last
-    layer's MMAs take both operands from shared memory (H written by the previous epilogue with swizzled STS)."""
-    (name, lines), = _kernels(sass, "tc_sa_dual_kernelILi3ELi2E").items()
-    assert _count(lines, "FMNMX3") >= 16, name
-    assert _count(lines, r"SHFL(\.\w+)*") <= 16, f"{name}: the max-pool shuffles are back"
-    assert _count(lines, r"STS(\.\w+)*") >= 40, f"{name}: H is no longer written to shared memory"
-    rows = [v for k, v in _kernels(sass, "tc_sa_dual_kernelILi1ELi2E").items()][0]
-    assert _count(rows, r"SHFL(\.\w+)*") > 2 * _count(lines, r"SHFL(\.\w+)*")
+def test_wgmma_sequences_are_not_serialized(sass):
+    """Every HGMMA kernel issues its wgmma in straight-line groups: one WARPGROUP.ARRIVE per group, not one per HGMMA.  (ptxas
+    inserts an arrive before each wgmma -- and serialises them, warning C7520 -- when the issue sits on a runtime-predicated path.)"""
+    for pattern in ("tc_sa_kernel", "tc_dense_kernel", "knn_tc_kernel"):
+        for name, lines in _kernels(sass, pattern).items():
+            hgmma, arrive = _count(lines, r"HGMMA(\.\w+)*"), _count(lines, r"WARPGROUP\.ARRIVE")
+            assert arrive >= 1 and 4 * arrive <= hgmma, f"{name}: {arrive} WARPGROUP.ARRIVE for {hgmma} HGMMA -- the wgmma are serialized"

@@ -1,4 +1,4 @@
-"""tcgen05 path: the arithmetic-mode switch, and one dense tensor-core layer in isolation against fp64 (descriptor / TMEM layout /
+"""Tensor-core path: the arithmetic-mode switch, and one dense tensor-core layer in isolation against fp64 (descriptor / fragment layout /
 swizzle check: structured rows and columns that a layout mix-up would move)."""
 import numpy as np
 import pytest

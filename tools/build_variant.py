@@ -23,7 +23,7 @@ with cf.ThreadPoolExecutor(max_workers=8) as ex:
     for r in ex.map(lambda c: subprocess.run(c, capture_output=True, text=True), jobs):
         if r.returncode != 0:
             sys.exit(r.stdout + r.stderr)
-r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", lib, *objs, "-lcudart"], capture_output=True, text=True)
+r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", lib, *objs, "-lcudart"], capture_output=True, text=True)
 if r.returncode != 0:
     sys.exit(r.stdout + r.stderr)
 print(lib)

@@ -1,5 +1,5 @@
-// write_bw.cu -- ceiling for a pure write stream on B200 (what the F1 kernel's 134 MB output can reach at best).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o write_bw write_bw.cu && ./write_bw
+// write_bw.cu -- ceiling for a pure write stream on H100 (what the F1 kernel's 134 MB output can reach at best).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o write_bw write_bw.cu && ./write_bw
 // Variants: per-lane st.global.cs.v4 (streaming), plain st.global.v4, cp.async.bulk shared->global (16 KB chunks).
 // Each is timed (a) isolated: 256 MB read-flush of L2 in front (clean lines), one launch; (b) steady state: 20 launches
 // back to back into the same buffer (every byte has to reach HBM).
