@@ -285,7 +285,7 @@ PSA_API int psa_edgeconv_infer(int b, int n, int c, int k, const float* x, const
 /* DGCNN kNN graph with the X.X^T contraction on the tensor cores and an exact refine (csrc/knn_tc.cu): same result as
  * psa_knn_graph -- indices bit-identical to the canonical fp32 evaluation (dot as an fma chain over the channels,
  * adj = (|p|^2 + (-2 dot)) + |q|^2, k smallest, lower index first on ties; dgcnn/utils/tf_util.py:638-671) -- for
- * 128 <= n <= 2048, c <= 64, k <= 64; other shapes (or a workspace smaller than psa_knn_graph_workspace_bytes) run the
+ * 128 <= n <= 2048, c <= 64, k <= 32; other shapes (or a workspace smaller than psa_knn_graph_workspace_bytes) run the
  * fp32 kernel of psa_knn_graph.  workspace: bf16x3 images of the clouds, their canonical norms, the exhaustive-row worklist. */
 PSA_API size_t psa_knn_graph_workspace_bytes(int b, int n, int c, int k);
 PSA_API int psa_knn_graph_ws(int b, int n, int c, int k, const float* x, int* nn_idx, void* workspace, size_t workspace_bytes,

@@ -8,7 +8,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("PSA_LIB_PATH") or os.path.join(_HERE, "libpsa.so")   # PSA_LIB_PATH: instrumented builds of tools/
+LIB_PATH = os.path.join(_HERE, "libpsa.so")
 
 PSA_MAX_MLP_LAYERS = 4
 

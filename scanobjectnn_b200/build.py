@@ -21,7 +21,6 @@ NVCC_FLAGS = [
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-Xcompiler", "-fvisibility=hidden",
-    *os.environ.get("PSA_EXTRA_NVCC_FLAGS", "").split(),      # debug builds only, e.g. -DPSA_KNN_ERRSTAT (tools/knn_tc_timing.py)
 ]
 
 

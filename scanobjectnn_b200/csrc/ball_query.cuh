@@ -472,9 +472,5 @@ __device__ __forceinline__ int bq_extract_bitmap_sub(const unsigned* __restrict_
     for (int l = cnt + sub; l < nsample; l += LPQ) idxrow[l] = fillv;
     return cnt;
 }
-template <int WPS>
-__device__ __forceinline__ int bq_extract_bitmap_sub8(const unsigned* __restrict__ bitmap, int nsample, int* __restrict__ idxrow, int lane, bool active) {
-    return bq_extract_bitmap_sub<8, WPS>(bitmap, nsample, idxrow, lane, active);
-}
 
 }  // namespace psa

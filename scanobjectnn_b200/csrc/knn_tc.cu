@@ -409,11 +409,6 @@ __global__ void __launch_bounds__(kKtThreads, 1) knn_tc_kernel(const __grid_cons
                     can = knn_canonical(xq, xc + (size_t)col * a.c, a.c, sqqo, __ldg(sqo + col));
                 }
                 lcan[e * 128 + r] = can;
-#ifdef PSA_KNN_ERRSTAT
-                // diagnostic build (tools/knn_tc_timing.py): largest observed |fine - canonical| / E2 over the ambiguous entries
-                atomicMax(a.flag_count + 1, __float_as_uint(fabsf(ladj[e * 128 + r] - can) / (0.5f * delta)));
-                atomicAdd(a.flag_count + 2, 1u);
-#endif
             }
         }
         asm volatile("bar.sync 2, %0;" ::"n"(128 * kKtRowT) : "memory");
@@ -521,6 +516,7 @@ extern "C" int psa_knn_graph(int b, int n, int c, int k, const float* x, int* nn
 extern "C" int psa_knn_graph_ws(int b, int n, int c, int k, const float* x, int* nn_idx, void* workspace, size_t workspace_bytes,
                                 psa_stream_t stream) {
     PSA_REQUIRE(b >= 0 && n >= 0 && c >= 0 && k >= 0, "knn_graph: negative dimension");
+    PSA_REQUIRE(k <= n || b == 0, "knn_graph: k=%d exceeds the number of points n=%d", k, n);
     if (b == 0 || n == 0 || k == 0) return PSA_OK;
     const size_t need = psa_knn_graph_workspace_bytes(b, n, c, k);
     if (need == 0 || workspace == nullptr || workspace_bytes < need || b > 65535) return psa_knn_graph(b, n, c, k, x, nn_idx, stream);
@@ -539,7 +535,7 @@ extern "C" int psa_knn_graph_ws(int b, int n, int c, int k, const float* x, int*
     float* sqc = reinterpret_cast<float*>(ws);
     ws += ((size_t)b * npad * 4 + 255) & ~(size_t)255;
     float* mu = reinterpret_cast<float*>(ws);
-    PSA_CUDA(cudaMemsetAsync(flag_count, 0, 4 * sizeof(unsigned), st));       // [0] worklist length (+ [1..2] PSA_KNN_ERRSTAT diagnostics)
+    PSA_CUDA(cudaMemsetAsync(flag_count, 0, 4 * sizeof(unsigned), st));       // [0] worklist length
     knn_centre_kernel<<<b, 64 * kKtMeanLanes, 0, st>>>(n, c, x, mu);
     knn_prep_kernel<<<dim3(NT, b), 128, 0, st>>>(n, npad, c, x, mu, image, sq, sqc);
     int rc = check_launch("knn_prep_kernel");

@@ -9,8 +9,8 @@
 //   coalesced streaming store of (B,m,K,C1) + idx/pts_cnt + per-channel sum / sum-of-squares for the BN statistics.
 // HBM traffic = algorithmic traffic: B*(12n + 12m) in, 4*B*m*K*(C1+1) + 4*B*m out  (137.3 MB at B=32,N=2048,m=512,K=32,
 // C1=64) -- a pure write-bound kernel, the one BASELINE.json's ">= 70 % of the HBM roofline" target is defined on.
-#include <stdlib.h>
-
+// Two kernels: the streaming kernel below whenever f1s_plan accepts the shape (n <= 4096, nsample <= 128, <= 110 KB of
+// shared memory), the round-1 kernel sa_conv1_prebn_kernel (+ f1_stats_reduce_kernel for the statistics) otherwise.
 #include <atomic>
 
 #include "ball_query.cuh"
@@ -140,7 +140,7 @@ sa_conv1_prebn_kernel(const __grid_constant__ F1Args a) {
 
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Streaming F1 kernel (round 2, default): the same front as above, organised so that the only thing the SMs do for most of
+// Streaming F1 kernel (round 2, wherever f1s_plan fits): the same front as above, organised so that the only thing the SMs do for most of
 // the launch is stream the (B,m,K,C1) tensor out.
 //   * persistent CTAs (2 per SM, 12 warps), each owning a contiguous range of the B*m queries; when the grid is a multiple of
 //     B every CTA stays inside one cloud (ranges that cross a cloud boundary reload the cloud and re-ramp the pipeline);
@@ -163,7 +163,6 @@ sa_conv1_prebn_kernel(const __grid_constant__ F1Args a) {
 // Statistics: per-CTA partials in a fixed order, the last CTA to finish (ticket) adds them in fp64 in CTA order:
 // deterministic, one launch.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int kF1SThreads = 256;
 constexpr int kF1WThreads = 384;           // streaming kernel: one warpgroup of search warps + two of worker warps
 constexpr int kF1NP = 4;
 constexpr int kF1Batch = 8;                // smallest full batch (two queries per worker warp, four worker warps): sizes the grid
@@ -189,16 +188,10 @@ struct F1SArgs {
     float* partial;        // (gridDim.x, 2, C1)
     float* stats;          // (2, C1) or null
     int ticket;            // index into g_f1_tickets
-    unsigned long long* tlog;   // PSA_F1_TIMING builds: (gridDim.x, 8) globaltimer stamps, else null
 };
 
 __device__ __forceinline__ void named_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(int id, int count) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory"); }
-__device__ __forceinline__ unsigned long long gtime() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
 
 // Batches of a cloud segment: 2, 4, then kF1Batch queries -- the first stores of a CTA start after a 2-query search.
 __host__ __device__ inline int f1s_batch_size(int t, int qb) { return t == 0 ? 2 : (t == 1 ? 4 : qb); }
@@ -217,16 +210,6 @@ __host__ __device__ inline size_t f1s_smem_bytes(int n, int nsample, int np, int
     if (ringr < 12288) ringr = 12288;
     return (size_t)n * 16 + ringb + ringr;
 }
-
-#ifdef PSA_F1_TIMING
-__device__ __forceinline__ long long clock_after_smem(const volatile int* w) {
-    const int dep = *w;
-    long long t;
-    asm volatile("mov.u64 %0, %%clock64;" : "=l"(t) : "r"(dep) : "memory");
-    return t;
-}
-#define F1CLK() clock_after_smem(reinterpret_cast<const volatile int*>(centres))
-#endif
 
 // float pairs in 64-bit registers, each half rounded on its own (sm_90 has no packed f32x2 instructions: two scalar ops each)
 typedef unsigned long long u64;
@@ -272,16 +255,6 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
     const size_t slot_bytes = (size_t)QB * K * (sizeof(int) + sizeof(float4));                    // idx rows | centred rows
     __shared__ int4 s_hdrB[kF1Ring];                       // (first query - q_begin, queries [0 = stop], last batch of a cloud with more to come, -)
     __shared__ int2 s_hdrR[kF1Ring];                       // (first query - q_begin, queries [0 = stop])
-#ifdef PSA_F1_TIMING
-    if (tid == 0 && a.tlog) {
-        a.tlog[blockIdx.x * 8 + 0] = gtime();
-        unsigned smid;
-        asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-        a.tlog[blockIdx.x * 8 + 7] = smid;
-    }
-    long long tacc[3] = {0, 0, 0};                         // per stage (thread 0 of the stage): waiting for input, waiting for output space, working
-    long long tc0 = 0, tc1 = 0;
-#endif
 
     float2 ssum[2], ssq[2];                                // this lane's four channels (conv warps)
     ssum[0] = ssum[1] = ssq[0] = ssq[1] = make_float2(0.f, 0.f);
@@ -395,9 +368,6 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                     px[j] = f2_pack(c[0], c[3]); py[j] = f2_pack(c[1], c[4]); pz[j] = f2_pack(c[2], c[5]);
                 }
             }
-#ifdef PSA_F1_TIMING
-            if (tid == 0 && a.tlog && q == q_begin) a.tlog[blockIdx.x * 8 + 1] = gtime();
-#endif
             const u64 thr2 = f2_pack(a.thr, a.thr);
             // the NEXT batch's centres are fetched under the current search
             for (int bi = 0; gq0 < seg_end; ++bi, ++ring_pos) {
@@ -413,13 +383,7 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                         ncx = __ldg(p2); ncy = __ldg(p2 + 1); ncz = __ldg(p2 + 2);
                     }
                 }
-#ifdef PSA_F1_TIMING
-                tc0 = F1CLK();
-#endif
                 if (!TWO && ring_pos >= kF1Ring) named_bar_sync(BAR_BEMPTY + slot, 2 * PT); // slot drained by the extraction
-#ifdef PSA_F1_TIMING
-                tc1 = F1CLK(); tacc[1] += tc1 - tc0;
-#endif
                 if (warp == 0 && lane < nqb) centres[bslot * QB + lane] = make_float4(cqx, cqy, cqz, 0.f);
                 if (!TWO && tid == 0) s_hdrB[slot] = make_int4((int)(gq0 - q_begin), nqb, (gq0 + nqb == seg_end && seg_end < q_end) ? 1 : 0, 0);
                 // ---- exhaustive test on float pairs: per point 3 FADD + FMUL + 2 FFMA (the reference's
@@ -465,10 +429,6 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                     __threadfence_block();
                     named_bar_arrive(BAR_BFULL + slot, 2 * PT);                             // bitmaps + centres (+ the cloud copy) ready
                 }
-#ifdef PSA_F1_TIMING
-                tacc[2] += F1CLK() - tc1;
-                if (tid == 0 && a.tlog && ring_pos == 0) a.tlog[blockIdx.x * 8 + 4] = gtime();
-#endif
                 gq0 += nqb;
             }
             q = seg_end;
@@ -492,32 +452,16 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                     if (p >= kF1Ring) named_bar_sync(BAR_BEMPTY + p % kF1Ring, 2 * PT);
             }
         }
-#ifdef PSA_F1_TIMING
-        if (tid == 0 && a.tlog) {
-            a.tlog[blockIdx.x * 8 + 3] = gtime();
-            unsigned long long* t2 = a.tlog + 3 * kNumSMs * 8 + blockIdx.x * 16;
-            t2[0] = 0; t2[1] = tacc[1]; t2[2] = tacc[2];
-        }
-#endif
     } else if (!TWO && warp < 2 * NP) {
         // =========================================== EXTRACT ===========================================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
         const int ew = warp - NP, et = tid - PT;
         for (int ring_pos = 0;; ++ring_pos) {
             const int slot = ring_pos % kF1Ring;
-#ifdef PSA_F1_TIMING
-            tc0 = F1CLK();
-#endif
             named_bar_sync(BAR_BFULL + slot, 2 * PT);
-#ifdef PSA_F1_TIMING
-            tc1 = F1CLK(); tacc[0] += tc1 - tc0;
-#endif
             const int4 hdr = s_hdrB[slot];
             const int nqb = hdr.y;
             if (ring_pos >= kF1Ring) named_bar_sync(BAR_REMPTY + slot, RCNT);               // rows slot drained by the conv warps
-#ifdef PSA_F1_TIMING
-            tc0 = F1CLK(); tacc[1] += tc0 - tc1;
-#endif
             if (nqb == 0) {                                                                 // stop: pass it on, take the outstanding releases
                 named_bar_arrive(BAR_BEMPTY + slot, 2 * PT);
                 if (et == 0) s_hdrR[slot] = make_int2(0, 0);
@@ -533,16 +477,7 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
             __threadfence_block();
             named_bar_arrive(BAR_RFULL + slot, RCNT);
             if (hdr.z) named_bar_arrive(BAR_CLOUD, 2 * PT);                                 // last batch of this cloud: its copy is free
-#ifdef PSA_F1_TIMING
-            tacc[2] += F1CLK() - tc0;
-#endif
         }
-#ifdef PSA_F1_TIMING
-        if (tid == PT && a.tlog) {
-            unsigned long long* t2 = a.tlog + 3 * kNumSMs * 8 + blockIdx.x * 16;
-            t2[3] = tacc[0]; t2[4] = tacc[1]; t2[5] = tacc[2];
-        }
-#endif
     } else {
         // =========================================== CONV + STORE ===========================================
         // lane mapping: LPR = C1/4 lanes cover one row (4 consecutive channels each), so a warp store instruction writes
@@ -561,14 +496,7 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
         for (int ring_pos = 0;; ++ring_pos) {
             const int slot = ring_pos % kF1Ring;
             const float4* sd = reinterpret_cast<const float4*>(ring + slot * slot_bytes + (size_t)QB * K * sizeof(int));
-#ifdef PSA_F1_TIMING
-            tc0 = F1CLK();
-#endif
             named_bar_sync(BAR_RFULL + slot, RCNT);
-#ifdef PSA_F1_TIMING
-            tc1 = F1CLK(); tacc[0] += tc1 - tc0;
-            if (tid == CONV0 * 32 && a.tlog && ring_pos == 0) a.tlog[blockIdx.x * 8 + 2] = gtime();
-#endif
             const int2 hdr = s_hdrR[slot];
             const int nqb = hdr.y;
             if (nqb == 0) { named_bar_arrive(BAR_REMPTY + slot, RCNT); break; }               // stop marker
@@ -611,17 +539,7 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
                 }
             }
             named_bar_arrive(BAR_REMPTY + slot, RCNT);
-#ifdef PSA_F1_TIMING
-            tacc[2] += F1CLK() - tc1;
-#endif
         }
-#ifdef PSA_F1_TIMING
-        if (tid == CONV0 * 32 && a.tlog) {
-            a.tlog[blockIdx.x * 8 + 5] = gtime();
-            unsigned long long* t2 = a.tlog + 3 * kNumSMs * 8 + blockIdx.x * 16;
-            t2[6] = tacc[0]; t2[7] = 0; t2[8] = tacc[2];
-        }
-#endif
     }
 
     // back to the launch allocation (80 registers each) for the common epilogue
@@ -693,256 +611,6 @@ sa_conv1_stream_kernel(const __grid_constant__ F1SArgs a) {
             if (tid == 0) g_f1_tickets[a.ticket] = 0u;     // ready for the next launch that draws this ticket
         }
     }
-#ifdef PSA_F1_TIMING
-    if (tid == 0 && a.tlog) a.tlog[blockIdx.x * 8 + 6] = gtime();
-#endif
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Synchronous streaming F1 kernel: no warp specialisation.  In the producer / consumer kernel above the four consumer warps sit
-// at the FULL barrier ~80 % of the time (the exhaustive search is the long pole, the stores are fire-and-forget), so here ALL
-// eight warps do every phase of a batch in turn:
-//   search    each warp holds PPT points per lane in registers (point k = 32 (warp + 8 i) + lane) and tests them against the
-//             batch's queries; one ballot per 32-point word IS that word of the query's hit bitmap;
-//   extract   8 lanes per query read the nsample lowest set bits out in order (idx rows, pts_cnt);
-//   rows      centred coordinates (dx,dy,dz,j) of the batch's rows into shared memory, idx to global memory;
-//   conv      LPR lanes per row x 4 channels, weights in registers, whole rows per store instruction (512 contiguous bytes),
-//             streaming stores, BN statistics in registers.
-// The stores of batch t drain while batch t+1 is searched; 2-3 CTAs per SM interleave their phases.  Batches ramp 2, 4, 8, 16
-// queries so the first stores leave ~3 us after launch.
-// ---------------------------------------------------------------------------------------------------------------------
-constexpr int kF1YBatch = 16;
-__host__ __device__ inline int f1y_batch_size(int t) { return t == 0 ? 2 : (t == 1 ? 4 : (t == 2 ? 8 : kF1YBatch)); }
-__host__ __device__ inline size_t f1y_smem_bytes(int n, int nsample, int ppt) {
-    const int bw = 8 * ppt < 32 ? 32 : 8 * ppt;
-    size_t rest = (size_t)kF1YBatch * bw * 4 + (size_t)kF1YBatch * nsample * (sizeof(int) + sizeof(float4)) + kF1YBatch * sizeof(float4);
-    if (rest < 8192 + 2048) rest = 8192 + 2048;              // the statistics epilogue reuses this area (up to 8 KB + 2 KB)
-    return (size_t)n * 16 + rest;
-}
-
-template <int NV, bool HAS_U, int PPT>
-__global__ void __launch_bounds__(kF1SThreads, PPT <= 8 ? 3 : 2)
-sa_conv1_sync_kernel(const __grid_constant__ F1SArgs a) {
-    constexpr int BW = 8 * PPT < 32 ? 32 : 8 * PPT;        // bitmap words per query
-    constexpr int LPR = NV * 8;                            // lanes per row (4 channels each): 16 (C1 = 64) or 32 (C1 = 128)
-    constexpr int RPI = 32 / LPR;                          // rows per store instruction
-    extern __shared__ __align__(16) float smem_f[];
-    const int n = a.n, K = a.nsample, C1 = a.C1;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    float4* cloud4 = reinterpret_cast<float4*>(smem_f);
-    unsigned* bitmaps = reinterpret_cast<unsigned*>(cloud4 + n);                                  // kF1YBatch x BW
-    int* sidx = reinterpret_cast<int*>(bitmaps + kF1YBatch * BW);                                 // kF1YBatch x K
-    float4* sd = reinterpret_cast<float4*>(sidx + kF1YBatch * K);                                 // kF1YBatch x K
-    float4* sctr = sd + kF1YBatch * K;                                                            // kF1YBatch
-    float* scratch = reinterpret_cast<float*>(bitmaps);                                           // epilogue reuse
-#ifdef PSA_F1_TIMING
-    if (tid == 0 && a.tlog) a.tlog[blockIdx.x * 8 + 0] = gtime();
-#endif
-    for (int i = tid; i < kF1YBatch * BW; i += kF1SThreads) bitmaps[i] = 0u;     // words no warp owns (BW > 8 PPT) stay zero
-
-    // conv: this lane's four channels
-    const int lr = lane / LPR, lc = (lane % LPR) * 4;
-    const float4 wx4 = __ldg(reinterpret_cast<const float4*>(a.w1 + lc));
-    const float4 wy4 = __ldg(reinterpret_cast<const float4*>(a.w1 + C1 + lc));
-    const float4 wz4 = __ldg(reinterpret_cast<const float4*>(a.w1 + 2 * C1 + lc));
-    const float4 b4 = a.bias ? __ldg(reinterpret_cast<const float4*>(a.bias + lc)) : make_float4(0.f, 0.f, 0.f, 0.f);
-    const float2 wxa = make_float2(wx4.x, wx4.y), wxb = make_float2(wx4.z, wx4.w), wya = make_float2(wy4.x, wy4.y), wyb = make_float2(wy4.z, wy4.w);
-    const float2 wza = make_float2(wz4.x, wz4.y), wzb = make_float2(wz4.z, wz4.w), ba = make_float2(b4.x, b4.y), bb = make_float2(b4.z, b4.w);
-    float2 ssum[2], ssq[2];
-    ssum[0] = ssum[1] = ssq[0] = ssq[1] = make_float2(0.f, 0.f);
-
-    const long long T = (long long)a.b * a.m;
-    const long long q_begin = T * blockIdx.x / gridDim.x, q_end = T * (blockIdx.x + 1) / gridDim.x;
-    bool first = true;
-    for (long long q = q_begin; q < q_end;) {
-        const long long cloud = q / a.m;
-        const long long seg_end = min(q_end, (cloud + 1) * (long long)a.m);
-        const float* gx = a.xyz + (size_t)cloud * n * 3;
-        const float* ucloud = HAS_U ? a.uf + (size_t)cloud * n * C1 + lc : nullptr;
-        // ---- this cloud: PPT points per thread in registers, float4 copy in shared memory ----
-        __syncthreads();                                       // the previous cloud's copy / batch buffers are no longer read
-        float2 px[PPT / 2], py[PPT / 2], pz[PPT / 2];
-        unsigned valid = 0u;
-        const float pinf = __int_as_float(0x7f800000);
-#pragma unroll
-        for (int i = 0; i < PPT; ++i) {
-            const int k = 32 * (warp + 8 * i) + lane;
-            float x = pinf, y = pinf, z = pinf;                // slots past the cloud: out of reach of every finite query
-            if (k < n) {
-                x = __ldg(gx + 3 * k); y = __ldg(gx + 3 * k + 1); z = __ldg(gx + 3 * k + 2);
-                cloud4[k] = make_float4(x, y, z, __int_as_float(k));
-                valid |= 1u << i;
-            }
-            if (i & 1) { px[i >> 1].y = x; py[i >> 1].y = y; pz[i >> 1].y = z; }
-            else { px[i >> 1].x = x; py[i >> 1].x = y; pz[i >> 1].x = z; }
-        }
-        __syncthreads();
-#ifdef PSA_F1_TIMING
-        if (tid == 0 && a.tlog && first) a.tlog[blockIdx.x * 8 + 1] = gtime();
-#endif
-        long long gq0 = q;
-        for (int bi = 0; gq0 < seg_end; ++bi) {
-            const int nqb = min(f1y_batch_size(bi), (int)(seg_end - gq0));
-            // ---- search ----
-            float cqx = 0.f, cqy = 0.f, cqz = 0.f;
-            if (lane < nqb) {
-                const float* p2 = a.new_xyz + (size_t)(gq0 + lane) * 3;
-                cqx = __ldg(p2); cqy = __ldg(p2 + 1); cqz = __ldg(p2 + 2);
-                if (warp == 0) sctr[lane] = make_float4(cqx, cqy, cqz, 0.f);
-            }
-            if (!a.none) {
-                for (int qi = 0; qi < nqb; ++qi) {
-                    const float qx = __shfl_sync(0xffffffffu, cqx, qi), qy = __shfl_sync(0xffffffffu, cqy, qi), qz = __shfl_sync(0xffffffffu, cqz, qi);
-                    const float2 nqx = make_float2(-qx, -qx), nqy = make_float2(-qy, -qy), nqz = make_float2(-qz, -qz);
-                    unsigned mine = 0u;                        // lane i keeps word i of this warp's share, stored once
-                    const bool qfinite = fabsf(qx) <= 3.0e38f && fabsf(qy) <= 3.0e38f && fabsf(qz) <= 3.0e38f;   // warp-uniform
-                    if (qfinite) {
-#pragma unroll
-                        for (int i = 0; i < PPT; i += 2) {
-                            const float2 d = bq_dist2_pair(px[i >> 1], py[i >> 1], pz[i >> 1], nqx, nqy, nqz);
-                            // !(d > thr): a NaN distance (NaN point) counts as inside, exactly like the reference's max(sqrtf(NaN),1e-20f) < r
-                            const unsigned w0 = __ballot_sync(0xffffffffu, !(d.x > a.thr));
-                            const unsigned w1 = __ballot_sync(0xffffffffu, !(d.y > a.thr));
-                            if (lane == i) mine = w0;
-                            if (lane == i + 1) mine = w1;
-                        }
-                    } else {
-                        // non-finite query: every distance is NaN = inside; only the slots past the cloud are masked out
-#pragma unroll
-                        for (int i = 0; i < PPT; i += 2) {
-                            const float2 d = bq_dist2_pair(px[i >> 1], py[i >> 1], pz[i >> 1], nqx, nqy, nqz);
-                            const unsigned w0 = __ballot_sync(0xffffffffu, !(d.x > a.thr) && ((valid >> i) & 1u));
-                            const unsigned w1 = __ballot_sync(0xffffffffu, !(d.y > a.thr) && ((valid >> (i + 1)) & 1u));
-                            if (lane == i) mine = w0;
-                            if (lane == i + 1) mine = w1;
-                        }
-                    }
-                    if (lane < PPT) bitmaps[qi * BW + warp + 8 * lane] = mine;
-                }
-            }
-            __syncthreads();                                   // bitmaps complete
-#ifdef PSA_F1_TIMING
-            if (tid == 0 && a.tlog && first && bi == 0) a.tlog[blockIdx.x * 8 + 4] = gtime();
-#endif
-            // ---- bitmaps -> ordered idx rows: 8 lanes per query, 4 queries per warp pass ----
-            for (int q0 = warp * 4; q0 < nqb; q0 += 32) {
-                const int qi = q0 + (lane >> 3);
-                const bool act = qi < nqb;
-                const int cnt = bq_extract_bitmap_sub8<BW / 8>(bitmaps + qi * BW, K, sidx + qi * K, lane, act);
-                if (act && a.pts_cnt != nullptr && (lane & 7) == 0) a.pts_cnt[gq0 + qi] = cnt;
-            }
-            __syncthreads();                                   // idx rows complete
-            // ---- centred rows + idx to global memory ----
-            const int nrows = nqb * K;
-            int* gidx = a.idx + (size_t)gq0 * K;
-            for (int r = tid; r < nrows; r += kF1SThreads) {
-                const int j = sidx[r];
-                const float4 ctr = sctr[r / K];
-                const float4 pt = cloud4[j];
-                gidx[r] = j;
-                sd[r] = make_float4(pt.x - ctr.x, pt.y - ctr.y, pt.z - ctr.z, __int_as_float(j));
-            }
-            __syncthreads();
-#ifdef PSA_F1_TIMING
-            if (tid == 0 && a.tlog && first && bi == 0) a.tlog[blockIdx.x * 8 + 2] = gtime();
-#endif
-            // ---- conv + streaming stores: four rows per lane and trip, whole rows per store instruction ----
-            float* outl = a.pre + (size_t)gq0 * K * C1 + lc;
-            for (int r0 = warp * 4 * RPI; r0 < nrows; r0 += 8 * 4 * RPI) {
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int r = r0 + u * RPI + lr;
-                    if (r < nrows) {
-                        const float4 d = sd[r];
-                        const float2 dx = make_float2(d.x, d.x), dy = make_float2(d.y, d.y), dz = make_float2(d.z, d.z);
-                        float2 s0 = ba, s1 = bb;
-                        if (HAS_U) {
-                            const float4 uu = __ldg(reinterpret_cast<const float4*>(ucloud + (unsigned)__float_as_int(d.w) * (unsigned)C1));
-                            s0 = fadd2_rn(s0, make_float2(uu.x, uu.y)); s1 = fadd2_rn(s1, make_float2(uu.z, uu.w));
-                        }
-                        const float2 v0 = ffma2_rn(dz, wza, ffma2_rn(dy, wya, ffma2_rn(dx, wxa, s0)));
-                        const float2 v1 = ffma2_rn(dz, wzb, ffma2_rn(dy, wyb, ffma2_rn(dx, wxb, s1)));
-                        __stcs(reinterpret_cast<float4*>(outl + (unsigned)r * (unsigned)C1), make_float4(v0.x, v0.y, v1.x, v1.y));
-                        ssum[0] = fadd2_rn(ssum[0], v0); ssum[1] = fadd2_rn(ssum[1], v1);
-                        ssq[0] = ffma2_rn(v0, v0, ssq[0]); ssq[1] = ffma2_rn(v1, v1, ssq[1]);
-                    }
-                }
-            }
-            gq0 += nqb;
-            // (the next batch's search only writes the bitmaps; the batch buffers are rewritten after its first barrier, which every
-            //  warp reaches only after finishing this conv phase)
-        }
-        first = false;
-        q = seg_end;
-    }
-#ifdef PSA_F1_TIMING
-    if (tid == 0 && a.tlog) a.tlog[blockIdx.x * 8 + 5] = gtime();
-#endif
-
-    if (a.stats != nullptr) {
-        __syncthreads();
-        float* sstat = scratch;                            // 8 warps x 2 x C1 floats = up to 8 KB
-#pragma unroll
-        for (int p = 0; p < 2; ++p) {
-#pragma unroll
-            for (int o = LPR; o < 32; o <<= 1) {
-                ssum[p].x += __shfl_xor_sync(0xffffffffu, ssum[p].x, o); ssum[p].y += __shfl_xor_sync(0xffffffffu, ssum[p].y, o);
-                ssq[p].x += __shfl_xor_sync(0xffffffffu, ssq[p].x, o); ssq[p].y += __shfl_xor_sync(0xffffffffu, ssq[p].y, o);
-            }
-            if (lane < LPR) {
-                float* w = sstat + (size_t)warp * 2 * C1;
-                const int c = lane * 4 + 2 * p;
-                *reinterpret_cast<float2*>(w + c) = ssum[p];
-                *reinterpret_cast<float2*>(w + C1 + c) = ssq[p];
-            }
-        }
-        __syncthreads();
-        float* dst = a.partial + (size_t)blockIdx.x * 2 * C1;
-        for (int e = tid; e < 2 * C1; e += kF1SThreads) {
-            float t = 0.f;
-#pragma unroll
-            for (int w = 0; w < 8; ++w) t += sstat[(size_t)w * 2 * C1 + e];      // fixed order
-            dst[e] = t;
-        }
-        // last CTA to arrive adds the CTA partials (fp64) in a fixed tree: deterministic whatever the finishing order
-        __shared__ unsigned s_last;
-        __threadfence();
-        __syncthreads();
-        if (tid == 0) s_last = (atomicAdd(&g_f1_tickets[a.ticket], 1u) == gridDim.x - 1) ? 1u : 0u;
-        __syncthreads();
-        if (s_last) {
-            __threadfence();
-            const int E4 = 2 * C1 / 4;                                     // 32 (C1 = 64) or 64 (C1 = 128)
-            const int RL = kF1SThreads / E4;                               // 8 or 4
-            const int e4 = tid % E4, rl = tid / E4;
-            double acc[4] = {0.0, 0.0, 0.0, 0.0};
-            const float4* part4 = reinterpret_cast<const float4*>(a.partial);
-            for (unsigned p0 = rl; p0 < gridDim.x; p0 += 10 * RL) {
-                float4 v[10];
-#pragma unroll
-                for (int u = 0; u < 10; ++u) {
-                    const unsigned p = p0 + u * RL;
-                    v[u] = p < gridDim.x ? __ldcg(part4 + (size_t)p * E4 + e4) : make_float4(0.f, 0.f, 0.f, 0.f);
-                }
-#pragma unroll
-                for (int u = 0; u < 10; ++u) { acc[0] += (double)v[u].x; acc[1] += (double)v[u].y; acc[2] += (double)v[u].z; acc[3] += (double)v[u].w; }
-            }
-            double* sred = reinterpret_cast<double*>(scratch);             // RL x 2*C1 doubles = 8 KB
-            __syncthreads();
-#pragma unroll
-            for (int c = 0; c < 4; ++c) sred[(size_t)rl * 2 * C1 + e4 * 4 + c] = acc[c];
-            __syncthreads();
-            for (int e = tid; e < 2 * C1; e += kF1SThreads) {
-                double t = 0.0;
-                for (int r = 0; r < RL; ++r) t += sred[(size_t)r * 2 * C1 + e];
-                a.stats[e] = (float)t;
-            }
-            if (tid == 0) g_f1_tickets[a.ticket] = 0u;
-        }
-    }
-#ifdef PSA_F1_TIMING
-    if (tid == 0 && a.tlog) a.tlog[blockIdx.x * 8 + 6] = gtime();
-#endif
 }
 
 // stats[0..C1) = sum, stats[C1..2C1) = sum of squares, over all rows; CTA partials added in index order in fp64
@@ -966,12 +634,6 @@ int launch_dense_raw(long long rows, int K, int N, const float* x, const float* 
     d.rows = rows; d.K = K; d.N = N; d.pool_k = 1; d.relu = 0;
     d.x = x; d.W = W; d.scale = nullptr; d.shift = nullptr; d.out = out;
     return launch_dense(d, st);
-}
-// 0 = producer / consumer streaming kernel where it applies, 1 = round-1 kernel, 3 = synchronous streaming kernel;
-// PSA_F1_VARIANT in the environment (A/B runs of tools/ only)
-static int f1_variant() {
-    static const int v = [] { const char* e = getenv("PSA_F1_VARIANT"); return e ? atoi(e) : 0; }();
-    return v;
 }
 static void f1_grid(int b, int m, int* q_per_cta, dim3* grid) {
     int chunks = (2 * kNumSMs + b - 1) / b;
@@ -1009,9 +671,9 @@ extern "C" size_t psa_sa_conv1_prebn_workspace_bytes(int b, int n, int m, int c,
     if (want_stats) {
         int q; dim3 g;
         f1_grid(b, m, &q, &g);
-        size_t parts = (size_t)g.x * g.y;
-        if (parts < 3 * (size_t)kNumSMs) parts = 3 * (size_t)kNumSMs;      // the streaming kernels run up to 3 CTAs per SM
-        bytes += parts * 2 * C1 * sizeof(float) + 256 + 3 * (size_t)kNumSMs * 24 * sizeof(unsigned long long);   // CTA partials (+ timing stamps of debug builds)
+        size_t parts = (size_t)g.x * g.y;                                   // round-1 kernel: partials at offset 0
+        if (parts < 2 * (size_t)kNumSMs) parts = 2 * (size_t)kNumSMs;      // streaming kernel: up to 2 CTAs per SM, at offset 256
+        bytes += parts * 2 * C1 * sizeof(float) + 256;
     }
     return bytes;
 }
@@ -1046,39 +708,15 @@ extern "C" int psa_sa_conv1_prebn(int b, int n, int m, int c, float radius, int 
     {   // ---- streaming kernel (persistent CTAs, producer/consumer warps) whenever the cloud fits its shared-memory plan ----
         int ctas = 0, np = 0, pptp = 0;
         size_t ssm = 0;
-        if (f1_variant() != 1 && f1s_plan(b, n, m, nsample, &np, &pptp, &ctas, &ssm)) {
+        if (f1s_plan(b, n, m, nsample, &np, &pptp, &ctas, &ssm)) {
             F1SArgs s;
             s.b = b; s.n = n; s.m = m; s.nsample = nsample; s.C1 = C1; s.thr = a.thr; s.none = a.none;
             s.xyz = xyz; s.new_xyz = new_xyz; s.uf = a.uf; s.w1 = w1; s.bias = bias; s.pre = pre;
-            s.idx = idx; s.pts_cnt = pts_cnt; s.partial = nullptr; s.stats = stats; s.ticket = 0; s.tlog = nullptr;
+            s.idx = idx; s.pts_cnt = pts_cnt; s.partial = nullptr; s.stats = stats; s.ticket = 0;
             if (stats) {
                 static std::atomic<unsigned> call_no{0};
                 s.ticket = (int)(call_no.fetch_add(1u) % kF1Tickets);
                 s.partial = reinterpret_cast<float*>(ws + 256);
-#ifdef PSA_F1_TIMING
-                s.tlog = reinterpret_cast<unsigned long long*>(ws + 256 + (size_t)3 * kNumSMs * 2 * C1 * sizeof(float));
-#endif
-            }
-            if (f1_variant() == 3) {
-                // synchronous kernel (all warps do every phase; A/B runs: 61 us vs 57 us for the producer / consumer kernel at SA1): points per thread 4 / 8 / 16 for n <= 1024 / 2048 / 4096
-                const int ppt = n <= 1024 ? 4 : (n <= 2048 ? 8 : 16);
-                const size_t ysm = f1y_smem_bytes(n, nsample, ppt);
-                const long long T = (long long)b * m;
-                const long long units = (T + 7) / 8;
-                const int per_sm = (ppt <= 8 && ysm <= 72 * 1024) ? 3 : 2;      // matches the kernel's __launch_bounds__
-                const int yctas = (int)(units < (long long)per_sm * kNumSMs ? units : (long long)per_sm * kNumSMs);
-#define PSA_F1Y_LAUNCH(NV_, U_, PPT_)                                                                                         \
-    do {                                                                                                                     \
-        PSA_CUDA(cudaFuncSetAttribute(sa_conv1_sync_kernel<NV_, U_, PPT_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ysm)); \
-        sa_conv1_sync_kernel<NV_, U_, PPT_><<<yctas, kF1SThreads, ysm, st>>>(s);                                             \
-    } while (0)
-#define PSA_F1Y_U(NV_, PPT_) do { if (s.uf) PSA_F1Y_LAUNCH(NV_, true, PPT_); else PSA_F1Y_LAUNCH(NV_, false, PPT_); } while (0)
-#define PSA_F1Y_P(NV_) do { if (ppt == 4) PSA_F1Y_U(NV_, 4); else if (ppt == 8) PSA_F1Y_U(NV_, 8); else PSA_F1Y_U(NV_, 16); } while (0)
-                if (C1 == 64) PSA_F1Y_P(2); else PSA_F1Y_P(4);
-#undef PSA_F1Y_P
-#undef PSA_F1Y_U
-#undef PSA_F1Y_LAUNCH
-                return check_launch("sa_conv1_sync_kernel");
             }
 #define PSA_F1S_LAUNCH(NV_, U_, PP_)                                                                                          \
     do {                                                                                                                     \

@@ -1234,12 +1234,3 @@ extern "C" int psa_mlp_image_plan(int usage, long long rows, int pool_k, int c, 
     for (int l = 0; l < a.nl; ++l) { nt[1 + l] = tc_sa_image_nt(); row0[1 + l] = 0; bytes[1 + l] = tc_plan_image_bytes(a.Kd[l], a.Ntot[l]); }
     return PSA_OK;
 }
-
-#ifdef PSA_TC_TIMING
-extern "C" __attribute__((visibility("default"))) int psa_debug_tc_timing(unsigned long long* out8, int reset) {
-    cudaDeviceSynchronize();
-    if (out8) cudaMemcpyFromSymbol(out8, psa::g_tc_timing, 8 * sizeof(unsigned long long));
-    if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(psa::g_tc_timing, z, sizeof(z)); }
-    return 0;
-}
-#endif

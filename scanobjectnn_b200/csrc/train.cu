@@ -6,7 +6,6 @@
 // scatter) is a fixed-order sum -- per-CTA partials in a fixed thread order, partials added in index order in fp64.  The
 // reference's gradient kernels are float atomicAdd scatters (tf_grouping_g.cu:61-78, tf_sampling_g.cu:183-192).
 #include <math.h>
-#include <stdlib.h>
 
 #include "train_gemm.cuh"
 
@@ -17,10 +16,6 @@ bool tc_train_fwd_eligible(long long rows, int K, int N);
 size_t tc_dense_image_bytes(int K, int N);
 int launch_tc_dense_train(long long rows, int K, int N, const float* x, const float* in_scale, const float* in_shift, int in_relu,
                           const float* W, const float* bias, float* y, float* stat_partial, uint8_t* image_ws, cudaStream_t st);
-static int train_tc_enabled() {
-    static const int v = [] { const char* e = getenv("PSA_TRAIN_FP32_ONLY"); return (e && atoi(e)) ? 0 : 1; }();
-    return v;
-}
 
 // out[e] = sum_p partial[p * len + e] in a FIXED tree: block = 32 outputs x 32 chunk lanes; lane c adds its contiguous range of
 // partials in ascending order (fp64, eight loads in flight), the 32 chunk sums are added in lane order.  Deterministic, and
@@ -435,8 +430,8 @@ extern "C" int psa_train_dense_fwd(long long rows, int K, int N, const psa_act_i
         PSA_REQUIRE(workspace != nullptr && workspace_bytes >= (size_t)tiles_m * 2 * N * sizeof(float), "train_dense_fwd: workspace too small");
         o.stat_partial = reinterpret_cast<float*>(workspace);
     }
-    // wide layers: tcgen05 path (bf16x3 operands, fp32 accumulate) when the input is a plain (rows, K) tensor without dropout
-    if (train_tc_enabled() && tc_train_fwd_eligible(rows, K, N) && in->ld == K && in->mask == nullptr) {
+    // wide layers: wgmma path (bf16x3 operands, fp32 accumulate) when the input is a plain (rows, K) tensor without dropout
+    if (tc_train_fwd_eligible(rows, K, N) && in->ld == K && in->mask == nullptr) {
         const size_t stat_bytes = ((size_t)tiles_m * 2 * N * sizeof(float) + 255) & ~(size_t)255;
         PSA_REQUIRE(workspace != nullptr && workspace_bytes >= stat_bytes + tc_dense_image_bytes(K, N), "train_dense_fwd: workspace too small");
         float* sp = stats ? reinterpret_cast<float*>(workspace) : nullptr;

@@ -369,21 +369,16 @@ def knn(adj_matrix: torch.Tensor, k: int = 20) -> torch.Tensor:
     return nn_idx
 
 
-_KNN_FP32_ONLY = False      # tests / A-B runs: force the fp32 kernel
-
-
 def knn_graph(point_cloud: torch.Tensor, k: int = 20) -> torch.Tensor:
     """knn(pairwise_distance(point_cloud), k) fused -- no (B,N,N) matrix."""
     pc = _dev(_squeeze_pc(point_cloud), torch.float32, "point_cloud", 3)
     b, n, c = pc.shape
     nn_idx = torch.empty((b, n, k), dtype=torch.int32, device=pc.device)
     lib = _lib.load()
-    need = 0 if _KNN_FP32_ONLY else lib.psa_knn_graph_workspace_bytes(b, n, c, k)
-    if need:        # tensor-core contraction + exact refine (csrc/knn_tc.cu); same indices as the fp32 kernel
-        ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=pc.device)
-        check(lib.psa_knn_graph_ws(b, n, c, k, _ptr(pc), _ptr(nn_idx), _ptr(ws), C.c_size_t(need), _stream()), "knn_graph")
-    else:
-        check(lib.psa_knn_graph(b, n, c, k, _ptr(pc), _ptr(nn_idx), _stream()), "knn_graph")
+    # tensor-core contraction + exact refine (csrc/knn_tc.cu) where it applies, the fp32 kernel otherwise: same indices
+    need = lib.psa_knn_graph_workspace_bytes(b, n, c, k)
+    ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=pc.device) if need else None
+    check(lib.psa_knn_graph_ws(b, n, c, k, _ptr(pc), _ptr(nn_idx), _ptr(ws), C.c_size_t(need), _stream()), "knn_graph")
     return nn_idx
 
 

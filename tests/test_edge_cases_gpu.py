@@ -69,6 +69,8 @@ def test_knn_graph_k_limits_and_errors():
         ops.knn_graph(x, 33)                      # a warp keeps at most 32 neighbours per row
     with pytest.raises(ValueError):
         ops.knn_graph(torch.rand((1, 10, 3), device="cuda"), 20)   # k > n: tf.nn.top_k rejects it too
+    with pytest.raises(ValueError):
+        ops.knn_graph(torch.rand((1, 0, 3), device="cuda"), 20)    # also for an empty cloud
 
 
 def test_shared_mlp_argument_errors():

@@ -207,7 +207,10 @@ def test_pointnet2_cls_ssg_matches_oracle(kind, mlp_mode):
                                                  # n % 4 != 0: the scalar cloud load (no 16-byte alignment per cloud); tail of a 16-point lane
                                                  ("ball", 301, 40, 0.3, 20, 0, 64, 3), ("shell", 1023, 100, 0.25, 32, 0, 64, 2),
                                                  # B = 32 clouds: nine CTAs per cloud, none crosses a cloud boundary
-                                                 ("ball", 2048, 512, 0.2, 32, 0, 64, 32)])
+                                                 ("ball", 2048, 512, 0.2, 32, 0, 64, 32),
+                                                 # beyond the streaming kernel's plan -> round-1 kernel: n > 4096 (scan mode), and
+                                                 # nsample 128 at n = 4096 (> 110 KB of shared memory; grid mode, 16 points per thread)
+                                                 ("ball", 8192, 256, 0.1, 32, 0, 64, 2), ("ball", 4096, 256, 0.2, 128, 0, 64, 2)])
 def test_sa_conv1_prebn_training_front(kind, n, m, r, k, c, c1, b):
     """variant F1: pre-BN conv1 output + BN batch statistics vs the fp64 restatement of
     query_ball_point -> group_point -> centre -> concat -> conv2d + bias_add (pointnet_util.py:44-50,117-123)."""

@@ -6,7 +6,7 @@ import pytest
 import torch
 
 from oracle import oracle as orc
-from scanobjectnn_b200 import ops
+from scanobjectnn_b200 import _lib, ops
 from scanobjectnn_b200.synthetic import make_clouds
 
 from . import gpu_util as G
@@ -331,13 +331,10 @@ def test_knn_graph_tensor_core_path_is_index_exact(kind, n, c, k):
         assert got[1].min() >= 0 and got[1].max() < n
         return
     assert np.array_equal(got, orc.dgcnn_knn(x, k))
-    ops._KNN_FP32_ONLY = True
-    try:
-        assert np.array_equal(got, G.npy(ops.knn_graph(xt, k)))
-    finally:
-        ops._KNN_FP32_ONLY = False
+    fp32 = torch.empty((2, n, k), dtype=torch.int32, device="cuda")     # the public fp32 entry point, called directly
+    assert _lib.load().psa_knn_graph(2, n, c, k, G._p(xt), G._p(fp32), None) == 0
+    assert np.array_equal(got, G.npy(fp32))
 
 
 def _lib_ws(b, n, c, k):
-    from scanobjectnn_b200 import _lib
     return _lib.load().psa_knn_graph_workspace_bytes(b, n, c, k)

@@ -1,6 +1,5 @@
-"""Tensor-core kNN graph (csrc/knn_tc.cu) at B=32, N=2048, k=20: time per phase (prep / main / exhaustive rows) with CUDA events
-between the launches (PSA_KNN_PHASES build not needed: the three kernels are separate launches), number of rows that went to the
-exhaustive kernel, fp32 kernel beside it."""
+"""Tensor-core kNN graph (psa_knn_graph_ws, csrc/knn_tc.cu) at B=32, N=2048, k=20 on four cloud types: time per call with CUDA
+events, number of rows that went to the exhaustive kernel, and the fp32 kernel (psa_knn_graph) beside it: time, index equality."""
 import ctypes as C
 import json
 import os
@@ -10,8 +9,20 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch
 
-from scanobjectnn_b200 import _lib, ops
+from scanobjectnn_b200 import _lib
 from scanobjectnn_b200.synthetic import make_clouds
+
+
+def median_us(run, warmup, reps):
+    for _ in range(warmup):
+        assert run() == 0
+    ts = []
+    for _ in range(reps):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(); run(); e1.record(); torch.cuda.synchronize()
+        ts.append(e0.elapsed_time(e1) * 1e3)
+    return sorted(ts)[reps // 2]
+
 
 lib = _lib.load()
 B, N, K = 32, 2048, 20
@@ -24,35 +35,14 @@ for name, x in (("c64_gauss", torch.randn((B, N, 64), device="cuda")), ("c3_ball
     need = lib.psa_knn_graph_workspace_bytes(B, N, c, K)
     ws = torch.zeros(need // 4 + 1, dtype=torch.float32, device="cuda")
     idx = torch.empty((B, N, K), dtype=torch.int32, device="cuda")
+    ref = torch.empty_like(idx)
     st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     vp = lambda t: C.c_void_p(t.data_ptr())
-    run = lambda: lib.psa_knn_graph_ws(B, N, c, K, vp(x), vp(idx), vp(ws), C.c_size_t(need), st)
-    for _ in range(3):
-        assert run() == 0
-    torch.cuda.synchronize()
+    tc_us = median_us(lambda: lib.psa_knn_graph_ws(B, N, c, K, vp(x), vp(idx), vp(ws), C.c_size_t(need), st), 3, 7)
     npad = (N + 127) // 128 * 128
     off = (B * (npad // 128) * 49152 + ((B * npad * 4 + 255) & ~255) + ((B * N * 4 + 255) & ~255)) // 4
     flagged = int(ws[off:off + 1].view(torch.int32).item())
-    # PSA_KNN_ERRSTAT build only (python tools/build_variant.py errstat -DPSA_KNN_ERRSTAT; PSA_LIB_PATH=...): the largest observed
-    # |fine - canonical| in units of the bound E2 and the number of canonically evaluated (ambiguous) entries; zeros otherwise
-    err_over_e2 = float(ws[off + 1:off + 2].view(torch.float32).item())
-    ambiguous = int(ws[off + 2:off + 3].view(torch.int32).item())
-    ts = []
-    for _ in range(7):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); run(); e1.record(); torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1) * 1e3)
-    ts.sort()
-    ops._KNN_FP32_ONLY = True
-    for _ in range(2):
-        ref = ops.knn_graph(x, K)
-    t2 = []
-    for _ in range(5):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(); ref = ops.knn_graph(x, K); e1.record(); torch.cuda.synchronize()
-        t2.append(e0.elapsed_time(e1) * 1e3)
-    t2.sort()
-    ops._KNN_FP32_ONLY = False
-    out[name] = {"max_err_over_E2": err_over_e2, "ambiguous_entries_per_row": ambiguous / (B * N), "tc_us": ts[len(ts) // 2], "fp32_us": t2[len(t2) // 2], "rows_to_exhaustive_kernel": flagged, "rows": B * N,
+    fp32_us = median_us(lambda: lib.psa_knn_graph(B, N, c, K, vp(x), vp(ref), st), 2, 5)
+    out[name] = {"tc_us": tc_us, "fp32_us": fp32_us, "rows_to_exhaustive_kernel": flagged, "rows": B * N,
                  "equal": bool(torch.equal(idx, ref))}
 print(json.dumps(out))
