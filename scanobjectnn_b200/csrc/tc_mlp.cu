@@ -2,7 +2,7 @@
 // (wgmma, A from registers, B from shared memory), hand-written PTX wrappers in tc_common.cuh.
 //
 // What the reference does (pointnet2/utils/pointnet_util.py:113-127): group_point -> (B,m,K,3+C) tensor -> three
-// cuDNN 1x1 convs over B*m*K rows -> reduce_max.  What the kernels here do per 128-row tile (128/K neighbourhoods):
+// cuDNN 1x1 convs over B*m*K rows -> reduce_max.  What the kernels here do per tile (64 or 128 rows):
 //
 //   layer 1   is never a GEMM over grouped rows.  (x_j - c) . Wx + f_j . Wf  =  U[j] + (x_j - c) . Wx   with
 //             U = points . W1[3:,:] computed ONCE per source point (K-fold fewer rows, a dense-layer launch); each
@@ -139,8 +139,10 @@ __global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float
 
 // ------------------------------------------------------------------------------------------------------------------
 // tc_sa_kernel -- one set-abstraction level (e.g. PointNet++ SA2: 131 -> 128 -> 128 -> 256 over 64-point neighbourhoods).
-//   CTA = 256 threads = two warpgroups = one 128-row tile (128 / K neighbourhoods) at a time, tiles claimed dynamically
-//   (persistent CTAs; a CTA that starts late or shares its SM with another stream simply takes fewer).
+//   CTA = 256 threads = two warpgroups, persistent (as many per SM as fit), tiles claimed dynamically (a CTA that starts late or
+//   shares its SM with another stream simply takes fewer).  K <= 64: each warpgroup works on its own 64-row tiles (64 / K
+//   neighbourhoods), out of step with the other, so one's gathers and FMA epilogues overlap the other's wgmma; K = 128 or a
+//   streamed last layer: the two work together on 128-row tiles.  NL = 2: layer 1's gathers are issued one tile ahead.
 //   * layer 1 on the FMA pipe: each thread evaluates U[j] + (x_j - c) . Wx (+ c . Wc), the folded affine and ReLU for the
 //     rows and channels of ITS A fragment and splits the result into NP pieces -- straight into registers;
 //   * inner tensor layers: wgmma with A from registers, B = weight image in shared memory; the D fragment goes through
@@ -209,10 +211,13 @@ __device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[
     for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
 }
 
+// named barrier `id` (1..15) over `count` threads: synchronises one unit of tc_sa_kernel without holding up the other
+__device__ __forceinline__ void unit_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
+
 // Specialised on the level shape: C1 = width of layer 1 (64 | 128), NL = tensor layers (1 | 2), N0 = width of the inner tensor
 // layer when NL = 2 (64 | 128).  The last layer's width is a runtime multiple of 64.
 template <int NP, int C1, int NL, int N0>
-__global__ void __launch_bounds__(kSaThreads, 1)
+__global__ void __launch_bounds__(kSaThreads, NP == 2 && C1 == 64 && N0 == 64 ? 2 : 1)     // 64-64-x levels: two CTAs per SM
 tc_sa_kernel(const __grid_constant__ TcArgs a) {
     static_assert((C1 == 64 || C1 == 128) && (NL == 1 || (NL == 2 && (N0 == 64 || N0 == 128))), "unsupported level shape");
     constexpr int last = NL - 1;
@@ -224,7 +229,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     __shared__ __align__(8) uint64_t s_rbar;                 // resident weights landed
     __shared__ __align__(8) uint64_t s_wbar[2];              // ring slot landed
     __shared__ float s_red[8][64];
-    __shared__ unsigned int s_tile;
+    __shared__ unsigned int s_tile[2][2];                    // [unit][slot]: claimed tiles
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
@@ -279,36 +284,83 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     uint32_t q_used = 0;                                      // ring uses consumed (fills issued: q_used + 2)
     if (resident) mbar_wait(&s_rbar, 0);
 
-    const int K = a.K, G = 128 / K;
+    // A tile is worked on by one unit of threads.  K <= 64: each warpgroup is a unit of its own with a 64-row tile, so the two
+    // run out of step -- one's gathers, FMA layer and epilogue overlap the other's wgmma.  K = 128 (a neighbourhood spans 128
+    // rows) and a streamed last layer (its ring is consumed by the whole CTA in step): both warpgroups form one unit, 128 rows.
+    // Units synchronise on their own named barrier; no CTA-wide barrier is left in the tile loop.
+    const int K = a.K;
+    const bool joint = K == 128 || a.stream_last;
+    const int G = (joint ? 128 : 64) / K;                     // neighbourhoods per tile
+    const int unit = joint ? 0 : warp >> 2;
+    const int ubar = 1 + unit, uthreads = joint ? 256 : 128;  // the unit's named barrier
+    const int ut = joint ? tid : tid & 127, uw0 = joint ? 0 : 4 * unit;   // thread index in the unit, first warp of the unit
     const long long ntiles = (a.groups + G - 1) / G;
-    const int rl[2] = {warp * 16 + g, warp * 16 + g + 8};     // this thread's two tile rows
-    for (;;) {
-        if (tid == 0) s_tile = atomicAdd(a.tile_counter, 1u);
-        __syncthreads();
-        const long long tile = (long long)s_tile;
-        if (tile >= ntiles) break;
+    const int rl[2] = {(warp - uw0) * 16 + g, (warp - uw0) * 16 + g + 8};   // this thread's two tile rows
+
+    // Layer 1's inputs for this thread's two rows are gathered one tile ahead (NL = 2), during the previous tile's last layer:
+    // stage A (neighbour index, centre) after the first chunk's pooling barrier, stage B (neighbour coordinates, U row) after
+    // its second one.  The 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per
+    // SM, so registers are plentiful); other levels load them in layer 1.
+    constexpr bool kHoldU = NP == 2 && C1 == 128;
+    constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the tile:
+                                                              // measured faster there, the tile is too short to hide the loads
+    constexpr int kUH = kHoldU ? C1 / 8 : 1;                  // float2 per row held
+    int jn[2];
+    long long gidn[2];
+    float cx[2], cy[2], cz[2], px[2], py[2], pz[2];
+    const float* urow[2];
+    float2 uh[2][kUH];
+    auto gather_a = [&](long long tl) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            gidn[i] = tl * G + rl[i] / K;
+            cx[i] = cy[i] = cz[i] = 0.f;
+            jn[i] = 0;
+            if (gidn[i] < a.groups) {
+                jn[i] = __ldg(a.idx + gidn[i] * K + (rl[i] % K));
+                const float* c = a.new_xyz + (size_t)gidn[i] * 3;
+                cx[i] = __ldg(c); cy[i] = __ldg(c + 1); cz[i] = __ldg(c + 2);
+            }
+        }
+    };
+    auto gather_b = [&]() {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            px[i] = py[i] = pz[i] = 0.f;
+            urow[i] = nullptr;
+            if (gidn[i] < a.groups) {
+                const long long bi = gidn[i] / a.m;
+                const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
+                px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
+                if (a.uf) urow[i] = a.uf + ((size_t)bi * a.n + jn[i]) * C1;
+            }
+            if constexpr (kHoldU) {
+                if (urow[i] != nullptr) {
+#pragma unroll
+                    for (int q = 0; q < kUH; ++q) uh[i][q] = __ldg(reinterpret_cast<const float2*>(urow[i] + 8 * q + 2 * t));
+                }
+            }
+        }
+    };
+
+    // the next tile is claimed while this one is computed: slot it & 1 of s_tile is written at the top of iteration it - 1 and
+    // read after that iteration's first pooling barrier; the barrier after it orders the read before the next write of the slot
+    if (ut == 0) s_tile[unit][0] = atomicAdd(a.tile_counter, 1u);
+    unit_bar_sync(ubar, uthreads);
+    long long tile = (long long)s_tile[unit][0];
+    if (kAhead) { gather_a(tile); gather_b(); }
+    for (uint32_t it = 0; tile < ntiles; ++it) {
+        if (ut == 0) s_tile[unit][(it + 1) & 1] = atomicAdd(a.tile_counter, 1u);
+        if (!kAhead) { gather_a(tile); gather_b(); }
         const long long g0 = tile * G;
+        long long next = ntiles;                              // read after the first pooling barrier
 
         // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
         uint32_t A[NP][8][4];
         {
-            float dx[2], dy[2], dz[2], cx[2], cy[2], cz[2];
-            const float* urow[2];
+            float dx[2], dy[2], dz[2];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const long long gid = g0 + rl[i] / K;
-                dx[i] = dy[i] = dz[i] = cx[i] = cy[i] = cz[i] = 0.f;
-                urow[i] = nullptr;
-                if (gid < a.groups) {
-                    const long long bi = gid / a.m;
-                    const int j = __ldg(a.idx + gid * K + (rl[i] % K));
-                    const float* p = a.xyz + ((size_t)bi * a.n + j) * 3;
-                    const float* c = a.new_xyz + (size_t)gid * 3;
-                    cx[i] = __ldg(c); cy[i] = __ldg(c + 1); cz[i] = __ldg(c + 2);
-                    dx[i] = __ldg(p) - cx[i]; dy[i] = __ldg(p + 1) - cy[i]; dz[i] = __ldg(p + 2) - cz[i];
-                    if (a.uf) urow[i] = a.uf + ((size_t)bi * a.n + j) * C1;
-                }
-            }
+            for (int i = 0; i < 2; ++i) { dx[i] = px[i] - cx[i]; dy[i] = py[i] - cy[i]; dz[i] = pz[i] - cz[i]; }
 #pragma unroll
             for (int s = 0; s < C1 / 16; ++s) {
                 {
@@ -320,7 +372,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                                      wz = *reinterpret_cast<const float2*>(w1x + 2 * C1 + k);
 #pragma unroll
                         for (int i = 0; i < 2; ++i) {
-                            float2 v = urow[i] ? ffma2_rn(__ldg(reinterpret_cast<const float2*>(urow[i] + k)), sc, sh) : sh;
+                            float2 uv;
+                            if constexpr (kHoldU) uv = uh[i][2 * s + h];
+                            else uv = urow[i] ? __ldg(reinterpret_cast<const float2*>(urow[i] + k)) : sh;
+                            float2 v = urow[i] ? ffma2_rn(uv, sc, sh) : sh;
                             if (a.w1c != nullptr) {        // EdgeConv: the part of the first layer that acts on the centre x_i
                                 const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
                                              cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
@@ -383,21 +438,24 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                         if (g == 0) s_red[warp][8 * j + 2 * t + e] = m;
                     }
                 }
-                __syncthreads();                                  // every warp's maxima are in s_red; ring slot consumed
+                unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in s_red; ring slot consumed
+                if (nc == 0) { next = (long long)s_tile[unit][(it + 1) & 1]; if (kAhead) gather_a(next); }
                 if (a.stream_last) {
                     if (tid == 0) sa_fill_ring(q_used + 2, a.image[last], NCL, L, base, s_wbar);
                     ++q_used;
                 }
-                if (tid < G * 64) {
-                    const int grp = tid >> 6, cl = tid & 63, wpg = K / 16;
-                    float mx = s_red[grp * wpg][cl];
-                    for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[grp * wpg + w][cl]);
+                if (ut < G * 64) {
+                    const int grp = ut >> 6, cl = ut & 63, wpg = K / 16;
+                    float mx = s_red[uw0 + grp * wpg][cl];
+                    for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[uw0 + grp * wpg + w][cl]);
                     const long long og = g0 + grp;
                     if (og < a.groups) a.out[(size_t)og * N + nc * 64 + cl] = mx;
                 }
-                __syncthreads();                                  // s_red is reused by the next chunk
+                unit_bar_sync(ubar, uthreads);                    // s_red is reused by the next chunk
+                if (kAhead && nc == 0) gather_b();
             }
         }
+        tile = next;
     }
     if constexpr (NP == 2) {
         if (f16x2_overflowed(ovf)) atomicOr(a.ovf, 1u);
@@ -789,23 +847,31 @@ size_t tc_sa_workspace_bytes(const TcArgs& a, int b, int n, int c) {
 static int tc_sa_image_nt() { return kSaNt | image_flag(g_tc_np); }
 
 template <int NP, int C1, int NL, int N0>
-static int launch_tc_sa_shape(const TcArgs& a, int ctas, size_t smem, cudaStream_t st) {
+static int launch_tc_sa_shape(const TcArgs& a, long long ctas_needed, size_t smem, cudaStream_t st) {
     PSA_CUDA(cudaFuncSetAttribute(tc_sa_kernel<NP, C1, NL, N0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // persistent CTAs: as many as are resident at once (two per SM for the smaller levels), never more than there is work for
+    int dev = 0, sms = 0, per_sm = 0;
+    PSA_CUDA(cudaGetDevice(&dev));
+    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PSA_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_sa_kernel<NP, C1, NL, N0>, kSaThreads, smem));
+    const long long resident = (long long)sms * (per_sm > 0 ? per_sm : 1);
+    const int ctas = (int)(ctas_needed < 1 ? 1 : ctas_needed < resident ? ctas_needed : resident);
     tc_sa_kernel<NP, C1, NL, N0><<<ctas, kSaThreads, smem, st>>>(a);
     return check_launch("tc_sa_kernel");
 }
 
 template <int NP>
 static int launch_tc_sa_np(TcArgs& a, cudaStream_t st) {
-    const int G = 128 / a.K;
+    // tiles of one unit (see tc_sa_kernel): 64 rows per warpgroup, or 128 rows per CTA when K = 128 or the last layer streams
+    const bool joint = a.K == 128 || a.stream_last;
+    const int G = (joint ? 128 : 64) / a.K;
     const long long ntiles = (a.groups + G - 1) / G;
+    const long long ctas_needed = joint ? ntiles : (ntiles + 1) / 2;     // two units per CTA
     const size_t smem = (size_t)tc_sa_layout(a).total + 1024;
-    int ctas = (int)(ntiles < kNumSMs ? ntiles : kNumSMs);
-    if (ctas < 1) ctas = 1;
     // shapes accepted by tc_sa_eligible: C1 in {64, 128}, one or two tensor layers, an inner layer 64 or 128 wide
-    if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas, smem, st);
-    if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas, smem, st);
-    return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 128, 2, 64>(a, ctas, smem, st) : launch_tc_sa_shape<NP, 128, 2, 128>(a, ctas, smem, st);
+    if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas_needed, smem, st);
+    if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas_needed, smem, st);
+    return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 128, 2, 64>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 128, 2, 128>(a, ctas_needed, smem, st);
 }
 
 // One set-abstraction level on the SA kernel (`a` = eligibility result for the current split): weight images, the U GEMM
