@@ -76,6 +76,7 @@ struct TcArgs {
     int relu[kMaxTcLayers];
     int Kd[kMaxTcLayers], Ntot[kMaxTcLayers];
     int stream_last;       // 1: the last layer's weights do not fit next to the others -> one 64-channel chunk at a time
+    int joint;             // tc_sa_kernel: both warpgroups on one 128-row pass, every row computed (set by the launcher)
     unsigned int* tile_counter;   // zeroed before the launch: tiles are handed out dynamically (CTAs that start late or
                                   // share their SM with another stream's kernels simply take fewer)
     int np;                       // operand pieces: 2 (fp16x2) or 3 (bf16x3)
@@ -139,10 +140,12 @@ __global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float
 
 // ------------------------------------------------------------------------------------------------------------------
 // tc_sa_kernel -- one set-abstraction level (e.g. PointNet++ SA2: 131 -> 128 -> 128 -> 256 over 64-point neighbourhoods).
-//   CTA = 256 threads = two warpgroups, persistent (as many per SM as fit), tiles claimed dynamically (a CTA that starts late or
-//   shares its SM with another stream simply takes fewer).  K <= 64: each warpgroup works on its own 64-row tiles (64 / K
-//   neighbourhoods), out of step with the other, so one's gathers and FMA epilogues overlap the other's wgmma; K = 128 or a
-//   streamed last layer: the two work together on 128-row tiles.  NL = 2: layer 1's gathers are issued one tile ahead.
+//   CTA = 256 threads = two warpgroups, persistent (as many per SM as fit), chunks of neighbourhoods claimed dynamically (a CTA
+//   that starts late or shares its SM with another stream simply takes fewer).  K <= 64: each warpgroup works on its own
+//   64-row passes, out of step with the other, so one's gathers and FMA epilogues overlap the other's wgmma, and computes only
+//   the rows of each neighbourhood before its ball-query padding (16-row slots packed back to back); K = 128 or a streamed
+//   last layer: the two work together on 128-row passes of whole neighbourhoods.  NL = 2: layer 1's gathers are issued one
+//   pass ahead.
 //   * layer 1 on the FMA pipe: each thread evaluates U[j] + (x_j - c) . Wx (+ c . Wc), the folded affine and ReLU for the
 //     rows and channels of ITS A fragment and splits the result into NP pieces -- straight into registers;
 //   * inner tensor layers: wgmma with A from registers, B = weight image in shared memory; the D fragment goes through
@@ -181,6 +184,14 @@ __host__ __device__ inline TcSaLayout tc_sa_layout(const TcArgs& a) {
     L.total = off;
     return L;
 }
+
+// neighbourhoods per chunk, the work a unit of tc_sa_kernel claims at a time: one 128-row pass for a joint unit (K = 128 or a
+// streamed last layer), 512 rows before padding is skipped for a warpgroup unit -- few enough chunks per unit stay that the
+// end of the grid is balanced (PointNet++ SA2: 512 chunks for 264 units), enough neighbourhoods per chunk that its last pass
+// is mostly full
+__host__ __device__ inline int sa_chunk(int K, bool joint) { return (joint ? 128 : 512) / K; }
+// shared memory of the pooling carry (a warpgroup unit's running max of a neighbourhood that spans two passes), after the layout
+__host__ __device__ inline uint32_t sa_carry_bytes(const TcArgs& a) { return a.joint ? 0u : 2u * a.Ntot[a.nl - 1] * 4u; }
 
 // thread 0: use q of the streamed last layer's ring = 64-channel chunk q % ncl into slot q & 1
 __device__ __forceinline__ void sa_fill_ring(uint32_t q, const uint8_t* image, int ncl, const TcSaLayout& L, uint8_t* base, uint64_t* bars) {
@@ -228,8 +239,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_rbar;                 // resident weights landed
     __shared__ __align__(8) uint64_t s_wbar[2];              // ring slot landed
-    __shared__ float s_red[8][64];
-    __shared__ unsigned int s_tile[2][2];                    // [unit][slot]: claimed tiles
+    __shared__ __align__(16) float s_red[8][64];
+    __shared__ unsigned int s_claim[2];                      // [unit]: the chunk claimed after the current one
+    __shared__ int s_slots[2][2][16];                        // [unit][table]: 16-row slots of each neighbourhood of a chunk
+    __shared__ long long s_desc[2][2][8];                    // [unit][pass parity][warp]: pooling run that starts at the warp
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
@@ -284,56 +297,111 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     uint32_t q_used = 0;                                      // ring uses consumed (fills issued: q_used + 2)
     if (resident) mbar_wait(&s_rbar, 0);
 
-    // A tile is worked on by one unit of threads.  K <= 64: each warpgroup is a unit of its own with a 64-row tile, so the two
-    // run out of step -- one's gathers, FMA layer and epilogue overlap the other's wgmma.  K = 128 (a neighbourhood spans 128
-    // rows) and a streamed last layer (its ring is consumed by the whole CTA in step): both warpgroups form one unit, 128 rows.
-    // Units synchronise on their own named barrier; no CTA-wide barrier is left in the tile loop.
+    // Work is done by units of threads.  K <= 64: each warpgroup is a unit of its own, so the two run out of step -- one's
+    // gathers, FMA layer and epilogue overlap the other's wgmma.  K = 128 (a neighbourhood spans 128 rows) and a streamed last
+    // layer (its ring is consumed by the whole CTA in step): both warpgroups form one unit.  Units synchronise on their own
+    // named barrier; no CTA-wide barrier is left in the loop.
+    //   A unit claims a chunk of C consecutive neighbourhoods at a time and computes it in passes of one 16-row slot per warp.
+    // The ball query pads a neighbourhood by repeating its first index, and a max does not change when a row is repeated: a
+    // neighbourhood whose entries from L on all equal idx[0] only needs its first L rows, ceil(L / 16) slots.  The slots of a
+    // chunk are packed back to back, so a neighbourhood may start in one pass and end in the next; its running max is carried
+    // in the unit's shared memory.  Warps past the chunk's last slot recompute that slot and store nothing.  Joint units keep
+    // every row: a chunk is then one 128-row pass, as before.
     const int K = a.K;
-    const bool joint = K == 128 || a.stream_last;
-    const int G = (joint ? 128 : 64) / K;                     // neighbourhoods per tile
+    const bool joint = a.joint;
+    const int W = joint ? 8 : 4;                             // warps of the unit = slots per pass
+    const int C = sa_chunk(K, joint);                         // neighbourhoods per chunk (<= 16)
     const int unit = joint ? 0 : warp >> 2;
-    const int ubar = 1 + unit, uthreads = joint ? 256 : 128;  // the unit's named barrier
+    const int ubar = 1 + unit, uthreads = 32 * W;             // the unit's named barrier
     const int ut = joint ? tid : tid & 127, uw0 = joint ? 0 : 4 * unit;   // thread index in the unit, first warp of the unit
-    const long long ntiles = (a.groups + G - 1) / G;
-    const int rl[2] = {(warp - uw0) * 16 + g, (warp - uw0) * 16 + g + 8};   // this thread's two tile rows
+    const int wl = warp - uw0;                                // warp index in the unit
+    const unsigned nchunks = (unsigned)((a.groups + C - 1) / C);
+    float* carry = reinterpret_cast<float*>(base + L.total) + (size_t)unit * a.Ntot[last];   // warpgroup units: Ntot[last] floats
 
-    // Layer 1's inputs for this thread's two rows are gathered one tile ahead (NL = 2), during the previous tile's last layer:
-    // stage A (neighbour index, centre) after the first chunk's pooling barrier, stage B (neighbour coordinates, U row) after
-    // its second one.  The 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per
-    // SM, so registers are plentiful); other levels load them in layer 1.
-    constexpr bool kHoldU = NP == 2 && C1 == 128;
-    constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the tile:
-                                                              // measured faster there, the tile is too short to hide the loads
-    constexpr int kUH = kHoldU ? C1 / 8 : 1;                  // float2 per row held
-    int jn[2];
-    long long gidn[2];
-    float cx[2], cy[2], cz[2], px[2], py[2], pz[2];
-    const float* urow[2];
-    float2 uh[2][kUH];
-    auto gather_a = [&](long long tl) {
+    // slot counts of chunk ch into table b, by the whole unit (read after a unit barrier).  L = 1 + the last j with
+    // idx[j] != idx[0] (1 when all are equal), from a ballot per 32 entries; a warp covers 128 entries = 4 neighbourhoods of 32
+    // or 2 of 64.  Neighbourhoods past the end take no slot.
+    auto fill_table = [&](unsigned ch, int b) {
+        const long long g0 = (long long)ch * C;
+        if (joint) {
+            if (ut < C) s_slots[unit][b][ut] = g0 + ut < a.groups ? K / 16 : 0;
+            return;
+        }
+        const long long r0 = g0 * K + wl * 128, rows = a.groups * K;
+        int v[4];
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-            gidn[i] = tl * G + rl[i] / K;
-            cx[i] = cy[i] = cz[i] = 0.f;
-            jn[i] = 0;
-            if (gidn[i] < a.groups) {
-                jn[i] = __ldg(a.idx + gidn[i] * K + (rl[i] % K));
-                const float* c = a.new_xyz + (size_t)gidn[i] * 3;
-                cx[i] = __ldg(c); cy[i] = __ldg(c + 1); cz[i] = __ldg(c + 2);
+        for (int q = 0; q < 4; ++q) v[q] = r0 + 32 * q + lane < rows ? __ldg(a.idx + r0 + 32 * q + lane) : 0;
+        if (K == 32) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const unsigned d = __ballot_sync(0xffffffffu, v[q] != __shfl_sync(0xffffffffu, v[q], 0));
+                const int nb = 4 * wl + q, Ln = d ? 32 - __clz(d) : 1;
+                if (lane == 0) s_slots[unit][b][nb] = g0 + nb < a.groups ? (Ln + 15) >> 4 : 0;
+            }
+        } else {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int f = __shfl_sync(0xffffffffu, v[2 * h], 0);
+                const unsigned lo = __ballot_sync(0xffffffffu, v[2 * h] != f), hi = __ballot_sync(0xffffffffu, v[2 * h + 1] != f);
+                const int nb = 2 * wl + h, Ln = hi ? 64 - __clz(hi) : lo ? 32 - __clz(lo) : 1;
+                if (lane == 0) s_slots[unit][b][nb] = g0 + nb < a.groups ? (Ln + 15) >> 4 : 0;
             }
         }
     };
+
+    // Layer 1's inputs for this thread's two rows are gathered one pass ahead (NL = 2), during the previous pass's last layer:
+    // stage A (neighbour index, centre) after the first chunk's pooling barrier -- after the second one when the pass opens a
+    // chunk, whose slot table is filled in between -- and stage B (neighbour coordinates, U row) after the second one.  The
+    // 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM, so registers are
+    // plentiful); other levels load them in layer 1.
+    constexpr bool kHoldU = NP == 2 && C1 == 128;
+    constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the pass:
+                                                              // measured faster there, the pass is too short to hide the loads
+    constexpr int kUH = kHoldU ? C1 / 8 : 1;                  // float2 per row held
+    int incl = 0, T = 0;                                      // slots of the chunk gather_a last read: prefix (lane i: neighbourhoods
+                                                              // 0..i), total
+    int jn[2];
+    long long gn = 0;                                         // the neighbourhood of this warp's slot
+    float cx = 0.f, cy = 0.f, cz = 0.f, px[2], py[2], pz[2];
+    const float* urow[2];
+    float2 uh[2][kUH];
+    // stage A of pass p of chunk ch (slot table b); lane 0 records the warp's pooling run in s_desc[unit][d]
+    auto gather_a = [&](unsigned ch, int b, int p, int d) {
+        if (p == 0) {                                         // a new chunk: prefix of its slot table
+            incl = lane < C ? s_slots[unit][b][lane] : 0;
+#pragma unroll
+            for (int o = 1; o < 16; o <<= 1) {
+                const int y = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += y;
+            }
+            T = __shfl_sync(0xffffffffu, incl, C - 1);
+        }
+        const int s = p * W + wl, ss = min(s, T - 1);
+        const int nb = __popc(__ballot_sync(0xffffffffu, incl <= ss) & ((1u << C) - 1u));
+        const int end = __shfl_sync(0xffffffffu, incl, nb), start = nb ? __shfl_sync(0xffffffffu, incl, nb - 1) : 0;
+        gn = (long long)ch * C + nb;
+        const int row = 16 * (ss - start) + g;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) jn[i] = __ldg(a.idx + gn * K + row + 8 * i);
+        const float* c = a.new_xyz + (size_t)gn * 3;
+        cx = __ldg(c); cy = __ldg(c + 1); cz = __ldg(c + 2);
+        if (lane == 0) {
+            // a run = the warps of one neighbourhood in this pass: [len, carried in from the last pass, carried out to the next]
+            long long run = 0;
+            if (s < T && (wl == 0 || s == start)) {
+                const int pe = (p + 1) * W;
+                run = gn << 8 | (long long)(min(end, pe) - s) | (s > start ? 16 : 0) | (end > pe ? 32 : 0);
+            }
+            s_desc[unit][d][wl] = run;
+        }
+    };
     auto gather_b = [&]() {
+        const long long bi = gn / a.m;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            px[i] = py[i] = pz[i] = 0.f;
-            urow[i] = nullptr;
-            if (gidn[i] < a.groups) {
-                const long long bi = gidn[i] / a.m;
-                const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
-                px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
-                if (a.uf) urow[i] = a.uf + ((size_t)bi * a.n + jn[i]) * C1;
-            }
+            const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
+            px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
+            urow[i] = a.uf ? a.uf + ((size_t)bi * a.n + jn[i]) * C1 : nullptr;
             if constexpr (kHoldU) {
                 if (urow[i] != nullptr) {
 #pragma unroll
@@ -343,24 +411,27 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         }
     };
 
-    // the next tile is claimed while this one is computed: slot it & 1 of s_tile is written at the top of iteration it - 1 and
-    // read after that iteration's first pooling barrier; the barrier after it orders the read before the next write of the slot
-    if (ut == 0) s_tile[unit][0] = atomicAdd(a.tile_counter, 1u);
+    // The chunk after the current one is claimed at the top of the current one's first pass and read after the first pooling
+    // barrier of its last pass; the barrier after that orders the read before the next claim.
+    if (ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
     unit_bar_sync(ubar, uthreads);
-    long long tile = (long long)s_tile[unit][0];
-    if (kAhead) { gather_a(tile); gather_b(); }
-    for (uint32_t it = 0; tile < ntiles; ++it) {
-        if (ut == 0) s_tile[unit][(it + 1) & 1] = atomicAdd(a.tile_counter, 1u);
-        if (!kAhead) { gather_a(tile); gather_b(); }
-        const long long g0 = tile * G;
-        long long next = ntiles;                              // read after the first pooling barrier
+    unsigned ch = s_claim[unit];
+    if (ch < nchunks) fill_table(ch, 0);
+    unit_bar_sync(ubar, uthreads);
+    int buf = 0, p = 0;                                       // slot table and pass index of the current chunk
+    if (kAhead && ch < nchunks) { gather_a(ch, 0, 0, 0); gather_b(); }
+    for (uint32_t it = 0; ch < nchunks; ++it) {
+        if (p == 0 && ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
+        if (!kAhead) { gather_a(ch, buf, p, it & 1); gather_b(); }
+        unsigned nch = ch;                                    // the next pass: chunk, slot table, pass index
+        int nbuf = buf, np = p + 1;
 
         // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
         uint32_t A[NP][8][4];
         {
             float dx[2], dy[2], dz[2];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) { dx[i] = px[i] - cx[i]; dy[i] = py[i] - cy[i]; dz[i] = pz[i] - cz[i]; }
+            for (int i = 0; i < 2; ++i) { dx[i] = px[i] - cx; dy[i] = py[i] - cy; dz[i] = pz[i] - cz; }
 #pragma unroll
             for (int s = 0; s < C1 / 16; ++s) {
                 {
@@ -379,11 +450,11 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                             if (a.w1c != nullptr) {        // EdgeConv: the part of the first layer that acts on the centre x_i
                                 const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
                                              cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
-                                v = ffma2_rn(make_float2(cz[i], cz[i]), cwz, ffma2_rn(make_float2(cy[i], cy[i]), cwy, ffma2_rn(make_float2(cx[i], cx[i]), cwx, v)));
+                                v = ffma2_rn(make_float2(cz, cz), cwz, ffma2_rn(make_float2(cy, cy), cwy, ffma2_rn(make_float2(cx, cx), cwx, v)));
                             }
                             v = ffma2_rn(make_float2(dz[i], dz[i]), wz, ffma2_rn(make_float2(dy[i], dy[i]), wy, ffma2_rn(make_float2(dx[i], dx[i]), wx, v)));
                             if (a.relu1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
-                            put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);     // rows past the end carry finite values, never stored
+                            put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);
                         }
                     }
                 }
@@ -438,24 +509,44 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                         if (g == 0) s_red[warp][8 * j + 2 * t + e] = m;
                     }
                 }
+                // a run carried in from the last pass only starts at warp 0; its partial max is read before the barrier, since
+                // a run of this pass may carry its own out through the same words after it
+                const float2 cin = !joint && wl == 0 ? reinterpret_cast<const float2*>(carry)[nc * 32 + lane] : make_float2(0.f, 0.f);
                 unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in s_red; ring slot consumed
-                if (nc == 0) { next = (long long)s_tile[unit][(it + 1) & 1]; if (kAhead) gather_a(next); }
+                if (nc == 0) {
+                    if (np * W < T) {
+                        if (kAhead) gather_a(ch, buf, np, (it + 1) & 1);
+                    } else {                                      // the next pass opens the claimed chunk
+                        nch = s_claim[unit]; nbuf = buf ^ 1; np = 0;
+                        if (nch < nchunks) fill_table(nch, nbuf);
+                    }
+                }
                 if (a.stream_last) {
                     if (tid == 0) sa_fill_ring(q_used + 2, a.image[last], NCL, L, base, s_wbar);
                     ++q_used;
                 }
-                if (ut < G * 64) {
-                    const int grp = ut >> 6, cl = ut & 63, wpg = K / 16;
-                    float mx = s_red[uw0 + grp * wpg][cl];
-                    for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[uw0 + grp * wpg + w][cl]);
-                    const long long og = g0 + grp;
-                    if (og < a.groups) a.out[(size_t)og * N + nc * 64 + cl] = mx;
+                {                                                 // the run starting at this warp's slot, two columns per lane
+                    const long long run = s_desc[unit][it & 1][wl];
+                    const int len = (int)(run & 15);
+                    if (len != 0) {
+                        const float2* red = reinterpret_cast<const float2*>(&s_red[warp][0]) + lane;
+                        float2 mx = red[0];
+#pragma unroll
+                        for (int w = 1; w < 8; ++w)
+                            if (w < len) { const float2 v = red[32 * w]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); }
+                        if (run & 16) { mx.x = fmaxf(mx.x, cin.x); mx.y = fmaxf(mx.y, cin.y); }
+                        if (run & 32) reinterpret_cast<float2*>(carry)[nc * 32 + lane] = mx;
+                        else *reinterpret_cast<float2*>(a.out + (size_t)(run >> 8) * N + nc * 64 + 2 * lane) = mx;
+                    }
                 }
-                unit_bar_sync(ubar, uthreads);                    // s_red is reused by the next chunk
-                if (kAhead && nc == 0) gather_b();
+                unit_bar_sync(ubar, uthreads);                    // s_red is reused by the next chunk; the slot table is filled
+                if (kAhead && nc == 0 && nch < nchunks) {
+                    if (np == 0) gather_a(nch, nbuf, 0, (it + 1) & 1);
+                    gather_b();
+                }
             }
         }
-        tile = next;
+        ch = nch; buf = nbuf; p = np;
     }
     if constexpr (NP == 2) {
         if (f16x2_overflowed(ovf)) atomicOr(a.ovf, 1u);
@@ -862,12 +953,15 @@ static int launch_tc_sa_shape(const TcArgs& a, long long ctas_needed, size_t sme
 
 template <int NP>
 static int launch_tc_sa_np(TcArgs& a, cudaStream_t st) {
-    // tiles of one unit (see tc_sa_kernel): 64 rows per warpgroup, or 128 rows per CTA when K = 128 or the last layer streams
-    const bool joint = a.K == 128 || a.stream_last;
-    const int G = (joint ? 128 : 64) / a.K;
-    const long long ntiles = (a.groups + G - 1) / G;
-    const long long ctas_needed = joint ? ntiles : (ntiles + 1) / 2;     // two units per CTA
-    const size_t smem = (size_t)tc_sa_layout(a).total + 1024;
+    // chunks of one unit (see tc_sa_kernel): a unit is a warpgroup, or the whole CTA when K = 128 or the last layer streams.
+    // The pooling carry of warpgroup units sits after the layout, in the shared memory the SM has above the budget
+    // tc_sa_eligible checks; a level whose carry does not fit there keeps joint units (4 KB are left for the static arrays).
+    a.joint = a.K == 128 || a.stream_last;
+    if (!a.joint && tc_sa_layout(a).total + 1024 + sa_carry_bytes(a) > 223u * 1024u) a.joint = 1;
+    const int C = sa_chunk(a.K, a.joint);
+    const long long nchunks = (a.groups + C - 1) / C;
+    const long long ctas_needed = a.joint ? nchunks : (nchunks + 1) / 2;   // two units per CTA
+    const size_t smem = (size_t)tc_sa_layout(a).total + 1024 + sa_carry_bytes(a);
     // shapes accepted by tc_sa_eligible: C1 in {64, 128}, one or two tensor layers, an inner layer 64 or 128 wide
     if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas_needed, smem, st);
     if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas_needed, smem, st);
