@@ -70,6 +70,9 @@ constexpr uint32_t kFmtF16 = 0, kFmtBF16 = 1;
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 __device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;\n" ::: "memory"); }
+// wait until at most N committed groups are pending (N = 1: the group committed last may still run)
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
 // accumulators are written asynchronously: after wg_wait_all, pin every read of them behind the wait
 __device__ __forceinline__ void wg_fence_acc(float (&d)[32]) {
 #pragma unroll

@@ -77,6 +77,7 @@ struct TcArgs {
     int Kd[kMaxTcLayers], Ntot[kMaxTcLayers];
     int stream_last;       // 1: the last layer's weights do not fit next to the others -> one 64-channel chunk at a time
     int joint;             // tc_sa_kernel: both warpgroups on one 128-row pass, every row computed (set by the launcher)
+    int pool_chunks;       // tc_sa_kernel: 64-channel chunks of the last layer pooled together (set by the launcher)
     unsigned int* tile_counter;   // zeroed before the launch: tiles are handed out dynamically (CTAs that start late or
                                   // share their SM with another stream's kernels simply take fewer)
     int np;                       // operand pieces: 2 (fp16x2) or 3 (bf16x3)
@@ -105,6 +106,19 @@ __device__ __forceinline__ float warp_rowmax16(float lo, float hi) {
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 8));
     m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 16));
     return m;
+}
+// the same max, reduce-scattered over a whole 64-column chunk: with v[2j + e] = this thread's max over rows g, g + 8 of column
+// 8j + 2t + e, each step across lane bit 4, 3, 2 (= bit 2, 1, 0 of g) keeps the half of the columns whose j has that bit of g,
+// 8 + 4 + 2 shuffles, and lane (g, t) ends with the 16-row max of columns 8g + 2t, 8g + 2t + 1.  One step: keep v[0..H) or
+// v[H..2H) by `up`, the partner across lane bit 2H keeps the other half (the caller does the first step as it forms v, so
+// that only half of the 16 values are live at once).
+template <int H, int S>
+__device__ __forceinline__ void colmax_halve(float (&v)[S], bool up) {
+#pragma unroll
+    for (int i = 0; i < H; ++i) {
+        const float lo = v[i], hi = v[H + i];
+        v[i] = fmaxf(up ? hi : lo, __shfl_xor_sync(0xffffffffu, up ? lo : hi, 2 * H));
+    }
 }
 __device__ __forceinline__ float warp_rowsum16(float v) {
     v += __shfl_xor_sync(0xffffffffu, v, 4);
@@ -192,6 +206,8 @@ __host__ __device__ inline TcSaLayout tc_sa_layout(const TcArgs& a) {
 __host__ __device__ inline int sa_chunk(int K, bool joint) { return (joint ? 128 : 512) / K; }
 // shared memory of the pooling carry (a warpgroup unit's running max of a neighbourhood that spans two passes), after the layout
 __host__ __device__ inline uint32_t sa_carry_bytes(const TcArgs& a) { return a.joint ? 0u : 2u * a.Ntot[a.nl - 1] * 4u; }
+// shared memory of the pooling buffer, after the carry: each warp's column maxima of `chunks` 64-channel chunks
+__host__ __device__ inline uint32_t sa_red_bytes(int chunks) { return 8u * 64u * 4u * (uint32_t)chunks; }
 
 // thread 0: use q of the streamed last layer's ring = 64-channel chunk q % ncl into slot q & 1
 __device__ __forceinline__ void sa_fill_ring(uint32_t q, const uint8_t* image, int ncl, const TcSaLayout& L, uint8_t* base, uint64_t* bars) {
@@ -203,8 +219,9 @@ __device__ __forceinline__ void sa_fill_ring(uint32_t q, const uint8_t* image, i
 
 // D[64 x 64 NCH] (+)= A . W over KS steps of 16 input channels, all piece pairs of Split<NP>: straight-line wgmma (no predicated
 // issue, so ptxas keeps the whole sequence asynchronous).  Output chunk c reads the weight blocks at wb + c * cstride.
+// sa_mma_issue commits the group and returns with it in flight; sa_mma waits for it.
 template <int NP, int KS, int NCH>
-__device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[NP][8][4], uint32_t wb, uint32_t cstride) {
+__device__ __forceinline__ void sa_mma_issue(float (&d)[NCH][32], const uint32_t (&A)[NP][8][4], uint32_t wb, uint32_t cstride) {
     constexpr uint32_t bb = tc_block_bytes(kSaNt, NP), piece = kSaNt * 128u;
     wg_fence();
 #pragma unroll
@@ -217,6 +234,10 @@ __device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[
                               wg_desc(wb + (uint32_t)c * cstride + (uint32_t)(s >> 2) * bb + Split<NP>::w(tt) * piece + (uint32_t)(s & 3) * 32u),
                               (tt | s) ? 1u : 0u);
     wg_commit();
+}
+template <int NP, int KS, int NCH>
+__device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[NP][8][4], uint32_t wb, uint32_t cstride) {
+    sa_mma_issue<NP, KS, NCH>(d, A, wb, cstride);
     wg_wait_all();
 #pragma unroll
     for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
@@ -228,18 +249,21 @@ __device__ __forceinline__ void unit_bar_sync(int id, int count) { asm volatile(
 // Specialised on the level shape: C1 = width of layer 1 (64 | 128), NL = tensor layers (1 | 2), N0 = width of the inner tensor
 // layer when NL = 2 (64 | 128).  The last layer's width is a runtime multiple of 64.
 template <int NP, int C1, int NL, int N0>
-__global__ void __launch_bounds__(kSaThreads, NP == 2 && C1 == 64 && N0 == 64 ? 2 : 1)     // 64-64-x levels: two CTAs per SM
+__global__ void __launch_bounds__(kSaThreads, NP == 2 && C1 == 64 && (NL == 1 || N0 == 64) ? 2 : 1)   // 64-(64-)x: two CTAs per SM
 tc_sa_kernel(const __grid_constant__ TcArgs a) {
     static_assert((C1 == 64 || C1 == 128) && (NL == 1 || (NL == 2 && (N0 == 64 || N0 == 128))), "unsupported level shape");
     constexpr int last = NL - 1;
     constexpr int KSL = (NL == 2 ? N0 : C1) / 16;            // K steps of the last layer
+    // a second last-layer accumulator (the next chunk's wgmma run during this one's epilogue) costs 32 registers: the levels
+    // whose layers before the last are 64 wide keep one, so that they stay small enough for two CTAs per SM
+    constexpr bool kDouble = !(C1 == 64 && (NL == 1 || N0 == 64));
     if (a.run_if != nullptr && *a.run_if == 0u) return;      // np = 3 rerun of a launch that stayed inside the fp16 range: nothing to do
     constexpr uint32_t bb = tc_block_bytes(kSaNt, NP);
-    uint32_t ovf = 0u;                                        // np = 2: packed |max| of every leading piece this thread stores
+    uint32_t ovf = 0u;                                        // np = 2: packed |max| of every leading piece this thread stores ..
+    bool ovf_seen = false;                                    // .. folded in once per pass, so that `ovf` lives only in layers 1..L-1
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_rbar;                 // resident weights landed
     __shared__ __align__(8) uint64_t s_wbar[2];              // ring slot landed
-    __shared__ __align__(16) float s_red[8][64];
     __shared__ unsigned int s_claim[2];                      // [unit]: the chunk claimed after the current one
     __shared__ int s_slots[2][2][16];                        // [unit][table]: 16-row slots of each neighbourhood of a chunk
     __shared__ long long s_desc[2][2][8];                    // [unit][pass parity][warp]: pooling run that starts at the warp
@@ -294,7 +318,6 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         }
         if (a.stream_last) { sa_fill_ring(0, a.image[last], NCL, L, base, s_wbar); sa_fill_ring(1, a.image[last], NCL, L, base, s_wbar); }
     }
-    uint32_t q_used = 0;                                      // ring uses consumed (fills issued: q_used + 2)
     if (resident) mbar_wait(&s_rbar, 0);
 
     // Work is done by units of threads.  K <= 64: each warpgroup is a unit of its own, so the two run out of step -- one's
@@ -317,6 +340,8 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     const int wl = warp - uw0;                                // warp index in the unit
     const unsigned nchunks = (unsigned)((a.groups + C - 1) / C);
     float* carry = reinterpret_cast<float*>(base + L.total) + (size_t)unit * a.Ntot[last];   // warpgroup units: Ntot[last] floats
+    const int NG = a.pool_chunks, rs = 64 * NG;               // chunks pooled together, floats per warp row of `red`
+    float* red = reinterpret_cast<float*>(base + L.total + sa_carry_bytes(a)) + (size_t)warp * rs;   // this warp's row
 
     // slot counts of chunk ch into table b, by the whole unit (read after a unit barrier).  L = 1 + the last j with
     // idx[j] != idx[0] (1 when all are equal), from a ballot per 32 entries; a warp covers 128 entries = 4 neighbourhoods of 32
@@ -349,19 +374,21 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         }
     };
 
-    // Layer 1's inputs for this thread's two rows are gathered one pass ahead (NL = 2), during the previous pass's last layer:
-    // stage A (neighbour index, centre) after the first chunk's pooling barrier -- after the second one when the pass opens a
-    // chunk, whose slot table is filled in between -- and stage B (neighbour coordinates, U row) after the second one.  The
-    // 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM, so registers are
-    // plentiful); other levels load them in layer 1.
+    // Layer 1's inputs for this thread's two rows are gathered one pass ahead (NL = 2), while the previous pass's last-layer
+    // wgmma run: stage A (neighbour index, centre) once the first chunk is issued, stage B (neighbour coordinates, U row) once
+    // the last one is.  The next pass's slot table must be filled by then; it is not when the next pass opens a chunk claimed
+    // in this very pass (the table is filled between the pooling barriers), and both stages then follow the first pooling.
+    // The 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM); other levels
+    // load them in layer 1.
     constexpr bool kHoldU = NP == 2 && C1 == 128;
     constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the pass:
                                                               // measured faster there, the pass is too short to hide the loads
     constexpr int kUH = kHoldU ? C1 / 8 : 1;                  // float2 per row held
-    int incl = 0, T = 0;                                      // slots of the chunk gather_a last read: prefix (lane i: neighbourhoods
-                                                              // 0..i), total
+    int incl = 0;                                             // slots of the chunk gather_a last read, prefix (lane i: neighbourhoods
+                                                              // 0..i); the chunk's total is lane C - 1's, one shuffle away
     int jn[2];
     long long gn = 0;                                         // the neighbourhood of this warp's slot
+    bool carry_next = false;                                  // warp 0: the gathered pass continues a run of the pass before
     float cx = 0.f, cy = 0.f, cz = 0.f, px[2], py[2], pz[2];
     const float* urow[2];
     float2 uh[2][kUH];
@@ -374,8 +401,8 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                 const int y = __shfl_up_sync(0xffffffffu, incl, o);
                 if (lane >= o) incl += y;
             }
-            T = __shfl_sync(0xffffffffu, incl, C - 1);
         }
+        const int T = __shfl_sync(0xffffffffu, incl, C - 1);
         const int s = p * W + wl, ss = min(s, T - 1);
         const int nb = __popc(__ballot_sync(0xffffffffu, incl <= ss) & ((1u << C) - 1u));
         const int end = __shfl_sync(0xffffffffu, incl, nb), start = nb ? __shfl_sync(0xffffffffu, incl, nb - 1) : 0;
@@ -385,6 +412,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         for (int i = 0; i < 2; ++i) jn[i] = __ldg(a.idx + gn * K + row + 8 * i);
         const float* c = a.new_xyz + (size_t)gn * 3;
         cx = __ldg(c); cy = __ldg(c + 1); cz = __ldg(c + 2);
+        carry_next = wl == 0 && s < T && s > start;
         if (lane == 0) {
             // a run = the warps of one neighbourhood in this pass: [len, carried in from the last pass, carried out to the next]
             long long run = 0;
@@ -403,7 +431,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
             px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
             urow[i] = a.uf ? a.uf + ((size_t)bi * a.n + jn[i]) * C1 : nullptr;
             if constexpr (kHoldU) {
-                if (urow[i] != nullptr) {
+                if (a.uf != nullptr) {
 #pragma unroll
                     for (int q = 0; q < kUH; ++q) uh[i][q] = __ldg(reinterpret_cast<const float2*>(urow[i] + 8 * q + 2 * t));
                 }
@@ -411,20 +439,20 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         }
     };
 
-    // The chunk after the current one is claimed at the top of the current one's first pass and read after the first pooling
-    // barrier of its last pass; the barrier after that orders the read before the next claim.
+    // The chunk after the current one is claimed at the top of the current one's first pass, read after the first pooling
+    // barrier of that pass and its slot table filled before the second; the barriers order the read before the next claim
+    // and the table before the gather that reads it.
     if (ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
     unit_bar_sync(ubar, uthreads);
-    unsigned ch = s_claim[unit];
+    unsigned ch = s_claim[unit], claimed = 0;
     if (ch < nchunks) fill_table(ch, 0);
     unit_bar_sync(ubar, uthreads);
     int buf = 0, p = 0;                                       // slot table and pass index of the current chunk
     if (kAhead && ch < nchunks) { gather_a(ch, 0, 0, 0); gather_b(); }
-    for (uint32_t it = 0; ch < nchunks; ++it) {
+    uint32_t it = 0;                                          // passes of this unit
+    for (; ch < nchunks; ++it) {
         if (p == 0 && ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
         if (!kAhead) { gather_a(ch, buf, p, it & 1); gather_b(); }
-        unsigned nch = ch;                                    // the next pass: chunk, slot table, pass index
-        int nbuf = buf, np = p + 1;
 
         // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
         uint32_t A[NP][8][4];
@@ -446,7 +474,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                             float2 uv;
                             if constexpr (kHoldU) uv = uh[i][2 * s + h];
                             else uv = urow[i] ? __ldg(reinterpret_cast<const float2*>(urow[i] + k)) : sh;
-                            float2 v = urow[i] ? ffma2_rn(uv, sc, sh) : sh;
+                            float2 v = a.uf ? ffma2_rn(uv, sc, sh) : sh;
                             if (a.w1c != nullptr) {        // EdgeConv: the part of the first layer that acts on the centre x_i
                                 const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
                                              cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
@@ -484,78 +512,133 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                 }
             }
         }
+        if constexpr (NP == 2) { ovf_seen = ovf_seen || f16x2_overflowed(ovf); ovf = 0u; }   // every leading piece is stored
         {
-            // ---- last layer, 64 output channels at a time, max-pooled over each neighbourhood ----
+            // ---- last layer, 64 output channels at a time, max-pooled over each neighbourhood once per NG chunks ----
+            // kDouble: chunk nc + 1's group is issued before chunk nc's epilogue and runs during it (wait_group 1)
             const int N = a.Ntot[last];
-            for (int nc = 0; nc < NCL; ++nc) {
+            const bool carry_in = carry_next;                 // warp 0 folds the carried run max into its pooled maxima
+            // the next pass continues this chunk, or opens `claimed`
+            const bool same = (p + 1) * W < __shfl_sync(0xffffffffu, incl, C - 1);
+            // gather the next pass in the shadow of this one's last layer: its slot table is ready unless the chunk was claimed
+            // in this pass, and then the gather follows the first pooling
+            const bool ahead = kAhead && (same || (p > 0 && claimed < nchunks));
+            const bool after_pool = kAhead && !same && p == 0;
+            auto issue = [&](float (&acc)[1][32], int nc) {
                 uint32_t wb;
-                if (a.stream_last) {
-                    mbar_wait(&s_wbar[q_used & 1], (q_used >> 1) & 1u);
-                    wb = smem_u32(base + L.ring[q_used & 1]);
+                if (a.stream_last) {                              // ring use q = chunk nc of pass it (every pass runs all NCL)
+                    const uint32_t q = it * (uint32_t)NCL + (uint32_t)nc;
+                    mbar_wait(&s_wbar[q & 1], (q >> 1) & 1u);
+                    wb = smem_u32(base + L.ring[q & 1]);
                 } else {
                     wb = smem_u32(base + L.w[last]) + (uint32_t)(nc * (KSL / 4)) * bb;
                 }
-                float d[1][32];
-                sa_mma<NP, KSL, 1>(d, A, wb, 0u);
+                sa_mma_issue<NP, KSL, 1>(acc, A, wb, 0u);
+            };
+            // affine + ReLU of chunk nc, this warp's 16-row column maxima (and warp 0's carried run max) into its row of `red`
+            auto epilogue = [&](float (&acc)[1][32], int nc) {
+                wg_fence_acc(acc[0]);
+                auto rowmax = [&](int j) {                        // columns 8j + 2t, + 1: max over rows g, g + 8
+                    const int col = nc * 64 + 8 * j + 2 * t;
+                    const float2 sc = *reinterpret_cast<const float2*>(slL + col), sh = *reinterpret_cast<const float2*>(tlL + col);
+                    float lo0 = fmaf(acc[0][4 * j], sc.x, sh.x), hi0 = fmaf(acc[0][4 * j + 2], sc.x, sh.x);
+                    float lo1 = fmaf(acc[0][4 * j + 1], sc.y, sh.y), hi1 = fmaf(acc[0][4 * j + 3], sc.y, sh.y);
+                    if (a.relu[last]) { lo0 = fmaxf(lo0, 0.f); hi0 = fmaxf(hi0, 0.f); lo1 = fmaxf(lo1, 0.f); hi1 = fmaxf(hi1, 0.f); }
+                    return make_float2(fmaxf(lo0, hi0), fmaxf(lo1, hi1));
+                };
+                float v[8];
+                const bool up = (g >> 2) & 1;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int col = nc * 64 + 8 * j + 2 * t + e;
-                        const float sc = slL[col], sh = tlL[col];
-                        float lo = fmaf(d[0][4 * j + e], sc, sh), hi = fmaf(d[0][4 * j + 2 + e], sc, sh);
-                        if (a.relu[last]) { lo = fmaxf(lo, 0.f); hi = fmaxf(hi, 0.f); }
-                        const float m = warp_rowmax16(lo, hi);
-                        if (g == 0) s_red[warp][8 * j + 2 * t + e] = m;
-                    }
+                for (int j = 0; j < 4; ++j) {                     // first step of the butterfly: column blocks j and j + 4
+                    const float2 lo = rowmax(j), hi = rowmax(j + 4);
+                    v[2 * j] = fmaxf(up ? hi.x : lo.x, __shfl_xor_sync(0xffffffffu, up ? lo.x : hi.x, 16));
+                    v[2 * j + 1] = fmaxf(up ? hi.y : lo.y, __shfl_xor_sync(0xffffffffu, up ? lo.y : hi.y, 16));
                 }
-                // a run carried in from the last pass only starts at warp 0; its partial max is read before the barrier, since
-                // a run of this pass may carry its own out through the same words after it
-                const float2 cin = !joint && wl == 0 ? reinterpret_cast<const float2*>(carry)[nc * 32 + lane] : make_float2(0.f, 0.f);
-                unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in s_red; ring slot consumed
-                if (nc == 0) {
-                    if (np * W < T) {
-                        if (kAhead) gather_a(ch, buf, np, (it + 1) & 1);
-                    } else {                                      // the next pass opens the claimed chunk
-                        nch = s_claim[unit]; nbuf = buf ^ 1; np = 0;
-                        if (nch < nchunks) fill_table(nch, nbuf);
-                    }
+                colmax_halve<4>(v, (g >> 1) & 1);
+                colmax_halve<2>(v, g & 1);
+                float2 m = make_float2(v[0], v[1]);
+                const int x = 8 * g + 2 * t;
+                float* dst = red + (nc % NG) * 64 + x;
+                {   // written by the last pass; this pass writes it after a pooling barrier.  Every warp loads and selects, so
+                    // that no branch sits inside the wgmma group in flight; without a carry the load reads its own `red` words
+                    const float2 c = *reinterpret_cast<const float2*>(carry_in ? carry + nc * 64 + x : dst);
+                    m.x = carry_in ? fmaxf(m.x, c.x) : m.x;
+                    m.y = carry_in ? fmaxf(m.y, c.y) : m.y;
                 }
-                if (a.stream_last) {
-                    if (tid == 0) sa_fill_ring(q_used + 2, a.image[last], NCL, L, base, s_wbar);
-                    ++q_used;
+                *reinterpret_cast<float2*>(dst) = m;
+            };
+            // chunks [gi NG, gi NG + NG) are in `red`: combine the run starting at each warp's slot, two columns per lane
+            auto pool = [&](int gi) {
+                unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in red; ring slot consumed
+                if (gi == 0 && p == 0) {                          // the chunk claimed at the top of this pass
+                    claimed = s_claim[unit];
+                    if (claimed < nchunks) fill_table(claimed, buf ^ 1);
                 }
-                {                                                 // the run starting at this warp's slot, two columns per lane
-                    const long long run = s_desc[unit][it & 1][wl];
-                    const int len = (int)(run & 15);
-                    if (len != 0) {
-                        const float2* red = reinterpret_cast<const float2*>(&s_red[warp][0]) + lane;
-                        float2 mx = red[0];
+                if (a.stream_last && tid == 0)                    // NG = 1: ring use gi of this pass is consumed
+                    sa_fill_ring(it * (uint32_t)NCL + (uint32_t)gi + 2u, a.image[last], NCL, L, base, s_wbar);
+                const long long run = s_desc[unit][it & 1][wl];
+                const int len = (int)(run & 15);
+                if (len != 0) {
+                    for (int c = 0; c < NG; ++c) {
+                        const float2* r = reinterpret_cast<const float2*>(red + c * 64) + lane;
+                        float2 mx = r[0];
 #pragma unroll
                         for (int w = 1; w < 8; ++w)
-                            if (w < len) { const float2 v = red[32 * w]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); }
-                        if (run & 16) { mx.x = fmaxf(mx.x, cin.x); mx.y = fmaxf(mx.y, cin.y); }
-                        if (run & 32) reinterpret_cast<float2*>(carry)[nc * 32 + lane] = mx;
-                        else *reinterpret_cast<float2*>(a.out + (size_t)(run >> 8) * N + nc * 64 + 2 * lane) = mx;
+                            if (w < len) { const float2 v = r[w * rs / 2]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); }
+                        const int col = (gi * NG + c) * 64 + 2 * lane;
+                        if (run & 32) *reinterpret_cast<float2*>(carry + col) = mx;
+                        else *reinterpret_cast<float2*>(a.out + (size_t)(run >> 8) * N + col) = mx;
                     }
                 }
-                unit_bar_sync(ubar, uthreads);                    // s_red is reused by the next chunk; the slot table is filled
-                if (kAhead && nc == 0 && nch < nchunks) {
-                    if (np == 0) gather_a(nch, nbuf, 0, (it + 1) & 1);
-                    gather_b();
+                unit_bar_sync(ubar, uthreads);                    // red is reused by the next group; the slot table is filled
+                if (gi == 0 && after_pool && claimed < nchunks) { gather_a(claimed, buf ^ 1, 0, (it + 1) & 1); gather_b(); }
+            };
+            // Every path below issues and waits in straight lines, and every group ends in wait_group 0 before pooling: ptxas
+            // keeps the wgmma asynchronous only when it can see which group a wait retires on every path.  Stage B of the
+            // gather is issued on every path that waits for the last chunk (NCL - 1), before that wait and after the epilogue
+            // of the chunk before it: whatever the group size, it follows stage A in every pass that gathers ahead.
+            float d0[1][32];
+            for (int c0 = 0; c0 < NCL; c0 += NG) {
+                const int end = c0 + NG;
+                issue(d0, c0);
+                if (ahead && c0 == 0) gather_a(same ? ch : claimed, same ? buf : buf ^ 1, same ? p + 1 : 0, (it + 1) & 1);
+                if constexpr (kDouble) {
+                    float d1[1][32];
+                    int nc = c0;
+                    for (; nc + 2 < end; nc += 2) {
+                        issue(d1, nc + 1); wg_wait<1>(); epilogue(d0, nc);
+                        issue(d0, nc + 2); wg_wait<1>(); epilogue(d1, nc + 1);
+                    }
+                    if (nc + 1 < end) {
+                        issue(d1, nc + 1); wg_wait<1>(); epilogue(d0, nc);
+                        if (ahead && nc + 2 == NCL) gather_b();
+                        wg_wait<0>(); epilogue(d1, nc + 1);
+                    } else {
+                        if (ahead && nc + 1 == NCL) gather_b();
+                        wg_wait<0>(); epilogue(d0, nc);
+                    }
+                } else {
+                    for (int nc = c0;;) {
+                        if (ahead && nc + 1 == NCL) gather_b();
+                        wg_wait<0>(); epilogue(d0, nc);
+                        if (++nc == end) break;
+                        issue(d0, nc);
+                    }
                 }
+                pool(c0 / NG);
             }
+            if (!same) { ch = claimed; buf ^= 1; p = 0; }
+            else ++p;
         }
-        ch = nch; buf = nbuf; p = np;
     }
     if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf)) atomicOr(a.ovf, 1u);
+        if (ovf_seen) atomicOr(a.ovf, 1u);
         if (tid == 0)
             for (int l = 0; l < NL; ++l)
                 if (a.wflag[l] != nullptr && *a.wflag[l] != 0u) atomicOr(a.ovf, 1u);
     }
     if (tid == 0 && a.stream_last)                                    // the two fills issued ahead must land before the CTA exits
-        for (uint32_t q = q_used; q < q_used + 2; ++q) mbar_wait(&s_wbar[q & 1], (q >> 1) & 1u);
+        for (uint32_t q = it * (uint32_t)NCL; q < it * (uint32_t)NCL + 2u; ++q) mbar_wait(&s_wbar[q & 1], (q >> 1) & 1u);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -954,14 +1037,23 @@ static int launch_tc_sa_shape(const TcArgs& a, long long ctas_needed, size_t sme
 template <int NP>
 static int launch_tc_sa_np(TcArgs& a, cudaStream_t st) {
     // chunks of one unit (see tc_sa_kernel): a unit is a warpgroup, or the whole CTA when K = 128 or the last layer streams.
-    // The pooling carry of warpgroup units sits after the layout, in the shared memory the SM has above the budget
-    // tc_sa_eligible checks; a level whose carry does not fit there keeps joint units (4 KB are left for the static arrays).
+    // The pooling carry of warpgroup units and the pooling buffer sit after the layout, in the shared memory the SM has above
+    // the budget tc_sa_eligible checks (4 KB are left for the static arrays).  The buffer holds as many of the last layer's
+    // 64-channel chunks as fit (all of them for the PointNet++ levels: one pooling per pass); a streamed last layer pools each
+    // chunk before its ring slot is refilled.  A level whose carry and one-chunk buffer do not fit keeps joint units.
+    const uint32_t limit = 223u * 1024u;
     a.joint = a.K == 128 || a.stream_last;
-    if (!a.joint && tc_sa_layout(a).total + 1024 + sa_carry_bytes(a) > 223u * 1024u) a.joint = 1;
+    if (!a.joint && tc_sa_layout(a).total + 1024 + sa_carry_bytes(a) + sa_red_bytes(1) > limit) a.joint = 1;
+    const size_t used = (size_t)tc_sa_layout(a).total + 1024 + sa_carry_bytes(a);
+    const int ncl = a.Ntot[a.nl - 1] / 64;
+    a.pool_chunks = 1;
+    if (!a.stream_last)
+        for (int ng = ncl; ng > 1; --ng)
+            if (ncl % ng == 0 && used + sa_red_bytes(ng) <= limit) { a.pool_chunks = ng; break; }
     const int C = sa_chunk(a.K, a.joint);
     const long long nchunks = (a.groups + C - 1) / C;
     const long long ctas_needed = a.joint ? nchunks : (nchunks + 1) / 2;   // two units per CTA
-    const size_t smem = (size_t)tc_sa_layout(a).total + 1024 + sa_carry_bytes(a);
+    const size_t smem = used + sa_red_bytes(a.pool_chunks);
     // shapes accepted by tc_sa_eligible: C1 in {64, 128}, one or two tensor layers, an inner layer 64 or 128 wide
     if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas_needed, smem, st);
     if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas_needed, smem, st);
