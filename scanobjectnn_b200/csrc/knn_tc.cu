@@ -44,10 +44,6 @@ constexpr int kKtBins = 256;
 constexpr int kKtCap = 96;                        // list entries per row
 constexpr int kKtMaxN = 2048;                     // candidates per cloud on this path (shared-memory budget)
 
-__device__ __forceinline__ void mbar_arrive1(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
-}
-
 // ---- centre: a translation vector per cloud (mean of every 8th point, fixed order).  Distances do not depend on it mathematically;
 // the tensor-core passes run on x - mu so that their error bounds scale with the cloud's EXTENT, not with its offset from the origin
 // (post-ReLU feature clouds sit far from it: |x|^2 ~ 100 x the neighbour distances, and bounds relative to |x|^2 would admit

@@ -40,6 +40,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
             : "memory");
     } while (!done);
 }
+__device__ __forceinline__ void mbar_arrive1(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
 
 // ---- bulk async copy global -> shared (TMA engine, 1-D, no tensor map), completion on an mbarrier ----
@@ -51,6 +54,18 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                      smem_u32(smem_dst)),
                  "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
+}
+
+// ---- per-thread async copies global -> shared (cp.async); the thread's copies issued so far arrive on an mbarrier when done ----
+__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"(smem_dst), "l"(gmem_src) : "memory");
+}
+// counts as one of the barrier's expected arrivals (.noinc)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint64_t* bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
 
 // ---- descriptors ----

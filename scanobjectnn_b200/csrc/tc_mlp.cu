@@ -16,8 +16,9 @@
 //
 // Kernels (both templated on NP, the pieces per operand -- Split<NP> in tc_common.cuh):
 //   tc_sa_kernel<NP,..>       SA level (specialised on its shape); optional centre weights = multi-layer EdgeConv over 3-D points
-//   tc_dense_kernel<NP,NC>    dense layer, 64 NC output channels per CTA; also the training-mode forward (previous batch norm
-//                             applied on load, column statistics in the epilogue)
+//   tc_dense_kernel<NP,NC>    dense layer, persistent over 128-row x 64 NC-channel tiles, a producer warp feeding two consumer
+//                             warpgroups; also the training-mode forward (previous batch norm applied on load, column
+//                             statistics in the epilogue)
 // fp32 parity: operands are quantised by this code, so the tensor core only ever sees exactly representable values; fp32
 // accumulation in the tensor core truncates, hence small terms first and K cut into <= 128-wide pieces (tests hold 1e-5 vs fp64).
 //   NP = 2 (inference default): two fp16 pieces, three MMAs per product; every kernel tracks the leading pieces it stores and raises
@@ -666,185 +667,277 @@ struct TcDenseArgs {
     unsigned int* ovf = nullptr;
     const unsigned int* run_if = nullptr;
     const unsigned int* wflag = nullptr;
+    // zeroed before the launch: tiles are claimed from it (a CTA that starts late or shares its SM with another stream's
+    // kernels simply takes fewer); null: CTA i takes tiles i, i + grid, ...
+    unsigned int* tile_counter = nullptr;
 };
 
-// CTA = 256 threads = two warpgroups = 128 rows x Nt = 64 NC output channels.  K is walked in 64-wide blocks: the block's x is
-// read straight into A fragments (the previous layer's batch norm + ReLU applied on the fly in training mode) while its weight
-// block lands through a four-slot TMA ring; each block's wgmma sum is added to fp32 register accumulators, so the tensor core's
-// accumulation never runs over more than 64 K however long the dot product is.  Epilogue in the fragment layout: xyz side input,
-// affine, ReLU, then either float2 stores (+ per-tile column statistics) or the max over pool_k rows.
-constexpr int kDenseThreads = 256, kDenseStages = 4;
+// Persistent, warp-specialised.  CTA = two consumer warpgroups (rows 0-63 / 64-127 of a 128-row x Nt = 64 NC tile) + a
+// producer warpgroup, of which one warp works; setmaxnreg moves the registers to the consumers.  The producer claims tiles and
+// streams their 64-wide K blocks through a ring of stages, each holding the block's x rows (fp32, padded rows: conflict-free
+// fragment reads) and its weight block, one full mbarrier per stage; consumers release a stage through its empty mbarrier
+// (one arrival per warp).  The ring runs across tiles, so the next tile's first blocks land during this tile's epilogue.
+//   Per block the consumers issue the wgmma group, split the NEXT block's x (shared memory -> A fragments, batch norm + ReLU
+// of training mode, fp16 range tracking) while it runs, then wait and add the block's sum to the fp32 accumulators: the tensor
+// core's accumulation never runs over more than 64 K however long the dot product is, and every output sees the same sums
+// in the same order whatever the schedule.  One group in flight at a time, so every wait retires the same group on every path.
+//   Epilogue in the fragment layout: xyz side input, affine, ReLU, then either float2 stores (+ per-tile column statistics) or
+// the max over pool_k rows; the cross-warp part synchronises the consumers on a named barrier.
+constexpr int kDenseThreads = 384, kDenseConsumers = 256;
+constexpr uint32_t kDenseXRow = 64u * 4u + 32u;           // bytes per staged x row: 8-bank offset between rows g and g + 1
+constexpr uint32_t kDenseXBytes = 128u * kDenseXRow;
+constexpr uint32_t kDenseRingBudget = 210u * 1024u;       // the ring's shared memory (next to s_red and the barriers)
+__host__ __device__ constexpr uint32_t dense_stage_bytes(int NP, int NC) { return tc_block_bytes(64 * NC, NP) + kDenseXBytes; }
+__host__ __device__ constexpr int dense_stages(int NP, int NC) {
+    return kDenseRingBudget / dense_stage_bytes(NP, NC) < 4u ? (int)(kDenseRingBudget / dense_stage_bytes(NP, NC)) : 4;
+}
 
 template <int NP, int NC>
 __global__ void __launch_bounds__(kDenseThreads, 1)
 tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
     if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr int Nt = 64 * NC;
-    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u;
-    uint32_t ovf = 0u;
+    constexpr int Nt = 64 * NC, S = dense_stages(NP, NC);
+    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = dense_stage_bytes(NP, NC);
+    static_assert(S >= 2, "the ring needs two stages");
     extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_wfull[kDenseStages];
+    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
+    __shared__ int s_tile[S];                                       // the tile a stage belongs to, -1: no more tiles
     __shared__ float s_red[2][8][Nt];
-    __shared__ __align__(16) float s_vec[5][Nt];     // scale, shift, three xyz rows of W for this CTA's output channels
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int g = lane >> 2, t = lane & 3;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int KC = a.Kp / 64;
-    const int nt = blockIdx.y;
-    const long long row0 = (long long)blockIdx.x * 128;
-    const uint8_t* img = a.image + (size_t)nt * KC * bb;
-    for (int i = tid; i < Nt; i += kDenseThreads) {
-        const int c = nt * Nt + i;
-        s_vec[0][i] = a.scale ? __ldg(a.scale + c) : 1.f;
-        s_vec[1][i] = a.shift ? __ldg(a.shift + c) : 0.f;
-        s_vec[2][i] = a.xyz3 ? __ldg(a.w3 + c) : 0.f;
-        s_vec[3][i] = a.xyz3 ? __ldg(a.w3 + a.N + c) : 0.f;
-        s_vec[4][i] = a.xyz3 ? __ldg(a.w3 + 2 * a.N + c) : 0.f;
-    }
+    const int KC = a.Kp / 64, NTC = a.N / Nt;
+    const long long ntiles = (a.rows + 127) / 128 * NTC;
     if (tid == 0) {
-        for (int i = 0; i < kDenseStages; ++i) mbar_init(&s_wfull[i], 1);
+        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 32); mbar_init(&s_empty[i], kDenseConsumers / 32); }
         fence_mbar_init();
     }
     __syncthreads();
-    auto load_block = [&](int kb) {       // thread 0
-        uint64_t* bar = &s_wfull[kb % kDenseStages];
-        mbar_expect_tx(bar, bb);
-        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (kb % kDenseStages) * bb + o, img + (size_t)kb * bb + o, min(16384u, bb - o), bar);
-    };
-    if (tid == 0)
-        for (int kb = 0; kb < kDenseStages && kb < KC; ++kb) load_block(kb);
 
-    const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
-    const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
-    const bool vec2 = ((a.K & 1) == 0) && ((reinterpret_cast<uintptr_t>(a.x) & 7) == 0);
-    auto load_x2 = [&](int i, int k) {    // x[r_i][k], x[r_i][k + 1] (zero past the end), batch norm + ReLU of training mode
-        float2 x = make_float2(0.f, 0.f);
-        if (v[i]) {
-            const float* xr = a.x + (size_t)r[i] * a.K + k;
-            if (vec2 && k + 1 < a.K) x = __ldg(reinterpret_cast<const float2*>(xr));
-            else { if (k < a.K) x.x = __ldg(xr); if (k + 1 < a.K) x.y = __ldg(xr + 1); }
-            if (a.in_scale != nullptr) {
-                if (k < a.K) { x.x = fmaf(x.x, __ldg(a.in_scale + k), __ldg(a.in_shift + k)); if (a.in_relu) x.x = fmaxf(x.x, 0.f); }
-                if (k + 1 < a.K) { x.y = fmaf(x.y, __ldg(a.in_scale + k + 1), __ldg(a.in_shift + k + 1)); if (a.in_relu) x.y = fmaxf(x.y, 0.f); }
-            }
-        }
-        return x;
-    };
-
-    float acc[NC][32];
-    for (int kb = 0; kb < KC; ++kb) {
-        uint32_t A[NP][4][4];
-#pragma unroll
-        for (int s = 0; s < 4; ++s)
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const float2 x = load_x2(i, kb * 64 + 16 * s + 8 * h + 2 * t);
-                    put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
+    if (warp >= kDenseConsumers / 32) {
+        // ---- producer ----
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+        if (warp != kDenseConsumers / 32) return;
+        const bool vec = (a.K & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0;    // rows of x are 16-byte aligned
+        uint32_t q = 0;                                             // ring uses
+        for (long long i = 0;; ++i) {
+            long long tile = 0;
+            if (lane == 0) tile = a.tile_counter != nullptr ? (long long)atomicAdd(a.tile_counter, 1u) : (long long)blockIdx.x + i * gridDim.x;
+            tile = __shfl_sync(0xffffffffu, tile, 0);
+            const bool done = tile >= ntiles;
+            const long long row0 = tile / NTC * 128;
+            const int nt = (int)(tile % NTC), nrows = done ? 0 : (int)min(128LL, a.rows - row0);
+            for (int kb = 0; kb < KC; ++kb, ++q) {
+                const int s = (int)(q % S);
+                if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
+                if (lane == 0) {
+                    s_tile[s] = done ? -1 : (int)tile;
+                    if (done) {
+                        mbar_arrive1(&s_full[s]);
+                    } else {
+                        mbar_expect_tx(&s_full[s], bb);
+                        const uint8_t* src = a.image + ((size_t)nt * KC + kb) * bb;
+                        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
+                    }
                 }
-        mbar_wait(&s_wfull[kb % kDenseStages], (uint32_t)((kb / kDenseStages) & 1));
-        const uint32_t wb = smem_u32(base) + (uint32_t)(kb % kDenseStages) * bb;
-        float d[NC][32];
-        wg_fence();
-#pragma unroll
-        for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+                if (!done) {
+                    // x rows [row0, row0 + nrows) x columns [64 kb, 64 kb + kw): 16-byte async copies, a warp covering two rows per
+                    // instruction, or 4-byte ones for odd K / unaligned x.  Rows past `rows` and columns past K are left stale: the
+                    // consumers read them as zero.
+                    const uint32_t xs = smem_u32(base + (uint32_t)s * SB + bb);
+                    const float* xb = a.x + (size_t)row0 * a.K + kb * 64;
+                    const int kw = min(64, a.K - kb * 64);
+                    if (vec) {
+                        for (int e = lane; e < nrows * 16; e += 32) {
+                            const int r = e >> 4, c = (e & 15) * 4;
+                            if (c < kw) cp_async16(xs + (uint32_t)r * kDenseXRow + (uint32_t)c * 4u, xb + (size_t)r * a.K + c);
+                        }
+                    } else {
+                        for (int e = lane; e < nrows * 64; e += 32) {
+                            const int r = e >> 6, c = e & 63;
+                            if (c < kw) cp_async4(xs + (uint32_t)r * kDenseXRow + (uint32_t)c * 4u, xb + (size_t)r * a.K + c);
+                        }
+                    }
+                }
+                cp_async_mbar_arrive(&s_full[s]);                  // one arrival per lane, once its copies have landed
+                if (done) break;
+            }
+            if (done) return;
+        }
+    }
+
+    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+    const int g = lane >> 2, t = lane & 3;
+    uint32_t ovf = 0u;
+    uint32_t q = 0;                                                 // ring uses
+    for (;;) {
+        mbar_wait(&s_full[q % S], (q / S) & 1u);
+        const int tile = s_tile[q % S];
+        if (tile < 0) break;
+        const long long row0 = (long long)(tile / NTC) * 128;
+        const int nt = tile % NTC;
+        const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
+        const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
+
+        // x block of ring use u -> A fragments: rows past `rows` and columns past K read as zero (as the staged bytes there
+        // are stale), then the previous layer's batch norm + ReLU of training mode
+        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t u, int kb) {
+            const float* xs = reinterpret_cast<const float*>(base + (u % S) * SB + bb);
 #pragma unroll
             for (int s = 0; s < 4; ++s)
 #pragma unroll
-                for (int c = 0; c < NC; ++c)
-                    wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
-                                  wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)c * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
-        wg_commit();
-        wg_wait_all();
+                for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int c = 0; c < NC; ++c) {
-            wg_fence_acc(d[c]);
+                    for (int i = 0; i < 2; ++i) {
+                        const int kl = 16 * s + 8 * h + 2 * t, k = kb * 64 + kl;
+                        float2 x = make_float2(0.f, 0.f);
+                        if (v[i]) {
+                            const float2 y = *reinterpret_cast<const float2*>(xs + (warp * 16 + g + 8 * i) * (int)(kDenseXRow / 4) + kl);
+                            if (k < a.K) x.x = y.x;
+                            if (k + 1 < a.K) x.y = y.y;
+                            if (a.in_scale != nullptr) {
+                                if (k < a.K) { x.x = fmaf(x.x, __ldg(a.in_scale + k), __ldg(a.in_shift + k)); if (a.in_relu) x.x = fmaxf(x.x, 0.f); }
+                                if (k + 1 < a.K) { x.y = fmaf(x.y, __ldg(a.in_scale + k + 1), __ldg(a.in_shift + k + 1)); if (a.in_relu) x.y = fmaxf(x.y, 0.f); }
+                            }
+                        }
+                        put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
+                    }
+        };
+        float acc[NC][32];
+        // block kb (ring use u): issue its group on A, prepare block kb + 1 into An while it runs, wait, release the stage, add.
+        // bf16x3 128-wide tiles issue one 64-channel chunk per group (the next block is prepared under the second), so that
+        // two A buffers, the accumulators and one chunk's sum fit the consumers' 232 registers.
+        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
+        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t u, int kb) {
+            const uint32_t wb = smem_u32(base + (u % S) * SB);
 #pragma unroll
-            for (int q = 0; q < 32; ++q) acc[c][q] = kb ? acc[c][q] + d[c][q] : d[c][q];
+            for (int c0 = 0; c0 < NC; c0 += CG) {
+                float d[CG][32];
+                wg_fence();
+#pragma unroll
+                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+#pragma unroll
+                    for (int s = 0; s < 4; ++s)
+#pragma unroll
+                        for (int c = 0; c < CG; ++c)
+                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
+                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
+                wg_commit();
+                if (c0 + CG == NC && kb + 1 < KC) {
+                    mbar_wait(&s_full[(u + 1) % S], ((u + 1) / S) & 1u);
+                    prep(An, u + 1, kb + 1);
+                }
+                wg_wait_all();
+                if (c0 + CG == NC) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive1(&s_empty[u % S]);           // x read, weights consumed: the stage may be refilled
+                }
+#pragma unroll
+                for (int c = 0; c < CG; ++c) {
+                    wg_fence_acc(d[c]);
+#pragma unroll
+                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
+                }
+            }
+        };
+        {
+            uint32_t A0[NP][4][4], A1[NP][4][4];
+            prep(A0, q, 0);
+            for (int kb = 0;; kb += 2) {
+                step(A0, A1, q + kb, kb);
+                if (kb + 1 == KC) break;
+                step(A1, A0, q + kb + 1, kb + 1);
+                if (kb + 2 == KC) break;
+            }
         }
-        __syncthreads();                                             // both warpgroups are done with this weight slot
-        if (tid == 0 && kb + kDenseStages < KC) load_block(kb + kDenseStages);
-    }
+        q += KC;
 
-    // ---- epilogue ----
-    float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
-    if (a.xyz3 != nullptr)
-#pragma unroll
-        for (int i = 0; i < 2; ++i)
-            if (v[i])
-#pragma unroll
-                for (int q = 0; q < 3; ++q) xs[i][q] = __ldg(a.xyz3 + (size_t)r[i] * 3 + q);
-#pragma unroll
-    for (int c = 0; c < NC; ++c)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const int cl = c * 64 + 8 * j + 2 * t;
-            float y[2][2];
+        // ---- epilogue ----
+        float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+        if (a.xyz3 != nullptr)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
+                if (v[i])
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz3 + (size_t)r[i] * 3 + k);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int cl = c * 64 + 8 * j + 2 * t;
+                float y[2][2];
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                    float x = acc[c][4 * j + 2 * i + e];
-                    if (a.xyz3 != nullptr) x = fmaf(xs[i][2], s_vec[4][cl + e], fmaf(xs[i][1], s_vec[3][cl + e], fmaf(xs[i][0], s_vec[2][cl + e], x)));
-                    x = fmaf(x, s_vec[0][cl + e], s_vec[1][cl + e]);
-                    if (a.relu) x = fmaxf(x, 0.f);
-                    y[i][e] = x;
-                }
-            if (a.pool_k == 1) {
+                    const int col = nt * Nt + cl + e;
+                    const float sc = a.scale ? __ldg(a.scale + col) : 1.f, sh = a.shift ? __ldg(a.shift + col) : 0.f;
+                    float w0 = 0.f, w1 = 0.f, w2 = 0.f;
+                    if (a.xyz3 != nullptr) { w0 = __ldg(a.w3 + col); w1 = __ldg(a.w3 + a.N + col); w2 = __ldg(a.w3 + 2 * a.N + col); }
 #pragma unroll
-                for (int i = 0; i < 2; ++i)
-                    if (v[i]) *reinterpret_cast<float2*>(a.out + (size_t)r[i] * a.N + nt * Nt + cl) = make_float2(y[i][0], y[i][1]);
-                if (a.stat_partial != nullptr) {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        float ssum = 0.f, ssq = 0.f;
-#pragma unroll
-                        for (int i = 0; i < 2; ++i)
-                            if (v[i]) { ssum += y[i][e]; ssq = fmaf(y[i][e], y[i][e], ssq); }
-                        ssum = warp_rowsum16(ssum);
-                        ssq = warp_rowsum16(ssq);
-                        if (g == 0) { s_red[0][warp][cl + e] = ssum; s_red[1][warp][cl + e] = ssq; }
+                    for (int i = 0; i < 2; ++i) {
+                        float x = acc[c][4 * j + 2 * i + e];
+                        if (a.xyz3 != nullptr) x = fmaf(xs[i][2], w2, fmaf(xs[i][1], w1, fmaf(xs[i][0], w0, x)));
+                        x = fmaf(x, sc, sh);
+                        if (a.relu) x = fmaxf(x, 0.f);
+                        y[i][e] = x;
                     }
                 }
-            } else {
+                if (a.pool_k == 1) {
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const float m = warp_rowmax16(v[0] ? y[0][e] : -FLT_MAX, v[1] ? y[1][e] : -FLT_MAX);
-                    if (g == 0) s_red[0][warp][cl + e] = m;
+                    for (int i = 0; i < 2; ++i)
+                        if (v[i]) *reinterpret_cast<float2*>(a.out + (size_t)r[i] * a.N + nt * Nt + cl) = make_float2(y[i][0], y[i][1]);
+                    if (a.stat_partial != nullptr) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float ssum = 0.f, ssq = 0.f;
+#pragma unroll
+                            for (int i = 0; i < 2; ++i)
+                                if (v[i]) { ssum += y[i][e]; ssq = fmaf(y[i][e], y[i][e], ssq); }
+                            ssum = warp_rowsum16(ssum);
+                            ssq = warp_rowsum16(ssq);
+                            if (g == 0) { s_red[0][warp][cl + e] = ssum; s_red[1][warp][cl + e] = ssq; }
+                        }
+                    }
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float m = warp_rowmax16(v[0] ? y[0][e] : -FLT_MAX, v[1] ? y[1][e] : -FLT_MAX);
+                        if (g == 0) s_red[0][warp][cl + e] = m;
+                    }
                 }
             }
-        }
-    if (a.pool_k == 1) {
-        if (a.stat_partial != nullptr) {
-            // per-tile column statistics, the eight warps' 16-row partials folded in warp order (deterministic)
-            __syncthreads();
-            for (int cl = tid; cl < Nt; cl += kDenseThreads) {
-                float t0 = 0.f, t1 = 0.f;
-                for (int w = 0; w < 8; ++w) { t0 += s_red[0][w][cl]; t1 += s_red[1][w][cl]; }
-                float* dst = a.stat_partial + (size_t)blockIdx.x * 2 * a.N;
-                dst[nt * Nt + cl] = t0;
-                dst[a.N + nt * Nt + cl] = t1;
+        if (a.pool_k == 1) {
+            if (a.stat_partial != nullptr) {
+                // per-tile column statistics, the eight warps' 16-row partials folded in warp order (deterministic)
+                unit_bar_sync(1, kDenseConsumers);
+                for (int cl = tid; cl < Nt; cl += kDenseConsumers) {
+                    float t0 = 0.f, t1 = 0.f;
+                    for (int w = 0; w < 8; ++w) { t0 += s_red[0][w][cl]; t1 += s_red[1][w][cl]; }
+                    float* dst = a.stat_partial + (size_t)(tile / NTC) * 2 * a.N;
+                    dst[nt * Nt + cl] = t0;
+                    dst[a.N + nt * Nt + cl] = t1;
+                }
+                unit_bar_sync(1, kDenseConsumers);                         // s_red is rewritten by the next tile
             }
-        }
-    } else {
-        __syncthreads();
-        const bool big = a.pool_k > 128;                             // the whole 128-row tile lies inside one group
-        const int wpg = big ? 8 : a.pool_k / 16;                     // warps per pooling group
-        for (int e = tid; e < (8 / wpg) * Nt; e += kDenseThreads) {
-            const int grp = e / Nt, cl = e % Nt;
-            const long long rs = row0 + grp * wpg * 16;
-            if (rs >= a.rows) continue;
-            float mx = s_red[0][grp * wpg][cl];
-            for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[0][grp * wpg + w][cl]);
-            const long long wg = rs / a.pool_k;
-            if (!big) {
-                a.out[(size_t)wg * a.N + nt * Nt + cl] = mx;
-            } else {
-                int code = __float_as_int(mx);
-                code = code >= 0 ? code : code ^ 0x7fffffff;
-                atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + nt * Nt + cl, code);
+        } else {
+            unit_bar_sync(1, kDenseConsumers);
+            const bool big = a.pool_k > 128;                             // the whole 128-row tile lies inside one group
+            const int wpg = big ? 8 : a.pool_k / 16;                     // warps per pooling group
+            for (int e = tid; e < (8 / wpg) * Nt; e += kDenseConsumers) {
+                const int grp = e / Nt, cl = e % Nt;
+                const long long rs = row0 + grp * wpg * 16;
+                if (rs >= a.rows) continue;
+                float mx = s_red[0][grp * wpg][cl];
+                for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[0][grp * wpg + w][cl]);
+                const long long wg = rs / a.pool_k;
+                if (!big) {
+                    a.out[(size_t)wg * a.N + nt * Nt + cl] = mx;
+                } else {
+                    int code = __float_as_int(mx);
+                    code = code >= 0 ? code : code ^ 0x7fffffff;
+                    atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + nt * Nt + cl, code);
+                }
             }
+            unit_bar_sync(1, kDenseConsumers);
         }
     }
     if constexpr (NP == 2) {
@@ -872,8 +965,13 @@ size_t tc_dense_image_bytes(int K, int N) { return tc_dense_image_off3(K, N) + t
 // bytes of a prebuilt image of the current split: mode 0 = fp16x2 blocks + their bf16x3 twin, mode 2 = bf16x3 blocks
 static size_t tc_plan_image_bytes(int Kp, int N) { return g_tc_np == 2 ? tc_image_alloc_bytes(Kp, N, 2) + tc_image_alloc_bytes(Kp, N, 3) : tc_image_alloc_bytes(Kp, N, 3); }
 
-// tile width of a dense layer's weight image, with the format flag of the current split
-int tc_dense_nt(int N) { return ((N % 128) == 0 ? 128 : 64) | image_flag(g_tc_np); }
+// tile width of a dense layer (and of its weight image), with the format flag of the current split: 128 when N allows it and
+// 128-wide tiles keep more than half of the SMs busy (one persistent CTA per SM), else 64.  Narrow tiles read x once per 64
+// channels instead of once per 128: measured on SA3 (H100), 64-wide won for 64 tiles of 128 (layer 0) and lost for 128 (layer 1).
+int tc_dense_nt(long long rows, int N) {
+    const bool wide = (N % 128) == 0 && 2 * ((rows + 127) / 128 * (N / 128)) > kNumSMs;
+    return (wide ? 128 : 64) | image_flag(g_tc_np);
+}
 
 // builds the image of W (K x N, rows K..Kp zero) in the format `Nt` carries (width | format flag); zeroes the trailer first
 static int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* image, cudaStream_t st, const unsigned int* run_if = nullptr) {
@@ -891,38 +989,49 @@ static const unsigned int* image_trailer(const uint8_t* image, int Kp, int N, in
     return reinterpret_cast<const unsigned int*>(image + ((tc_image_bytes(Kp, N, np) + 255) & ~(size_t)255));
 }
 
+template <int NP, int NC>
+static int launch_tc_dense_shape(const TcDenseArgs& a, cudaStream_t st) {
+    const size_t smem = (size_t)dense_stages(NP, NC) * dense_stage_bytes(NP, NC) + 1024;
+    PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // persistent CTAs: as many as are resident at once, never more than there are tiles
+    int dev = 0, sms = 0, per_sm = 0;
+    PSA_CUDA(cudaGetDevice(&dev));
+    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PSA_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_dense_kernel<NP, NC>, kDenseThreads, smem));
+    const long long tiles = (a.rows + 127) / 128 * (a.N / (64 * NC)), resident = (long long)sms * (per_sm > 0 ? per_sm : 1);
+    tc_dense_kernel<NP, NC><<<(unsigned)(tiles < resident ? tiles : resident), kDenseThreads, smem, st>>>(a);
+    return check_launch("tc_dense_kernel");
+}
+
 // one launch of a dense layer with NP pieces; `image` holds the weights in that format
 template <int NP>
 static int launch_tc_dense_np(TcDenseArgs& a, int Nt, cudaStream_t st) {
-    const dim3 grid((unsigned)((a.rows + 127) / 128), a.N / Nt);
     const bool big = a.pool_k > 128;
     if (big) { int rc0 = launch_fill_ord_neg_inf(a.rows / a.pool_k * a.N, a.out, st, a.run_if); if (rc0 != PSA_OK) return rc0; }
-    const size_t smem = kDenseStages * (size_t)tc_block_bytes(Nt, NP) + 1024;
-    if (Nt == 128) {
-        PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tc_dense_kernel<NP, 2><<<grid, kDenseThreads, smem, st>>>(a);
-    } else {
-        PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        tc_dense_kernel<NP, 1><<<grid, kDenseThreads, smem, st>>>(a);
-    }
-    int rc = check_launch("tc_dense_kernel");
+    const int rc = Nt == 128 ? launch_tc_dense_shape<NP, 2>(a, st) : launch_tc_dense_shape<NP, 1>(a, st);
     if (rc != PSA_OK) return rc;
     if (big) return launch_decode_ord(a.rows / a.pool_k * a.N, a.out, st, a.run_if);
     return PSA_OK;
 }
 
+// the zeroed 256-byte word region of psa_shared_mlp / psa_sa_group_all_infer: range flag of layer l at [l], the tile counters
+// of layer l and of its rerun at [kTileCounterWords + 2 l, + 1]
+constexpr int kTileCounterWords = PSA_MAX_MLP_LAYERS;
+
 // out = relu?((x . W [+ xyz3 . w3]) * scale + shift) on the tensor cores, optional max over runs of pool_k rows.
 //   prebuilt : image of W in the CURRENT split's format (psa_prepare_weight_image), or null
 //   ws_img   : tc_dense_image_bytes(K, N) of scratch (missing images are built here)
 //   flag     : one zeroed device word (np = 2: raised when a value left the fp16 range; the bf16x3 rerun is conditional on it)
+//   counters : two zeroed device words, the tile counters of the launch and of its rerun
 int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const float* x, const float* W, const float* scale,
-                    const float* shift, float* out, const uint8_t* prebuilt, uint8_t* ws_img, unsigned int* flag, cudaStream_t st,
-                    const float* xyz3 = nullptr, const float* w3 = nullptr) {
+                    const float* shift, float* out, const uint8_t* prebuilt, uint8_t* ws_img, unsigned int* flag, unsigned int* counters,
+                    cudaStream_t st, const float* xyz3 = nullptr, const float* w3 = nullptr) {
     const int Kp = (K + 63) & ~63;
-    const int Nt = (N % 128) == 0 ? 128 : 64;
+    const int Nt = tc_dense_nt(rows, N) & ~kImageFlags;
     TcDenseArgs a;
     a.rows = rows; a.K = K; a.Kp = Kp; a.N = N; a.pool_k = pool_k; a.relu = relu;
     a.x = x; a.scale = scale; a.shift = shift; a.out = out; a.xyz3 = xyz3; a.w3 = w3;
+    a.tile_counter = counters;
     uint8_t* img3 = ws_img + tc_dense_image_off3(K, N);
     int rc;
     if (g_tc_np == 3) {
@@ -943,16 +1052,16 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
         rc = build_image(K, Kp, N, Nt | kImageBf16x3, W, img3, st, flag);
         if (rc != PSA_OK) return rc;
     }
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.run_if = flag;
+    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.run_if = flag; a.tile_counter = counters + 1;
     return launch_tc_dense_np<3>(a, Nt, st);
 }
 
 // Training-mode forward of one layer on tc_dense_kernel: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
 // statistics.  The weights change every step, so the image is rebuilt into `image_ws` (tc_dense_image_bytes(K, N)) per call.
-// bf16x3 only: batch-statistics activations are not range-checked.
+// bf16x3 only: batch-statistics activations are not range-checked.  No zeroed word comes with the call: the tiles are taken in
+// a static order.
 bool tc_train_fwd_eligible(long long rows, int K, int N) {
-    // one CTA per 128-row tile with a fixed prologue / epilogue: pays off from two K blocks up (K = 64 layers stay on the fp32
-    // FMA kernel)
+    // pays off from two K blocks up (K = 64 layers stay on the fp32 FMA kernel)
     return rows >= 128 && K >= 128 && K <= 512 && N >= 128 && (N % 128) == 0;
 }
 int launch_tc_dense_train(long long rows, int K, int N, const float* x, const float* in_scale, const float* in_shift, int in_relu,
@@ -1067,7 +1176,7 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     int rc = PSA_OK;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     unsigned int* words = reinterpret_cast<unsigned int*>(ws);     // [0] tile counter, [1] tile counter of the rerun, [2] range flag of
-    PSA_CUDA(cudaMemsetAsync(ws, 0, 256, st));                     // the level, [3] range flag of the U GEMM
+    PSA_CUDA(cudaMemsetAsync(ws, 0, 256, st));                     // the level, [3] range flag of the U GEMM, [4, 5] its tile counters
     ws += 256;
     uint8_t* img2[kMaxTcLayers];
     uint8_t* img3[kMaxTcLayers];
@@ -1082,8 +1191,8 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
         uint8_t* uimg = ws + (((size_t)b * n * a.C1 * sizeof(float) + 255) & ~(size_t)255);
         const float* w1f = mlp->weight[0] + (size_t)3 * a.C1;
         if (tc_dense_eligible((long long)b * n, c, a.C1, 1)) {
-            rc = launch_tc_dense((long long)b * n, c, a.C1, 1, 0, points, w1f, nullptr, nullptr, ufw, prebuilt_image(mlp, 0, 3, tc_dense_nt(a.C1)), uimg,
-                                 words + 3, st);
+            rc = launch_tc_dense((long long)b * n, c, a.C1, 1, 0, points, w1f, nullptr, nullptr, ufw, prebuilt_image(mlp, 0, 3, tc_dense_nt((long long)b * n, a.C1)),
+                                 uimg, words + 3, words + 4, st);
         } else {
             DenseArgs d;
             d.rows = (long long)b * n; d.K = c; d.N = a.C1; d.pool_k = 1; d.relu = 0;
@@ -1196,7 +1305,7 @@ extern "C" size_t psa_shared_mlp_workspace_bytes(long long rows, const psa_mlp* 
         for (int l = 0; l < mlp->n_layers; ++l) { size_t f = fc_small_workspace_bytes(mlp->channels[l], mlp->channels[l + 1]); fc = f > fc ? f : fc; }
         bytes += (fc + 255) & ~(size_t)255;
     }
-    return bytes + 256;       // range flags of the tensor-core layers (one word per layer), last
+    return bytes + 256;       // range flags of the tensor-core layers (one word per layer) and their tile counters, last
 }
 
 extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const psa_mlp* mlp, float* out,
@@ -1233,8 +1342,8 @@ extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const 
         const int pk = (l == L - 1) ? pool_k : 1;
         float* dst = (l == L - 1) ? out : ((l & 1) ? ws1 : ws0);
         if (g_mlp_mode != 1 && tc_dense_eligible(rows, K, N, pk)) {
-            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, mlp->weight[l], mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, 0, tc_dense_nt(N)),
-                                 img, flags + l, st);
+            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, mlp->weight[l], mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, 0, tc_dense_nt(rows, N)),
+                                 img, flags + l, flags + kTileCounterWords + 2 * l, st);
         } else {
             DenseArgs d;
             d.rows = rows; d.K = K; d.N = N; d.pool_k = pk; d.relu = mlp->relu[l];
@@ -1292,8 +1401,8 @@ extern "C" int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, con
         float* dst = (l == L - 1) ? out : ((l & 1) ? ws1 : ws0);
         const float* W = (l == 0) ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l];
         if (tc_dense_eligible(rows, K, N, pk)) {
-            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, W, mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, l == 0 ? 3 : 0, tc_dense_nt(N)),
-                                 img, flags + l, st, l == 0 ? xyz : nullptr, l == 0 ? mlp->weight[0] : nullptr);
+            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, W, mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, l == 0 ? 3 : 0, tc_dense_nt(rows, N)),
+                                 img, flags + l, flags + kTileCounterWords + 2 * l, st, l == 0 ? xyz : nullptr, l == 0 ? mlp->weight[0] : nullptr);
         } else {
             PSA_SUPPORTED(l > 0, "sa_group_all: layer 0 must run on the tensor-core path");
             DenseArgs d;
@@ -1434,7 +1543,7 @@ extern "C" int psa_edgeconv_infer(int b, int n, int c, int k, const float* x, co
     if (tc_dense_eligible(rows, c, 2 * N, 1)) {
         unsigned int* flag = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(workspace) + need - 256);
         PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
-        rc = launch_tc_dense(rows, c, 2 * N, 1, 0, x, Wc, nullptr, nullptr, AB, nullptr, ws, flag, st);
+        rc = launch_tc_dense(rows, c, 2 * N, 1, 0, x, Wc, nullptr, nullptr, AB, nullptr, ws, flag, flag + 1, st);
     } else {
         DenseArgs d;
         d.rows = rows; d.K = c; d.N = 2 * N; d.pool_k = 1; d.relu = 0;
@@ -1475,14 +1584,14 @@ extern "C" int psa_mlp_image_plan(int usage, long long rows, int pool_k, int c, 
             const int r0 = (usage == PSA_USAGE_SA_GROUP_ALL && l == 0) ? 3 : 0;
             const int K = mlp->channels[l] - r0, N = mlp->channels[l + 1];
             const int pk = (l == L - 1) ? pool_k : 1;
-            if (K >= 1 && tc_dense_eligible(rows, K, N, pk)) { nt[l] = tc_dense_nt(N); row0[l] = r0; bytes[l] = tc_plan_image_bytes((K + 63) & ~63, N); }
+            if (K >= 1 && tc_dense_eligible(rows, K, N, pk)) { nt[l] = tc_dense_nt(rows, N); row0[l] = r0; bytes[l] = tc_plan_image_bytes((K + 63) & ~63, N); }
         }
         return PSA_OK;
     }
     PSA_REQUIRE(usage == PSA_USAGE_SA_MODULE, "mlp_image_plan: unknown usage %d", usage);
     TcArgs a;
     if (!tc_sa_eligible(mlp, c, nsample, &a)) return PSA_OK;
-    if (c > 0 && tc_dense_eligible(rows, c, a.C1, 1)) { nt[0] = tc_dense_nt(a.C1); row0[0] = 3; bytes[0] = tc_plan_image_bytes((c + 63) & ~63, a.C1); }
+    if (c > 0 && tc_dense_eligible(rows, c, a.C1, 1)) { nt[0] = tc_dense_nt(rows, a.C1); row0[0] = 3; bytes[0] = tc_plan_image_bytes((c + 63) & ~63, a.C1); }
     for (int l = 0; l < a.nl; ++l) { nt[1 + l] = tc_sa_image_nt(); row0[1 + l] = 0; bytes[1 + l] = tc_plan_image_bytes(a.Kd[l], a.Ntot[l]); }
     return PSA_OK;
 }
