@@ -395,6 +395,34 @@ PSA_API int psa_sa_conv1_bwd(int b, int n, int m, int nsample, int C1, const flo
                              const int* idx, const psa_grad_in* g, float* dW_xyz, float* dU, void* workspace,
                              size_t workspace_bytes, psa_stream_t stream);
 
+/* Training-mode single-layer EdgeConv (dgcnn/models/dgcnn.py:41-47, dgcnn/utils/tf_util.py:115-173,462-499):
+ *   out_ic = max_j relu(BN(y_ij)),  y_ij = [x_i, x_j - x_i] . W + bias,  BN with the batch statistics of all b*n*k edges.
+ * Replaces get_edge_feature (tf_util.py:674-706) + conv2d + batch_norm(is_training=True) + relu + reduce_max and their gradients
+ * without any (b,n,k,.) tensor: with Q = x (W_a - W_b) + bias and P = x W_b (W_a = rows 0..c of W, W_b = rows c..2c), every
+ * edge value is y_ij = Q_i + P_nn(i,j), recomputed from the (b*n, 2 C_out) buffer PQ = [Q | P] in every pass.  x (b,n,c),
+ * nn_idx (b,n,k) int32 with within-cloud indices in [0, n), W (2c, C_out), bias (C_out) or NULL.  C_out a multiple of 32,
+ * at most 256 (else PSA_ERR_UNSUPPORTED); any c >= 1, k >= 1; the backward takes n <= 51200.  One workspace serves the three
+ * calls: psa_edgeconv_train_workspace_bytes() bytes, 256-byte aligned.  Every reduction runs in a fixed order: bit-reproducible.
+ *
+ * forward 1: PQ (b*n, 2 C_out) and stats (2, C_out) = per-channel [sum y, sum y^2] over the edges; then psa_bn_finalize with
+ *            count = b*n*k gives scale, shift, mean_inv and updates the moving averages. */
+PSA_API size_t psa_edgeconv_train_workspace_bytes(int b, int n, int c, int k, int C_out);
+PSA_API int psa_edgeconv_train_fwd(int b, int n, int c, int k, int C_out, const float* x, const int* nn_idx, const float* W,
+                                   const float* bias, float* PQ, float* stats, void* workspace, size_t workspace_bytes,
+                                   psa_stream_t stream);
+/* forward 2: pooled (b*n, C_out) = max_j relu(y_ij * scale + shift) and ties (b*n, C_out) = how many edges reach that maximum
+ * bit for bit -- uint8 when k <= 255, int32 otherwise. */
+PSA_API int psa_edgeconv_train_pool(int b, int n, int k, int C_out, const int* nn_idx, const float* PQ, const float* scale,
+                                    const float* shift, float* pooled, void* ties, psa_stream_t stream);
+/* backward: dout (b*n, C_out) = gradient of pooled, split evenly among the tied edges of a positive maximum (torch.amax / TF
+ * reduce_max) -> dW (2c, C_out), dgamma, dbeta (C_out), dx (b*n, c).  The conv bias under batch norm has an exactly zero
+ * gradient (not written).  The kNN graph carries no gradient.  scale, shift, gamma, mean_inv as the forward used them. */
+PSA_API int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, const float* x, const int* nn_idx, const float* W,
+                                   const float* PQ, const float* scale, const float* shift, const float* gamma,
+                                   const float* mean_inv, const float* pooled, const void* ties, const float* dout, float* dW,
+                                   float* dgamma, float* dbeta, float* dx, void* workspace, size_t workspace_bytes,
+                                   psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

@@ -19,6 +19,13 @@ void set_error(const char* fmt, ...);
 // scatter.cu: stable counting sort of a cloud's (entry -> destination) pairs; offsets (b, n+1), list (b, mk)
 int launch_group_csr(int b, int n, int mk, const int* idx, int* offsets, int* list, cudaStream_t st);
 
+// train.cu: out[e] = sum_p partial[p * len + e] in a fixed order (fp64)
+int reduce_partials(int nparts, int len, const float* partial, float* out, cudaStream_t st);
+// train.cu: batch-norm backward from (nparts, 2, C) partials [sum dz | sum dz * xhat] over `rows` rows -> dgamma, dbeta and the
+// coefficients of dy = ca * dz + cb * y + cc (psa_bn_bwd_coeffs)
+int launch_bn_bwd_final(int nparts, int C, long long rows, const float* partial, const float* gamma, const float* mean_inv, float* dgamma,
+                        float* dbeta, float* ca, float* cb, float* cc, cudaStream_t st);
+
 inline int check_launch(const char* what) {
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) {

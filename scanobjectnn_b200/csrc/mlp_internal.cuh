@@ -29,3 +29,6 @@ int launch_fill_ord_neg_inf(long long total, float* out, cudaStream_t st, const 
 int launch_decode_ord(long long total, float* out, cudaStream_t st, const unsigned int* run_if = nullptr);         // int codes -> floats, in place
 
 }  // namespace psa
+
+// tc_mlp.cu: W (2c, N) of a single-layer EdgeConv -> Wc (c, 2N) = [W_a - W_b | W_b] (grid-stride over the c * 2N entries)
+__global__ void edge_wc_kernel(int c, int N, const float* __restrict__ W, float* __restrict__ Wc);

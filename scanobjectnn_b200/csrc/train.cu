@@ -48,7 +48,7 @@ __global__ void __launch_bounds__(1024) reduce_partials_kernel(int nparts, int l
     }
 }
 
-static int reduce_partials(int nparts, int len, const float* partial, float* out, cudaStream_t st) {
+int reduce_partials(int nparts, int len, const float* partial, float* out, cudaStream_t st) {
     reduce_partials_kernel<<<(len + 31) / 32, 1024, 0, st>>>(nparts, len, partial, out);
     return check_launch("reduce_partials_kernel");
 }
@@ -251,6 +251,12 @@ bn_bwd_final_kernel(int nparts, int C, double inv_rows, const float* __restrict_
     ca[c] = (float)(gm * inv);
     cb[c] = (float)(-gm * inv * inv * dg * inv_rows);
     cc[c] = (float)(gm * inv * (mu * inv * dg - db) * inv_rows);
+}
+
+int launch_bn_bwd_final(int nparts, int C, long long rows, const float* partial, const float* gamma, const float* mean_inv, float* dgamma,
+                        float* dbeta, float* ca, float* cb, float* cc, cudaStream_t st) {
+    bn_bwd_final_kernel<<<(C + 31) / 32, 1024, 0, st>>>(nparts, C, 1.0 / (double)rows, partial, gamma, mean_inv, dgamma, dbeta, ca, cb, cc);
+    return check_launch("bn_bwd_final_kernel");
 }
 
 // ---- first-layer backward of a set-abstraction level ----
@@ -584,8 +590,7 @@ extern "C" int psa_bn_bwd_coeffs(long long rows, int C, const psa_grad_in* g, co
     bn_bwd_partial_kernel<<<(unsigned)blocks, kBnbThreads, 0, st>>>(gi, units, C, mean_inv, upb, partial);
     int rc = check_launch("bn_bwd_partial_kernel");
     if (rc != PSA_OK) return rc;
-    bn_bwd_final_kernel<<<(C + 31) / 32, 1024, 0, st>>>((int)blocks, C, 1.0 / (double)rows, partial, gamma, mean_inv, dgamma, dbeta, ca, cb, cc);
-    return check_launch("bn_bwd_final_kernel");
+    return launch_bn_bwd_final((int)blocks, C, rows, partial, gamma, mean_inv, dgamma, dbeta, ca, cb, cc, st);
 }
 
 static size_t conv1_bwd_partial_bytes(int C1) { return ((size_t)kBnbMaxBlocks * 3 * C1 * sizeof(float) + 255) & ~(size_t)255; }

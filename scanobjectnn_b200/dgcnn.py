@@ -75,13 +75,16 @@ def _backbone(point_cloud, params, end_points, k=K_NEIGHBORS):
 
 def _edge_conv_training(x, k, layers, bn_decay, params, idx=None):
     """pairwise_distance -> knn -> get_edge_feature -> conv2d(+BN+ReLU)... -> reduce_max over k (dgcnn.py:31-44) in training mode.
-    The neighbour graph carries no gradient; the edge tensor [x_i, x_j - x_i] is built from the differentiable group_point
-    (GroupPointGrad) and torch glue, the convolutions run as mlp_training (batch statistics over all B*N*k edges)."""
-    from .training import mlp_training
+    The neighbour graph carries no gradient; batch statistics over all B*N*k edges.  A single layer (dgcnn1..4) runs as the fused
+    edgeconv_training (no per-edge tensor); deeper stacks (the T-net's, C = 3) build the edge tensor [x_i, x_j - x_i] from the
+    differentiable group_point (GroupPointGrad) and torch glue and run the convolutions as mlp_training."""
+    from .training import edgeconv_training, mlp_training
     b, n, c = x.shape
     if idx is None:
         with torch.no_grad():
             idx = ops.knn_graph(x.detach().contiguous(), k)
+    if len(layers) == 1:
+        return edgeconv_training(x, idx, layers[0][0], bn_decay, params), idx
     neigh = ops.group_point(x.contiguous(), idx)                               # (B,N,k,C), differentiable in x
     centre = x.unsqueeze(2).expand(b, n, k, c)
     edge = torch.cat([centre, neigh - centre], dim=-1)                         # get_edge_feature, dgcnn/utils/tf_util.py:674-706

@@ -320,6 +320,84 @@ def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore) -> to
     return out.view(*shape[:-1], out.shape[-1])
 
 
+class EdgeConvTrainer(_TrainOps):
+    """Training-mode single-layer EdgeConv (dgcnn.py:41-47: get_edge_feature -> conv2d + batch norm + ReLU -> reduce_max over k) on
+    the fused kernels of csrc/edgeconv_train.cu: one product over the b*n points and gather passes; no (B,N,k,.) tensor is stored.
+    Batch statistics over all b*n*k edges; the max's gradient is split evenly among tied edges, as torch.amax / TF reduce_max do."""
+
+    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scope: str, device=None):
+        self.lib = _lib.load()
+        self.params = params
+        self.dev = torch.device(device) if device is not None else params.device
+        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
+        params._flat = self.fp
+        self.b, self.n, self.c, self.k = b, n, c, k
+        self.layer = ly = _Layer(self.fp, scope, 0, True, self.dev)       # rows = 0: the per-edge activations are never stored
+        if ly.K != 2 * c:
+            raise ValueError(f"{scope}: weights of shape {tuple(ly.W.shape)}, an EdgeConv over {c} channels needs ({2 * c}, C_out)")
+        rows, N = b * n, ly.N
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        self.PQ = torch.empty((rows, 2 * N), **f32)
+        self.pooled = torch.empty((rows, N), **f32)
+        self.ties = torch.empty((rows, N), dtype=torch.uint8 if k <= 255 else torch.int32, device=self.dev)
+        self.d_in = torch.empty((rows, c), **f32)
+        self.ws_bytes = self.lib.psa_edgeconv_train_workspace_bytes(b, n, c, k, N)
+        if self.ws_bytes == 0:
+            raise _lib.PsaError(f"{scope}: EdgeConv training needs C_out a multiple of 32, at most 256 (got {N})")
+        self.ws = torch.empty(self.ws_bytes // 4 + 64, **f32)
+
+    def forward(self, x: torch.Tensor, nn_idx: torch.Tensor, bn_decay: float = 0.5) -> torch.Tensor:
+        b, n, c, k, ly = self.b, self.n, self.c, self.k, self.layer
+        assert x.shape == (b, n, c) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+        assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
+        self.x, self.nn_idx = x, nn_idx
+        self._c(self.lib.psa_edgeconv_train_fwd(b, n, c, k, ly.N, _p(x), _p(nn_idx), _p(ly.W), _p(ly.b), _p(self.PQ), _p(ly.stats), _p(self.ws),
+                                                C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_fwd")
+        self._bn_finalize(ly, b * n * k, bn_decay)
+        self._c(self.lib.psa_edgeconv_train_pool(b, n, k, ly.N, _p(nn_idx), _p(self.PQ), _p(ly.scale), _p(ly.shift), _p(self.pooled), _p(self.ties),
+                                                 _stream()), "edgeconv_train_pool")
+        return self.pooled
+
+    def backward(self, dout: torch.Tensor) -> torch.Tensor:
+        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); the layer's gradients go to the flat bucket"""
+        b, n, c, k, ly = self.b, self.n, self.c, self.k, self.layer
+        dout = dout.contiguous()
+        self._c(self.lib.psa_edgeconv_train_bwd(b, n, c, k, ly.N, _p(self.x), _p(self.nn_idx), _p(ly.W), _p(self.PQ), _p(ly.scale), _p(ly.shift),
+                                                _p(ly.gamma), _p(ly.mean_inv), _p(self.pooled), _p(self.ties), _p(dout), _p(ly.dW), _p(ly.dgamma),
+                                                _p(ly.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_bwd")
+        ly.db.zero_()          # sum over the edges of dy = 0 under batch norm
+        return self.d_in
+
+
+class _EdgeConvFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, flat, x, nn_idx, trainer, bn_decay):
+        ctx.trainer = trainer
+        return trainer.forward(x, nn_idx, bn_decay).clone()
+
+    @staticmethod
+    def backward(ctx, dout):
+        tr = ctx.trainer
+        dx = tr.backward(dout)
+        return _flat_grad_of_layers(tr.fp, [tr.layer]), dx.view(tr.b, tr.n, tr.c).clone(), None, None, None
+
+
+def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope: str, bn_decay, params: VariableStore) -> torch.Tensor:
+    """Training-mode single-layer EdgeConv with autograd: x (B, N, C), nn_idx (B, N, k) int32 -> (B, N, C_out) =
+    max_j relu(BN([x_i, x_j - x_i] . W + b)), BN over all B*N*k edges.  The graph carries no gradient.  Buffers are cached on
+    `params` per (scope, shape); the variables' gradients land in the flat bucket."""
+    b, n, c = x.shape
+    k = nn_idx.shape[-1]
+    key = ("edgeconv", scope, b, n, c, k)
+    cache = params.__dict__.setdefault("_trainers", {})
+    if key not in cache:
+        cache[key] = EdgeConvTrainer(params, b, n, c, k, scope, device=x.device)
+    tr = cache[key]
+    tr.fp.flat.requires_grad_(True)
+    out = _EdgeConvFn.apply(tr.fp.flat, x.contiguous(), nn_idx.to(torch.int32).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
+    return out.view(b, n, -1)
+
+
 class PointNet2ClsTrainer(_TrainOps):
     """Training engine of pointnet2_cls_ssg (or any stack of LevelSpec + FC head with the same structure)."""
 
