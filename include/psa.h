@@ -423,6 +423,36 @@ PSA_API int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, const 
                                    float* dgamma, float* dbeta, float* dx, void* workspace, size_t workspace_bytes,
                                    psa_stream_t stream);
 
+/* Training mode of a two-layer EdgeConv (DGCNN's input transform net, transform_nets.py:18-27): out_ic = max_j relu(BN2(relu(BN1(
+ * [x_i, x_j - x_i] . W1 + b1)) . W2 + b2)), both batch norms with batch statistics over all E = b*n*k edges.  No per-edge tensor
+ * is stored in the forward; the backward keeps one, the (E, C1) gradient of layer 1.  Layer 1 is the single-layer op above:
+ * psa_edgeconv_train_fwd with C_out = C1 gives PQ (b*n, 2 C1) and its statistics, psa_bn_finalize(C1, E, ...) its affine.  C1 = 64,
+ * C2 = 128 and k <= 32 (else PSA_ERR_UNSUPPORTED); any c >= 1; the backward takes n <= 51200.  One workspace of
+ * psa_edgeconv2_train_workspace_bytes() bytes, 256-byte aligned, serves all calls including the layer-1 forward.  The per-edge
+ * products run on the tensor cores (three bf16 pieces per operand); every reduction runs in a fixed order: bit-reproducible.
+ *
+ * forward: stats2 (2, C2) = per-channel [sum y2, sum y2^2] over the edges; then psa_bn_finalize(C2, E, ...). */
+PSA_API size_t psa_edgeconv2_train_workspace_bytes(int b, int n, int c, int k, int C1, int C2);
+PSA_API int psa_edgeconv2_train_fwd(int b, int n, int c, int k, int C1, int C2, const int* nn_idx, const float* PQ,
+                                    const float* scale1, const float* shift1, const float* W2, const float* bias2, float* stats2,
+                                    void* workspace, size_t workspace_bytes, psa_stream_t stream);
+/* pool: pooled (b*n, C2) = max_j relu(y2_ij * scale2 + shift2); mask (b*n, C2) = bit j set for every edge that reaches the
+ * maximum bit for bit; ywin (b*n, C2) = y2 of the first of them (pre batch norm). */
+PSA_API int psa_edgeconv2_train_pool(int b, int n, int c, int k, int C1, int C2, const int* nn_idx, const float* PQ,
+                                     const float* scale1, const float* shift1, const float* W2, const float* bias2,
+                                     const float* scale2, const float* shift2, float* pooled, unsigned int* mask, float* ywin,
+                                     void* workspace, size_t workspace_bytes, psa_stream_t stream);
+/* backward: dout (b*n, C2) = gradient of pooled, split evenly among the masked edges of a positive maximum -> dW1 (2c, C1),
+ * dgamma1, dbeta1 (C1), dW2 (C1, C2), dgamma2, dbeta2 (C2), dx (b*n, c).  Both conv biases have exactly zero gradient under
+ * batch norm (not written); the kNN graph carries no gradient. */
+PSA_API int psa_edgeconv2_train_bwd(int b, int n, int c, int k, int C1, int C2, const float* x, const int* nn_idx,
+                                    const float* W1, const float* PQ, const float* scale1, const float* shift1,
+                                    const float* gamma1, const float* mean_inv1, const float* W2, const float* bias2,
+                                    const float* gamma2, const float* mean_inv2, const float* pooled, const unsigned int* mask,
+                                    const float* ywin, const float* dout, float* dW1, float* dgamma1, float* dbeta1, float* dW2,
+                                    float* dgamma2, float* dbeta2, float* dx, void* workspace, size_t workspace_bytes,
+                                    psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

@@ -187,12 +187,20 @@ edge_train_bn_sums_kernel(long long points, int n, int k, int N, const float* __
     }
 }
 
+// dz of edge (i, j): read from DZ (b*n*k, N) when given (a layer under another layer), else the max's gradient routed to the edges
+// whose activation equals the pooled maximum (R = 0 where the maximum is not positive)
+template <int VEC>
+__device__ __forceinline__ float edge_dz(const float* __restrict__ DZ, size_t edge, int N, int c0, int v, float y, const float (&sc)[VEC],
+                                         const float (&sh)[VEC], const float (&mx)[VEC], const float (&r)[VEC]) {
+    return DZ != nullptr ? __ldg(DZ + edge * N + c0 + v) : (edge_act(y, sc[v], sh[v]) == mx[v] ? r[v] : 0.f);
+}
+
 // backward pass 2: G[p][0:N] = dQ_p = sum_j dy_pj in j order
 template <int VEC>
 __global__ void __launch_bounds__(kEdgeWarps * 32)
 edge_train_dq_kernel(long long points, int n, int k, int N, const float* __restrict__ PQ, const int* __restrict__ nn_idx,
                      const float* __restrict__ scale, const float* __restrict__ shift, const float* __restrict__ coef,
-                     const float* __restrict__ pooled, const float* __restrict__ R, float* __restrict__ G) {
+                     const float* __restrict__ pooled, const float* __restrict__ R, const float* __restrict__ DZ, float* __restrict__ G) {
     const int lane = threadIdx.x & 31, c0 = lane * VEC;
     float sc[VEC], sh[VEC], ca[VEC], cb[VEC], cc[VEC];
     load_vec<VEC>(sc, scale + c0);
@@ -205,19 +213,23 @@ edge_train_dq_kernel(long long points, int n, int k, int N, const float* __restr
         const size_t o = (size_t)p * N + c0;
         float a[VEC], mx[VEC], r[VEC], acc[VEC];
         load_vec<VEC>(a, PQ + (size_t)p * 2 * N + c0);
-        load_vec<VEC>(mx, pooled + o);
-        load_vec<VEC>(r, R + o);
+        if (DZ == nullptr) {
+            load_vec<VEC>(mx, pooled + o);
+            load_vec<VEC>(r, R + o);
+        }
 #pragma unroll
         for (int v = 0; v < VEC; ++v) acc[v] = 0.f;
+        size_t edge = (size_t)p * k;
         for_each_neighbour(nn_idx + (size_t)p * k, k, lane, [&](int nb) {
             float bv[VEC];
             load_vec<VEC>(bv, PQ + (size_t)(base + nb) * 2 * N + N + c0);
 #pragma unroll
             for (int v = 0; v < VEC; ++v) {
                 const float y = __fadd_rn(a[v], bv[v]);
-                const float dz = edge_act(y, sc[v], sh[v]) == mx[v] ? r[v] : 0.f;       // r = 0 where the maximum is not positive
+                const float dz = edge_dz<VEC>(DZ, edge, N, c0, v, y, sc, sh, mx, r);
                 acc[v] += fmaf(ca[v], dz, fmaf(cb[v], y, cc[v]));
             }
+            ++edge;
         });
 #pragma unroll
         for (int v = 0; v < VEC; ++v) G[(size_t)p * 2 * N + c0 + v] = acc[v];
@@ -229,7 +241,8 @@ template <int VEC>
 __global__ void __launch_bounds__(kEdgeWarps * 32)
 edge_train_dp_kernel(long long points, int n, int k, int N, const float* __restrict__ PQ, const float* __restrict__ scale,
                      const float* __restrict__ shift, const float* __restrict__ coef, const float* __restrict__ pooled,
-                     const float* __restrict__ R, const int* __restrict__ offsets, const int* __restrict__ list, float* __restrict__ G) {
+                     const float* __restrict__ R, const float* __restrict__ DZ, const int* __restrict__ offsets, const int* __restrict__ list,
+                     float* __restrict__ G) {
     const int lane = threadIdx.x & 31, c0 = lane * VEC;
     float sc[VEC], sh[VEC], ca[VEC], cb[VEC], cc[VEC];
     load_vec<VEC>(sc, scale + c0);
@@ -252,16 +265,19 @@ edge_train_dp_kernel(long long points, int n, int k, int N, const float* __restr
             const int cnt = min(32, t1 - e0);
             const int mine = lane < cnt ? __ldg(lst + e0 + lane) : 0;
             for (int jj = 0; jj < cnt; ++jj) {
-                const long long i = cloud * n + __shfl_sync(0xffffffffu, mine, jj) / k;         // entry = i_local * k + j
-                const size_t o = (size_t)i * N + c0;
+                const int entry = __shfl_sync(0xffffffffu, mine, jj);                         // entry = i_local * k + j
+                const long long i = cloud * n + entry / k;
+                const size_t o = (size_t)i * N + c0, edge = (size_t)(cloud * nk + entry);
                 float a[VEC], mx[VEC], r[VEC];
                 load_vec<VEC>(a, PQ + (size_t)i * 2 * N + c0);
-                load_vec<VEC>(mx, pooled + o);
-                load_vec<VEC>(r, R + o);
+                if (DZ == nullptr) {
+                    load_vec<VEC>(mx, pooled + o);
+                    load_vec<VEC>(r, R + o);
+                }
 #pragma unroll
                 for (int v = 0; v < VEC; ++v) {
                     const float y = __fadd_rn(a[v], bp[v]);
-                    const float dz = edge_act(y, sc[v], sh[v]) == mx[v] ? r[v] : 0.f;
+                    const float dz = edge_dz<VEC>(DZ, edge, N, c0, v, y, sc, sh, mx, r);
                     acc[v] += fmaf(ca[v], dz, fmaf(cb[v], y, cc[v]));
                 }
             }
@@ -289,19 +305,28 @@ struct FwdLayout {
         total = dense + al256(psa_train_dense_workspace_bytes(rows, c, 2 * N));
     }
 };
-struct BwdLayout {
-    size_t g, r, w2, coef, part, csr, dense, total;
-    BwdLayout(int b, int n, int c, int k, int N) {
+// the tail shared with the two-layer backward (edge_layer_tail): G, the [W_a | W_b] copy, the reverse neighbour lists, the dense products
+struct TailLayout {
+    size_t g, w2, csr, dense, total;
+    TailLayout(int b, int n, int c, int k, int N) {
         const long long rows = (long long)b * n;
         g = 0;
-        r = g + al256((size_t)rows * 2 * N * sizeof(float));
-        w2 = r + al256((size_t)rows * N * sizeof(float));
-        coef = w2 + al256((size_t)c * 2 * N * sizeof(float));
-        part = coef + al256((size_t)3 * N * sizeof(float));
-        csr = part + al256((size_t)edge_tiles(rows) * 2 * N * sizeof(float));
+        w2 = g + al256((size_t)rows * 2 * N * sizeof(float));
+        csr = w2 + al256((size_t)c * 2 * N * sizeof(float));
         dense = csr + al256(((size_t)b * (n + 1) + (size_t)rows * k) * sizeof(int));
         const size_t dw = psa_train_dense_workspace_bytes(rows, c, N), dx = psa_train_dense_workspace_bytes(rows, c, 2 * N);
         total = dense + al256(dw > dx ? dw : dx);
+    }
+};
+struct BwdLayout {
+    size_t r, coef, part, tail, total;
+    BwdLayout(int b, int n, int c, int k, int N) {
+        const long long rows = (long long)b * n;
+        r = 0;
+        coef = r + al256((size_t)rows * N * sizeof(float));
+        part = coef + al256((size_t)3 * N * sizeof(float));
+        tail = part + al256((size_t)edge_tiles(rows) * 2 * N * sizeof(float));
+        total = tail + TailLayout(b, n, c, k, N).total;
     }
 };
 
@@ -340,6 +365,48 @@ using namespace psa;
         case 7: KERNEL<7><<<GRID, kEdgeWarps * 32, SMEM, st>>>(__VA_ARGS__); break;                \
         default: KERNEL<8><<<GRID, kEdgeWarps * 32, SMEM, st>>>(__VA_ARGS__); break;               \
     }
+
+
+size_t psa::edge_tail_workspace_bytes(int b, int n, int c, int k, int N) { return TailLayout(b, n, c, k, N).total; }
+
+// dQ per centre, dP through the reverse neighbour lists, then dW = [x^T dQ ; x^T (dP - dQ)] and dx = [dQ | dP - dQ] . [W_a | W_b]^T
+int psa::edge_layer_tail(int b, int n, int c, int k, int N, const float* x, const int* nn_idx, const float* W, const float* PQ, const float* scale,
+                         const float* shift, const float* coef, const float* pooled, const float* R, const float* dz, float* dW, float* dx,
+                         void* workspace, cudaStream_t st) {
+    const long long rows = (long long)b * n;
+    const TailLayout L(b, n, c, k, N);
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    float* G = reinterpret_cast<float*>(ws + L.g);                  // (rows, 2N) = [dQ | dP - dQ]
+    float* W2 = reinterpret_cast<float*>(ws + L.w2);                // (c, 2N) = [W_a | W_b]
+    int* offsets = reinterpret_cast<int*>(ws + L.csr);
+    int* list = offsets + (size_t)b * (n + 1);
+    void* dense_ws = ws + L.dense;
+    const size_t dense_bytes = L.total - L.dense;
+    psa_stream_t stream = reinterpret_cast<psa_stream_t>(st);
+    PSA_EDGE_DISPATCH(edge_train_dq_kernel, edge_grid(rows), 0, rows, n, k, N, PQ, nn_idx, scale, shift, coef, pooled, R, dz, G);
+    int rc = check_launch("edge_train_dq_kernel");
+    if (rc != PSA_OK) return rc;
+    rc = launch_group_csr(b, n, n * k, nn_idx, offsets, list, st);
+    if (rc != PSA_OK) return rc;
+    PSA_EDGE_DISPATCH(edge_train_dp_kernel, edge_grid(rows), 0, rows, n, k, N, PQ, scale, shift, coef, pooled, R, dz, offsets, list, G);
+    rc = check_launch("edge_train_dp_kernel");
+    if (rc != PSA_OK) return rc;
+    // dW_a = x^T dQ, dW_b = x^T (dP - dQ): straight into the two row blocks of dW (2c, N)
+    psa_act_in in = {};
+    in.x = x; in.ld = c;
+    const psa_grad_in gq = plain_grad(G, 2 * N, N), gd = plain_grad(G + N, 2 * N, N);
+    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gq, dW, dense_ws, dense_bytes, stream);
+    if (rc != PSA_OK) return rc;
+    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gd, dW + (size_t)c * N, dense_ws, dense_bytes, stream);
+    if (rc != PSA_OK) return rc;
+    // dx = [dQ | dP - dQ] . [W_a | W_b]^T: one product over 2N columns
+    PSA_CUDA(cudaMemcpy2DAsync(W2, (size_t)2 * N * sizeof(float), W, (size_t)N * sizeof(float), (size_t)N * sizeof(float), c,
+                               cudaMemcpyDeviceToDevice, st));
+    PSA_CUDA(cudaMemcpy2DAsync(W2 + N, (size_t)2 * N * sizeof(float), W + (size_t)c * N, (size_t)N * sizeof(float), (size_t)N * sizeof(float), c,
+                               cudaMemcpyDeviceToDevice, st));
+    const psa_grad_in gg = plain_grad(G, 2 * N, 2 * N);
+    return psa_train_dense_bwd_input(rows, c, 2 * N, &gg, W2, dx, c, 0, dense_ws, dense_bytes, stream);
+}
 
 extern "C" size_t psa_edgeconv_train_workspace_bytes(int b, int n, int c, int k, int C_out) {
     if (b < 1 || n < 1 || c < 1 || k < 1 || C_out < 1 || C_out % 32 != 0 || C_out > kEdgeMaxN) return 0;
@@ -406,15 +473,9 @@ extern "C" int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, con
     const long long rows = (long long)b * n, tiles = edge_tiles(rows);
     const BwdLayout L(b, n, c, k, N);
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    float* G = reinterpret_cast<float*>(ws + L.g);                  // (rows, 2N) = [dQ | dP - dQ]
     float* R = reinterpret_cast<float*>(ws + L.r);                  // (rows, N) routed gradient of a tied edge
-    float* W2 = reinterpret_cast<float*>(ws + L.w2);                // (c, 2N) = [W_a | W_b]
     float* coef = reinterpret_cast<float*>(ws + L.coef);            // (3, N) = ca, cb, cc
     float* partial = reinterpret_cast<float*>(ws + L.part);
-    int* offsets = reinterpret_cast<int*>(ws + L.csr);
-    int* list = offsets + (size_t)b * (n + 1);
-    void* dense_ws = ws + L.dense;
-    const size_t dense_bytes = L.total - L.dense;
     // batch-norm sums over all b*n*k edges -> dgamma, dbeta, ca, cb, cc
     PSA_EDGE_DISPATCH(edge_train_bn_sums_kernel, tile_grid(tiles), 0, rows, n, k, N, PQ, nn_idx, scale, shift, mean_inv, pooled, ties, dout, tiles,
                       R, partial);
@@ -422,28 +483,5 @@ extern "C" int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, con
     if (rc != PSA_OK) return rc;
     rc = launch_bn_bwd_final((int)tiles, N, rows * k, partial, gamma, mean_inv, dgamma, dbeta, coef, coef + N, coef + 2 * N, st);
     if (rc != PSA_OK) return rc;
-    // dQ per centre, dP through the reverse neighbour lists
-    PSA_EDGE_DISPATCH(edge_train_dq_kernel, edge_grid(rows), 0, rows, n, k, N, PQ, nn_idx, scale, shift, coef, pooled, R, G);
-    rc = check_launch("edge_train_dq_kernel");
-    if (rc != PSA_OK) return rc;
-    rc = launch_group_csr(b, n, n * k, nn_idx, offsets, list, st);
-    if (rc != PSA_OK) return rc;
-    PSA_EDGE_DISPATCH(edge_train_dp_kernel, edge_grid(rows), 0, rows, n, k, N, PQ, scale, shift, coef, pooled, R, offsets, list, G);
-    rc = check_launch("edge_train_dp_kernel");
-    if (rc != PSA_OK) return rc;
-    // dW_a = x^T dQ, dW_b = x^T (dP - dQ): straight into the two row blocks of dW (2c, N)
-    psa_act_in in = {};
-    in.x = x; in.ld = c;
-    const psa_grad_in gq = plain_grad(G, 2 * N, N), gd = plain_grad(G + N, 2 * N, N);
-    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gq, dW, dense_ws, dense_bytes, stream);
-    if (rc != PSA_OK) return rc;
-    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gd, dW + (size_t)c * N, dense_ws, dense_bytes, stream);
-    if (rc != PSA_OK) return rc;
-    // dx = [dQ | dP - dQ] . [W_a | W_b]^T: one product over 2N columns
-    PSA_CUDA(cudaMemcpy2DAsync(W2, (size_t)2 * N * sizeof(float), W, (size_t)N * sizeof(float), (size_t)N * sizeof(float), c,
-                               cudaMemcpyDeviceToDevice, st));
-    PSA_CUDA(cudaMemcpy2DAsync(W2 + N, (size_t)2 * N * sizeof(float), W + (size_t)c * N, (size_t)N * sizeof(float), (size_t)N * sizeof(float), c,
-                               cudaMemcpyDeviceToDevice, st));
-    const psa_grad_in gg = plain_grad(G, 2 * N, 2 * N);
-    return psa_train_dense_bwd_input(rows, c, 2 * N, &gg, W2, dx, c, 0, dense_ws, dense_bytes, stream);
+    return edge_layer_tail(b, n, c, k, N, x, nn_idx, W, PQ, scale, shift, coef, pooled, R, nullptr, dW, dx, ws + L.tail, st);
 }

@@ -27,6 +27,13 @@ int edgeconv_simt(int b, int n, int c, int k, const float* x, const int* nn_idx,
 // `run_if` non-null: no-op unless *run_if != 0 (device-side condition, see tc_mlp.cu)
 int launch_fill_ord_neg_inf(long long total, float* out, cudaStream_t st, const unsigned int* run_if = nullptr);   // out := order-preserving int code of -inf
 int launch_decode_ord(long long total, float* out, cudaStream_t st, const unsigned int* run_if = nullptr);         // int codes -> floats, in place
+// edgeconv_train.cu: the backward of an EdgeConv layer that sees x (y_ij = Q_i + P_nn(i,j), PQ (b*n, 2N)) once its batch-norm coefficients
+// coef (3, N) are known -> dW (2c, N), dx (b*n, c).  dz (b*n*k, N) gives the gradient w.r.t. the layer's batch-norm output per edge; when it
+// is null, the max's gradient is routed by (pooled, R) as the single-layer op does.  workspace: edge_tail_workspace_bytes, 256-byte aligned.
+size_t edge_tail_workspace_bytes(int b, int n, int c, int k, int N);
+int edge_layer_tail(int b, int n, int c, int k, int N, const float* x, const int* nn_idx, const float* W, const float* PQ, const float* scale,
+                    const float* shift, const float* coef, const float* pooled, const float* R, const float* dz, float* dW, float* dx,
+                    void* workspace, cudaStream_t st);
 
 }  // namespace psa
 

@@ -75,21 +75,14 @@ def _backbone(point_cloud, params, end_points, k=K_NEIGHBORS):
 
 def _edge_conv_training(x, k, layers, bn_decay, params, idx=None):
     """pairwise_distance -> knn -> get_edge_feature -> conv2d(+BN+ReLU)... -> reduce_max over k (dgcnn.py:31-44) in training mode.
-    The neighbour graph carries no gradient; batch statistics over all B*N*k edges.  A single layer (dgcnn1..4) runs as the fused
-    edgeconv_training (no per-edge tensor); deeper stacks (the T-net's, C = 3) build the edge tensor [x_i, x_j - x_i] from the
-    differentiable group_point (GroupPointGrad) and torch glue and run the convolutions as mlp_training."""
-    from .training import edgeconv_training, mlp_training
-    b, n, c = x.shape
+    The neighbour graph carries no gradient; batch statistics over all B*N*k edges.  The single-layer EdgeConvs (dgcnn1..4) and the
+    T-net's two-layer one run as the fused edgeconv_training: no per-edge tensor."""
+    from .training import edgeconv_training
     if idx is None:
         with torch.no_grad():
             idx = ops.knn_graph(x.detach().contiguous(), k)
-    if len(layers) == 1:
-        return edgeconv_training(x, idx, layers[0][0], bn_decay, params), idx
-    neigh = ops.group_point(x.contiguous(), idx)                               # (B,N,k,C), differentiable in x
-    centre = x.unsqueeze(2).expand(b, n, k, c)
-    edge = torch.cat([centre, neigh - centre], dim=-1)                         # get_edge_feature, dgcnn/utils/tf_util.py:674-706
-    y = mlp_training(edge.reshape(b * n * k, 2 * c), layers, bn_decay, params)
-    return y.view(b, n, k, -1).amax(dim=2), idx                                # tf.reduce_max(axis=-2)
+    scopes = [scope for scope, _ in layers]
+    return edgeconv_training(x, idx, scopes[0] if len(scopes) == 1 else scopes, bn_decay, params), idx
 
 
 def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, dropout: bool = True, k=K_NEIGHBORS, graphs=None, bga: bool = False):

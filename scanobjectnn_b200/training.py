@@ -382,19 +382,108 @@ class _EdgeConvFn(torch.autograd.Function):
         return _flat_grad_of_layers(tr.fp, [tr.layer]), dx.view(tr.b, tr.n, tr.c).clone(), None, None, None
 
 
-def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope: str, bn_decay, params: VariableStore) -> torch.Tensor:
-    """Training-mode single-layer EdgeConv with autograd: x (B, N, C), nn_idx (B, N, k) int32 -> (B, N, C_out) =
-    max_j relu(BN([x_i, x_j - x_i] . W + b)), BN over all B*N*k edges.  The graph carries no gradient.  Buffers are cached on
-    `params` per (scope, shape); the variables' gradients land in the flat bucket."""
+class EdgeConv2Trainer(_TrainOps):
+    """Training-mode two-layer EdgeConv (transform_nets.py:18-27: get_edge_feature -> conv2d + BN + ReLU -> conv2d + BN + ReLU ->
+    reduce_max over k) on csrc/edgeconv2_train.cu: layer 1 is the single-layer op's point product, the per-edge 64 -> 128 product runs
+    on the tensor cores and is recomputed in every pass; no (B,N,k,.) tensor is stored in the forward.  Batch statistics over all
+    b*n*k edges in both layers; the max's gradient is split evenly among tied edges."""
+
+    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scopes, device=None):
+        self.lib = _lib.load()
+        self.params = params
+        self.dev = torch.device(device) if device is not None else params.device
+        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
+        params._flat = self.fp
+        self.b, self.n, self.c, self.k = b, n, c, k
+        self.layers = [_Layer(self.fp, s, 0, True, self.dev) for s in scopes]     # rows = 0: the per-edge activations are never stored
+        l1, l2 = self.layers
+        if l1.K != 2 * c:
+            raise ValueError(f"{l1.scope}: weights of shape {tuple(l1.W.shape)}, an EdgeConv over {c} channels needs ({2 * c}, C1)")
+        if l2.K != l1.N:
+            raise ValueError(f"{l2.scope}: weights of shape {tuple(l2.W.shape)}, the second layer needs ({l1.N}, C2)")
+        rows, N = b * n, l2.N
+        self.ws_bytes = self.lib.psa_edgeconv2_train_workspace_bytes(b, n, c, k, l1.N, N)
+        if self.ws_bytes == 0:
+            raise _lib.PsaError(f"{l1.scope}, {l2.scope}: two-layer EdgeConv training needs C1 = 64, C2 = 128 and k <= 32 "
+                                f"(got C1 = {l1.N}, C2 = {N}, k = {k})")
+        f32 = dict(dtype=torch.float32, device=self.dev)
+        self.PQ = torch.empty((rows, 2 * l1.N), **f32)
+        self.pooled = torch.empty((rows, N), **f32)
+        self.mask = torch.empty((rows, N), dtype=torch.int32, device=self.dev)
+        self.ywin = torch.empty((rows, N), **f32)
+        self.d_in = torch.empty((rows, c), **f32)
+        self.ws = torch.empty(self.ws_bytes // 4 + 64, **f32)
+
+    def forward(self, x: torch.Tensor, nn_idx: torch.Tensor, bn_decay: float = 0.5) -> torch.Tensor:
+        b, n, c, k = self.b, self.n, self.c, self.k
+        l1, l2 = self.layers
+        assert x.shape == (b, n, c) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
+        assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
+        self.x, self.nn_idx = x, nn_idx
+        lib, ws, wsb = self.lib, _p(self.ws), C.c_size_t(self.ws_bytes)
+        self._c(lib.psa_edgeconv_train_fwd(b, n, c, k, l1.N, _p(x), _p(nn_idx), _p(l1.W), _p(l1.b), _p(self.PQ), _p(l1.stats), ws, wsb, _stream()),
+                "edgeconv_train_fwd")
+        self._bn_finalize(l1, b * n * k, bn_decay)
+        self._c(lib.psa_edgeconv2_train_fwd(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
+                                            _p(l2.stats), ws, wsb, _stream()), "edgeconv2_train_fwd")
+        self._bn_finalize(l2, b * n * k, bn_decay)
+        self._c(lib.psa_edgeconv2_train_pool(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
+                                             _p(l2.scale), _p(l2.shift), _p(self.pooled), _p(self.mask), _p(self.ywin), ws, wsb, _stream()),
+                "edgeconv2_train_pool")
+        return self.pooled
+
+    def backward(self, dout: torch.Tensor) -> torch.Tensor:
+        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); both layers' gradients go to the flat bucket"""
+        b, n, c, k = self.b, self.n, self.c, self.k
+        l1, l2 = self.layers
+        dout = dout.contiguous()
+        self._c(self.lib.psa_edgeconv2_train_bwd(b, n, c, k, l1.N, l2.N, _p(self.x), _p(self.nn_idx), _p(l1.W), _p(self.PQ), _p(l1.scale),
+                                                 _p(l1.shift), _p(l1.gamma), _p(l1.mean_inv), _p(l2.W), _p(l2.b), _p(l2.gamma), _p(l2.mean_inv),
+                                                 _p(self.pooled), _p(self.mask), _p(self.ywin), _p(dout), _p(l1.dW), _p(l1.dgamma), _p(l1.dbeta),
+                                                 _p(l2.dW), _p(l2.dgamma), _p(l2.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                 _stream()), "edgeconv2_train_bwd")
+        l1.db.zero_()          # sum over the edges of dy = 0 under batch norm, in both layers
+        l2.db.zero_()
+        return self.d_in
+
+
+class _EdgeConv2Fn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, flat, x, nn_idx, trainer, bn_decay):
+        ctx.trainer = trainer
+        return trainer.forward(x, nn_idx, bn_decay).clone()
+
+    @staticmethod
+    def backward(ctx, dout):
+        tr = ctx.trainer
+        dx = tr.backward(dout)
+        return _flat_grad_of_layers(tr.fp, tr.layers), dx.view(tr.b, tr.n, tr.c).clone(), None, None, None
+
+
+def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, params: VariableStore) -> torch.Tensor:
+    """Training-mode EdgeConv with autograd: x (B, N, C), nn_idx (B, N, k) int32 -> (B, N, C_out) = max_j relu(BN([x_i, x_j - x_i] . W + b)),
+    BN over all B*N*k edges.  `scope` is one scope, or a sequence of two for the two-layer EdgeConv (conv + BN + ReLU twice, then the
+    max; C1 = 64, C2 = 128), which runs as one autograd node.  The graph carries no gradient.  Buffers are cached on `params` per
+    (scopes, shape); the variables' gradients land in the flat bucket."""
     b, n, c = x.shape
     k = nn_idx.shape[-1]
-    key = ("edgeconv", scope, b, n, c, k)
+    scopes = (scope,) if isinstance(scope, str) else tuple(scope)
+    if len(scopes) not in (1, 2):
+        raise ValueError(f"edgeconv_training: one or two scopes, got {len(scopes)}")
     cache = params.__dict__.setdefault("_trainers", {})
-    if key not in cache:
-        cache[key] = EdgeConvTrainer(params, b, n, c, k, scope, device=x.device)
+    if len(scopes) == 1:
+        key = ("edgeconv", scopes[0], b, n, c, k)
+        if key not in cache:
+            cache[key] = EdgeConvTrainer(params, b, n, c, k, scopes[0], device=x.device)
+        fn = _EdgeConvFn
+    else:
+        key = ("edgeconv2", scopes, b, n, c, k)
+        if key not in cache:
+            cache[key] = EdgeConv2Trainer(params, b, n, c, k, scopes, device=x.device)
+        fn = _EdgeConv2Fn
     tr = cache[key]
     tr.fp.flat.requires_grad_(True)
-    out = _EdgeConvFn.apply(tr.fp.flat, x.contiguous(), nn_idx.to(torch.int32).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
+    out = fn.apply(tr.fp.flat, x.contiguous(), nn_idx.to(torch.int32).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
     return out.view(b, n, -1)
 
 

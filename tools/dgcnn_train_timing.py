@@ -1,12 +1,12 @@
-"""DGCNN training at B=32, N=2048, k=20: the fused training-mode EdgeConv (training.edgeconv_training, csrc/edgeconv_train.cu)
-against the materialising composition it replaced in dgcnn.py (group_point -> [x_i, x_j - x_i] -> mlp_training over B*N*k edge
-rows -> amax over k), in one process, alternating the two.
+"""DGCNN training at B=32, N=2048, k=20: the fused training-mode EdgeConvs (training.edgeconv_training, csrc/edgeconv_train.cu
+and csrc/edgeconv2_train.cu) against the materialising composition they replaced in dgcnn.py (group_point -> [x_i, x_j - x_i] ->
+mlp_training over B*N*k edge rows -> amax over k), in one process, alternating the two.
 
-  per layer   for each EdgeConv shape of dgcnn1..4 (2C -> C_out = 6 -> 64, 128 -> 64, 128 -> 128): forward and forward + backward
-              time (CUDA events, median of repeats after warm-up), the rise of torch.cuda.max_memory_allocated over one forward +
-              backward, and the largest output / input-gradient difference between the two
-  whole step  dgcnn.get_model(is_training=True) + get_loss + backward, clouds/s; the composition is substituted for the single-layer
-              EdgeConvs inside this script only
+  per layer   for each EdgeConv shape of dgcnn1..4 (2C -> C_out = 6 -> 64, 128 -> 64, 128 -> 128) and the T-net's two-layer one
+              (6 -> 64 -> 128): forward and forward + backward time (CUDA events, median of repeats after warm-up), the rise of
+              torch.cuda.max_memory_allocated over one forward + backward, and the largest output / input-gradient difference
+  whole step  dgcnn.get_model(is_training=True) + get_loss + backward, clouds/s; the composition is substituted for every EdgeConv
+              (T-net included) inside this script only
 
 Prints the card name and power limit, then one JSON line.  Usage: python tools/dgcnn_train_timing.py [--reps 15] [--steps 10]"""
 import argparse
@@ -27,20 +27,22 @@ from scanobjectnn_b200.tf_util import VariableStore
 from scanobjectnn_b200.training import edgeconv_training, mlp_training
 
 B, N, K = 32, 2048, 20
-SHAPES = [("dgcnn1", 3, 64), ("dgcnn2", 64, 64), ("dgcnn4", 64, 128)]          # (scope, C, C_out): 2C -> C_out
+TNET = ("transform_net1/tconv1", "transform_net1/tconv2")
+SHAPES = [(("dgcnn1",), 3, [64]), (("dgcnn2",), 64, [64]), (("dgcnn4",), 64, [128]), (TNET, 3, [64, 128])]   # (scopes, C, widths)
 
 
-def composition(x, idx, scope, bn_decay, params):
+def composition(x, idx, scopes, bn_decay, params):
     b, n, c = x.shape
     k = idx.shape[-1]
+    scopes = (scopes,) if isinstance(scopes, str) else scopes
     centre = x.unsqueeze(2).expand(b, n, k, c)
     edge = torch.cat([centre, ops.group_point(x.contiguous(), idx) - centre], dim=-1)
-    y = mlp_training(edge.reshape(b * n * k, 2 * c), [(scope, True)], bn_decay, params)
+    y = mlp_training(edge.reshape(b * n * k, 2 * c), [(s, True) for s in scopes], bn_decay, params)
     return y.view(b, n, k, -1).amax(dim=2)
 
 
-def fused(x, idx, scope, bn_decay, params):
-    return edgeconv_training(x, idx, scope, bn_decay, params)
+def fused(x, idx, scopes, bn_decay, params):
+    return edgeconv_training(x, idx, scopes[0] if len(scopes) == 1 else scopes, bn_decay, params)
 
 
 def card():
@@ -60,14 +62,16 @@ def event_ms(fn):
 def per_layer(reps):
     res = {}
     rng = np.random.default_rng(0)
-    for scope, c, cout in SHAPES:
+    for scope, c, widths in SHAPES:
+        cout = widths[-1]
         x = torch.tensor(rng.standard_normal((B, N, c)).astype(np.float32), device="cuda", requires_grad=True)
         idx = ops.knn_graph(x.detach(), K)
         R = torch.tensor(rng.standard_normal((B, N, cout)).astype(np.float32), device="cuda")
         stores = {}
         for name in ("composition", "fused"):
             stores[name] = VariableStore(device="cuda", seed=1)
-            stores[name].add_conv2d(scope, 2 * c, cout, randomize_bn=True)
+            for s_, cin, w_ in zip(scope, [2 * c] + widths[:-1], widths):
+                stores[name].add_conv2d(s_, cin, w_, randomize_bn=True)
         paths = {"composition": composition, "fused": fused}
 
         def fwd(name):
@@ -99,7 +103,7 @@ def per_layer(reps):
                 t[name]["fwd"].append(event_ms(lambda: fwd(name)))
                 t[name]["fwd_bwd"].append(event_ms(lambda: fwd_bwd(name)))
         rel = lambda a, b: float((a - b).abs().max() / b.abs().max())                     # noqa: E731
-        res[f"{2 * c}->{cout}"] = {
+        res["->".join(str(v) for v in [2 * c] + widths)] = {
             **{name: {"fwd_ms": float(np.median(t[name]["fwd"])), "fwd_bwd_ms": float(np.median(t[name]["fwd_bwd"])),
                       "peak_alloc_rise_mib": mem[name]} for name in paths},
             "speedup_fwd_bwd": float(np.median(t["composition"]["fwd_bwd"]) / np.median(t["fused"]["fwd_bwd"])),
@@ -120,12 +124,10 @@ def whole_step(steps):
     fused_edge = dgcnn._edge_conv_training
 
     def composition_edge(x, k, layers, bn_decay, params, idx=None):
-        if len(layers) > 1:
-            return fused_edge(x, k, layers, bn_decay, params, idx)
         if idx is None:
             with torch.no_grad():
                 idx = ops.knn_graph(x.detach().contiguous(), k)
-        return composition(x, idx, layers[0][0], bn_decay, params), idx
+        return composition(x, idx, tuple(s for s, _ in layers), bn_decay, params), idx
 
     stores = {name: dgcnn.init_params(seed=2) for name in ("composition", "fused")}
     edge_fns = {"composition": composition_edge, "fused": fused_edge}
