@@ -347,8 +347,8 @@ typedef struct psa_grad_in {
 PSA_API size_t psa_train_dense_workspace_bytes(long long rows, int K, int N);
 PSA_API int psa_train_dense_fwd(long long rows, int K, int N, const psa_act_in* in, const float* W, const float* bias,
                                 float* y, float* stats, void* workspace, size_t workspace_bytes, psa_stream_t stream);
-/* dx (rows, K - col_skip) = dy (rows, N) . W^T restricted to input channels >= col_skip (the xyz channels of a
- * concatenated input carry no gradient that anyone consumes). */
+/* dx (rows, K - col_skip) = dy (rows, N) . W^T restricted to input channels >= col_skip (e.g. the feature columns of a
+ * concatenated [xyz, points] input; the coordinate columns come from a second product over the first rows of W). */
 PSA_API int psa_train_dense_bwd_input(long long rows, int K, int N, const psa_grad_in* g, const float* W, float* dx,
                                       long long ld_dx, int col_skip, void* workspace, size_t workspace_bytes,
                                       psa_stream_t stream);
@@ -394,6 +394,21 @@ PSA_API size_t psa_sa_conv1_bwd_workspace_bytes(int b, int n, int m, int nsample
 PSA_API int psa_sa_conv1_bwd(int b, int n, int m, int nsample, int C1, const float* xyz, const float* new_xyz,
                              const int* idx, const psa_grad_in* g, float* dW_xyz, float* dU, void* workspace,
                              size_t workspace_bytes, psa_stream_t stream);
+
+/* Coordinate gradient of the fused first layer (the reference's GroupPointGrad of grouped_xyz plus the "- tile(new_xyz)" term,
+ * pointnet_util.py:40-46, tf_grouping.py:43-47).  With dy0 = g over the b*m*nsample grouped rows (the same psa_grad_in as
+ * psa_sa_conv1_bwd) and W_xyz (3, C1) = the coordinate rows of the first weight (16-byte aligned), every row r = (cloud, q, k) gives
+ * v_r = W_xyz . dy0_r, and
+ *   dxyz (b, n, 3)     = sum over the rows r with idx_r = p of v_r, each point's rows added in ascending row order (stable
+ *                        counting sort of idx, as in psa_sa_conv1_bwd's dU);
+ *   dnew_xyz (b, m, 3) = -(v_{q,0} + v_{q,1} + ...), added in slot order.
+ * Padding rows (copies of slot 0) and empty balls (idx = 0) are rows like any other.  The gradient with respect to the input
+ * cloud is dxyz + GatherPointGrad(dnew_xyz + whatever else new_xyz receives, fps_idx) (psa_gather_point_grad).  Both outputs are
+ * fully written; no float atomics, every sum in a fixed order: bit-reproducible.  C1 a multiple of 4, at most 1024 (else
+ * PSA_ERR_UNSUPPORTED).  workspace: psa_sa_conv1_bwd_xyz_workspace_bytes(...). */
+PSA_API size_t psa_sa_conv1_bwd_xyz_workspace_bytes(int b, int n, int m, int nsample);
+PSA_API int psa_sa_conv1_bwd_xyz(int b, int n, int m, int nsample, int C1, const float* W_xyz, const int* idx, const psa_grad_in* g,
+                                 float* dxyz, float* dnew_xyz, void* workspace, size_t workspace_bytes, psa_stream_t stream);
 
 /* Training-mode single-layer EdgeConv (dgcnn/models/dgcnn.py:41-47, dgcnn/utils/tf_util.py:115-173,462-499):
  *   out_ic = max_j relu(BN(y_ij)),  y_ij = [x_i, x_j - x_i] . W + bias,  BN with the batch statistics of all b*n*k edges.

@@ -88,6 +88,7 @@ SIGNATURES = {
     "psa_train_pool_fwd": [_ll, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_bn_bwd_coeffs": [_ll, _i, _gin, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "psa_sa_conv1_bwd": [_i, _i, _i, _i, _i, _p, _p, _p, _gin, _p, _p, _p, _sz, _p],
+    "psa_sa_conv1_bwd_xyz": [_i, _i, _i, _i, _i, _p, _p, _gin, _p, _p, _p, _sz, _p],
     "psa_edgeconv_train_fwd": [_i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "psa_edgeconv_train_pool": [_i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p],
     "psa_edgeconv_train_bwd": [_i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
@@ -102,7 +103,7 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_sa_module_workspace_bytes", "psa_sa_conv1_prebn_workspace_bytes", "psa_sa_group_all_workspace_bytes", "psa_edgeconv_workspace_bytes",
                 "psa_train_dense_workspace_bytes", "psa_bn_bwd_workspace_bytes", "psa_sa_conv1_bwd_workspace_bytes", "psa_knn_graph_workspace_bytes",
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
-                "psa_edgeconv2_train_workspace_bytes")
+                "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes")
 
 _lib = None
 
@@ -137,6 +138,8 @@ def load() -> C.CDLL:
     lib.psa_bn_bwd_workspace_bytes.restype = C.c_size_t
     lib.psa_sa_conv1_bwd_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
     lib.psa_sa_conv1_bwd_workspace_bytes.restype = C.c_size_t
+    lib.psa_sa_conv1_bwd_xyz_workspace_bytes.argtypes = [_i, _i, _i, _i]
+    lib.psa_sa_conv1_bwd_xyz_workspace_bytes.restype = C.c_size_t
     lib.psa_knn_graph_workspace_bytes.argtypes = [_i, _i, _i, _i]
     lib.psa_knn_graph_workspace_bytes.restype = C.c_size_t
     lib.psa_scatter_workspace_bytes.argtypes = [_i, _i, _ll]

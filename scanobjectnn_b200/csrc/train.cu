@@ -334,6 +334,79 @@ group_grad_csr_kernel(const GradIn g, int n, int mk, int C1, long long total_poi
     }
 }
 
+// ---- coordinate gradient of the fused first layer (psa_sa_conv1_bwd_xyz) ----
+// One warp per query: groups of LPR lanes (4 channels per lane) take one grouped row each, RPW = 32 / LPR rows per step.  Each row
+// gives v_r = W_xyz . dy0_r (three dot products over C1, lane partials in channel order, then a butterfly inside the group), stored
+// as a float4 for the point-side pass; the query's dnew = -(v_0 + v_1 + ... ) is added in slot order by lane 0.  Fixed order.
+template <int LPR>
+__global__ void __launch_bounds__(256)
+conv1_vxyz_kernel(const GradIn g, long long queries, int nsample, int C1, const float* __restrict__ w, float4* __restrict__ v,
+                  float* __restrict__ dnew) {
+    constexpr int RPW = 32 / LPR;
+    const int lane = threadIdx.x & 31, sub = lane % LPR, rs = lane / LPR;
+    const long long q = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (q >= queries) return;
+    float sx = 0.f, sy = 0.f, sz = 0.f;                                     // lane 0: running slot-order sum of the query
+    for (int k0 = 0; k0 < nsample; k0 += RPW) {
+        const int k = k0 + rs;
+        float ax = 0.f, ay = 0.f, az = 0.f;
+        if (k < nsample) {
+            const long long r = q * nsample + k;
+            for (int c = 4 * sub; c < C1; c += 4 * LPR) {
+                const float4 d = g.get4(r, c);
+                const float4 wx = __ldg(reinterpret_cast<const float4*>(w + c));
+                const float4 wy = __ldg(reinterpret_cast<const float4*>(w + C1 + c));
+                const float4 wz = __ldg(reinterpret_cast<const float4*>(w + 2 * C1 + c));
+                ax = fmaf(wx.w, d.w, fmaf(wx.z, d.z, fmaf(wx.y, d.y, fmaf(wx.x, d.x, ax))));
+                ay = fmaf(wy.w, d.w, fmaf(wy.z, d.z, fmaf(wy.y, d.y, fmaf(wy.x, d.x, ay))));
+                az = fmaf(wz.w, d.w, fmaf(wz.z, d.z, fmaf(wz.y, d.y, fmaf(wz.x, d.x, az))));
+            }
+        }
+#pragma unroll
+        for (int o = LPR / 2; o > 0; o >>= 1) {
+            ax += __shfl_xor_sync(0xffffffffu, ax, o);
+            ay += __shfl_xor_sync(0xffffffffu, ay, o);
+            az += __shfl_xor_sync(0xffffffffu, az, o);
+        }
+        if (sub == 0 && k < nsample) v[q * nsample + k] = make_float4(ax, ay, az, 0.f);
+#pragma unroll
+        for (int j = 0; j < RPW; ++j) {                                     // the step's rows, in slot order
+            const float bx = __shfl_sync(0xffffffffu, ax, j * LPR), by = __shfl_sync(0xffffffffu, ay, j * LPR);
+            const float bz = __shfl_sync(0xffffffffu, az, j * LPR);
+            if (k0 + j < nsample) { sx += bx; sy += by; sz += bz; }
+        }
+    }
+    if (lane == 0) { dnew[q * 3] = -sx; dnew[q * 3 + 1] = -sy; dnew[q * 3 + 2] = -sz; }
+}
+
+// dxyz[p] = sum of v over the rows that grouped point p, in ascending row order (the CSR of launch_group_csr); one thread per point
+__global__ void __launch_bounds__(256)
+point_vsum_csr_kernel(int n, int mk, long long total_points, const int* __restrict__ offsets, const int* __restrict__ list,
+                      const float4* __restrict__ v, float* __restrict__ dxyz) {
+    const long long pt = (long long)blockIdx.x * 256 + threadIdx.x;
+    if (pt >= total_points) return;
+    const long long cloud = pt / n;
+    const int j = (int)(pt - cloud * n);
+    const int* off = offsets + (size_t)cloud * (n + 1);
+    const int* lst = list + (size_t)cloud * mk;
+    const float4* vc = v + (size_t)cloud * mk;
+    const int t0 = __ldg(off + j), t1 = __ldg(off + j + 1);
+    float x = 0.f, y = 0.f, z = 0.f;
+    int t = t0;
+    for (; t + 3 < t1; t += 4) {                                            // four rows in flight, added in list order
+        float4 d[4];
+#pragma unroll
+        for (int u = 0; u < 4; ++u) d[u] = __ldg(vc + __ldg(lst + t + u));
+#pragma unroll
+        for (int u = 0; u < 4; ++u) { x += d[u].x; y += d[u].y; z += d[u].z; }
+    }
+    for (; t < t1; ++t) {
+        const float4 d = __ldg(vc + __ldg(lst + t));
+        x += d.x; y += d.y; z += d.z;
+    }
+    dxyz[pt * 3] = x; dxyz[pt * 3 + 1] = y; dxyz[pt * 3 + 2] = z;
+}
+
 // ---- bias gradient of a layer WITHOUT batch norm: db[c] = sum_r dy[r][c]; block = one column, fixed-order tree ----
 __global__ void __launch_bounds__(256) bias_grad_kernel(const GradIn g, long long rows, float* __restrict__ db) {
     __shared__ float red[256];
@@ -633,6 +706,43 @@ extern "C" int psa_sa_conv1_bwd(int b, int n, int m, int nsample, int C1, const 
         return check_launch("group_grad_csr_kernel");
     }
     return PSA_OK;
+}
+
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+extern "C" size_t psa_sa_conv1_bwd_xyz_workspace_bytes(int b, int n, int m, int nsample) {
+    if (b <= 0 || n <= 0 || m <= 0 || nsample <= 0) return 256;
+    const size_t rows = (size_t)b * m * nsample;
+    // per-row v (float4) | CSR offsets (b, n+1) | row lists (b, m*nsample)
+    return align256(rows * sizeof(float4)) + align256((size_t)b * (n + 1) * sizeof(int)) + rows * sizeof(int);
+}
+
+extern "C" int psa_sa_conv1_bwd_xyz(int b, int n, int m, int nsample, int C1, const float* W_xyz, const int* idx, const psa_grad_in* g,
+                                    float* dxyz, float* dnew_xyz, void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    PSA_REQUIRE(b >= 1 && n >= 1 && m >= 1 && nsample >= 1, "sa_conv1_bwd_xyz: bad dims b=%d n=%d m=%d nsample=%d", b, n, m, nsample);
+    PSA_REQUIRE((long long)m * nsample <= 0x7fffffffLL, "sa_conv1_bwd_xyz: m*nsample exceeds int32");
+    PSA_SUPPORTED(C1 % 4 == 0 && C1 >= 4 && C1 <= 1024, "sa_conv1_bwd_xyz: C1=%d", C1);
+    PSA_REQUIRE(W_xyz && idx && g && dxyz && dnew_xyz, "sa_conv1_bwd_xyz: null buffer");
+    PSA_REQUIRE((reinterpret_cast<uintptr_t>(W_xyz) & 15) == 0, "sa_conv1_bwd_xyz: W_xyz must be 16-byte aligned");
+    const size_t need = psa_sa_conv1_bwd_xyz_workspace_bytes(b, n, m, nsample);
+    PSA_REQUIRE(workspace && workspace_bytes >= need, "sa_conv1_bwd_xyz: workspace of %zu bytes required, got %zu", need, workspace_bytes);
+    cudaStream_t st = as_stream(stream);
+    const GradIn gi(*g);
+    const long long queries = (long long)b * m, rows = queries * nsample;
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    float4* v = reinterpret_cast<float4*>(ws);
+    int* offsets = reinterpret_cast<int*>(ws + align256((size_t)rows * sizeof(float4)));
+    int* list = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(offsets) + align256((size_t)b * (n + 1) * sizeof(int)));
+    const unsigned qblocks = (unsigned)((queries + 7) / 8);
+    if (C1 <= 32) conv1_vxyz_kernel<8><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
+    else if (C1 <= 64) conv1_vxyz_kernel<16><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
+    else conv1_vxyz_kernel<32><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
+    int rc = check_launch("conv1_vxyz_kernel");
+    if (rc != PSA_OK) return rc;
+    rc = launch_group_csr(b, n, m * nsample, idx, offsets, list, st);
+    if (rc != PSA_OK) return rc;
+    const long long pts = (long long)b * n;
+    point_vsum_csr_kernel<<<(unsigned)((pts + 255) / 256), 256, 0, st>>>(n, m * nsample, pts, offsets, list, v, dxyz);
+    return check_launch("point_vsum_csr_kernel");
 }
 
 extern "C" int psa_train_bias_grad(long long rows, int N, const psa_grad_in* g, float* db, psa_stream_t stream) {

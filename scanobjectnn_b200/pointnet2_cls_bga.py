@@ -32,6 +32,10 @@ def init_params(num_class=NUM_CLASSES, seed=0, device="cuda", randomize_bn=False
 def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *, params: VariableStore, return_end_points: bool = False):
     if is_training:
         return _get_model_training(point_cloud, bn_decay, num_class, params, return_end_points)
+    from .training import wants_input_grad
+    if wants_input_grad(point_cloud):
+        # inference mode with an input gradient: the training kernels with batch norm on the moving averages, no dropout
+        return _get_model_training(point_cloud, bn_decay, num_class, params, return_end_points, dropout=False, frozen=True)
     batch_size = point_cloud.shape[0]
     end_points = {}
     l0_xyz = point_cloud[:, :, 0:3].contiguous()
@@ -65,16 +69,19 @@ def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *,
     return (class_pred, seg_pred, end_points) if return_end_points else (class_pred, seg_pred)
 
 
-def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, return_end_points: bool, dropout: bool = True):
+def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, return_end_points: bool, dropout: bool = True,
+                        frozen: bool = False):
     """Training-mode forward (pointnet2_cls_bga.py:21-75 with is_training=True): every layer with batch-statistics batch norm, dropout
     (keep 0.5) after fc1 / fc2 / seg_fc1, PyTorch autograd over the hand-written level / MLP / interpolation kernels
     (training.py: sa_module_training, mlp_training; ops.three_interpolate).  Gradients of the variables arrive on
-    ``params._flat.flat.grad`` (and per name through ``params._flat`` views)."""
+    ``params._flat.flat.grad`` (and per name through ``params._flat`` views).  frozen=True (with dropout=False): inference mode with
+    batch norm on the moving averages, for a point cloud that requires grad -- input gradients only."""
     from .training import mlp_training
     f = torch.nn.functional
     b = point_cloud.shape[0]
     l0_xyz = point_cloud[:, :, 0:3].contiguous()
-    sa = dict(mlp2=None, is_training=True, bn_decay=bn_decay, params=params)
+    sa = dict(mlp2=None, is_training=not frozen, bn_decay=bn_decay, params=params)
+    mlp = lambda x, layers: mlp_training(x, layers, bn_decay, params, frozen=frozen)  # noqa: E731
     l1_xyz, l1_points, _ = pointnet_sa_module(l0_xyz, None, npoint=512, radius=0.2, nsample=64, mlp=[64, 64, 128], group_all=False, scope="layer1", **sa)
     l2_xyz, l2_points, _ = pointnet_sa_module(l1_xyz, l1_points, npoint=128, radius=0.4, nsample=64, mlp=[128, 128, 256], group_all=False, scope="layer2",
                                               **sa)
@@ -82,15 +89,15 @@ def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore,
                                               scope="layer3", **sa)
     net = l3_points.reshape(b, -1)
     drop = (lambda t: f.dropout(t, 0.5, training=True)) if dropout else (lambda t: t)
-    net = drop(mlp_training(net, [("fc1", True)], bn_decay, params))                     # fc1 -> dp1
-    net = mlp_training(net, [("fc2", True)], bn_decay, params)
+    net = drop(mlp(net, [("fc1", True)]))                     # fc1 -> dp1
+    net = mlp(net, [("fc2", True)])
     class_vector = net.unsqueeze(1)                                                      # taken BEFORE dp2 (pointnet2_cls_bga.py:45-48)
-    class_pred = mlp_training(drop(net), [("fc3", False)], bn_decay, params)
-    l2_points = pointnet_fp_module(l2_xyz, l3_xyz, l2_points, class_vector, [256, 256], True, bn_decay, scope="fa_layer1", params=params)
-    l1_points = pointnet_fp_module(l1_xyz, l2_xyz, l1_points, l2_points, [256, 128], True, bn_decay, scope="fa_layer2", params=params)
-    l0_points = pointnet_fp_module(l0_xyz, l1_xyz, None, l1_points, [128, 128, 128], True, bn_decay, scope="fa_layer3", params=params)
-    feats = mlp_training(l0_points, [("seg_fc1", True)], bn_decay, params)
-    seg_pred = mlp_training(drop(feats), [("seg_fc2", False)], bn_decay, params)
+    class_pred = mlp(drop(net), [("fc3", False)])
+    l2_points = pointnet_fp_module(l2_xyz, l3_xyz, l2_points, class_vector, [256, 256], not frozen, bn_decay, scope="fa_layer1", params=params)
+    l1_points = pointnet_fp_module(l1_xyz, l2_xyz, l1_points, l2_points, [256, 128], not frozen, bn_decay, scope="fa_layer2", params=params)
+    l0_points = pointnet_fp_module(l0_xyz, l1_xyz, None, l1_points, [128, 128, 128], not frozen, bn_decay, scope="fa_layer3", params=params)
+    feats = mlp(l0_points, [("seg_fc1", True)])
+    seg_pred = mlp(drop(feats), [("seg_fc2", False)])
     end_points = dict(feats=feats, l1_xyz=l1_xyz, l2_xyz=l2_xyz, l1_points=l1_points, l2_points=l2_points, l3_points=l3_points)
     return (class_pred, seg_pred, end_points) if return_end_points else (class_pred, seg_pred)
 

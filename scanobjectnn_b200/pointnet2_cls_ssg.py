@@ -36,9 +36,12 @@ def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *,
     is_training=True: batch-statistics batch norm in every layer (moving averages updated with ``bn_decay``), dropout in
     the head, and logits that carry a grad_fn -- ``get_loss(...).backward()`` runs the hand-written backward kernels and
     leaves the gradient of every variable in ``params._flat.grad_of(name)`` (training.py)."""
-    if is_training:
-        from .training import get_model_training
-        logits, tr = get_model_training(point_cloud, bn_decay, num_class, params)
+    from .training import get_model_training, wants_input_grad
+    frozen = not is_training and wants_input_grad(point_cloud)
+    if is_training or frozen:
+        # frozen: inference mode with a gradient w.r.t. the point cloud (batch norm on the moving averages, no dropout, the training
+        # kernels); calls that need no gradient stay on the fused inference kernels below
+        logits, tr = get_model_training(point_cloud, bn_decay, num_class, params, frozen=frozen)
         lv = tr.levels
         end_points = {"l0_xyz": point_cloud, "l1_xyz": lv[0].new_xyz, "l1_points": lv[0].pooled.view(point_cloud.shape[0], lv[0].m, -1),
                       "l1_indices": lv[0].idx, "l2_xyz": lv[1].new_xyz, "l2_points": lv[1].pooled.view(point_cloud.shape[0], lv[1].m, -1),

@@ -80,6 +80,17 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp, mlp2, group_al
         spec = LevelSpec(scope, None if group_all else npoint, None if group_all else radius, None if group_all else nsample, list(mlp),
                          group_all=bool(group_all))
         return sa_module_training(xyz, points, spec, bn_decay, params)
+    from .training import wants_input_grad
+    if wants_input_grad(xyz, points):
+        # inference mode with an input gradient (saliency, adversarial perturbation): the training kernels with batch norm on the
+        # moving averages (training.py, frozen=True); calls that need no gradient stay on the fused kernels below
+        if not (pooling == "max" and mlp2 is None and use_xyz and not knn and bn and new_xyz is None):
+            raise NotImplementedError("input gradients of pointnet_sa_module(is_training=False) cover max pooling, use_xyz, ball query, "
+                                      "bn=True, no mlp2 and no caller-sampled new_xyz")
+        from .training import LevelSpec, sa_module_training
+        spec = LevelSpec(scope, None if group_all else npoint, None if group_all else radius, None if group_all else nsample, list(mlp),
+                         group_all=bool(group_all))
+        return sa_module_training(xyz, points, spec, bn_decay, params, frozen=True)
     scopes = _mlp_scopes(scope, mlp)
     if pooling != "max":
         # pointnet_util.py:128-146 -- unused by the in-scope models, so the grouped rows are materialised: group -> per-row
@@ -173,9 +184,13 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay,
     """pointnet_util.pointnet_fp_module (pointnet_util.py:199-229): three_nn + inverse-distance weights +
     three_interpolate in ONE launch (the reference runs them on the CPU), concat skip features, 1x1 convs."""
     scopes = [f"{scope}/conv_{i}" for i in range(len(mlp))]
-    if is_training:
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(xyz1, xyz2, points1, points2)
+    if is_training or frozen:
         # three_nn and the inverse-distance weights carry no gradient (they depend on coordinates only); three_interpolate is
         # differentiable in points2 (ThreeInterpolateGrad), the concat is autograd's, the MLP runs with batch-statistics batch norm
+        # frozen (inference mode with an input gradient): the same, with batch norm on the moving averages; the three-NN weights are
+        # constants (the reference's NoGradient('ThreeNN'))
         if not bn:
             raise NotImplementedError("pointnet_fp_module(is_training=True) needs bn=True (what the in-scope models use)")
         from .training import mlp_training
@@ -183,7 +198,7 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay,
             _, _, idx, weight = ops.three_nn_interpolate(xyz1, xyz2, points2.detach(), return_aux=True)
         interpolated = ops.three_interpolate(points2, idx, weight)
         new_points1 = torch.cat([interpolated, points1], dim=2) if points1 is not None else interpolated
-        return mlp_training(new_points1, [(sc, True) for sc in scopes], bn_decay, params)
+        return mlp_training(new_points1, [(sc, True) for sc in scopes], bn_decay, params, frozen=frozen)
     interpolated = ops.three_nn_interpolate(xyz1, xyz2, points2)
     new_points1 = torch.cat([interpolated, points1], dim=2) if points1 is not None else interpolated
     return ops.shared_mlp(new_points1, params.mlp(scopes))

@@ -119,8 +119,13 @@ def _require_inference(is_training):
             "(training.py: sa_module_training, mlp_training, PointNet2ClsTrainer) -- see INTEGRATION.md")
 
 
-def _layer_training(inputs, scope, activation_fn, bn, bn_decay, params):
-    """one conv / fully-connected layer in training mode (training.mlp_training): conv+BN+ReLU or a plain linear layer"""
+def _wants_input_grad(inputs):
+    return torch.is_grad_enabled() and inputs.requires_grad
+
+
+def _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=False):
+    """one conv / fully-connected layer in training mode (training.mlp_training): conv+BN+ReLU or a plain linear layer.
+    frozen=True: inference mode with an input gradient (batch norm on the moving averages)."""
     if bn and activation_fn is not None:
         kind = True
     elif not bn and activation_fn is None:
@@ -128,7 +133,7 @@ def _layer_training(inputs, scope, activation_fn, bn, bn_decay, params):
     else:
         raise NotImplementedError("training mode covers conv/fc + batch norm + ReLU and plain linear layers (what the models use)")
     from .training import mlp_training
-    return mlp_training(inputs, [(scope, kind)], bn_decay, params)
+    return mlp_training(inputs, [(scope, kind)], bn_decay, params, frozen=frozen)
 
 
 def conv2d(inputs, num_output_channels, kernel_size, scope, stride=(1, 1), padding="SAME", data_format="NHWC",
@@ -138,6 +143,8 @@ def conv2d(inputs, num_output_channels, kernel_size, scope, stride=(1, 1), paddi
         raise NotImplementedError("only 1x1 / stride-1 / NHWC convolutions are on the point-set-abstraction path")
     if is_training:
         return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params)
+    if _wants_input_grad(inputs):
+        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=True)
     relu = activation_fn is not None
     mlp = params.mlp([scope], [relu])
     if mlp.channels[-1] != num_output_channels:
@@ -149,6 +156,8 @@ def fully_connected(inputs, num_outputs, scope, activation_fn="relu", bn=False, 
                     params: VariableStore):
     if is_training:
         return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params)
+    if _wants_input_grad(inputs):
+        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=True)
     relu = activation_fn is not None
     mlp = params.mlp([scope], [relu])
     if mlp.channels[-1] != num_outputs:

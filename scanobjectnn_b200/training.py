@@ -25,7 +25,7 @@ import torch
 
 from . import _lib, ops
 from ._lib import PsaActIn, PsaGradIn, check
-from .tf_util import VariableStore
+from .tf_util import BN_EPS, VariableStore
 
 _p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())  # noqa: E731
 
@@ -188,6 +188,10 @@ class _Level:
     dU: torch.Tensor = None
     x_cat: torch.Tensor = None                  # group_all: [xyz, points] rows
     d_in: torch.Tensor = None                   # gradient w.r.t. the level's input features (B*n, c_in)
+    fps_idx: torch.Tensor = None                # (B, m) int32: the sampled centroids (not group_all)
+    dxyz: torch.Tensor = None                   # (B*n, 3): GroupPointGrad of the grouped coordinates (group_all: the xyz columns)
+    dnew: torch.Tensor = None                   # (B*m, 3): gradient reaching new_xyz through "- new_xyz" inside this level
+    dW_scratch: torch.Tensor = None             # frozen batch norm: psa_sa_conv1_bwd's dW_xyz, not a variable gradient
 
 
 class _TrainOps:
@@ -200,9 +204,25 @@ class _TrainOps:
         self._c(self.lib.psa_bn_finalize(ly.N, count, _p(ly.stats), _p(ly.gamma), _p(ly.beta), C.c_float(decay), _p(ly.mov_mean),
                                          _p(ly.mov_var), _p(ly.scale), _p(ly.shift), _p(ly.mean_inv), _stream()), "bn_finalize")
 
-    def _dense_fwd(self, ly: _Layer, a: PsaActIn):
+    def _dense_fwd(self, ly: _Layer, a: PsaActIn, stats: bool = True):
         self._c(self.lib.psa_train_dense_fwd(ly.rows, ly.K, ly.N, C.byref(a), _p(ly.W), _p(ly.b), _p(ly.y),
-                                             _p(ly.stats) if ly.bn else None, _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "train_dense_fwd")
+                                             _p(ly.stats) if ly.bn and stats else None, _p(self.ws), C.c_size_t(self.ws_bytes), _stream()),
+                "train_dense_fwd")
+
+    @staticmethod
+    def _bn_frozen(ly: _Layer):
+        """inference-mode batch norm: the moving averages folded into scale / shift (VariableStore.folded's arithmetic), and the
+        backward coefficients dy = scale * dz (ca = scale, cb = cc = 0).  The moving averages are read, never written."""
+        inv = ly.gamma * torch.rsqrt(ly.mov_var + BN_EPS)
+        ly.scale.copy_(inv)
+        ly.shift.copy_(ly.beta - ly.mov_mean * inv)
+        ly.ca.copy_(inv)
+        ly.cb.zero_()
+        ly.cc.zero_()
+
+    def _dense_bwd_input(self, ly: _Layer, g: PsaGradIn, dx: torch.Tensor, col_skip: int = 0):
+        self._c(self.lib.psa_train_dense_bwd_input(ly.rows, ly.K, ly.N, C.byref(g), _p(ly.W), _p(dx), dx.shape[-1], col_skip, _p(self.ws),
+                                                   C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
 
     def _layer_bwd(self, ly: _Layer, g_nocoef: PsaGradIn, g: PsaGradIn, a_in: PsaActIn, dx: torch.Tensor | None, col_skip: int = 0):
         """gradients of one conv/fc(+BN+relu) layer: BN sums/coefficients, dW, (db), dx."""
@@ -235,11 +255,13 @@ def _flat_grad_of_layers(fp: FlatParams, layers) -> torch.Tensor:
 class MlpTrainer(_TrainOps):
     """Training-mode shared MLP on dense rows -- tf_util.conv1d / conv2d(1x1) / fully_connected chains with batch-statistics batch
     norm + ReLU (tf_util.py:120-185,512-531): the FP modules' MLPs, FC heads, per-point heads.  layers = [(scope, bn), ...];
-    a layer with bn=False has no activation (the reference's logits layers)."""
+    a layer with bn=False has no activation (the reference's logits layers).  frozen=True: inference mode -- batch norm on the
+    moving averages (never updated), and a backward that gives the input gradient only."""
 
-    def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None):
+    def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None, frozen: bool = False):
         self.lib = _lib.load()
         self.params = params
+        self.frozen = frozen
         self.dev = torch.device(device) if device is not None else params.device
         self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
         params._flat = self.fp
@@ -268,8 +290,10 @@ class MlpTrainer(_TrainOps):
         self.x = x
         a = _raw_in(x)
         for ly in self.layers:
-            self._dense_fwd(ly, a)
-            if ly.bn:
+            if ly.bn and self.frozen:
+                self._bn_frozen(ly)
+            self._dense_fwd(ly, a, not self.frozen)
+            if ly.bn and not self.frozen:
                 self._bn_finalize(ly, ly.rows, bn_decay)
             a = ly.act_in()
         last = self.layers[-1]
@@ -287,7 +311,10 @@ class MlpTrainer(_TrainOps):
             ly = self.layers[i]
             a_in = self.layers[i - 1].act_in() if i > 0 else _raw_in(self.x)
             dx = self.dh[i - 1] if i > 0 else self.d_in
-            self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
+            if self.frozen:
+                self._dense_bwd_input(ly, _grad_dense(ly, dh, True), dx)
+            else:
+                self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
             dh = dx
         return self.d_in
 
@@ -302,19 +329,22 @@ class _MlpFn(torch.autograd.Function):
     def backward(ctx, dout):
         tr = ctx.trainer
         dx = tr.backward(dout)
-        return _flat_grad_of_layers(tr.fp, tr.layers), dx.clone(), None, None
+        return (None if tr.frozen else _flat_grad_of_layers(tr.fp, tr.layers)), dx.clone(), None, None
 
 
-def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore) -> torch.Tensor:
+def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False) -> torch.Tensor:
     """Training-mode shared MLP with autograd: x (..., C_in) -> (..., C_out); layers = [(scope, bn), ...].  Buffers are cached on
-    `params` per (scopes, shape)."""
+    `params` per (scopes, shape).  frozen=True: inference mode (moving averages, input gradient only)."""
     shape = x.shape
     rows = x.numel() // shape[-1]
-    key = ("mlp", tuple(layers), rows, shape[-1])
+    key = ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1])
     cache = params.__dict__.setdefault("_trainers", {})
     if key not in cache:
-        cache[key] = MlpTrainer(params, rows, shape[-1], list(layers), device=x.device)
+        cache[key] = MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen)
     tr = cache[key]
+    if frozen:
+        out = _MlpFn.apply(None, x.reshape(rows, shape[-1]).contiguous(), tr, 0.0)
+        return out.view(*shape[:-1], out.shape[-1])
     tr.fp.flat.requires_grad_(True)
     out = _MlpFn.apply(tr.fp.flat, x.reshape(rows, shape[-1]).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
     return out.view(*shape[:-1], out.shape[-1])
@@ -488,12 +518,16 @@ def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, pa
 
 
 class PointNet2ClsTrainer(_TrainOps):
-    """Training engine of pointnet2_cls_ssg (or any stack of LevelSpec + FC head with the same structure)."""
+    """Training engine of pointnet2_cls_ssg (or any stack of LevelSpec + FC head with the same structure).
+
+    frozen=True: inference-mode differentiation -- batch norm on the moving averages (never updated), no dropout, the same
+    forward kernels; the backward gives input gradients only (coordinates, features) and leaves the flat gradient bucket alone."""
 
     def __init__(self, params: VariableStore, batch: int, npoints: int, num_class: int = 15, levels=None, head=None,
-                 device=None, process_group=None, in_channels: int = 0):
+                 device=None, process_group=None, in_channels: int = 0, frozen: bool = False):
         self.lib = _lib.load()
         self.params = params
+        self.frozen = frozen
         self.dev = torch.device(device) if device is not None else params.device
         self.B, self.N0, self.num_class = batch, npoints, num_class
         self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
@@ -526,11 +560,16 @@ class PointNet2ClsTrainer(_TrainOps):
             lv.pooled = torch.empty((batch * m, sp.mlp[-1]), **f32)
             lv.argk = torch.empty((batch * m, sp.mlp[-1]), dtype=torch.int32, device=dev)
             lv.dh = [torch.empty((rows, sp.mlp[i]), **f32) for i in range(L - 1)]
+            lv.dxyz = torch.empty((batch * n, 3), **f32)
             if sp.group_all:
                 lv.x_cat = torch.empty((batch * n, 3 + c), **f32)
                 if c:
                     lv.d_in = torch.empty((batch * n, c), **f32)
             else:
+                lv.dnew = torch.empty((batch * m, 3), **f32)
+                ws_bytes = max(ws_bytes, lib.psa_sa_conv1_bwd_xyz_workspace_bytes(batch, n, m, k), lib.psa_scatter_workspace_bytes(batch, n, m))
+                if frozen:
+                    lv.dW_scratch = torch.empty((3, sp.mlp[0]), **f32)
                 lv.idx = torch.empty((batch, m, k), dtype=torch.int32, device=dev)
                 lv.cnt = torch.empty((batch, m), dtype=torch.int32, device=dev)
                 c1 = sp.mlp[0]
@@ -549,7 +588,7 @@ class PointNet2ClsTrainer(_TrainOps):
             width = width if width is not None else num_class
             ly = _Layer(self.fp, scope, batch, bn, dev)
             assert ly.K == cin and ly.N == width, (scope, ly.W.shape)
-            if keep is not None:
+            if keep is not None and not frozen:          # no dropout in inference mode
                 ly.mask = torch.ones((batch, width), **f32)
             self.head.append(ly)
             self.keep.append(keep)
@@ -573,11 +612,16 @@ class PointNet2ClsTrainer(_TrainOps):
                 ly.mask.copy_((r < keep).to(torch.float32) / keep)
 
     # ------------------------------------------------------------------------------------------------
-    def forward(self, xyz: torch.Tensor, bn_decay: float = 0.5, points: torch.Tensor | None = None) -> torch.Tensor:
+    def forward(self, xyz: torch.Tensor, bn_decay: float = 0.5, points: torch.Tensor | None = None, sampled=None) -> torch.Tensor:
         """Training-mode forward (batch statistics, moving averages updated with `bn_decay`) -> logits (B, num_class); without a head
-        -> the last level's pooled features (B*m, C).  `points` (B, N, in_channels): input features of the first level."""
+        -> the last level's pooled features (B*m, C).  `points` (B, N, in_channels): input features of the first level.  `sampled`:
+        (fps_idx, new_xyz) of the first level, already sampled by the caller.  A frozen trainer ignores `bn_decay`."""
         lib = self.lib
         B = self.B
+        frozen = self.frozen
+        if frozen:
+            for ly in [ly for lv in self.levels for ly in lv.layers] + [ly for ly in self.head if ly.bn]:
+                self._bn_frozen(ly)
         assert xyz.shape == (B, self.N0, 3) and xyz.is_cuda and xyz.dtype == torch.float32
         assert (points is None) == (self.in_channels == 0), "points must be given exactly when the trainer was built with in_channels > 0"
         cur_xyz, cur_pts = xyz.contiguous(), None
@@ -594,18 +638,23 @@ class PointNet2ClsTrainer(_TrainOps):
                 lv.x_cat[:, :3].copy_(cur_xyz.reshape(-1, 3))
                 if cur_pts is not None:
                     lv.x_cat[:, 3:].copy_(cur_pts.reshape(B * lv.n, -1))
-                self._dense_fwd(L0, _raw_in(lv.x_cat))
+                self._dense_fwd(L0, _raw_in(lv.x_cat), not frozen)
                 lv.new_xyz = torch.zeros((B, 1, 3), dtype=torch.float32, device=self.dev)
             else:
-                _, lv.new_xyz = ops.farthest_point_sample_and_gather(lv.m, cur_xyz)
+                if sampled is not None and lv is self.levels[0]:
+                    lv.fps_idx, lv.new_xyz = sampled
+                else:
+                    lv.fps_idx, lv.new_xyz = ops.farthest_point_sample_and_gather(lv.m, cur_xyz)
                 self._c(lib.psa_sa_conv1_prebn(B, lv.n, lv.m, lv.c_in, C.c_float(sp.radius), lv.k, _p(cur_xyz), _p(lv.new_xyz), _p(cur_pts),
-                                               _p(L0.W), _p(L0.b), L0.N, _p(L0.y), _p(lv.idx), _p(lv.cnt), _p(L0.stats), _p(self.ws),
-                                               C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_prebn")
-            self._bn_finalize(L0, L0.rows, bn_decay)
+                                               _p(L0.W), _p(L0.b), L0.N, _p(L0.y), _p(lv.idx), _p(lv.cnt), None if frozen else _p(L0.stats),
+                                               _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_prebn")
+            if not frozen:
+                self._bn_finalize(L0, L0.rows, bn_decay)
             prev = L0
             for ly in lv.layers[1:]:
-                self._dense_fwd(ly, prev.act_in())
-                self._bn_finalize(ly, ly.rows, bn_decay)
+                self._dense_fwd(ly, prev.act_in(), not frozen)
+                if not frozen:
+                    self._bn_finalize(ly, ly.rows, bn_decay)
                 prev = ly
             self._c(lib.psa_train_pool_fwd(B * lv.m, lv.k, prev.N, _p(prev.y), _p(prev.scale), _p(prev.shift), _p(lv.pooled), _p(lv.argk),
                                            _stream()), "train_pool_fwd")
@@ -615,17 +664,20 @@ class PointNet2ClsTrainer(_TrainOps):
             return feat
         a = _raw_in(feat)
         for ly in self.head:
-            self._dense_fwd(ly, a)
-            if ly.bn:
+            self._dense_fwd(ly, a, not frozen)
+            if ly.bn and not frozen:
                 self._bn_finalize(ly, ly.rows, bn_decay)
             a = ly.act_in()
         return self.head[-1].y
 
     # ------------------------------------------------------------------------------------------------
-    def backward(self, dlogits: torch.Tensor):
-        """Gradients of every trainable variable for d(loss)/d(logits) = dlogits, into the flat gradient bucket."""
+    def backward(self, dlogits: torch.Tensor, xyz_grad: bool = False):
+        """Gradients of every trainable variable for d(loss)/d(logits) = dlogits, into the flat gradient bucket (a frozen trainer: input
+        gradients only, the bucket is not touched).  xyz_grad: also each level's coordinate parts (lv.dxyz, lv.dnew; see
+        input_xyz_grad); nothing else changes with it."""
         lib = self.lib
         B = self.B
+        frozen = self.frozen
         # ---- head ----  (a bare level stack: dlogits is the gradient of the last level's pooled features)
         dh = dlogits.contiguous()
         if not self.head:
@@ -635,7 +687,10 @@ class PointNet2ClsTrainer(_TrainOps):
             ly = self.head[i]
             a_in = self.head[i - 1].act_in() if i > 0 else _raw_in(feat)
             dx = self.head_dh[i - 1] if i > 0 else self.d_feat
-            self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
+            if frozen:
+                self._dense_bwd_input(ly, _grad_dense(ly, dh, True), dx)
+            else:
+                self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
             dh = dx
         # ---- set-abstraction levels, last to first ----
         dpool = self.d_feat
@@ -652,7 +707,10 @@ class PointNet2ClsTrainer(_TrainOps):
                 else:
                     g0 = _grad_dense(ly, lv.dh[l], False)
                     g1 = _grad_dense(ly, lv.dh[l], True)
-                self._layer_bwd(ly, g0, g1, lv.layers[l - 1].act_in(), lv.dh[l - 1])
+                if frozen:
+                    self._dense_bwd_input(ly, g1, lv.dh[l - 1])
+                else:
+                    self._layer_bwd(ly, g0, g1, lv.layers[l - 1].act_in(), lv.dh[l - 1])
             L0 = lv.layers[0]
             if L == 1:
                 g0 = _grad_pooled(L0, dpool, lv.pooled, lv.argk, lv.k, False)
@@ -661,22 +719,56 @@ class PointNet2ClsTrainer(_TrainOps):
                 g0 = _grad_dense(L0, lv.dh[0], False)
                 g1 = _grad_dense(L0, lv.dh[0], True)
             if sp.group_all:
-                self._layer_bwd(L0, g0, g1, _raw_in(lv.x_cat), lv.d_in, col_skip=3)
+                if frozen:
+                    if lv.d_in is not None:
+                        self._dense_bwd_input(L0, g1, lv.d_in, col_skip=3)
+                else:
+                    self._layer_bwd(L0, g0, g1, _raw_in(lv.x_cat), lv.d_in, col_skip=3)
+                if xyz_grad:
+                    # the coordinate columns of dx: a second product over the first three rows of W (the feature columns above are unchanged)
+                    self._c(lib.psa_train_dense_bwd_input(L0.rows, 3, L0.N, C.byref(g1), _p(L0.W), _p(lv.dxyz), 3, 0, _p(self.ws),
+                                                          C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
             else:
-                self._c(lib.psa_bn_bwd_coeffs(L0.rows, L0.N, C.byref(g0), _p(L0.gamma), _p(L0.mean_inv), _p(L0.dgamma), _p(L0.dbeta),
-                                              _p(L0.ca), _p(L0.cb), _p(L0.cc), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "bn_bwd_coeffs")
-                L0.db.zero_()
-                self._c(lib.psa_sa_conv1_bwd(B, lv.n, lv.m, lv.k, L0.N, _p(cur_xyz), _p(lv.new_xyz), _p(lv.idx), C.byref(g1), _p(L0.dW[:3]),
-                                             _p(lv.dU), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_bwd")
+                if not frozen:
+                    self._c(lib.psa_bn_bwd_coeffs(L0.rows, L0.N, C.byref(g0), _p(L0.gamma), _p(L0.mean_inv), _p(L0.dgamma), _p(L0.dbeta),
+                                                  _p(L0.ca), _p(L0.cb), _p(L0.cc), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "bn_bwd_coeffs")
+                    L0.db.zero_()
+                if not frozen or lv.c_in:
+                    # frozen: only for dU (the dW_xyz it also writes goes to scratch)
+                    self._c(lib.psa_sa_conv1_bwd(B, lv.n, lv.m, lv.k, L0.N, _p(cur_xyz), _p(lv.new_xyz), _p(lv.idx), C.byref(g1),
+                                                 _p(lv.dW_scratch if frozen else L0.dW[:3]), _p(lv.dU), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                 _stream()), "sa_conv1_bwd")
                 if lv.c_in:
                     pts = cur_pts.reshape(B * lv.n, lv.c_in)
                     gU = _plain_grad(lv.dU)
                     wf = L0.W[3:]
-                    self._c(lib.psa_train_dense_bwd_weight(B * lv.n, lv.c_in, L0.N, C.byref(_raw_in(pts)), C.byref(gU), _p(L0.dW[3:]), _p(self.ws),
-                                                           C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_weight")
+                    if not frozen:
+                        self._c(lib.psa_train_dense_bwd_weight(B * lv.n, lv.c_in, L0.N, C.byref(_raw_in(pts)), C.byref(gU), _p(L0.dW[3:]),
+                                                               _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_weight")
                     self._c(lib.psa_train_dense_bwd_input(B * lv.n, lv.c_in, L0.N, C.byref(gU), _p(wf), _p(lv.d_in), lv.c_in, 0, _p(self.ws),
                                                           C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
+                if xyz_grad:
+                    self._c(lib.psa_sa_conv1_bwd_xyz(B, lv.n, lv.m, lv.k, L0.N, _p(L0.W), _p(lv.idx), C.byref(g1), _p(lv.dxyz), _p(lv.dnew),
+                                                     _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_bwd_xyz")
             dpool = lv.d_in
+
+    def input_xyz_grad(self) -> torch.Tensor:
+        """After backward(..., xyz_grad=True): the gradient w.r.t. the input cloud (B, N0, 3).  Levels last to first:
+        d new_xyz = this level's -sum term + the next level's input-coordinate gradient, then d xyz_in = the rows' GroupPointGrad +
+        GatherPointGrad(d new_xyz, fps_idx).  The group-all level's new_xyz is the constant origin."""
+        lib, B = self.lib, self.B
+        dnext = None
+        for lv in reversed(self.levels):
+            if lv.spec.group_all:
+                d = lv.dxyz
+            else:
+                dn = lv.dnew if dnext is None else lv.dnew + dnext.view(-1, 3)
+                gp = torch.empty_like(lv.dxyz)
+                self._c(lib.psa_gather_point_grad(B, lv.n, lv.m, _p(dn), _p(lv.fps_idx), _p(gp), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                  _stream()), "gather_point_grad")
+                d = gp.add_(lv.dxyz)
+            dnext = d
+        return dnext.view(B, self.N0, 3)
 
     # ------------------------------------------------------------------------------------------------
     def loss_and_grad(self, logits: torch.Tensor, labels: torch.Tensor):
@@ -709,7 +801,8 @@ class PointNet2ClsTrainer(_TrainOps):
 
 
 class _TrainFn(torch.autograd.Function):
-    """get_model(is_training=True) for autograd users: logits whose backward fills the flat gradient bucket."""
+    """get_model(is_training=True) for autograd users: logits whose backward fills the flat gradient bucket, and gives the gradient
+    of the input cloud when it requires one.  A frozen trainer (inference mode) is applied with flat=None: input gradient only."""
 
     @staticmethod
     def forward(ctx, flat, trainer, xyz, bn_decay):
@@ -719,59 +812,87 @@ class _TrainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dlogits):
         tr = ctx.trainer
-        tr.backward(dlogits.contiguous())
-        return tr.fp.grad.clone(), None, None, None
+        want_xyz = ctx.needs_input_grad[2]
+        tr.backward(dlogits.contiguous(), xyz_grad=want_xyz)
+        dxyz = tr.input_xyz_grad().clone() if want_xyz else None
+        return (None if tr.frozen else tr.fp.grad.clone()), None, dxyz, None
 
 
 class _LevelFn(torch.autograd.Function):
     """One pointnet_sa_module(is_training=True): pooled features whose backward returns the gradient of the input features and
-    of this level's variables (a flat bucket that is zero outside the level -- several levels may share one store)."""
+    of this level's variables (a flat bucket that is zero outside the level -- several levels may share one store), and, when
+    asked for, the level's coordinate parts: the rows' GroupPointGrad for xyz and the "- new_xyz" term for new_xyz (new_xyz itself
+    comes from the differentiable gather_point, so autograd adds GatherPointGrad and whatever later levels send).  A frozen
+    trainer (inference mode) gives input gradients only (flat=None)."""
 
     @staticmethod
-    def forward(ctx, flat, points, trainer, xyz, bn_decay):
+    def forward(ctx, flat, points, xyz, new_xyz, trainer, bn_decay, fps_idx):
         ctx.trainer = trainer
         ctx.has_points = points is not None
-        out = trainer.forward(xyz, bn_decay, points)
+        sampled = None if fps_idx is None else (fps_idx, new_xyz.detach().contiguous())
+        out = trainer.forward(xyz.contiguous(), bn_decay, points, sampled=sampled)
         lv = trainer.levels[-1]
         return out.clone().view(trainer.B, lv.m, -1)
 
     @staticmethod
     def backward(ctx, dout):
         tr = ctx.trainer
-        tr.backward(dout.contiguous())
-        g = _flat_grad_of_layers(tr.fp, [ly for lv in tr.levels for ly in lv.layers])
-        dp = tr.levels[0].d_in.view(tr.B, tr.N0, tr.in_channels).clone() if ctx.has_points else None
-        return g, dp, None, None, None
+        need = ctx.needs_input_grad
+        want_xyz = need[2] or need[3]
+        tr.backward(dout.contiguous(), xyz_grad=want_xyz)
+        g = None if tr.frozen else _flat_grad_of_layers(tr.fp, [ly for lv in tr.levels for ly in lv.layers])
+        lv = tr.levels[0]
+        dp = lv.d_in.view(tr.B, tr.N0, tr.in_channels).clone() if ctx.has_points and need[1] else None
+        dxyz = lv.dxyz.view(tr.B, tr.N0, 3).clone() if need[2] else None
+        dnew = lv.dnew.view(tr.B, lv.m, 3).clone() if need[3] and not lv.spec.group_all else None
+        return g, dp, dxyz, dnew, None, None, None
 
 
-def sa_module_training(xyz, points, spec: LevelSpec, bn_decay, params: VariableStore):
+def wants_input_grad(*tensors) -> bool:
+    """inference-mode calls take the frozen-batch-norm autograd path when gradients are being recorded and an input asks for one"""
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+def sa_module_training(xyz, points, spec: LevelSpec, bn_decay, params: VariableStore, frozen: bool = False):
     """Training-mode pointnet_sa_module (max pooling, use_xyz): -> (new_xyz, new_points (B,m,C) with a grad_fn, idx).  The level's
     buffers are cached on `params` per (scope, shape); gradients of its variables arrive in `params._flat.grad_of(name)` /
-    through autograd on `params._flat.flat`, the gradient of `points` through autograd."""
+    through autograd on `params._flat.flat`, the gradients of `points` and `xyz` through autograd.  frozen=True: inference mode
+    (batch norm on the moving averages, which stay put; input gradients only)."""
     b, n, _ = xyz.shape
     c = 0 if points is None else points.shape[-1]
-    key = ("level", spec.scope, b, n, c, spec.npoint, spec.radius, spec.nsample, tuple(spec.mlp), spec.group_all)
+    key = ("level_frozen" if frozen else "level", spec.scope, b, n, c, spec.npoint, spec.radius, spec.nsample, tuple(spec.mlp), spec.group_all)
     cache = params.__dict__.setdefault("_trainers", {})
     if key not in cache:
-        cache[key] = PointNet2ClsTrainer(params, b, n, levels=[spec], head=[], device=xyz.device, in_channels=c)
+        cache[key] = PointNet2ClsTrainer(params, b, n, levels=[spec], head=[], device=xyz.device, in_channels=c, frozen=frozen)
     tr = cache[key]
-    tr.fp.flat.requires_grad_(True)
-    out = _LevelFn.apply(tr.fp.flat, points, tr, xyz, 0.5 if bn_decay is None else float(bn_decay))
+    if not frozen:
+        tr.fp.flat.requires_grad_(True)
+    if spec.group_all:
+        fps_idx, new_xyz = None, None
+    else:
+        fps_idx, new_xyz = ops.farthest_point_sample_and_gather(spec.npoint, xyz)
+        if wants_input_grad(xyz):
+            new_xyz = ops.gather_point(xyz, fps_idx)       # same values as the fused gather, differentiable (GatherPointGrad)
+    out = _LevelFn.apply(None if frozen else tr.fp.flat, points, xyz, new_xyz, tr, 0.5 if bn_decay is None else float(bn_decay), fps_idx)
     lv = tr.levels[0]
     idx = lv.idx
     if spec.group_all:            # sample_and_group_all: one group holding every point in order (pointnet_util.py:75-77)
         idx = torch.arange(n, dtype=torch.int32, device=xyz.device).view(1, 1, n).repeat(b, 1, 1)
-    return lv.new_xyz, out, idx
+        new_xyz = lv.new_xyz
+    return new_xyz, out, idx
 
 
-def get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, levels=None, head=None):
-    """Training-mode forward of the classifier; the trainer (buffers, flat parameter bucket) is cached on `params`."""
-    key = (tuple(point_cloud.shape), num_class)
+def get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, levels=None, head=None, frozen: bool = False):
+    """Training-mode forward of the classifier; the trainer (buffers, flat parameter bucket) is cached on `params`.  frozen=True:
+    inference-mode forward (moving averages, no dropout) whose backward gives the gradient of the input cloud only."""
+    key = (tuple(point_cloud.shape), num_class) if not frozen else ("frozen", tuple(point_cloud.shape), num_class)
     cache = params.__dict__.setdefault("_trainers", {})
     if key not in cache:
         cache[key] = PointNet2ClsTrainer(params, point_cloud.shape[0], point_cloud.shape[1], num_class, levels=levels, head=head,
-                                         device=point_cloud.device)
+                                         device=point_cloud.device, frozen=frozen)
     tr = cache[key]
+    if frozen:
+        return _TrainFn.apply(None, tr, point_cloud, 0.0), tr
     tr.fp.flat.requires_grad_(True)
     tr.draw_dropout()
     return _TrainFn.apply(tr.fp.flat, tr, point_cloud, 0.5 if bn_decay is None else float(bn_decay)), tr
