@@ -30,12 +30,11 @@ def init_params(num_class=NUM_CLASSES, seed=0, device="cuda", randomize_bn=False
 
 
 def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *, params: VariableStore, return_end_points: bool = False):
-    if is_training:
-        return _get_model_training(point_cloud, bn_decay, num_class, params, return_end_points)
     from .training import wants_input_grad
-    if wants_input_grad(point_cloud):
-        # inference mode with an input gradient: the training kernels with batch norm on the moving averages, no dropout
-        return _get_model_training(point_cloud, bn_decay, num_class, params, return_end_points, dropout=False, frozen=True)
+    frozen = not is_training and wants_input_grad(point_cloud)
+    if is_training or frozen:
+        # frozen: inference mode with an input gradient -- the training kernels with batch norm on the moving averages, no dropout
+        return _get_model_training(point_cloud, bn_decay, num_class, params, return_end_points, dropout=not frozen, frozen=frozen)
     batch_size = point_cloud.shape[0]
     end_points = {}
     l0_xyz = point_cloud[:, :, 0:3].contiguous()

@@ -71,26 +71,20 @@ def pointnet_sa_module(xyz, points, npoint, radius, nsample, mlp, mlp2, group_al
     xyz))), e.g. on a side stream -- FPS of level l+1 only depends on level l's centroids, not on its features."""
     if pooling not in ("max", "avg", "weighted_avg", "max_and_avg"):
         raise ValueError(f"unknown pooling {pooling!r}")
-    if is_training:
-        # batch-statistics batch norm + autograd through the level (training.py); the configuration the in-scope models train with
-        if not (pooling == "max" and mlp2 is None and use_xyz and not knn and bn and new_xyz is None):
-            raise NotImplementedError("pointnet_sa_module(is_training=True) covers max pooling, use_xyz, ball query, bn=True, no mlp2 "
-                                      "(what pointnet2_cls_ssg / _bga train with); other configurations run in inference mode only")
-        from .training import LevelSpec, sa_module_training
-        spec = LevelSpec(scope, None if group_all else npoint, None if group_all else radius, None if group_all else nsample, list(mlp),
-                         group_all=bool(group_all))
-        return sa_module_training(xyz, points, spec, bn_decay, params)
     from .training import wants_input_grad
-    if wants_input_grad(xyz, points):
-        # inference mode with an input gradient (saliency, adversarial perturbation): the training kernels with batch norm on the
-        # moving averages (training.py, frozen=True); calls that need no gradient stay on the fused kernels below
+    frozen = not is_training and wants_input_grad(xyz, points)
+    if is_training or frozen:
+        # batch-statistics batch norm + autograd through the level (training.py); the configuration the in-scope models train with.
+        # frozen: inference mode with an input gradient (saliency, adversarial perturbation) -- the same kernels with batch norm on the
+        # moving averages; calls that need no gradient stay on the fused kernels below
         if not (pooling == "max" and mlp2 is None and use_xyz and not knn and bn and new_xyz is None):
-            raise NotImplementedError("input gradients of pointnet_sa_module(is_training=False) cover max pooling, use_xyz, ball query, "
-                                      "bn=True, no mlp2 and no caller-sampled new_xyz")
+            raise NotImplementedError("pointnet_sa_module(is_training=True) and input gradients of pointnet_sa_module(is_training=False) "
+                                      "cover max pooling, use_xyz, ball query, bn=True, no mlp2 and no caller-sampled new_xyz (what "
+                                      "pointnet2_cls_ssg / _bga train with); other configurations run in inference mode without gradients")
         from .training import LevelSpec, sa_module_training
         spec = LevelSpec(scope, None if group_all else npoint, None if group_all else radius, None if group_all else nsample, list(mlp),
                          group_all=bool(group_all))
-        return sa_module_training(xyz, points, spec, bn_decay, params, frozen=True)
+        return sa_module_training(xyz, points, spec, bn_decay, params, frozen=frozen)
     scopes = _mlp_scopes(scope, mlp)
     if pooling != "max":
         # pointnet_util.py:128-146 -- unused by the in-scope models, so the grouped rows are materialised: group -> per-row

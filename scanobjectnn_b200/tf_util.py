@@ -119,11 +119,7 @@ def _require_inference(is_training):
             "(training.py: sa_module_training, mlp_training, PointNet2ClsTrainer) -- see INTEGRATION.md")
 
 
-def _wants_input_grad(inputs):
-    return torch.is_grad_enabled() and inputs.requires_grad
-
-
-def _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=False):
+def _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen):
     """one conv / fully-connected layer in training mode (training.mlp_training): conv+BN+ReLU or a plain linear layer.
     frozen=True: inference mode with an input gradient (batch norm on the moving averages)."""
     if bn and activation_fn is not None:
@@ -141,10 +137,10 @@ def conv2d(inputs, num_output_channels, kernel_size, scope, stride=(1, 1), paddi
     """tf_util.conv2d restricted to what the hot path uses: 1x1 kernels, stride 1, NHWC, ReLU or None."""
     if tuple(kernel_size) != (1, 1) or tuple(stride) != (1, 1) or data_format != "NHWC":
         raise NotImplementedError("only 1x1 / stride-1 / NHWC convolutions are on the point-set-abstraction path")
-    if is_training:
-        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params)
-    if _wants_input_grad(inputs):
-        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=True)
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(inputs)        # inference mode with an input gradient: frozen batch norm
+    if is_training or frozen:
+        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen)
     relu = activation_fn is not None
     mlp = params.mlp([scope], [relu])
     if mlp.channels[-1] != num_output_channels:
@@ -154,10 +150,10 @@ def conv2d(inputs, num_output_channels, kernel_size, scope, stride=(1, 1), paddi
 
 def fully_connected(inputs, num_outputs, scope, activation_fn="relu", bn=False, bn_decay=None, is_training=False, *,
                     params: VariableStore):
-    if is_training:
-        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params)
-    if _wants_input_grad(inputs):
-        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen=True)
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(inputs)        # inference mode with an input gradient: frozen batch norm
+    if is_training or frozen:
+        return _layer_training(inputs, scope, activation_fn, bn, bn_decay, params, frozen)
     relu = activation_fn is not None
     mlp = params.mlp([scope], [relu])
     if mlp.channels[-1] != num_outputs:

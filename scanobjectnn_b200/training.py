@@ -119,56 +119,36 @@ class _Layer:
             self.ca = torch.empty(self.N, **f32)
             self.cb = torch.empty(self.N, **f32)
             self.cc = torch.empty(self.N, **f32)
+        else:
+            self.scale = self.shift = self.ca = self.cb = self.cc = None
         self.mask = None      # dropout mask applied to this layer's OUTPUT (rows, N), or None
 
     def act_in(self) -> PsaActIn:
         """this layer's output as the next layer's input"""
-        a = PsaActIn()
-        a.x = self.y.data_ptr(); a.ld = self.N
-        if self.bn:
-            a.scale = self.scale.data_ptr(); a.shift = self.shift.data_ptr(); a.relu = 1
-        else:
-            a.scale = None; a.shift = None; a.relu = 0
-        a.mask = self.mask.data_ptr() if self.mask is not None else None
-        return a
+        return PsaActIn(x=_p(self.y), ld=self.N, scale=_p(self.scale), shift=_p(self.shift), mask=_p(self.mask), relu=int(self.bn))
 
 
+# psa_act_in / psa_grad_in descriptors: fields not named are 0 / NULL
 def _raw_in(x: torch.Tensor) -> PsaActIn:
-    a = PsaActIn()
-    a.x = x.data_ptr(); a.ld = x.shape[-1]; a.scale = None; a.shift = None; a.mask = None; a.relu = 0
-    return a
+    return PsaActIn(x=_p(x), ld=x.shape[-1])
 
 
-def _grad_dense(layer: _Layer, dh: torch.Tensor, with_coeffs: bool) -> PsaGradIn:
-    g = PsaGradIn()
-    g.y = layer.y.data_ptr(); g.ld = layer.N
-    if layer.bn:
-        g.s = layer.scale.data_ptr(); g.t = layer.shift.data_ptr(); g.relu = 1
-    else:
-        g.s = None; g.t = None; g.relu = 0
-    if layer.bn and with_coeffs:
-        g.ca = layer.ca.data_ptr(); g.cb = layer.cb.data_ptr(); g.cc = layer.cc.data_ptr()
-    else:
-        g.ca = None; g.cb = None; g.cc = None
-    g.dh = dh.data_ptr(); g.ld_dh = dh.shape[-1]
-    g.mask = layer.mask.data_ptr() if layer.mask is not None else None
-    g.dp = None; g.pv = None; g.argk = None; g.pool_k = 1; g.C = layer.N; g.mode = 0
-    return g
+def _grad_in(ly: _Layer, **dz) -> PsaGradIn:
+    """dy of layer `ly` with its batch-norm coefficients (psa_bn_bwd_coeffs ignores them and fills them in); dz's source in `dz`"""
+    return PsaGradIn(y=_p(ly.y), ld=ly.N, s=_p(ly.scale), t=_p(ly.shift), relu=int(ly.bn), ca=_p(ly.ca), cb=_p(ly.cb), cc=_p(ly.cc),
+                     C=ly.N, **dz)
 
 
-def _grad_pooled(layer: _Layer, dp: torch.Tensor, pv: torch.Tensor, argk: torch.Tensor, pool_k: int, with_coeffs: bool) -> PsaGradIn:
-    g = _grad_dense(layer, dp, with_coeffs)
-    g.dh = None; g.ld_dh = 0; g.mask = None
-    g.dp = dp.data_ptr(); g.pv = pv.data_ptr(); g.argk = argk.data_ptr(); g.pool_k = pool_k; g.C = layer.N; g.mode = 1
-    return g
+def _grad_dense(ly: _Layer, dh: torch.Tensor) -> PsaGradIn:
+    return _grad_in(ly, dh=_p(dh), ld_dh=dh.shape[-1], mask=_p(ly.mask), pool_k=1)
+
+
+def _grad_pooled(ly: _Layer, dp: torch.Tensor, pv: torch.Tensor, argk: torch.Tensor, pool_k: int) -> PsaGradIn:
+    return _grad_in(ly, dp=_p(dp), pv=_p(pv), argk=_p(argk), pool_k=pool_k, mode=1)
 
 
 def _plain_grad(dh: torch.Tensor) -> PsaGradIn:
-    g = PsaGradIn()
-    g.y = None; g.ld = 0; g.s = None; g.t = None; g.relu = 0; g.ca = None; g.cb = None; g.cc = None
-    g.dh = dh.data_ptr(); g.ld_dh = dh.shape[-1]; g.mask = None
-    g.dp = None; g.pv = None; g.argk = None; g.pool_k = 1; g.C = dh.shape[-1]; g.mode = 0
-    return g
+    return PsaGradIn(dh=_p(dh), ld_dh=dh.shape[-1], pool_k=1, C=dh.shape[-1])
 
 
 @dataclass
@@ -195,50 +175,88 @@ class _Level:
 
 
 class _TrainOps:
-    """Per-layer training operations shared by the trainers below (they provide self.lib, self.ws, self.ws_bytes)."""
+    """Per-layer training operations shared by the trainers below (they provide self.ws, self.ws_bytes).
 
-    def _c(self, rc, what):
-        check(rc, what)
+    frozen=True: inference-mode batch norm -- the moving averages (never updated) folded into every layer at the start of each
+    forward, no batch statistics or psa_bn_finalize, and a backward of input products only that leaves the flat gradient
+    bucket alone."""
+
+    def __init__(self, params: VariableStore, device, frozen: bool):
+        self.lib = _lib.load()
+        self.params = params
+        self.frozen = frozen
+        self.dev = torch.device(device) if device is not None else params.device
+        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
+        params._flat = self.fp
 
     def _bn_finalize(self, ly: _Layer, count: int, decay: float):
-        self._c(self.lib.psa_bn_finalize(ly.N, count, _p(ly.stats), _p(ly.gamma), _p(ly.beta), C.c_float(decay), _p(ly.mov_mean),
-                                         _p(ly.mov_var), _p(ly.scale), _p(ly.shift), _p(ly.mean_inv), _stream()), "bn_finalize")
+        """batch statistics over `count` rows -> scale / shift, moving averages updated; nothing without batch statistics"""
+        if ly.bn and not self.frozen:
+            check(self.lib.psa_bn_finalize(ly.N, count, _p(ly.stats), _p(ly.gamma), _p(ly.beta), C.c_float(decay), _p(ly.mov_mean),
+                                           _p(ly.mov_var), _p(ly.scale), _p(ly.shift), _p(ly.mean_inv), _stream()), "bn_finalize")
 
-    def _dense_fwd(self, ly: _Layer, a: PsaActIn, stats: bool = True):
-        self._c(self.lib.psa_train_dense_fwd(ly.rows, ly.K, ly.N, C.byref(a), _p(ly.W), _p(ly.b), _p(ly.y),
-                                             _p(ly.stats) if ly.bn and stats else None, _p(self.ws), C.c_size_t(self.ws_bytes), _stream()),
-                "train_dense_fwd")
+    def _layer_fwd(self, ly: _Layer, a: PsaActIn, decay: float):
+        """y = a . W + b (+ batch statistics), then batch norm's scale / shift"""
+        check(self.lib.psa_train_dense_fwd(ly.rows, ly.K, ly.N, C.byref(a), _p(ly.W), _p(ly.b), _p(ly.y),
+                                           _p(ly.stats) if ly.bn and not self.frozen else None, _p(self.ws), C.c_size_t(self.ws_bytes),
+                                           _stream()), "train_dense_fwd")
+        self._bn_finalize(ly, ly.rows, decay)
 
-    @staticmethod
-    def _bn_frozen(ly: _Layer):
+    def _chain_fwd(self, layers, a: PsaActIn, decay: float):
+        """a chain of dense layers on input `a`; the output is layers[-1].y"""
+        for ly in layers:
+            self._layer_fwd(ly, a, decay)
+            a = ly.act_in()
+
+    def _fold_frozen(self, layers):
         """inference-mode batch norm: the moving averages folded into scale / shift (VariableStore.folded's arithmetic), and the
         backward coefficients dy = scale * dz (ca = scale, cb = cc = 0).  The moving averages are read, never written."""
-        inv = ly.gamma * torch.rsqrt(ly.mov_var + BN_EPS)
-        ly.scale.copy_(inv)
-        ly.shift.copy_(ly.beta - ly.mov_mean * inv)
-        ly.ca.copy_(inv)
-        ly.cb.zero_()
-        ly.cc.zero_()
+        if not self.frozen:
+            return
+        for ly in layers:
+            if ly.bn:
+                inv = ly.gamma * torch.rsqrt(ly.mov_var + BN_EPS)
+                ly.scale.copy_(inv)
+                ly.shift.copy_(ly.beta - ly.mov_mean * inv)
+                ly.ca.copy_(inv)
+                ly.cb.zero_()
+                ly.cc.zero_()
 
-    def _dense_bwd_input(self, ly: _Layer, g: PsaGradIn, dx: torch.Tensor, col_skip: int = 0):
-        self._c(self.lib.psa_train_dense_bwd_input(ly.rows, ly.K, ly.N, C.byref(g), _p(ly.W), _p(dx), dx.shape[-1], col_skip, _p(self.ws),
-                                                   C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
-
-    def _layer_bwd(self, ly: _Layer, g_nocoef: PsaGradIn, g: PsaGradIn, a_in: PsaActIn, dx: torch.Tensor | None, col_skip: int = 0):
-        """gradients of one conv/fc(+BN+relu) layer: BN sums/coefficients, dW, (db), dx."""
-        lib = self.lib
+    def _bn_bwd(self, ly: _Layer, g: PsaGradIn):
+        """batch-norm sums and dy's coefficients, or the bias gradient of a layer without batch norm; nothing when frozen"""
+        if self.frozen:
+            return
         if ly.bn:
-            self._c(lib.psa_bn_bwd_coeffs(ly.rows, ly.N, C.byref(g_nocoef), _p(ly.gamma), _p(ly.mean_inv), _p(ly.dgamma), _p(ly.dbeta),
-                                          _p(ly.ca), _p(ly.cb), _p(ly.cc), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "bn_bwd_coeffs")
+            check(self.lib.psa_bn_bwd_coeffs(ly.rows, ly.N, C.byref(g), _p(ly.gamma), _p(ly.mean_inv), _p(ly.dgamma), _p(ly.dbeta),
+                                             _p(ly.ca), _p(ly.cb), _p(ly.cc), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "bn_bwd_coeffs")
             ly.db.zero_()          # sum_r dy = 0 under batch norm
         else:
-            self._c(lib.psa_train_bias_grad(ly.rows, ly.N, C.byref(g), _p(ly.db), _stream()), "train_bias_grad")
-        if a_in is not None:
-            self._c(lib.psa_train_dense_bwd_weight(ly.rows, ly.K, ly.N, C.byref(a_in), C.byref(g), _p(ly.dW), _p(self.ws), C.c_size_t(self.ws_bytes),
-                                                   _stream()), "train_dense_bwd_weight")
+            check(self.lib.psa_train_bias_grad(ly.rows, ly.N, C.byref(g), _p(ly.db), _stream()), "train_bias_grad")
+
+    def _products(self, g: PsaGradIn, rows: int, K: int, N: int, W, dW, a_in: PsaActIn | None, dx: torch.Tensor | None, col_skip: int = 0):
+        """dW (K, N) = a_in^T . dy (not when frozen) and dx = dy . W^T over the input columns >= col_skip; None skips either"""
+        if a_in is not None and not self.frozen:
+            check(self.lib.psa_train_dense_bwd_weight(rows, K, N, C.byref(a_in), C.byref(g), _p(dW), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                      _stream()), "train_dense_bwd_weight")
         if dx is not None:
-            self._c(lib.psa_train_dense_bwd_input(ly.rows, ly.K, ly.N, C.byref(g), _p(ly.W), _p(dx), dx.shape[-1], col_skip, _p(self.ws),
-                                                  C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
+            check(self.lib.psa_train_dense_bwd_input(rows, K, N, C.byref(g), _p(W), _p(dx), dx.shape[-1], col_skip, _p(self.ws),
+                                                     C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
+
+    def _layer_bwd(self, ly: _Layer, g: PsaGradIn, a_in: PsaActIn | None, dx: torch.Tensor | None, col_skip: int = 0):
+        """gradients of one conv/fc(+BN+relu) layer: BN sums/coefficients or db, dW, dx."""
+        self._bn_bwd(ly, g)
+        self._products(g, ly.rows, ly.K, ly.N, ly.W, ly.dW, a_in, dx, col_skip)
+
+    def _chain_bwd(self, layers, g: PsaGradIn, dh, a0: PsaActIn, dx: torch.Tensor):
+        """backward of a chain of dense layers: g = the top layer's dy, dh[l] = buffer for the gradient w.r.t. layer l's output
+        (l < L-1), a0 = the first layer's input, dx = where the gradient w.r.t. a0 goes"""
+        for i in range(len(layers) - 1, -1, -1):
+            if i < len(layers) - 1:
+                g = _grad_dense(layers[i], dh[i])
+            if i > 0:
+                self._layer_bwd(layers[i], g, layers[i - 1].act_in(), dh[i - 1])
+            else:
+                self._layer_bwd(layers[i], g, a0, dx)
 
 
 def _flat_grad_of_layers(fp: FlatParams, layers) -> torch.Tensor:
@@ -259,12 +277,7 @@ class MlpTrainer(_TrainOps):
     moving averages (never updated), and a backward that gives the input gradient only."""
 
     def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None, frozen: bool = False):
-        self.lib = _lib.load()
-        self.params = params
-        self.frozen = frozen
-        self.dev = torch.device(device) if device is not None else params.device
-        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
-        params._flat = self.fp
+        super().__init__(params, device, frozen)
         self.rows, self.in_channels = rows, in_channels
         f32 = dict(dtype=torch.float32, device=self.dev)
         self.layers: list[_Layer] = []
@@ -288,48 +301,55 @@ class MlpTrainer(_TrainOps):
     def forward(self, x: torch.Tensor, bn_decay: float = 0.5) -> torch.Tensor:
         assert x.shape == (self.rows, self.in_channels) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
         self.x = x
-        a = _raw_in(x)
-        for ly in self.layers:
-            if ly.bn and self.frozen:
-                self._bn_frozen(ly)
-            self._dense_fwd(ly, a, not self.frozen)
-            if ly.bn and not self.frozen:
-                self._bn_finalize(ly, ly.rows, bn_decay)
-            a = ly.act_in()
+        self._fold_frozen(self.layers)
+        self._chain_fwd(self.layers, _raw_in(x), bn_decay)
         last = self.layers[-1]
         if not last.bn:
             return last.y
         # the stack's output is the activated tensor: relu(BN(y)) through the pooling kernel with runs of one row
-        self._c(self.lib.psa_train_pool_fwd(self.rows, 1, last.N, _p(last.y), _p(last.scale), _p(last.shift), _p(self.out), _p(self.argk),
-                                            _stream()), "train_pool_fwd")
+        check(self.lib.psa_train_pool_fwd(self.rows, 1, last.N, _p(last.y), _p(last.scale), _p(last.shift), _p(self.out), _p(self.argk),
+                                          _stream()), "train_pool_fwd")
         return self.out
 
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
         """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x; the layers' gradients go to the flat bucket"""
-        dh = dout.contiguous()
-        for i in range(len(self.layers) - 1, -1, -1):
-            ly = self.layers[i]
-            a_in = self.layers[i - 1].act_in() if i > 0 else _raw_in(self.x)
-            dx = self.dh[i - 1] if i > 0 else self.d_in
-            if self.frozen:
-                self._dense_bwd_input(ly, _grad_dense(ly, dh, True), dx)
-            else:
-                self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
-            dh = dx
+        dout = dout.contiguous()
+        self._chain_bwd(self.layers, _grad_dense(self.layers[-1], dout), self.dh, _raw_in(self.x), self.d_in)
         return self.d_in
 
 
-class _MlpFn(torch.autograd.Function):
+class _NodeFn(torch.autograd.Function):
+    """An MlpTrainer / EdgeConvTrainer / EdgeConv2Trainer as one autograd node: trainer.forward(x, *args, bn_decay), whose backward
+    returns the gradient of x and of the trainer's variables (a flat bucket that is zero outside them: several nodes share one
+    store; a frozen trainer is applied with flat=None and gives the input gradient only)."""
+
     @staticmethod
-    def forward(ctx, flat, x, trainer, bn_decay):
-        ctx.trainer = trainer
-        return trainer.forward(x, bn_decay).clone()
+    def forward(ctx, flat, x, trainer, args, bn_decay):
+        ctx.trainer, ctx.x_shape = trainer, x.shape
+        return trainer.forward(x, *args, bn_decay).clone()
 
     @staticmethod
     def backward(ctx, dout):
         tr = ctx.trainer
         dx = tr.backward(dout)
-        return (None if tr.frozen else _flat_grad_of_layers(tr.fp, tr.layers)), dx.clone(), None, None
+        return (None if tr.frozen else _flat_grad_of_layers(tr.fp, tr.layers)), dx.view(ctx.x_shape).clone(), None, None, None
+
+
+def _cached(params: VariableStore, key, make):
+    """the trainer cached on `params` under `key`, made on first use (its buffers are allocated once per configuration and shape)"""
+    cache = params.__dict__.setdefault("_trainers", {})
+    if key not in cache:
+        cache[key] = make()
+    return cache[key]
+
+
+def _flat_and_decay(tr: _TrainOps, bn_decay):
+    """the autograd input that carries the variables' gradients and the moving-average decay (tf_util's default 0.5 for None);
+    (None, 0.0) for a frozen trainer, which neither updates nor differentiates the variables"""
+    if tr.frozen:
+        return None, 0.0
+    tr.fp.flat.requires_grad_(True)
+    return tr.fp.flat, 0.5 if bn_decay is None else float(bn_decay)
 
 
 def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False) -> torch.Tensor:
@@ -337,16 +357,10 @@ def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, froze
     `params` per (scopes, shape).  frozen=True: inference mode (moving averages, input gradient only)."""
     shape = x.shape
     rows = x.numel() // shape[-1]
-    key = ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1])
-    cache = params.__dict__.setdefault("_trainers", {})
-    if key not in cache:
-        cache[key] = MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen)
-    tr = cache[key]
-    if frozen:
-        out = _MlpFn.apply(None, x.reshape(rows, shape[-1]).contiguous(), tr, 0.0)
-        return out.view(*shape[:-1], out.shape[-1])
-    tr.fp.flat.requires_grad_(True)
-    out = _MlpFn.apply(tr.fp.flat, x.reshape(rows, shape[-1]).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
+    tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1]),
+                 lambda: MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen))
+    flat, decay = _flat_and_decay(tr, bn_decay)
+    out = _NodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), tr, (), decay)
     return out.view(*shape[:-1], out.shape[-1])
 
 
@@ -356,13 +370,10 @@ class EdgeConvTrainer(_TrainOps):
     Batch statistics over all b*n*k edges; the max's gradient is split evenly among tied edges, as torch.amax / TF reduce_max do."""
 
     def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scope: str, device=None):
-        self.lib = _lib.load()
-        self.params = params
-        self.dev = torch.device(device) if device is not None else params.device
-        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
-        params._flat = self.fp
+        super().__init__(params, device, False)
         self.b, self.n, self.c, self.k = b, n, c, k
-        self.layer = ly = _Layer(self.fp, scope, 0, True, self.dev)       # rows = 0: the per-edge activations are never stored
+        ly = _Layer(self.fp, scope, 0, True, self.dev)       # rows = 0: the per-edge activations are never stored
+        self.layers = [ly]
         if ly.K != 2 * c:
             raise ValueError(f"{scope}: weights of shape {tuple(ly.W.shape)}, an EdgeConv over {c} channels needs ({2 * c}, C_out)")
         rows, N = b * n, ly.N
@@ -377,39 +388,26 @@ class EdgeConvTrainer(_TrainOps):
         self.ws = torch.empty(self.ws_bytes // 4 + 64, **f32)
 
     def forward(self, x: torch.Tensor, nn_idx: torch.Tensor, bn_decay: float = 0.5) -> torch.Tensor:
-        b, n, c, k, ly = self.b, self.n, self.c, self.k, self.layer
+        b, n, c, k, (ly,) = self.b, self.n, self.c, self.k, self.layers
         assert x.shape == (b, n, c) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
         assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
         self.x, self.nn_idx = x, nn_idx
-        self._c(self.lib.psa_edgeconv_train_fwd(b, n, c, k, ly.N, _p(x), _p(nn_idx), _p(ly.W), _p(ly.b), _p(self.PQ), _p(ly.stats), _p(self.ws),
-                                                C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_fwd")
+        check(self.lib.psa_edgeconv_train_fwd(b, n, c, k, ly.N, _p(x), _p(nn_idx), _p(ly.W), _p(ly.b), _p(self.PQ), _p(ly.stats), _p(self.ws),
+                                              C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_fwd")
         self._bn_finalize(ly, b * n * k, bn_decay)
-        self._c(self.lib.psa_edgeconv_train_pool(b, n, k, ly.N, _p(nn_idx), _p(self.PQ), _p(ly.scale), _p(ly.shift), _p(self.pooled), _p(self.ties),
-                                                 _stream()), "edgeconv_train_pool")
+        check(self.lib.psa_edgeconv_train_pool(b, n, k, ly.N, _p(nn_idx), _p(self.PQ), _p(ly.scale), _p(ly.shift), _p(self.pooled), _p(self.ties),
+                                               _stream()), "edgeconv_train_pool")
         return self.pooled
 
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
         """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); the layer's gradients go to the flat bucket"""
-        b, n, c, k, ly = self.b, self.n, self.c, self.k, self.layer
+        b, n, c, k, (ly,) = self.b, self.n, self.c, self.k, self.layers
         dout = dout.contiguous()
-        self._c(self.lib.psa_edgeconv_train_bwd(b, n, c, k, ly.N, _p(self.x), _p(self.nn_idx), _p(ly.W), _p(self.PQ), _p(ly.scale), _p(ly.shift),
-                                                _p(ly.gamma), _p(ly.mean_inv), _p(self.pooled), _p(self.ties), _p(dout), _p(ly.dW), _p(ly.dgamma),
-                                                _p(ly.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_bwd")
+        check(self.lib.psa_edgeconv_train_bwd(b, n, c, k, ly.N, _p(self.x), _p(self.nn_idx), _p(ly.W), _p(self.PQ), _p(ly.scale), _p(ly.shift),
+                                              _p(ly.gamma), _p(ly.mean_inv), _p(self.pooled), _p(self.ties), _p(dout), _p(ly.dW), _p(ly.dgamma),
+                                              _p(ly.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_bwd")
         ly.db.zero_()          # sum over the edges of dy = 0 under batch norm
         return self.d_in
-
-
-class _EdgeConvFn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, flat, x, nn_idx, trainer, bn_decay):
-        ctx.trainer = trainer
-        return trainer.forward(x, nn_idx, bn_decay).clone()
-
-    @staticmethod
-    def backward(ctx, dout):
-        tr = ctx.trainer
-        dx = tr.backward(dout)
-        return _flat_grad_of_layers(tr.fp, [tr.layer]), dx.view(tr.b, tr.n, tr.c).clone(), None, None, None
 
 
 class EdgeConv2Trainer(_TrainOps):
@@ -419,11 +417,7 @@ class EdgeConv2Trainer(_TrainOps):
     b*n*k edges in both layers; the max's gradient is split evenly among tied edges."""
 
     def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scopes, device=None):
-        self.lib = _lib.load()
-        self.params = params
-        self.dev = torch.device(device) if device is not None else params.device
-        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
-        params._flat = self.fp
+        super().__init__(params, device, False)
         self.b, self.n, self.c, self.k = b, n, c, k
         self.layers = [_Layer(self.fp, s, 0, True, self.dev) for s in scopes]     # rows = 0: the per-edge activations are never stored
         l1, l2 = self.layers
@@ -451,15 +445,15 @@ class EdgeConv2Trainer(_TrainOps):
         assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
         self.x, self.nn_idx = x, nn_idx
         lib, ws, wsb = self.lib, _p(self.ws), C.c_size_t(self.ws_bytes)
-        self._c(lib.psa_edgeconv_train_fwd(b, n, c, k, l1.N, _p(x), _p(nn_idx), _p(l1.W), _p(l1.b), _p(self.PQ), _p(l1.stats), ws, wsb, _stream()),
-                "edgeconv_train_fwd")
+        check(lib.psa_edgeconv_train_fwd(b, n, c, k, l1.N, _p(x), _p(nn_idx), _p(l1.W), _p(l1.b), _p(self.PQ), _p(l1.stats), ws, wsb, _stream()),
+              "edgeconv_train_fwd")
         self._bn_finalize(l1, b * n * k, bn_decay)
-        self._c(lib.psa_edgeconv2_train_fwd(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
-                                            _p(l2.stats), ws, wsb, _stream()), "edgeconv2_train_fwd")
+        check(lib.psa_edgeconv2_train_fwd(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
+                                          _p(l2.stats), ws, wsb, _stream()), "edgeconv2_train_fwd")
         self._bn_finalize(l2, b * n * k, bn_decay)
-        self._c(lib.psa_edgeconv2_train_pool(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
-                                             _p(l2.scale), _p(l2.shift), _p(self.pooled), _p(self.mask), _p(self.ywin), ws, wsb, _stream()),
-                "edgeconv2_train_pool")
+        check(lib.psa_edgeconv2_train_pool(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
+                                           _p(l2.scale), _p(l2.shift), _p(self.pooled), _p(self.mask), _p(self.ywin), ws, wsb, _stream()),
+              "edgeconv2_train_pool")
         return self.pooled
 
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
@@ -467,27 +461,14 @@ class EdgeConv2Trainer(_TrainOps):
         b, n, c, k = self.b, self.n, self.c, self.k
         l1, l2 = self.layers
         dout = dout.contiguous()
-        self._c(self.lib.psa_edgeconv2_train_bwd(b, n, c, k, l1.N, l2.N, _p(self.x), _p(self.nn_idx), _p(l1.W), _p(self.PQ), _p(l1.scale),
-                                                 _p(l1.shift), _p(l1.gamma), _p(l1.mean_inv), _p(l2.W), _p(l2.b), _p(l2.gamma), _p(l2.mean_inv),
-                                                 _p(self.pooled), _p(self.mask), _p(self.ywin), _p(dout), _p(l1.dW), _p(l1.dgamma), _p(l1.dbeta),
-                                                 _p(l2.dW), _p(l2.dgamma), _p(l2.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes),
-                                                 _stream()), "edgeconv2_train_bwd")
+        check(self.lib.psa_edgeconv2_train_bwd(b, n, c, k, l1.N, l2.N, _p(self.x), _p(self.nn_idx), _p(l1.W), _p(self.PQ), _p(l1.scale),
+                                               _p(l1.shift), _p(l1.gamma), _p(l1.mean_inv), _p(l2.W), _p(l2.b), _p(l2.gamma), _p(l2.mean_inv),
+                                               _p(self.pooled), _p(self.mask), _p(self.ywin), _p(dout), _p(l1.dW), _p(l1.dgamma), _p(l1.dbeta),
+                                               _p(l2.dW), _p(l2.dgamma), _p(l2.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                               _stream()), "edgeconv2_train_bwd")
         l1.db.zero_()          # sum over the edges of dy = 0 under batch norm, in both layers
         l2.db.zero_()
         return self.d_in
-
-
-class _EdgeConv2Fn(torch.autograd.Function):
-    @staticmethod
-    def forward(ctx, flat, x, nn_idx, trainer, bn_decay):
-        ctx.trainer = trainer
-        return trainer.forward(x, nn_idx, bn_decay).clone()
-
-    @staticmethod
-    def backward(ctx, dout):
-        tr = ctx.trainer
-        dx = tr.backward(dout)
-        return _flat_grad_of_layers(tr.fp, tr.layers), dx.view(tr.b, tr.n, tr.c).clone(), None, None, None
 
 
 def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, params: VariableStore) -> torch.Tensor:
@@ -500,20 +481,12 @@ def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, pa
     scopes = (scope,) if isinstance(scope, str) else tuple(scope)
     if len(scopes) not in (1, 2):
         raise ValueError(f"edgeconv_training: one or two scopes, got {len(scopes)}")
-    cache = params.__dict__.setdefault("_trainers", {})
     if len(scopes) == 1:
-        key = ("edgeconv", scopes[0], b, n, c, k)
-        if key not in cache:
-            cache[key] = EdgeConvTrainer(params, b, n, c, k, scopes[0], device=x.device)
-        fn = _EdgeConvFn
+        tr = _cached(params, ("edgeconv", scopes[0], b, n, c, k), lambda: EdgeConvTrainer(params, b, n, c, k, scopes[0], device=x.device))
     else:
-        key = ("edgeconv2", scopes, b, n, c, k)
-        if key not in cache:
-            cache[key] = EdgeConv2Trainer(params, b, n, c, k, scopes, device=x.device)
-        fn = _EdgeConv2Fn
-    tr = cache[key]
-    tr.fp.flat.requires_grad_(True)
-    out = fn.apply(tr.fp.flat, x.contiguous(), nn_idx.to(torch.int32).contiguous(), tr, 0.5 if bn_decay is None else float(bn_decay))
+        tr = _cached(params, ("edgeconv2", scopes, b, n, c, k), lambda: EdgeConv2Trainer(params, b, n, c, k, scopes, device=x.device))
+    flat, decay = _flat_and_decay(tr, bn_decay)
+    out = _NodeFn.apply(flat, x.contiguous(), tr, (nn_idx.to(torch.int32).contiguous(),), decay)
     return out.view(b, n, -1)
 
 
@@ -525,13 +498,8 @@ class PointNet2ClsTrainer(_TrainOps):
 
     def __init__(self, params: VariableStore, batch: int, npoints: int, num_class: int = 15, levels=None, head=None,
                  device=None, process_group=None, in_channels: int = 0, frozen: bool = False):
-        self.lib = _lib.load()
-        self.params = params
-        self.frozen = frozen
-        self.dev = torch.device(device) if device is not None else params.device
+        super().__init__(params, device, frozen)
         self.B, self.N0, self.num_class = batch, npoints, num_class
-        self.fp = params._flat if getattr(params, "_flat", None) is not None else FlatParams(params)
-        params._flat = self.fp
         self.pg = process_group
         self.world = torch.distributed.get_world_size(process_group) if (process_group is not None or
                                                                           (torch.distributed.is_available() and torch.distributed.is_initialized())) else 1
@@ -616,12 +584,8 @@ class PointNet2ClsTrainer(_TrainOps):
         """Training-mode forward (batch statistics, moving averages updated with `bn_decay`) -> logits (B, num_class); without a head
         -> the last level's pooled features (B*m, C).  `points` (B, N, in_channels): input features of the first level.  `sampled`:
         (fps_idx, new_xyz) of the first level, already sampled by the caller.  A frozen trainer ignores `bn_decay`."""
-        lib = self.lib
         B = self.B
-        frozen = self.frozen
-        if frozen:
-            for ly in [ly for lv in self.levels for ly in lv.layers] + [ly for ly in self.head if ly.bn]:
-                self._bn_frozen(ly)
+        self._fold_frozen([ly for lv in self.levels for ly in lv.layers] + self.head)
         assert xyz.shape == (B, self.N0, 3) and xyz.is_cuda and xyz.dtype == torch.float32
         assert (points is None) == (self.in_channels == 0), "points must be given exactly when the trainer was built with in_channels > 0"
         cur_xyz, cur_pts = xyz.contiguous(), None
@@ -638,36 +602,26 @@ class PointNet2ClsTrainer(_TrainOps):
                 lv.x_cat[:, :3].copy_(cur_xyz.reshape(-1, 3))
                 if cur_pts is not None:
                     lv.x_cat[:, 3:].copy_(cur_pts.reshape(B * lv.n, -1))
-                self._dense_fwd(L0, _raw_in(lv.x_cat), not frozen)
+                self._layer_fwd(L0, _raw_in(lv.x_cat), bn_decay)
                 lv.new_xyz = torch.zeros((B, 1, 3), dtype=torch.float32, device=self.dev)
             else:
                 if sampled is not None and lv is self.levels[0]:
                     lv.fps_idx, lv.new_xyz = sampled
                 else:
                     lv.fps_idx, lv.new_xyz = ops.farthest_point_sample_and_gather(lv.m, cur_xyz)
-                self._c(lib.psa_sa_conv1_prebn(B, lv.n, lv.m, lv.c_in, C.c_float(sp.radius), lv.k, _p(cur_xyz), _p(lv.new_xyz), _p(cur_pts),
-                                               _p(L0.W), _p(L0.b), L0.N, _p(L0.y), _p(lv.idx), _p(lv.cnt), None if frozen else _p(L0.stats),
-                                               _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_prebn")
-            if not frozen:
+                check(self.lib.psa_sa_conv1_prebn(B, lv.n, lv.m, lv.c_in, C.c_float(sp.radius), lv.k, _p(cur_xyz), _p(lv.new_xyz), _p(cur_pts),
+                                                  _p(L0.W), _p(L0.b), L0.N, _p(L0.y), _p(lv.idx), _p(lv.cnt), None if self.frozen else _p(L0.stats),
+                                                  _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_prebn")
                 self._bn_finalize(L0, L0.rows, bn_decay)
-            prev = L0
-            for ly in lv.layers[1:]:
-                self._dense_fwd(ly, prev.act_in(), not frozen)
-                if not frozen:
-                    self._bn_finalize(ly, ly.rows, bn_decay)
-                prev = ly
-            self._c(lib.psa_train_pool_fwd(B * lv.m, lv.k, prev.N, _p(prev.y), _p(prev.scale), _p(prev.shift), _p(lv.pooled), _p(lv.argk),
-                                           _stream()), "train_pool_fwd")
+            self._chain_fwd(lv.layers[1:], L0.act_in(), bn_decay)
+            top = lv.layers[-1]
+            check(self.lib.psa_train_pool_fwd(B * lv.m, lv.k, top.N, _p(top.y), _p(top.scale), _p(top.shift), _p(lv.pooled), _p(lv.argk),
+                                              _stream()), "train_pool_fwd")
             cur_xyz, cur_pts = lv.new_xyz, lv.pooled.view(B, lv.m, -1)
         feat = self.levels[-1].pooled                                   # (B, C)
         if not self.head:
             return feat
-        a = _raw_in(feat)
-        for ly in self.head:
-            self._dense_fwd(ly, a, not frozen)
-            if ly.bn and not frozen:
-                self._bn_finalize(ly, ly.rows, bn_decay)
-            a = ly.act_in()
+        self._chain_fwd(self.head, _raw_in(feat), bn_decay)
         return self.head[-1].y
 
     # ------------------------------------------------------------------------------------------------
@@ -675,88 +629,49 @@ class PointNet2ClsTrainer(_TrainOps):
         """Gradients of every trainable variable for d(loss)/d(logits) = dlogits, into the flat gradient bucket (a frozen trainer: input
         gradients only, the bucket is not touched).  xyz_grad: also each level's coordinate parts (lv.dxyz, lv.dnew; see
         input_xyz_grad); nothing else changes with it."""
-        lib = self.lib
         B = self.B
-        frozen = self.frozen
         # ---- head ----  (a bare level stack: dlogits is the gradient of the last level's pooled features)
         dh = dlogits.contiguous()
-        if not self.head:
+        if self.head:
+            self._chain_bwd(self.head, _grad_dense(self.head[-1], dh), self.head_dh, _raw_in(self.levels[-1].pooled), self.d_feat)
+        else:
             self.d_feat.copy_(dh.reshape(self.d_feat.shape))
-        feat = self.levels[-1].pooled
-        for i in range(len(self.head) - 1, -1, -1):
-            ly = self.head[i]
-            a_in = self.head[i - 1].act_in() if i > 0 else _raw_in(feat)
-            dx = self.head_dh[i - 1] if i > 0 else self.d_feat
-            if frozen:
-                self._dense_bwd_input(ly, _grad_dense(ly, dh, True), dx)
-            else:
-                self._layer_bwd(ly, _grad_dense(ly, dh, False), _grad_dense(ly, dh, True), a_in, dx)
-            dh = dx
         # ---- set-abstraction levels, last to first ----
         dpool = self.d_feat
         for li in range(len(self.levels) - 1, -1, -1):
             lv = self.levels[li]
-            sp = lv.spec
-            L = len(lv.layers)
             cur_xyz, cur_pts = self.in_xyz[li]
-            for l in range(L - 1, 0, -1):
-                ly = lv.layers[l]
-                if l == L - 1:
-                    g0 = _grad_pooled(ly, dpool, lv.pooled, lv.argk, lv.k, False)
-                    g1 = _grad_pooled(ly, dpool, lv.pooled, lv.argk, lv.k, True)
-                else:
-                    g0 = _grad_dense(ly, lv.dh[l], False)
-                    g1 = _grad_dense(ly, lv.dh[l], True)
-                if frozen:
-                    self._dense_bwd_input(ly, g1, lv.dh[l - 1])
-                else:
-                    self._layer_bwd(ly, g0, g1, lv.layers[l - 1].act_in(), lv.dh[l - 1])
             L0 = lv.layers[0]
-            if L == 1:
-                g0 = _grad_pooled(L0, dpool, lv.pooled, lv.argk, lv.k, False)
-                g1 = _grad_pooled(L0, dpool, lv.pooled, lv.argk, lv.k, True)
-            else:
-                g0 = _grad_dense(L0, lv.dh[0], False)
-                g1 = _grad_dense(L0, lv.dh[0], True)
-            if sp.group_all:
-                if frozen:
-                    if lv.d_in is not None:
-                        self._dense_bwd_input(L0, g1, lv.d_in, col_skip=3)
-                else:
-                    self._layer_bwd(L0, g0, g1, _raw_in(lv.x_cat), lv.d_in, col_skip=3)
+            g = _grad_pooled(lv.layers[-1], dpool, lv.pooled, lv.argk, lv.k)
+            if len(lv.layers) > 1:
+                self._chain_bwd(lv.layers[1:], g, lv.dh[1:], L0.act_in(), lv.dh[0])
+                g = _grad_dense(L0, lv.dh[0])
+            if lv.spec.group_all:
+                self._layer_bwd(L0, g, _raw_in(lv.x_cat), lv.d_in, col_skip=3)
                 if xyz_grad:
                     # the coordinate columns of dx: a second product over the first three rows of W (the feature columns above are unchanged)
-                    self._c(lib.psa_train_dense_bwd_input(L0.rows, 3, L0.N, C.byref(g1), _p(L0.W), _p(lv.dxyz), 3, 0, _p(self.ws),
-                                                          C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
+                    self._products(g, L0.rows, 3, L0.N, L0.W, None, None, lv.dxyz)
             else:
-                if not frozen:
-                    self._c(lib.psa_bn_bwd_coeffs(L0.rows, L0.N, C.byref(g0), _p(L0.gamma), _p(L0.mean_inv), _p(L0.dgamma), _p(L0.dbeta),
-                                                  _p(L0.ca), _p(L0.cb), _p(L0.cc), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "bn_bwd_coeffs")
-                    L0.db.zero_()
-                if not frozen or lv.c_in:
+                self._bn_bwd(L0, g)
+                if not self.frozen or lv.c_in:
                     # frozen: only for dU (the dW_xyz it also writes goes to scratch)
-                    self._c(lib.psa_sa_conv1_bwd(B, lv.n, lv.m, lv.k, L0.N, _p(cur_xyz), _p(lv.new_xyz), _p(lv.idx), C.byref(g1),
-                                                 _p(lv.dW_scratch if frozen else L0.dW[:3]), _p(lv.dU), _p(self.ws), C.c_size_t(self.ws_bytes),
-                                                 _stream()), "sa_conv1_bwd")
+                    check(self.lib.psa_sa_conv1_bwd(B, lv.n, lv.m, lv.k, L0.N, _p(cur_xyz), _p(lv.new_xyz), _p(lv.idx), C.byref(g),
+                                                    _p(lv.dW_scratch if self.frozen else L0.dW[:3]), _p(lv.dU), _p(self.ws),
+                                                    C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_bwd")
                 if lv.c_in:
-                    pts = cur_pts.reshape(B * lv.n, lv.c_in)
-                    gU = _plain_grad(lv.dU)
-                    wf = L0.W[3:]
-                    if not frozen:
-                        self._c(lib.psa_train_dense_bwd_weight(B * lv.n, lv.c_in, L0.N, C.byref(_raw_in(pts)), C.byref(gU), _p(L0.dW[3:]),
-                                                               _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_weight")
-                    self._c(lib.psa_train_dense_bwd_input(B * lv.n, lv.c_in, L0.N, C.byref(gU), _p(wf), _p(lv.d_in), lv.c_in, 0, _p(self.ws),
-                                                          C.c_size_t(self.ws_bytes), _stream()), "train_dense_bwd_input")
+                    # the feature rows of W: two dense products on the source points, dU = GroupPointGrad of dy
+                    self._products(_plain_grad(lv.dU), B * lv.n, lv.c_in, L0.N, L0.W[3:], L0.dW[3:], _raw_in(cur_pts.reshape(B * lv.n, lv.c_in)),
+                                   lv.d_in)
                 if xyz_grad:
-                    self._c(lib.psa_sa_conv1_bwd_xyz(B, lv.n, lv.m, lv.k, L0.N, _p(L0.W), _p(lv.idx), C.byref(g1), _p(lv.dxyz), _p(lv.dnew),
-                                                     _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_bwd_xyz")
+                    check(self.lib.psa_sa_conv1_bwd_xyz(B, lv.n, lv.m, lv.k, L0.N, _p(L0.W), _p(lv.idx), C.byref(g), _p(lv.dxyz), _p(lv.dnew),
+                                                        _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "sa_conv1_bwd_xyz")
             dpool = lv.d_in
 
     def input_xyz_grad(self) -> torch.Tensor:
         """After backward(..., xyz_grad=True): the gradient w.r.t. the input cloud (B, N0, 3).  Levels last to first:
         d new_xyz = this level's -sum term + the next level's input-coordinate gradient, then d xyz_in = the rows' GroupPointGrad +
         GatherPointGrad(d new_xyz, fps_idx).  The group-all level's new_xyz is the constant origin."""
-        lib, B = self.lib, self.B
+        B = self.B
         dnext = None
         for lv in reversed(self.levels):
             if lv.spec.group_all:
@@ -764,8 +679,8 @@ class PointNet2ClsTrainer(_TrainOps):
             else:
                 dn = lv.dnew if dnext is None else lv.dnew + dnext.view(-1, 3)
                 gp = torch.empty_like(lv.dxyz)
-                self._c(lib.psa_gather_point_grad(B, lv.n, lv.m, _p(dn), _p(lv.fps_idx), _p(gp), _p(self.ws), C.c_size_t(self.ws_bytes),
-                                                  _stream()), "gather_point_grad")
+                check(self.lib.psa_gather_point_grad(B, lv.n, lv.m, _p(dn), _p(lv.fps_idx), _p(gp), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                     _stream()), "gather_point_grad")
                 d = gp.add_(lv.dxyz)
             dnext = d
         return dnext.view(B, self.N0, 3)
@@ -773,7 +688,7 @@ class PointNet2ClsTrainer(_TrainOps):
     # ------------------------------------------------------------------------------------------------
     def loss_and_grad(self, logits: torch.Tensor, labels: torch.Tensor):
         """mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) -> loss (1,) and d loss / d logits."""
-        self._c(self.lib.psa_softmax_xent(self.B, self.num_class, _p(logits), _p(labels), _p(self.loss), _p(self.dlogits), _stream()), "softmax_xent")
+        check(self.lib.psa_softmax_xent(self.B, self.num_class, _p(logits), _p(labels), _p(self.loss), _p(self.dlogits), _stream()), "softmax_xent")
         return self.loss, self.dlogits
 
     def allreduce_grads(self):
@@ -784,8 +699,8 @@ class PointNet2ClsTrainer(_TrainOps):
     def adam(self, lr: float, beta1=0.9, beta2=0.999, eps=1e-8):
         fp = self.fp
         fp.step_count += 1
-        self._c(self.lib.psa_adam_step(fp.total, _p(fp.flat), _p(fp.grad), _p(fp.adam_m), _p(fp.adam_v), C.c_float(lr), C.c_float(beta1),
-                                       C.c_float(beta2), C.c_float(eps), fp.step_count, C.c_float(1.0 / self.world), _stream()), "adam_step")
+        check(self.lib.psa_adam_step(fp.total, _p(fp.flat), _p(fp.grad), _p(fp.adam_m), _p(fp.adam_v), C.c_float(lr), C.c_float(beta1),
+                                     C.c_float(beta2), C.c_float(eps), fp.step_count, C.c_float(1.0 / self.world), _stream()), "adam_step")
         self.params.invalidate()
 
     def train_step(self, xyz: torch.Tensor, labels: torch.Tensor, lr: float = 1e-3, bn_decay: float = 0.5, dropout: bool = True):
@@ -861,19 +776,15 @@ def sa_module_training(xyz, points, spec: LevelSpec, bn_decay, params: VariableS
     b, n, _ = xyz.shape
     c = 0 if points is None else points.shape[-1]
     key = ("level_frozen" if frozen else "level", spec.scope, b, n, c, spec.npoint, spec.radius, spec.nsample, tuple(spec.mlp), spec.group_all)
-    cache = params.__dict__.setdefault("_trainers", {})
-    if key not in cache:
-        cache[key] = PointNet2ClsTrainer(params, b, n, levels=[spec], head=[], device=xyz.device, in_channels=c, frozen=frozen)
-    tr = cache[key]
-    if not frozen:
-        tr.fp.flat.requires_grad_(True)
+    tr = _cached(params, key, lambda: PointNet2ClsTrainer(params, b, n, levels=[spec], head=[], device=xyz.device, in_channels=c, frozen=frozen))
+    flat, decay = _flat_and_decay(tr, bn_decay)
     if spec.group_all:
         fps_idx, new_xyz = None, None
     else:
         fps_idx, new_xyz = ops.farthest_point_sample_and_gather(spec.npoint, xyz)
         if wants_input_grad(xyz):
             new_xyz = ops.gather_point(xyz, fps_idx)       # same values as the fused gather, differentiable (GatherPointGrad)
-    out = _LevelFn.apply(None if frozen else tr.fp.flat, points, xyz, new_xyz, tr, 0.5 if bn_decay is None else float(bn_decay), fps_idx)
+    out = _LevelFn.apply(flat, points, xyz, new_xyz, tr, decay, fps_idx)
     lv = tr.levels[0]
     idx = lv.idx
     if spec.group_all:            # sample_and_group_all: one group holding every point in order (pointnet_util.py:75-77)
@@ -886,13 +797,9 @@ def get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, 
     """Training-mode forward of the classifier; the trainer (buffers, flat parameter bucket) is cached on `params`.  frozen=True:
     inference-mode forward (moving averages, no dropout) whose backward gives the gradient of the input cloud only."""
     key = (tuple(point_cloud.shape), num_class) if not frozen else ("frozen", tuple(point_cloud.shape), num_class)
-    cache = params.__dict__.setdefault("_trainers", {})
-    if key not in cache:
-        cache[key] = PointNet2ClsTrainer(params, point_cloud.shape[0], point_cloud.shape[1], num_class, levels=levels, head=head,
-                                         device=point_cloud.device, frozen=frozen)
-    tr = cache[key]
-    if frozen:
-        return _TrainFn.apply(None, tr, point_cloud, 0.0), tr
-    tr.fp.flat.requires_grad_(True)
-    tr.draw_dropout()
-    return _TrainFn.apply(tr.fp.flat, tr, point_cloud, 0.5 if bn_decay is None else float(bn_decay)), tr
+    tr = _cached(params, key, lambda: PointNet2ClsTrainer(params, point_cloud.shape[0], point_cloud.shape[1], num_class, levels=levels,
+                                                          head=head, device=point_cloud.device, frozen=frozen))
+    flat, decay = _flat_and_decay(tr, bn_decay)
+    if not frozen:
+        tr.draw_dropout()
+    return _TrainFn.apply(flat, tr, point_cloud, decay), tr
