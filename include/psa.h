@@ -420,7 +420,9 @@ PSA_API int psa_sa_conv1_bwd_xyz(int b, int n, int m, int nsample, int C1, const
  * calls: psa_edgeconv_train_workspace_bytes() bytes, 256-byte aligned.  Every reduction runs in a fixed order: bit-reproducible.
  *
  * forward 1: PQ (b*n, 2 C_out) and stats (2, C_out) = per-channel [sum y, sum y^2] over the edges; then psa_bn_finalize with
- *            count = b*n*k gives scale, shift, mean_inv and updates the moving averages. */
+ *            count = b*n*k gives scale, shift, mean_inv and updates the moving averages.  stats == NULL: PQ only, for frozen batch
+ *            norm (inference mode: scale = gamma / sqrt(moving_var + 1e-3), shift = beta - moving_mean * scale, computed by the
+ *            caller), whose backward is psa_edgeconv_frozen_bwd. */
 PSA_API size_t psa_edgeconv_train_workspace_bytes(int b, int n, int c, int k, int C_out);
 PSA_API int psa_edgeconv_train_fwd(int b, int n, int c, int k, int C_out, const float* x, const int* nn_idx, const float* W,
                                    const float* bias, float* PQ, float* stats, void* workspace, size_t workspace_bytes,
@@ -437,6 +439,12 @@ PSA_API int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, const 
                                    const float* mean_inv, const float* pooled, const void* ties, const float* dout, float* dW,
                                    float* dgamma, float* dbeta, float* dx, void* workspace, size_t workspace_bytes,
                                    psa_stream_t stream);
+/* backward with frozen batch norm (after psa_edgeconv_train_fwd with stats == NULL and psa_edgeconv_train_pool on the frozen
+ * scale / shift): dout routed to the tied edges of a positive maximum as above, dy = scale * dz -> dx (b*n, c) only; no
+ * batch-norm sums and no variable gradients.  Same limits and workspace as psa_edgeconv_train_bwd. */
+PSA_API int psa_edgeconv_frozen_bwd(int b, int n, int c, int k, int C_out, const float* x, const int* nn_idx, const float* W,
+                                    const float* PQ, const float* scale, const float* shift, const float* pooled, const void* ties,
+                                    const float* dout, float* dx, void* workspace, size_t workspace_bytes, psa_stream_t stream);
 
 /* Training mode of a two-layer EdgeConv (DGCNN's input transform net, transform_nets.py:18-27): out_ic = max_j relu(BN2(relu(BN1(
  * [x_i, x_j - x_i] . W1 + b1)) . W2 + b2)), both batch norms with batch statistics over all E = b*n*k edges.  No per-edge tensor
@@ -467,6 +475,16 @@ PSA_API int psa_edgeconv2_train_bwd(int b, int n, int c, int k, int C1, int C2, 
                                     const float* ywin, const float* dout, float* dW1, float* dgamma1, float* dbeta1, float* dW2,
                                     float* dgamma2, float* dbeta2, float* dx, void* workspace, size_t workspace_bytes,
                                     psa_stream_t stream);
+/* Frozen batch norm (inference mode) in both layers: the forward is psa_edgeconv_train_fwd with stats == NULL followed by
+ * psa_edgeconv2_train_pool on the frozen scale1 / shift1 / scale2 / shift2 (no psa_edgeconv2_train_fwd).  backward: dout routed
+ * to the masked edges of a positive maximum, dy2 = scale2 * dz2, dy1 = scale1 * dz1 -> dx (b*n, c) only; no batch-norm sums and
+ * no variable gradients.  pooled, mask, ywin as the pool wrote them; bias2 may be NULL.  Same limits and workspace as
+ * psa_edgeconv2_train_bwd. */
+PSA_API int psa_edgeconv2_frozen_bwd(int b, int n, int c, int k, int C1, int C2, const float* x, const int* nn_idx,
+                                     const float* W1, const float* PQ, const float* scale1, const float* shift1, const float* W2,
+                                     const float* bias2, const float* scale2, const float* pooled, const unsigned int* mask,
+                                     const float* ywin, const float* dout, float* dx, void* workspace, size_t workspace_bytes,
+                                     psa_stream_t stream);
 
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */

@@ -95,6 +95,8 @@ SIGNATURES = {
     "psa_edgeconv2_train_fwd": [_i, _i, _i, _i, _i, _i, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "psa_edgeconv2_train_pool": [_i, _i, _i, _i, _i, _i] + [_p] * 12 + [_sz, _p],
     "psa_edgeconv2_train_bwd": [_i, _i, _i, _i, _i, _i] + [_p] * 24 + [_sz, _p],
+    "psa_edgeconv_frozen_bwd": [_i, _i, _i, _i, _i] + [_p] * 11 + [_sz, _p],
+    "psa_edgeconv2_frozen_bwd": [_i, _i, _i, _i, _i, _i] + [_p] * 15 + [_sz, _p],
     "psa_softmax_xent": [_i, _i, _p, _p, _p, _p, _p],
     "psa_pool_rows": [_ll, _i, _i, _i, _p, _p, _p, _p],
     "psa_adam_step": [_ll, _p, _p, _p, _p, _f, _f, _f, _f, _i, _f, _p],

@@ -388,21 +388,25 @@ __global__ void __launch_bounds__(kE2Threads, 1) edge2_train_kernel(E2Args a) {
 }
 
 // layer 2's batch-norm sums are point-sized: the masked edges of a positive maximum all carry dz2 = R, and share the winning value.
-// One thread per channel walks the 64 centres of a unit in order: partial[unit] = [sum dz2 | sum dz2 * xhat2]
+// One thread per channel walks the 64 centres of a unit in order: partial[unit] = [sum dz2 | sum dz2 * xhat2].  partial == NULL (frozen
+// batch norm): R only, ywin and mean_inv are not read.
 __global__ void __launch_bounds__(kE2C2) edge2_bn2_sums_kernel(long long points, const float* __restrict__ pooled, const uint32_t* __restrict__ mask,
                                                                const float* __restrict__ ywin, const float* __restrict__ mean_inv,
                                                                const float* __restrict__ dout, float* __restrict__ R, float* __restrict__ partial) {
     const int c = threadIdx.x;
-    const float mu = __ldg(mean_inv + c), inv = __ldg(mean_inv + kE2C2 + c);
+    const bool sums = partial != nullptr;
+    const float mu = sums ? __ldg(mean_inv + c) : 0.f, inv = sums ? __ldg(mean_inv + kE2C2 + c) : 0.f;
     float sb = 0.f, sg = 0.f;
     for (long long p = (long long)blockIdx.x * kE2Rows; p < points && p < ((long long)blockIdx.x + 1) * kE2Rows; ++p) {
         const size_t o = (size_t)p * kE2C2 + c;
         const float cnt = (float)__popc(__ldg(mask + o));
         const float r = __ldg(pooled + o) > 0.f ? __fdiv_rn(__ldg(dout + o), cnt) : 0.f;
         R[o] = r;
+        if (!sums) continue;
         sb = fmaf(r, cnt, sb);
         sg = fmaf(r * cnt, (__ldg(ywin + o) - mu) * inv, sg);
     }
+    if (!sums) return;
     partial[(size_t)blockIdx.x * 2 * kE2C2 + c] = sb;
     partial[(size_t)blockIdx.x * 2 * kE2C2 + kE2C2 + c] = sg;
 }
@@ -607,4 +611,42 @@ extern "C" int psa_edgeconv2_train_bwd(int b, int n, int c, int k, int C1, int C
     rc = launch_bn_bwd_final((int)units, kE2C1, edges, part1, gamma1, mean_inv1, dgamma1, dbeta1, coef1, coef1 + kE2C1, coef1 + 2 * kE2C1, st);
     if (rc != PSA_OK) return rc;
     return edge_layer_tail(b, n, c, k, kE2C1, x, nn_idx, W1, PQ, scale1, shift1, coef1, nullptr, nullptr, dz1, dW1, dx, ws + L.tail, st);
+}
+
+extern "C" int psa_edgeconv2_frozen_bwd(int b, int n, int c, int k, int C1, int C2, const float* x, const int* nn_idx, const float* W1,
+                                        const float* PQ, const float* scale1, const float* shift1, const float* W2, const float* bias2,
+                                        const float* scale2, const float* pooled, const unsigned int* mask, const float* ywin, const float* dout,
+                                        float* dx, void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    int rc = e2_check("edgeconv2_frozen_bwd", b, n, c, k, C1, C2);
+    if (rc != PSA_OK) return rc;
+    PSA_SUPPORTED(n <= kE2MaxCloud, "edgeconv2_frozen_bwd: n=%d points per cloud exceed %d (reverse neighbour lists)", n, kE2MaxCloud);
+    PSA_REQUIRE(x && nn_idx && W1 && PQ && scale1 && shift1 && W2 && scale2 && pooled && mask && ywin && dout && dx,
+                "edgeconv2_frozen_bwd: null buffer");
+    rc = e2_check_ws("edgeconv2_frozen_bwd", workspace, workspace_bytes, psa_edgeconv2_train_workspace_bytes(b, n, c, k, C1, C2));
+    if (rc != PSA_OK) return rc;
+    cudaStream_t st = as_stream(stream);
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    const E2Layout L(b, n, c, k);
+    const long long points = (long long)b * n, units = e2_units(points);
+    float* coef1 = reinterpret_cast<float*>(ws + L.coef1);
+    float* coef2 = reinterpret_cast<float*>(ws + L.coef2);
+    float* dz1 = reinterpret_cast<float*>(ws + L.dz1);
+    float* R = reinterpret_cast<float*>(ws + L.r);
+    rc = e2_images(W2, ws, L, true, st);
+    if (rc != PSA_OK) return rc;
+    // layer 2: the max's gradient routed to the masked edges (no batch-norm sums), dy2 = scale2 * dz2
+    edge2_bn2_sums_kernel<<<(unsigned)units, kE2C2, 0, st>>>(points, pooled, mask, ywin, nullptr, dout, R, nullptr);
+    rc = check_launch("edge2_bn2_sums_kernel");
+    if (rc != PSA_OK) return rc;
+    rc = frozen_coef(kE2C2, scale2, coef2, st);
+    if (rc != PSA_OK) return rc;
+    // dz1 = (dy2 . W2^T) [h1 > 0]
+    E2Args a = e2_args(b, n, k, nn_idx, PQ, scale1, shift1, bias2, ws, L);
+    a.mask = const_cast<uint32_t*>(mask); a.R = R; a.coef2 = coef2; a.dz1 = dz1;
+    rc = e2_launch<kE2Dh1>(a, st);
+    if (rc != PSA_OK) return rc;
+    // layer 1: dy1 = scale1 * dz1, then dQ, dP and dx (R is dead here)
+    rc = frozen_coef(kE2C1, scale1, coef1, st);
+    if (rc != PSA_OK) return rc;
+    return edge_layer_tail(b, n, c, k, kE2C1, x, nn_idx, W1, PQ, scale1, shift1, coef1, nullptr, nullptr, dz1, nullptr, dx, ws + L.tail, st);
 }

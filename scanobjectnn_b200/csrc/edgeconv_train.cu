@@ -138,7 +138,31 @@ edge_train_pool_kernel(long long points, int n, int k, int N, const float* __res
     }
 }
 
-// backward pass 1: R_ic = dout_ic / ties_ic where pooled_ic > 0 (else 0); partial[tile] = [sum dz | sum dz * xhat] over the tile's edges
+// R_ic = dout_ic / ties_ic where pooled_ic > 0, else 0 (the max's gradient per tied edge), for the warp's VEC channels of point p
+template <int VEC>
+__device__ __forceinline__ void edge_route(size_t o, const float* __restrict__ pooled, const void* __restrict__ ties, bool wide,
+                                           const float* __restrict__ dout, float* __restrict__ R, float (&mx)[VEC], float (&r)[VEC]) {
+    load_vec<VEC>(mx, pooled + o);
+#pragma unroll
+    for (int v = 0; v < VEC; ++v) {
+        r[v] = mx[v] > 0.f ? __fdiv_rn(__ldg(dout + o + v), (float)load_tie(ties, o + v, wide)) : 0.f;
+        R[o + v] = r[v];
+    }
+}
+
+// frozen batch norm's backward pass 1: R alone (there are no batch-norm sums)
+template <int VEC>
+__global__ void __launch_bounds__(kEdgeWarps * 32)
+edge_route_kernel(long long points, int k, int N, const float* __restrict__ pooled, const void* __restrict__ ties, const float* __restrict__ dout,
+                  float* __restrict__ R) {
+    const int c0 = (threadIdx.x & 31) * VEC;
+    for (long long p = (long long)blockIdx.x * kEdgeWarps + (threadIdx.x >> 5); p < points; p += (long long)gridDim.x * kEdgeWarps) {
+        float mx[VEC], r[VEC];
+        edge_route<VEC>((size_t)p * N + c0, pooled, ties, k > 255, dout, R, mx, r);
+    }
+}
+
+// backward pass 1: R (edge_route); partial[tile] = [sum dz | sum dz * xhat] over the tile's edges
 template <int VEC>
 __global__ void __launch_bounds__(kEdgeWarps * 32)
 edge_train_bn_sums_kernel(long long points, int n, int k, int N, const float* __restrict__ PQ, const int* __restrict__ nn_idx,
@@ -161,15 +185,9 @@ edge_train_bn_sums_kernel(long long points, int n, int k, int N, const float* __
             const long long p = tile * kEdgeTile + u;
             if (p >= points) break;
             const long long base = (p / n) * n;
-            const size_t o = (size_t)p * N + c0;
             float a[VEC], mx[VEC], r[VEC];
             load_vec<VEC>(a, PQ + (size_t)p * 2 * N + c0);
-            load_vec<VEC>(mx, pooled + o);
-#pragma unroll
-            for (int v = 0; v < VEC; ++v) {
-                r[v] = mx[v] > 0.f ? __fdiv_rn(__ldg(dout + o + v), (float)load_tie(ties, o + v, wide)) : 0.f;
-                R[o + v] = r[v];
-            }
+            edge_route<VEC>((size_t)p * N + c0, pooled, ties, wide, dout, R, mx, r);
             for_each_neighbour(nn_idx + (size_t)p * k, k, lane, [&](int nb) {
                 float bv[VEC];
                 load_vec<VEC>(bv, PQ + (size_t)(base + nb) * 2 * N + N + c0);
@@ -391,14 +409,16 @@ int psa::edge_layer_tail(int b, int n, int c, int k, int N, const float* x, cons
     PSA_EDGE_DISPATCH(edge_train_dp_kernel, edge_grid(rows), 0, rows, n, k, N, PQ, scale, shift, coef, pooled, R, dz, offsets, list, G);
     rc = check_launch("edge_train_dp_kernel");
     if (rc != PSA_OK) return rc;
-    // dW_a = x^T dQ, dW_b = x^T (dP - dQ): straight into the two row blocks of dW (2c, N)
-    psa_act_in in = {};
-    in.x = x; in.ld = c;
-    const psa_grad_in gq = plain_grad(G, 2 * N, N), gd = plain_grad(G + N, 2 * N, N);
-    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gq, dW, dense_ws, dense_bytes, stream);
-    if (rc != PSA_OK) return rc;
-    rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gd, dW + (size_t)c * N, dense_ws, dense_bytes, stream);
-    if (rc != PSA_OK) return rc;
+    if (dW != nullptr) {
+        // dW_a = x^T dQ, dW_b = x^T (dP - dQ): straight into the two row blocks of dW (2c, N)
+        psa_act_in in = {};
+        in.x = x; in.ld = c;
+        const psa_grad_in gq = plain_grad(G, 2 * N, N), gd = plain_grad(G + N, 2 * N, N);
+        rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gq, dW, dense_ws, dense_bytes, stream);
+        if (rc != PSA_OK) return rc;
+        rc = psa_train_dense_bwd_weight(rows, c, N, &in, &gd, dW + (size_t)c * N, dense_ws, dense_bytes, stream);
+        if (rc != PSA_OK) return rc;
+    }
     // dx = [dQ | dP - dQ] . [W_a | W_b]^T: one product over 2N columns
     PSA_CUDA(cudaMemcpy2DAsync(W2, (size_t)2 * N * sizeof(float), W, (size_t)N * sizeof(float), (size_t)N * sizeof(float), c,
                                cudaMemcpyDeviceToDevice, st));
@@ -406,6 +426,12 @@ int psa::edge_layer_tail(int b, int n, int c, int k, int N, const float* x, cons
                                cudaMemcpyDeviceToDevice, st));
     const psa_grad_in gg = plain_grad(G, 2 * N, 2 * N);
     return psa_train_dense_bwd_input(rows, c, 2 * N, &gg, W2, dx, c, 0, dense_ws, dense_bytes, stream);
+}
+
+int psa::frozen_coef(int N, const float* scale, float* coef, cudaStream_t st) {
+    PSA_CUDA(cudaMemcpyAsync(coef, scale, (size_t)N * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    PSA_CUDA(cudaMemsetAsync(coef + N, 0, (size_t)2 * N * sizeof(float), st));
+    return PSA_OK;
 }
 
 extern "C" size_t psa_edgeconv_train_workspace_bytes(int b, int n, int c, int k, int C_out) {
@@ -419,7 +445,7 @@ extern "C" int psa_edgeconv_train_fwd(int b, int n, int c, int k, int C_out, con
     const int N = C_out;
     int rc = check_dims("edgeconv_train_fwd", b, n, c, k, N);
     if (rc != PSA_OK) return rc;
-    PSA_REQUIRE(x && nn_idx && W && PQ && stats, "edgeconv_train_fwd: null buffer");
+    PSA_REQUIRE(x && nn_idx && W && PQ, "edgeconv_train_fwd: null buffer");
     rc = check_ws("edgeconv_train_fwd", workspace, workspace_bytes, psa_edgeconv_train_workspace_bytes(b, n, c, k, N));
     if (rc != PSA_OK) return rc;
     cudaStream_t st = as_stream(stream);
@@ -438,7 +464,7 @@ extern "C" int psa_edgeconv_train_fwd(int b, int n, int c, int k, int C_out, con
     psa_act_in in = {};
     in.x = x; in.ld = c;
     rc = psa_train_dense_fwd(rows, c, 2 * N, &in, Wc, bias2, PQ, nullptr, ws + L.dense, L.total - L.dense, stream);
-    if (rc != PSA_OK) return rc;
+    if (rc != PSA_OK || stats == nullptr) return rc;            // no stats: frozen batch norm, PQ only
     PSA_EDGE_DISPATCH(edge_train_stats_kernel, tile_grid(tiles), 0, rows, n, k, N, PQ, nn_idx, tiles, partial);
     rc = check_launch("edge_train_stats_kernel");
     if (rc != PSA_OK) return rc;
@@ -484,4 +510,29 @@ extern "C" int psa_edgeconv_train_bwd(int b, int n, int c, int k, int C_out, con
     rc = launch_bn_bwd_final((int)tiles, N, rows * k, partial, gamma, mean_inv, dgamma, dbeta, coef, coef + N, coef + 2 * N, st);
     if (rc != PSA_OK) return rc;
     return edge_layer_tail(b, n, c, k, N, x, nn_idx, W, PQ, scale, shift, coef, pooled, R, nullptr, dW, dx, ws + L.tail, st);
+}
+
+extern "C" int psa_edgeconv_frozen_bwd(int b, int n, int c, int k, int C_out, const float* x, const int* nn_idx, const float* W, const float* PQ,
+                                       const float* scale, const float* shift, const float* pooled, const void* ties, const float* dout, float* dx,
+                                       void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    const int N = C_out;
+    int rc = check_dims("edgeconv_frozen_bwd", b, n, c, k, N);
+    if (rc != PSA_OK) return rc;
+    PSA_SUPPORTED(n <= kEdgeMaxCloud, "edgeconv_frozen_bwd: n=%d points per cloud exceed %d (reverse neighbour lists)", n, kEdgeMaxCloud);
+    PSA_REQUIRE(x && nn_idx && W && PQ && scale && shift && pooled && ties && dout && dx, "edgeconv_frozen_bwd: null buffer");
+    rc = check_ws("edgeconv_frozen_bwd", workspace, workspace_bytes, psa_edgeconv_train_workspace_bytes(b, n, c, k, N));
+    if (rc != PSA_OK) return rc;
+    cudaStream_t st = as_stream(stream);
+    const long long rows = (long long)b * n;
+    const BwdLayout L(b, n, c, k, N);
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+    float* R = reinterpret_cast<float*>(ws + L.r);
+    float* coef = reinterpret_cast<float*>(ws + L.coef);
+    // the max's gradient routed to the tied edges (no batch-norm sums), then dy = scale * dz
+    PSA_EDGE_DISPATCH(edge_route_kernel, edge_grid(rows), 0, rows, k, N, pooled, ties, dout, R);
+    rc = check_launch("edge_route_kernel");
+    if (rc != PSA_OK) return rc;
+    rc = frozen_coef(N, scale, coef, st);
+    if (rc != PSA_OK) return rc;
+    return edge_layer_tail(b, n, c, k, N, x, nn_idx, W, PQ, scale, shift, coef, pooled, R, nullptr, nullptr, dx, ws + L.tail, st);
 }

@@ -29,11 +29,14 @@ int launch_fill_ord_neg_inf(long long total, float* out, cudaStream_t st, const 
 int launch_decode_ord(long long total, float* out, cudaStream_t st, const unsigned int* run_if = nullptr);         // int codes -> floats, in place
 // edgeconv_train.cu: the backward of an EdgeConv layer that sees x (y_ij = Q_i + P_nn(i,j), PQ (b*n, 2N)) once its batch-norm coefficients
 // coef (3, N) are known -> dW (2c, N), dx (b*n, c).  dz (b*n*k, N) gives the gradient w.r.t. the layer's batch-norm output per edge; when it
-// is null, the max's gradient is routed by (pooled, R) as the single-layer op does.  workspace: edge_tail_workspace_bytes, 256-byte aligned.
+// is null, the max's gradient is routed by (pooled, R) as the single-layer op does.  dW null: dx only (frozen batch norm).
+// workspace: edge_tail_workspace_bytes, 256-byte aligned.
 size_t edge_tail_workspace_bytes(int b, int n, int c, int k, int N);
 int edge_layer_tail(int b, int n, int c, int k, int N, const float* x, const int* nn_idx, const float* W, const float* PQ, const float* scale,
                     const float* shift, const float* coef, const float* pooled, const float* R, const float* dz, float* dW, float* dx,
                     void* workspace, cudaStream_t st);
+// frozen batch norm's backward coefficients dy = scale * dz: coef (3, N) := (scale, 0, 0)
+int frozen_coef(int N, const float* scale, float* coef, cudaStream_t st);
 
 }  // namespace psa
 

@@ -1,9 +1,12 @@
-"""dgcnn/models/dgcnn.py and dgcnn_bga.py on the libpsa kernels (inference, and training through autograd over the same kernels: is_training=True).
+"""dgcnn/models/dgcnn.py and dgcnn_bga.py on the libpsa kernels (inference, and training through autograd over the same kernels: is_training=True;
+inference with a gradient w.r.t. the point cloud runs the training kernels with batch norm frozen on the moving averages).
 
 Every `pairwise_distance -> knn -> get_edge_feature -> conv2d -> reduce_max` group of the reference
 (dgcnn.py:31-80) is two launches here: the fused kNN graph (no (B,N,N) matrix) and the fused EdgeConv
 (gather [x_i, x_j - x_i] + MLP + max over k, no (B,N,k,2C) tensor)."""
 from __future__ import annotations
+
+from functools import partial
 
 import torch
 
@@ -73,7 +76,7 @@ def _backbone(point_cloud, params, end_points, k=K_NEIGHBORS):
     return nets, glob
 
 
-def _edge_conv_training(x, k, layers, bn_decay, params, idx=None):
+def _edge_conv_training(x, k, layers, bn_decay, params, idx=None, frozen=False):
     """pairwise_distance -> knn -> get_edge_feature -> conv2d(+BN+ReLU)... -> reduce_max over k (dgcnn.py:31-44) in training mode.
     The neighbour graph carries no gradient; batch statistics over all B*N*k edges.  The single-layer EdgeConvs (dgcnn1..4) and the
     T-net's two-layer one run as the fused edgeconv_training: no per-edge tensor."""
@@ -82,34 +85,39 @@ def _edge_conv_training(x, k, layers, bn_decay, params, idx=None):
         with torch.no_grad():
             idx = ops.knn_graph(x.detach().contiguous(), k)
     scopes = [scope for scope, _ in layers]
-    return edgeconv_training(x, idx, scopes[0] if len(scopes) == 1 else scopes, bn_decay, params), idx
+    return edgeconv_training(x, idx, scopes[0] if len(scopes) == 1 else scopes, bn_decay, params, frozen=frozen), idx
 
 
-def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, dropout: bool = True, k=K_NEIGHBORS, graphs=None, bga: bool = False):
+def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, dropout: bool = True, k=K_NEIGHBORS, graphs=None, bga: bool = False,
+                        frozen: bool = False):
     """dgcnn.get_model with is_training=True (dgcnn.py:24-102, transform_nets.py:10-55): batch-statistics batch norm everywhere,
     dropout (keep 0.5) after fc1 and fc2, PyTorch autograd over the hand-written kernels.  `graphs` (tests): the five neighbour
     graphs to use instead of recomputing them -- the graphs are piecewise-constant functions of the parameters, which a finite
-    difference must not cross."""
-    from .training import mlp_training
+    difference must not cross.  frozen=True: inference mode differentiable in the point cloud -- batch norm on the moving averages
+    (never updated), no dropout, and no gradient for any variable (the T-net's transform_XYZ is read detached, so nothing reaches
+    the flat parameter vector)."""
+    from .training import mlp_training as _mlp_training
     f = torch.nn.functional
     b, n, _ = point_cloud.shape
     end_points = {}
+    dropout = dropout and not frozen
+    mlp_training = partial(_mlp_training, frozen=frozen)
     drop = (lambda t: f.dropout(t, 0.5, training=True)) if dropout else (lambda t: t)
     # input transform net on the raw cloud
     sc = "transform_net1"
     net, idx0 = _edge_conv_training(point_cloud, k, [(f"{sc}/tconv1", True), (f"{sc}/tconv2", True)], bn_decay, params,
-                                    None if graphs is None else graphs[0])                                                # (B,N,128)
+                                    None if graphs is None else graphs[0], frozen)                                        # (B,N,128)
     end_points["nn_idx0"] = idx0
     net = mlp_training(net, [(f"{sc}/tconv3", True)], bn_decay, params).amax(dim=1)                                       # (B,1024)
     net = mlp_training(net, [(f"{sc}/tfc1", True), (f"{sc}/tfc2", True)], bn_decay, params)                               # (B,256)
-    fp = params._flat
-    w, bias = fp.live(f"{sc}/transform_XYZ/weights"), fp.live(f"{sc}/transform_XYZ/biases")
+    names = (f"{sc}/transform_XYZ/weights", f"{sc}/transform_XYZ/biases")
+    w, bias = (params[v].detach() for v in names) if frozen else (params._flat.live(v) for v in names)
     transform = (net @ w + bias + torch.eye(3, device=w.device).flatten()).reshape(b, 3, 3)
     x = torch.bmm(point_cloud, transform)
     end_points.update(transform=transform, point_cloud_transformed=x)
     nets = []
     for i, scope in enumerate(["dgcnn1", "dgcnn2", "dgcnn3", "dgcnn4"]):
-        x, idx = _edge_conv_training(x, k, [(scope, True)], bn_decay, params, None if graphs is None else graphs[i + 1])
+        x, idx = _edge_conv_training(x, k, [(scope, True)], bn_decay, params, None if graphs is None else graphs[i + 1], frozen)
         end_points[f"nn_idx{i + 1}"] = idx
         end_points[f"net{i + 1}"] = x
         nets.append(x)
@@ -132,9 +140,12 @@ def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore,
 
 
 def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *, params: VariableStore):
-    """dgcnn.get_model (dgcnn.py:24-102): (B,N,3) -> (logits (B,num_class), end_points)."""
-    if is_training:
-        return _get_model_training(point_cloud, bn_decay, num_class, params)
+    """dgcnn.get_model (dgcnn.py:24-102): (B,N,3) -> (logits (B,num_class), end_points).  Inference mode with a point cloud that
+    requires a gradient (and gradients enabled) runs the training kernels on frozen batch norm, so the logits differentiate in it."""
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(point_cloud)
+    if is_training or frozen:
+        return _get_model_training(point_cloud, bn_decay, num_class, params, frozen=frozen)
     end_points = {}
     _, net = _backbone(point_cloud, params, end_points)                      # tf.reduce_max over N already applied
     end_points["global"] = net
@@ -143,9 +154,12 @@ def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *,
 
 
 def get_model_bga(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *, params: VariableStore, return_end_points: bool = False):
-    """dgcnn_bga.get_model (dgcnn_bga.py:27-134): -> (class_pred (B,num_class), seg_pred (B,N,2), end_points)."""
-    if is_training:
-        cp, sp, ep = _get_model_training(point_cloud, bn_decay, num_class, params, bga=True)
+    """dgcnn_bga.get_model (dgcnn_bga.py:27-134): -> (class_pred (B,num_class), seg_pred (B,N,2), end_points).  Differentiable in
+    the point cloud in inference mode as get_model is."""
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(point_cloud)
+    if is_training or frozen:
+        cp, sp, ep = _get_model_training(point_cloud, bn_decay, num_class, params, bga=True, frozen=frozen)
         return (cp, sp, ep) if return_end_points else (cp, sp)
     end_points = {}
     b, n, _ = point_cloud.shape

@@ -1,8 +1,11 @@
 """pointnet/models/pointnet_cls.py (vanilla PointNet, BASELINE.json configs[0]: the reference's plumbing case) on the same
 dense kernels: every layer is a per-point shared MLP (`psa_shared_mlp`), the symmetric function is its fused max-pool.
 get_model(point_cloud, is_training, bn_decay, num_class) -> (logits (B,num_class), end_points).  Inference, and training through
-autograd over training.mlp_training (is_training=True)."""
+autograd over training.mlp_training (is_training=True), and inference differentiable in the point cloud (the same nodes with batch
+norm frozen on the moving averages) when the cloud requires a gradient."""
 from __future__ import annotations
+
+from functools import partial
 
 import torch
 
@@ -49,29 +52,32 @@ def transform_net(x, params: VariableStore, scope: str, K: int):
     return (g @ w + bias).reshape(b, K, K)
 
 
-def _transform_net_training(x, params: VariableStore, scope: str, K: int, bn_decay):
-    from .training import mlp_training
+def _transform_net_training(x, params: VariableStore, scope: str, K: int, bn_decay, frozen: bool = False):
+    from .training import mlp_training as _mlp_training
+    mlp_training = partial(_mlp_training, frozen=frozen)
     b = x.shape[0]
     g = mlp_training(x, [(f"{scope}/tconv1", True), (f"{scope}/tconv2", True), (f"{scope}/tconv3", True)], bn_decay, params).amax(dim=1)
     g = mlp_training(g, [(f"{scope}/tfc1", True), (f"{scope}/tfc2", True)], bn_decay, params)
     name = "transform_XYZ" if K == 3 else "transform_feat"
-    fp = params._flat
-    w, bias = fp.live(f"{scope}/{name}/weights"), fp.live(f"{scope}/{name}/biases")
+    names = (f"{scope}/{name}/weights", f"{scope}/{name}/biases")
+    w, bias = (params[v].detach() for v in names) if frozen else (params._flat.live(v) for v in names)
     return (g @ w + bias + torch.eye(K, device=w.device).flatten()).reshape(b, K, K)
 
 
-def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, dropout: bool = True):
+def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore, dropout: bool = True, frozen: bool = False):
     """pointnet_cls.get_model with is_training=True (pointnet_cls.py:21-75): batch-statistics batch norm in every layer, dropout
     (keep 0.7) after fc1 and fc2, autograd over training.mlp_training nodes; the T-nets' matrices are torch ops on live views of
-    the flat parameter vector."""
-    from .training import mlp_training
+    the flat parameter vector.  frozen=True: inference mode differentiable in the point cloud -- batch norm on the moving averages
+    (never updated), no dropout, the T-nets' matrices read detached: no variable receives a gradient."""
+    from .training import mlp_training as _mlp_training
+    mlp_training = partial(_mlp_training, frozen=frozen)
     f = torch.nn.functional
-    drop = (lambda t: f.dropout(t, 0.3, training=True)) if dropout else (lambda t: t)
+    drop = (lambda t: f.dropout(t, 0.3, training=True)) if dropout and not frozen else (lambda t: t)
     end_points = {}
-    t1 = _transform_net_training(point_cloud.contiguous(), params, "transform_net1", 3, bn_decay)
+    t1 = _transform_net_training(point_cloud.contiguous(), params, "transform_net1", 3, bn_decay, frozen)
     x = torch.bmm(point_cloud, t1)
     net = mlp_training(x, [("conv1", True), ("conv2", True)], bn_decay, params)
-    t2 = _transform_net_training(net, params, "transform_net2", 64, bn_decay)
+    t2 = _transform_net_training(net, params, "transform_net2", 64, bn_decay, frozen)
     end_points["transform"] = t2
     net = torch.bmm(net, t2)
     net = mlp_training(net, [("conv3", True), ("conv4", True), ("conv5", True)], bn_decay, params).amax(dim=1)
@@ -82,8 +88,10 @@ def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore,
 
 
 def get_model(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES, *, params: VariableStore):
-    if is_training:
-        return _get_model_training(point_cloud, bn_decay, num_class, params)
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(point_cloud)
+    if is_training or frozen:
+        return _get_model_training(point_cloud, bn_decay, num_class, params, frozen=frozen)
     b, n, _ = point_cloud.shape
     end_points = {}
     t1 = transform_net(point_cloud, params, "transform_net1", 3)

@@ -367,10 +367,11 @@ def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, froze
 class EdgeConvTrainer(_TrainOps):
     """Training-mode single-layer EdgeConv (dgcnn.py:41-47: get_edge_feature -> conv2d + batch norm + ReLU -> reduce_max over k) on
     the fused kernels of csrc/edgeconv_train.cu: one product over the b*n points and gather passes; no (B,N,k,.) tensor is stored.
-    Batch statistics over all b*n*k edges; the max's gradient is split evenly among tied edges, as torch.amax / TF reduce_max do."""
+    Batch statistics over all b*n*k edges; the max's gradient is split evenly among tied edges, as torch.amax / TF reduce_max do.
+    frozen=True: inference mode -- batch norm on the moving averages (never updated), and a backward that gives dx only."""
 
-    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scope: str, device=None):
-        super().__init__(params, device, False)
+    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scope: str, device=None, frozen: bool = False):
+        super().__init__(params, device, frozen)
         self.b, self.n, self.c, self.k = b, n, c, k
         ly = _Layer(self.fp, scope, 0, True, self.dev)       # rows = 0: the per-edge activations are never stored
         self.layers = [ly]
@@ -392,17 +393,25 @@ class EdgeConvTrainer(_TrainOps):
         assert x.shape == (b, n, c) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
         assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
         self.x, self.nn_idx = x, nn_idx
-        check(self.lib.psa_edgeconv_train_fwd(b, n, c, k, ly.N, _p(x), _p(nn_idx), _p(ly.W), _p(ly.b), _p(self.PQ), _p(ly.stats), _p(self.ws),
-                                              C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_fwd")
+        self._fold_frozen(self.layers)
+        check(self.lib.psa_edgeconv_train_fwd(b, n, c, k, ly.N, _p(x), _p(nn_idx), _p(ly.W), _p(ly.b), _p(self.PQ),
+                                              None if self.frozen else _p(ly.stats), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()),
+              "edgeconv_train_fwd")
         self._bn_finalize(ly, b * n * k, bn_decay)
         check(self.lib.psa_edgeconv_train_pool(b, n, k, ly.N, _p(nn_idx), _p(self.PQ), _p(ly.scale), _p(ly.shift), _p(self.pooled), _p(self.ties),
                                                _stream()), "edgeconv_train_pool")
         return self.pooled
 
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
-        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); the layer's gradients go to the flat bucket"""
+        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); the layer's gradients go to the flat bucket
+        (not when frozen)"""
         b, n, c, k, (ly,) = self.b, self.n, self.c, self.k, self.layers
         dout = dout.contiguous()
+        if self.frozen:
+            check(self.lib.psa_edgeconv_frozen_bwd(b, n, c, k, ly.N, _p(self.x), _p(self.nn_idx), _p(ly.W), _p(self.PQ), _p(ly.scale), _p(ly.shift),
+                                                   _p(self.pooled), _p(self.ties), _p(dout), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes),
+                                                   _stream()), "edgeconv_frozen_bwd")
+            return self.d_in
         check(self.lib.psa_edgeconv_train_bwd(b, n, c, k, ly.N, _p(self.x), _p(self.nn_idx), _p(ly.W), _p(self.PQ), _p(ly.scale), _p(ly.shift),
                                               _p(ly.gamma), _p(ly.mean_inv), _p(self.pooled), _p(self.ties), _p(dout), _p(ly.dW), _p(ly.dgamma),
                                               _p(ly.dbeta), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "edgeconv_train_bwd")
@@ -414,10 +423,11 @@ class EdgeConv2Trainer(_TrainOps):
     """Training-mode two-layer EdgeConv (transform_nets.py:18-27: get_edge_feature -> conv2d + BN + ReLU -> conv2d + BN + ReLU ->
     reduce_max over k) on csrc/edgeconv2_train.cu: layer 1 is the single-layer op's point product, the per-edge 64 -> 128 product runs
     on the tensor cores and is recomputed in every pass; no (B,N,k,.) tensor is stored in the forward.  Batch statistics over all
-    b*n*k edges in both layers; the max's gradient is split evenly among tied edges."""
+    b*n*k edges in both layers; the max's gradient is split evenly among tied edges.  frozen=True: inference mode -- batch norm on the
+    moving averages (never updated) in both layers, and a backward that gives dx only."""
 
-    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scopes, device=None):
-        super().__init__(params, device, False)
+    def __init__(self, params: VariableStore, b: int, n: int, c: int, k: int, scopes, device=None, frozen: bool = False):
+        super().__init__(params, device, frozen)
         self.b, self.n, self.c, self.k = b, n, c, k
         self.layers = [_Layer(self.fp, s, 0, True, self.dev) for s in scopes]     # rows = 0: the per-edge activations are never stored
         l1, l2 = self.layers
@@ -445,22 +455,30 @@ class EdgeConv2Trainer(_TrainOps):
         assert nn_idx.shape == (b, n, k) and nn_idx.dtype == torch.int32 and nn_idx.is_contiguous()
         self.x, self.nn_idx = x, nn_idx
         lib, ws, wsb = self.lib, _p(self.ws), C.c_size_t(self.ws_bytes)
-        check(lib.psa_edgeconv_train_fwd(b, n, c, k, l1.N, _p(x), _p(nn_idx), _p(l1.W), _p(l1.b), _p(self.PQ), _p(l1.stats), ws, wsb, _stream()),
-              "edgeconv_train_fwd")
-        self._bn_finalize(l1, b * n * k, bn_decay)
-        check(lib.psa_edgeconv2_train_fwd(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
-                                          _p(l2.stats), ws, wsb, _stream()), "edgeconv2_train_fwd")
-        self._bn_finalize(l2, b * n * k, bn_decay)
+        self._fold_frozen(self.layers)
+        check(lib.psa_edgeconv_train_fwd(b, n, c, k, l1.N, _p(x), _p(nn_idx), _p(l1.W), _p(l1.b), _p(self.PQ), None if self.frozen else _p(l1.stats),
+                                         ws, wsb, _stream()), "edgeconv_train_fwd")
+        if not self.frozen:            # frozen: layer 2's scale / shift are already folded, no statistics pass
+            self._bn_finalize(l1, b * n * k, bn_decay)
+            check(lib.psa_edgeconv2_train_fwd(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
+                                              _p(l2.stats), ws, wsb, _stream()), "edgeconv2_train_fwd")
+            self._bn_finalize(l2, b * n * k, bn_decay)
         check(lib.psa_edgeconv2_train_pool(b, n, c, k, l1.N, l2.N, _p(nn_idx), _p(self.PQ), _p(l1.scale), _p(l1.shift), _p(l2.W), _p(l2.b),
                                            _p(l2.scale), _p(l2.shift), _p(self.pooled), _p(self.mask), _p(self.ywin), ws, wsb, _stream()),
               "edgeconv2_train_pool")
         return self.pooled
 
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
-        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); both layers' gradients go to the flat bucket"""
+        """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x (b*n, c); both layers' gradients go to the flat bucket
+        (not when frozen)"""
         b, n, c, k = self.b, self.n, self.c, self.k
         l1, l2 = self.layers
         dout = dout.contiguous()
+        if self.frozen:
+            check(self.lib.psa_edgeconv2_frozen_bwd(b, n, c, k, l1.N, l2.N, _p(self.x), _p(self.nn_idx), _p(l1.W), _p(self.PQ), _p(l1.scale),
+                                                    _p(l1.shift), _p(l2.W), _p(l2.b), _p(l2.scale), _p(self.pooled), _p(self.mask), _p(self.ywin),
+                                                    _p(dout), _p(self.d_in), _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "edgeconv2_frozen_bwd")
+            return self.d_in
         check(self.lib.psa_edgeconv2_train_bwd(b, n, c, k, l1.N, l2.N, _p(self.x), _p(self.nn_idx), _p(l1.W), _p(self.PQ), _p(l1.scale),
                                                _p(l1.shift), _p(l1.gamma), _p(l1.mean_inv), _p(l2.W), _p(l2.b), _p(l2.gamma), _p(l2.mean_inv),
                                                _p(self.pooled), _p(self.mask), _p(self.ywin), _p(dout), _p(l1.dW), _p(l1.dgamma), _p(l1.dbeta),
@@ -471,20 +489,24 @@ class EdgeConv2Trainer(_TrainOps):
         return self.d_in
 
 
-def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, params: VariableStore) -> torch.Tensor:
+def edgeconv_training(x: torch.Tensor, nn_idx: torch.Tensor, scope, bn_decay, params: VariableStore, frozen: bool = False) -> torch.Tensor:
     """Training-mode EdgeConv with autograd: x (B, N, C), nn_idx (B, N, k) int32 -> (B, N, C_out) = max_j relu(BN([x_i, x_j - x_i] . W + b)),
     BN over all B*N*k edges.  `scope` is one scope, or a sequence of two for the two-layer EdgeConv (conv + BN + ReLU twice, then the
     max; C1 = 64, C2 = 128), which runs as one autograd node.  The graph carries no gradient.  Buffers are cached on `params` per
-    (scopes, shape); the variables' gradients land in the flat bucket."""
+    (scopes, shape); the variables' gradients land in the flat bucket.  frozen=True: inference mode (batch norm on the moving averages,
+    which stay put; the gradient of x only)."""
     b, n, c = x.shape
     k = nn_idx.shape[-1]
     scopes = (scope,) if isinstance(scope, str) else tuple(scope)
     if len(scopes) not in (1, 2):
         raise ValueError(f"edgeconv_training: one or two scopes, got {len(scopes)}")
+    tag = "_frozen" if frozen else ""
     if len(scopes) == 1:
-        tr = _cached(params, ("edgeconv", scopes[0], b, n, c, k), lambda: EdgeConvTrainer(params, b, n, c, k, scopes[0], device=x.device))
+        tr = _cached(params, ("edgeconv" + tag, scopes[0], b, n, c, k),
+                     lambda: EdgeConvTrainer(params, b, n, c, k, scopes[0], device=x.device, frozen=frozen))
     else:
-        tr = _cached(params, ("edgeconv2", scopes, b, n, c, k), lambda: EdgeConv2Trainer(params, b, n, c, k, scopes, device=x.device))
+        tr = _cached(params, ("edgeconv2" + tag, scopes, b, n, c, k),
+                     lambda: EdgeConv2Trainer(params, b, n, c, k, scopes, device=x.device, frozen=frozen))
     flat, decay = _flat_and_decay(tr, bn_decay)
     out = _NodeFn.apply(flat, x.contiguous(), tr, (nn_idx.to(torch.int32).contiguous(),), decay)
     return out.view(b, n, -1)
