@@ -220,6 +220,16 @@ PSA_API size_t psa_shared_mlp_workspace_bytes(long long rows, const psa_mlp* mlp
 PSA_API int psa_shared_mlp(long long rows, int pool_k, const float* x, const psa_mlp* mlp, float* out,
                            void* workspace, size_t workspace_bytes, psa_stream_t stream);
 
+/* psa_shared_mlp (pool_k = 1) whose first layer also takes one input row per group of group_rows consecutive rows:
+ *   layer 0:  relu?( (x[r] . W0 + group_add[r / group_rows]) * scale0 + shift0 ),  group_add (rows / group_rows, C_1)
+ * and the later layers as in psa_shared_mlp.  This is a 1x1 conv over concat([x, tile(g, group_rows)]) (pointnet/models/
+ * pointnet_seg.py:81-88) without the concatenation: with W = [W_x ; W_g] (x rows first), group_add = g . W_g is one
+ * psa_shared_mlp call over the groups, and the layer over the rows has K = C_0 = the width of x only.  group_rows must
+ * divide rows (else PSA_ERR_INVALID_ARGUMENT); groups need not align with the kernels' row tiles.  Same workspace as
+ * psa_shared_mlp (psa_shared_mlp_workspace_bytes). */
+PSA_API int psa_shared_mlp_grouped(long long rows, long long group_rows, const float* x, const psa_mlp* mlp, const float* group_add,
+                                   float* out, void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
 /* Fused set-abstraction level, inference mode (pointnet_sa_module, pointnet_util.py:87-154 with
  * sample_and_group :22-56 inside): for every query j of new_xyz
  *   idx_j  = query_ball_point(radius, nsample, xyz, new_xyz)[j]           (or caller-provided idx)
@@ -365,6 +375,22 @@ PSA_API int psa_pool_rows(long long groups, int pool_k, int C, int mode, const f
 /* Bias gradient of a layer that is NOT followed by batch norm: db (N) = sum_r dy[r][:].  (Under batch norm the conv / fc bias
  * has an identically zero gradient -- sum_r dy = 0 -- and the training path writes exact zeros there.) */
 PSA_API int psa_train_bias_grad(long long rows, int N, const psa_grad_in* g, float* db, psa_stream_t stream);
+
+/* Training mode of psa_shared_mlp_grouped's first layer (the conv over concat([x, tile(g)]) of pointnet/models/pointnet_seg.py:81-88
+ * with batch statistics).  Forward: y (rows, N) = in (rows, K) . W (K, N) + group_add[r / group_rows] + bias, and stats (2, N) of y
+ * including the group term, so that batch norm sees what the conv over the concatenation produces.  One pass of the fp32 GEMM
+ * behind psa_train_dense_fwd (any shape; no tensor-core path).  workspace: psa_train_dense_workspace_bytes(rows, K, N).
+ * Backward: dx and dW of the rows come from psa_train_dense_bwd_input / _bwd_weight with W; the group rows' gradient is
+ *   d group_add (rows / group_rows, N) = sum of dy over each group's rows  (psa_train_bias_grad_grouped),
+ * whose products with W_g give dg and dW_g (psa_train_dense_bwd_input / _bwd_weight over the groups).  Under batch norm the
+ * whole-batch sum of dy is zero but the per-group sums are not.  Sums in a fixed order: bit-reproducible.  group_rows must
+ * divide rows (else PSA_ERR_INVALID_ARGUMENT); at most 65535 groups (else PSA_ERR_UNSUPPORTED).  psa_train_bias_grad is the
+ * group_rows = rows case. */
+PSA_API int psa_train_dense_fwd_grouped(long long rows, long long group_rows, int K, int N, const psa_act_in* in, const float* W,
+                                        const float* bias, const float* group_add, float* y, float* stats, void* workspace,
+                                        size_t workspace_bytes, psa_stream_t stream);
+PSA_API int psa_train_bias_grad_grouped(long long rows, long long group_rows, int N, const psa_grad_in* g, float* db,
+                                        psa_stream_t stream);
 
 /* Batch statistics -> BN affine.  stats (2, C) sums over `count` rows; gamma, beta (C) ->
  * scale = gamma / sqrt(var + 1e-3), shift = beta - mean * scale, mean_inv (2, C) = [mean, 1/sqrt(var + eps)];

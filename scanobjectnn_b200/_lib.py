@@ -71,6 +71,7 @@ SIGNATURES = {
     "psa_get_edge_feature": [_i, _i, _i, _i, _p, _p, _p, _p],
     "psa_knn_graph_ws": [_i, _i, _i, _i, _p, _p, _p, C.c_size_t, _p],
     "psa_shared_mlp": [C.c_longlong, _i, _p, C.POINTER(PsaMlp), _p, _p, C.c_size_t, _p],
+    "psa_shared_mlp_grouped": [_ll, _ll, _p, C.POINTER(PsaMlp), _p, _p, _p, _sz, _p],
     "psa_sa_module_infer": [_i, _i, _i, _i, _f, _i, _p, _p, _p, _p, C.POINTER(PsaMlp), _p, _p, _p, _p, C.c_size_t, _p],
     "psa_sa_conv1_prebn": [_i, _i, _i, _i, _f, _i, _p, _p, _p, _p, _p, _i, _p, _p, _p, _p, _p, C.c_size_t, _p],
     "psa_sa_group_all_infer": [_i, _i, _i, _p, _p, C.POINTER(PsaMlp), _p, _p, C.c_size_t, _p],
@@ -84,6 +85,8 @@ SIGNATURES = {
     "psa_train_dense_bwd_input": [_ll, _i, _i, _gin, _p, _p, _ll, _i, _p, _sz, _p],
     "psa_train_dense_bwd_weight": [_ll, _i, _i, _ain, _gin, _p, _p, _sz, _p],
     "psa_train_bias_grad": [_ll, _i, _gin, _p, _p],
+    "psa_train_dense_fwd_grouped": [_ll, _ll, _i, _i, _ain, _p, _p, _p, _p, _p, _p, _sz, _p],
+    "psa_train_bias_grad_grouped": [_ll, _ll, _i, _gin, _p, _p],
     "psa_bn_finalize": [_i, _ll, _p, _p, _p, _f, _p, _p, _p, _p, _p, _p],
     "psa_train_pool_fwd": [_ll, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_bn_bwd_coeffs": [_ll, _i, _gin, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],

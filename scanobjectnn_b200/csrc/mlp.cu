@@ -360,7 +360,7 @@ fused_group_mlp_kernel(const __grid_constant__ FusedArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Dense single layer: out = relu?((x . W) * scale + shift) with optional max over runs of pool_k rows.
+// Dense single layer: out = relu?((x . W [+ group_add[r / group_rows]]) * scale + shift) with optional max over runs of pool_k rows.
 // A streamed from global in [BM][BK] chunks (cp.async when the row pitch allows 16-byte copies).
 // ------------------------------------------------------------------------------------------------------------
 constexpr int LDA_D = BK + 4;   // 20 floats = 80 B rows: 16-byte aligned, conflict-light
@@ -427,6 +427,21 @@ dense_layer_kernel(const __grid_constant__ DenseArgs a) {
     }
     const int tile_rows = (int)min((long long)BM, a.rows - row0);
     const int pk = a.pool_k;
+    if (a.group_add != nullptr) {      // the per-group input (pool_k == 1), in a pass of its own: the epilogue is the same code without it
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int row = ty * 8 + i;
+            if (row >= tile_rows) break;
+            const float* ga = a.group_add + (row0 + row) / a.group_rows * a.N;
+#pragma unroll
+            for (int h = 0; h < TN / 4; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int col = n0 + h * 64 + tx * 4 + j;
+                    if (col < a.N) acc[i][h * 4 + j] += __ldg(ga + col);
+                }
+        }
+    }
     if (pk == 1) {
 #pragma unroll
         for (int h = 0; h < TN / 4; ++h) {

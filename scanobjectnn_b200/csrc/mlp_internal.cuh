@@ -14,6 +14,9 @@ struct DenseArgs {
     const float* scale;  // (N) or null
     const float* shift;  // (N)
     float* out;          // (rows, N) or (rows/pool_k, N)
+    // optional per-row-group input, pool_k == 1 only: row r adds group_add[r / group_rows] (N) to x . W before the affine
+    const float* group_add = nullptr;
+    long long group_rows = 0;
 };
 
 

@@ -670,6 +670,10 @@ struct TcDenseArgs {
     // zeroed before the launch: tiles are claimed from it (a CTA that starts late or shares its SM with another stream's
     // kernels simply takes fewer); null: CTA i takes tiles i, i + grid, ...
     unsigned int* tile_counter = nullptr;
+    // optional per-row-group input (pool_k == 1): row r adds group_add[r / group_rows] (N) before scale/shift, e.g. the
+    // per-cloud product of a global feature tiled over the cloud's points
+    const float* group_add = nullptr;
+    long long group_rows = 0;
 };
 
 // Persistent, warp-specialised.  CTA = two consumer warpgroups (rows 0-63 / 64-127 of a 128-row x Nt = 64 NC tile) + a
@@ -681,7 +685,7 @@ struct TcDenseArgs {
 // of training mode, fp16 range tracking) while it runs, then wait and add the block's sum to the fp32 accumulators: the tensor
 // core's accumulation never runs over more than 64 K however long the dot product is, and every output sees the same sums
 // in the same order whatever the schedule.  One group in flight at a time, so every wait retires the same group on every path.
-//   Epilogue in the fragment layout: xyz side input, affine, ReLU, then either float2 stores (+ per-tile column statistics) or
+//   Epilogue in the fragment layout: xyz side input, per-group input, affine, ReLU, then either float2 stores (+ per-tile column statistics) or
 // the max over pool_k rows; the cross-warp part synchronises the consumers on a named barrier.
 constexpr int kDenseThreads = 384, kDenseConsumers = 256;
 constexpr uint32_t kDenseXRow = 64u * 4u + 32u;           // bytes per staged x row: 8-bank offset between rows g and g + 1
@@ -860,6 +864,22 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
                 if (v[i])
 #pragma unroll
                     for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz3 + (size_t)r[i] * 3 + k);
+        // the per-group input, added to the accumulators in a pass of its own so that the loop below is the same code with or
+        // without it.  Rows g and g + 8 may lie in different groups, and groups need not align with the 128-row tiles.
+        if (a.group_add != nullptr)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+                if (v[i]) {
+                    const float* ga = a.group_add + (size_t)(r[i] / a.group_rows) * a.N + nt * Nt + 2 * t;
+#pragma unroll
+                    for (int c = 0; c < NC; ++c)
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                            const float2 u = __ldg(reinterpret_cast<const float2*>(ga + c * 64 + 8 * j));
+                            acc[c][4 * j + 2 * i] += u.x;
+                            acc[c][4 * j + 2 * i + 1] += u.y;
+                        }
+                }
 #pragma unroll
         for (int c = 0; c < NC; ++c)
 #pragma unroll
@@ -1018,19 +1038,22 @@ static int launch_tc_dense_np(TcDenseArgs& a, int Nt, cudaStream_t st) {
 // of layer l and of its rerun at [kTileCounterWords + 2 l, + 1]
 constexpr int kTileCounterWords = PSA_MAX_MLP_LAYERS;
 
-// out = relu?((x . W [+ xyz3 . w3]) * scale + shift) on the tensor cores, optional max over runs of pool_k rows.
+// out = relu?((x . W [+ xyz3 . w3] [+ group_add[r / group_rows]]) * scale + shift) on the tensor cores, optional max over runs of
+// pool_k rows (not with group_add).
 //   prebuilt : image of W in the CURRENT split's format (psa_prepare_weight_image), or null
 //   ws_img   : tc_dense_image_bytes(K, N) of scratch (missing images are built here)
 //   flag     : one zeroed device word (np = 2: raised when a value left the fp16 range; the bf16x3 rerun is conditional on it)
 //   counters : two zeroed device words, the tile counters of the launch and of its rerun
 int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const float* x, const float* W, const float* scale,
                     const float* shift, float* out, const uint8_t* prebuilt, uint8_t* ws_img, unsigned int* flag, unsigned int* counters,
-                    cudaStream_t st, const float* xyz3 = nullptr, const float* w3 = nullptr) {
+                    cudaStream_t st, const float* xyz3 = nullptr, const float* w3 = nullptr, const float* group_add = nullptr,
+                    long long group_rows = 0) {
     const int Kp = (K + 63) & ~63;
     const int Nt = tc_dense_nt(rows, N) & ~kImageFlags;
     TcDenseArgs a;
     a.rows = rows; a.K = K; a.Kp = Kp; a.N = N; a.pool_k = pool_k; a.relu = relu;
     a.x = x; a.scale = scale; a.shift = shift; a.out = out; a.xyz3 = xyz3; a.w3 = w3;
+    a.group_add = group_add; a.group_rows = group_rows;
     a.tile_counter = counters;
     uint8_t* img3 = ws_img + tc_dense_image_off3(K, N);
     int rc;
@@ -1308,14 +1331,11 @@ extern "C" size_t psa_shared_mlp_workspace_bytes(long long rows, const psa_mlp* 
     return bytes + 256;       // range flags of the tensor-core layers (one word per layer) and their tile counters, last
 }
 
-extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const psa_mlp* mlp, float* out,
-                              void* workspace, size_t workspace_bytes, psa_stream_t stream) {
-    int rc = validate_mlp_public(mlp, "shared_mlp");
-    if (rc != PSA_OK) return rc;
-    PSA_REQUIRE(rows >= 0 && pool_k >= 1, "shared_mlp: rows=%lld pool_k=%d", rows, pool_k);
-    if (rows == 0) return PSA_OK;
-    PSA_REQUIRE(rows % pool_k == 0, "shared_mlp: rows=%lld is not a multiple of pool_k=%d", rows, pool_k);
-    PSA_REQUIRE(x && out, "shared_mlp: null buffer");
+// The layer chain of psa_shared_mlp and psa_shared_mlp_grouped (arguments validated by the caller; group_add: layer 0's per-group input,
+// or null).
+static int shared_mlp_chain(long long rows, int pool_k, const float* x, const psa_mlp* mlp, const float* group_add, long long group_rows,
+                            float* out, void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    int rc;
     const int L = mlp->n_layers;
     const size_t need = psa_shared_mlp_workspace_bytes(rows, mlp);
     PSA_REQUIRE(workspace != nullptr && workspace_bytes >= need, "shared_mlp: workspace of %zu bytes required (got %zu)", need, workspace_bytes);
@@ -1341,20 +1361,44 @@ extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const 
         const int K = mlp->channels[l], N = mlp->channels[l + 1];
         const int pk = (l == L - 1) ? pool_k : 1;
         float* dst = (l == L - 1) ? out : ((l & 1) ? ws1 : ws0);
+        const float* gadd = l == 0 ? group_add : nullptr;
         if (g_mlp_mode != 1 && tc_dense_eligible(rows, K, N, pk)) {
             rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, mlp->weight[l], mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, 0, tc_dense_nt(rows, N)),
-                                 img, flags + l, flags + kTileCounterWords + 2 * l, st);
+                                 img, flags + l, flags + kTileCounterWords + 2 * l, st, nullptr, nullptr, gadd, group_rows);
         } else {
             DenseArgs d;
             d.rows = rows; d.K = K; d.N = N; d.pool_k = pk; d.relu = mlp->relu[l];
             d.x = cur; d.W = mlp->weight[l]; d.scale = mlp->scale[l]; d.shift = mlp->shift[l]; d.out = dst;
-            rc = (rows <= 32 && pk == 1) ? launch_fc_small(d, fc_partial, st) : launch_dense(d, st);
+            d.group_add = gadd; d.group_rows = group_rows;
+            rc = (rows <= 32 && pk == 1 && gadd == nullptr) ? launch_fc_small(d, fc_partial, st) : launch_dense(d, st);
         }
         if (rc != PSA_OK) return rc;
         img += tc_dense_image_bytes(K, N < 64 ? 64 : N);
         cur = dst;
     }
     return PSA_OK;
+}
+
+extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const psa_mlp* mlp, float* out,
+                              void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    int rc = validate_mlp_public(mlp, "shared_mlp");
+    if (rc != PSA_OK) return rc;
+    PSA_REQUIRE(rows >= 0 && pool_k >= 1, "shared_mlp: rows=%lld pool_k=%d", rows, pool_k);
+    if (rows == 0) return PSA_OK;
+    PSA_REQUIRE(rows % pool_k == 0, "shared_mlp: rows=%lld is not a multiple of pool_k=%d", rows, pool_k);
+    PSA_REQUIRE(x && out, "shared_mlp: null buffer");
+    return shared_mlp_chain(rows, pool_k, x, mlp, nullptr, 0, out, workspace, workspace_bytes, stream);
+}
+
+extern "C" int psa_shared_mlp_grouped(long long rows, long long group_rows, const float* x, const psa_mlp* mlp, const float* group_add,
+                                      float* out, void* workspace, size_t workspace_bytes, psa_stream_t stream) {
+    int rc = validate_mlp_public(mlp, "shared_mlp_grouped");
+    if (rc != PSA_OK) return rc;
+    PSA_REQUIRE(rows >= 0 && group_rows >= 1, "shared_mlp_grouped: rows=%lld group_rows=%lld", rows, group_rows);
+    PSA_REQUIRE(rows % group_rows == 0, "shared_mlp_grouped: group_rows=%lld does not divide rows=%lld", group_rows, rows);
+    if (rows == 0) return PSA_OK;
+    PSA_REQUIRE(x && group_add && out, "shared_mlp_grouped: null buffer");
+    return shared_mlp_chain(rows, 1, x, mlp, group_add, group_rows, out, workspace, workspace_bytes, stream);
 }
 
 // pointnet_sa_module(group_all=True) (pointnet_util.py:59-84,113-127): rows = [xyz, points] (xyz first), MLP, max over the

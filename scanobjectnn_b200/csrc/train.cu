@@ -53,11 +53,11 @@ int reduce_partials(int nparts, int len, const float* partial, float* out, cudaS
     return check_launch("reduce_partials_kernel");
 }
 
-template <int BM, int BN, bool A_KC, bool B_NC, class FA, class FB>
+template <int BM, int BN, bool A_KC, bool B_NC, bool GROUP = false, class FA, class FB>
 static int launch_gemm(const FA& fa, const FB& fb, const GemmOut& o, long long M, int N, long long Kc, int splits, long long k_per_split,
                        cudaStream_t st) {
     dim3 grid((unsigned)((N + BN - 1) / BN), (unsigned)((M + BM - 1) / BM), (unsigned)splits);
-    train_gemm_kernel<BM, BN, A_KC, B_NC, FA, FB><<<grid, kGemmThreads, 0, st>>>(fa, fb, o, M, N, Kc, k_per_split);
+    train_gemm_kernel<BM, BN, A_KC, B_NC, FA, FB, GROUP><<<grid, kGemmThreads, 0, st>>>(fa, fb, o, M, N, Kc, k_per_split);
     return check_launch("train_gemm_kernel");
 }
 
@@ -407,19 +407,21 @@ point_vsum_csr_kernel(int n, int mk, long long total_points, const int* __restri
     dxyz[pt * 3] = x; dxyz[pt * 3 + 1] = y; dxyz[pt * 3 + 2] = z;
 }
 
-// ---- bias gradient of a layer WITHOUT batch norm: db[c] = sum_r dy[r][c]; block = one column, fixed-order tree ----
-__global__ void __launch_bounds__(256) bias_grad_kernel(const GradIn g, long long rows, float* __restrict__ db) {
+// ---- bias gradient of a layer WITHOUT batch norm: db[c] = sum_r dy[r][c]; block = one column of one group of group_rows rows (a single
+// group of all rows for the bias), fixed-order tree: db[grp][c] = sum over the group's rows ----
+__global__ void __launch_bounds__(256) bias_grad_kernel(const GradIn g, long long group_rows, float* __restrict__ db) {
     __shared__ float red[256];
     const int c = blockIdx.x;
+    const long long r0 = (long long)blockIdx.y * group_rows, r1 = r0 + group_rows;
     float t = 0.f;
-    for (long long r = threadIdx.x; r < rows; r += 256) t += g.get(r, c);
+    for (long long r = r0 + threadIdx.x; r < r1; r += 256) t += g.get(r, c);
     red[threadIdx.x] = t;
     __syncthreads();
     for (int o = 128; o > 0; o >>= 1) {
         if ((int)threadIdx.x < o) red[threadIdx.x] += red[threadIdx.x + o];
         __syncthreads();
     }
-    if (threadIdx.x == 0) db[c] = red[0];
+    if (threadIdx.x == 0) db[(size_t)blockIdx.y * gridDim.x + c] = red[0];
 }
 
 // ---- loss ----
@@ -543,6 +545,34 @@ extern "C" int psa_train_dense_fwd(long long rows, int K, int N, const psa_act_i
     }
     if (N <= 64) rc = launch_gemm<128, 64, true, true>(fa, fb, o, rows, N, K, 1, (long long)K + kGemmBK, st);
     else rc = launch_gemm<128, 128, true, true>(fa, fb, o, rows, N, K, 1, (long long)K + kGemmBK, st);
+    if (rc != PSA_OK) return rc;
+    if (stats != nullptr) return reduce_partials((int)tiles_m, 2 * N, o.stat_partial, stats, st);
+    return PSA_OK;
+}
+
+extern "C" int psa_train_dense_fwd_grouped(long long rows, long long group_rows, int K, int N, const psa_act_in* in, const float* W,
+                                           const float* bias, const float* group_add, float* y, float* stats, void* workspace,
+                                           size_t workspace_bytes, psa_stream_t stream) {
+    PSA_REQUIRE(rows >= 0 && group_rows >= 1 && K >= 1 && N >= 1, "train_dense_fwd_grouped: bad dims rows=%lld group_rows=%lld K=%d N=%d",
+                rows, group_rows, K, N);
+    PSA_REQUIRE(rows % group_rows == 0, "train_dense_fwd_grouped: group_rows=%lld does not divide rows=%lld", group_rows, rows);
+    if (rows == 0) return PSA_OK;
+    PSA_REQUIRE(in && in->x && W && group_add && y, "train_dense_fwd_grouped: null buffer");
+    cudaStream_t st = as_stream(stream);
+    const long long tiles_m = (rows + 127) / 128;
+    GemmOut o;
+    o.out = y; o.ld_out = N; o.bias = bias; o.col_skip = 0; o.stat_partial = nullptr;
+    o.group_add = group_add; o.group_rows = group_rows;
+    if (stats != nullptr) {
+        PSA_REQUIRE(workspace != nullptr && workspace_bytes >= (size_t)tiles_m * 2 * N * sizeof(float), "train_dense_fwd_grouped: workspace too small");
+        o.stat_partial = reinterpret_cast<float*>(workspace);
+    }
+    // one pass of the fp32 GEMM, the group rows added in its epilogue before the statistics
+    const ActIn fa(*in);
+    const MatIn fb{W, N};
+    int rc;
+    if (N <= 64) rc = launch_gemm<128, 64, true, true, true>(fa, fb, o, rows, N, K, 1, (long long)K + kGemmBK, st);
+    else rc = launch_gemm<128, 128, true, true, true>(fa, fb, o, rows, N, K, 1, (long long)K + kGemmBK, st);
     if (rc != PSA_OK) return rc;
     if (stats != nullptr) return reduce_partials((int)tiles_m, 2 * N, o.stat_partial, stats, st);
     return PSA_OK;
@@ -749,6 +779,15 @@ extern "C" int psa_train_bias_grad(long long rows, int N, const psa_grad_in* g, 
     PSA_REQUIRE(rows >= 1 && N >= 1 && g && db, "train_bias_grad: bad arguments");
     const GradIn gi(*g);
     bias_grad_kernel<<<N, 256, 0, as_stream(stream)>>>(gi, rows, db);
+    return check_launch("bias_grad_kernel");
+}
+
+extern "C" int psa_train_bias_grad_grouped(long long rows, long long group_rows, int N, const psa_grad_in* g, float* db, psa_stream_t stream) {
+    PSA_REQUIRE(rows >= 1 && group_rows >= 1 && N >= 1 && g && db, "train_bias_grad_grouped: bad arguments");
+    PSA_REQUIRE(rows % group_rows == 0, "train_bias_grad_grouped: group_rows=%lld does not divide rows=%lld", group_rows, rows);
+    PSA_SUPPORTED(rows / group_rows <= 65535, "train_bias_grad_grouped: %lld groups (at most 65535)", rows / group_rows);
+    const GradIn gi(*g);
+    bias_grad_kernel<<<dim3((unsigned)N, (unsigned)(rows / group_rows)), 256, 0, as_stream(stream)>>>(gi, group_rows, db);
     return check_launch("bias_grad_kernel");
 }
 

@@ -140,12 +140,16 @@ struct GemmOut {
     const float* bias;     // per output column, or null
     int col_skip;          // output columns [0, col_skip) are dropped, column c lands at c - col_skip
     float* stat_partial;   // (tiles_m, 2, N) per-tile column sums / sums of squares of the stored values, or null
+    // GROUP instantiations: output row m adds group_add[m / group_rows] (N) before the bias (a per-group input row, e.g. a
+    // global feature's product tiled over a cloud's points)
+    const float* group_add = nullptr;
+    long long group_rows = 0;
 };
 
 // Operand conventions.  A is logically (M, Kc), B is (Kc, N).
 //   A_KC  : functor indexed (row = m, col = kc), contiguous along kc.      !A_KC: functor indexed (row = kc, col = m).
 //   B_NC  : functor indexed (row = kc, col = n), contiguous along n.       !B_NC: functor indexed (row = n, col = kc).
-template <int BM, int BN, bool A_KC, bool B_NC, class FA, class FB>
+template <int BM, int BN, bool A_KC, bool B_NC, class FA, class FB, bool GROUP = false>
 __global__ void __launch_bounds__(kGemmThreads, 2)
 train_gemm_kernel(const FA fa, const FB fb, const GemmOut o, long long M, int N, long long Kc, long long k_per_split) {
     constexpr int TM = BM / 16, TN = BN / 16;                 // 8 or 4
@@ -297,6 +301,13 @@ train_gemm_kernel(const FA fa, const FB fb, const GemmOut o, long long M, int N,
         for (int jh = 0; jh < TN / 4; ++jh) {
             const int n = n0 + (jh == 1 ? BN / 2 : 0) + tx * 4;
             float v[4] = {acc[i][jh * 2].x, acc[i][jh * 2].y, acc[i][jh * 2 + 1].x, acc[i][jh * 2 + 1].y};
+            if constexpr (GROUP) {
+                if (m < M) {
+                    const float* ga = o.group_add + (size_t)(m / o.group_rows) * N;
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) if (n + u < N) v[u] += __ldg(ga + n + u);
+                }
+            }
             if (o.bias != nullptr) {
 #pragma unroll
                 for (int u = 0; u < 4; ++u) if (n + u < N) v[u] += __ldg(o.bias + n + u);

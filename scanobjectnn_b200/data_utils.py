@@ -50,6 +50,12 @@ def load_withmask_h5(h5_filename):
         return f["data"][:], f["label"][:], f["mask"][:]
 
 
+def load_parts_h5(h5_filename):
+    """data_utils.py:271-277 -> (data, label, parts (M,N) per-point part labels)."""
+    with _h5py().File(h5_filename, "r") as f:
+        return f["data"][:], f["label"][:], f["parts"][:]
+
+
 def convert_to_binary_mask(masks):
     """data_utils.py:280-290: 1 = object, 0 = background (mask == -1), float64 like the reference."""
     masks = np.asarray(masks)
@@ -69,3 +75,21 @@ def get_current_data_h5(pcs, labels, num_points, rng: np.random.Generator | None
     if return_indices:
         return sampled, np.asarray(labels)[order], idx_pts[:num_points].astype(np.int32), order
     return sampled, np.asarray(labels)[order]
+
+
+def get_current_data_withmask_h5(pcs, labels, masks, num_points, shuffle: bool = True, rng: np.random.Generator | None = None):
+    """data_utils.py:188-210: get_current_data_h5 that carries the per-point masks (M,N) along with the points.  ``shuffle=False``
+    keeps the first num_points points and the cloud order.  Returns (sampled, labels, sampled_mask)."""
+    idx_pts = np.arange(pcs.shape[1])
+    order = np.arange(len(labels))
+    if shuffle:
+        rng = np.random.default_rng() if rng is None else rng
+        idx_pts = rng.permutation(pcs.shape[1])
+        order = rng.permutation(len(labels))
+    return pcs[:, idx_pts[:num_points], :][order], np.asarray(labels)[order], masks[:, idx_pts[:num_points]][order]
+
+
+def get_current_data_parts_h5(pcs, labels, parts, num_points, rng: np.random.Generator | None = None):
+    """data_utils.py:212-229: get_current_data_h5 that carries the per-point part labels (M,N).  Returns (sampled, labels,
+    sampled_parts)."""
+    return get_current_data_withmask_h5(pcs, labels, parts, num_points, True, rng)

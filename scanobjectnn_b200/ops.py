@@ -18,7 +18,7 @@ from ._lib import PsaMlp, check
 __all__ = [
     "farthest_point_sample", "gather_point", "query_ball_point", "group_point", "select_top_k", "knn_point",
     "three_nn", "three_interpolate", "three_nn_interpolate", "pairwise_distance", "knn", "knn_graph",
-    "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "sa_module_infer",
+    "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "shared_mlp_grouped", "sa_module_infer",
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
 ]
 
@@ -484,6 +484,30 @@ def shared_mlp(x: torch.Tensor, mlp: MlpParams, pool_k: int = 1) -> torch.Tensor
         out = torch.empty((rows // max(pool_k, 1), cl), dtype=torch.float32, device=x.device)
     check(lib.psa_shared_mlp(rows, pool_k, _ptr(x), mlp.prepared(0, rows, pool_k), _ptr(out), _ptr(ws), C.c_size_t(need), _stream()),
           "shared_mlp")
+    return out
+
+
+def shared_mlp_grouped(x: torch.Tensor, mlp: MlpParams, group_add: torch.Tensor) -> torch.Tensor:
+    """shared_mlp whose first layer also adds one row of group_add (G, C_1) per group of rows/G consecutive rows before its
+    affine: x (..., C_0) -> (..., C_L).  With the first weight split as [W_x; W_g], shared_mlp_grouped(x, mlp_x, g . W_g) is
+    shared_mlp(concat([x, tile(g)]), mlp) without the concatenation (psa_shared_mlp_grouped)."""
+    x = _dev(x, torch.float32, "x")
+    group_add = _dev(group_add, torch.float32, "group_add", 2)
+    c0 = x.shape[-1]
+    if c0 != mlp.channels[0]:
+        raise ValueError(f"shared_mlp_grouped: input width {c0} != {mlp.channels[0]}")
+    rows = x.numel() // c0
+    groups = group_add.shape[0]
+    if group_add.shape[1] != mlp.channels[1]:
+        raise ValueError(f"shared_mlp_grouped: group_add width {group_add.shape[1]} != {mlp.channels[1]}")
+    if groups < 1 or rows % groups:
+        raise ValueError(f"shared_mlp_grouped: {groups} groups do not divide {rows} rows")
+    lib = _lib.load()
+    need = lib.psa_shared_mlp_workspace_bytes(rows, mlp.ref)
+    ws = torch.empty((max(need, 4) + 3) // 4, dtype=torch.float32, device=x.device) if need else None
+    out = torch.empty((*x.shape[:-1], mlp.channels[-1]), dtype=torch.float32, device=x.device)
+    check(lib.psa_shared_mlp_grouped(rows, rows // groups, _ptr(x), mlp.prepared(0, rows), _ptr(group_add), _ptr(out), _ptr(ws),
+                                     C.c_size_t(need), _stream()), "shared_mlp_grouped")
     return out
 
 

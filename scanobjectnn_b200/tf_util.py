@@ -89,6 +89,18 @@ class VariableStore(dict):
             self._cache[key] = ops.MlpParams(layers)
         return self._cache[key]
 
+    def grouped_mlp(self, scopes, point_rows: int):
+        """The chain ``scopes`` (ReLU after every layer) whose first layer reads concat([point features (point_rows), global
+        feature]), split for ops.shared_mlp_grouped: (the chain with the first layer's point rows, the plain product over its global
+        rows)."""
+        key = ("grouped_mlp", tuple(scopes), point_rows)
+        if key not in self._cache:
+            layers = [self.folded(s) for s in scopes]
+            w, sc, sh, r = layers[0]
+            glob = ops.MlpParams([(w[point_rows:].contiguous(), None, torch.zeros_like(sh), False)])
+            self._cache[key] = (ops.MlpParams([(w[:point_rows].contiguous(), sc, sh, r)] + layers[1:]), glob)
+        return self._cache[key]
+
     def invalidate(self):
         """Drop the folded conv+BN tensors / prepared weight images.  Called automatically when a variable is assigned,
         updated or deleted; call it yourself after an IN-PLACE edit of a weight tensor.  Inference engines / CUDA graphs

@@ -274,20 +274,37 @@ class MlpTrainer(_TrainOps):
     """Training-mode shared MLP on dense rows -- tf_util.conv1d / conv2d(1x1) / fully_connected chains with batch-statistics batch
     norm + ReLU (tf_util.py:120-185,512-531): the FP modules' MLPs, FC heads, per-point heads.  layers = [(scope, bn), ...];
     a layer with bn=False has no activation (the reference's logits layers).  frozen=True: inference mode -- batch norm on the
-    moving averages (never updated), and a backward that gives the input gradient only."""
+    moving averages (never updated), and a backward that gives the input gradient only.
 
-    def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None, frozen: bool = False):
+    group_channels > 0: the first layer reads concat([x, tile(g)]) with g (groups, group_channels) one row per group of
+    rows / groups consecutive rows (PointNet's segmentation heads, pointnet/models/pointnet_seg.py:81-88).  The first
+    in_channels rows of its weight multiply x, the others g, and the concatenation is never built: g . W_g is a product over the
+    groups that psa_train_dense_fwd_grouped adds per row, and its gradient is the per-group sum of dy
+    (psa_train_bias_grad_grouped)."""
+
+    def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None, frozen: bool = False, groups: int = 0,
+                 group_channels: int = 0):
         super().__init__(params, device, frozen)
-        self.rows, self.in_channels = rows, in_channels
+        self.rows, self.in_channels, self.group_channels = rows, in_channels, group_channels
         f32 = dict(dtype=torch.float32, device=self.dev)
         self.layers: list[_Layer] = []
-        cin, ws_bytes = in_channels, 0
+        cin, ws_bytes = in_channels + group_channels, 0
         for scope, bn in layers:
             ly = _Layer(self.fp, scope, rows, bn, self.dev)
             assert ly.K == cin, (scope, ly.W.shape, cin)
             ws_bytes = max(ws_bytes, self.lib.psa_train_dense_workspace_bytes(rows, ly.K, ly.N), self.lib.psa_bn_bwd_workspace_bytes(ly.N))
             self.layers.append(ly)
             cin = ly.N
+        if group_channels:
+            assert groups >= 1 and rows % groups == 0, (rows, groups)
+            first = self.layers[0]
+            self.groups = groups
+            self.W_x, self.W_g = first.W[:in_channels], first.W[in_channels:]
+            self.dW_x, self.dW_g = first.dW[:in_channels], first.dW[in_channels:]
+            self.g_add = torch.empty((groups, first.N), **f32)
+            self.d_add = torch.empty((groups, first.N), **f32)
+            self.d_g = torch.empty((groups, group_channels), **f32)
+            ws_bytes = max(ws_bytes, self.lib.psa_train_dense_workspace_bytes(groups, group_channels, first.N))
         self.dh = [torch.empty((rows, ly.N), **f32) for ly in self.layers[:-1]]
         self.d_in = torch.empty((rows, in_channels), **f32)
         last = self.layers[-1]
@@ -298,11 +315,24 @@ class MlpTrainer(_TrainOps):
         self.ws = torch.empty(ws_bytes // 4 + 64, **f32)
         self.ws_bytes = ws_bytes
 
-    def forward(self, x: torch.Tensor, bn_decay: float = 0.5) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, bn_decay: float = 0.5, g: torch.Tensor | None = None) -> torch.Tensor:
         assert x.shape == (self.rows, self.in_channels) and x.is_cuda and x.dtype == torch.float32 and x.is_contiguous()
         self.x = x
         self._fold_frozen(self.layers)
-        self._chain_fwd(self.layers, _raw_in(x), bn_decay)
+        if self.group_channels:
+            assert g is not None and g.shape == (self.groups, self.group_channels) and g.is_contiguous()
+            self.g = g
+            first = self.layers[0]
+            check(self.lib.psa_train_dense_fwd(self.groups, self.group_channels, first.N, C.byref(_raw_in(g)), _p(self.W_g), None,
+                                               _p(self.g_add), None, _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "train_dense_fwd")
+            check(self.lib.psa_train_dense_fwd_grouped(self.rows, self.rows // self.groups, self.in_channels, first.N, C.byref(_raw_in(x)),
+                                                       _p(self.W_x), _p(first.b), _p(self.g_add),
+                                                       _p(first.y), _p(first.stats) if first.bn and not self.frozen else None,
+                                                       _p(self.ws), C.c_size_t(self.ws_bytes), _stream()), "train_dense_fwd_grouped")
+            self._bn_finalize(first, self.rows, bn_decay)
+            self._chain_fwd(self.layers[1:], first.act_in(), bn_decay)
+        else:
+            self._chain_fwd(self.layers, _raw_in(x), bn_decay)
         last = self.layers[-1]
         if not last.bn:
             return last.y
@@ -314,8 +344,20 @@ class MlpTrainer(_TrainOps):
     def backward(self, dout: torch.Tensor) -> torch.Tensor:
         """dout = gradient w.r.t. forward()'s return value -> gradient w.r.t. x; the layers' gradients go to the flat bucket"""
         dout = dout.contiguous()
-        self._chain_bwd(self.layers, _grad_dense(self.layers[-1], dout), self.dh, _raw_in(self.x), self.d_in)
-        return self.d_in
+        if not self.group_channels:
+            self._chain_bwd(self.layers, _grad_dense(self.layers[-1], dout), self.dh, _raw_in(self.x), self.d_in)
+            return self.d_in
+        # grouped first layer: (gradient w.r.t. x, gradient w.r.t. g)
+        first, top = self.layers[0], _grad_dense(self.layers[-1], dout)
+        if len(self.layers) > 1:
+            self._chain_bwd(self.layers[1:], top, self.dh[1:], first.act_in(), self.dh[0])
+            top = _grad_dense(first, self.dh[0])
+        self._bn_bwd(first, top)
+        self._products(top, self.rows, self.in_channels, first.N, self.W_x, self.dW_x, _raw_in(self.x), self.d_in)
+        check(self.lib.psa_train_bias_grad_grouped(self.rows, self.rows // self.groups, first.N, C.byref(top), _p(self.d_add), _stream()),
+              "train_bias_grad_grouped")
+        self._products(_plain_grad(self.d_add), self.groups, self.group_channels, first.N, self.W_g, self.dW_g, _raw_in(self.g), self.d_g)
+        return self.d_in, self.d_g
 
 
 class _NodeFn(torch.autograd.Function):
@@ -335,6 +377,21 @@ class _NodeFn(torch.autograd.Function):
         return (None if tr.frozen else _flat_grad_of_layers(tr.fp, tr.layers)), dx.view(ctx.x_shape).clone(), None, None, None
 
 
+class _GroupedNodeFn(torch.autograd.Function):
+    """A grouped MlpTrainer as one autograd node: trainer.forward(x, bn_decay, g), differentiable in x, g and the variables."""
+
+    @staticmethod
+    def forward(ctx, flat, x, g, trainer, bn_decay):
+        ctx.trainer = trainer
+        return trainer.forward(x, bn_decay, g).clone()
+
+    @staticmethod
+    def backward(ctx, dout):
+        tr = ctx.trainer
+        dx, dg = tr.backward(dout)
+        return (None if tr.frozen else _flat_grad_of_layers(tr.fp, tr.layers)), dx.clone(), dg.clone(), None, None
+
+
 def _cached(params: VariableStore, key, make):
     """the trainer cached on `params` under `key`, made on first use (its buffers are allocated once per configuration and shape)"""
     cache = params.__dict__.setdefault("_trainers", {})
@@ -352,15 +409,26 @@ def _flat_and_decay(tr: _TrainOps, bn_decay):
     return tr.fp.flat, 0.5 if bn_decay is None else float(bn_decay)
 
 
-def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False) -> torch.Tensor:
+def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False,
+                 group: torch.Tensor | None = None) -> torch.Tensor:
     """Training-mode shared MLP with autograd: x (..., C_in) -> (..., C_out); layers = [(scope, bn), ...].  Buffers are cached on
-    `params` per (scopes, shape).  frozen=True: inference mode (moving averages, input gradient only)."""
+    `params` per (scopes, shape).  frozen=True: inference mode (moving averages, input gradient only).  group (G, C_g): the first
+    layer reads concat([x, tile(group)]), one row of `group` per x.numel() / C_in / G consecutive rows (e.g. per cloud), without
+    building the concatenation; its weight has C_in + C_g rows, x's first."""
     shape = x.shape
     rows = x.numel() // shape[-1]
-    tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1]),
-                 lambda: MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen))
-    flat, decay = _flat_and_decay(tr, bn_decay)
-    out = _NodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), tr, (), decay)
+    if group is None:
+        tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1]),
+                     lambda: MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen))
+        flat, decay = _flat_and_decay(tr, bn_decay)
+        out = _NodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), tr, (), decay)
+    else:
+        gs = group.shape
+        tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1], "group", gs[0], gs[-1]),
+                     lambda: MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen, groups=gs[0],
+                                        group_channels=gs[-1]))
+        flat, decay = _flat_and_decay(tr, bn_decay)
+        out = _GroupedNodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), group.contiguous(), tr, decay)
     return out.view(*shape[:-1], out.shape[-1])
 
 
