@@ -196,3 +196,31 @@ def pointnet_fp_module(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay,
     interpolated = ops.three_nn_interpolate(xyz1, xyz2, points2)
     new_points1 = torch.cat([interpolated, points1], dim=2) if points1 is not None else interpolated
     return ops.shared_mlp(new_points1, params.mlp(scopes))
+
+
+def pointnet_fp_module_broadcast(xyz1, xyz2, points1, points2, mlp, is_training, bn_decay, scope, bn=True, *, params: VariableStore):
+    """pointnet_fp_module for a known level of ONE point (xyz2 (B,1,3), points2 (B,1,C2), e.g. after a group-all level), without
+    building tile(points2) or its concatenation with points1.
+
+    With one known point the reference's interpolation is a broadcast, exactly: three_nn leaves the two missing neighbours at their
+    initial distance 1e40, inf in float (tf_interpolate.cpp:60-103), and index 0, so the weights (1/max(d,1e-10)) / sum
+    (pointnet_util.py:211-216) are (1, 0, 0) and the interpolated rows are points2 itself.  The first layer's input is then
+    concat([tile(points2), points1]), whose weight rows for points2 come first: those C2 rows run once per cloud (B rows) and the
+    point layer adds the result per group of N1 rows (ops.shared_mlp_grouped; in training mode training.mlp_training(...,
+    group=points2, group_first=True), differentiable in points1 and points2).  Results are those of pointnet_fp_module up to the order
+    of the sums.  A non-finite coordinate makes the reference's weights NaN (inf / inf); this layer does not reproduce that."""
+    if xyz2.shape[1] != 1 or points2.shape[1] != 1:
+        raise ValueError(f"pointnet_fp_module_broadcast: the known level must have one point, got xyz2 {tuple(xyz2.shape)}, "
+                         f"points2 {tuple(points2.shape)}")
+    if points1 is None or not bn:
+        raise NotImplementedError("pointnet_fp_module_broadcast needs skip features points1 and bn=True; use pointnet_fp_module")
+    scopes = [f"{scope}/conv_{i}" for i in range(len(mlp))]
+    b, c2 = points2.shape[0], points2.shape[-1]
+    g = points2.reshape(b, c2)
+    from .training import wants_input_grad
+    frozen = not is_training and wants_input_grad(xyz1, xyz2, points1, points2)
+    if is_training or frozen:
+        from .training import mlp_training
+        return mlp_training(points1, [(sc, True) for sc in scopes], bn_decay, params, frozen=frozen, group=g, group_first=True)
+    rows_mlp, global_mlp = params.grouped_mlp(scopes, points1.shape[-1], group_first=True)
+    return ops.shared_mlp_grouped(points1, rows_mlp, ops.shared_mlp(g, global_mlp))

@@ -53,6 +53,13 @@ class VariableStore(dict):
         if bn:
             self._bn(scope, cout, randomize_bn)
 
+    def add_conv1d(self, scope, cin, cout, bn=True, randomize_bn=False):
+        """tf_util.conv1d with kernel_size 1: the weights are (1, Cin, Cout), the same values add_conv2d would draw"""
+        self[f"{scope}/weights"] = self._xavier((1, cin, cout), cin, cout)
+        self[f"{scope}/biases"] = torch.zeros(cout, device=self.device)
+        if bn:
+            self._bn(scope, cout, randomize_bn)
+
     def add_fc(self, scope, cin, cout, bn=True, randomize_bn=False):
         self[f"{scope}/weights"] = self._xavier((cin, cout), cin, cout)
         self[f"{scope}/biases"] = torch.zeros(cout, device=self.device)
@@ -89,16 +96,18 @@ class VariableStore(dict):
             self._cache[key] = ops.MlpParams(layers)
         return self._cache[key]
 
-    def grouped_mlp(self, scopes, point_rows: int):
+    def grouped_mlp(self, scopes, point_rows: int, group_first: bool = False):
         """The chain ``scopes`` (ReLU after every layer) whose first layer reads concat([point features (point_rows), global
-        feature]), split for ops.shared_mlp_grouped: (the chain with the first layer's point rows, the plain product over its global
-        rows)."""
-        key = ("grouped_mlp", tuple(scopes), point_rows)
+        feature]), or concat([global feature, point features]) with group_first, split for ops.shared_mlp_grouped: (the chain with
+        the first layer's point rows, the plain product over its global rows)."""
+        key = ("grouped_mlp", tuple(scopes), point_rows, group_first)
         if key not in self._cache:
             layers = [self.folded(s) for s in scopes]
             w, sc, sh, r = layers[0]
-            glob = ops.MlpParams([(w[point_rows:].contiguous(), None, torch.zeros_like(sh), False)])
-            self._cache[key] = (ops.MlpParams([(w[:point_rows].contiguous(), sc, sh, r)] + layers[1:]), glob)
+            split = w.shape[0] - point_rows if group_first else point_rows
+            w_pts, w_glob = (w[split:], w[:split]) if group_first else (w[:split], w[split:])
+            glob = ops.MlpParams([(w_glob.contiguous(), None, torch.zeros_like(sh), False)])
+            self._cache[key] = (ops.MlpParams([(w_pts.contiguous(), sc, sh, r)] + layers[1:]), glob)
         return self._cache[key]
 
     def invalidate(self):

@@ -280,10 +280,11 @@ class MlpTrainer(_TrainOps):
     rows / groups consecutive rows (PointNet's segmentation heads, pointnet/models/pointnet_seg.py:81-88).  The first
     in_channels rows of its weight multiply x, the others g, and the concatenation is never built: g . W_g is a product over the
     groups that psa_train_dense_fwd_grouped adds per row, and its gradient is the per-group sum of dy
-    (psa_train_bias_grad_grouped)."""
+    (psa_train_bias_grad_grouped).  group_first: the first layer reads concat([tile(g), x]) instead, so the first group_channels
+    rows of its weight multiply g (a feature-propagation level whose known level is one point, pointnet2_cls_partseg's fa_layer1)."""
 
     def __init__(self, params: VariableStore, rows: int, in_channels: int, layers, device=None, frozen: bool = False, groups: int = 0,
-                 group_channels: int = 0):
+                 group_channels: int = 0, group_first: bool = False):
         super().__init__(params, device, frozen)
         self.rows, self.in_channels, self.group_channels = rows, in_channels, group_channels
         f32 = dict(dtype=torch.float32, device=self.dev)
@@ -299,8 +300,10 @@ class MlpTrainer(_TrainOps):
             assert groups >= 1 and rows % groups == 0, (rows, groups)
             first = self.layers[0]
             self.groups = groups
-            self.W_x, self.W_g = first.W[:in_channels], first.W[in_channels:]
-            self.dW_x, self.dW_g = first.dW[:in_channels], first.dW[in_channels:]
+            x_rows, g_rows = ((slice(group_channels, None), slice(0, group_channels)) if group_first else
+                              (slice(0, in_channels), slice(in_channels, None)))
+            self.W_x, self.W_g = first.W[x_rows], first.W[g_rows]
+            self.dW_x, self.dW_g = first.dW[x_rows], first.dW[g_rows]
             self.g_add = torch.empty((groups, first.N), **f32)
             self.d_add = torch.empty((groups, first.N), **f32)
             self.d_g = torch.empty((groups, group_channels), **f32)
@@ -410,11 +413,11 @@ def _flat_and_decay(tr: _TrainOps, bn_decay):
 
 
 def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False,
-                 group: torch.Tensor | None = None) -> torch.Tensor:
+                 group: torch.Tensor | None = None, group_first: bool = False) -> torch.Tensor:
     """Training-mode shared MLP with autograd: x (..., C_in) -> (..., C_out); layers = [(scope, bn), ...].  Buffers are cached on
     `params` per (scopes, shape).  frozen=True: inference mode (moving averages, input gradient only).  group (G, C_g): the first
     layer reads concat([x, tile(group)]), one row of `group` per x.numel() / C_in / G consecutive rows (e.g. per cloud), without
-    building the concatenation; its weight has C_in + C_g rows, x's first."""
+    building the concatenation; its weight has C_in + C_g rows, x's first (group_first: group's first, concat([tile(group), x]))."""
     shape = x.shape
     rows = x.numel() // shape[-1]
     if group is None:
@@ -424,9 +427,9 @@ def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, froze
         out = _NodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), tr, (), decay)
     else:
         gs = group.shape
-        tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1], "group", gs[0], gs[-1]),
+        tr = _cached(params, ("mlp_frozen" if frozen else "mlp", tuple(layers), rows, shape[-1], "group", gs[0], gs[-1], group_first),
                      lambda: MlpTrainer(params, rows, shape[-1], list(layers), device=x.device, frozen=frozen, groups=gs[0],
-                                        group_channels=gs[-1]))
+                                        group_channels=gs[-1], group_first=group_first))
         flat, decay = _flat_and_decay(tr, bn_decay)
         out = _GroupedNodeFn.apply(flat, x.reshape(rows, shape[-1]).contiguous(), group.contiguous(), tr, decay)
     return out.view(*shape[:-1], out.shape[-1])
