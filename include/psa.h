@@ -258,10 +258,15 @@ PSA_API int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, const 
  * multiple of 128) and nsample 32/64/128 on tc_sa_kernel, dense layers with N = 64 or a multiple of 128 on tc_dense_kernel
  * -- the layers after the first run on the Hopper tensor cores (wgmma) with fp32 accumulation; other shapes
  * run on the fp32-FMA kernels.  The fp32 operands are split into exactly representable 16-bit pieces:
- *   0 (default): two fp16 pieces per operand (22 mantissa bits), three MMAs per product  a1w2 + a2w1 + a1w1  -- the same error
- *      against fp64 as an fp32 FMA chain (1e-5 contract of the tests).  fp16 covers |v| < 65504: every kernel tracks the pieces
- *      it stores (weights too) and raises a device-side flag when a value leaves that range; the call then reruns the op with
- *      bf16x3 operands (launched unconditionally, a no-op unless the flag is set), so results are valid for any fp32 input.
+ *   0 (default): two fp16 pieces per operand, three MMAs per product  a1w2 + a2w1 + a1w1.  Each output column of a weight image
+ *      is scaled by a power of two 2^e_n that brings its largest |w| into [2^10, 2^11) before the split, and 2^-e_n is folded into
+ *      the layer's scale (exact): every weight keeps 22 bits relative to the largest weight of its column, at any weight scale.
+ *      Activations are split unscaled and keep an absolute 2^-25 (fp16's subnormal step), which is below the 1e-5 contract
+ *      of the tests for the O(1) post-batch-norm activations and coordinates the models feed their layers; with batch norm
+ *      calibrated to the data (folded scales up to 31.6 gamma) the layers stay within 1e-5 of fp64.  fp16 covers |v| < 65504:
+ *      the kernels track the activation pieces they store and raise a device-side flag when one leaves that range or a weight
+ *      is not finite; the call then reruns the op with bf16x3 operands (launched unconditionally, a no-op unless the flag is set),
+ *      so results are valid for any fp32 input.
  *   2: three bf16 pieces per operand, six MMAs per product (small terms first) -- any magnitude, twice the tensor work.
  *   1: fp32-FMA kernels only.
  * Weight images (psa_prepare_weight_image) are format-specific: psa_mlp_image_plan returns the format of the current mode in its

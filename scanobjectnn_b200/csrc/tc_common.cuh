@@ -144,8 +144,9 @@ __device__ __forceinline__ bool f16x2_overflowed(uint32_t m) { return (m & 0x7c0
 //   NP = 3: three bf16 pieces (a = a1 + a2 + a3 exactly), six MMAs  a1w3 + a2w2 + a3w1 + a1w2 + a2w1 + a1w1  (small products first: the
 //           accumulator add truncates) -- any fp32 magnitude;
 //   NP = 2: two fp16 pieces (22 mantissa bits; the tail below 2^-24 absolute is dropped), three MMAs  a1w2 + a2w1 + a1w1 -- half
-//           the tensor work, same accuracy against fp64 as the fp32 FMA kernels, valid while |a| < 65504 (the kernels track the
-//           stored pieces and raise a flag otherwise; the launcher then reruns the op on the NP = 3 instantiation).
+//           the tensor work, valid while |a| < 65504 (the kernels track the stored activation pieces and raise a flag otherwise;
+//           the launcher then reruns the op on the NP = 3 instantiation).  Weights are split after a per-column power-of-two
+//           scaling (tc_mlp.cu), so they keep 22 bits at any scale; activations keep an absolute 2^-25.
 template <int NP> struct Split;
 template <> struct Split<3> {
     static constexpr uint32_t kFmt = kFmtBF16;

@@ -21,9 +21,10 @@
 //                             statistics in the epilogue)
 // fp32 parity: operands are quantised by this code, so the tensor core only ever sees exactly representable values; fp32
 // accumulation in the tensor core truncates, hence small terms first and K cut into <= 128-wide pieces (tests hold 1e-5 vs fp64).
-//   NP = 2 (inference default): two fp16 pieces, three MMAs per product; every kernel tracks the leading pieces it stores and raises
-//           a device-side flag when a value leaves the fp16 range -- the launchers then rerun the op on the NP = 3 instantiation
-//           (enqueued unconditionally, a no-op unless the flag is set: `run_if`);
+//   NP = 2 (inference default): two fp16 pieces, three MMAs per product, weights scaled per output column by a power of two (see
+//           the weight images below); every kernel tracks the leading activation pieces it stores and raises a device-side flag
+//           when one leaves the fp16 range or a weight is not finite -- the launchers then rerun the op on the NP = 3
+//           instantiation (enqueued unconditionally, a no-op unless the flag is set: `run_if`);
 //   NP = 3 (psa_set_mlp_mode(2), the guarded rerun, the training forward): three bf16 pieces, six MMAs per product.
 // Levels the SA kernel cannot hold run on the fp32-FMA fused kernel of mlp.cu.
 #include <float.h>
@@ -47,12 +48,22 @@ constexpr int kMaxTcLayers = 2;
 //   block (nt, kc) covers output channels [nt*Nt, nt*Nt+Nt) x input channels [kc*64, kc*64+64): NP 16-bit pieces
 //   (every piece exactly representable), each [Nt][64] K-major SWIZZLE_128B, Nt*128 B per piece; blocks stored in (nt major,
 //   kc minor) order.  2 NP bytes per weight.
+//   fp16x2 images hold column n of W times 2^e_n, with e_n chosen so that the column's largest |w| lands in [2^10, 2^11)
+//   (tc_col_scale_kernel): the two fp16 pieces then keep 22 bits relative to that weight whatever the scale of the weights.
+//   Unscaled, a weight below 0.125 has a subnormal second piece and keeps only an absolute 2^-25, which batch norm calibrated
+//   to small weights multiplies by up to 31.6 gamma.  The image carries 2^-e_n per column; the kernels fold it into the scale
+//   of their epilogue, and bring what they add to the accumulators before it into the same units (exact: powers of two).
 // ------------------------------------------------------------------------------------------------------------------
 // np = pieces per weight: 3 (bf16x3, 6 bytes per weight) or 2 (fp16x2, 4 bytes); see Split<NP> in tc_common.cuh
 __host__ __device__ constexpr uint32_t tc_block_bytes(int Nt, int np) { return (uint32_t)Nt * 128u * (uint32_t)np; }
 __host__ __device__ inline size_t tc_image_bytes(int K, int N, int np) { return (size_t)K * N * 2u * (size_t)np; }     // independent of the tile width
-// an image allocation = the blocks + a 256-byte trailer whose first word is set when a weight left the fp16 range (np = 2)
-__host__ __device__ inline size_t tc_image_alloc_bytes(int K, int N, int np) { return ((tc_image_bytes(K, N, np) + 255) & ~(size_t)255) + 256; }
+// an image allocation = the blocks, np = 2: the N column factors 2^-e_n (fp32), then a 256-byte trailer whose first word is set
+// when a weight is not finite (np = 2)
+__host__ __device__ inline size_t tc_image_colscale_off(int K, int N, int np) { return (tc_image_bytes(K, N, np) + 255) & ~(size_t)255; }
+__host__ __device__ inline size_t tc_image_trailer_off(int K, int N, int np) {
+    return tc_image_colscale_off(K, N, np) + (np == 2 ? ((size_t)N * 4u + 255) & ~(size_t)255 : 0);
+}
+__host__ __device__ inline size_t tc_image_alloc_bytes(int K, int N, int np) { return tc_image_trailer_off(K, N, np) + 256; }
 
 struct TcArgs {
     long long groups;      // neighbourhoods = b*m
@@ -82,9 +93,10 @@ struct TcArgs {
     unsigned int* tile_counter;   // zeroed before the launch: tiles are handed out dynamically (CTAs that start late or
                                   // share their SM with another stream's kernels simply take fewer)
     int np;                       // operand pieces: 2 (fp16x2) or 3 (bf16x3)
-    unsigned int* ovf;            // np = 2: set to 1 when an activation or weight left the fp16 range (the result is then invalid)
+    unsigned int* ovf;            // np = 2: set to 1 when an activation left the fp16 range or a weight is not finite (the result is then invalid)
     const unsigned int* run_if;   // non-null: the launch is a no-op unless *run_if != 0 (the np = 3 rerun of a flagged launch)
-    const unsigned int* wflag[kMaxTcLayers];   // np = 2: trailer word of each weight image
+    const unsigned int* wflag[kMaxTcLayers];     // np = 2: trailer word of each weight image
+    const float* colscale[kMaxTcLayers];         // np = 2: column factors 2^-e_n of each weight image (folded into the layer's scale)
 };
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -133,24 +145,57 @@ constexpr int kImageF16x2 = 0x200;       // .. or two fp16 pieces
 constexpr int kImageFlags = kImageBf16x3 | kImageF16x2;
 __host__ __device__ inline int image_flag(int np) { return np == 2 ? kImageF16x2 : kImageBf16x3; }
 
+// fp16x2 images: the column factor 2^-e_n of every column of W (K x N) into colscale.  Block (32, 8): 32 columns, the rows strided
+// over 8 threads.  A column holding a non-finite weight keeps e_n = 0 and sets the trailer word (the op is then rerun with bf16x3
+// operands, which give what fp32 gives); finite weights scaled this way cannot leave the fp16 range.  e_n <= 64 keeps 2^-e_n and
+// the scales it is folded into normal (columns of weights below 2^-54 are scaled by 2^64 only).
+__global__ void __launch_bounds__(256) tc_col_scale_kernel(int K, int N, const float* __restrict__ W, float* __restrict__ colscale,
+                                                           unsigned int* __restrict__ trailer) {
+    __shared__ float s_max[8][32];
+    __shared__ int s_bad[8][32];
+    const int n = blockIdx.x * 32 + threadIdx.x;
+    float m = 0.f;
+    bool bad = false;
+    if (n < N)
+        for (int k = threadIdx.y; k < K; k += 8) {
+            const float w = __ldg(W + (size_t)k * N + n);
+            bad = bad || !isfinite(w);
+            m = fmaxf(m, fabsf(w));
+        }
+    s_max[threadIdx.y][threadIdx.x] = m;
+    s_bad[threadIdx.y][threadIdx.x] = bad;
+    __syncthreads();
+    if (threadIdx.y != 0 || n >= N) return;
+    for (int y = 1; y < 8; ++y) { m = fmaxf(m, s_max[y][threadIdx.x]); bad = bad || s_bad[y][threadIdx.x]; }
+    int e = 0;
+    if (!bad && m > 0.f) e = min(137 - (int)(__float_as_uint(m) >> 23), 64);   // m in [2^(E-127), 2^(E-126)): m 2^e in [2^10, 2^11)
+    colscale[n] = __int_as_float((127 - e) << 23);
+    if (bad) atomicOr(trailer, 1u);
+}
+
+// 1 / x, exactly, for a normal power of two x (the column factors): the exponent field mirrored about the bias, one integer
+// subtraction instead of a correctly rounded reciprocal's slow path
+__device__ __forceinline__ float pow2_rcp(float x) { return __int_as_float(0x7f000000 - __float_as_int(x)); }
+
+// colscale: fp16x2, the column factors of tc_col_scale_kernel (the weights are stored divided by them, exactly); bf16x3: null
 template <int NP>
-__global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float* __restrict__ W, uint8_t* __restrict__ image,
-                                       unsigned int* __restrict__ trailer, const unsigned int* __restrict__ run_if) {
+__global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float* __restrict__ W, const float* __restrict__ colscale,
+                                       uint8_t* __restrict__ image, const unsigned int* __restrict__ run_if) {
     if (run_if != nullptr && *run_if == 0u) return;
     const int KC = Kp / 64;
     const uint32_t bb = tc_block_bytes(Nt, NP), piece = (uint32_t)Nt * 128u;
-    uint32_t ovf = 0u;
+    uint32_t unused = 0u;                  // split_pair's range tracking: scaled finite weights stay inside the fp16 range
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < Kp * N; e += gridDim.x * blockDim.x) {
         const int n = e % N, k = e / N;
-        const float w = k < K ? __ldg(W + e) : 0.f;
+        float w = k < K ? __ldg(W + e) : 0.f;
+        if (NP == 2) w *= pow2_rcp(__ldg(colscale + n));
         uint32_t pc[NP];
-        split_pair<NP>(w, 0.f, pc, ovf);
+        split_pair<NP>(w, 0.f, pc, unused);
         uint8_t* blk = image + (size_t)((n / Nt) * KC + (k >> 6)) * bb;
         const uint32_t off = swz_off_bf16(n % Nt, k & 63, Nt);
 #pragma unroll
         for (int i = 0; i < NP; ++i) *reinterpret_cast<uint16_t*>(blk + i * piece + off) = (uint16_t)(pc[i] & 0xffffu);
     }
-    if (NP == 2 && f16x2_overflowed(ovf)) atomicOr(trailer, 1u);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -290,10 +335,11 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         w1c[i] = a.w1c ? __ldg(a.w1c + i) * sc : 0.f;
     }
     for (int i = tid; i < C1; i += kSaThreads) { s1[i] = a.s1 ? __ldg(a.s1 + i) : 1.f; t1[i] = __ldg(a.t1 + i); }
+    // the column factors of the fp16x2 weight images are folded into the tensor layers' scales
 #pragma unroll
     for (int l = 0; l < NL; ++l)
         for (int i = tid; i < a.Ntot[l]; i += kSaThreads) {
-            (l == 0 ? sl0 : slL)[i] = a.s[l] ? __ldg(a.s[l] + i) : 1.f;
+            (l == 0 ? sl0 : slL)[i] = (a.s[l] ? __ldg(a.s[l] + i) : 1.f) * (NP == 2 ? __ldg(a.colscale[l] + i) : 1.f);
             (l == 0 ? tl0 : tlL)[i] = __ldg(a.t[l] + i);
         }
     if (tid == 0) {
@@ -667,6 +713,7 @@ struct TcDenseArgs {
     unsigned int* ovf = nullptr;
     const unsigned int* run_if = nullptr;
     const unsigned int* wflag = nullptr;
+    const float* colscale = nullptr;   // np = 2: column factors 2^-e_n of the weight image (folded into the epilogue's scale)
     // zeroed before the launch: tiles are claimed from it (a CTA that starts late or shares its SM with another stream's
     // kernels simply takes fewer); null: CTA i takes tiles i, i + grid, ...
     unsigned int* tile_counter = nullptr;
@@ -707,6 +754,7 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
     __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
     __shared__ int s_tile[S];                                       // the tile a stage belongs to, -1: no more tiles
     __shared__ float s_red[2][8][Nt];
+    __shared__ __align__(16) float s_aff[2][3][Nt];                 // [tile parity]: scale x column factor, shift, 1 / column factor
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     const int KC = a.Kp / 64, NTC = a.N / Nt;
@@ -774,12 +822,24 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
     const int g = lane >> 2, t = lane & 3;
     uint32_t ovf = 0u;
     uint32_t q = 0;                                                 // ring uses
-    for (;;) {
+    for (uint32_t par = 0;; par ^= 1u) {
         mbar_wait(&s_full[q % S], (q / S) & 1u);
         const int tile = s_tile[q % S];
         if (tile < 0) break;
         const long long row0 = (long long)(tile / NTC) * 128;
         const int nt = tile % NTC;
+        // the tile's affine through shared memory, loaded once per column under the K loop and read by the epilogue after the
+        // barrier in front of it; fp16x2: the column factor 2^-e_n joins the scale, its inverse brings what the epilogue adds to
+        // the accumulators into their units.  Two buffers by tile parity: the write for this tile follows the barrier of the last
+        // one, so it cannot overtake the epilogue of the tile before.
+        float (&aff)[3][Nt] = s_aff[par];
+        if (tid < Nt) {
+            const int col = nt * Nt + tid;
+            const float cs = NP == 2 ? __ldg(a.colscale + col) : 1.f;
+            aff[0][tid] = (a.scale ? __ldg(a.scale + col) : 1.f) * cs;
+            aff[1][tid] = a.shift ? __ldg(a.shift + col) : 0.f;
+            aff[2][tid] = NP == 2 ? pow2_rcp(cs) : 1.f;
+        }
         const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
         const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
 
@@ -857,6 +917,7 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
         q += KC;
 
         // ---- epilogue ----
+        unit_bar_sync(1, kDenseConsumers);                          // the tile's affine is in `aff`
         float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
         if (a.xyz3 != nullptr)
 #pragma unroll
@@ -865,7 +926,9 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
 #pragma unroll
                     for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz3 + (size_t)r[i] * 3 + k);
         // the per-group input, added to the accumulators in a pass of its own so that the loop below is the same code with or
-        // without it.  Rows g and g + 8 may lie in different groups, and groups need not align with the 128-row tiles.
+        // without it.  Rows g and g + 8 may lie in different groups, and groups need not align with the 128-row tiles.  fp16x2:
+        // the accumulators hold the product times 2^e_n, and so must what is added to them (exact, the rounding of the sum is
+        // that of the unscaled one)
         if (a.group_add != nullptr)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
@@ -876,8 +939,9 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
 #pragma unroll
                         for (int j = 0; j < 8; ++j) {
                             const float2 u = __ldg(reinterpret_cast<const float2*>(ga + c * 64 + 8 * j));
-                            acc[c][4 * j + 2 * i] += u.x;
-                            acc[c][4 * j + 2 * i + 1] += u.y;
+                            const float2 f = *reinterpret_cast<const float2*>(&aff[2][c * 64 + 8 * j + 2 * t]);
+                            acc[c][4 * j + 2 * i] = fmaf(u.x, f.x, acc[c][4 * j + 2 * i]);
+                            acc[c][4 * j + 2 * i + 1] = fmaf(u.y, f.y, acc[c][4 * j + 2 * i + 1]);
                         }
                 }
 #pragma unroll
@@ -889,9 +953,12 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int col = nt * Nt + cl + e;
-                    const float sc = a.scale ? __ldg(a.scale + col) : 1.f, sh = a.shift ? __ldg(a.shift + col) : 0.f;
+                    const float sc = aff[0][cl + e], sh = aff[1][cl + e];
                     float w0 = 0.f, w1 = 0.f, w2 = 0.f;
-                    if (a.xyz3 != nullptr) { w0 = __ldg(a.w3 + col); w1 = __ldg(a.w3 + a.N + col); w2 = __ldg(a.w3 + 2 * a.N + col); }
+                    if (a.xyz3 != nullptr) {
+                        const float f = aff[2][cl + e];
+                        w0 = __ldg(a.w3 + col) * f; w1 = __ldg(a.w3 + a.N + col) * f; w2 = __ldg(a.w3 + 2 * a.N + col) * f;
+                    }
 #pragma unroll
                     for (int i = 0; i < 2; ++i) {
                         float x = acc[c][4 * j + 2 * i + e];
@@ -993,20 +1060,27 @@ int tc_dense_nt(long long rows, int N) {
     return (wide ? 128 : 64) | image_flag(g_tc_np);
 }
 
-// builds the image of W (K x N, rows K..Kp zero) in the format `Nt` carries (width | format flag); zeroes the trailer first
+// builds the image of W (K x N, rows K..Kp zero) in the format `Nt` carries (width | format flag); fp16x2: zeroes the trailer and
+// computes the column factors first
 static int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* image, cudaStream_t st, const unsigned int* run_if = nullptr) {
-    const int np = (Nt & kImageF16x2) ? 2 : 3;
-    unsigned int* trailer = reinterpret_cast<unsigned int*>(image + ((tc_image_bytes(Kp, N, np) + 255) & ~(size_t)255));
-    if (np == 2) {
+    if (Nt & kImageF16x2) {
+        unsigned int* trailer = reinterpret_cast<unsigned int*>(image + tc_image_trailer_off(Kp, N, 2));
+        float* colscale = reinterpret_cast<float*>(image + tc_image_colscale_off(Kp, N, 2));
         PSA_CUDA(cudaMemsetAsync(trailer, 0, 256, st));
-        tc_prep_weights_kernel<2><<<(Kp * N + 255) / 256, 256, 0, st>>>(K, Kp, N, Nt & ~kImageFlags, W, image, trailer, run_if);
+        tc_col_scale_kernel<<<(N + 31) / 32, dim3(32, 8), 0, st>>>(K, N, W, colscale, trailer);
+        int rc = check_launch("tc_col_scale_kernel");
+        if (rc != PSA_OK) return rc;
+        tc_prep_weights_kernel<2><<<(Kp * N + 255) / 256, 256, 0, st>>>(K, Kp, N, Nt & ~kImageFlags, W, colscale, image, run_if);
     } else {
-        tc_prep_weights_kernel<3><<<(Kp * N + 255) / 256, 256, 0, st>>>(K, Kp, N, Nt & ~kImageFlags, W, image, trailer, run_if);
+        tc_prep_weights_kernel<3><<<(Kp * N + 255) / 256, 256, 0, st>>>(K, Kp, N, Nt & ~kImageFlags, W, nullptr, image, run_if);
     }
     return check_launch("tc_prep_weights_kernel");
 }
-static const unsigned int* image_trailer(const uint8_t* image, int Kp, int N, int np) {
-    return reinterpret_cast<const unsigned int*>(image + ((tc_image_bytes(Kp, N, np) + 255) & ~(size_t)255));
+static const unsigned int* image_trailer(const uint8_t* image, int Kp, int N) {
+    return reinterpret_cast<const unsigned int*>(image + tc_image_trailer_off(Kp, N, 2));
+}
+static const float* image_colscale(const uint8_t* image, int Kp, int N) {
+    return reinterpret_cast<const float*>(image + tc_image_colscale_off(Kp, N, 2));
 }
 
 template <int NP, int NC>
@@ -1064,7 +1138,7 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
     }
     if (prebuilt == nullptr) { rc = build_image(K, Kp, N, Nt | kImageF16x2, W, ws_img, st); if (rc != PSA_OK) return rc; }
     a.image = prebuilt ? prebuilt : ws_img;
-    a.ovf = flag; a.wflag = image_trailer(a.image, Kp, N, 2);
+    a.ovf = flag; a.wflag = image_trailer(a.image, Kp, N); a.colscale = image_colscale(a.image, Kp, N);
     rc = launch_tc_dense_np<2>(a, Nt, st);
     if (rc != PSA_OK) return rc;
     // guarded rerun, a no-op unless the fp16x2 pass raised the flag.  A prebuilt image carries its bf16x3 twin behind the fp16x2
@@ -1075,7 +1149,7 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
         rc = build_image(K, Kp, N, Nt | kImageBf16x3, W, img3, st, flag);
         if (rc != PSA_OK) return rc;
     }
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.run_if = flag; a.tile_counter = counters + 1;
+    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = flag; a.tile_counter = counters + 1;
     return launch_tc_dense_np<3>(a, Nt, st);
 }
 
@@ -1230,7 +1304,9 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
         t.xyz = xyz; t.new_xyz = new_xyz; t.idx = idx; t.out = out; t.uf = uf;
         t.w1x = mlp->weight[0]; t.s1 = mlp->scale[0]; t.t1 = mlp->shift[0]; t.relu1 = mlp->relu[0];
         t.ovf = nullptr; t.run_if = nullptr; t.w1c = w1c;
-        for (int l = 0; l < t.nl; ++l) { t.s[l] = mlp->scale[1 + l]; t.t[l] = mlp->shift[1 + l]; t.relu[l] = mlp->relu[1 + l]; t.wflag[l] = nullptr; }
+        for (int l = 0; l < t.nl; ++l) {
+            t.s[l] = mlp->scale[1 + l]; t.t[l] = mlp->shift[1 + l]; t.relu[l] = mlp->relu[1 + l]; t.wflag[l] = nullptr; t.colscale[l] = nullptr;
+        }
     };
     fill(a);
     for (int l = 0; l < a.nl; ++l) {
@@ -1239,7 +1315,7 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
         uint8_t* own = a.np == 2 ? img2[l] : img3[l];
         if (pre == nullptr) { rc = build_image(a.Kd[l], a.Kd[l], a.Ntot[l], nt_img, mlp->weight[1 + l], own, st); if (rc != PSA_OK) return rc; }
         a.image[l] = pre ? pre : own;
-        if (a.np == 2) a.wflag[l] = image_trailer(a.image[l], a.Kd[l], a.Ntot[l], 2);
+        if (a.np == 2) { a.wflag[l] = image_trailer(a.image[l], a.Kd[l], a.Ntot[l]); a.colscale[l] = image_colscale(a.image[l], a.Kd[l], a.Ntot[l]); }
     }
     a.tile_counter = words;
     if (a.np == 3) return launch_tc_sa_np<3>(a, st);

@@ -257,9 +257,9 @@ def test_sa_conv1_prebn_nonfinite_inputs_keep_reference_indices():
 
 @pytest.mark.parametrize("where", ["features", "weights", "inner"])
 def test_fp16_range_guard_reruns_on_bf16x3(where):
-    """mode 0 splits operands into two fp16 pieces (|value| < 65504).  Features, weights or an inner activation beyond that range
-    raise the device-side flag and the op is rerun with bf16x3 operands inside the same call: the result still meets the contract
-    (relative to its own magnitude); nothing is clamped, nothing becomes inf."""
+    """mode 0 splits operands into two fp16 pieces (|value| < 65504).  Features or an inner activation beyond that range raise the
+    device-side flag and the op is rerun with bf16x3 operands inside the same call; weights beyond it are scaled into it per
+    column.  The result still meets the contract (relative to its own magnitude); nothing is clamped, nothing becomes inf."""
     p = _store(91)
     mlp = [128, 128, 256]
     add_sa_module_params(p, "sa", 3 + 64, mlp, randomize_bn=True)
