@@ -404,6 +404,13 @@ PSA_API int psa_bn_finalize(int C, long long count, const float* stats, const fl
                             float decay, float* moving_mean, float* moving_var, float* scale, float* shift,
                             float* mean_inv, psa_stream_t stream);
 
+/* The same from the layer's output y (rows, C) itself: the mean, then the centred sum of squares, both in fp64.  For layers whose
+ * output is materialised and short (the FC head, rows = batch): there the mean of a column can be large against its spread, and a
+ * variance taken as E[y^2] - mean^2 from fp32 sums loses its digits. */
+PSA_API int psa_bn_finalize_rows(long long rows, int C, const float* y, const float* gamma, const float* beta, float decay,
+                                 float* moving_mean, float* moving_var, float* scale, float* shift, float* mean_inv,
+                                 psa_stream_t stream);
+
 /* relu(BN(y)) then max over each run of pool_k rows: pooled (groups, C), argk (groups, C) = first winning row. */
 PSA_API int psa_train_pool_fwd(long long groups, int pool_k, int C, const float* y, const float* scale,
                                const float* shift, float* pooled, int* argk, psa_stream_t stream);

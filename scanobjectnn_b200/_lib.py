@@ -88,6 +88,7 @@ SIGNATURES = {
     "psa_train_dense_fwd_grouped": [_ll, _ll, _i, _i, _ain, _p, _p, _p, _p, _p, _p, _sz, _p],
     "psa_train_bias_grad_grouped": [_ll, _ll, _i, _gin, _p, _p],
     "psa_bn_finalize": [_i, _ll, _p, _p, _p, _f, _p, _p, _p, _p, _p, _p],
+    "psa_bn_finalize_rows": [_ll, _i, _p, _p, _p, _f, _p, _p, _p, _p, _p, _p],
     "psa_train_pool_fwd": [_ll, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_bn_bwd_coeffs": [_ll, _i, _gin, _p, _p, _p, _p, _p, _p, _p, _p, _sz, _p],
     "psa_sa_conv1_bwd": [_i, _i, _i, _i, _i, _p, _p, _p, _gin, _p, _p, _p, _sz, _p],

@@ -93,14 +93,11 @@ __global__ void __launch_bounds__(1024) col_stats_kernel(long long M, int N, con
 }
 
 // ---- batch-norm finalize ----
-__global__ void bn_finalize_kernel(int C, double inv_count, const float* __restrict__ stats, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float decay, float* __restrict__ moving_mean,
-                                   float* __restrict__ moving_var, float* __restrict__ scale, float* __restrict__ shift,
-                                   float* __restrict__ mean_inv) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    const double mean = (double)stats[c] * inv_count;
-    double var = (double)stats[C + c] * inv_count - mean * mean;       // biased (tf.nn.moments / contrib batch_norm)
+// one channel: batch mean and biased variance -> scale / shift, mean_inv, moving averages
+__device__ __forceinline__ void bn_finalize_channel(int C, int c, double mean, double var, const float* __restrict__ gamma,
+                                                    const float* __restrict__ beta, float decay, float* __restrict__ moving_mean,
+                                                    float* __restrict__ moving_var, float* __restrict__ scale, float* __restrict__ shift,
+                                                    float* __restrict__ mean_inv) {
     if (var < 0.0) var = 0.0;
     const double inv = 1.0 / sqrt(var + 1e-3);
     const float sc = (float)((double)gamma[c] * inv);
@@ -109,6 +106,54 @@ __global__ void bn_finalize_kernel(int C, double inv_count, const float* __restr
     if (mean_inv != nullptr) { mean_inv[c] = (float)mean; mean_inv[C + c] = (float)inv; }
     if (moving_mean != nullptr) moving_mean[c] = decay * moving_mean[c] + (1.f - decay) * (float)mean;
     if (moving_var != nullptr) moving_var[c] = decay * moving_var[c] + (1.f - decay) * (float)var;
+}
+
+__global__ void bn_finalize_kernel(int C, double inv_count, const float* __restrict__ stats, const float* __restrict__ gamma,
+                                   const float* __restrict__ beta, float decay, float* __restrict__ moving_mean,
+                                   float* __restrict__ moving_var, float* __restrict__ scale, float* __restrict__ shift,
+                                   float* __restrict__ mean_inv) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const double mean = (double)stats[c] * inv_count;
+    const double var = (double)stats[C + c] * inv_count - mean * mean;    // biased (tf.nn.moments / contrib batch_norm)
+    bn_finalize_channel(C, c, mean, var, gamma, beta, decay, moving_mean, moving_var, scale, shift, mean_inv);
+}
+
+// the same from a materialised y (M, N) in two fp64 passes: the mean, then the centred sum of squares.  E[y^2] - mean^2 from fp32
+// sums loses the variance of a column whose mean is large against its spread: DGCNN's fc1 / T-net tfc1 after the max over the
+// points, where mean^2 / var reaches ~4000 and 1/sigma lost ~1e-4.  Block = 32 columns x 32 row lanes, fixed-order tree.
+__global__ void __launch_bounds__(1024)
+bn_finalize_rows_kernel(long long M, int N, const float* __restrict__ y, const float* __restrict__ gamma, const float* __restrict__ beta,
+                        float decay, float* __restrict__ moving_mean, float* __restrict__ moving_var, float* __restrict__ scale,
+                        float* __restrict__ shift, float* __restrict__ mean_inv) {
+    __shared__ double red[32][33];
+    __shared__ double mean_s[32];
+    const int ex = threadIdx.x & 31, rl = threadIdx.x >> 5;
+    const int n = blockIdx.x * 32 + ex;
+    double s = 0.0;
+    if (n < N)
+        for (long long m = rl; m < M; m += 32) s += (double)y[m * N + n];
+    red[rl][ex] = s;
+    __syncthreads();
+    if (rl == 0) {
+        double a = 0.0;
+#pragma unroll
+        for (int k = 0; k < 32; ++k) a += red[k][ex];
+        mean_s[ex] = a / (double)M;
+    }
+    __syncthreads();
+    const double mean = mean_s[ex];
+    double q = 0.0;
+    if (n < N)
+        for (long long m = rl; m < M; m += 32) { const double d = (double)y[m * N + n] - mean; q += d * d; }
+    red[rl][ex] = q;                                           // the mean's tree was read before the barrier above
+    __syncthreads();
+    if (rl == 0 && n < N) {
+        double b = 0.0;
+#pragma unroll
+        for (int k = 0; k < 32; ++k) b += red[k][ex];
+        bn_finalize_channel(N, n, mean, b / (double)M, gamma, beta, decay, moving_mean, moving_var, scale, shift, mean_inv);
+    }
 }
 
 // ---- max-pool over runs of pool_k rows with the first winning row ----
@@ -641,6 +686,14 @@ extern "C" int psa_bn_finalize(int C, long long count, const float* stats, const
     bn_finalize_kernel<<<(C + 127) / 128, 128, 0, as_stream(stream)>>>(C, 1.0 / (double)count, stats, gamma, beta, decay, moving_mean, moving_var,
                                                                         scale, shift, mean_inv);
     return check_launch("bn_finalize_kernel");
+}
+
+extern "C" int psa_bn_finalize_rows(long long rows, int C, const float* y, const float* gamma, const float* beta, float decay,
+                                    float* moving_mean, float* moving_var, float* scale, float* shift, float* mean_inv, psa_stream_t stream) {
+    PSA_REQUIRE(rows >= 1 && C >= 1 && y && gamma && beta && scale && shift, "bn_finalize_rows: bad arguments");
+    bn_finalize_rows_kernel<<<(C + 31) / 32, 1024, 0, as_stream(stream)>>>(rows, C, y, gamma, beta, decay, moving_mean, moving_var, scale,
+                                                                           shift, mean_inv);
+    return check_launch("bn_finalize_rows_kernel");
 }
 
 extern "C" int psa_train_pool_fwd(long long groups, int pool_k, int C, const float* y, const float* scale, const float* shift, float* pooled,

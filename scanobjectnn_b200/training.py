@@ -48,6 +48,7 @@ class LevelSpec:
 SSG_LEVELS = [LevelSpec("layer1", 512, 0.2, 32, [64, 64, 128]), LevelSpec("layer2", 128, 0.4, 64, [128, 128, 256]),
               LevelSpec("layer3", None, None, None, [256, 512, 1024], group_all=True)]
 SSG_HEAD = [("fc1", 512, True, 0.5), ("fc2", 256, True, 0.5), ("fc3", None, False, None)]   # (scope, width, bn, keep_prob)
+STATS_FROM_ROWS = 1024       # dense layers of at most this many rows take batch statistics from their output (psa_bn_finalize_rows)
 
 
 class FlatParams:
@@ -196,11 +197,18 @@ class _TrainOps:
                                            _p(ly.mov_var), _p(ly.scale), _p(ly.shift), _p(ly.mean_inv), _stream()), "bn_finalize")
 
     def _layer_fwd(self, ly: _Layer, a: PsaActIn, decay: float):
-        """y = a . W + b (+ batch statistics), then batch norm's scale / shift"""
+        """y = a . W + b (+ batch statistics), then batch norm's scale / shift.  A layer of at most STATS_FROM_ROWS rows (the FC head,
+        rows = batch) takes its statistics from y in two fp64 passes instead of the GEMM's sums: after a max over the points a column's
+        mean can be ~60 times its spread, and E[y^2] - mean^2 from fp32 sums then loses the variance's digits."""
+        from_rows = ly.bn and not self.frozen and ly.rows <= STATS_FROM_ROWS
         check(self.lib.psa_train_dense_fwd(ly.rows, ly.K, ly.N, C.byref(a), _p(ly.W), _p(ly.b), _p(ly.y),
-                                           _p(ly.stats) if ly.bn and not self.frozen else None, _p(self.ws), C.c_size_t(self.ws_bytes),
-                                           _stream()), "train_dense_fwd")
-        self._bn_finalize(ly, ly.rows, decay)
+                                           _p(ly.stats) if ly.bn and not self.frozen and not from_rows else None, _p(self.ws),
+                                           C.c_size_t(self.ws_bytes), _stream()), "train_dense_fwd")
+        if from_rows:
+            check(self.lib.psa_bn_finalize_rows(ly.rows, ly.N, _p(ly.y), _p(ly.gamma), _p(ly.beta), C.c_float(decay), _p(ly.mov_mean),
+                                                _p(ly.mov_var), _p(ly.scale), _p(ly.shift), _p(ly.mean_inv), _stream()), "bn_finalize_rows")
+        else:
+            self._bn_finalize(ly, ly.rows, decay)
 
     def _chain_fwd(self, layers, a: PsaActIn, decay: float):
         """a chain of dense layers on input `a`; the output is layers[-1].y"""

@@ -4,10 +4,11 @@ restatements evaluated on the GPU path's own neighbour graphs.  Bounds as in tes
 1e-5 of max(1, |largest|), gradients 1e-4 relative to the largest entry.
 
 A max (over k neighbours, or over the N points) whose runner-up lies within 1e-5 of it may be won by another element in fp32 than in
-float64, and then routes its gradient elsewhere; likewise a head activation whose pre-relu value lies within 1e-5 of zero may fall on
-the other side of the relu (under batch statistics that changes the gradient of its whole column).  These are properties of the max
-and the relu, not errors.  The model tests find such elements on the float64 side and zero the gradient arriving at them on both
-sides (a hook on the same tensor of each), as test_edgeconv2_train_gpu.py does for the op's output."""
+float64, and then routes its gradient elsewhere; likewise a head activation, or a maximum, whose pre-relu value lies within 1e-5 of
+zero on either side may fall on the other side of the relu (under batch statistics that changes the gradient of its whole column).
+These are properties of the max and the relu, not errors.  The model tests, frozen and training alike, find such elements on the
+float64 side and zero the gradient arriving at them on both sides (a hook on the same tensor of each), as test_edgeconv2_train_gpu.py
+does for the op's output."""
 import ctypes as C
 
 import numpy as np
@@ -69,6 +70,20 @@ def _near_zero(z):
         return z.abs() < 1e-5 * float(z.abs().max())
 
 
+def _near_zero_max(pre, dim, scale):
+    """True where the max over `dim` of the pre-relu values lies within 1e-5 of `scale` of the relu's zero, on either side: a maximum
+    slightly below zero in float64 may lie slightly above it in fp32, and then carries the whole gradient"""
+    with torch.no_grad():
+        return pre.amax(dim=dim).abs() < 1e-5 * scale
+
+
+def _inner_flip(pre, inner):
+    """True where the edge that wins the max over k (dim 2) of `pre` (b, n, k, c) has a unit of `inner` (b, n, k, c1), the pre-relu
+    values of the layer below, within 1e-5 (of the largest magnitude) of zero"""
+    with torch.no_grad():
+        return _near_zero(inner).any(dim=-1).gather(2, pre.argmax(dim=2))
+
+
 def _zero_at(t, mask):
     t.register_hook(lambda g: g.masked_fill(mask, 0.0))
 
@@ -80,9 +95,9 @@ def _p64(p):
     return {k: v.detach().double() for k, v in p.items()}
 
 
-def _layer(h, P, scope, frozen, bn=True, relu=True):
+def _layer(h, P, scope, frozen, bn=True, relu=True, stats=None):
     """conv2d / fully_connected (+ batch norm + relu): batch norm on the moving averages (frozen) or on the batch statistics over
-    every row (biased variance), eps 1e-3"""
+    every row (biased variance), eps 1e-3; the batch statistics are recorded in `stats[scope]` when a dict is given"""
     w = P[f"{scope}/weights"]
     y = h @ w.reshape(-1, w.shape[-1]) + P[f"{scope}/biases"]
     if not bn:
@@ -92,6 +107,8 @@ def _layer(h, P, scope, frozen, bn=True, relu=True):
     else:
         dims = tuple(range(y.dim() - 1))
         mean, var = y.mean(dims), y.var(dims, unbiased=False)
+        if stats is not None:
+            stats[scope] = (mean.detach(), var.detach())
     z = (y - mean) / torch.sqrt(var + 1e-3) * P[f"{scope}/bn/gamma"] + P[f"{scope}/bn/beta"]
     return torch.relu(z) if relu else z
 
@@ -111,21 +128,30 @@ class _Masks:
     def __init__(self):
         self.edge, self.pool, self.act = [], {}, {}
 
-    def edge_max(self, z):
+    def edge_max(self, z, pre=None, inner=None):
+        """max over k of the activated edge values z; given their pre-relu values `pre`, a maximum within 1e-5 of the relu's zero on
+        either side is ambiguous too, and given a fused first layer's pre-relu values `inner` (b, n, k, c1), so is a maximum whose
+        edge has a unit of that layer within 1e-5 of zero (the kernel's relu may fall the other way there)"""
         amb = _ambiguous(z, 2)
+        if pre is not None:
+            amb |= _near_zero_max(pre, 2, float(z.detach().abs().max()))
+        if inner is not None:
+            amb |= _inner_flip(pre, inner)
         out = z.amax(dim=2)
         _zero_at(out, amb)
         self.edge.append(amb)
         return out
 
-    def point_max(self, y, scope):
+    def point_max(self, y, scope, pre=None):
         amb = _ambiguous(y, 1)
+        if pre is not None:
+            amb |= _near_zero_max(pre, 1, float(y.detach().abs().max()))
         _zero_at(y, amb.unsqueeze(1))
         self.pool[scope] = amb
         return y.amax(dim=1)
 
-    def head_layer(self, h, P, scope, frozen):
-        z = _layer(h, P, scope, frozen, relu=False)
+    def head_layer(self, h, P, scope, frozen, stats=None):
+        z = _layer(h, P, scope, frozen, relu=False, stats=stats)
         near = _near_zero(z)
         out = torch.relu(z)
         _zero_at(out, near)
@@ -159,24 +185,30 @@ class _Masks:
         monkeypatch.setattr(training, "mlp_training", mlp_training)
 
 
-def _dgcnn64(x, P, graphs, frozen, masks: _Masks, detach_transform=False):
-    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55) in float64, dropout off, on the given neighbour graphs -> logits"""
+def _dgcnn64(x, P, graphs, frozen, masks: _Masks, detach_transform=False, stats=None):
+    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55) in float64, dropout off, on the given neighbour graphs -> logits;
+    stats (a dict): every layer's batch statistics, by scope"""
     b, n, _ = x.shape
-    L = lambda h, s, **kw: _layer(h, P, s, frozen, **kw)        # noqa: E731
+    L = lambda h, s, **kw: _layer(h, P, s, frozen, stats=stats, **kw)        # noqa: E731
     sc = "transform_net1"
-    h = masks.edge_max(L(L(_edges(x, graphs[0]), f"{sc}/tconv1"), f"{sc}/tconv2"))
-    h = masks.point_max(L(h, f"{sc}/tconv3"), f"{sc}/tconv3")
+    y1 = L(_edges(x, graphs[0]), f"{sc}/tconv1", relu=False)
+    y = L(torch.relu(y1), f"{sc}/tconv2", relu=False)
+    h = masks.edge_max(torch.relu(y), pre=y, inner=y1)
+    y = L(h, f"{sc}/tconv3", relu=False)
+    h = masks.point_max(torch.relu(y), f"{sc}/tconv3", pre=y)
     h = L(L(h, f"{sc}/tfc1"), f"{sc}/tfc2")
     t = (h @ P[f"{sc}/transform_XYZ/weights"] + P[f"{sc}/transform_XYZ/biases"] + torch.eye(3, dtype=x.dtype, device=x.device).flatten())
     t = t.reshape(b, 3, 3)
     h = torch.bmm(x, t.detach() if detach_transform else t)
     nets = []
     for i, s in enumerate(["dgcnn1", "dgcnn2", "dgcnn3", "dgcnn4"]):
-        h = masks.edge_max(L(_edges(h, graphs[i + 1]), s))
+        y = L(_edges(h, graphs[i + 1]), s, relu=False)
+        h = masks.edge_max(torch.relu(y), pre=y)
         nets.append(h)
-    g = masks.point_max(L(torch.cat(nets, dim=-1), "agg"), "agg")
+    y = L(torch.cat(nets, dim=-1), "agg", relu=False)
+    g = masks.point_max(torch.relu(y), "agg", pre=y)
     for s in ("fc1", "fc2"):
-        g = masks.head_layer(g, P, s, frozen)
+        g = masks.head_layer(g, P, s, frozen, stats)
     return L(g, "fc3", bn=False)
 
 
