@@ -524,6 +524,41 @@ PSA_API int psa_edgeconv2_frozen_bwd(int b, int n, int c, int k, int C1, int C2,
                                      const float* ywin, const float* dout, float* dx, void* workspace, size_t workspace_bytes,
                                      psa_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * SpiderCNN, inference mode (SpiderCNN/utils/tf_util.py:127-235 spiderConv, :363-377 topk_pool,
+ * :407-429 group_norm_for_conv)
+ * ------------------------------------------------------------------------------------------- */
+
+/* One spiderConv layer up to its group norm, without the (b,n,k,c*T) product tensor of the reference:
+ *   y[p][o] = bias[o] + sum_j sum_c sum_t  h[nn(p,j)][c] * g_t(delta[p][j]) * W[j][c*T + t][o]
+ *   h = relu(feat * feat_scale[b][c] + feat_shift[b][c])   (the previous layer's group norm + ReLU, per cloud b),
+ *       or feat itself when feat_scale == NULL (no ReLU: the first layer reads the coordinates);
+ *   g_t(d) = sum_m taylor[m][t] * mono_m(d) over the 20 monomials of degree <= 3, in the order of the reference's
+ *       variables: x, y, z, xyz, xy, yz, xz, 1 (`biases`), xx, yy, zz, xxy, xyy, xxz, xzz, yyz, yzz, xxx, yyy, zzz.
+ * delta (b,n,k,3) = group_point(xyz, nn_idx) - xyz; nn_idx (b,n,k) int32 in [0, n); feat (b,n,c); feat_scale,
+ * feat_shift (b,c) or NULL; taylor (20,T); W (k, c*T, c_out) = the [1,k] conv's kernel; bias (c_out) -> y (b,n,c_out),
+ * pre-group-norm.  The conv runs as one GEMM over the b*n points whose operand is gathered and scaled while it is
+ * staged (tensor cores for c % 32 == 0, k*c*T % 64 == 0, c_out % 64 == 0, the fp32-FMA kernel otherwise and in mode 1;
+ * the arithmetic modes of psa_set_mlp_mode apply).  1 <= k <= 32.  workspace: psa_spider_conv_workspace_bytes(),
+ * 256-byte aligned. */
+PSA_API size_t psa_spider_conv_workspace_bytes(int b, int n, int c, int k, int T, int c_out);
+PSA_API int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_out, const float* delta, const int* nn_idx,
+                                  const float* feat, const float* feat_scale, const float* feat_shift, const float* taylor,
+                                  const float* W, const float* bias, float* y, void* workspace, size_t workspace_bytes,
+                                  psa_stream_t stream);
+
+/* Group norm of y (b,n,c) as a per-cloud affine: `groups` contiguous channel groups (groups divides c); per (cloud, group)
+ * the mean and then the centred variance (biased) over the group's channels and the n points, both in fp64 ->
+ * scale[b][ch] = gamma[ch] / sqrt(var + eps), shift[b][ch] = beta[ch] - mean * scale.  out (b,n,c) or NULL:
+ * y * scale + shift, then a ReLU if relu != 0. */
+PSA_API int psa_group_norm_affine(int b, int n, int c, int groups, float eps, const float* y, const float* gamma,
+                                  const float* beta, float* scale, float* shift, float* out, int relu, psa_stream_t stream);
+
+/* tf.nn.top_k over the points of h = y * scale + shift (+ ReLU if relu != 0; scale == NULL: h = y), k == 2:
+ * y (b,n,c), scale, shift (b,c) -> out[b][offset + ch][r] of out (b, out_channels, 2), r = 0 the largest.  n >= 2. */
+PSA_API int psa_topk_pool(int b, int n, int c, int k, const float* y, const float* scale, const float* shift, int relu,
+                          float* out, int out_channels, int offset, psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

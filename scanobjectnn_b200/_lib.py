@@ -101,6 +101,10 @@ SIGNATURES = {
     "psa_edgeconv2_train_bwd": [_i, _i, _i, _i, _i, _i] + [_p] * 24 + [_sz, _p],
     "psa_edgeconv_frozen_bwd": [_i, _i, _i, _i, _i] + [_p] * 11 + [_sz, _p],
     "psa_edgeconv2_frozen_bwd": [_i, _i, _i, _i, _i, _i] + [_p] * 15 + [_sz, _p],
+    # SpiderCNN (inference)
+    "psa_spider_conv_infer": [_i, _i, _i, _i, _i, _i] + [_p] * 9 + [_p, _sz, _p],
+    "psa_group_norm_affine": [_i, _i, _i, _i, _f, _p, _p, _p, _p, _p, _p, _i, _p],
+    "psa_topk_pool": [_i, _i, _i, _i, _p, _p, _p, _i, _p, _i, _i, _p],
     "psa_softmax_xent": [_i, _i, _p, _p, _p, _p, _p],
     "psa_pool_rows": [_ll, _i, _i, _i, _p, _p, _p, _p],
     "psa_adam_step": [_ll, _p, _p, _p, _p, _f, _f, _f, _f, _i, _f, _p],
@@ -109,7 +113,7 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_sa_module_workspace_bytes", "psa_sa_conv1_prebn_workspace_bytes", "psa_sa_group_all_workspace_bytes", "psa_edgeconv_workspace_bytes",
                 "psa_train_dense_workspace_bytes", "psa_bn_bwd_workspace_bytes", "psa_sa_conv1_bwd_workspace_bytes", "psa_knn_graph_workspace_bytes",
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
-                "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes")
+                "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes", "psa_spider_conv_workspace_bytes")
 
 _lib = None
 
@@ -154,6 +158,8 @@ def load() -> C.CDLL:
     lib.psa_edgeconv_train_workspace_bytes.restype = C.c_size_t
     lib.psa_edgeconv2_train_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
     lib.psa_edgeconv2_train_workspace_bytes.restype = C.c_size_t
+    lib.psa_spider_conv_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
+    lib.psa_spider_conv_workspace_bytes.restype = C.c_size_t
     lib.psa_version.restype = C.c_int
     lib.psa_sm_arch.restype = C.c_int
     lib.psa_last_error.restype = C.c_char_p

@@ -41,6 +41,16 @@ int edge_layer_tail(int b, int n, int c, int k, int N, const float* x, const int
 // frozen batch norm's backward coefficients dy = scale * dz: coef (3, N) := (scale, 0, 0)
 int frozen_coef(int N, const float* scale, float* coef, cudaStream_t st);
 
+// tc_mlp.cu, shared with spider.cu: the arithmetic mode of psa_set_mlp_mode (0, 1, 2), the operand pieces of its tensor-core
+// launches (2 or 3), the tile width (| format flag) of a dense layer, and the weight images (layout in tc_mlp.cu).
+int mlp_mode();
+int tc_np();
+int tc_dense_nt(long long rows, int N);
+// image of W (K x N, rows K..Kp zero) in the format `Nt` carries (width | format flag); `run_if` non-null: built only if *run_if != 0
+int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* image, cudaStream_t st, const unsigned int* run_if = nullptr);
+const unsigned int* image_trailer(const uint8_t* image, int Kp, int N);   // fp16x2 image: the non-finite-weight word
+const float* image_colscale(const uint8_t* image, int Kp, int N);         // fp16x2 image: the column factors 2^-e_n
+
 }  // namespace psa
 
 // tc_mlp.cu: W (2c, N) of a single-layer EdgeConv -> Wc (c, 2N) = [W_a - W_b | W_b] (grid-stride over the c * 2N entries)

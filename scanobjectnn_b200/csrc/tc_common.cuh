@@ -178,6 +178,27 @@ __device__ __forceinline__ void split_pair(float h0, float h1, uint32_t (&p)[NP]
     }
 }
 
+// ---- weight images (built by tc_mlp.cu's build_image; layout described there) ----
+// np = pieces per weight: 3 (bf16x3, 6 bytes per weight) or 2 (fp16x2, 4 bytes); see Split<NP> above
+__host__ __device__ constexpr uint32_t tc_block_bytes(int Nt, int np) { return (uint32_t)Nt * 128u * (uint32_t)np; }
+__host__ __device__ inline size_t tc_image_bytes(int K, int N, int np) { return (size_t)K * N * 2u * (size_t)np; }     // independent of the tile width
+// an image allocation = the blocks, np = 2: the N column factors 2^-e_n (fp32), then a 256-byte trailer whose first word is set
+// when a weight is not finite (np = 2)
+__host__ __device__ inline size_t tc_image_colscale_off(int K, int N, int np) { return (tc_image_bytes(K, N, np) + 255) & ~(size_t)255; }
+__host__ __device__ inline size_t tc_image_trailer_off(int K, int N, int np) {
+    return tc_image_colscale_off(K, N, np) + (np == 2 ? ((size_t)N * 4u + 255) & ~(size_t)255 : 0);
+}
+__host__ __device__ inline size_t tc_image_alloc_bytes(int K, int N, int np) { return tc_image_trailer_off(K, N, np) + 256; }
+
+constexpr int kImageBf16x3 = 0x100;      // flags in psa_mlp.image_nt / psa_mlp_image_plan: image holds three bf16 pieces ..
+constexpr int kImageF16x2 = 0x200;       // .. or two fp16 pieces
+constexpr int kImageFlags = kImageBf16x3 | kImageF16x2;
+__host__ __device__ inline int image_flag(int np) { return np == 2 ? kImageF16x2 : kImageBf16x3; }
+
+// 1 / x, exactly, for a normal power of two x (the column factors): the exponent field mirrored about the bias, one integer
+// subtraction instead of a correctly rounded reciprocal's slow path
+__device__ __forceinline__ float pow2_rcp(float x) { return __int_as_float(0x7f000000 - __float_as_int(x)); }
+
 // byte offset of element (n, k) of a [N][K] K-major SWIZZLE_128B tile
 __device__ __forceinline__ uint32_t swz_off_f32(uint32_t n, uint32_t k, uint32_t N) {
     return (k >> 5) * (N * 128u) + (n >> 3) * 1024u + (n & 7u) * 128u + ((((k & 31u) >> 2) ^ (n & 7u)) << 4) + (k & 3u) * 4u;

@@ -54,16 +54,7 @@ constexpr int kMaxTcLayers = 2;
 //   to small weights multiplies by up to 31.6 gamma.  The image carries 2^-e_n per column; the kernels fold it into the scale
 //   of their epilogue, and bring what they add to the accumulators before it into the same units (exact: powers of two).
 // ------------------------------------------------------------------------------------------------------------------
-// np = pieces per weight: 3 (bf16x3, 6 bytes per weight) or 2 (fp16x2, 4 bytes); see Split<NP> in tc_common.cuh
-__host__ __device__ constexpr uint32_t tc_block_bytes(int Nt, int np) { return (uint32_t)Nt * 128u * (uint32_t)np; }
-__host__ __device__ inline size_t tc_image_bytes(int K, int N, int np) { return (size_t)K * N * 2u * (size_t)np; }     // independent of the tile width
-// an image allocation = the blocks, np = 2: the N column factors 2^-e_n (fp32), then a 256-byte trailer whose first word is set
-// when a weight is not finite (np = 2)
-__host__ __device__ inline size_t tc_image_colscale_off(int K, int N, int np) { return (tc_image_bytes(K, N, np) + 255) & ~(size_t)255; }
-__host__ __device__ inline size_t tc_image_trailer_off(int K, int N, int np) {
-    return tc_image_colscale_off(K, N, np) + (np == 2 ? ((size_t)N * 4u + 255) & ~(size_t)255 : 0);
-}
-__host__ __device__ inline size_t tc_image_alloc_bytes(int K, int N, int np) { return tc_image_trailer_off(K, N, np) + 256; }
+// (the byte layout helpers tc_block_bytes .. tc_image_alloc_bytes are in tc_common.cuh, shared with spider.cu)
 
 struct TcArgs {
     long long groups;      // neighbourhoods = b*m
@@ -140,11 +131,6 @@ __device__ __forceinline__ float warp_rowsum16(float v) {
     return v;
 }
 
-constexpr int kImageBf16x3 = 0x100;      // flags in psa_mlp.image_nt / psa_mlp_image_plan: image holds three bf16 pieces ..
-constexpr int kImageF16x2 = 0x200;       // .. or two fp16 pieces
-constexpr int kImageFlags = kImageBf16x3 | kImageF16x2;
-__host__ __device__ inline int image_flag(int np) { return np == 2 ? kImageF16x2 : kImageBf16x3; }
-
 // fp16x2 images: the column factor 2^-e_n of every column of W (K x N) into colscale.  Block (32, 8): 32 columns, the rows strided
 // over 8 threads.  A column holding a non-finite weight keeps e_n = 0 and sets the trailer word (the op is then rerun with bf16x3
 // operands, which give what fp32 gives); finite weights scaled this way cannot leave the fp16 range.  e_n <= 64 keeps 2^-e_n and
@@ -172,10 +158,6 @@ __global__ void __launch_bounds__(256) tc_col_scale_kernel(int K, int N, const f
     colscale[n] = __int_as_float((127 - e) << 23);
     if (bad) atomicOr(trailer, 1u);
 }
-
-// 1 / x, exactly, for a normal power of two x (the column factors): the exponent field mirrored about the bias, one integer
-// subtraction instead of a correctly rounded reciprocal's slow path
-__device__ __forceinline__ float pow2_rcp(float x) { return __int_as_float(0x7f000000 - __float_as_int(x)); }
 
 // colscale: fp16x2, the column factors of tc_col_scale_kernel (the weights are stored divided by them, exactly); bf16x3: null
 template <int NP>
@@ -1062,7 +1044,7 @@ int tc_dense_nt(long long rows, int N) {
 
 // builds the image of W (K x N, rows K..Kp zero) in the format `Nt` carries (width | format flag); fp16x2: zeroes the trailer and
 // computes the column factors first
-static int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* image, cudaStream_t st, const unsigned int* run_if = nullptr) {
+int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* image, cudaStream_t st, const unsigned int* run_if) {
     if (Nt & kImageF16x2) {
         unsigned int* trailer = reinterpret_cast<unsigned int*>(image + tc_image_trailer_off(Kp, N, 2));
         float* colscale = reinterpret_cast<float*>(image + tc_image_colscale_off(Kp, N, 2));
@@ -1076,10 +1058,10 @@ static int build_image(int K, int Kp, int N, int Nt, const float* W, uint8_t* im
     }
     return check_launch("tc_prep_weights_kernel");
 }
-static const unsigned int* image_trailer(const uint8_t* image, int Kp, int N) {
+const unsigned int* image_trailer(const uint8_t* image, int Kp, int N) {
     return reinterpret_cast<const unsigned int*>(image + tc_image_trailer_off(Kp, N, 2));
 }
-static const float* image_colscale(const uint8_t* image, int Kp, int N) {
+const float* image_colscale(const uint8_t* image, int Kp, int N) {
     return reinterpret_cast<const float*>(image + tc_image_colscale_off(Kp, N, 2));
 }
 
@@ -1347,6 +1329,7 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
 using namespace psa;
 
 static std::atomic<int> g_mlp_mode{0};
+int psa::mlp_mode() { return g_mlp_mode; }
 extern "C" PSA_API int psa_set_mlp_mode(int mode) {
     PSA_REQUIRE(mode == 0 || mode == 1 || mode == 2,
                 "set_mlp_mode: mode must be 0 (tensor cores, fp16x2 operands with the range guard), 1 (fp32 FMA kernels only) or 2 (tensor cores, bf16x3)");

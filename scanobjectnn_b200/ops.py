@@ -20,6 +20,7 @@ __all__ = [
     "three_nn", "three_interpolate", "three_nn_interpolate", "pairwise_distance", "knn", "knn_graph",
     "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "shared_mlp_grouped", "sa_module_infer",
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
+    "spider_conv", "group_norm_affine", "topk_pool",
 ]
 
 
@@ -619,6 +620,85 @@ def edgeconv_infer(x, nn_idx, mlp: MlpParams) -> torch.Tensor:
     ws = torch.empty((need + 3) // 4, dtype=torch.float32, device=x.device) if need else None
     check(lib.psa_edgeconv_infer(b, n, c, k, _ptr(x), _ptr(nn_idx), mlp.ref, _ptr(out), _ptr(ws), C.c_size_t(need), _stream()),
           "edgeconv_infer")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# SpiderCNN
+# ------------------------------------------------------------------------------------------------
+def spider_conv(delta, nn_idx, feat, taylor, weights, bias, feat_scale=None, feat_shift=None) -> torch.Tensor:
+    """One spiderConv layer up to its group norm, without the (B,N,k,C*T) product tensor (psa_spider_conv_infer):
+    delta (B,N,k,3), nn_idx (B,N,k) int32, feat (B,N,C), taylor (20,T) (monomial order of include/psa.h), weights
+    (1,k,C*T,C_out) or (k,C*T,C_out), bias (C_out) -> pre-group-norm y (B,N,C_out).  feat_scale / feat_shift (B,C): the
+    previous layer's group norm, applied with a ReLU as feat is read; None: feat is read as it is."""
+    delta = _dev(delta, torch.float32, "delta", 4)
+    nn_idx = _dev(nn_idx, torch.int32, "nn_idx", 3)
+    feat = _dev(feat, torch.float32, "feat", 3)
+    taylor = _dev(taylor, torch.float32, "taylor", 2)
+    weights = _dev(weights, torch.float32, "weights")
+    bias = _dev(bias, torch.float32, "bias", 1)
+    b, n, c = feat.shape
+    k = nn_idx.shape[2]
+    t = taylor.shape[1]
+    c_out = bias.shape[0]
+    if tuple(nn_idx.shape[:2]) != (b, n) or tuple(delta.shape) != (b, n, k, 3):
+        raise ValueError(f"spider_conv: nn_idx {tuple(nn_idx.shape)} / delta {tuple(delta.shape)} do not match feat {tuple(feat.shape)}")
+    if taylor.shape[0] != 20 or weights.numel() != k * c * t * c_out or weights.shape[-1] != c_out:
+        raise ValueError(f"spider_conv: taylor {tuple(taylor.shape)} / weights {tuple(weights.shape)} do not match k={k} C={c} C_out={c_out}")
+    if (feat_scale is None) != (feat_shift is None):
+        raise ValueError("spider_conv: feat_scale and feat_shift go together")
+    if feat_scale is not None:
+        feat_scale = _dev(feat_scale, torch.float32, "feat_scale", 2)
+        feat_shift = _dev(feat_shift, torch.float32, "feat_shift", 2)
+        if tuple(feat_scale.shape) != (b, c) or tuple(feat_shift.shape) != (b, c):
+            raise ValueError(f"spider_conv: feat_scale / feat_shift must be ({b}, {c})")
+    y = torch.empty((b, n, c_out), dtype=torch.float32, device=feat.device)
+    lib = _lib.load()
+    need = lib.psa_spider_conv_workspace_bytes(b, n, c, k, t, c_out)
+    ws = torch.empty((max(need, 4) + 3) // 4, dtype=torch.float32, device=feat.device)
+    check(lib.psa_spider_conv_infer(b, n, c, k, t, c_out, _ptr(delta), _ptr(nn_idx), _ptr(feat), _ptr(feat_scale), _ptr(feat_shift),
+                                    _ptr(taylor), _ptr(weights), _ptr(bias), _ptr(y), _ptr(ws), C.c_size_t(need), _stream()),
+          "spider_conv")
+    return y
+
+
+def group_norm_affine(y, gamma, beta, groups: int, eps: float = 1e-6, apply: bool = False, relu: bool = False):
+    """Group norm of y (B,N,C) over `groups` contiguous channel groups as a per-cloud affine (psa_group_norm_affine):
+    -> (scale, shift) (B,C), or with apply=True (y * scale + shift [then ReLU], scale, shift)."""
+    y = _dev(y, torch.float32, "y", 3)
+    gamma = _dev(gamma, torch.float32, "gamma", 1)
+    beta = _dev(beta, torch.float32, "beta", 1)
+    b, n, c = y.shape
+    if gamma.numel() != c or beta.numel() != c:
+        raise ValueError(f"group_norm_affine: gamma / beta must have {c} entries")
+    if groups < 1 or c % groups:
+        raise ValueError(f"group_norm_affine: {groups} groups do not divide {c} channels")
+    scale = torch.empty((b, c), dtype=torch.float32, device=y.device)
+    shift = torch.empty((b, c), dtype=torch.float32, device=y.device)
+    out = torch.empty_like(y) if apply else None
+    check(_lib.load().psa_group_norm_affine(b, n, c, groups, C.c_float(eps), _ptr(y), _ptr(gamma), _ptr(beta), _ptr(scale), _ptr(shift),
+                                            _ptr(out), 1 if relu else 0, _stream()), "group_norm_affine")
+    return (out, scale, shift) if apply else (scale, shift)
+
+
+def topk_pool(y, k: int = 2, scale=None, shift=None, relu: bool = False, out=None, offset: int = 0) -> torch.Tensor:
+    """tf.nn.top_k over the points (SpiderCNN's topk_pool) of h = y [* scale + shift] [then ReLU]: y (B,N,C) -> (B,C,k), largest
+    first.  out (B,C_total,k): written at channels [offset, offset + C) and returned."""
+    y = _dev(y, torch.float32, "y", 3)
+    b, n, c = y.shape
+    if (scale is None) != (shift is None):
+        raise ValueError("topk_pool: scale and shift go together")
+    if scale is not None:
+        scale = _dev(scale, torch.float32, "scale", 2)
+        shift = _dev(shift, torch.float32, "shift", 2)
+        if tuple(scale.shape) != (b, c) or tuple(shift.shape) != (b, c):
+            raise ValueError(f"topk_pool: scale / shift must be ({b}, {c})")
+    if out is None:
+        out = torch.empty((b, c, k), dtype=torch.float32, device=y.device)
+    elif not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 3 and out.shape[0] == b and out.shape[2] == k):
+        raise ValueError(f"topk_pool: out must be a contiguous float32 CUDA tensor ({b}, C_total, {k})")
+    check(_lib.load().psa_topk_pool(b, n, c, k, _ptr(y), _ptr(scale), _ptr(shift), 1 if relu else 0, _ptr(out), out.shape[1], offset,
+                                    _stream()), "topk_pool")
     return out
 
 

@@ -4,7 +4,9 @@
   TF checkpoint name map is the identity;
 * ``conv2d`` 1x1 / ``fully_connected`` (+bias +batch norm +ReLU) in inference mode, executed by the hand-written
   dense-layer kernel (pointnet2/utils/tf_util.py:120-185, 512-531; dgcnn/utils/tf_util.py:115-173, 462-499);
-* DGCNN's graph functions (dgcnn/utils/tf_util.py:638-706).
+* DGCNN's graph functions (dgcnn/utils/tf_util.py:638-706);
+* SpiderCNN's ``spiderConv``, ``group_norm_for_conv`` and ``topk_pool`` in inference mode (SpiderCNN/utils/tf_util.py:127-235,
+  363-377, 407-429).
 """
 from __future__ import annotations
 
@@ -16,6 +18,12 @@ from . import ops
 from .ops import get_edge_feature, knn, knn_graph, pairwise_distance  # noqa: F401
 
 BN_EPS = 1e-3   # tf.contrib.layers.batch_norm default (pointnet2 tf_util.py:526-531); explicit in dgcnn tf_util.py:498
+GN_EPS = 1e-6   # group_norm_for_conv's default (SpiderCNN/utils/tf_util.py:407)
+# spiderConv's Taylor variables in the order the reference creates them (tf_util.py:181-205); "biases" is the constant term.
+# This is also the row order of the (20, T) coefficient matrix of ops.spider_conv / psa_spider_conv_infer.
+TAYLOR_TERMS = ("weight_x", "weight_y", "weight_z", "weight_xyz", "weight_xy", "weight_yz", "weight_xz", "biases", "weight_xx",
+                "weight_yy", "weight_zz", "weight_xxy", "weight_xyy", "weight_xxz", "weight_xzz", "weight_yyz", "weight_yzz",
+                "weight_xxx", "weight_yyy", "weight_zzz")
 
 
 class VariableStore(dict):
@@ -65,6 +73,30 @@ class VariableStore(dict):
         self[f"{scope}/biases"] = torch.zeros(cout, device=self.device)
         if bn:
             self._bn(scope, cout, randomize_bn)
+
+    def add_spider_conv(self, scope, cin, cout, k=20, taylor_channel=5):
+        """spiderConv's variables under ``scope`` (e.g. ``fanConv1/taylor``) with gn=True, bn=False: the 20 Taylor vectors
+        (1,1,1,T) (Xavier with TF's 4-D fans 1 and T; ``biases`` zero), the [1,k] conv (1,k,cin*T,cout) (fans k*cin*T and
+        k*cout), its biases and the group norm's gamma / beta."""
+        t = taylor_channel
+        for name in TAYLOR_TERMS:
+            shape = (1, 1, 1, t)
+            self[f"{scope}/{name}"] = torch.zeros(shape, device=self.device) if name == "biases" else self._xavier(shape, 1, t)
+        self[f"{scope}/conv/weights"] = self._xavier((1, k, cin * t, cout), k * cin * t, k * cout)
+        self[f"{scope}/conv/biases"] = torch.zeros(cout, device=self.device)
+        self[f"{scope}/conv/gn/gamma"] = torch.ones(cout, device=self.device)
+        self[f"{scope}/conv/gn/beta"] = torch.zeros(cout, device=self.device)
+
+    def spider(self, scope):
+        """(taylor (20,T), conv weights (k, cin*T, cout), conv biases, gn gamma, gn beta) of a spiderConv ``scope``, as
+        ops.spider_conv / ops.group_norm_affine take them; cached like ``folded``."""
+        key = ("spider", scope)
+        if key not in self._cache:
+            taylor = torch.cat([self[f"{scope}/{name}"].reshape(1, -1).float() for name in TAYLOR_TERMS]).contiguous()
+            w = self[f"{scope}/conv/weights"].float()
+            self._cache[key] = (taylor, w.reshape(w.shape[-3:]).contiguous(), self[f"{scope}/conv/biases"].float().contiguous(),
+                                self[f"{scope}/conv/gn/gamma"].float().contiguous(), self[f"{scope}/conv/gn/beta"].float().contiguous())
+        return self._cache[key]
 
     # --- inference-mode folding: y = relu((x.W) * scale + shift) ---
     def folded(self, scope, relu=True):
@@ -180,6 +212,39 @@ def fully_connected(inputs, num_outputs, scope, activation_fn="relu", bn=False, 
     if mlp.channels[-1] != num_outputs:
         raise ValueError(f"{scope}: stored weights have {mlp.channels[-1]} outputs, asked for {num_outputs}")
     return ops.shared_mlp(inputs, mlp)
+
+
+def spiderConv(feat, idx, delta, num_conv, taylor_channel, bn=False, is_training=None, bn_decay=None, gn=False, G=32,
+               is_multi_GPU=False, activation_fn="relu", scope="taylor", *, params: VariableStore):
+    """tf_util.spiderConv (SpiderCNN/utils/tf_util.py:127-235) in inference mode, for the configuration SpiderCNN uses: gn=True,
+    bn=False, ReLU.  feat (B,N,C), idx (B,N,k) int32, delta (B,N,k,3) -> (B,N,num_conv).  ``scope`` is the full variable scope
+    (``fanConv1/taylor``).  The model itself chains ops.spider_conv on the pre-norm outputs and never builds this tensor."""
+    _require_inference(is_training)
+    if bn or not gn or activation_fn is None:
+        raise NotImplementedError("spiderConv: only gn=True, bn=False with a ReLU (SpiderCNN's configuration) is implemented")
+    taylor, w, bias, gamma, beta = params.spider(scope)
+    if taylor.shape[1] != taylor_channel or w.shape[-1] != num_conv:
+        raise ValueError(f"{scope}: stored variables have T={taylor.shape[1]}, {w.shape[-1]} outputs; asked for {taylor_channel}, {num_conv}")
+    y = ops.spider_conv(delta, idx, feat, taylor, w, bias)
+    out, _, _ = ops.group_norm_affine(y, gamma, beta, min(G, num_conv), GN_EPS, apply=True, relu=True)
+    return out
+
+
+def group_norm_for_conv(x, G=32, esp=GN_EPS, scope="gn", *, params: VariableStore):
+    """tf_util.group_norm_for_conv (SpiderCNN/utils/tf_util.py:407-429) on x (B,N,C) or (B,N,1,C): G = min(G, C) contiguous
+    channel groups, statistics per cloud, gamma / beta from ``scope/gamma``, ``scope/beta``."""
+    shape = x.shape
+    x3 = x.reshape(shape[0], -1, shape[-1])
+    c = shape[-1]
+    out, _, _ = ops.group_norm_affine(x3, params[f"{scope}/gamma"].float(), params[f"{scope}/beta"].float(), min(G, c), esp, apply=True)
+    return out.reshape(shape)
+
+
+def topk_pool(inputs, scope, k=2):
+    """tf_util.topk_pool (SpiderCNN/utils/tf_util.py:363-377): (B,N,C) -> (B,C,k), the k largest values over the points."""
+    if k != 2:
+        raise NotImplementedError("topk_pool: only k = 2 (what SpiderCNN uses) is implemented")
+    return ops.topk_pool(inputs, k)
 
 
 def dropout(inputs, is_training, scope, keep_prob=0.5, noise_shape=None):
