@@ -19,6 +19,8 @@
 //   tc_dense_kernel<NP,NC>    dense layer, persistent over 128-row x 64 NC-channel tiles, a producer warp feeding two consumer
 //                             warpgroups; also the training-mode forward (previous batch norm applied on load, column
 //                             statistics in the epilogue)
+//   tc_group_all_kernel<..>   a three-layer group-all level with 128 points per cloud, fp16x2: one four-CTA cluster per cloud,
+//                             the activations between the layers kept in the cluster's shared memory
 // fp32 parity: operands are quantised by this code, so the tensor core only ever sees exactly representable values; fp32
 // accumulation in the tensor core truncates, hence small terms first and K cut into <= 128-wide pieces (tests hold 1e-5 vs fp64).
 //   NP = 2 (inference default): two fp16 pieces, three MMAs per product, weights scaled per output column by a power of two (see
@@ -31,6 +33,7 @@
 #include <stdlib.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "common.cuh"
 #include "mlp_internal.cuh"
@@ -1094,6 +1097,22 @@ static int launch_tc_dense_np(TcDenseArgs& a, int Nt, cudaStream_t st) {
 // of layer l and of its rerun at [kTileCounterWords + 2 l, + 1]
 constexpr int kTileCounterWords = PSA_MAX_MLP_LAYERS;
 
+// the guarded bf16x3 rerun of a dense layer (`a`: the layer's arguments; its np = 2 fields are reset), a no-op unless *run_if != 0.
+// A prebuilt image carries its bf16x3 twin behind the fp16x2 blocks (psa_prepare_weight_image); otherwise the twin is built into
+// ws_img (tc_dense_image_bytes(K, N)), conditionally too.
+static int launch_tc_dense_rerun(TcDenseArgs a, int Nt, const float* W, const uint8_t* prebuilt, uint8_t* ws_img, const unsigned int* run_if,
+                                 unsigned int* counter, cudaStream_t st) {
+    uint8_t* img3 = ws_img + tc_dense_image_off3(a.K, a.N);
+    if (prebuilt != nullptr) {
+        img3 = const_cast<uint8_t*>(prebuilt) + tc_image_alloc_bytes(a.Kp, a.N, 2);
+    } else {
+        const int rc = build_image(a.K, a.Kp, a.N, Nt | kImageBf16x3, W, img3, st, run_if);
+        if (rc != PSA_OK) return rc;
+    }
+    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = run_if; a.tile_counter = counter;
+    return launch_tc_dense_np<3>(a, Nt, st);
+}
+
 // out = relu?((x . W [+ xyz3 . w3] [+ group_add[r / group_rows]]) * scale + shift) on the tensor cores, optional max over runs of
 // pool_k rows (not with group_add).
 //   prebuilt : image of W in the CURRENT split's format (psa_prepare_weight_image), or null
@@ -1123,16 +1142,7 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
     a.ovf = flag; a.wflag = image_trailer(a.image, Kp, N); a.colscale = image_colscale(a.image, Kp, N);
     rc = launch_tc_dense_np<2>(a, Nt, st);
     if (rc != PSA_OK) return rc;
-    // guarded rerun, a no-op unless the fp16x2 pass raised the flag.  A prebuilt image carries its bf16x3 twin behind the fp16x2
-    // blocks (psa_prepare_weight_image); otherwise the twin is built here, conditionally too.
-    if (prebuilt != nullptr) {
-        img3 = const_cast<uint8_t*>(prebuilt) + tc_image_alloc_bytes(Kp, N, 2);
-    } else {
-        rc = build_image(K, Kp, N, Nt | kImageBf16x3, W, img3, st, flag);
-        if (rc != PSA_OK) return rc;
-    }
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = flag; a.tile_counter = counters + 1;
-    return launch_tc_dense_np<3>(a, Nt, st);
+    return launch_tc_dense_rerun(a, Nt, W, prebuilt, ws_img, flag, counters + 1, st);   // a no-op unless the fp16x2 pass raised the flag
 }
 
 // Training-mode forward of one layer on tc_dense_kernel: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
@@ -1324,6 +1334,393 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     return launch_tc_sa_np<3>(a3, st);
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// tc_group_all_kernel -- a whole three-layer group-all level (pointnet_sa_module(group_all=True) with 128 points per cloud)
+// in one launch, fp16x2 operands.  A 128-row tile of tc_dense_kernel is exactly one cloud here, so a thread-block cluster of
+// four CTAs owns one cloud and the activations between the layers never leave it:
+//   * CTA rank r computes columns [r N_l / 4, (r + 1) N_l / 4) of each layer for all 128 rows: layer 0 (K = c, the xyz rows of
+//     W1 as the epilogue side input) and layer 1 in one 64- or 128-column pass each, the last layer in 128-column passes, each
+//     followed by the max over the 128 rows -- a plain store of out[cloud, col];
+//   * the slices of layers 0 and 1 stay in the CTA's own shared memory as fp32 after the affine and ReLU, in the padded rows of
+//     tc_dense_kernel's x stages (kDenseXRow), one 128 x 64 block per 64 columns.  K block kb of layer l + 1 lives in the CTA
+//     that owns those columns of layer l: the consumers read it with ld.shared::cluster and split it into A fragments while
+//     block kb - 1's wgmma group runs, as tc_dense_kernel does with its staged x.  Layer 0's input rows are read from global
+//     memory the same way (4 KB of 32-byte sectors per block and warp, from L2: the four CTAs of a cloud read the same rows);
+//   * one producer warp streams the weight blocks of all three layers through one ring of 32 KB stages (cp.async.bulk from
+//     the layers' fp16x2 images, whatever their tile width), so the next layer's first blocks land during this layer's epilogue.
+// Arithmetic is tc_dense_kernel's: per 64-wide K block a fresh wgmma sum over the Split<2> pieces in the same order, added into
+// fp32 accumulators in increasing kb, then the same epilogue -- every element is bitwise what the three-launch chain computes.
+// Like it, the kernel raises *ovf when a leading piece it stores leaves the fp16 range or a weight image is flagged; the
+// launcher queues the chain's bf16x3 reruns behind it, conditional on that word.
+// Synchronisation across the cluster (mbarriers only: the producer warps have returned by then and must not be waited for):
+//   1. every CTA's barriers are initialised before any peer arrives on them: one cluster barrier of all threads at the start,
+//      before any warp returns;
+//   2. a layer's slice is complete in every CTA before a peer reads it: the consumers finish their stores, meet on a named
+//      barrier, and four threads arrive (release, cluster scope) on s_ready[l] of each of the four CTAs; the consumers of every
+//      CTA wait on their own s_ready[l] (acquire, cluster scope) before the next layer's first read;
+//   3. no CTA exits while a peer may still read its slices: the same handshake on s_done after the last layer's last read.
+//      Slices are written once, so nothing is overwritten while a peer may read it.
+// ------------------------------------------------------------------------------------------------------------------
+struct TcGroupAllArgs {
+    int c;                             // input features (K of layer 0), a multiple of 64
+    int N[3];                          // layer widths
+    int Nt[3];                         // tile width of each layer's weight image (64 | 128)
+    const float* points;               // (b, 128, c), 16-byte aligned
+    const float* xyz;                  // (b, 128, 3)
+    const float* w3;                   // (3, N[0]): the xyz rows of layer 0's weights
+    const uint8_t* image[3];           // fp16x2 weight images (blocks, column factors, trailer)
+    const float* colscale[3];
+    const unsigned int* wflag[3];
+    const float* scale[3];             // or null
+    const float* shift[3];             // or null
+    int relu[3];
+    float* out;                        // (b, N[2])
+    unsigned int* ovf;                 // raised when the result is invalid (the bf16x3 reruns then replace it)
+};
+
+constexpr int kGaStages = 3;
+constexpr uint32_t kGaStageBytes = 32768u;      // one K block of 128 weight columns, two fp16 pieces
+constexpr uint32_t kGaSmemBudget = 222u * 1024u;
+// dynamic shared memory: 1 KB alignment, the ring, the slices of layers 0 and 1 (W0 + W1 columns), the affine of every layer
+__host__ __device__ inline uint32_t group_all_smem(int W0, int W1, int W2) {
+    return 1024u + kGaStages * kGaStageBytes + (uint32_t)(W0 + W1) / 64u * kDenseXBytes + 12u * (uint32_t)(W0 + W1 + W2);
+}
+
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+    return r;
+}
+// the shared::cluster address of the same variable in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+__device__ __forceinline__ float2 ld_cluster_f32x2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+// arrive on the mbarrier at shared::cluster address `addr` (any CTA of the cluster), releasing this thread's prior writes -- and
+// those ordered before them by a barrier -- at cluster scope
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t addr) {
+    asm volatile("fence.acq_rel.cluster;\n\tmbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n" ::"r"(addr) : "memory");
+}
+__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
+    uint32_t done;
+    const uint32_t addr = smem_u32(bar);
+    do {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}\n"
+            : "=r"(done)
+            : "r"(addr), "r"(parity)
+            : "memory");
+    } while (!done);
+}
+
+// NC0, NC1: 64-column chunks of the layer-0 and layer-1 slices (one pass each); the last layer runs in 128-column passes
+template <int NC0, int NC1>
+__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kDenseThreads, 1)
+tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
+    constexpr int NP = 2, S = kGaStages;
+    constexpr uint32_t piece = 8192u, chunk = 16384u;               // a 64-column chunk of a stage: its two pieces
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t s_full[S], s_empty[S], s_ready[2], s_done;
+    __shared__ float s_red[8][128];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t rank = cluster_ctarank();
+    const int cloud = blockIdx.x >> 2;
+    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    constexpr int W0 = 64 * NC0, W1 = 64 * NC1;                     // slice widths
+    const int W2 = a.N[2] / 4;
+    uint8_t* slice0 = base + S * kGaStageBytes;
+    uint8_t* slice1 = slice0 + NC0 * kDenseXBytes;
+    float* aff0 = reinterpret_cast<float*>(slice1 + NC1 * kDenseXBytes);   // per layer: scale x column factor, shift, 1 / column factor
+    float* aff1 = aff0 + 3 * W0;
+    float* aff2 = aff1 + 3 * W1;
+    {
+        float* aff[3] = {aff0, aff1, aff2};
+        const int W[3] = {W0, W1, W2};
+#pragma unroll
+        for (int l = 0; l < 3; ++l)
+            for (int i = tid; i < W[l]; i += kDenseThreads) {
+                const int col = (int)rank * W[l] + i;
+                const float cs = __ldg(a.colscale[l] + col);
+                aff[l][i] = (a.scale[l] ? __ldg(a.scale[l] + col) : 1.f) * cs;
+                aff[l][W[l] + i] = a.shift[l] ? __ldg(a.shift[l] + col) : 0.f;
+                aff[l][2 * W[l] + i] = pow2_rcp(cs);
+            }
+    }
+    if (tid == 0) {
+        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], kDenseConsumers / 32); }
+        mbar_init(&s_ready[0], 4); mbar_init(&s_ready[1], 4); mbar_init(&s_done, 4);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    cluster_sync_all();                                             // hazard 1: the peers' barriers are initialised
+    const int KC[3] = {a.c / 64, 4 * W0 / 64, 4 * W1 / 64};
+
+    if (warp >= kDenseConsumers / 32) {
+        // ---- producer: the weight blocks of every pass, in the consumers' order ----
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+        if (warp != kDenseConsumers / 32) return;
+        uint32_t u = 0;                                             // ring uses
+#pragma unroll
+        for (int l = 0; l < 3; ++l) {
+            const int pw = l == 0 ? W0 : l == 1 ? W1 : 128, passes = l == 2 ? W2 / 128 : 1, Nt = a.Nt[l];
+            for (int p = 0; p < passes; ++p) {
+                const int j0 = ((int)rank * (l == 0 ? W0 : l == 1 ? W1 : W2) + p * pw) / 64;   // first 64-column chunk of the pass
+                for (int kb = 0; kb < KC[l]; ++kb, ++u) {
+                    const int s = (int)(u % S);
+                    if (u >= (uint32_t)S) mbar_wait(&s_empty[s], ((u / S) - 1u) & 1u);
+                    if (lane == 0) {
+                        mbar_expect_tx(&s_full[s], (uint32_t)(pw / 64) * chunk);
+                        for (int c = 0; c < pw / 64; ++c) {
+                            uint8_t* dst = base + (uint32_t)s * kGaStageBytes + (uint32_t)c * chunk;
+                            const int j = j0 + c;
+                            if (Nt == 64) {                         // block (j, kb) is the chunk, both pieces
+                                bulk_g2s(dst, a.image[l] + ((size_t)j * KC[l] + kb) * chunk, chunk, &s_full[s]);
+                            } else {                                // half j & 1 of each piece of block (j / 2, kb)
+                                const uint8_t* src = a.image[l] + ((size_t)(j >> 1) * KC[l] + kb) * (2u * chunk) + (uint32_t)(j & 1) * piece;
+                                bulk_g2s(dst, src, piece, &s_full[s]);
+                                bulk_g2s(dst + piece, src + 2u * piece, piece, &s_full[s]);
+                            }
+                        }
+                    }
+                }
+            }
+        }
+        return;
+    }
+
+    // ---- consumers: warp w holds rows 16w + g and 16w + g + 8 of the cloud ----
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+    const int g = lane >> 2, t = lane & 3;
+    const int rl[2] = {warp * 16 + g, warp * 16 + g + 8};
+    uint32_t ovf = 0u;
+    uint32_t u = 0;                                                 // ring uses
+
+    // one pass of layer L: 64 NC columns starting at column `lc` of this CTA's slice
+    auto pass = [&](auto Ltag, auto NCtag, int lc) {
+        constexpr int L = decltype(Ltag)::value, NC = decltype(NCtag)::value;
+        const int nkb = KC[L];
+        // K block kb of the layer's input -> A fragments (16 float2 loads in flight per thread)
+        auto prep = [&](uint32_t (&A)[NP][4][4], int kb) {
+            if constexpr (L == 0) {
+                const float* xb = a.points + (size_t)cloud * 128 * a.c + kb * 64;
+#pragma unroll
+                for (int s = 0; s < 4; ++s)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const float2 x = __ldg(reinterpret_cast<const float2*>(xb + (size_t)rl[i] * a.c + 16 * s + 8 * h + 2 * t));
+                            put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
+                        }
+            } else {
+                constexpr int Wp = L == 1 ? W0 : W1;                // the input's slice width: block kb is in CTA kb * 64 / Wp
+                const uint32_t src = mapa_shared(smem_u32(L == 1 ? slice0 : slice1) + (uint32_t)((kb * 64) % Wp / 64) * kDenseXBytes,
+                                                 (uint32_t)(kb * 64 / Wp));
+#pragma unroll
+                for (int s = 0; s < 4; ++s)
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const float2 x = ld_cluster_f32x2(src + (uint32_t)rl[i] * kDenseXRow + (uint32_t)(16 * s + 8 * h + 2 * t) * 4u);
+                            put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
+                        }
+            }
+        };
+        float acc[NC][32];
+        // block kb (ring use u): issue its group on A, prepare block kb + 1 into An while it runs, wait, release the stage, add
+        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], int kb) {
+            const int s = (int)(u % S);
+            mbar_wait(&s_full[s], (u / S) & 1u);
+            const uint32_t wb = smem_u32(base) + (uint32_t)s * kGaStageBytes;
+            float d[NC][32];
+            wg_fence();
+#pragma unroll
+            for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+                    for (int c = 0; c < NC; ++c)
+                        wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][ks][0], A[Split<NP>::a(tt)][ks][1], A[Split<NP>::a(tt)][ks][2], A[Split<NP>::a(tt)][ks][3],
+                                      wg_desc(wb + (uint32_t)c * chunk + Split<NP>::w(tt) * piece + (uint32_t)ks * 32u), (tt | ks) ? 1u : 0u);
+            wg_commit();
+            if (kb + 1 < nkb) prep(An, kb + 1);
+            wg_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive1(&s_empty[s]);               // weights consumed: the stage may be refilled
+            ++u;
+#pragma unroll
+            for (int c = 0; c < NC; ++c) {
+                wg_fence_acc(d[c]);
+#pragma unroll
+                for (int e = 0; e < 32; ++e) acc[c][e] = kb ? acc[c][e] + d[c][e] : d[c][e];
+            }
+        };
+        {
+            uint32_t A0[NP][4][4], A1[NP][4][4];
+            prep(A0, 0);
+            for (int kb = 0;; kb += 2) {
+                step(A0, A1, kb);
+                if (kb + 1 == nkb) break;
+                step(A1, A0, kb + 1);
+                if (kb + 2 == nkb) break;
+            }
+        }
+
+        // ---- epilogue: tc_dense_kernel's, in the fragment layout ----
+        constexpr int W = L == 0 ? W0 : L == 1 ? W1 : 0;
+        const int Wl = L == 2 ? W2 : W;
+        const float* aff = L == 0 ? aff0 : L == 1 ? aff1 : aff2;
+        float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+        if constexpr (L == 0)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz + ((size_t)cloud * 128 + rl[i]) * 3 + k);
+#pragma unroll
+        for (int c = 0; c < NC; ++c)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int cl = c * 64 + 8 * j + 2 * t, ls = lc + cl;   // column in the pass, in the slice
+                float y[2][2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float sc = aff[ls + e], sh = aff[Wl + ls + e];
+                    float w0 = 0.f, w1 = 0.f, w2 = 0.f;
+                    if constexpr (L == 0) {
+                        const int col = (int)rank * W0 + ls + e;
+                        const float f = aff[2 * Wl + ls + e];
+                        w0 = __ldg(a.w3 + col) * f; w1 = __ldg(a.w3 + a.N[0] + col) * f; w2 = __ldg(a.w3 + 2 * a.N[0] + col) * f;
+                    }
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        float x = acc[c][4 * j + 2 * i + e];
+                        if constexpr (L == 0) x = fmaf(xs[i][2], w2, fmaf(xs[i][1], w1, fmaf(xs[i][0], w0, x)));
+                        x = fmaf(x, sc, sh);
+                        if (a.relu[L]) x = fmaxf(x, 0.f);
+                        y[i][e] = x;
+                    }
+                }
+                if constexpr (L < 2) {
+                    uint8_t* sl = (L == 0 ? slice0 : slice1) + (ls >> 6) * kDenseXBytes + (ls & 63) * 4;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) *reinterpret_cast<float2*>(sl + rl[i] * kDenseXRow) = make_float2(y[i][0], y[i][1]);
+                } else {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const float m = warp_rowmax16(y[0][e], y[1][e]);
+                        if (g == 0) s_red[warp][cl + e] = m;
+                    }
+                }
+            }
+        unit_bar_sync(1, kDenseConsumers);
+        if constexpr (L < 2) {
+            // hazard 2: the slice is complete in this CTA -> tell every CTA of the cluster, then wait until all four are
+            if (tid < 4) mbar_arrive_cluster(mapa_shared(smem_u32(&s_ready[L]), (uint32_t)tid));
+            mbar_wait_cluster(&s_ready[L], 0);
+        } else {
+            for (int cl = tid; cl < 64 * NC; cl += kDenseConsumers) {
+                float mx = s_red[0][cl];
+                for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_red[w][cl]);
+                a.out[(size_t)cloud * a.N[2] + (size_t)rank * W2 + lc + cl] = mx;
+            }
+            unit_bar_sync(1, kDenseConsumers);                      // s_red is rewritten by the next pass
+        }
+    };
+    pass(std::integral_constant<int, 0>{}, std::integral_constant<int, NC0>{}, 0);
+    pass(std::integral_constant<int, 1>{}, std::integral_constant<int, NC1>{}, 0);
+    for (int lc = 0; lc < W2; lc += 128) pass(std::integral_constant<int, 2>{}, std::integral_constant<int, 2>{}, lc);
+
+    // hazard 3: the last reads of the peers' slices are done (their values are in the wgmma groups retired above)
+    if (tid < 4) mbar_arrive_cluster(mapa_shared(smem_u32(&s_done), (uint32_t)tid));
+    if (f16x2_overflowed(ovf) || (tid == 0 && (*a.wflag[0] | *a.wflag[1] | *a.wflag[2]) != 0u)) atomicOr(a.ovf, 1u);
+    mbar_wait_cluster(&s_done, 0);
+}
+
+// Can this group-all level run as one tc_group_all_kernel launch?  fp16x2 mode, three layers, 128 points per cloud, c a multiple
+// of 64 with 16-byte-aligned rows, layer widths N0, N1 in {256, 512} (not both 512: the two slices and the ring must fit in
+// shared memory) and N2 a multiple of 512, and a cluster of four such CTAs must fit on the device.  Returns the kernel's
+// shared memory, 0 when not eligible.
+template <int NC0, int NC1>
+static size_t group_all_fits(const psa_mlp* mlp) {
+    const size_t smem = group_all_smem(64 * NC0, 64 * NC1, mlp->channels[3] / 4);
+    if (smem > kGaSmemBudget) return 0;
+    if (cudaFuncSetAttribute(tc_group_all_kernel<NC0, NC1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 0;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(4, 1, 1);
+    cfg.blockDim = dim3(kDenseThreads, 1, 1);
+    cfg.dynamicSmemBytes = smem;
+    int clusters = 0;
+    if (cudaOccupancyMaxActiveClusters(&clusters, tc_group_all_kernel<NC0, NC1>, &cfg) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
+    return clusters > 0 ? smem : 0;
+}
+static size_t group_all_eligible(int n, int c, const float* points, const psa_mlp* mlp) {
+    if (g_tc_np != 2 || mlp->n_layers != 3 || n != 128 || c < 64 || c % 64 != 0 || (reinterpret_cast<uintptr_t>(points) & 15) != 0) return 0;
+    const int N0 = mlp->channels[1], N1 = mlp->channels[2], N2 = mlp->channels[3];
+    if (N2 % 512 != 0) return 0;
+    if (N0 == 256 && N1 == 256) return group_all_fits<1, 1>(mlp);
+    if (N0 == 256 && N1 == 512) return group_all_fits<1, 2>(mlp);
+    if (N0 == 512 && N1 == 256) return group_all_fits<2, 1>(mlp);
+    return 0;
+}
+
+// The group-all level of psa_sa_group_all_infer on tc_group_all_kernel (group_all_eligible said yes, `smem`), then the chain's
+// three bf16x3 layer launches, conditional on the kernel's range flag: the output is then what psa_set_mlp_mode(2) gives.
+// Workspace as the chain's: intermediate rows ws0 / ws1 (used by the reruns only), per-layer images from `img`, the zeroed word
+// region `words` (the flag is its free word [kTileCounterWords - 1], the reruns' tile counters those of the chain).
+static int sa_group_all_cluster(int b, int c, const float* xyz, const float* points, const psa_mlp* mlp, float* out, float* ws0, float* ws1,
+                                uint8_t* img, unsigned int* words, size_t smem, cudaStream_t st) {
+    const long long rows = (long long)b * 128;
+    unsigned int* flag = words + kTileCounterWords - 1;
+    TcGroupAllArgs g{};
+    g.c = c; g.points = points; g.xyz = xyz; g.w3 = mlp->weight[0]; g.out = out; g.ovf = flag;
+    const uint8_t* pre[3];
+    uint8_t* ws_img[3];
+    int rc;
+    for (int l = 0; l < 3; ++l) {
+        const int K = l == 0 ? c : mlp->channels[l], N = mlp->channels[l + 1], Nt = tc_dense_nt(rows, N);
+        const float* W = l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l];
+        pre[l] = prebuilt_image(mlp, l, l == 0 ? 3 : 0, Nt);
+        ws_img[l] = img;
+        img += tc_dense_image_bytes(K, N);
+        if (pre[l] == nullptr) { rc = build_image(K, K, N, Nt, W, ws_img[l], st); if (rc != PSA_OK) return rc; }
+        const uint8_t* image = pre[l] ? pre[l] : ws_img[l];
+        g.N[l] = N; g.Nt[l] = Nt & ~kImageFlags; g.image[l] = image;
+        g.colscale[l] = image_colscale(image, K, N); g.wflag[l] = image_trailer(image, K, N);
+        g.scale[l] = mlp->scale[l]; g.shift[l] = mlp->shift[l]; g.relu[l] = mlp->relu[l];
+    }
+    const int N0 = mlp->channels[1], N1 = mlp->channels[2];
+    if (N0 == 256 && N1 == 256) tc_group_all_kernel<1, 1><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
+    else if (N0 == 256) tc_group_all_kernel<1, 2><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
+    else tc_group_all_kernel<2, 1><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
+    rc = check_launch("tc_group_all_kernel");
+    if (rc != PSA_OK) return rc;
+    const float* cur = points;
+    for (int l = 0; l < 3; ++l) {
+        const int K = l == 0 ? c : mlp->channels[l], N = mlp->channels[l + 1];
+        TcDenseArgs a;
+        a.rows = rows; a.K = K; a.Kp = K; a.N = N; a.pool_k = l == 2 ? 128 : 1; a.relu = mlp->relu[l];
+        a.x = cur; a.scale = mlp->scale[l]; a.shift = mlp->shift[l]; a.out = l == 2 ? out : (l & 1) ? ws1 : ws0;
+        a.xyz3 = l == 0 ? xyz : nullptr; a.w3 = l == 0 ? mlp->weight[0] : nullptr;
+        rc = launch_tc_dense_rerun(a, g.Nt[l], l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l], pre[l], ws_img[l], flag,
+                                   words + kTileCounterWords + 2 * l + 1, st);
+        if (rc != PSA_OK) return rc;
+        cur = a.out;
+    }
+    return PSA_OK;
+}
+
 }  // namespace psa
 
 using namespace psa;
@@ -1497,6 +1894,11 @@ extern "C" int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, con
     cudaStream_t st = as_stream(stream);
     unsigned int* flags = reinterpret_cast<unsigned int*>(wsb + need - 256);
     PSA_CUDA(cudaMemsetAsync(flags, 0, 256, st));
+    // one cluster of four CTAs per cloud when the level allows it; otherwise one launch per layer
+    if (g_mlp_mode == 0) {
+        const size_t smem = group_all_eligible(n, c, points, mlp);
+        if (smem != 0) return sa_group_all_cluster(b, c, xyz, points, mlp, out, ws0, ws1, img, flags, smem, st);
+    }
     const float* cur = points;
     for (int l = 0; l < L; ++l) {
         const int K = (l == 0) ? c : mlp->channels[l], N = mlp->channels[l + 1];
