@@ -481,7 +481,9 @@ __global__ void softmax_xent_kernel(int b, int c, const float* __restrict__ logi
         float se = 0.f;
         for (int i = 0; i < c; ++i) se += expf(l[i] - mx);
         const int lab = labels[r];
-        rowloss[r] = (logf(se) + mx) - l[lab];
+        // log(se) - (l[lab] - mx): both terms are of the loss's size.  (log(se) + mx) - l[lab] would round at the scale of the
+        // logits, an error that grows with a common offset of the row that leaves the loss itself unchanged.
+        rowloss[r] = logf(se) - (l[lab] - mx);
         const float invb = 1.f / (float)b;
         for (int i = 0; i < c; ++i) dlogits[(size_t)r * c + i] = (expf(l[i] - mx) / se - (i == lab ? 1.f : 0.f)) * invb;
     }

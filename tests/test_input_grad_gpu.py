@@ -164,27 +164,55 @@ SMALL_LEVELS = [LevelSpec("layer1", 64, 0.3, 16, [64, 64, 128]), LevelSpec("laye
 HEAD = [("fc1", True), ("fc2", True), ("fc3", False)]
 
 
-def _bn64(y, p, scope, frozen):
-    g, be = p[f"{scope}/bn/gamma"].double(), p[f"{scope}/bn/beta"].double()
+def _bn64(y, p, scope, frozen, stats=None):
+    """batch norm in y's dtype; in training mode the batch statistics (mean, biased variance) are also left in `stats[scope]`"""
+    g, be = p[f"{scope}/bn/gamma"].to(y.dtype), p[f"{scope}/bn/beta"].to(y.dtype)
     if frozen:
-        mean, var = p[f"{scope}/bn/moving_mean"].double(), p[f"{scope}/bn/moving_variance"].double()
+        mean, var = p[f"{scope}/bn/moving_mean"].to(y.dtype), p[f"{scope}/bn/moving_variance"].to(y.dtype)
     else:
         red = tuple(range(y.dim() - 1))
         mean = y.mean(dim=red)
         var = ((y - mean) ** 2).mean(dim=red)
+        if stats is not None:
+            stats[scope] = (mean.detach(), var.detach())
     return (y - mean) / torch.sqrt(var + 1e-3) * g + be
 
 
-def _ssg64(xyz, p, levels, frozen, masks):
-    """pointnet2_cls_ssg (or bga's classification branch) restated in float64 torch ops on the trainers' FPS / ball-query indices"""
-    B = xyz.shape[0]
+def _gated_relu(z, ly, info):
+    """relu(z) with the run's decision: the gate of trainer layer `ly`, fmaf(y, scale, shift) > 0 (its sign is exact in float64);
+    the elements where z's own sign decides otherwise are counted as flips"""
+    with torch.no_grad():
+        gate = ((ly.y.double() * ly.scale.double() + ly.shift.double()) > 0).view(z.shape)
+        info["flips"] += int(((z > 0) != gate).sum())
+        info["units"] += gate.numel()
+    return z * gate
+
+
+def _argk_pool(h, lv, info):
+    """the max over dim 2 taken at the run's winner lv.argk (its first winning row), so the gradient goes where the kernel sends it;
+    info["pool_gap"]: how far below h's own maximum that row lies, relative to h's largest entry"""
+    B, m, _, c = h.shape
+    out = h.gather(2, lv.argk.long().view(B, m, 1, c)).squeeze(2)
+    with torch.no_grad():
+        gap = float((h.amax(dim=2) - out).max()) / max(float(h.abs().max()), 1e-30)
+        info["pool_gap"] = max(info["pool_gap"], gap)
+    return out
+
+
+def _ssg64(xyz, p, levels, frozen, masks, run=None, info=None):
+    """pointnet2_cls_ssg (or bga's classification branch) restated in torch ops of xyz's dtype on the trainers' FPS / ball-query
+    indices.  run: the PointNet2ClsTrainer whose discrete decisions are taken instead of the restatement's own -- every batch-normed
+    layer's relu gate (_gated_relu) and every level's max-pool winner (_argk_pool); `info` then collects the batch statistics
+    ("stats"), the flipped gates ("flips" of "units") and the largest pool gap ("pool_gap")."""
+    B, dt = xyz.shape[0], xyz.dtype
     ar = torch.arange(B, device=xyz.device)
+    stats = None if info is None else info.setdefault("stats", {})
     cur_xyz, cur_pts = xyz, None
     for lv in levels:
         sp = lv.spec
         if sp.group_all:
             h = (cur_xyz if cur_pts is None else torch.cat([cur_xyz, cur_pts], -1))[:, None]
-            new_xyz = torch.zeros((B, 1, 3), dtype=torch.float64, device=xyz.device)
+            new_xyz = torch.zeros((B, 1, 3), dtype=dt, device=xyz.device)
         else:
             new_xyz = cur_xyz[ar[:, None], lv.fps_idx.long()]
             idx = lv.idx.long()
@@ -193,16 +221,18 @@ def _ssg64(xyz, p, levels, frozen, masks):
                 h = torch.cat([h, cur_pts[ar[:, None, None], idx]], -1)
         for i in range(len(sp.mlp)):
             s = f"{sp.scope}/conv{i}"
-            w = p[f"{s}/weights"].double()
-            h = torch.relu(_bn64(h @ w.reshape(-1, w.shape[-1]) + p[f"{s}/biases"].double(), p, s, frozen))
-        cur_xyz, cur_pts = new_xyz, h.amax(dim=2)
+            w = p[f"{s}/weights"].to(dt)
+            z = _bn64(h @ w.reshape(-1, w.shape[-1]) + p[f"{s}/biases"].to(dt), p, s, frozen, stats)
+            h = torch.relu(z) if run is None else _gated_relu(z, lv.layers[i], info)
+        cur_xyz, cur_pts = new_xyz, h.amax(dim=2) if run is None else _argk_pool(h, lv, info)
     h = cur_pts.reshape(B, -1)
-    for scope, bn in HEAD:
-        h = h @ p[f"{scope}/weights"].double() + p[f"{scope}/biases"].double()
+    for j, (scope, bn) in enumerate(HEAD):
+        h = h @ p[f"{scope}/weights"].to(dt) + p[f"{scope}/biases"].to(dt)
         if bn:
-            h = torch.relu(_bn64(h, p, scope, frozen))
+            z = _bn64(h, p, scope, frozen, stats)
+            h = torch.relu(z) if run is None else _gated_relu(z, run.head[j], info)
         if scope in masks:
-            h = h * masks[scope].double()
+            h = h * masks[scope].to(dt)
     return h
 
 
