@@ -559,6 +559,38 @@ PSA_API int psa_group_norm_affine(int b, int n, int c, int groups, float eps, co
 PSA_API int psa_topk_pool(int b, int n, int c, int k, const float* y, const float* scale, const float* shift, int relu,
                           float* out, int out_channels, int offset, psa_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * 3DmFV-Net, inference mode (3DmFV-Net/utils/tf_util.py:578-652 get_3dmfv, :254-311 conv3d, :406-429 pools)
+ * Grid activations are (b * r^3, c) in voxel-major row order: row = voxel * b + cloud, voxel = (d * r + h) * r + w.
+ * ------------------------------------------------------------------------------------------- */
+
+/* The modified Fisher vector of get_3dmfv(flatten=False) before its final transpose: points (b,n,3), w (G), mu (G,3), sigma
+ * (G,3) (standard deviations) -> out (b,G,20), columns [d_pi max, sum | d_mu max xyz, min xyz, sum xyz | d_sigma max xyz, min
+ * xyz, sum xyz], power- (sign(v) |v|^0.5) and L2-normalised over the G Gaussians per (cloud, column).  The soft assignment is
+ * evaluated in the log domain, log w - sum_d log sigma - |z|^2 / 2 shifted by its maximum over the Gaussians: where the
+ * reference's fp32 densities all underflow it returns NaN, this op the finite limit.  Terms and sums in fp64, every reduction
+ * in a fixed order (bit-identical reruns), no (b,n,G) buffer.  One block per cloud; PSA_ERR_UNSUPPORTED when n and G do not fit
+ * its shared memory (about 8 * (2n + 27G) + 12n bytes <= 220 KB). */
+PSA_API int psa_fisher_vector(int b, int n, int G, const float* points, const float* w, const float* mu, const float* sigma,
+                              float* out, psa_stream_t stream);
+
+/* One tf_util.conv3d layer on an r^3 grid, SAME padding, stride 1, k in {1, 3, 5}: x rows (b*r^3) of stride ldx, c channels;
+ * W = the TF kernel (k,k,k,c,c_out), read as a (k^3 c, c_out) matrix; out[row * ldo + o] = relu?((x * W)[row][o] * scale[o] +
+ * shift[o]) (scale NULL: + shift only), the folded bias and batch norm.  The row strides let each inception branch read and
+ * write its slice of the concatenated output in place.  Tensor cores for c % 64 == 0, c_out % 32 == 0, x 16-byte aligned with
+ * ldx % 4 == 0, out 8-byte aligned with ldo even and scale / shift 8-byte aligned (a tile issues no MMA for a tap outside the
+ * grid for all its rows; the tap loop is split across CTAs and the partials added in a fixed order), the fp32-FMA kernel
+ * otherwise and in mode 1; the arithmetic modes of psa_set_mlp_mode apply.  workspace: psa_conv3d_workspace_bytes() queried
+ * in the mode of the call (0 when the shape or the mode takes the FMA kernel), 256-byte aligned. */
+PSA_API size_t psa_conv3d_workspace_bytes(int b, int r, int k, int c, int c_out);
+PSA_API int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const float* x, long long ldx, const float* W,
+                             const float* scale, const float* shift, int relu, float* out, long long ldo, void* workspace,
+                             size_t workspace_bytes, psa_stream_t stream);
+
+/* The inception module's pools on voxel-major rows x (b*r^3, c): kind 0 = SAME 3^3 average, stride 1, divided by the number
+ * of in-grid cells -> (b*r^3, c); kind 1 = SAME 2^3 max, stride 2, padded at the far end -> (b*ceil(r/2)^3, c). */
+PSA_API int psa_pool3d(int b, int r, int c, int kind, const float* x, float* out, psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

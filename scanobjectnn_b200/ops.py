@@ -20,7 +20,7 @@ __all__ = [
     "three_nn", "three_interpolate", "three_nn_interpolate", "pairwise_distance", "knn", "knn_graph",
     "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "shared_mlp_grouped", "sa_module_infer",
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
-    "spider_conv", "group_norm_affine", "topk_pool",
+    "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d",
 ]
 
 
@@ -699,6 +699,93 @@ def topk_pool(y, k: int = 2, scale=None, shift=None, relu: bool = False, out=Non
         raise ValueError(f"topk_pool: out must be a contiguous float32 CUDA tensor ({b}, C_total, {k})")
     check(_lib.load().psa_topk_pool(b, n, c, k, _ptr(y), _ptr(scale), _ptr(shift), 1 if relu else 0, _ptr(out), out.shape[1], offset,
                                     _stream()), "topk_pool")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# 3DmFV-Net
+# ------------------------------------------------------------------------------------------------
+def fisher_vector(points, w, mu, sigma) -> torch.Tensor:
+    """get_3dmfv(flatten=False) before its final transpose (psa_fisher_vector): points (B,N,3), w (G), mu (G,3), sigma (G,3)
+    standard deviations -> (B,G,20), power- and L2-normalised.  Computed in fp64 without any (B,N,G) tensor."""
+    points = _dev(points, torch.float32, "points", 3)
+    w = _dev(w, torch.float32, "w", 1)
+    mu = _dev(mu, torch.float32, "mu", 2)
+    sigma = _dev(sigma, torch.float32, "sigma", 2)
+    b, n, d = points.shape
+    g = w.shape[0]
+    if d != 3 or tuple(mu.shape) != (g, 3) or tuple(sigma.shape) != (g, 3):
+        raise ValueError(f"fisher_vector: points {tuple(points.shape)}, w {tuple(w.shape)}, mu {tuple(mu.shape)}, sigma "
+                         f"{tuple(sigma.shape)}: expected (B,N,3), (G), (G,3), (G,3)")
+    out = torch.empty((b, g, 20), dtype=torch.float32, device=points.device)
+    check(_lib.load().psa_fisher_vector(b, n, g, _ptr(points), _ptr(w), _ptr(mu), _ptr(sigma), _ptr(out), _stream()), "fisher_vector")
+    return out
+
+
+def _rows_view(t: torch.Tensor, name: str) -> torch.Tensor:
+    """a 2-D float32 CUDA tensor whose rows may be strided (a column slice of a wider buffer), or a contiguous copy"""
+    if not isinstance(t, torch.Tensor) or t.dim() != 2:
+        raise ValueError(f"{name}: expected a 2-D tensor (voxel rows, channels)")
+    if t.stride(1) == 1 and t.stride(0) >= t.shape[1]:
+        _dev(t[:0], torch.float32, name)          # device / dtype checks without a copy
+        return t
+    return _dev(t, torch.float32, name)
+
+
+def conv3d(x, r: int, weights, scale, shift, relu: bool = True, out=None, offset: int = 0) -> torch.Tensor:
+    """One tf_util.conv3d layer (SAME, stride 1) with folded batch norm on voxel-major rows (psa_conv3d_infer): x (B*r^3, C), row =
+    voxel * B + cloud (a column slice of a wider buffer is read in place); weights (k,k,k,C,C_out) or (k^3*C, C_out) with k in
+    {1, 3, 5}; scale (C_out) or None, shift (C_out) -> relu?((x * W) * scale + shift) (B*r^3, C_out).  out (B*r^3, C_total):
+    written at channels [offset, offset + C_out) and returned."""
+    x = _rows_view(x, "x")
+    weights = _dev(weights, torch.float32, "weights")
+    shift = _dev(shift, torch.float32, "shift", 1)
+    rows, c = x.shape
+    c_out = shift.shape[0]
+    vox = r ** 3
+    if r < 1 or rows % vox:
+        raise ValueError(f"conv3d: {rows} rows are not a multiple of r^3 = {vox}")
+    kk = weights.numel() // (c * c_out) if c * c_out else 0
+    k = {1: 1, 27: 3, 125: 5}.get(kk)
+    if k is None or weights.numel() != kk * c * c_out or weights.shape[-1] != c_out:
+        raise ValueError(f"conv3d: weights {tuple(weights.shape)} are not (k,k,k,{c},{c_out}) with k in (1, 3, 5)")
+    if weights.dim() == 5 and tuple(weights.shape) != (k, k, k, c, c_out):
+        raise ValueError(f"conv3d: weights {tuple(weights.shape)} are not ({k},{k},{k},{c},{c_out})")
+    if scale is not None:
+        scale = _dev(scale, torch.float32, "scale", 1)
+        if scale.shape[0] != c_out:
+            raise ValueError(f"conv3d: scale must have {c_out} entries")
+    if out is None:
+        out = torch.empty((rows, c_out), dtype=torch.float32, device=x.device)
+        view = out
+    else:
+        if not (out.is_cuda and out.dtype == torch.float32 and out.is_contiguous() and out.dim() == 2 and out.shape[0] == rows):
+            raise ValueError(f"conv3d: out must be a contiguous float32 CUDA tensor ({rows}, C_total)")
+        if offset < 0 or offset + c_out > out.shape[1]:
+            raise ValueError(f"conv3d: channels [{offset}, {offset + c_out}) do not fit out's {out.shape[1]}")
+        view = out[:, offset:]
+    b = rows // vox
+    lib = _lib.load()
+    need = lib.psa_conv3d_workspace_bytes(b, r, k, c, c_out)
+    ws = torch.empty((max(need, 4) + 3) // 4, dtype=torch.float32, device=x.device)
+    check(lib.psa_conv3d_infer(b, r, k, c, c_out, _ptr(x), x.stride(0), _ptr(weights), _ptr(scale), _ptr(shift), 1 if relu else 0,
+                               _ptr(view), out.stride(0), _ptr(ws), C.c_size_t(need), _stream()), "conv3d")
+    return out
+
+
+def pool3d(x, r: int, kind: str) -> torch.Tensor:
+    """The inception module's pools on voxel-major rows x (B*r^3, C) (psa_pool3d): 'avg' = SAME 3^3 average, stride 1, over the
+    in-grid cells -> (B*r^3, C); 'max' = SAME 2^3 max, stride 2 -> (B*ceil(r/2)^3, C)."""
+    x = _dev(x, torch.float32, "x", 2)
+    rows, c = x.shape
+    if r < 1 or rows % r ** 3:
+        raise ValueError(f"pool3d: {rows} rows are not a multiple of r^3 = {r ** 3}")
+    if kind not in ("avg", "max"):
+        raise ValueError(f"pool3d: kind must be 'avg' or 'max', got {kind!r}")
+    b = rows // r ** 3
+    ro = r if kind == "avg" else (r + 1) // 2
+    out = torch.empty((b * ro ** 3, c), dtype=torch.float32, device=x.device)
+    check(_lib.load().psa_pool3d(b, r, c, 0 if kind == "avg" else 1, _ptr(x), _ptr(out), _stream()), "pool3d")
     return out
 
 

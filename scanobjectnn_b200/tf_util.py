@@ -74,6 +74,13 @@ class VariableStore(dict):
         if bn:
             self._bn(scope, cout, randomize_bn)
 
+    def add_conv3d(self, scope, k, cin, cout, randomize_bn=False):
+        """tf_util.conv3d with bn=True (3DmFV-Net/utils/tf_util.py:254-311): weights (k,k,k,cin,cout) with Xavier limits from TF's
+        5-D fans k^3*cin and k^3*cout, zero biases, and the batch norm under ``scope/bn``."""
+        self[f"{scope}/weights"] = self._xavier((k, k, k, cin, cout), k ** 3 * cin, k ** 3 * cout)
+        self[f"{scope}/biases"] = torch.zeros(cout, device=self.device)
+        self._bn(scope, cout, randomize_bn)
+
     def add_spider_conv(self, scope, cin, cout, k=20, taylor_channel=5):
         """spiderConv's variables under ``scope`` (e.g. ``fanConv1/taylor``) with gn=True, bn=False: the 20 Taylor vectors
         (1,1,1,T) (Xavier with TF's 4-D fans 1 and T; ``biases`` zero), the [1,k] conv (1,k,cin*T,cout) (fans k*cin*T and
