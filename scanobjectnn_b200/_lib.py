@@ -7,6 +7,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libpsa.so")
 
@@ -172,6 +174,16 @@ def load() -> C.CDLL:
     lib.psa_last_error.restype = C.c_char_p
     _lib = lib
     return lib
+
+
+def ptr(t: torch.Tensor | None) -> C.c_void_p:
+    """A tensor's device pointer for the C ABI; NULL for None."""
+    return C.c_void_p(0 if t is None else t.data_ptr())
+
+
+def stream() -> C.c_void_p:
+    """The current torch CUDA stream, for the entry points' stream argument."""
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def check(rc: int, what: str) -> None:

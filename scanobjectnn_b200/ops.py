@@ -14,6 +14,8 @@ import torch
 
 from . import _lib
 from ._lib import PsaMlp, check
+from ._lib import ptr as _ptr
+from ._lib import stream as _stream
 
 __all__ = [
     "farthest_point_sample", "gather_point", "query_ball_point", "group_point", "select_top_k", "knn_point",
@@ -22,10 +24,6 @@ __all__ = [
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
     "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d",
 ]
-
-
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
 def _dev(t: torch.Tensor, dtype: torch.dtype, name: str, ndim: int | None = None) -> torch.Tensor:
@@ -38,10 +36,6 @@ def _dev(t: torch.Tensor, dtype: torch.dtype, name: str, ndim: int | None = None
     if ndim is not None and t.dim() != ndim:
         raise ValueError(f"{name}: expected a {ndim}-D tensor, got shape {tuple(t.shape)}")
     return t.contiguous()
-
-
-def _ptr(t: torch.Tensor | None) -> C.c_void_p:
-    return C.c_void_p(0 if t is None else t.data_ptr())
 
 
 def _scatter_ws(b: int, n_dst: int, entries: int, device) -> tuple[torch.Tensor, C.c_size_t]:

@@ -25,14 +25,9 @@ import torch
 
 from . import _lib, ops
 from ._lib import PsaActIn, PsaGradIn, check
+from ._lib import ptr as _p
+from ._lib import stream as _stream
 from .tf_util import BN_EPS, VariableStore
-
-_p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())  # noqa: E731
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
 
 @dataclass
 class LevelSpec:

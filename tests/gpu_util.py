@@ -6,6 +6,7 @@ import numpy as np
 import torch
 
 from oracle import oracle as orc
+from scanobjectnn_b200._lib import ptr
 
 
 def cu(a, dtype=None):
@@ -19,16 +20,12 @@ def npy(t):
     return t.detach().cpu().numpy()
 
 
-def _p(t):
-    return C.c_void_p(t.data_ptr())
-
-
 def ref_fps(xyz_t, m):
     b, n, _ = xyz_t.shape
     temp = torch.empty((32, n), dtype=torch.float32, device="cuda")
     out = torch.zeros((b, m), dtype=torch.int32, device="cuda")
     torch.cuda.synchronize()
-    rc = orc.refgpu().ref_fps(b, n, m, _p(xyz_t), _p(temp), _p(out), 1)
+    rc = orc.refgpu().ref_fps(b, n, m, ptr(xyz_t), ptr(temp), ptr(out), 1)
     assert rc == 0, rc
     return out
 
@@ -39,7 +36,7 @@ def ref_query_ball_point(radius, nsample, xyz1_t, xyz2_t, fill=0):
     idx = torch.full((b, m, nsample), fill, dtype=torch.int32, device="cuda")
     cnt = torch.zeros((b, m), dtype=torch.int32, device="cuda")
     torch.cuda.synchronize()
-    rc = orc.refgpu().ref_query_ball_point(b, n, m, C.c_float(radius), nsample, _p(xyz1_t), _p(xyz2_t), _p(idx), _p(cnt), 1)
+    rc = orc.refgpu().ref_query_ball_point(b, n, m, C.c_float(radius), nsample, ptr(xyz1_t), ptr(xyz2_t), ptr(idx), ptr(cnt), 1)
     assert rc == 0, rc
     return idx, cnt
 
@@ -49,7 +46,7 @@ def ref_group_point(points_t, idx_t):
     _, m, k = idx_t.shape
     out = torch.empty((b, m, k, c), dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
-    rc = orc.refgpu().ref_group_point(b, n, c, m, k, _p(points_t), _p(idx_t), _p(out), 1)
+    rc = orc.refgpu().ref_group_point(b, n, c, m, k, ptr(points_t), ptr(idx_t), ptr(out), 1)
     assert rc == 0, rc
     return out
 
@@ -59,7 +56,7 @@ def ref_selection_sort(k, dist_t):
     outi = torch.empty((b, m, n), dtype=torch.int32, device="cuda")
     out = torch.empty((b, m, n), dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
-    rc = orc.refgpu().ref_selection_sort(b, n, m, k, _p(dist_t), _p(outi), _p(out), 1)
+    rc = orc.refgpu().ref_selection_sort(b, n, m, k, ptr(dist_t), ptr(outi), ptr(out), 1)
     assert rc == 0, rc
     return outi, out
 
@@ -69,7 +66,7 @@ def ref_gather_point(inp_t, idx_t):
     m = idx_t.shape[1]
     out = torch.empty((b, m, 3), dtype=torch.float32, device="cuda")
     torch.cuda.synchronize()
-    rc = orc.refgpu().ref_gather_point(b, n, m, _p(inp_t), _p(idx_t), _p(out), 1)
+    rc = orc.refgpu().ref_gather_point(b, n, m, ptr(inp_t), ptr(idx_t), ptr(out), 1)
     assert rc == 0, rc
     return out
 

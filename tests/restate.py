@@ -1,0 +1,491 @@
+"""The float64 torch restatements of the models that the GPU tests compare against, and the pieces they share.
+
+A restatement evaluates a model with torch ops in the dtype of its input (float64; float32 as the yardstick of what fp32 itself
+resolves), on the GPU run's own discrete choices: neighbour graphs, FPS and ball-query indices.
+
+Where fp32 and float64 can legitimately disagree, the comparisons leave the element out on both sides instead of widening a bound.
+A max (over k neighbours, or over the N points) whose runner-up lies within 1e-5 of it may be won by another element in fp32 than
+in float64, and then routes its gradient elsewhere; likewise a head activation, or a maximum, whose pre-relu value lies within 1e-5
+of zero on either side may fall on the other side of the relu (under batch statistics that changes the gradient of its whole
+column).  These are properties of the max and the relu, not errors.  `Masks` finds such elements on the float64 side and zeroes the
+gradient arriving at them on both sides (a hook on the same tensor of each).  Layers that run inside one autograd node on the GPU,
+where no hook reaches, take the run's own relu decisions (and max-pool winners) from `RunDecisions` instead.
+
+Nothing here touches a GPU at import time."""
+import numpy as np
+import torch
+
+from scanobjectnn_b200 import training
+from scanobjectnn_b200.pointnet_seg import HEAD as SEG_HEAD
+from scanobjectnn_b200.tf_util import BN_EPS, VariableStore
+
+MOVING = ("/moving_mean", "/moving_variance")
+SSG_HEAD = [("fc1", True), ("fc2", True), ("fc3", False)]
+EC2 = ("t/tconv1", "t/tconv2")                   # the two scopes of the two-layer EdgeConv stores
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# variables
+# ---------------------------------------------------------------------------------------------------------------------
+def params_as(p, dtype, grad=False):
+    """a detached copy of every variable in `dtype`; leaves of autograd when `grad`"""
+    return {k: v.detach().to(dtype, copy=True).requires_grad_(grad) for k, v in p.items()}
+
+
+def flat_grad(p, name, g=None):
+    """variable `name`'s slice of a gradient of the flat parameter vector: by default the one autograd left on it"""
+    fp = p._flat
+    v = fp.views[name]
+    off = (v.data_ptr() - fp.flat.data_ptr()) // 4
+    return (fp.flat.grad if g is None else g)[off:off + v.numel()].view(v.shape)
+
+
+def moving(p):
+    """a copy of every batch norm's moving averages"""
+    return {k: v.clone() for k, v in p.items() if k.endswith(MOVING)}
+
+
+def perturb_tnets(p, seed):
+    """the reference initialises the T-nets' transform layers to zero, which leaves the T-nets without a gradient: draw them from
+    N(0, 0.01) instead"""
+    with torch.no_grad():
+        for name in ("transform_net1/transform_XYZ/weights", "transform_net2/transform_feat/weights"):
+            if name in p:
+                p[name].normal_(0, 0.01, generator=torch.Generator(device="cuda").manual_seed(seed))
+
+
+def grid_x(b, n, c, seed):
+    """coordinates on the 1/16 grid: with edgeconv_store's weights every edge value is exact in fp32"""
+    return np.random.default_rng(seed).integers(-32, 33, (b, n, c)).astype(np.float32) / 16.0
+
+
+def edgeconv_store(c, cout, seed, scope="e"):
+    """one conv2d(2c -> cout) + batch norm with weights, bias, gamma and beta on dyadic grids"""
+    rng = np.random.default_rng(seed)
+    p = VariableStore(device="cuda", seed=seed)
+    p.add_conv2d(scope, 2 * c, cout)
+    p[f"{scope}/weights"] = torch.tensor(rng.integers(-16, 17, (1, 1, 2 * c, cout)) / 64.0, dtype=torch.float32, device="cuda")
+    p[f"{scope}/biases"] = torch.tensor(rng.integers(-8, 9, cout) / 64.0, dtype=torch.float32, device="cuda")
+    p[f"{scope}/bn/gamma"] = torch.tensor(1.0 + rng.integers(-32, 33, cout) / 64.0, dtype=torch.float32, device="cuda")
+    p[f"{scope}/bn/beta"] = torch.tensor(rng.integers(-8, 9, cout) / 64.0, dtype=torch.float32, device="cuda")
+    return p
+
+
+def edgeconv2_store(c, seed):
+    """the two layers EC2 of DGCNN's T-net EdgeConv (2c -> 64 -> 128), batch norm randomised, biases N(0, 0.1)"""
+    p = VariableStore(device="cuda", seed=seed)
+    p.add_conv2d(EC2[0], 2 * c, 64, randomize_bn=True)
+    p.add_conv2d(EC2[1], 64, 128, randomize_bn=True)
+    rng = np.random.default_rng(seed)
+    for s, n in zip(EC2, (64, 128)):
+        p[f"{s}/biases"] = torch.tensor(rng.standard_normal(n) * 0.1, dtype=torch.float32, device="cuda")
+    return p
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# one layer, and the run's decisions it can take
+# ---------------------------------------------------------------------------------------------------------------------
+class RunDecisions:
+    """A GPU run's discrete decisions, by scope: every batch-normed layer's relu gate fmaf(y, scale, shift) > 0 (exact in float64)
+    in `gates`, in training mode the batch statistics (mean, 1 / sqrt(var + eps)) its batch norm used in `stats`, and every level's
+    max-pool winners in `argk`.  Read from a PointNet2ClsTrainer, or from a VariableStore: the last run of each MLP and level
+    trainer it caches for that mode.  stats=False leaves the batch statistics out, so a restatement keeps float64's own."""
+
+    def __init__(self, src, frozen, stats=True):
+        if isinstance(src, VariableStore):
+            trainers = src.__dict__.get("_trainers", {}).items()
+            layers = [ly for key, tr in trainers if key[0] == ("mlp_frozen" if frozen else "mlp") for ly in tr.layers]
+            levels = [tr.levels[0] for key, tr in trainers if key[0] == ("level_frozen" if frozen else "level")]
+        else:
+            layers, levels = src.head, src.levels
+        self.gates, self.stats = {}, {}
+        for ly in layers + [ly for lv in levels for ly in lv.layers]:
+            if ly.bn:
+                self.gates[ly.scope] = (ly.y.double() * ly.scale.double() + ly.shift.double()) > 0
+                if stats and not frozen:
+                    self.stats[ly.scope] = ly.mean_inv
+        self.argk = {lv.spec.scope: lv.argk for lv in levels}
+
+
+def layer(h, P, scope, frozen, *, bn=True, relu=True, stats=None, run=None, info=None):
+    """conv2d / fully_connected (+ batch norm + relu) in h's dtype.  Batch norm on the moving averages (frozen) or on the batch
+    statistics over every row (biased variance), eps BN_EPS; the batch statistics are recorded in `stats[scope]` when a dict is given.
+
+    With a `run` (RunDecisions) the relu is z * the run's gate, and `info` counts the gates that differ from float64's own ("flips"
+    of "units").  In training mode the batch statistics then take the run's values, float64's derivative: fp32 sums of y and y^2
+    give the variance with an error relative to E[y^2], not to the variance, and that error is bounded on its own
+    (info["stat_err"], relative to E[y^2]) instead of through every later layer."""
+    dt = h.dtype
+    w = P[f"{scope}/weights"].to(dt)
+    y = h @ w.reshape(-1, w.shape[-1]) + P[f"{scope}/biases"].to(dt)
+    if not bn:
+        return y
+    if frozen:
+        mean, var = P[f"{scope}/bn/moving_mean"].to(dt), P[f"{scope}/bn/moving_variance"].to(dt)
+    else:
+        dims = tuple(range(y.dim() - 1))
+        mean, var = y.mean(dims), y.var(dims, unbiased=False)
+        if run is not None and scope in run.stats:
+            rmean, rinv = run.stats[scope][0].to(dt), run.stats[scope][1].to(dt)
+            rvar = 1.0 / (rinv * rinv) - BN_EPS
+            ms = float((y.detach() ** 2).mean(dims).max())
+            info["stat_err"] = max(info["stat_err"], float((rmean - mean.detach()).abs().max()) / ms ** 0.5,
+                                   float((rvar - var.detach()).abs().max()) / ms)
+            mean, var = mean + (rmean - mean).detach(), var + (rvar - var).detach()
+        if stats is not None:
+            stats[scope] = (mean.detach(), var.detach())
+    z = (y - mean) / torch.sqrt(var + BN_EPS) * P[f"{scope}/bn/gamma"].to(dt) + P[f"{scope}/bn/beta"].to(dt)
+    if not relu:
+        return z
+    if run is not None and scope in run.gates:
+        gate = run.gates[scope].view(z.shape)
+        info["flips"] += int((gate != (z > 0)).sum())
+        info["units"] += gate.numel()
+        return z * gate
+    return torch.relu(z)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the exclusion rule
+# ---------------------------------------------------------------------------------------------------------------------
+def ambiguous(z, dim):
+    """True where the max over `dim` has a runner-up of a different value within 1e-5 (of the largest activation) of it, or is a
+    positive maximum within that distance of the relu's zero"""
+    with torch.no_grad():
+        mx = z.amax(dim=dim, keepdim=True)
+        below = torch.where(z < mx, z, torch.full_like(z, -1.0)).amax(dim=dim)
+        tol = 1e-5 * float(z.abs().max())
+        mx = mx.squeeze(dim)
+        return ((mx - below) < tol) | ((mx > 0) & (mx < tol))
+
+
+def near_zero(z):
+    """True where a pre-relu value lies within 1e-5 (of the largest magnitude) of zero"""
+    with torch.no_grad():
+        return z.abs() < 1e-5 * float(z.abs().max())
+
+
+def near_zero_max(pre, dim, scale):
+    """True where the max over `dim` of the pre-relu values lies within 1e-5 of `scale` of the relu's zero, on either side: a maximum
+    slightly below zero in float64 may lie slightly above it in fp32, and then carries the whole gradient"""
+    with torch.no_grad():
+        return pre.amax(dim=dim).abs() < 1e-5 * scale
+
+
+def inner_flip(pre, inner):
+    """True where the edge that wins the max over k (dim 2) of `pre` (b, n, k, c) has a unit of `inner` (b, n, k, c1), the pre-relu
+    values of the layer below, within 1e-5 (of the largest magnitude) of zero"""
+    with torch.no_grad():
+        return near_zero(inner).any(dim=-1).gather(2, pre.argmax(dim=2))
+
+
+def zero_at(t, mask):
+    t.register_hook(lambda g: g.masked_fill(mask, 0.0))
+
+
+class Masks:
+    """The elements a comparison leaves out, in the order the model reaches them: `edge` for the maxima over k neighbours (EdgeConv
+    outputs, set-abstraction levels), `pool` for the maxima over the N points, keyed by scope, `act` for the head's near-zero relu
+    inputs, keyed by scope.
+
+    Masks(replay=first), or first.replay(), looks for none: it applies the masks `first` recorded, whatever the values and the
+    `pre` / `inner` arguments, so that a second pass (in float32, or on the run's batch statistics, which move values by far less
+    than 1e-5 but may move a few across it) leaves out the same elements."""
+
+    def __init__(self, replay=None):
+        self.edge, self.pool, self.act = [], {}, {}
+        self._first = replay
+
+    def replay(self):
+        return Masks(replay=self)
+
+    def edge_max(self, z, pre=None, inner=None):
+        """max over k of the activated edge values z; given their pre-relu values `pre`, a maximum within 1e-5 of the relu's zero on
+        either side is ambiguous too, and given a fused first layer's pre-relu values `inner` (b, n, k, c1), so is a maximum whose
+        edge has a unit of that layer within 1e-5 of zero (the kernel's relu may fall the other way there)"""
+        if self._first is not None:
+            amb = self._first.edge[len(self.edge)]
+        else:
+            amb = ambiguous(z, 2)
+            if pre is not None:
+                amb |= near_zero_max(pre, 2, float(z.detach().abs().max()))
+            if inner is not None:
+                amb |= inner_flip(pre, inner)
+        out = z.amax(dim=2)
+        zero_at(out, amb)
+        self.edge.append(amb)
+        return out
+
+    def point_max(self, y, scope, pre=None):
+        if self._first is not None:
+            amb = self._first.pool[scope]
+        else:
+            amb = ambiguous(y, 1)
+            if pre is not None:
+                amb |= near_zero_max(pre, 1, float(y.detach().abs().max()))
+        zero_at(y, amb.unsqueeze(1))
+        self.pool[scope] = amb
+        return y.amax(dim=1)
+
+    def head_layer(self, h, P, scope, frozen, **kw):
+        """layer(), its relu's near-zero inputs left out"""
+        z = layer(h, P, scope, frozen, relu=False, **kw)
+        near = self._first.act[scope] if self._first is not None else near_zero(z)
+        out = torch.relu(z)
+        zero_at(out, near)
+        self.act[scope] = near
+        return out
+
+    def count(self):
+        ms = self.edge + list(self.pool.values()) + list(self.act.values())
+        return sum(int(m.sum()) for m in ms), sum(m.numel() for m in ms)
+
+    def patch(self, monkeypatch):
+        """zero the gradient at the same elements on the GPU path: hooks on the outputs of its EdgeConv and set-abstraction nodes
+        (`edge`, in the order the model calls them) and of its MLP nodes (`pool` and `act`, by the node's last scope)"""
+        edge, pool, act = iter(self.edge), self.pool, self.act
+        ec, sa, mlp = training.edgeconv_training, training.sa_module_training, training.mlp_training
+
+        def edgeconv_training(*a, **kw):
+            out = ec(*a, **kw)
+            zero_at(out, next(edge))
+            return out
+
+        def sa_module_training(*a, **kw):
+            new_xyz, out, idx = sa(*a, **kw)
+            zero_at(out, next(edge))
+            return new_xyz, out, idx
+
+        def mlp_training(x, layers, *a, **kw):
+            out = mlp(x, layers, *a, **kw)
+            scope = layers[-1][0]
+            if scope in pool:
+                zero_at(out, pool[scope].unsqueeze(1))
+            if scope in act:
+                zero_at(out, act[scope])
+            return out
+
+        monkeypatch.setattr(training, "edgeconv_training", edgeconv_training)
+        monkeypatch.setattr(training, "sa_module_training", sa_module_training)
+        monkeypatch.setattr(training, "mlp_training", mlp_training)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# model pieces
+# ---------------------------------------------------------------------------------------------------------------------
+def edges(x, idx):
+    """the EdgeConv input [x_i, x_j - x_i] (b, n, k, 2c) over the neighbour graph idx (b, n, k)"""
+    b, n, c = x.shape
+    k = idx.shape[-1]
+    neigh = x[torch.arange(b, device=x.device).view(b, 1, 1), idx.long()]
+    centre = x.unsqueeze(2).expand(b, n, k, c)
+    return torch.cat([centre, neigh - centre], dim=-1)
+
+
+def tnet(h, P, scope, K, L, masks):
+    """PointNet's transform net (pointnet/models/transform_nets.py) on h (b, n, c) -> (b, K, K); L: the caller's layer()"""
+    g = masks.point_max(L(L(L(h, f"{scope}/tconv1"), f"{scope}/tconv2"), f"{scope}/tconv3"), f"{scope}/tconv3")
+    g = L(L(g, f"{scope}/tfc1"), f"{scope}/tfc2")
+    name = "transform_XYZ" if K == 3 else "transform_feat"
+    eye = torch.eye(K, dtype=h.dtype, device=h.device).flatten()
+    return (g @ P[f"{scope}/{name}/weights"] + P[f"{scope}/{name}/biases"] + eye).reshape(h.shape[0], K, K)
+
+
+def sa_level(xyz, pts, fps=None, ball=None):
+    """a set-abstraction level's grouping on given int64 FPS and ball-query indices -> (new_xyz, rows (b, m, k, 3 + c): the
+    coordinates relative to their centre, then the features); without indices group all: one group of every point, centre 0"""
+    if fps is None:
+        return torch.zeros_like(xyz[:, :1]), (xyz if pts is None else torch.cat([xyz, pts], -1))[:, None]
+    ar = torch.arange(xyz.shape[0], device=xyz.device)
+    new_xyz = xyz[ar[:, None], fps]
+    h = xyz[ar[:, None, None], ball] - new_xyz[:, :, None, :]
+    if pts is not None:
+        h = torch.cat([h, pts[ar[:, None, None], ball]], -1)
+    return new_xyz, h
+
+
+def interpolate(xyz1, xyz2, points2):
+    """three_nn (tf_interpolate.cpp:60-103: squared distances, neighbours not found stay at 1e40 = inf in float, index 0), weights
+    (1/max(d,1e-10)) / sum (pointnet_util.py:211-216), no gradient through them, and three_interpolate"""
+    b = xyz1.shape[0]
+    with torch.no_grad():
+        d = ((xyz1.detach()[:, :, None, :] - xyz2.detach()[:, None, :, :]) ** 2).sum(-1)
+        if d.shape[-1] < 3:
+            d = torch.cat([d, torch.full((*d.shape[:2], 3 - d.shape[-1]), float("inf"), dtype=d.dtype, device=d.device)], dim=-1)
+        dist, idx = d.topk(3, dim=-1, largest=False, sorted=True)
+        idx[torch.isinf(dist)] = 0
+        inv = 1.0 / dist.clamp_min(1e-10)
+        w = inv / inv.sum(-1, keepdim=True)
+    ar = torch.arange(b, device=xyz1.device)[:, None, None]
+    return (points2[ar, idx] * w[..., None]).sum(dim=2)
+
+
+def _argk_pool(h, argk, info):
+    """the max over dim 2 taken at the run's winner argk (its first winning row), so the gradient goes where the kernel sends it;
+    info["pool_gap"]: how far below h's own maximum that row lies, relative to h's largest entry"""
+    B, m, _, c = h.shape
+    out = h.gather(2, argk.long().view(B, m, 1, c)).squeeze(2)
+    with torch.no_grad():
+        gap = float((h.amax(dim=2) - out).max()) / max(float(h.abs().max()), 1e-30)
+        info["pool_gap"] = max(info["pool_gap"], gap)
+    return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the models
+# ---------------------------------------------------------------------------------------------------------------------
+def ssg(xyz, p, levels, frozen, masks, run=None, info=None):
+    """pointnet2_cls_ssg (or bga's classification branch) restated in torch ops of xyz's dtype on the levels' FPS / ball-query
+    indices; `masks`: the head's dropout masks, by scope.  run: the PointNet2ClsTrainer whose discrete decisions are taken instead of
+    the restatement's own -- every batch-normed layer's relu gate and every level's max-pool winner (batch statistics stay
+    float64's); `info` then collects the batch statistics ("stats"), the flipped gates ("flips" of "units") and the largest pool gap
+    ("pool_gap")."""
+    dec = None if run is None else RunDecisions(run, frozen, stats=False)
+    stats = None if info is None else info.setdefault("stats", {})
+    L = lambda h, s, **kw: layer(h, p, s, frozen, stats=stats, run=dec, info=info, **kw)        # noqa: E731
+    cur_xyz, cur_pts = xyz, None
+    for lv in levels:
+        sp = lv.spec
+        new_xyz, h = sa_level(cur_xyz, cur_pts, *((None, None) if sp.group_all else (lv.fps_idx.long(), lv.idx.long())))
+        for i in range(len(sp.mlp)):
+            h = L(h, f"{sp.scope}/conv{i}")
+        cur_xyz, cur_pts = new_xyz, h.amax(dim=2) if dec is None else _argk_pool(h, dec.argk[sp.scope], info)
+    h = cur_pts.reshape(xyz.shape[0], -1)
+    for scope, bn in SSG_HEAD:
+        h = L(h, scope, bn=bn)
+        if scope in masks:
+            h = h * masks[scope].to(h.dtype)
+    return h
+
+
+def dgcnn(x, P, graphs, frozen, masks, detach_transform=False, stats=None):
+    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55), dropout off, on the given neighbour graphs -> logits; stats (a
+    dict): every layer's batch statistics, by scope"""
+    b = x.shape[0]
+    L = lambda h, s, **kw: layer(h, P, s, frozen, stats=stats, **kw)        # noqa: E731
+    sc = "transform_net1"
+    y1 = L(edges(x, graphs[0]), f"{sc}/tconv1", relu=False)
+    y = L(torch.relu(y1), f"{sc}/tconv2", relu=False)
+    h = masks.edge_max(torch.relu(y), pre=y, inner=y1)
+    y = L(h, f"{sc}/tconv3", relu=False)
+    h = masks.point_max(torch.relu(y), f"{sc}/tconv3", pre=y)
+    h = L(L(h, f"{sc}/tfc1"), f"{sc}/tfc2")
+    t = (h @ P[f"{sc}/transform_XYZ/weights"] + P[f"{sc}/transform_XYZ/biases"] + torch.eye(3, dtype=x.dtype, device=x.device).flatten())
+    t = t.reshape(b, 3, 3)
+    h = torch.bmm(x, t.detach() if detach_transform else t)
+    nets = []
+    for i, s in enumerate(["dgcnn1", "dgcnn2", "dgcnn3", "dgcnn4"]):
+        y = L(edges(h, graphs[i + 1]), s, relu=False)
+        h = masks.edge_max(torch.relu(y), pre=y)
+        nets.append(h)
+    y = L(torch.cat(nets, dim=-1), "agg", relu=False)
+    g = masks.point_max(torch.relu(y), "agg", pre=y)
+    for s in ("fc1", "fc2"):
+        g = masks.head_layer(g, P, s, frozen, stats=stats)
+    return L(g, "fc3", bn=False)
+
+
+def pointnet(x, P, masks):
+    """pointnet_cls.get_model (pointnet_cls.py:21-75) with frozen batch norm -> (logits, feature transform)"""
+    L = lambda h, s, **kw: layer(h, P, s, True, **kw)        # noqa: E731
+    h = torch.bmm(x, tnet(x, P, "transform_net1", 3, L, masks))
+    h = L(L(h, "conv1"), "conv2")
+    t2 = tnet(h, P, "transform_net2", 64, L, masks)
+    h = torch.bmm(h, t2)
+    g = masks.point_max(L(L(L(h, "conv3"), "conv4"), "conv5"), "conv5")
+    for s in ("fc1", "fc2"):
+        g = masks.head_layer(g, P, s, True)
+    return L(g, "fc3", bn=False), t2
+
+
+def pointnet_seg(x, P, frozen, masks, classify, run=None):
+    """pointnet_seg (classify) or pointnet_partseg, dropout off, building tile + concat as the reference does
+    (pointnet/models/pointnet_seg.py:24-134, pointnet_partseg.py:23-124) -> ([class_pred,] seg_pred, feature transform,
+    {"stats", "flips", "units", "stat_err"}); run: RunDecisions"""
+    b, n, _ = x.shape
+    info = {"stats": {}, "flips": 0, "units": 0, "stat_err": 0.0}
+    kw = dict(stats=info["stats"], run=run, info=info)
+    L = lambda h, s, **k: layer(h, P, s, frozen, **kw, **k)        # noqa: E731
+    h = L(L(torch.bmm(x, tnet(x, P, "transform_net1", 3, L, masks)), "conv1"), "conv2")
+    t2 = tnet(h, P, "transform_net2", 64, L, masks)
+    point_feat = torch.bmm(h, t2)
+    g = masks.point_max(L(L(L(point_feat, "conv3"), "conv4"), "conv5"), "conv5")
+    out = []
+    if classify:
+        c = g
+        for s in ("fc1", "fc2"):
+            c = masks.head_layer(c, P, s, frozen, **kw)
+        out.append(L(c, "fc3", bn=False))
+    h = torch.cat([point_feat, g.unsqueeze(1).expand(b, n, g.shape[-1])], dim=2)          # tile + concat
+    for s in SEG_HEAD:
+        h = L(h, s)
+    out.append(L(h, "conv10", bn=False))
+    return out, t2, info
+
+
+def pointnet2_partseg(x, P, frozen, masks, idx, run=None):
+    """pointnet2_cls_partseg, dropout off, on the given level indices [(fps, ball)] * 2, building fa_layer1's input as the reference
+    does (pointnet2/models/pointnet2_cls_partseg.py:20-87, pointnet_util.py:199-229) -> (seg_pred, {"stats", "flips", "units",
+    "stat_err"}); run: RunDecisions"""
+    info = {"stats": {}, "flips": 0, "units": 0, "stat_err": 0.0}
+    L = lambda h, s, **kw: layer(h, P, s, frozen, stats=info["stats"], run=run, info=info, **kw)        # noqa: E731
+
+    def level(xyz, pts, scope, fps=None, ball=None):
+        new_xyz, h = sa_level(xyz, pts, fps, ball)
+        for i in range(3):
+            h = L(h, f"{scope}/conv{i}")
+        return new_xyz, masks.edge_max(h)
+
+    def fp(xyz1, xyz2, pts1, pts2, scope, n):
+        h = interpolate(xyz1, xyz2, pts2)
+        h = torch.cat([h, pts1], dim=2) if pts1 is not None else h          # tile + concat for fa_layer1
+        for i in range(n):
+            h = L(h, f"{scope}/conv_{i}")
+        return h
+
+    (f1, i1), (f2, i2) = idx
+    l1_xyz, l1 = level(x, None, "layer1", f1, i1)
+    l2_xyz, l2 = level(l1_xyz, l1, "layer2", f2, i2)
+    l3_xyz, l3 = level(l2_xyz, l2, "layer3")
+    l2 = fp(l2_xyz, l3_xyz, l2, l3, "fa_layer1", 2)
+    l1 = fp(l1_xyz, l2_xyz, l1, l2, "fa_layer2", 2)
+    l0 = fp(x, l1_xyz, None, l1, "fa_layer3", 3)
+    return L(L(l0, "seg_fc1"), "seg_fc2", bn=False), info
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# metrics
+# ---------------------------------------------------------------------------------------------------------------------
+def rel(got, want):
+    """max |got - want| relative to the largest entry of want"""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    return float(np.abs(got - want).max() / max(1e-30, np.abs(want).max()))
+
+
+def out_err(got, want):
+    """max |got - want| relative to max(1, the largest entry of want)"""
+    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
+    return float(np.abs(got - want).max() / max(1.0, np.abs(want).max()))
+
+
+def err(got, want, scale=None):
+    """max |got - want| of two tensors relative to `scale`, by default the largest entry of want"""
+    want = want.detach().double()
+    scale = float(want.abs().max()) if scale is None else scale
+    return float((got.detach().double() - want).abs().max()) / max(scale, 1e-30)
+
+
+def within(e, e32, tol, factor):
+    """the bound, or where the float32 restatement itself misses it, `factor` times the float32 restatement's error"""
+    return e < tol or e <= factor * e32
+
+
+def grad_errors(p, P, P32):
+    """per variable: (max|run - float64|, max|float32 restatement - float64|), and the largest float64 entry"""
+    errs, scale = {}, 0.0
+    for name in p._flat.names:
+        want = P[name].grad if P[name].grad is not None else torch.zeros_like(P[name])
+        g32 = P32[name].grad if P32[name].grad is not None else torch.zeros_like(P32[name])
+        errs[name] = (float((flat_grad(p, name).double() - want).abs().max()), float((g32.double() - want).abs().max()))
+        scale = max(scale, float(want.abs().max()))
+    return errs, scale

@@ -401,7 +401,7 @@ def test_pointnet_cls_calibrated(model_case, monkeypatch):
     _close(G.npy(logits), mo.mlp_chain(G.npy(glob), p, ["fc1", "fc2", "fc3"], [True, True, False]), f"pointnet logits {tag}")
 
 
-def _dgcnn64(xyz, p, k=20):
+def _dgcnn_oracle_logits(xyz, p, k=20):
     """dgcnn.get_model in float64 on the oracle's own graphs (only used to calibrate: every layer in forward order)"""
     t = mo.edgeconv(xyz, orc.dgcnn_knn(xyz, k), p, ["transform_net1/tconv1", "transform_net1/tconv2"])
     t = mo.mlp_chain(t, p, ["transform_net1/tconv3"]).max(axis=1)
@@ -425,7 +425,7 @@ def test_dgcnn_stagewise_calibrated(model_case, monkeypatch):
                                                                    generator=torch.Generator(device="cuda").manual_seed(5))
     _scale_weights(p, s)
     cal = make_clouds("ball", b, n, seed=905)
-    done = calibrate(p, monkeypatch, lambda: _dgcnn64(cal, p))
+    done = calibrate(p, monkeypatch, lambda: _dgcnn_oracle_logits(cal, p))
     check_regime(p, done, s)
     xyz = make_clouds("ball", b, n, seed=906)
     cls, ep = dgcnn.get_model(G.cu(xyz), False, params=p)

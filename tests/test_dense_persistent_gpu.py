@@ -8,7 +8,7 @@ import torch
 
 from oracle import mlp_oracle as mo
 from scanobjectnn_b200 import _lib, ops
-from scanobjectnn_b200._lib import PsaActIn
+from scanobjectnn_b200._lib import PsaActIn, ptr, stream
 from scanobjectnn_b200.tf_util import VariableStore
 
 from . import gpu_util as G
@@ -60,13 +60,11 @@ def test_training_forward_is_bitwise_repeatable():
     ws = torch.empty(need // 4 + 16, device="cuda")
     a = PsaActIn()
     a.x = xd.data_ptr(); a.ld = K; a.mask = None; a.relu = 1; a.scale = sd.data_ptr(); a.shift = td.data_ptr()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
     outs = []
     for _ in range(2):
         y = torch.empty((rows, N), device="cuda")
         stats = torch.empty((2, N), device="cuda")
-        assert lib.psa_train_dense_fwd(rows, K, N, C.byref(a), C.c_void_p(Wd.data_ptr()), C.c_void_p(bd.data_ptr()), C.c_void_p(y.data_ptr()),
-                                       C.c_void_p(stats.data_ptr()), C.c_void_p(ws.data_ptr()), C.c_size_t(need), st) == 0
+        assert lib.psa_train_dense_fwd(rows, K, N, C.byref(a), ptr(Wd), ptr(bd), ptr(y), ptr(stats), ptr(ws), C.c_size_t(need), stream()) == 0
         outs.append((y, stats))
     assert torch.equal(outs[0][0], outs[1][0]) and torch.equal(outs[0][1], outs[1][1])
     h = np.maximum(G.npy(xd).astype(np.float64) * G.npy(sd) + G.npy(td), 0)

@@ -1,11 +1,11 @@
 """DGCNN's training step (dgcnn._get_model_training: batch statistics everywhere, dropout off) against a float64 restatement,
 variable by variable, and each of its fused EdgeConv ops in isolation on the model's own activations.
 
-1. The model: one step on the graphs of a first run, against test_input_grad_dgcnn_gpu's _dgcnn64 on the same graphs.  Each tensor is
+1. The model: one step on the graphs of a first run, against restate.dgcnn on the same graphs.  Each tensor is
    compared relative to its own largest entry: the logits and every batch-norm layer's moving averages within 1e-5, every variable's
    slice of the flat gradient (the T-net's included) and x.grad within 1e-4.  A bias followed by batch norm has a gradient of exactly
-   zero.  Near-tied maxima, maxima near the relu's zero and near-zero head activations are masked on both sides as in
-   test_input_grad_dgcnn_gpu.py.  Next to each error stands that of the restatement evaluated in float32 with the same masks; where
+   zero.  Near-tied maxima, maxima near the relu's zero and near-zero head activations are masked on both sides by the exclusion
+   rule of tests/restate.py.  Next to each error stands that of the restatement evaluated in float32 with the same masks; where
    float32 itself misses the bound, the step must stay within 2x of it.
 2. The ops: the input, graph and arriving gradient of every EdgeConv of a GPU step (dgcnn1..4 and the T-net's tconv1 + tconv2) are
    captured, and the op is run again on exactly those inputs against the float64 formula (output, batch statistics, dW, dgamma, dbeta,
@@ -20,9 +20,13 @@ import pytest
 import torch
 
 from scanobjectnn_b200 import _lib, dgcnn, training
+from scanobjectnn_b200._lib import ptr, stream
+from scanobjectnn_b200.synthetic import make_clouds
 from scanobjectnn_b200.tf_util import VariableStore
 
-from .test_input_grad_dgcnn_gpu import _dgcnn64, _dgcnn_setup, _edges, _layer, _Masks, _p64, _rel, _zero_at
+from . import gpu_util as G
+from . import restate
+from .restate import Masks, edges, err, flat_grad, layer, params_as, perturb_tnets, rel, within
 
 OTOL, GTOL = 1e-5, 1e-4
 DECAY = 0.5                      # the model's bn_decay
@@ -41,63 +45,24 @@ def _loss_weights(b, seed):
 
 def _first_run(b, n, seed):
     """the store, the cloud and the five neighbour graphs of a first training-mode forward (which also moves the moving averages)"""
-    p, x0 = _dgcnn_setup(b, n, seed)
+    p = dgcnn.init_params(seed=seed, randomize_bn=True)
+    perturb_tnets(p, seed)
+    x0 = G.cu(make_clouds("ball", b, n, seed=seed + 100))
     _, ep = dgcnn._get_model_training(x0, DECAY, dgcnn.NUM_CLASSES, p, dropout=False)
     return p, x0, [ep[f"nn_idx{i}"] for i in range(5)]
-
-
-def _flat_grad(p, name):
-    """the gradient of variable `name` as autograd left it on the flat parameter vector"""
-    fp = p._flat
-    v = fp.views[name]
-    off = (v.data_ptr() - fp.flat.data_ptr()) // 4
-    return fp.flat.grad[off:off + v.numel()].view(v.shape)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 1. the model-level step
 # ---------------------------------------------------------------------------------------------------------------------
-class _SameMasks(_Masks):
-    """replays the maxima and head activations another _Masks found, so that a float32 evaluation of the restatement masks the same
-    elements as the float64 one"""
-
-    def __init__(self, src: _Masks):
-        super().__init__()
-        self.src = src
-
-    def edge_max(self, z, pre=None, inner=None):
-        amb = self.src.edge[len(self.edge)]
-        out = z.amax(dim=2)
-        _zero_at(out, amb)
-        self.edge.append(amb)
-        return out
-
-    def point_max(self, y, scope, pre=None):
-        self.pool[scope] = amb = self.src.pool[scope]
-        _zero_at(y, amb.unsqueeze(1))
-        return y.amax(dim=1)
-
-    def head_layer(self, h, P, scope, frozen, stats=None):
-        out = torch.relu(_layer(h, P, scope, frozen, relu=False, stats=stats))
-        self.act[scope] = near = self.src.act[scope]
-        _zero_at(out, near)
-        return out
-
-
-def _restatement(x0, P0, trainable, graphs, R, masks, dtype):
-    """_dgcnn64 in `dtype` with the loss (logits * R).sum() differentiated -> (logits, x.grad, variables, batch statistics)"""
-    P = {k: v.to(dtype, copy=True).requires_grad_(k in trainable) for k, v in P0.items()}
+def _restatement(x0, P0, graphs, R, masks, dtype):
+    """restate.dgcnn in `dtype` with the loss (logits * R).sum() differentiated -> (logits, x.grad, variables, batch statistics)"""
+    P = params_as(P0, dtype, grad=True)
     x = x0.to(dtype, copy=True).requires_grad_(True)
     stats = {}
-    logits = _dgcnn64(x, P, graphs, False, masks, stats=stats)
+    logits = restate.dgcnn(x, P, graphs, False, masks, stats=stats)
     (logits * R.to(dtype)).sum().backward()
     return logits.detach(), x.grad, P, stats
-
-
-def _err(got, want, scale=None):
-    want = want.detach().double()
-    scale = float(want.abs().max()) if scale is None else scale
-    return float((got.detach().double() - want).abs().max()) / max(scale, 1e-30)
 
 
 def _step_against_float64(b, n, seed, monkeypatch):
@@ -106,11 +71,11 @@ def _step_against_float64(b, n, seed, monkeypatch):
     counts)"""
     p, x0, graphs = _first_run(b, n, seed)
     R = _loss_weights(b, seed)
-    P0 = _p64(p)                                     # the moving averages the step starts from
+    P0 = params_as(p, torch.float64)                 # the moving averages the step starts from
     trainable = set(p._flat.names)
-    masks = _Masks()
-    l64, gx64, P, stats = _restatement(x0, P0, trainable, graphs, R, masks, torch.float64)
-    l32, gx32, P32, stats32 = _restatement(x0, P0, trainable, graphs, R, _SameMasks(masks), torch.float32)
+    masks = Masks()
+    l64, gx64, P, stats = _restatement(x0, P0, graphs, R, masks, torch.float64)
+    l32, gx32, P32, stats32 = _restatement(x0, P0, graphs, R, masks.replay(), torch.float32)
 
     p._flat.flat.grad = None
     with monkeypatch.context() as m:
@@ -120,10 +85,10 @@ def _step_against_float64(b, n, seed, monkeypatch):
         (logits * R).sum().backward()
     assert all(torch.equal(ep[f"nn_idx{i}"], graphs[i]) for i in range(5))
 
-    errs = {"logits": (_err(logits, l64), _err(l32, l64)), "x.grad": (_err(x.grad, gx64), _err(gx32, gx64))}
+    errs = {"logits": (err(logits, l64), err(l32, l64)), "x.grad": (err(x.grad, gx64), err(gx32, gx64))}
     bn_biases = {f"{s}/biases" for s in stats}
     for name in sorted(trainable):
-        got = _flat_grad(p, name)
+        got = flat_grad(p, name)
         if name in bn_biases:
             assert not bool(got.any()), f"{name}: a bias followed by batch norm must get a gradient of exactly zero"
             continue
@@ -131,22 +96,21 @@ def _step_against_float64(b, n, seed, monkeypatch):
         scale = float(want.abs().max())
         if name in POOLED_BETAS:
             scale = max(scale, float(P[name.replace("/beta", "/gamma")].grad.abs().max()))
-        errs[("grad", name)] = (_err(got, want, scale), _err(P32[name].grad, want, scale))
+        errs[("grad", name)] = (err(got, want, scale), err(P32[name].grad, want, scale))
     for scope, (mean, var) in stats.items():
         for i, suffix in enumerate(("moving_mean", "moving_variance")):
             name = f"{scope}/bn/{suffix}"
             want = (1 - DECAY) * (mean, var)[i] + DECAY * P0[name]
-            errs[("moving", name)] = (_err(p[name], want), _err((1 - DECAY) * stats32[scope][i].double() + DECAY * P0[name], want))
+            errs[("moving", name)] = (err(p[name], want), err((1 - DECAY) * stats32[scope][i].double() + DECAY * P0[name], want))
     assert {f"{s}/biases" for s in ("dgcnn1", "dgcnn4", "agg", "fc2", TNET[0], "transform_net1/tfc2")} <= bn_biases
     assert ("grad", "transform_net1/transform_XYZ/weights") in errs and ("grad", "fc3/biases") in errs
     return errs, masks.count()
 
 
 def _within(key, e, e32):
-    """the bound, or where float32 itself does not reach it, 2x the float32 restatement's error"""
+    """the bound of an output or a gradient, or where float32 itself does not reach it, 2x the float32 restatement's error"""
     output = key in ("logits", "out") or (isinstance(key, tuple) and (key[0] == "moving" or key[1] in ("moving_mean", "moving_variance")))
-    tol = OTOL if output else GTOL
-    return e < tol or e <= 2 * e32
+    return within(e, e32, OTOL if output else GTOL, 2)
 
 
 @pytest.mark.gpu
@@ -196,16 +160,16 @@ def _capture(b, n, seed, monkeypatch):
 
 def _formula(p, scopes, x, idx, dout, dtype, amb=None):
     """[x_i, x_j - x_i] -> (conv + batch norm + relu) per scope -> max over k in `dtype`, differentiated by torch autograd against
-    dout (zeroed at `amb`, by default the maxima _Masks.edge_max finds ambiguous) -> (amb, output, batch statistics by scope,
+    dout (zeroed at `amb`, by default the maxima Masks.edge_max finds ambiguous) -> (amb, output, batch statistics by scope,
     {quantity: tensor})"""
     P = {f"{s}/{v}": p[f"{s}/{v}"].detach().to(dtype, copy=True).requires_grad_(True) for s in scopes for v in BN_SUFFIXES[:4]}
     xd = x.detach().to(dtype, copy=True).requires_grad_(True)
-    stats, pre, h = {}, [], _edges(xd, idx)
+    stats, pre, h = {}, [], edges(xd, idx)
     for s in scopes:
-        pre.append(_layer(h, P, s, False, relu=False, stats=stats))
+        pre.append(layer(h, P, s, False, relu=False, stats=stats))
         h = torch.relu(pre[-1])
     if amb is None:
-        masks = _Masks()
+        masks = Masks()
         masks.edge_max(h, pre=pre[-1], inner=pre[0] if len(scopes) == 2 else None)
         amb = masks.edge[0]
     out = h.amax(dim=2)
@@ -232,18 +196,18 @@ def _op_against_float64(p, rec):
     (out * dout.masked_fill(amb, 0.0)).sum().backward()
     got = {"dx": xin.grad}
     for s in scopes:
-        got.update({(s, "dW"): _flat_grad(q, f"{s}/weights").reshape(-1, q[f"{s}/weights"].shape[-1]),
-                    (s, "dgamma"): _flat_grad(q, f"{s}/bn/gamma"), (s, "dbeta"): _flat_grad(q, f"{s}/bn/beta")})
-        assert not bool(_flat_grad(q, f"{s}/biases").any())
-    errs = {"out": (_rel(out.detach().cpu(), o64.cpu()), _rel(o32.cpu(), o64.cpu()))}
+        got.update({(s, "dW"): flat_grad(q, f"{s}/weights").reshape(-1, q[f"{s}/weights"].shape[-1]),
+                    (s, "dgamma"): flat_grad(q, f"{s}/bn/gamma"), (s, "dbeta"): flat_grad(q, f"{s}/bn/beta")})
+        assert not bool(flat_grad(q, f"{s}/biases").any())
+    errs = {"out": (rel(out.detach().cpu(), o64.cpu()), rel(o32.cpu(), o64.cpu()))}
     for s in scopes:
         for i, suffix in enumerate(("moving_mean", "moving_variance")):
             name = f"{s}/bn/{suffix}"
             want = (1 - OP_DECAY) * st64[s][i] + OP_DECAY * moving0[name]
             yard = (1 - OP_DECAY) * st32[s][i].double() + OP_DECAY * moving0[name]
-            errs[(s, suffix)] = (_rel(q[name].cpu(), want.cpu()), _rel(yard.cpu(), want.cpu()))
+            errs[(s, suffix)] = (rel(q[name].cpu(), want.cpu()), rel(yard.cpu(), want.cpu()))
     for key, want in g64.items():
-        errs[key] = (_rel(got[key].cpu(), want.cpu()), _rel(g32[key].cpu(), want.cpu()))
+        errs[key] = (rel(got[key].cpu(), want.cpu()), rel(g32[key].cpu(), want.cpu()))
     return errs, int(amb.sum()), amb.numel()
 
 
@@ -274,7 +238,7 @@ def test_head_batch_statistics_match_float64(b, n, seed):
     correctly rounded fp32 sums (psa_bn_finalize's input) is printed beside it."""
     p, _, _ = _first_run(b, n, seed)
     lib = _lib.load()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+    st = stream()
     ratio = 0.0
     for scope in ("transform_net1/tfc1", "fc1"):
         ly = next(ly for tr in p._trainers.values() for ly in tr.layers if ly.scope == scope)
@@ -288,23 +252,20 @@ def test_head_batch_statistics_match_float64(b, n, seed):
             f = lambda: torch.empty(ly.N, device="cuda")          # noqa: E731
             scale, shift, mean_inv, mm, mv = f(), f(), torch.empty((2, ly.N), device="cuda"), torch.zeros(ly.N, device="cuda"), f()
             mv.fill_(1.0)
-            args = (_p(ly.gamma), _p(ly.beta), C.c_float(OP_DECAY), _p(mm), _p(mv), _p(scale), _p(shift), _p(mean_inv), st)
+            args = (ptr(ly.gamma), ptr(ly.beta), C.c_float(OP_DECAY), ptr(mm), ptr(mv), ptr(scale), ptr(shift), ptr(mean_inv), st)
             if path == "rows":
-                assert lib.psa_bn_finalize_rows(b, ly.N, _p(y), *args) == 0
+                assert lib.psa_bn_finalize_rows(b, ly.N, ptr(y), *args) == 0
             else:
                 stats = torch.stack([y64.sum(0), (y64 * y64).sum(0)]).float()
-                assert lib.psa_bn_finalize(ly.N, b, _p(stats), *args) == 0
-            errs[path] = (_rel(mean_inv[0].cpu(), want[0].cpu()), float(((mean_inv[1].double() - want[1]) / want[1]).abs().max()))
+                assert lib.psa_bn_finalize(ly.N, b, ptr(stats), *args) == 0
+            errs[path] = (rel(mean_inv[0].cpu(), want[0].cpu()), float(((mean_inv[1].double() - want[1]) / want[1]).abs().max()))
             if path == "rows":
-                assert _rel(mm.cpu(), ((1 - OP_DECAY) * mean).cpu()) < 1e-6
-                assert _rel(mv.cpu(), (OP_DECAY + (1 - OP_DECAY) * var).cpu()) < 1e-6
+                assert rel(mm.cpu(), ((1 - OP_DECAY) * mean).cpu()) < 1e-6
+                assert rel(mv.cpu(), (OP_DECAY + (1 - OP_DECAY) * var).cpu()) < 1e-6
                 g64, b64 = ly.gamma.detach().double(), ly.beta.detach().double()
-                assert _rel(scale.cpu(), (g64 * want[1]).cpu()) < 1e-6 and _rel(shift.cpu(), (b64 - mean * g64 * want[1]).cpu()) < 1e-6
+                assert rel(scale.cpu(), (g64 * want[1]).cpu()) < 1e-6 and rel(shift.cpu(), (b64 - mean * g64 * want[1]).cpu()) < 1e-6
         print(f"[dgcnn head B={b} N={n} seed={seed}] {scope}: (mean, 1/sigma) errors by path {errs}")
         assert errs["rows"][0] < 1e-6 and errs["rows"][1] < 1e-6
     print(f"[dgcnn head B={b} N={n} seed={seed}] largest mean^2 / var: {ratio:.0f}")
     assert ratio > 100                                             # the regime that needs the centred variance
 
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())

@@ -17,66 +17,19 @@ from scanobjectnn_b200 import _lib, dgcnn, ops
 from scanobjectnn_b200.tf_util import VariableStore
 from scanobjectnn_b200.training import EdgeConv2Trainer, MlpTrainer, edgeconv_training, mlp_training
 
+from .restate import EC2, ambiguous, edgeconv2_store, edges, flat_grad, layer, params_as, rel
+
 OTOL, GTOL = 1e-5, 1e-4
 MODEL = (32, 2048, 20)
-S1, S2 = "t/tconv1", "t/tconv2"
-
-
-def _rel(got, want):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    return float(np.abs(got - want).max() / max(1e-30, np.abs(want).max()))
-
-
-def _store(c, seed):
-    p = VariableStore(device="cuda", seed=seed)
-    p.add_conv2d(S1, 2 * c, 64, randomize_bn=True)
-    p.add_conv2d(S2, 64, 128, randomize_bn=True)
-    rng = np.random.default_rng(seed)
-    for s, n in ((S1, 64), (S2, 128)):
-        p[f"{s}/biases"] = torch.tensor(rng.standard_normal(n) * 0.1, dtype=torch.float32, device="cuda")
-    return p
-
-
-def _seg(fp, g, name):
-    v = fp.views[name]
-    off = (v.data_ptr() - fp.flat.data_ptr()) // 4
-    return g[off:off + v.numel()].view(v.shape)
-
-
-def _params64(p):
-    out = {}
-    for s in (S1, S2):
-        w = p[f"{s}/weights"]
-        out[s] = [p[f"{s}/weights"].double().reshape(-1, w.shape[-1]).clone().requires_grad_(True)] + \
-                 [p[f"{s}/{v}"].double().clone().requires_grad_(True) for v in ("biases", "bn/gamma", "bn/beta")]
-    return out
+S1, S2 = EC2
 
 
 def _ref64(x, idx, P):
-    """[x_i, x_j - x_i] -> (conv + batch norm over all edges (biased variance, eps 1e-3) + relu) twice -> (max over k, z2, batch stats)"""
-    b, n, c = x.shape
-    k = idx.shape[-1]
-    neigh = x[torch.arange(b, device=x.device).view(b, 1, 1), idx.long()]
-    centre = x.unsqueeze(2).expand(b, n, k, c)
-    h = torch.cat([centre, neigh - centre], dim=-1)
-    stats = []
-    for s in (S1, S2):
-        w, bias, gamma, beta = P[s]
-        y = h @ w + bias
-        mean, var = y.mean((0, 1, 2)), y.var((0, 1, 2), unbiased=False)
-        stats.append((mean, var))
-        h = torch.relu((y - mean) / torch.sqrt(var + 1e-3) * gamma + beta)
+    """[x_i, x_j - x_i] -> (conv + batch norm over all edges (biased variance, eps 1e-3) + relu) twice -> (max over k, z2, batch
+    stats by scope)"""
+    stats = {}
+    h = layer(layer(edges(x, idx), P, S1, False, stats=stats), P, S2, False, stats=stats)
     return h.amax(dim=2), h, stats
-
-
-def _ambiguous(z):
-    """(b, n, C) True where the max over k has a runner-up of a different value within 1e-5 (of the largest activation) of it"""
-    with torch.no_grad():
-        mx = z.amax(dim=2, keepdim=True)
-        below = torch.where(z < mx, z, torch.full_like(z, -1.0)).amax(dim=2)
-        tol = 1e-5 * float(z.abs().max())
-        mx = mx.squeeze(2)
-        return ((mx - below) < tol) | ((mx > 0) & (mx < tol))
 
 
 def _composition(x, idx, bn_decay, params):
@@ -141,7 +94,7 @@ def test_edgeconv2_training_matches_float64(k):
     """outputs, both layers' moving averages and every gradient against torch autograd over the float64 formula; random graphs with
     self-loops, and one cloud made of duplicated points, so exact ties and their even split occur"""
     b, n, c = 3, 300, 3
-    p = _store(c, seed=k)
+    p = edgeconv2_store(c, seed=k)
     rng = np.random.default_rng(k)
     x_np = rng.standard_normal((b, n, c)).astype(np.float32)
     x_np[1, n // 2:] = x_np[1, :n // 2]                                             # cloud 1: every point twice
@@ -150,12 +103,13 @@ def test_edgeconv2_training_matches_float64(k):
     idx_np[1, :, 1 % k] = (np.arange(n) + n // 2) % n                               # ... and the point's duplicate
     x = torch.tensor(x_np, device="cuda", requires_grad=True)
     idx = torch.tensor(idx_np, device="cuda")
-    P = _params64(p)
+    P = params_as(p, torch.float64, grad=True)
+    names = [f"{s}/{v}" for s in (S1, S2) for v in ("weights", "biases", "bn/gamma", "bn/beta")]
     mov0 = {s: (p[f"{s}/bn/moving_mean"].double().clone(), p[f"{s}/bn/moving_variance"].double().clone()) for s in (S1, S2)}
 
     x64 = x.detach().double().requires_grad_(True)
     o64, z64, stats = _ref64(x64, idx, P)
-    amb = _ambiguous(z64)
+    amb = ambiguous(z64, 2)
     R = torch.tensor(rng.standard_normal((b, n, 128)).astype(np.float32), device="cuda")
     R[amb] = 0.0
     print(f"[edgeconv2 k={k}] ambiguous maxima masked: {int(amb.sum())} of {amb.numel()}")
@@ -165,20 +119,19 @@ def test_edgeconv2_training_matches_float64(k):
     assert out.shape == (b, n, 128) and out.grad_fn is not None
     fp = p._flat
     gflat, gx = torch.autograd.grad(out, [fp.flat, x], R)
-    want = torch.autograd.grad(o64, [x64] + P[S1] + P[S2], R.double())
+    want = dict(zip(["x"] + names, torch.autograd.grad(o64, [x64] + [P[v] for v in names], R.double())))
 
-    assert _rel(out.detach().cpu(), o64.detach().cpu()) < OTOL
-    for s, (mean, var) in zip((S1, S2), stats):
+    assert rel(out.detach().cpu(), o64.detach().cpu()) < OTOL
+    for s, (mean, var) in stats.items():
         mm0, mv0 = mov0[s]
-        assert _rel(p[f"{s}/bn/moving_mean"].cpu(), (0.9 * mm0 + 0.1 * mean.detach()).cpu()) < OTOL
-        assert _rel(p[f"{s}/bn/moving_variance"].cpu(), (0.9 * mv0 + 0.1 * var.detach()).cpu()) < OTOL
-    assert _rel(gx.cpu(), want[0].cpu()) < GTOL
-    for s, off in ((S1, 1), (S2, 5)):
-        w = p[f"{s}/weights"]
-        assert _rel(_seg(fp, gflat, f"{s}/weights").reshape(-1, w.shape[-1]).cpu(), want[off].cpu()) < GTOL, s
-        assert _rel(_seg(fp, gflat, f"{s}/bn/gamma").cpu(), want[off + 2].cpu()) < GTOL, s
-        assert _rel(_seg(fp, gflat, f"{s}/bn/beta").cpu(), want[off + 3].cpu()) < GTOL, s
-        assert not bool(_seg(fp, gflat, f"{s}/biases").any()) and not bool(fp.grad_of(f"{s}/biases").any())   # exactly zero under BN
+        assert rel(p[f"{s}/bn/moving_mean"].cpu(), (0.9 * mm0 + 0.1 * mean.detach()).cpu()) < OTOL
+        assert rel(p[f"{s}/bn/moving_variance"].cpu(), (0.9 * mv0 + 0.1 * var.detach()).cpu()) < OTOL
+    assert rel(gx.cpu(), want["x"].cpu()) < GTOL
+    for s in (S1, S2):
+        assert rel(flat_grad(p, f"{s}/weights", gflat).cpu(), want[f"{s}/weights"].cpu()) < GTOL, s
+        assert rel(flat_grad(p, f"{s}/bn/gamma", gflat).cpu(), want[f"{s}/bn/gamma"].cpu()) < GTOL, s
+        assert rel(flat_grad(p, f"{s}/bn/beta", gflat).cpu(), want[f"{s}/bn/beta"].cpu()) < GTOL, s
+        assert not bool(flat_grad(p, f"{s}/biases", gflat).any()) and not bool(fp.grad_of(f"{s}/biases").any())   # exactly zero under BN
     mask = p._trainers[("edgeconv2", (S1, S2), b, n, c, k)].mask
     cnt = np.unpackbits(mask.cpu().numpy().view(np.uint8)).reshape(tuple(mask.shape) + (32,)).sum(-1).astype(np.int64)
     assert cnt.min() >= 1
@@ -194,8 +147,8 @@ def test_edgeconv2_training_matches_the_materialising_composition_at_the_model_s
     x = torch.tensor(rng.standard_normal((b, n, c)).astype(np.float32), device="cuda", requires_grad=True)
     idx = ops.knn_graph(x.detach(), k)
     with torch.no_grad():
-        _, z64, _ = _ref64(x.detach().double(), idx, _params64(_store(c, seed=21)))
-        amb = _ambiguous(z64)
+        _, z64, _ = _ref64(x.detach().double(), idx, params_as(edgeconv2_store(c, seed=21), torch.float64))
+        amb = ambiguous(z64, 2)
         del z64
     torch.cuda.empty_cache()
     R = torch.tensor(rng.standard_normal((b, n, 128)).astype(np.float32), device="cuda")
@@ -204,15 +157,15 @@ def test_edgeconv2_training_matches_the_materialising_composition_at_the_model_s
     assert float(amb.double().mean()) < 0.01
     res = []
     for fn in (lambda p: edgeconv_training(x, idx, (S1, S2), 0.5, p), lambda p: _composition(x, idx, 0.5, p)):
-        p = _store(c, seed=21)
+        p = edgeconv2_store(c, seed=21)
         out = fn(p)
         gflat, gx = torch.autograd.grad(out, [p._flat.flat, x], R)
         fp = p._flat
-        res.append((out.detach(), gx) + tuple(_seg(fp, gflat, f"{s}/{v}").clone() for s in (S1, S2) for v in ("weights", "bn/gamma", "bn/beta")))
+        res.append((out.detach(), gx) + tuple(flat_grad(p, f"{s}/{v}", gflat).clone() for s in (S1, S2) for v in ("weights", "bn/gamma", "bn/beta")))
         del out, gflat, gx, p
         torch.cuda.empty_cache()
     names = ("out", "dx", "dW1", "dgamma1", "dbeta1", "dW2", "dgamma2", "dbeta2")
-    errs = {name: _rel(a.cpu(), bb.cpu()) for name, a, bb in zip(names, res[0], res[1])}
+    errs = {name: rel(a.cpu(), bb.cpu()) for name, a, bb in zip(names, res[0], res[1])}
     print("[edgeconv2 vs composition] max error relative to the largest entry:", {k_: f"{v:.2e}" for k_, v in errs.items()})
     assert errs["out"] < OTOL
     assert max(v for k_, v in errs.items() if k_ != "out") < GTOL
@@ -226,7 +179,7 @@ def test_edgeconv2_training_is_bit_reproducible_and_stores_no_edge_tensor():
     x = torch.tensor(rng.standard_normal((b, n, c)).astype(np.float32), device="cuda", requires_grad=True)
     idx = ops.knn_graph(x.detach(), k)
     R = torch.tensor(rng.standard_normal((b, n, 128)).astype(np.float32), device="cuda")
-    p = _store(c, seed=4)
+    p = edgeconv2_store(c, seed=4)
     gc.collect()                     # earlier tests' trainers must not be freed inside the measured window
     torch.cuda.empty_cache()
     torch.cuda.synchronize()
@@ -241,7 +194,7 @@ def test_edgeconv2_training_is_bit_reproducible_and_stores_no_edge_tensor():
             torch.cuda.synchronize()
             peak = torch.cuda.max_memory_allocated() - base
     del out, gflat, gx
-    q = _store(c, seed=4)
+    q = edgeconv2_store(c, seed=4)
     gc.collect()
     torch.cuda.empty_cache()
     torch.cuda.synchronize()

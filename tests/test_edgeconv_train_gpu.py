@@ -15,44 +15,15 @@ from scanobjectnn_b200 import _lib, ops
 from scanobjectnn_b200.tf_util import VariableStore
 from scanobjectnn_b200.training import EdgeConvTrainer, edgeconv_training, mlp_training
 
+from .restate import edgeconv_store, edges, flat_grad, grid_x, rel
+
 OTOL, GTOL = 1e-5, 1e-4          # outputs / gradients, relative to the largest entry (the bound of test_train_gpu.py)
 MODEL = (32, 2048, 20)           # DGCNN: B, N, k
 
 
-def _rel(got, want):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    return float(np.abs(got - want).max() / max(1e-30, np.abs(want).max()))
-
-
-def _store(c, cout, seed, scope="e"):
-    """one conv2d(2c -> cout) + batch norm with weights, bias, gamma and beta on dyadic grids"""
-    rng = np.random.default_rng(seed)
-    p = VariableStore(device="cuda", seed=seed)
-    p.add_conv2d(scope, 2 * c, cout)
-    p[f"{scope}/weights"] = torch.tensor(rng.integers(-16, 17, (1, 1, 2 * c, cout)) / 64.0, dtype=torch.float32, device="cuda")
-    p[f"{scope}/biases"] = torch.tensor(rng.integers(-8, 9, cout) / 64.0, dtype=torch.float32, device="cuda")
-    p[f"{scope}/bn/gamma"] = torch.tensor(1.0 + rng.integers(-32, 33, cout) / 64.0, dtype=torch.float32, device="cuda")
-    p[f"{scope}/bn/beta"] = torch.tensor(rng.integers(-8, 9, cout) / 64.0, dtype=torch.float32, device="cuda")
-    return p
-
-
-def _grid_x(b, n, c, seed):
-    return np.random.default_rng(seed).integers(-32, 33, (b, n, c)).astype(np.float32) / 16.0
-
-
-def _seg(fp, g, name):
-    v = fp.views[name]
-    off = (v.data_ptr() - fp.flat.data_ptr()) // 4
-    return g[off:off + v.numel()].view(v.shape)
-
-
 def _ref64(x, idx, W, bias, gamma, beta):
     """[x_i, x_j - x_i] . W + b -> batch norm over all edges (biased variance, eps 1e-3) -> relu -> amax over k, in float64"""
-    b, n, c = x.shape
-    k = idx.shape[-1]
-    neigh = x[torch.arange(b, device=x.device).view(b, 1, 1), idx.long()]
-    centre = x.unsqueeze(2).expand(b, n, k, c)
-    y = torch.cat([centre, neigh - centre], dim=-1) @ W + bias
+    y = edges(x, idx) @ W + bias
     mean, var = y.mean((0, 1, 2)), y.var((0, 1, 2), unbiased=False)
     z = torch.relu((y - mean) / torch.sqrt(var + 1e-3) * gamma + beta)
     return z.amax(dim=2), mean, var
@@ -108,8 +79,8 @@ def test_edgeconv_training_matches_float64(c, cout, k):
     """outputs, moving averages and every gradient against torch autograd over the float64 formula; random graphs with self-loops,
     and one cloud made of duplicated points, so tied maxima and their even split occur"""
     b, n = 3, 300
-    p = _store(c, cout, seed=c + cout + k)
-    x_np = _grid_x(b, n, c, seed=k)
+    p = edgeconv_store(c, cout, seed=c + cout + k)
+    x_np = grid_x(b, n, c, seed=k)
     x_np[1, n // 2:] = x_np[1, :n // 2]                                             # cloud 1: every point twice
     rng = np.random.default_rng(7)
     idx_np = rng.integers(0, n, (b, n, k)).astype(np.int32)
@@ -131,14 +102,14 @@ def test_edgeconv_training_matches_float64(c, cout, k):
     x64 = x.detach().double().requires_grad_(True)
     o64, mean, var = _ref64(x64, idx, w64, b64, g64, be64)
     want = torch.autograd.grad(o64, [x64, w64, b64, g64, be64], R.double())
-    assert _rel(out.detach().cpu(), o64.detach().cpu()) < OTOL
-    assert _rel(p[f"{s}/bn/moving_mean"].cpu(), (0.9 * mm0 + 0.1 * mean.detach()).cpu()) < OTOL
-    assert _rel(p[f"{s}/bn/moving_variance"].cpu(), (0.9 * mv0 + 0.1 * var.detach()).cpu()) < OTOL
-    assert _rel(gx.cpu(), want[0].cpu()) < GTOL
-    assert _rel(_seg(fp, gflat, f"{s}/weights").reshape(2 * c, cout).cpu(), want[1].cpu()) < GTOL
-    assert _rel(_seg(fp, gflat, f"{s}/bn/gamma").cpu(), want[3].cpu()) < GTOL
-    assert _rel(_seg(fp, gflat, f"{s}/bn/beta").cpu(), want[4].cpu()) < GTOL
-    assert not bool(_seg(fp, gflat, f"{s}/biases").any()) and not bool(fp.grad_of(f"{s}/biases").any())     # exactly zero under BN
+    assert rel(out.detach().cpu(), o64.detach().cpu()) < OTOL
+    assert rel(p[f"{s}/bn/moving_mean"].cpu(), (0.9 * mm0 + 0.1 * mean.detach()).cpu()) < OTOL
+    assert rel(p[f"{s}/bn/moving_variance"].cpu(), (0.9 * mv0 + 0.1 * var.detach()).cpu()) < OTOL
+    assert rel(gx.cpu(), want[0].cpu()) < GTOL
+    assert rel(flat_grad(p, f"{s}/weights", gflat).reshape(2 * c, cout).cpu(), want[1].cpu()) < GTOL
+    assert rel(flat_grad(p, f"{s}/bn/gamma", gflat).cpu(), want[3].cpu()) < GTOL
+    assert rel(flat_grad(p, f"{s}/bn/beta", gflat).cpu(), want[4].cpu()) < GTOL
+    assert not bool(flat_grad(p, f"{s}/biases", gflat).any()) and not bool(fp.grad_of(f"{s}/biases").any())     # exactly zero under BN
     ties = p._trainers[("edgeconv", s, b, n, c, k)].ties
     assert k == 1 or int(ties.max()) > 1                                           # the even split was exercised
 
@@ -148,19 +119,19 @@ def test_edgeconv_training_matches_the_materialising_composition_at_the_model_sh
     """B=32, N=2048, k=20, 128 -> 64 (dgcnn2..3), on the real kNN graph of the input"""
     b, n, k = MODEL
     c, cout = 64, 64
-    x = torch.tensor(_grid_x(b, n, c, seed=3), device="cuda", requires_grad=True)
+    x = torch.tensor(grid_x(b, n, c, seed=3), device="cuda", requires_grad=True)
     idx = ops.knn_graph(x.detach(), k)
     R = torch.tensor(np.random.default_rng(5).standard_normal((b, n, cout)).astype(np.float32), device="cuda")
     res = []
     for fn in (lambda p: edgeconv_training(x, idx, "dgcnn2", 0.5, p), lambda p: _old_path(x, idx, "dgcnn2", p)):
-        p = _store(c, cout, seed=21, scope="dgcnn2")
+        p = edgeconv_store(c, cout, seed=21, scope="dgcnn2")
         out = fn(p)
         gflat, gx = torch.autograd.grad(out, [p._flat.flat, x], R)
         fp = p._flat
-        res.append((out.detach(), gx, *(_seg(fp, gflat, f"dgcnn2/{v}").clone() for v in ("weights", "bn/gamma", "bn/beta", "biases"))))
+        res.append((out.detach(), gx, *(flat_grad(p, f"dgcnn2/{v}", gflat).clone() for v in ("weights", "bn/gamma", "bn/beta", "biases"))))
         del out, gflat, gx, p
         torch.cuda.empty_cache()
-    errs = {name: _rel(a.cpu(), bb.cpu()) for name, a, bb in zip(("out", "dx", "dW", "dgamma", "dbeta"), res[0], res[1])}
+    errs = {name: rel(a.cpu(), bb.cpu()) for name, a, bb in zip(("out", "dx", "dW", "dgamma", "dbeta"), res[0], res[1])}
     print("[edgeconv vs composition] max error relative to the largest entry:", {k_: f"{v:.2e}" for k_, v in errs.items()})
     assert errs["out"] < OTOL
     assert max(errs["dx"], errs["dW"], errs["dgamma"], errs["dbeta"]) < GTOL

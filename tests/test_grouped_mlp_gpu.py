@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from scanobjectnn_b200 import _lib, ops
-from scanobjectnn_b200._lib import PsaActIn, PsaGradIn, check
+from scanobjectnn_b200._lib import PsaActIn, PsaGradIn, check, ptr
 
 from . import gpu_util as G
 
@@ -70,10 +70,6 @@ def test_shared_mlp_grouped_rejects_bad_groups():
         ops.shared_mlp_grouped(G.cu(rng.standard_normal((10, 64)).astype(np.float32)), mlp, torch.zeros((3, 128), device="cuda"))
 
 
-def _p(t):
-    return C.c_void_p(0 if t is None else t.data_ptr())
-
-
 def _fwd_grouped(x, s_in, t_in, w, bias, ga, group_rows):
     lib = _lib.load()
     rows, k = x.shape
@@ -83,7 +79,7 @@ def _fwd_grouped(x, s_in, t_in, w, bias, ga, group_rows):
     need = lib.psa_train_dense_workspace_bytes(rows, k, n)
     ws = torch.empty(need, dtype=torch.uint8, device="cuda")
     ain = PsaActIn(x=x.data_ptr(), ld=k, scale=s_in.data_ptr(), shift=t_in.data_ptr(), mask=None, relu=1)
-    check(lib.psa_train_dense_fwd_grouped(rows, group_rows, k, n, C.byref(ain), _p(w), _p(bias), _p(ga), _p(y), _p(stats), _p(ws),
+    check(lib.psa_train_dense_fwd_grouped(rows, group_rows, k, n, C.byref(ain), ptr(w), ptr(bias), ptr(ga), ptr(y), ptr(stats), ptr(ws),
                                           C.c_size_t(need), None), "train_dense_fwd_grouped")
     return y, stats
 
@@ -115,7 +111,7 @@ def test_train_dense_fwd_grouped_matches_fp64_and_repeats(b, n):
 def _group_sums(rows, group_rows, c, gin):
     lib = _lib.load()
     out = torch.empty((rows // group_rows, c), device="cuda")
-    check(lib.psa_train_bias_grad_grouped(rows, group_rows, c, C.byref(gin), _p(out), None), "train_bias_grad_grouped")
+    check(lib.psa_train_bias_grad_grouped(rows, group_rows, c, C.byref(gin), ptr(out), None), "train_bias_grad_grouped")
     return out
 
 
@@ -143,5 +139,5 @@ def test_group_gradient_sums_match_fp64_and_repeat(b, n):
     assert (err < bound).all()
     # the whole batch as one group is the bias gradient, bit for bit
     db = torch.empty(c, device="cuda")
-    check(_lib.load().psa_train_bias_grad(rows, c, C.byref(gin), _p(db), None), "train_bias_grad")
+    check(_lib.load().psa_train_bias_grad(rows, c, C.byref(gin), ptr(db), None), "train_bias_grad")
     assert torch.equal(_group_sums(rows, rows, c, gin)[0], db)

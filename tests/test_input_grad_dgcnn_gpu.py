@@ -1,14 +1,8 @@
 """Gradients with respect to the input cloud of DGCNN and vanilla PointNet in inference mode (batch norm frozen on the moving averages:
 the training kernels with psa_edgeconv_frozen_bwd / psa_edgeconv2_frozen_bwd and frozen mlp_training nodes) against float64
 restatements evaluated on the GPU path's own neighbour graphs.  Bounds as in test_input_grad_gpu.py: outputs
-1e-5 of max(1, |largest|), gradients 1e-4 relative to the largest entry.
-
-A max (over k neighbours, or over the N points) whose runner-up lies within 1e-5 of it may be won by another element in fp32 than in
-float64, and then routes its gradient elsewhere; likewise a head activation, or a maximum, whose pre-relu value lies within 1e-5 of
-zero on either side may fall on the other side of the relu (under batch statistics that changes the gradient of its whole column).
-These are properties of the max and the relu, not errors.  The model tests, frozen and training alike, find such elements on the
-float64 side and zero the gradient arriving at them on both sides (a hook on the same tensor of each), as test_edgeconv2_train_gpu.py
-does for the op's output."""
+1e-5 of max(1, |largest|), gradients 1e-4 relative to the largest entry.  Ambiguous maxima and near-zero relu inputs are left out
+on both sides by the exclusion rule of tests/restate.py."""
 import ctypes as C
 
 import numpy as np
@@ -17,28 +11,13 @@ import torch
 
 from scanobjectnn_b200 import _lib, dgcnn, pointnet_cls, training
 from scanobjectnn_b200.synthetic import make_clouds
-from scanobjectnn_b200.tf_util import VariableStore
 
 from . import gpu_util as G
-from .test_edgeconv_train_gpu import _grid_x
-from .test_edgeconv_train_gpu import _store as _store1
+from . import restate
+from .restate import Masks, ambiguous, edgeconv_store, edges, grid_x, layer, moving, out_err, params_as, perturb_tnets, rel
 
 OTOL, GTOL = 1e-5, 1e-4
-S1, S2 = "t/tconv1", "t/tconv2"
-
-
-def _rel(got, want):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    return float(np.abs(got - want).max() / max(1e-30, np.abs(want).max()))
-
-
-def _out_err(got, want):
-    got, want = np.asarray(got, dtype=np.float64), np.asarray(want, dtype=np.float64)
-    return float(np.abs(got - want).max() / max(1.0, np.abs(want).max()))
-
-
-def _moving(p):
-    return {k: v.clone() for k, v in p.items() if k.endswith(("/moving_mean", "/moving_variance"))}
+S1, S2 = restate.EC2
 
 
 def _bit_equal(a: dict, b: dict):
@@ -53,171 +32,10 @@ def _randomize_moving(p, scopes, seed):
         p[f"{s}/bn/moving_variance"] = torch.tensor(rng.uniform(0.5, 2.0, c), dtype=torch.float32, device="cuda")
 
 
-def _ambiguous(z, dim):
-    """True where the max over `dim` has a runner-up of a different value within 1e-5 (of the largest activation) of it, or is a
-    positive maximum within that distance of the relu's zero"""
-    with torch.no_grad():
-        mx = z.amax(dim=dim, keepdim=True)
-        below = torch.where(z < mx, z, torch.full_like(z, -1.0)).amax(dim=dim)
-        tol = 1e-5 * float(z.abs().max())
-        mx = mx.squeeze(dim)
-        return ((mx - below) < tol) | ((mx > 0) & (mx < tol))
-
-
-def _near_zero(z):
-    """True where a pre-relu value lies within 1e-5 (of the largest magnitude) of zero"""
-    with torch.no_grad():
-        return z.abs() < 1e-5 * float(z.abs().max())
-
-
-def _near_zero_max(pre, dim, scale):
-    """True where the max over `dim` of the pre-relu values lies within 1e-5 of `scale` of the relu's zero, on either side: a maximum
-    slightly below zero in float64 may lie slightly above it in fp32, and then carries the whole gradient"""
-    with torch.no_grad():
-        return pre.amax(dim=dim).abs() < 1e-5 * scale
-
-
-def _inner_flip(pre, inner):
-    """True where the edge that wins the max over k (dim 2) of `pre` (b, n, k, c) has a unit of `inner` (b, n, k, c1), the pre-relu
-    values of the layer below, within 1e-5 (of the largest magnitude) of zero"""
-    with torch.no_grad():
-        return _near_zero(inner).any(dim=-1).gather(2, pre.argmax(dim=2))
-
-
-def _zero_at(t, mask):
-    t.register_hook(lambda g: g.masked_fill(mask, 0.0))
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# float64 restatements
-# ---------------------------------------------------------------------------------------------------------------------
-def _p64(p):
-    return {k: v.detach().double() for k, v in p.items()}
-
-
-def _layer(h, P, scope, frozen, bn=True, relu=True, stats=None):
-    """conv2d / fully_connected (+ batch norm + relu): batch norm on the moving averages (frozen) or on the batch statistics over
-    every row (biased variance), eps 1e-3; the batch statistics are recorded in `stats[scope]` when a dict is given"""
-    w = P[f"{scope}/weights"]
-    y = h @ w.reshape(-1, w.shape[-1]) + P[f"{scope}/biases"]
-    if not bn:
-        return y
-    if frozen:
-        mean, var = P[f"{scope}/bn/moving_mean"], P[f"{scope}/bn/moving_variance"]
-    else:
-        dims = tuple(range(y.dim() - 1))
-        mean, var = y.mean(dims), y.var(dims, unbiased=False)
-        if stats is not None:
-            stats[scope] = (mean.detach(), var.detach())
-    z = (y - mean) / torch.sqrt(var + 1e-3) * P[f"{scope}/bn/gamma"] + P[f"{scope}/bn/beta"]
-    return torch.relu(z) if relu else z
-
-
-def _edges(x, idx):
-    b, n, c = x.shape
-    k = idx.shape[-1]
-    neigh = x[torch.arange(b, device=x.device).view(b, 1, 1), idx.long()]
-    centre = x.unsqueeze(2).expand(b, n, k, c)
-    return torch.cat([centre, neigh - centre], dim=-1)
-
-
-class _Masks:
-    """the ambiguous maxima found by a restatement, in the order the model reaches them: `edge` for the EdgeConv outputs (max over k),
-    `pool` for the layers reduced over the N points, keyed by scope; `act` for the head's near-zero relu inputs, keyed by scope"""
-
-    def __init__(self):
-        self.edge, self.pool, self.act = [], {}, {}
-
-    def edge_max(self, z, pre=None, inner=None):
-        """max over k of the activated edge values z; given their pre-relu values `pre`, a maximum within 1e-5 of the relu's zero on
-        either side is ambiguous too, and given a fused first layer's pre-relu values `inner` (b, n, k, c1), so is a maximum whose
-        edge has a unit of that layer within 1e-5 of zero (the kernel's relu may fall the other way there)"""
-        amb = _ambiguous(z, 2)
-        if pre is not None:
-            amb |= _near_zero_max(pre, 2, float(z.detach().abs().max()))
-        if inner is not None:
-            amb |= _inner_flip(pre, inner)
-        out = z.amax(dim=2)
-        _zero_at(out, amb)
-        self.edge.append(amb)
-        return out
-
-    def point_max(self, y, scope, pre=None):
-        amb = _ambiguous(y, 1)
-        if pre is not None:
-            amb |= _near_zero_max(pre, 1, float(y.detach().abs().max()))
-        _zero_at(y, amb.unsqueeze(1))
-        self.pool[scope] = amb
-        return y.amax(dim=1)
-
-    def head_layer(self, h, P, scope, frozen, stats=None):
-        z = _layer(h, P, scope, frozen, relu=False, stats=stats)
-        near = _near_zero(z)
-        out = torch.relu(z)
-        _zero_at(out, near)
-        self.act[scope] = near
-        return out
-
-    def count(self):
-        ms = self.edge + list(self.pool.values()) + list(self.act.values())
-        return sum(int(m.sum()) for m in ms), sum(m.numel() for m in ms)
-
-    def patch(self, monkeypatch):
-        """zero the gradient at the same maxima on the GPU path: hooks on the outputs of its EdgeConv and pooled MLP nodes"""
-        edge, pool, act = iter(self.edge), self.pool, self.act
-        ec, mlp = training.edgeconv_training, training.mlp_training
-
-        def edgeconv_training(*a, **kw):
-            out = ec(*a, **kw)
-            _zero_at(out, next(edge))
-            return out
-
-        def mlp_training(x, layers, *a, **kw):
-            out = mlp(x, layers, *a, **kw)
-            scope = layers[-1][0]
-            if scope in pool:
-                _zero_at(out, pool[scope].unsqueeze(1))
-            if scope in act:
-                _zero_at(out, act[scope])
-            return out
-
-        monkeypatch.setattr(training, "edgeconv_training", edgeconv_training)
-        monkeypatch.setattr(training, "mlp_training", mlp_training)
-
-
-def _dgcnn64(x, P, graphs, frozen, masks: _Masks, detach_transform=False, stats=None):
-    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55) in float64, dropout off, on the given neighbour graphs -> logits;
-    stats (a dict): every layer's batch statistics, by scope"""
-    b, n, _ = x.shape
-    L = lambda h, s, **kw: _layer(h, P, s, frozen, stats=stats, **kw)        # noqa: E731
-    sc = "transform_net1"
-    y1 = L(_edges(x, graphs[0]), f"{sc}/tconv1", relu=False)
-    y = L(torch.relu(y1), f"{sc}/tconv2", relu=False)
-    h = masks.edge_max(torch.relu(y), pre=y, inner=y1)
-    y = L(h, f"{sc}/tconv3", relu=False)
-    h = masks.point_max(torch.relu(y), f"{sc}/tconv3", pre=y)
-    h = L(L(h, f"{sc}/tfc1"), f"{sc}/tfc2")
-    t = (h @ P[f"{sc}/transform_XYZ/weights"] + P[f"{sc}/transform_XYZ/biases"] + torch.eye(3, dtype=x.dtype, device=x.device).flatten())
-    t = t.reshape(b, 3, 3)
-    h = torch.bmm(x, t.detach() if detach_transform else t)
-    nets = []
-    for i, s in enumerate(["dgcnn1", "dgcnn2", "dgcnn3", "dgcnn4"]):
-        y = L(_edges(h, graphs[i + 1]), s, relu=False)
-        h = masks.edge_max(torch.relu(y), pre=y)
-        nets.append(h)
-    y = L(torch.cat(nets, dim=-1), "agg", relu=False)
-    g = masks.point_max(torch.relu(y), "agg", pre=y)
-    for s in ("fc1", "fc2"):
-        g = masks.head_layer(g, P, s, frozen, stats)
-    return L(g, "fc3", bn=False)
-
-
 def _dgcnn_setup(b, n, seed, bga=False, tnet_weights=True):
     p = dgcnn.init_params(seed=seed, randomize_bn=True, bga=bga)
-    if tnet_weights:             # zero in the reference's initialisation: give the T-net a gradient path
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        with torch.no_grad():
-            p["transform_net1/transform_XYZ/weights"].normal_(0, 0.01, generator=g)
+    if tnet_weights:
+        perturb_tnets(p, seed)
     x = G.cu(make_clouds("ball", b, n, seed=seed + 100))
     return p, x
 
@@ -236,12 +54,12 @@ def _dgcnn_against_float64(b, n, seed, monkeypatch, with_detached=False, frozen=
 
     _, ep = run(x0.clone().requires_grad_(True))
     graphs = [ep[f"nn_idx{i}"] for i in range(5)]
-    P = _p64(p)                  # training mode updates only the moving averages, which batch statistics do not read
+    P = params_as(p, torch.float64)                  # training mode updates only the moving averages, which batch statistics do not read
     want = []
     for detach in (False, True) if with_detached else (False,):
-        masks = _Masks()
+        masks = Masks()
         x64 = x0.double().requires_grad_(True)
-        l64 = _dgcnn64(x64, P, graphs, frozen, masks, detach_transform=detach)
+        l64 = restate.dgcnn(x64, P, graphs, frozen, masks, detach_transform=detach)
         (l64 * R.double()).sum().backward()
         want.append((l64.detach(), x64.grad, masks))
     masks = want[0][2]
@@ -311,7 +129,7 @@ def _flat_state(p):
 
 def _check_variables_untouched(p, moving0, flat0, grad0):
     fp = p._flat
-    assert _bit_equal(_moving(p), moving0), "inference mode must not update the moving averages"
+    assert _bit_equal(moving(p), moving0), "inference mode must not update the moving averages"
     assert torch.equal(fp.flat.detach(), flat0) and torch.equal(fp.grad, grad0), "inference mode must leave the flat buckets alone"
     assert fp.flat.grad is None
 
@@ -322,9 +140,9 @@ def test_frozen_edgeconv_matches_float64(c, cout, k):
     """eval-mode batch norm on randomised moving averages; dyadic-grid inputs (every edge value exact in fp32), self-loops and a
     cloud of duplicated points, so tied maxima and their even split occur"""
     b, n, s = 3, 300, "e"
-    p = _store1(c, cout, seed=c + cout + k)
+    p = edgeconv_store(c, cout, seed=c + cout + k)
     _randomize_moving(p, [s], seed=k)
-    x_np = _grid_x(b, n, c, seed=k)
+    x_np = grid_x(b, n, c, seed=k)
     x_np[1, n // 2:] = x_np[1, :n // 2]
     rng = np.random.default_rng(7)
     idx_np = rng.integers(0, n, (b, n, k)).astype(np.int32)
@@ -333,18 +151,18 @@ def test_frozen_edgeconv_matches_float64(c, cout, k):
     x = torch.tensor(x_np, device="cuda", requires_grad=True)
     idx = torch.tensor(idx_np, device="cuda")
     R = torch.tensor(np.random.default_rng(11).standard_normal((b, n, cout)).astype(np.float32), device="cuda")
-    P = _p64(p)
-    moving0 = _moving(p)
+    P = params_as(p, torch.float64)
+    moving0 = moving(p)
 
     out = training.edgeconv_training(x, idx, s, None, p, frozen=True)
     flat0, grad0 = _flat_state(p)
     assert out.shape == (b, n, cout) and out.grad_fn is not None
     (gx,) = torch.autograd.grad(out, [x], R)
     x64 = x.detach().double().requires_grad_(True)
-    o64 = _layer(_edges(x64, idx), P, s, True).amax(dim=2)
+    o64 = layer(edges(x64, idx), P, s, True).amax(dim=2)
     (want,) = torch.autograd.grad(o64, [x64], R.double())
-    assert _out_err(out.detach().cpu(), o64.detach().cpu()) < OTOL
-    assert _rel(gx.cpu(), want.cpu()) < GTOL
+    assert out_err(out.detach().cpu(), o64.detach().cpu()) < OTOL
+    assert rel(gx.cpu(), want.cpu()) < GTOL
     _check_variables_untouched(p, moving0, flat0, grad0)
     ties = p._trainers[("edgeconv_frozen", s, b, n, c, k)].ties
     assert k == 1 or int(ties.max()) > 1                                           # the even split was exercised
@@ -352,12 +170,7 @@ def test_frozen_edgeconv_matches_float64(c, cout, k):
 
 
 def _store2(c, seed):
-    p = VariableStore(device="cuda", seed=seed)
-    p.add_conv2d(S1, 2 * c, 64, randomize_bn=True)
-    p.add_conv2d(S2, 64, 128, randomize_bn=True)
-    rng = np.random.default_rng(seed)
-    for s, n in ((S1, 64), (S2, 128)):
-        p[f"{s}/biases"] = torch.tensor(rng.standard_normal(n) * 0.1, dtype=torch.float32, device="cuda")
+    p = restate.edgeconv2_store(c, seed)
     _randomize_moving(p, (S1, S2), seed + 1)
     return p
 
@@ -375,13 +188,13 @@ def test_frozen_edgeconv2_matches_float64(k):
     idx_np[1, :, 1 % k] = (np.arange(n) + n // 2) % n
     x = torch.tensor(x_np, device="cuda", requires_grad=True)
     idx = torch.tensor(idx_np, device="cuda")
-    P = _p64(p)
-    moving0 = _moving(p)
+    P = params_as(p, torch.float64)
+    moving0 = moving(p)
 
     x64 = x.detach().double().requires_grad_(True)
-    z64 = _layer(_layer(_edges(x64, idx), P, S1, True), P, S2, True)
+    z64 = layer(layer(edges(x64, idx), P, S1, True), P, S2, True)
     o64 = z64.amax(dim=2)
-    amb = _ambiguous(z64, 2)
+    amb = ambiguous(z64, 2)
     R = torch.tensor(rng.standard_normal((b, n, 128)).astype(np.float32), device="cuda")
     R[amb] = 0.0
     print(f"[frozen edgeconv2 k={k}] ambiguous maxima masked: {int(amb.sum())} of {amb.numel()}")
@@ -392,8 +205,8 @@ def test_frozen_edgeconv2_matches_float64(k):
     assert out.shape == (b, n, 128) and out.grad_fn is not None
     (gx,) = torch.autograd.grad(out, [x], R)
     (want,) = torch.autograd.grad(o64, [x64], R.double())
-    assert _out_err(out.detach().cpu(), o64.detach().cpu()) < OTOL
-    assert _rel(gx.cpu(), want.cpu()) < GTOL
+    assert out_err(out.detach().cpu(), o64.detach().cpu()) < OTOL
+    assert rel(gx.cpu(), want.cpu()) < GTOL
     _check_variables_untouched(p, moving0, flat0, grad0)
     mask = p._trainers[("edgeconv2_frozen", (S1, S2), b, n, c, k)].mask
     cnt = np.unpackbits(mask.cpu().numpy().view(np.uint8)).reshape(tuple(mask.shape) + (32,)).sum(-1).astype(np.int64)
@@ -411,10 +224,10 @@ def test_dgcnn_inference_input_grad_matches_float64(monkeypatch):
                                                                                    with_detached=True)
     print(f"[dgcnn frozen B={b} N={n}] ambiguous maxima masked: {masked} of {total}")
     assert masked <= 0.01 * total
-    assert _out_err(logits.cpu(), l64.cpu()) < OTOL
-    assert _rel(gx.cpu(), want.cpu()) < GTOL
-    assert _rel(want_detached.cpu(), want.cpu()) > 10 * GTOL           # the T-net's share is visible ...
-    assert _rel(gx.cpu(), want_detached.cpu()) > 10 * GTOL             # ... and the frozen path carries it
+    assert out_err(logits.cpu(), l64.cpu()) < OTOL
+    assert rel(gx.cpu(), want.cpu()) < GTOL
+    assert rel(want_detached.cpu(), want.cpu()) > 10 * GTOL           # the T-net's share is visible ...
+    assert rel(gx.cpu(), want_detached.cpu()) > 10 * GTOL             # ... and the frozen path carries it
 
 
 @pytest.mark.gpu
@@ -436,7 +249,7 @@ def test_dgcnn_inference_routes_by_requires_grad():
     assert torch.equal(ep["nn_idx0"], ep_f["nn_idx0"])
     assert torch.equal(logits.argmax(-1), fused.argmax(-1))
     on_fused_graphs, _ = dgcnn._get_model_training(x, None, dgcnn.NUM_CLASSES, p, graphs=[ep_f[f"nn_idx{i}"] for i in range(5)], frozen=True)
-    assert _rel(on_fused_graphs.detach().cpu(), fused.cpu()) < 1e-4
+    assert rel(on_fused_graphs.detach().cpu(), fused.cpu()) < 1e-4
     dgcnn.get_loss(logits, torch.zeros(b, dtype=torch.int64, device="cuda")).backward()
     assert bool(torch.isfinite(x.grad).all()) and float(x.grad.abs().max()) > 0
 
@@ -452,7 +265,7 @@ def test_dgcnn_bga_inference_input_grad_reaches_the_cloud():
     torch.nn.functional.cross_entropy(cp, labels).backward()
     assert p._flat.flat.requires_grad and p._flat.flat.grad is not None
     p._flat.flat.grad = None
-    moving0 = _moving(p)
+    moving0 = moving(p)
     grads = []
     for joint in (True, False):
         x = x0.clone().requires_grad_(True)
@@ -463,8 +276,8 @@ def test_dgcnn_bga_inference_input_grad_reaches_the_cloud():
         loss.backward()
         grads.append(x.grad)
     assert bool(torch.isfinite(grads[0]).all()) and float(grads[0].abs().max()) > 0
-    assert _rel(grads[0].cpu(), grads[1].cpu()) > 100 * GTOL, "the segmentation head's gradient did not reach the cloud"
-    assert _bit_equal(_moving(p), moving0)
+    assert rel(grads[0].cpu(), grads[1].cpu()) > 100 * GTOL, "the segmentation head's gradient did not reach the cloud"
+    assert _bit_equal(moving(p), moving0)
     assert p._flat.flat.grad is None
 
 
@@ -479,14 +292,14 @@ def test_dgcnn_training_input_grad(monkeypatch):
         x = x0.clone().requires_grad_(want_grad)
         logits, ep = dgcnn._get_model_training(x, 0.5, dgcnn.NUM_CLASSES, p, dropout=False)
         dgcnn.get_loss(logits, torch.arange(b, device="cuda") % dgcnn.NUM_CLASSES).backward()
-        runs.append((logits.detach(), p._flat.flat.grad.clone(), _moving(p), x.grad))
+        runs.append((logits.detach(), p._flat.flat.grad.clone(), moving(p), x.grad))
     assert torch.equal(runs[0][0], runs[1][0]) and torch.equal(runs[0][1], runs[1][1]) and _bit_equal(runs[0][2], runs[1][2])
     assert bool(torch.isfinite(runs[0][3]).all()) and float(runs[0][3].abs().max()) > 0 and runs[1][3] is None
     gx, want, _, _, _, masked, total = _dgcnn_against_float64(b, n, seed=7, monkeypatch=monkeypatch, frozen=False)
     print(f"[dgcnn training B={b} N={n}] masked: {masked} of {total}; x.grad error relative to the largest entry: "
-          f"{_rel(gx.cpu(), want.cpu()):.2e}")
+          f"{rel(gx.cpu(), want.cpu()):.2e}")
     assert masked <= 0.01 * total
-    assert _rel(gx.cpu(), want.cpu()) < GTOL
+    assert rel(gx.cpu(), want.cpu()) < GTOL
 
 
 @pytest.mark.gpu
@@ -507,44 +320,20 @@ def test_dgcnn_inference_input_grad_at_the_model_shape(monkeypatch):
     b, n = 32, 2048
     gx, want, _, logits, l64, masked, total = _dgcnn_against_float64(b, n, seed=11, monkeypatch=monkeypatch)
     print(f"[dgcnn frozen B={b} N={n}] ambiguous maxima masked: {masked} of {total}; "
-          f"x.grad error relative to the largest entry: {_rel(gx.cpu(), want.cpu()):.2e}")
+          f"x.grad error relative to the largest entry: {rel(gx.cpu(), want.cpu()):.2e}")
     assert masked <= 0.01 * total
-    assert _out_err(logits.cpu(), l64.cpu()) < OTOL
-    assert _rel(gx.cpu(), want.cpu()) < GTOL
+    assert out_err(logits.cpu(), l64.cpu()) < OTOL
+    assert rel(gx.cpu(), want.cpu()) < GTOL
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # 8. vanilla PointNet
 # ---------------------------------------------------------------------------------------------------------------------
-def _pointnet64(x, P, masks: _Masks):
-    """pointnet_cls.get_model (pointnet_cls.py:21-75) in float64 with frozen batch norm -> (logits, feature transform)"""
-    b = x.shape[0]
-    L = lambda h, s, **kw: _layer(h, P, s, True, **kw)        # noqa: E731
-
-    def tnet(h, scope, K):
-        g = masks.point_max(L(L(L(h, f"{scope}/tconv1"), f"{scope}/tconv2"), f"{scope}/tconv3"), f"{scope}/tconv3")
-        g = L(L(g, f"{scope}/tfc1"), f"{scope}/tfc2")
-        name = "transform_XYZ" if K == 3 else "transform_feat"
-        eye = torch.eye(K, dtype=x.dtype, device=x.device).flatten()
-        return (g @ P[f"{scope}/{name}/weights"] + P[f"{scope}/{name}/biases"] + eye).reshape(b, K, K)
-
-    h = torch.bmm(x, tnet(x, "transform_net1", 3))
-    h = L(L(h, "conv1"), "conv2")
-    t2 = tnet(h, "transform_net2", 64)
-    h = torch.bmm(h, t2)
-    g = masks.point_max(L(L(L(h, "conv3"), "conv4"), "conv5"), "conv5")
-    for s in ("fc1", "fc2"):
-        g = masks.head_layer(g, P, s, True)
-    return L(g, "fc3", bn=False), t2
-
-
 @pytest.mark.gpu
 def test_pointnet_inference_input_grad(monkeypatch):
     b, n = 8, 1024
     p = pointnet_cls.init_params(seed=2, randomize_bn=True)
-    with torch.no_grad():
-        for s, name in (("transform_net1", "transform_XYZ"), ("transform_net2", "transform_feat")):
-            p[f"{s}/{name}/weights"].normal_(0, 0.01, generator=torch.Generator(device="cuda").manual_seed(2))
+    perturb_tnets(p, 2)
     x0 = G.cu(make_clouds("ball", b, n, seed=12))
     labels = torch.tensor([3, 1, 4, 1, 5, 9, 2, 6], device="cuda")
     # routing: no gradient asked for -> the fused path, no trainer
@@ -562,11 +351,11 @@ def test_pointnet_inference_input_grad(monkeypatch):
     p.invalidate()                                           # the step updated the moving averages in place
     with torch.no_grad():
         fused, _ = pointnet_cls.get_model(x0, False, params=p)
-    moving0 = _moving(p)
+    moving0 = moving(p)
     # float64 restatement, then the frozen path with the same maxima masked
-    masks = _Masks()
+    masks = Masks()
     x64 = x0.double().requires_grad_(True)
-    l64, t64 = _pointnet64(x64, _p64(p), masks)
+    l64, t64 = restate.pointnet(x64, params_as(p, torch.float64), masks)
     f = torch.nn.functional
     reg = lambda t: 0.001 * 0.5 * ((torch.bmm(t, t.transpose(1, 2)) - torch.eye(64, dtype=t.dtype, device=t.device)) ** 2).sum()  # noqa: E731
     (f.cross_entropy(l64, labels) + reg(t64)).backward()
@@ -579,8 +368,8 @@ def test_pointnet_inference_input_grad(monkeypatch):
         logits, ep = pointnet_cls.get_model(x, False, params=p)
         assert logits.grad_fn is not None and ep["transform"].grad_fn is not None and set(ep) == set(ep_f)
         pointnet_cls.get_loss(logits, labels, ep).backward()
-    assert _out_err(logits.detach().cpu(), l64.detach().cpu()) < OTOL
-    assert _rel(logits.detach().cpu(), fused.cpu()) < 1e-4 and torch.equal(logits.argmax(-1), fused.argmax(-1))
-    assert _rel(x.grad.cpu(), x64.grad.cpu()) < GTOL
-    assert _bit_equal(_moving(p), moving0)
+    assert out_err(logits.detach().cpu(), l64.detach().cpu()) < OTOL
+    assert rel(logits.detach().cpu(), fused.cpu()) < 1e-4 and torch.equal(logits.argmax(-1), fused.argmax(-1))
+    assert rel(x.grad.cpu(), x64.grad.cpu()) < GTOL
+    assert _bit_equal(moving(p), moving0)
     assert p._flat.flat.grad is None

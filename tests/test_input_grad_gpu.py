@@ -10,27 +10,18 @@ import torch
 from oracle import oracle as orc
 from oracle import train_oracle as T
 from scanobjectnn_b200 import _lib, ops, pointnet2_cls_bga, pointnet2_cls_ssg
+from scanobjectnn_b200._lib import ptr, stream
 from scanobjectnn_b200.pointnet_util import add_sa_module_params, pointnet_sa_module
 from scanobjectnn_b200.synthetic import make_clouds
 from scanobjectnn_b200.tf_util import VariableStore
 from scanobjectnn_b200.training import LevelSpec, _plain_grad
 
 from . import gpu_util as G
+from . import restate
+from .restate import moving, rel
 
 pytestmark = pytest.mark.gpu
 GTOL = 1e-4
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _vp(t):
-    return C.c_void_p(0 if t is None else t.data_ptr())
-
-
-def _rel(got, want):
-    return float(np.abs(got - want).max() / max(1e-30, np.abs(want).max()))
 
 
 def _gather_grad(dnew, fps_idx, n):
@@ -65,14 +56,14 @@ def test_conv1_bwd_xyz_kernel_against_numpy(c1, far):
     dxyz, dnew = torch.empty((b, n, 3), device="cuda"), torch.empty((b, m, 3), device="cuda")
     need = lib.psa_sa_conv1_bwd_xyz_workspace_bytes(b, n, m, k)
     ws = torch.empty(need // 4 + 16, device="cuda")
-    args = (b, n, m, k, c1, _vp(Wd), _vp(idx_d), C.byref(g))
-    assert lib.psa_sa_conv1_bwd_xyz(*args, _vp(dxyz), _vp(dnew), _vp(ws), C.c_size_t(need), _st()) == 0
+    args = (b, n, m, k, c1, ptr(Wd), ptr(idx_d), C.byref(g))
+    assert lib.psa_sa_conv1_bwd_xyz(*args, ptr(dxyz), ptr(dnew), ptr(ws), C.c_size_t(need), stream()) == 0
     v = dy0.astype(np.float64) @ W.astype(np.float64).T             # (b, m, k, 3)
     want_dxyz = T.group_bwd(v, idx.astype(np.int64), n)
-    assert _rel(G.npy(dxyz), want_dxyz) < 1e-5
-    assert _rel(G.npy(dnew), -v.sum(axis=2)) < 1e-5
+    assert rel(G.npy(dxyz), want_dxyz) < 1e-5
+    assert rel(G.npy(dnew), -v.sum(axis=2)) < 1e-5
     dxyz2, dnew2 = torch.empty_like(dxyz), torch.empty_like(dnew)
-    assert lib.psa_sa_conv1_bwd_xyz(*args, _vp(dxyz2), _vp(dnew2), _vp(ws), C.c_size_t(need), _st()) == 0
+    assert lib.psa_sa_conv1_bwd_xyz(*args, ptr(dxyz2), ptr(dnew2), ptr(ws), C.c_size_t(need), stream()) == 0
     assert torch.equal(dxyz, dxyz2) and torch.equal(dnew, dnew2), "coordinate gradient must be bit-reproducible"
 
 
@@ -123,11 +114,11 @@ def test_one_level_training_xyz_grad(c, group_all, cloud, radius, k):
     (out * G.cu(R)).sum().backward()
     fps_idx = None if group_all else G.npy(ops.farthest_point_sample(m, xt.detach())).astype(np.int64)
     pooled, cache, _ = _oracle_level(xyz, pts, fps_idx, G.npy(idx).astype(np.int64), _level_layers(p, "lv", mlp), group_all)
-    assert _rel(G.npy(out), pooled) < 1e-5
+    assert rel(G.npy(out), pooled) < 1e-5
     dxyz, dpts, _ = T.sa_level_train_bwd(R.astype(np.float64), cache)
-    assert _rel(G.npy(xt.grad), dxyz[:, :N]) < GTOL
+    assert rel(G.npy(xt.grad), dxyz[:, :N]) < GTOL
     if c:
-        assert _rel(G.npy(pt.grad), dpts[:, :N]) < GTOL
+        assert rel(G.npy(pt.grad), dpts[:, :N]) < GTOL
 
 
 def test_two_levels_chain_through_gather_point():
@@ -149,91 +140,18 @@ def test_two_levels_chain_through_gather_point():
     pooled1, c1, _ = T.sa_level_train_fwd(xyz.astype(np.float64), None, f1, G.npy(idx1).astype(np.int64), _level_layers(p, "l1", mlp1))
     new1 = xyz.astype(np.float64)[np.arange(B)[:, None], f1]
     pooled2, c2, _ = T.sa_level_train_fwd(new1, pooled1, f2, G.npy(idx2).astype(np.int64), _level_layers(p, "l2", mlp2))
-    assert _rel(G.npy(l2_pts), pooled2) < 1e-5
+    assert rel(G.npy(l2_pts), pooled2) < 1e-5
     d_new1, dpts1, _ = T.sa_level_train_bwd(R2.astype(np.float64), c2)
     dxyz1, _, _ = T.sa_level_train_bwd(R1.astype(np.float64) + dpts1, c1)
     want = dxyz1 + _gather_grad(d_new1, f1, N)
-    assert _rel(G.npy(xt.grad), want) < GTOL
+    assert rel(G.npy(xt.grad), want) < GTOL
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# whole models: a float64 torch restatement on the trainer's own indices
+# whole models: restate.ssg on the trainer's own indices
 # ---------------------------------------------------------------------------------------------------------------------
 SMALL_LEVELS = [LevelSpec("layer1", 64, 0.3, 16, [64, 64, 128]), LevelSpec("layer2", 16, 0.6, 16, [128, 128, 256]),
                 LevelSpec("layer3", None, None, None, [256, 512, 1024], group_all=True)]
-HEAD = [("fc1", True), ("fc2", True), ("fc3", False)]
-
-
-def _bn64(y, p, scope, frozen, stats=None):
-    """batch norm in y's dtype; in training mode the batch statistics (mean, biased variance) are also left in `stats[scope]`"""
-    g, be = p[f"{scope}/bn/gamma"].to(y.dtype), p[f"{scope}/bn/beta"].to(y.dtype)
-    if frozen:
-        mean, var = p[f"{scope}/bn/moving_mean"].to(y.dtype), p[f"{scope}/bn/moving_variance"].to(y.dtype)
-    else:
-        red = tuple(range(y.dim() - 1))
-        mean = y.mean(dim=red)
-        var = ((y - mean) ** 2).mean(dim=red)
-        if stats is not None:
-            stats[scope] = (mean.detach(), var.detach())
-    return (y - mean) / torch.sqrt(var + 1e-3) * g + be
-
-
-def _gated_relu(z, ly, info):
-    """relu(z) with the run's decision: the gate of trainer layer `ly`, fmaf(y, scale, shift) > 0 (its sign is exact in float64);
-    the elements where z's own sign decides otherwise are counted as flips"""
-    with torch.no_grad():
-        gate = ((ly.y.double() * ly.scale.double() + ly.shift.double()) > 0).view(z.shape)
-        info["flips"] += int(((z > 0) != gate).sum())
-        info["units"] += gate.numel()
-    return z * gate
-
-
-def _argk_pool(h, lv, info):
-    """the max over dim 2 taken at the run's winner lv.argk (its first winning row), so the gradient goes where the kernel sends it;
-    info["pool_gap"]: how far below h's own maximum that row lies, relative to h's largest entry"""
-    B, m, _, c = h.shape
-    out = h.gather(2, lv.argk.long().view(B, m, 1, c)).squeeze(2)
-    with torch.no_grad():
-        gap = float((h.amax(dim=2) - out).max()) / max(float(h.abs().max()), 1e-30)
-        info["pool_gap"] = max(info["pool_gap"], gap)
-    return out
-
-
-def _ssg64(xyz, p, levels, frozen, masks, run=None, info=None):
-    """pointnet2_cls_ssg (or bga's classification branch) restated in torch ops of xyz's dtype on the trainers' FPS / ball-query
-    indices.  run: the PointNet2ClsTrainer whose discrete decisions are taken instead of the restatement's own -- every batch-normed
-    layer's relu gate (_gated_relu) and every level's max-pool winner (_argk_pool); `info` then collects the batch statistics
-    ("stats"), the flipped gates ("flips" of "units") and the largest pool gap ("pool_gap")."""
-    B, dt = xyz.shape[0], xyz.dtype
-    ar = torch.arange(B, device=xyz.device)
-    stats = None if info is None else info.setdefault("stats", {})
-    cur_xyz, cur_pts = xyz, None
-    for lv in levels:
-        sp = lv.spec
-        if sp.group_all:
-            h = (cur_xyz if cur_pts is None else torch.cat([cur_xyz, cur_pts], -1))[:, None]
-            new_xyz = torch.zeros((B, 1, 3), dtype=dt, device=xyz.device)
-        else:
-            new_xyz = cur_xyz[ar[:, None], lv.fps_idx.long()]
-            idx = lv.idx.long()
-            h = cur_xyz[ar[:, None, None], idx] - new_xyz[:, :, None, :]
-            if cur_pts is not None:
-                h = torch.cat([h, cur_pts[ar[:, None, None], idx]], -1)
-        for i in range(len(sp.mlp)):
-            s = f"{sp.scope}/conv{i}"
-            w = p[f"{s}/weights"].to(dt)
-            z = _bn64(h @ w.reshape(-1, w.shape[-1]) + p[f"{s}/biases"].to(dt), p, s, frozen, stats)
-            h = torch.relu(z) if run is None else _gated_relu(z, lv.layers[i], info)
-        cur_xyz, cur_pts = new_xyz, h.amax(dim=2) if run is None else _argk_pool(h, lv, info)
-    h = cur_pts.reshape(B, -1)
-    for j, (scope, bn) in enumerate(HEAD):
-        h = h @ p[f"{scope}/weights"].to(dt) + p[f"{scope}/biases"].to(dt)
-        if bn:
-            z = _bn64(h, p, scope, frozen, stats)
-            h = torch.relu(z) if run is None else _gated_relu(z, run.head[j], info)
-        if scope in masks:
-            h = h * masks[scope].to(dt)
-    return h
 
 
 def _trainer(p, frozen):
@@ -259,7 +177,7 @@ def test_ssg_training_mode_xyz_grad_and_unchanged_results():
     labels = G.cu(np.random.default_rng(0).integers(0, 15, B).astype(np.int64))
     _get_model_small(xyz, True, p)                                   # builds the trainer
     tr = _trainer(p, False)
-    mov = {k: v.clone() for k, v in p.items() if "moving" in k}
+    mov = moving(p)
     runs = []
     for want in (False, True):
         with torch.no_grad():
@@ -278,10 +196,10 @@ def test_ssg_training_mode_xyz_grad_and_unchanged_results():
     masks = {ly.scope: ly.mask for ly in tr.head if ly.mask is not None}
     x64 = x.detach().double().requires_grad_(True)
     # the moving averages moved during the run: the restatement uses batch statistics, so they do not enter
-    lg64 = _ssg64(x64, p, tr.levels, False, masks)
-    assert _rel(G.npy(l1), lg64.detach().cpu().numpy()) < 1e-4
+    lg64 = restate.ssg(x64, p, tr.levels, False, masks)
+    assert rel(G.npy(l1), lg64.detach().cpu().numpy()) < 1e-4
     torch.nn.functional.cross_entropy(lg64, labels).backward()
-    assert _rel(G.npy(x.grad), x64.grad.cpu().numpy()) < GTOL
+    assert rel(G.npy(x.grad), x64.grad.cpu().numpy()) < GTOL
 
 
 def test_ssg_inference_mode_xyz_grad():
@@ -289,7 +207,7 @@ def test_ssg_inference_mode_xyz_grad():
     p = _small_ssg_params(4)
     xyz = G.cu(make_clouds("ball", B, N, seed=12))
     labels = G.cu(np.random.default_rng(1).integers(0, 15, B).astype(np.int64))
-    mov = {k: v.clone() for k, v in p.items() if "moving" in k}
+    mov = moving(p)
     x = xyz.clone().requires_grad_(True)
     logits, _ = _get_model_small(x, False, p)
     tr = _trainer(p, True)
@@ -298,10 +216,10 @@ def test_ssg_inference_mode_xyz_grad():
     assert all(torch.equal(mov[k], p[k]) for k in mov), "inference mode must not move the moving averages"
     assert torch.equal(bucket, tr.fp.grad) and tr.fp.flat.grad is None, "inference mode leaves the gradient bucket alone"
     x64 = xyz.double().requires_grad_(True)
-    lg64 = _ssg64(x64, p, tr.levels, True, {})
+    lg64 = restate.ssg(x64, p, tr.levels, True, {})
     assert np.abs(G.npy(logits) - lg64.detach().cpu().numpy()).max() < 1e-5 * max(1.0, float(lg64.detach().abs().max()))
     torch.nn.functional.cross_entropy(lg64, labels).backward()
-    assert _rel(G.npy(x.grad), x64.grad.cpu().numpy()) < GTOL
+    assert rel(G.npy(x.grad), x64.grad.cpu().numpy()) < GTOL
 
 
 def test_ssg_get_model_inference_routes_on_requires_grad():
@@ -319,7 +237,7 @@ def test_ssg_get_model_inference_routes_on_requires_grad():
     logits, ep = pointnet2_cls_ssg.get_model(x, False, params=p)
     assert logits.requires_grad and ep["l1_indices"].shape == (B, 512, 32)
     assert torch.equal(logits.argmax(1), fused.argmax(1))
-    assert _rel(G.npy(logits), G.npy(fused)) < 1e-4
+    assert rel(G.npy(logits), G.npy(fused)) < 1e-4
     logits[:, 0].sum().backward()
     assert x.grad is not None and torch.isfinite(x.grad).all() and float(x.grad.abs().max()) > 0
 
@@ -352,7 +270,7 @@ def test_bga_both_heads_reach_xyz(is_training):
     xyz = G.cu(make_clouds("ball", B, N, seed=8))
     labels = G.cu(np.array([1, 4, 7, 11], dtype=np.int64))
     mask = G.cu((np.random.default_rng(0).random((B, N)) > 0.5).astype(np.int64))
-    mov = {k: v.clone() for k, v in p.items() if "moving" in k}
+    mov = moving(p)
     x = xyz.clone().requires_grad_(True)
     cp, sp = pointnet2_cls_bga.get_model(x, is_training, bn_decay=0.5, params=p)
     assert cp.requires_grad and sp.requires_grad
@@ -371,7 +289,7 @@ def test_bga_both_heads_reach_xyz(is_training):
     levels = [trainers[k].levels[0] for k in sorted(k for k in trainers if k[0] == "level_frozen")]
     assert [lv.spec.scope for lv in levels] == ["layer1", "layer2", "layer3"]
     x64 = xyz.double().requires_grad_(True)
-    lg64 = _ssg64(x64, p, levels, True, {})
+    lg64 = restate.ssg(x64, p, levels, True, {})
     assert np.abs(G.npy(cp2) - lg64.detach().cpu().numpy()).max() < 1e-5 * max(1.0, float(lg64.detach().abs().max()))
     torch.nn.functional.cross_entropy(lg64, labels).backward()
-    assert _rel(G.npy(x2.grad), x64.grad.cpu().numpy()) < GTOL
+    assert rel(G.npy(x2.grad), x64.grad.cpu().numpy()) < GTOL

@@ -332,7 +332,7 @@ def test_knn_graph_tensor_core_path_is_index_exact(kind, n, c, k):
         return
     assert np.array_equal(got, orc.dgcnn_knn(x, k))
     fp32 = torch.empty((2, n, k), dtype=torch.int32, device="cuda")     # the public fp32 entry point, called directly
-    assert _lib.load().psa_knn_graph(2, n, c, k, G._p(xt), G._p(fp32), None) == 0
+    assert _lib.load().psa_knn_graph(2, n, c, k, _lib.ptr(xt), _lib.ptr(fp32), None) == 0
     assert np.array_equal(got, G.npy(fp32))
 
 

@@ -3,7 +3,7 @@ restatement, variable by variable, over several consecutive steps; and the loss 
 
 1. The step.  train_step's order -- draw_dropout, forward (batch statistics), loss_and_grad, backward with the coordinate gradient,
    adam -- four times in a row, so every step after the first starts from moved weights, moving averages and non-zero Adam moments.
-   After each backward, test_input_grad_gpu's _ssg64 restates the model in float64 on the trainer's own FPS and ball-query indices
+   After each backward, restate.ssg restates the model in float64 on the trainer's own FPS and ball-query indices
    (which must equal the CPU oracle's), and takes the run's discrete decisions: each batch-normed layer's relu gate
    fmaf(y, scale, shift) > 0, each level's max-pool winner argk (its first winning row: a tie, or a ball-query padding row that
    duplicates a real row, gives the same gradients whichever copy it routes to) and the head's dropout masks.  Batch statistics are
@@ -28,10 +28,12 @@ import torch.nn.functional as F
 
 from oracle import oracle as orc
 from scanobjectnn_b200 import _lib, pointnet2_cls_ssg
+from scanobjectnn_b200._lib import ptr, stream
 from scanobjectnn_b200.synthetic import make_clouds
 from scanobjectnn_b200.training import PointNet2ClsTrainer
 
-from .test_input_grad_gpu import _ssg64
+from . import restate
+from .restate import err, params_as, within
 
 pytestmark = pytest.mark.gpu
 
@@ -43,25 +45,6 @@ SUB32 = 2.0 ** -149                 # the spacing of fp32's subnormals
 # The beta of the group-all level's last layer: a shift of it shifts every cloud's pooled feature alike, which fc1's batch norm
 # removes, so its exact gradient is zero wherever the maxima are positive.  Its error is taken relative to the layer's dgamma.
 POOLED_BETAS = ("layer3/conv2/bn/beta",)
-
-
-def _st():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _vp(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _err(got, want, scale=None):
-    want = want.detach().double()
-    scale = float(want.abs().max()) if scale is None else scale
-    return float((got.detach().double() - want).abs().max()) / max(scale, 1e-30)
-
-
-def _within(e, e32, tol):
-    """the bound, or where the float32 restatement itself misses it, 2x the float32 restatement's error"""
-    return e < tol or e <= 2 * e32
 
 
 def _lr_t(lr, step):
@@ -102,15 +85,14 @@ def _check_indices(tr):
 
 
 def _restate(tr, p, xyz, labels, dtype):
-    """_ssg64 on the run's decisions in `dtype`, mean cross-entropy differentiated -> (logits, x.grad, {variable: grad}, info)"""
-    names = set(tr.fp.names)
-    P = {k: v.detach().to(dtype, copy=True).requires_grad_(not tr.frozen and k in names) for k, v in p.items()}
+    """restate.ssg on the run's decisions in `dtype`, mean cross-entropy differentiated -> (logits, x.grad, {variable: grad}, info)"""
+    P = params_as(p, dtype, grad=not tr.frozen)
     x = xyz.detach().to(dtype, copy=True).requires_grad_(True)
     masks = {ly.scope: ly.mask for ly in tr.head if ly.mask is not None}
     info = {"flips": 0, "units": 0, "pool_gap": 0.0}
-    logits = _ssg64(x, P, tr.levels, tr.frozen, masks, run=tr, info=info)
+    logits = restate.ssg(x, P, tr.levels, tr.frozen, masks, run=tr, info=info)
     F.cross_entropy(logits, labels.long()).backward()
-    grads = {} if tr.frozen else {k: P[k].grad for k in names}
+    grads = {} if tr.frozen else {k: P[k].grad for k in tr.fp.names}
     return logits.detach(), x.grad, grads, info
 
 
@@ -119,13 +101,13 @@ def _step_errors(tr, p, xyz, labels, logits, moving_before):
     backward has run (with the coordinate gradient)"""
     l64, gx64, g64, info = _restate(tr, p, xyz, labels, torch.float64)
     l32, gx32, g32, info32 = _restate(tr, p, xyz, labels, torch.float32)
-    errs = {"logits": (_err(logits, l64), _err(l32, l64), OTOL), "x.grad": (_err(tr.input_xyz_grad(), gx64), _err(gx32, gx64), GTOL)}
+    errs = {"logits": (err(logits, l64), err(l32, l64), OTOL), "x.grad": (err(tr.input_xyz_grad(), gx64), err(gx32, gx64), GTOL)}
     # the loss kernel on the run's own logits
     gl = logits.detach().double()
     loss64 = float(F.cross_entropy(gl, labels.long()))
     dl64 = (torch.softmax(gl, 1) - F.one_hot(labels.long(), NUM_CLASS).double()) / tr.B
     errs["loss"] = (abs(float(tr.loss) - loss64) / max(1.0, loss64), 0.0, 1e-6)
-    errs["dlogits"] = (_err(tr.dlogits, dl64, 1.0 / tr.B), 0.0, 1e-6)
+    errs["dlogits"] = (err(tr.dlogits, dl64, 1.0 / tr.B), 0.0, 1e-6)
     if tr.frozen:
         return errs, info
     stats, stats32 = info["stats"], info32["stats"]
@@ -138,13 +120,13 @@ def _step_errors(tr, p, xyz, labels, logits, moving_before):
         scale = float(g64[name].abs().max())
         if name in POOLED_BETAS:
             scale = max(scale, float(g64[name.replace("/beta", "/gamma")].abs().max()))
-        errs[name] = (_err(got, g64[name], scale), _err(g32[name], g64[name], scale), GTOL)
+        errs[name] = (err(got, g64[name], scale), err(g32[name], g64[name], scale), GTOL)
     for scope in stats:
         for i, suffix in enumerate(("moving_mean", "moving_variance")):
             name = f"{scope}/bn/{suffix}"
             want = DECAY * moving_before[name] + (1 - DECAY) * stats[scope][i]
             yard = DECAY * moving_before[name] + (1 - DECAY) * stats32[scope][i].double()
-            errs[name] = (_err(p[name], want), _err(yard, want), OTOL)
+            errs[name] = (err(p[name], want), err(yard, want), OTOL)
     return errs, info
 
 
@@ -167,7 +149,7 @@ def _report(tag, errs, info, seconds):
 def _check_step(tag, errs, info):
     assert info["flips"] <= 1e-4 * info["units"], (tag, info["flips"], info["units"])
     assert info["pool_gap"] <= 1e-5, (tag, info["pool_gap"])
-    over = {k: f"{e:.2e} ({e32:.2e}) > {tol:.0e}" for k, (e, e32, tol) in errs.items() if not _within(e, e32, tol)}
+    over = {k: f"{e:.2e} ({e32:.2e}) > {tol:.0e}" for k, (e, e32, tol) in errs.items() if not within(e, e32, tol, 2)}
     assert not over, (tag, over)
 
 
@@ -219,7 +201,7 @@ def test_inference_mode_logits_and_xyz_grad_match_float64():
     tr = PointNet2ClsTrainer(p, b, n, NUM_CLASS, frozen=True)
     labels = torch.from_numpy(np.random.default_rng(0).integers(0, NUM_CLASS, b).astype(np.int32)).cuda()
     xyz = torch.from_numpy(make_clouds("ball", b, n, seed=2001)).cuda()
-    moving = {k: v.clone() for k, v in p.items() if "/moving_" in k}
+    moving = restate.moving(p)
     torch.cuda.reset_peak_memory_stats()
     t0 = time.perf_counter()
     logits = tr.forward(xyz)
@@ -240,7 +222,7 @@ def _softmax_xent(logits, labels):
     b, c = logits.shape
     loss = torch.full((1,), float("nan"), device="cuda")
     dl = torch.full((b, c), float("nan"), device="cuda")
-    _lib.check(_lib.load().psa_softmax_xent(b, c, _vp(logits), _vp(labels), _vp(loss), _vp(dl), _st()), "softmax_xent")
+    _lib.check(_lib.load().psa_softmax_xent(b, c, ptr(logits), ptr(labels), ptr(loss), ptr(dl), stream()), "softmax_xent")
     torch.cuda.synchronize()
     return loss, dl
 
@@ -310,8 +292,8 @@ def test_adam_step_matches_float64(count, step, gscale):
     outs = []
     for _ in range(2):
         p1, m1, v1 = p.clone(), m.clone(), v.clone()
-        _lib.check(lib.psa_adam_step(count, _vp(p1), _vp(g), _vp(m1), _vp(v1), C.c_float(LR), C.c_float(B1), C.c_float(B2), C.c_float(EPS),
-                                     step, C.c_float(gscale), _st()), "adam_step")
+        _lib.check(lib.psa_adam_step(count, ptr(p1), ptr(g), ptr(m1), ptr(v1), C.c_float(LR), C.c_float(B1), C.c_float(B2), C.c_float(EPS),
+                                     step, C.c_float(gscale), stream()), "adam_step")
         outs.append((p1, m1, v1))
     torch.cuda.synchronize()
     (p1, m1, v1), (p2, m2, v2) = outs
