@@ -538,9 +538,10 @@ PSA_API int psa_edgeconv2_frozen_bwd(int b, int n, int c, int k, int C1, int C2,
  * delta (b,n,k,3) = group_point(xyz, nn_idx) - xyz; nn_idx (b,n,k) int32 in [0, n); feat (b,n,c); feat_scale,
  * feat_shift (b,c) or NULL; taylor (20,T); W (k, c*T, c_out) = the [1,k] conv's kernel; bias (c_out) -> y (b,n,c_out),
  * pre-group-norm.  The conv runs as one GEMM over the b*n points whose operand is gathered and scaled while it is
- * staged (tensor cores for c % 32 == 0, k*c*T % 64 == 0, c_out % 64 == 0, the fp32-FMA kernel otherwise and in mode 1;
- * the arithmetic modes of psa_set_mlp_mode apply).  1 <= k <= 32.  workspace: psa_spider_conv_workspace_bytes(),
- * 256-byte aligned. */
+ * staged (tensor cores for b*n >= 128, c % 32 == 0, k*c*T % 64 == 0, c_out == 64 or c_out % 128 == 0, feat 16-byte
+ * aligned and feat_scale / feat_shift / bias / y 8-byte aligned; the fp32-FMA kernel otherwise and in mode 1; the arithmetic
+ * modes of psa_set_mlp_mode apply).  1 <= k <= 32.  workspace: psa_spider_conv_workspace_bytes(), sized for the tensor path
+ * whenever the dims allow it, 256-byte aligned. */
 PSA_API size_t psa_spider_conv_workspace_bytes(int b, int n, int c, int k, int T, int c_out);
 PSA_API int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_out, const float* delta, const int* nn_idx,
                                   const float* feat, const float* feat_scale, const float* feat_shift, const float* taylor,

@@ -77,11 +77,11 @@ struct SpiderArgs {
     const float* feat;         // (rows, c), 16-byte aligned
     const int* idx;            // (rows, k)
     const float* g;            // (rows * k, T)
-    const float* fs;           // (b, c) or null
+    const float* fs;           // (b, c) or null, 8-byte aligned on the tensor path
     const float* fu;
     const uint8_t* image;      // Wp in the format of NP, tile width 64 NC
-    const float* bias;         // (N)
-    float* y;                  // (rows, N)
+    const float* bias;         // (N), 8-byte aligned on the tensor path
+    float* y;                  // (rows, N), 8-byte aligned on the tensor path
     unsigned int* ovf = nullptr;            // np = 2: raised when an operand left the fp16 range or a weight is not finite
     const unsigned int* run_if = nullptr;   // non-null: no-op unless *run_if != 0
     const unsigned int* wflag = nullptr;
@@ -435,10 +435,15 @@ __global__ void __launch_bounds__(256) topk_pool_kernel(int n, int c, const floa
 // ------------------------------------------------------------------------------------------------------------------
 // launchers
 // ------------------------------------------------------------------------------------------------------------------
-static bool spider_tc_eligible(long long rows, int c, int k, int T, int N, const float* feat) {
+// the shapes and pointers the tensor path takes: cp.async reads feat in 16-byte chunks, the split step reads feat_scale / feat_shift
+// and the epilogue reads bias and writes y in float2.  A null pointer counts as aligned, so spider_ws sizes the workspace from the
+// dims alone; a misaligned pointer sends the call to the FMA kernel, which reads and writes one float at a time.
+static bool spider_tc_eligible(long long rows, int c, int k, int T, int N, const float* feat, const float* fs, const float* fu,
+                               const float* bias, const float* y) {
+    auto al = [](const void* p, uintptr_t m) { return p == nullptr || (reinterpret_cast<uintptr_t>(p) & m) == 0; };
     const long long K = (long long)k * T * c;
-    return rows >= 128 && c % 32 == 0 && K % 64 == 0 && N >= 64 && N % 64 == 0 && (N == 64 || N % 128 == 0) &&
-           (feat == nullptr || (reinterpret_cast<uintptr_t>(feat) & 15) == 0);
+    return rows >= 128 && c % 32 == 0 && K % 64 == 0 && N >= 64 && N % 64 == 0 && (N == 64 || N % 128 == 0) && al(feat, 15) &&
+           al(fs, 7) && al(fu, 7) && al(bias, 7) && al(y, 7);
 }
 
 struct SpiderWs {
@@ -451,7 +456,7 @@ static SpiderWs spider_ws(int b, int n, int c, int k, int T, int N) {
     const int K = k * T * c;
     size_t off = 256;                                        // word 0: range flag of the fp16x2 launch
     w.g = off; off += al256((size_t)rows * k * T * sizeof(float));
-    if (spider_tc_eligible(rows, c, k, T, N, nullptr)) {
+    if (spider_tc_eligible(rows, c, k, T, N, nullptr, nullptr, nullptr, nullptr, nullptr)) {
         w.wp = off; off += al256((size_t)K * N * sizeof(float));
         w.img2 = off; off += tc_image_alloc_bytes(K, N, 2);
         w.img3 = off; off += tc_image_alloc_bytes(K, N, 3);
@@ -509,7 +514,7 @@ extern "C" int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_ou
     spider_taylor_kernel<<<(unsigned)((pairs * T + 255) / 256), 256, 0, st>>>(pairs, T, delta, taylor, const_cast<float*>(a.g));
     int rc = check_launch("spider_taylor_kernel");
     if (rc != PSA_OK) return rc;
-    if (mlp_mode() == 1 || !spider_tc_eligible(rows, c, k, T, c_out, feat)) {
+    if (mlp_mode() == 1 || !spider_tc_eligible(rows, c, k, T, c_out, feat, feat_scale, feat_shift, bias, y)) {
         const dim3 grid((unsigned)((rows + 63) / 64), (unsigned)((c_out + 63) / 64));
         spider_fma_kernel<<<grid, 256, 0, st>>>(a, W);
         return check_launch("spider_fma_kernel");
