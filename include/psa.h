@@ -592,6 +592,56 @@ PSA_API int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const float*
  * of in-grid cells -> (b*r^3, c); kind 1 = SAME 2^3 max, stride 2, padded at the far end -> (b*ceil(r/2)^3, c). */
 PSA_API int psa_pool3d(int b, int r, int c, int kind, const float* x, float* out, psa_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * PointCNN, inference mode (PointCNN/pointcnn.py:10-52 xconv, pointfly.py:122-128, 163-176 knn_indices_general,
+ * :298-347 dense / conv2d / depthwise_conv2d / separable_conv2d).  Every layer with batch norm has no bias and applies
+ * ELU before the batch norm: a = elu(x . W) * s + t, s = gamma / sqrt(moving_variance + 1e-3), t = beta - moving_mean * s.
+ * ------------------------------------------------------------------------------------------- */
+
+/* knn_indices_general(queries, points, k*d, sort=True) followed by indices[:, :, ::d] (pointcnn.py:12-13): points (b,n,3),
+ * queries (b,m,3) -> idx (b,m,k) int32 in [0, n).  D = (|q|^2 + (-2 q.p)) + |p|^2 with the dot and the norms fma chains over
+ * x, y, z from 0 (the order of oracle/psa_oracle.c:orc_dgcnn_knn); the k*d smallest in ascending order, lower index first on
+ * ties (tf.nn.top_k), then every d-th entry from the first.  Duplicate points stay in the lists: the reference's unique=True
+ * (pointfly.py:142-144) adds to a local name only.  k*d <= 64 and k*d <= n. */
+PSA_API int psa_knn_dilated(int b, int n, int m, int k, int d, const float* points, const float* queries, int* idx,
+                            psa_stream_t stream);
+
+/* The weights of one X-Conv layer in TF's layouts, each with its batch norm as (s, t):
+ *   w_pts0 (3, c_pts)        `<tag>nn_fts_from_pts_0/kernel`     w_pts1 (c_pts, c_pts)  `<tag>nn_fts_from_pts/kernel`
+ *   w_x0   (1, K, 3, K*K)    `<tag>X_0/kernel`                   w_x1, w_x2 (1, K, K, K) `<tag>X_1/depthwise_weights`, X_2
+ *   w_dw   (1, K, c_in, dm)  `<tag>fts_conv/depthwise_kernel`, c_in = c_pts + c_prev.  X_2 has no ELU (pointcnn.py:37). */
+typedef struct psa_xconv {
+    int K, c_pts, c_prev, dm;
+    const float *w_pts0, *s_pts0, *t_pts0;
+    const float *w_pts1, *s_pts1, *t_pts1;
+    const float *w_x0, *s_x0, *t_x0;
+    const float *w_x1, *s_x1, *t_x1;
+    const float *w_x2, *s_x2, *t_x2;
+    const float* w_dw;
+} psa_xconv;
+
+/* One X-Conv layer up to the depthwise stage of its separable conv, per query (pointcnn.py:15-44):
+ *   local[j] = pts[idx[j]] - q;  lifted = dense(dense(local)) (K, c_pts);  F = [lifted | fts[idx[j]]] (K, c_in);
+ *   X0[a*K + b] = sum_{j,d} local[j][d] w_x0[j][d][a*K + b] (ELU, BN);  X1[b*K + m] = sum_a X0[a*K + b] w_x1[a][b][m] (ELU, BN);
+ *   X2 likewise from X1 with w_x2 (BN, no ELU);  fts_X[i][c] = sum_j X2[i*K + j] F[j][c];
+ *   out[c*dm + m] = sum_i fts_X[i][c] w_dw[i][c][m].
+ * pts (b,n,3), qrs (b,P,3), idx (b,P,K) int32 in [0, n), fts (b,n,c_prev) or NULL when c_prev == 0 -> out (b*P, c_in*dm).
+ * fp32 FMA, one tile of queries per block in shared memory: no (b,P,K,.) tensor reaches global memory.  1 <= K <= 16. */
+PSA_API int psa_xconv_core(int b, int n, int P, const float* pts, const float* qrs, const int* idx, const float* fts,
+                           const psa_xconv* layer, float* out, psa_stream_t stream);
+
+/* out[row * ldo + o] = elu((x . W)[row][o] + bias[o]) * scale[o] + shift[o] for o < N: x rows of stride ldx, K channels; W (K, N);
+ * bias (N) or NULL.  The row strides let a layer write its slice of a wider row (the global branch and the pointwise conv of
+ * the last X-Conv layer, pointcnn.py:47-50).  Tensor cores for rows >= 128, K % 4 == 0, ldx % 4 == 0 and x 16-byte aligned:
+ * the operand columns past K read as zero up to a multiple of 64, W is padded to 64-wide column blocks (taken 128 wide when
+ * their count is even) and only the N real columns are written; the fp32-FMA kernel otherwise and in mode 1.  The arithmetic
+ * modes of psa_set_mlp_mode apply.  workspace: psa_dense_elu_affine_workspace_bytes() queried in the mode of the call (0 when
+ * the dims or the mode take the FMA kernel), 256-byte aligned. */
+PSA_API size_t psa_dense_elu_affine_workspace_bytes(long long rows, int K, int N);
+PSA_API int psa_dense_elu_affine(long long rows, int K, int N, const float* x, long long ldx, const float* W, const float* bias,
+                                 const float* scale, const float* shift, float* out, long long ldo, void* workspace,
+                                 size_t workspace_bytes, psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

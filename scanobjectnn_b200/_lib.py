@@ -33,6 +33,13 @@ class PsaMlp(C.Structure):
     ]
 
 
+class PsaXconv(C.Structure):
+    """psa_xconv (include/psa.h): the weights of one PointCNN X-Conv layer."""
+    _fields_ = [("K", C.c_int), ("c_pts", C.c_int), ("c_prev", C.c_int), ("dm", C.c_int)] + [
+        (f, C.c_void_p) for f in ("w_pts0", "s_pts0", "t_pts0", "w_pts1", "s_pts1", "t_pts1", "w_x0", "s_x0", "t_x0", "w_x1", "s_x1",
+                                  "t_x1", "w_x2", "s_x2", "t_x2", "w_dw")]
+
+
 class PsaActIn(C.Structure):
     """psa_act_in (include/psa.h): forward input of a training-mode layer."""
     _fields_ = [("x", C.c_void_p), ("ld", C.c_longlong), ("scale", C.c_void_p), ("shift", C.c_void_p), ("mask", C.c_void_p),
@@ -111,6 +118,10 @@ SIGNATURES = {
     "psa_fisher_vector": [_i, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_conv3d_infer": [_i, _i, _i, _i, _i, _p, _ll, _p, _p, _p, _i, _p, _ll, _p, _sz, _p],
     "psa_pool3d": [_i, _i, _i, _i, _p, _p, _p],
+    # PointCNN (inference)
+    "psa_knn_dilated": [_i, _i, _i, _i, _i, _p, _p, _p, _p],
+    "psa_xconv_core": [_i, _i, _i, _p, _p, _p, _p, C.POINTER(PsaXconv), _p, _p],
+    "psa_dense_elu_affine": [_ll, _i, _i, _p, _ll, _p, _p, _p, _p, _p, _ll, _p, _sz, _p],
     "psa_softmax_xent": [_i, _i, _p, _p, _p, _p, _p],
     "psa_pool_rows": [_ll, _i, _i, _i, _p, _p, _p, _p],
     "psa_adam_step": [_ll, _p, _p, _p, _p, _f, _f, _f, _f, _i, _f, _p],
@@ -120,7 +131,7 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_train_dense_workspace_bytes", "psa_bn_bwd_workspace_bytes", "psa_sa_conv1_bwd_workspace_bytes", "psa_knn_graph_workspace_bytes",
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
                 "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes", "psa_spider_conv_workspace_bytes",
-                "psa_conv3d_workspace_bytes")
+                "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes")
 
 _lib = None
 
@@ -169,6 +180,8 @@ def load() -> C.CDLL:
     lib.psa_spider_conv_workspace_bytes.restype = C.c_size_t
     lib.psa_conv3d_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
     lib.psa_conv3d_workspace_bytes.restype = C.c_size_t
+    lib.psa_dense_elu_affine_workspace_bytes.argtypes = [_ll, _i, _i]
+    lib.psa_dense_elu_affine_workspace_bytes.restype = C.c_size_t
     lib.psa_version.restype = C.c_int
     lib.psa_sm_arch.restype = C.c_int
     lib.psa_last_error.restype = C.c_char_p

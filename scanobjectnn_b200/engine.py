@@ -79,3 +79,12 @@ def pointnet2_cls_ssg_engine(params, batch: int = 32, npoints: int = 2048, num_c
         return logits
 
     return InferenceEngine(forward, (batch, npoints, 3), (batch, num_class), slots=slots, device=device)
+
+
+def pointcnn_cls_engine(params, batch: int = 32, npoints: int = 1024, num_class: int = 15, slots: int = 3, device=None):
+    from . import pointcnn_cls
+
+    def forward(x):
+        return pointcnn_cls.get_model(x, False, num_class, params=params)
+
+    return InferenceEngine(forward, (batch, npoints, 3), (batch, 1, num_class), slots=slots, device=device)

@@ -22,7 +22,8 @@ __all__ = [
     "three_nn", "three_interpolate", "three_nn_interpolate", "pairwise_distance", "knn", "knn_graph",
     "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "shared_mlp_grouped", "sa_module_infer",
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
-    "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d",
+    "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d", "knn_dilated", "xconv_core",
+    "dense_elu_affine",
 ]
 
 
@@ -780,6 +781,100 @@ def pool3d(x, r: int, kind: str) -> torch.Tensor:
     ro = r if kind == "avg" else (r + 1) // 2
     out = torch.empty((b * ro ** 3, c), dtype=torch.float32, device=x.device)
     check(_lib.load().psa_pool3d(b, r, c, 0 if kind == "avg" else 1, _ptr(x), _ptr(out), _stream()), "pool3d")
+    return out
+
+
+# ------------------------------------------------------------------------------------------------
+# PointCNN (PointCNN/pointcnn.py:10-52, pointfly.py:122-128, 163-176, 298-347)
+# ------------------------------------------------------------------------------------------------
+KNN_DILATED_MAX = 64          # k * d entries a query keeps (psa_knn_dilated)
+XCONV_MAX_K = 16              # neighbours per query of psa_xconv_core
+XCONV_WEIGHTS = ("w_pts0", "s_pts0", "t_pts0", "w_pts1", "s_pts1", "t_pts1", "w_x0", "s_x0", "t_x0", "w_x1", "s_x1", "t_x1", "w_x2",
+                 "s_x2", "t_x2", "w_dw")
+
+
+def knn_dilated(points, queries, k: int, d: int = 1) -> torch.Tensor:
+    """knn_indices_general(queries, points, k*d, sort=True)[:, :, ::d] (psa_knn_dilated): points (B,N,3), queries (B,M,3) -> (B,M,k)
+    int32 indices into points, ascending distance, lower index first on ties, duplicate points kept."""
+    if k < 1 or d < 1 or k * d > KNN_DILATED_MAX:
+        raise ValueError(f"knn_dilated: k={k}, d={d}: need k, d >= 1 and k*d <= {KNN_DILATED_MAX}")
+    points = _dev(points, torch.float32, "points", 3)
+    queries = _dev(queries, torch.float32, "queries", 3)
+    b, n, c = points.shape
+    if c != 3 or queries.shape[0] != b or queries.shape[2] != 3:
+        raise ValueError(f"knn_dilated: points {tuple(points.shape)} / queries {tuple(queries.shape)} must be (B,N,3) / (B,M,3)")
+    if k * d > n:
+        raise ValueError(f"knn_dilated: k*d = {k * d} exceeds the {n} points")
+    m = queries.shape[1]
+    idx = torch.empty((b, m, k), dtype=torch.int32, device=points.device)
+    check(_lib.load().psa_knn_dilated(b, n, m, k, d, _ptr(points), _ptr(queries), _ptr(idx), _stream()), "knn_dilated")
+    return idx
+
+
+def xconv_core(pts, qrs, idx, fts, weights: dict, dm: int) -> torch.Tensor:
+    """One X-Conv layer up to the depthwise stage of its separable conv (psa_xconv_core): pts (B,N,3), qrs (B,P,3), idx (B,P,K) int32,
+    fts (B,N,C_prev) or None; ``weights`` maps the names of ops.XCONV_WEIGHTS to the TF-shaped tensors (include/psa.h) -> (B*P,
+    C_in*dm), C_in = C_pts + C_prev."""
+    b, p, k = idx.shape
+    w_pts0 = weights["w_pts0"]
+    c_pts = w_pts0.shape[-1]
+    c_prev = 0 if fts is None else fts.shape[-1]
+    if k < 1 or k > XCONV_MAX_K:
+        raise ValueError(f"xconv_core: K={k} must be in [1, {XCONV_MAX_K}]")
+    if tuple(weights["w_x0"].shape[-3:]) != (k, 3, k * k) or tuple(weights["w_dw"].shape[-3:-1]) != (k, c_pts + c_prev):
+        raise ValueError(f"xconv_core: X_0 {tuple(weights['w_x0'].shape)} / depthwise {tuple(weights['w_dw'].shape)} do not match K={k}, "
+                         f"C_in={c_pts + c_prev}")
+    if weights["w_dw"].shape[-1] != dm:
+        raise ValueError(f"xconv_core: the depthwise kernel has multiplier {weights['w_dw'].shape[-1]}, not {dm}")
+    pts = _dev(pts, torch.float32, "pts", 3)
+    qrs = _dev(qrs, torch.float32, "qrs", 3)
+    idx = _dev(idx, torch.int32, "idx", 3)
+    if fts is not None:
+        fts = _dev(fts, torch.float32, "fts", 3)
+        if tuple(fts.shape[:2]) != tuple(pts.shape[:2]):
+            raise ValueError(f"xconv_core: fts {tuple(fts.shape)} does not match pts {tuple(pts.shape)}")
+    n = pts.shape[1]
+    if qrs.shape[0] != b or qrs.shape[1] != p or pts.shape[0] != b:
+        raise ValueError(f"xconv_core: pts {tuple(pts.shape)} / qrs {tuple(qrs.shape)} / idx {tuple(idx.shape)} disagree")
+    ws = {name: _dev(weights[name], torch.float32, name) for name in XCONV_WEIGHTS}
+    layer = _lib.PsaXconv(k, c_pts, c_prev, dm, *[ws[name].data_ptr() for name in XCONV_WEIGHTS])
+    out = torch.empty((b * p, (c_pts + c_prev) * dm), dtype=torch.float32, device=pts.device)
+    check(_lib.load().psa_xconv_core(b, n, p, _ptr(pts), _ptr(qrs), _ptr(idx), _ptr(fts), C.byref(layer), _ptr(out), _stream()),
+          "xconv_core")
+    return out
+
+
+def dense_elu_affine(x, weights, scale, shift, bias=None, out=None, offset: int = 0) -> torch.Tensor:
+    """elu(x . W [+ bias]) * scale + shift (psa_dense_elu_affine), PointCNN's dense / conv layer with ELU before its batch norm: x (R, K)
+    (a column slice of a wider buffer is read in place), weights (K, N) or any TF shape (..., K, N) -> (R, N).  out (R, C_total):
+    written at channels [offset, offset + N) and returned."""
+    x = _rows_view(x, "x")
+    weights = _dev(weights, torch.float32, "weights")
+    rows, k = x.shape
+    n = weights.shape[-1]
+    if weights.numel() != k * n:
+        raise ValueError(f"dense_elu_affine: weights {tuple(weights.shape)} are not ({k}, N)")
+    scale = _dev(scale, torch.float32, "scale", 1)
+    shift = _dev(shift, torch.float32, "shift", 1)
+    if bias is not None:
+        bias = _dev(bias, torch.float32, "bias", 1)
+    for name, t in (("scale", scale), ("shift", shift), ("bias", bias)):
+        if t is not None and t.shape[0] != n:
+            raise ValueError(f"dense_elu_affine: {name} must have {n} entries")
+    if out is None:
+        out = torch.empty((rows, n), dtype=torch.float32, device=x.device)
+        view = out
+    else:
+        if not (out.is_cuda and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == rows):
+            raise ValueError(f"dense_elu_affine: out must be a float32 CUDA tensor ({rows}, C_total) with unit column stride")
+        if offset < 0 or offset + n > out.shape[1]:
+            raise ValueError(f"dense_elu_affine: channels [{offset}, {offset + n}) do not fit out's {out.shape[1]}")
+        view = out[:, offset:]
+    lib = _lib.load()
+    need = lib.psa_dense_elu_affine_workspace_bytes(rows, k, n)
+    ws = torch.empty((max(need, 4) + 3) // 4, dtype=torch.float32, device=x.device)
+    check(lib.psa_dense_elu_affine(rows, k, n, _ptr(x), x.stride(0), _ptr(weights), _ptr(bias), _ptr(scale), _ptr(shift), _ptr(view),
+                                   out.stride(0), _ptr(ws), C.c_size_t(need), _stream()), "dense_elu_affine")
     return out
 
 

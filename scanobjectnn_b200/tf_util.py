@@ -94,6 +94,40 @@ class VariableStore(dict):
         self[f"{scope}/conv/gn/gamma"] = torch.ones(cout, device=self.device)
         self[f"{scope}/conv/gn/beta"] = torch.zeros(cout, device=self.device)
 
+    def _glorot_normal(self, shape):
+        """tf.glorot_normal_initializer: a normal truncated at two standard deviations, stddev sqrt(2 / (fan_in + fan_out)) / 0.8796,
+        with TF's fans (the receptive field times the last two dimensions)"""
+        receptive = math.prod(shape[:-2]) if len(shape) > 2 else 1
+        fan_in, fan_out = shape[-2] * receptive, shape[-1] * receptive
+        std = math.sqrt(2.0 / (fan_in + fan_out)) / 0.87962566103423978
+        w = torch.empty(shape, dtype=torch.float32)
+        torch.nn.init.trunc_normal_(w, 0.0, std, -2 * std, 2 * std, generator=self._gen)
+        return w.to(self.device)
+
+    def add_pointfly(self, name, shape, bn=True, randomize_bn=False):
+        """A pointfly layer (PointCNN/pointfly.py:298-347) with with_bn=True: the kernel ``name`` of TF shape ``shape`` (Glorot normal)
+        and tf.layers.batch_normalization's variables under ``<layer>_bn/`` (``<layer>`` = ``name`` up to its last ``/``), over the
+        layer's outputs: shape[-1] channels, or in * multiplier for a depthwise kernel."""
+        self[name] = self._glorot_normal(shape)
+        if bn:
+            c = shape[-2] * shape[-1] if name.endswith("/depthwise_weights") else shape[-1]
+            scope = name.rsplit("/", 1)[0] + "_bn"
+            r = lambda lo, hi: (torch.rand(c, generator=self._gen) * (hi - lo) + lo).to(self.device)
+            self[f"{scope}/gamma"] = r(0.8, 1.2) if randomize_bn else torch.ones(c, device=self.device)
+            self[f"{scope}/beta"] = r(-0.1, 0.1) if randomize_bn else torch.zeros(c, device=self.device)
+            self[f"{scope}/moving_mean"] = r(-0.1, 0.1) if randomize_bn else torch.zeros(c, device=self.device)
+            self[f"{scope}/moving_variance"] = r(0.5, 1.5) if randomize_bn else torch.ones(c, device=self.device)
+
+    def elu_bn(self, layer):
+        """(s, t) of ``layer``'s inference-mode batch norm, applied after its ELU: s = gamma / sqrt(moving_variance + 1e-3),
+        t = beta - moving_mean * s (tf.layers.batch_normalization, pointfly.py:298-302), evaluated in fp64"""
+        key = ("elu_bn", layer)
+        if key not in self._cache:
+            g = lambda v: self[f"{layer}_bn/{v}"].double()
+            s = g("gamma") / torch.sqrt(g("moving_variance") + BN_EPS)
+            self._cache[key] = (s.float().contiguous(), (g("beta") - g("moving_mean") * s).float().contiguous())
+        return self._cache[key]
+
     def spider(self, scope):
         """(taylor (20,T), conv weights (k, cin*T, cout), conv biases, gn gamma, gn beta) of a spiderConv ``scope``, as
         ops.spider_conv / ops.group_norm_affine take them; cached like ``folded``."""
