@@ -130,7 +130,8 @@ def _get_model_training(point_cloud, bn_decay, num_class, params: VariableStore,
         net = mlp_training(net, [("fc2", True)], bn_decay, params)
         class_pred = mlp_training(drop(net), [("fc3", False)], bn_decay, params)
         concat = torch.cat([net.unsqueeze(1).expand(b, n, 256), out_max.unsqueeze(1).expand(b, n, 1024), *nets], dim=-1)
-        seg = mlp_training(concat, [("seg/conv1", True), ("seg/conv2", True)], bn_decay, params)
+        # seg/conv1 and seg/conv2 are built without bn_decay (dgcnn_bga.py:125-128): their moving averages always decay at the default 0.9
+        seg = mlp_training(concat, [("seg/conv1", True), ("seg/conv2", True)], None, params)
         if dropout:
             seg = f.dropout(seg, 0.3, training=True)                                                                      # keep_prob 0.7
         return class_pred, mlp_training(seg, [("seg/conv3", False)], bn_decay, params), end_points
@@ -175,3 +176,13 @@ def get_model_bga(point_cloud, is_training, bn_decay=None, num_class=NUM_CLASSES
 def get_loss(pred, label, end_points=None, num_class=NUM_CLASSES):
     """softmax cross-entropy with label smoothing 0.2 (dgcnn.py:105-111)."""
     return torch.nn.functional.cross_entropy(pred, label.long(), label_smoothing=0.2)
+
+
+def get_loss_bga(class_pred, seg_pred, gt_label, gt_mask, seg_weight=0.5):
+    """dgcnn_bga.get_loss (dgcnn_bga.py:137-152): (1-w)*mean CE(class) + w*mean over clouds of the mean per-point 2-way CE, without
+    get_loss's label smoothing -> (total, classify, seg)"""
+    f = torch.nn.functional
+    classify_loss = f.cross_entropy(class_pred, gt_label.long())
+    per_point = f.cross_entropy(seg_pred.reshape(-1, seg_pred.shape[-1]), gt_mask.reshape(-1).long(), reduction="none")
+    seg_loss = per_point.reshape(gt_mask.shape).mean(dim=1).mean()
+    return (1 - seg_weight) * classify_loss + seg_weight * seg_loss, classify_loss, seg_loss

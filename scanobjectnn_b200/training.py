@@ -44,6 +44,7 @@ SSG_LEVELS = [LevelSpec("layer1", 512, 0.2, 32, [64, 64, 128]), LevelSpec("layer
               LevelSpec("layer3", None, None, None, [256, 512, 1024], group_all=True)]
 SSG_HEAD = [("fc1", 512, True, 0.5), ("fc2", 256, True, 0.5), ("fc3", None, False, None)]   # (scope, width, bn, keep_prob)
 STATS_FROM_ROWS = 1024       # dense layers of at most this many rows take batch statistics from their output (psa_bn_finalize_rows)
+DEFAULT_BN_DECAY = 0.9       # the moving averages' decay for bn_decay=None (tf_util.py's batch_norm_template / batch_norm_dist_template)
 
 
 class FlatParams:
@@ -407,12 +408,13 @@ def _cached(params: VariableStore, key, make):
 
 
 def _flat_and_decay(tr: _TrainOps, bn_decay):
-    """the autograd input that carries the variables' gradients and the moving-average decay (tf_util's default 0.5 for None);
+    """the autograd input that carries the variables' gradients and the moving-average decay: 0.9 for None, the default of every
+    reference tf_util's batch_norm_template and batch_norm_dist_template (`decay = bn_decay if bn_decay is not None else 0.9`);
     (None, 0.0) for a frozen trainer, which neither updates nor differentiates the variables"""
     if tr.frozen:
         return None, 0.0
     tr.fp.flat.requires_grad_(True)
-    return tr.fp.flat, 0.5 if bn_decay is None else float(bn_decay)
+    return tr.fp.flat, DEFAULT_BN_DECAY if bn_decay is None else float(bn_decay)
 
 
 def mlp_training(x: torch.Tensor, layers, bn_decay, params: VariableStore, frozen: bool = False,

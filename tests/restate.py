@@ -114,7 +114,8 @@ def layer(h, P, scope, frozen, *, bn=True, relu=True, stats=None, run=None, info
     With a `run` (RunDecisions) the relu is z * the run's gate, and `info` counts the gates that differ from float64's own ("flips"
     of "units").  In training mode the batch statistics then take the run's values, float64's derivative: fp32 sums of y and y^2
     give the variance with an error relative to E[y^2], not to the variance, and that error is bounded on its own
-    (info["stat_err"], relative to E[y^2]) instead of through every later layer."""
+    (info["stat_err"], relative to E[y^2]) instead of through every later layer; info["own"] keeps h's dtype's own batch statistics,
+    by scope, for the moving averages."""
     dt = h.dtype
     w = P[f"{scope}/weights"].to(dt)
     y = h @ w.reshape(-1, w.shape[-1]) + P[f"{scope}/biases"].to(dt)
@@ -126,6 +127,7 @@ def layer(h, P, scope, frozen, *, bn=True, relu=True, stats=None, run=None, info
         dims = tuple(range(y.dim() - 1))
         mean, var = y.mean(dims), y.var(dims, unbiased=False)
         if run is not None and scope in run.stats:
+            info.setdefault("own", {})[scope] = (mean.detach(), var.detach())          # dtype's own batch statistics
             rmean, rinv = run.stats[scope][0].to(dt), run.stats[scope][1].to(dt)
             rvar = 1.0 / (rinv * rinv) - BN_EPS
             ms = float((y.detach() ** 2).mean(dims).max())
@@ -181,6 +183,22 @@ def inner_flip(pre, inner):
 
 def zero_at(t, mask):
     t.register_hook(lambda g: g.masked_fill(mask, 0.0))
+
+
+def dropper(drops):
+    """dropout that applies the given (mask, p) pairs in call order: t * mask / (1 - p); without `drops` the identity.  The returned
+    function's `left()` counts the pairs not yet applied."""
+    it = iter(drops or ())
+
+    def drop(t):
+        if drops is None:
+            return t
+        mask, p = next(it)
+        assert mask.shape == t.shape, (mask.shape, t.shape)
+        return t * mask.to(t.dtype) / (1 - p)
+
+    drop.left = lambda: sum(1 for _ in it)
+    return drop
 
 
 class Masks:
@@ -320,6 +338,35 @@ def interpolate(xyz1, xyz2, points2):
     return (points2[ar, idx] * w[..., None]).sum(dim=2)
 
 
+def pn2_levels(x, L, masks, idx):
+    """the three set-abstraction levels of pointnet2_cls_bga / _partseg ([64, 64, 128], [128, 128, 256], group all [256, 512, 1024])
+    on the given indices [(fps, ball)] * 2, max-pooled through masks.edge_max -> [(new_xyz, pooled)] * 3; L: the caller's layer()"""
+    out, xyz, pts = [], x, None
+    for scope, ind in (("layer1", idx[0]), ("layer2", idx[1]), ("layer3", (None, None))):
+        xyz, h = sa_level(xyz, pts, *ind)
+        for i in range(3):
+            h = L(h, f"{scope}/conv{i}")
+        pts = masks.edge_max(h)
+        out.append((xyz, pts))
+    return out
+
+
+def pn2_fp(xyz1, xyz2, pts1, pts2, L, scope, n):
+    """pointnet_fp_module (pointnet_util.py:199-229): interpolate pts2 onto xyz1, concatenate pts1, n layers"""
+    h = interpolate(xyz1, xyz2, pts2)
+    h = torch.cat([h, pts1], dim=2) if pts1 is not None else h          # a tile + concat for fa_layer1
+    for i in range(n):
+        h = L(h, f"{scope}/conv_{i}")
+    return h
+
+
+def pn2_indices(p, mode):
+    """per sampled level (fps_idx, ball-query idx) as int64, from the last run of the level trainers cached on store `p` for `mode`
+    ("level" or "level_frozen")"""
+    lv = {key[1]: tr.levels[0] for key, tr in p.__dict__["_trainers"].items() if key[0] == mode}
+    return [(lv[s].fps_idx.long(), lv[s].idx.long()) for s in ("layer1", "layer2")]
+
+
 def _argk_pool(h, argk, info):
     """the max over dim 2 taken at the run's winner argk (its first winning row), so the gradient goes where the kernel sends it;
     info["pool_gap"]: how far below h's own maximum that row lies, relative to h's largest entry"""
@@ -358,11 +405,14 @@ def ssg(xyz, p, levels, frozen, masks, run=None, info=None):
     return h
 
 
-def dgcnn(x, P, graphs, frozen, masks, detach_transform=False, stats=None):
-    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55), dropout off, on the given neighbour graphs -> logits; stats (a
-    dict): every layer's batch statistics, by scope"""
-    b = x.shape[0]
-    L = lambda h, s, **kw: layer(h, P, s, frozen, stats=stats, **kw)        # noqa: E731
+def dgcnn(x, P, graphs, frozen, masks, detach_transform=False, stats=None, bga=False, run=None, info=None, drops=None):
+    """dgcnn.get_model (dgcnn.py:24-102, transform_nets.py:10-55) on the given neighbour graphs -> logits; stats (a dict): every
+    layer's batch statistics, by scope.  bga: dgcnn_bga.get_model (dgcnn_bga.py:27-134) -> (class_pred, seg_pred), the segmentation
+    head on concat[class vector (fc2's output, before dp2), the pooled agg, net1..net4] (1600 channels).  run (RunDecisions) and
+    info as for layer(); drops: the dropout masks (dp1, dp2 and, with bga, the segmentation head's), see dropper()."""
+    b, n = x.shape[:2]
+    L = lambda h, s, **kw: layer(h, P, s, frozen, stats=stats, run=run, info=info, **kw)        # noqa: E731
+    drop = dropper(drops)
     sc = "transform_net1"
     y1 = L(edges(x, graphs[0]), f"{sc}/tconv1", relu=False)
     y = L(torch.relu(y1), f"{sc}/tconv2", relu=False)
@@ -380,9 +430,15 @@ def dgcnn(x, P, graphs, frozen, masks, detach_transform=False, stats=None):
         nets.append(h)
     y = L(torch.cat(nets, dim=-1), "agg", relu=False)
     g = masks.point_max(torch.relu(y), "agg", pre=y)
-    for s in ("fc1", "fc2"):
-        g = masks.head_layer(g, P, s, frozen, stats=stats)
-    return L(g, "fc3", bn=False)
+    kw = dict(stats=stats, run=run, info=info)
+    c = drop(masks.head_layer(g, P, "fc1", frozen, **kw))
+    c = masks.head_layer(c, P, "fc2", frozen, **kw)
+    class_pred = L(drop(c), "fc3", bn=False)
+    if not bga:
+        return class_pred
+    h = torch.cat([c.unsqueeze(1).expand(b, n, c.shape[-1]), g.unsqueeze(1).expand(b, n, g.shape[-1]), *nets], dim=-1)
+    h = L(L(h, "seg/conv1"), "seg/conv2")
+    return class_pred, L(drop(h), "seg/conv3", bn=False)
 
 
 def pointnet(x, P, masks):
@@ -429,28 +485,32 @@ def pointnet2_partseg(x, P, frozen, masks, idx, run=None):
     "stat_err"}); run: RunDecisions"""
     info = {"stats": {}, "flips": 0, "units": 0, "stat_err": 0.0}
     L = lambda h, s, **kw: layer(h, P, s, frozen, stats=info["stats"], run=run, info=info, **kw)        # noqa: E731
-
-    def level(xyz, pts, scope, fps=None, ball=None):
-        new_xyz, h = sa_level(xyz, pts, fps, ball)
-        for i in range(3):
-            h = L(h, f"{scope}/conv{i}")
-        return new_xyz, masks.edge_max(h)
-
-    def fp(xyz1, xyz2, pts1, pts2, scope, n):
-        h = interpolate(xyz1, xyz2, pts2)
-        h = torch.cat([h, pts1], dim=2) if pts1 is not None else h          # tile + concat for fa_layer1
-        for i in range(n):
-            h = L(h, f"{scope}/conv_{i}")
-        return h
-
-    (f1, i1), (f2, i2) = idx
-    l1_xyz, l1 = level(x, None, "layer1", f1, i1)
-    l2_xyz, l2 = level(l1_xyz, l1, "layer2", f2, i2)
-    l3_xyz, l3 = level(l2_xyz, l2, "layer3")
-    l2 = fp(l2_xyz, l3_xyz, l2, l3, "fa_layer1", 2)
-    l1 = fp(l1_xyz, l2_xyz, l1, l2, "fa_layer2", 2)
-    l0 = fp(x, l1_xyz, None, l1, "fa_layer3", 3)
+    (l1_xyz, l1), (l2_xyz, l2), (l3_xyz, l3) = pn2_levels(x, L, masks, idx)
+    l2 = pn2_fp(l2_xyz, l3_xyz, l2, l3, L, "fa_layer1", 2)
+    l1 = pn2_fp(l1_xyz, l2_xyz, l1, l2, L, "fa_layer2", 2)
+    l0 = pn2_fp(x, l1_xyz, None, l1, L, "fa_layer3", 3)
     return L(L(l0, "seg_fc1"), "seg_fc2", bn=False), info
+
+
+def pointnet2_bga(x, P, frozen, masks, idx, run=None, drops=None):
+    """pointnet2_cls_bga (pointnet2/models/pointnet2_cls_bga.py:21-75) on the given level indices [(fps, ball)] * 2 -> (class_pred,
+    seg_pred, {"stats", "flips", "units", "stat_err"[, "own"]}).  The class vector is fc2's output before dp2; fa_layer1 interpolates
+    it from the group-all level's single point (weights (1, 0, 0)) and concatenates l2_points.  run: RunDecisions; drops: the
+    dropout masks of dp1, dp2 and seg_dp1, see dropper()."""
+    info = {"stats": {}, "flips": 0, "units": 0, "stat_err": 0.0}
+    kw = dict(stats=info["stats"], run=run, info=info)
+    L = lambda h, s, **k: layer(h, P, s, frozen, **kw, **k)        # noqa: E731
+    drop = dropper(drops)
+    (l1_xyz, l1), (l2_xyz, l2), (l3_xyz, l3) = pn2_levels(x, L, masks, idx)
+    net = drop(masks.head_layer(l3.reshape(x.shape[0], -1), P, "fc1", frozen, **kw))
+    net = masks.head_layer(net, P, "fc2", frozen, **kw)
+    class_pred = L(drop(net), "fc3", bn=False)
+    l2 = pn2_fp(l2_xyz, l3_xyz, l2, net.unsqueeze(1), L, "fa_layer1", 2)
+    l1 = pn2_fp(l1_xyz, l2_xyz, l1, l2, L, "fa_layer2", 2)
+    l0 = pn2_fp(x, l1_xyz, None, l1, L, "fa_layer3", 3)
+    seg_pred = L(drop(L(l0, "seg_fc1")), "seg_fc2", bn=False)
+    assert drop.left() == 0, "dropout masks left over"
+    return class_pred, seg_pred, info
 
 
 # ---------------------------------------------------------------------------------------------------------------------
