@@ -8,8 +8,9 @@
 //                          warps gather each 64-channel block of one tap's neighbour rows with cp.async (a neighbour outside the
 //                          grid, or a row past the end, is zero-filled), a tile skips every tap outside the grid for all its rows,
 //                          and the tap loop of a tile is split across CTAs whose partials a second kernel adds in a fixed order.
-//                          Same ring, operand split and fp16x2 range guard as tc_spider_kernel (spider.cu).
+//                          Runs on the shared ring (ring_gemm.cuh).
 //   conv3d_fma_kernel      the same layer on the fp32 FMA pipe (mode 1, and shapes the tensor path does not take: c = 20)
+//   pad_cols_kernel        W padded with zero columns to the image width, for conv3d and PointCNN's dense layers (pointcnn.cu)
 //   pool3d_*_kernel        the SAME 3^3 stride-1 average (divided by the in-grid count) and the SAME 2^3 stride-2 max
 //
 // Row order of every grid activation: voxel-major, row = voxel * b + cloud, voxel = (d * r + h) * r + w.  A 128-row tile then
@@ -18,8 +19,7 @@
 #include <float.h>
 
 #include "common.cuh"
-#include "mlp_internal.cuh"
-#include "tc_common.cuh"
+#include "ring_gemm.cuh"
 
 namespace psa {
 
@@ -179,12 +179,10 @@ __device__ __forceinline__ int mask_next_g(const uint32_t* m, int from) {
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// tc_conv3d_kernel<NP, NC>: out (rows, N) = relu((A . W) * scale + shift) over work units (128-row tile, 64 NC-column tile,
-// split), persistent with a static unit order.  A[row][(tap, ch)] = x[neighbour(row, tap)][ch], or 0 outside the grid.  Unit
-// (tile, nt, sp) takes the active K blocks [nact sp / S, nact (sp + 1) / S) of its tile, in (tap, channel block) order; with
-// S > 1 it writes its partial (unscaled) to partial[sp] and conv3d_finalize_kernel adds the S partials in split order.
-// CTA = two consumer warpgroups (rows 0-63 / 64-127) + a producer warpgroup whose four warps each gather 32 rows of every block
-// while warp 0 also drops the block's weights in by TMA.  The consumers' K loop is tc_spider_kernel's.
+// tc_conv3d_kernel<NP, NC>: out (rows, N) = relu((A . W) * scale + shift) on the ring (ring_gemm.cuh), unit = (128-row tile, 64
+// NC-column tile, split).  A[row][(tap, ch)] = x[neighbour(row, tap)][ch], or 0 outside the grid.  Unit (tile, nt, sp) takes the
+// active K blocks [nact sp / S, nact (sp + 1) / S) of its tile, in (tap, channel block) order; with S > 1 it writes its partial
+// (unscaled) to partial[sp] and conv3d_finalize_kernel adds the S partials in split order.
 // ------------------------------------------------------------------------------------------------------------------
 struct Conv3dArgs {
     long long rows;            // b * r^3
@@ -193,219 +191,147 @@ struct Conv3dArgs {
     const float* x;            // (rows, ldx), 16-byte aligned, ldx % 4 == 0
     long long ldx;
     const uint32_t* tapmask;   // (tiles, 4)
-    const uint8_t* image;      // W (k^3 c, Np) in the format of NP, tile width 64 NC
     const float* scale;        // (N) or null
     const float* shift;        // (N)
     int relu;
     float* out;                // row stride ldo
     long long ldo;
     float* partial;            // (splits, rows, Np) when splits > 1
-    unsigned int* ovf = nullptr;
-    const unsigned int* run_if = nullptr;
-    const unsigned int* wflag = nullptr;
-    const float* colscale = nullptr;
+    RingArgs ring;             // W (k^3 c, Np) in the format of NP, tile width 64 NC
 };
-
-constexpr int kConvThreads = 384, kConvConsumers = 256;
-constexpr uint32_t kConvXRow = 64u * 4u + 32u;
-constexpr uint32_t kConvXBytes = 128u * kConvXRow;
-constexpr uint32_t kConvRingBudget = 206u * 1024u;
-__host__ __device__ constexpr uint32_t conv_stage_bytes(int NP, int NC) { return tc_block_bytes(64 * NC, NP) + kConvXBytes; }
-__host__ __device__ constexpr int conv_stages(int NP, int NC) {
-    return kConvRingBudget / conv_stage_bytes(NP, NC) < 4u ? (int)(kConvRingBudget / conv_stage_bytes(NP, NC)) : 4;
-}
 
 __device__ __forceinline__ void cp_async16_zfill(uint32_t smem_dst, const void* gmem_src, uint32_t src_bytes) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(smem_dst), "l"(gmem_src), "r"(src_bytes) : "memory");
 }
 
-template <int NP, int NC>
-__global__ void __launch_bounds__(kConvThreads, 1)
-tc_conv3d_kernel(const __grid_constant__ Conv3dArgs a) {
-    if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr int Nt = 64 * NC, S = conv_stages(NP, NC);
-    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = conv_stage_bytes(NP, NC);
-    static_assert(S >= 2, "the ring needs two stages");
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
-    __shared__ int s_zyx[128], s_cl[128];                           // the tile's rows: packed voxel coordinates (-1: past the end), cloud
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int CB = a.c / 64, NTC = a.Np / Nt, h = a.k / 2;
-    const long long tiles = (a.rows + 127) / 128, nunits = tiles * NTC * a.splits;
-    if (tid == 0) {
-        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 128); mbar_init(&s_empty[i], kConvConsumers / 32); }
-        fence_mbar_init();
-    }
-    __syncthreads();
+__device__ __forceinline__ int mask_active(const uint32_t* tm) {
+    return __popc(__ldg(tm)) + __popc(__ldg(tm + 1)) + __popc(__ldg(tm + 2)) + __popc(__ldg(tm + 3));
+}
 
-    if (warp >= kConvConsumers / 32) {
-        // ---- producers: warp pw gathers tile rows [32 pw, 32 pw + 32) ----
-        // 168 registers per thread at launch: the 128 x 128 the producers release are exactly the consumers' 256 x 64
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        const int pw = warp - kConvConsumers / 32;
-        uint32_t q = 0;
-        // (32-bit unit and row indices, rows < 2^31; the tile's mask re-read from L1 as the tap advances: 40 registers)
-        for (int unit = blockIdx.x; unit < (int)nunits; unit += gridDim.x) {
-            const int sp = unit % a.splits, nt = unit / a.splits % NTC, tile = unit / a.splits / NTC, row0 = tile * 128;
-            const uint32_t* tm = a.tapmask + tile * kMaskWords;
-            const int nact = (__popc(__ldg(tm)) + __popc(__ldg(tm + 1)) + __popc(__ldg(tm + 2)) + __popc(__ldg(tm + 3))) * CB;
-            const int j0 = nact * sp / a.splits, j1 = nact * (sp + 1) / a.splits;
-            if (j0 == j1) continue;
-            __syncwarp();                                            // the previous unit's reads of s_zyx are done
-            {
-                const int R = row0 + 32 * pw + lane;
-                int zyx = -1, cl = 0;
-                if (R < (int)a.rows) {
-                    const int v = R / a.b;
-                    cl = R - v * a.b;
-                    zyx = v / (a.r * a.r) << 16 | v / a.r % a.r << 8 | v % a.r;
-                }
-                s_zyx[32 * pw + lane] = zyx;
-                s_cl[32 * pw + lane] = cl;
+struct Conv3dOp {
+    const Conv3dArgs& a;
+    struct Smem {
+        int zyx[128], cl[128];                             // the unit's rows: packed voxel coordinates (-1: past the end), cloud
+    };
+    struct Unit {
+        int nb, col0, sp;
+        long long r[2];
+    };
+
+    __device__ int units(int Nt) const { return (int)((a.rows + 127) / 128 * (a.Np / Nt) * a.splits); }
+
+    // (32-bit unit and row indices, rows < 2^31; the tile's mask re-read from L1 as the tap advances: 40 registers)
+    template <class Put>
+    __device__ void produce(int unit, int Nt, int pw, int lane, Smem& sm, Put&& put) const {
+        const int CB = a.c / 64, NTC = a.Np / Nt, h = a.k / 2;
+        const int sp = unit % a.splits, nt = unit / a.splits % NTC, tile = unit / a.splits / NTC, row0 = tile * 128;
+        const uint32_t* tm = a.tapmask + tile * kMaskWords;
+        const int nact = mask_active(tm) * CB;
+        const int j0 = nact * sp / a.splits, j1 = nact * (sp + 1) / a.splits;
+        if (j0 == j1) return;
+        __syncwarp();                                      // the previous unit's reads of zyx are done
+        {
+            const int R = row0 + 32 * pw + lane;
+            int zyx = -1, cl = 0;
+            if (R < (int)a.rows) {
+                const int v = R / a.b;
+                cl = R - v * a.b;
+                zyx = v / (a.r * a.r) << 16 | v / a.r % a.r << 8 | v % a.r;
             }
-            __syncwarp();
-            int tap = -1;
-            for (int i = 0; i <= j0 / CB; ++i) tap = mask_next_g(tm, tap + 1);
-            int chunk = j0 % CB;
-            for (int j = j0; j < j1; ++j, ++q) {
-                const int s = (int)(q % S);
-                if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
-                if (pw == 0 && lane == 0) {
-                    mbar_expect_tx(&s_full[s], bb);
-                    const uint8_t* src = a.image + ((size_t)nt * a.KC + (size_t)tap * CB + chunk) * bb;
-                    for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
-                }
+            sm.zyx[32 * pw + lane] = zyx;
+            sm.cl[32 * pw + lane] = cl;
+        }
+        __syncwarp();
+        int tap = -1;
+        for (int i = 0; i <= j0 / CB; ++i) tap = mask_next_g(tm, tap + 1);
+        int chunk = j0 % CB;
+        for (int j = j0; j < j1; ++j) {
+            put((size_t)nt * a.KC + (size_t)tap * CB + chunk, [&](uint32_t xs) {
                 const int oz = tap / (a.k * a.k) - h, oy = tap / a.k % a.k - h, ox = tap % a.k - h;
                 const int cc = (lane & 15) * 4, ch = chunk * 64 + cc;
-                const uint32_t xs = smem_u32(base + (uint32_t)s * SB + bb);
                 for (int rr = lane >> 4; rr < 32; rr += 2) {
-                    const int row = 32 * pw + rr, zyx = s_zyx[row];
+                    const int row = 32 * pw + rr, zyx = sm.zyx[row];
                     const int z = (zyx >> 16) + oz, y = ((zyx >> 8) & 255) + oy, x = (zyx & 255) + ox;
                     const bool in = zyx >= 0 && z >= 0 && z < a.r && y >= 0 && y < a.r && x >= 0 && x < a.r;
-                    const float* src = in ? a.x + ((long long)((z * a.r + y) * a.r + x) * a.b + s_cl[row]) * a.ldx + ch : a.x;
-                    cp_async16_zfill(xs + (uint32_t)row * kConvXRow + (uint32_t)cc * 4u, src, in ? 16u : 0u);
+                    const float* src = in ? a.x + ((long long)((z * a.r + y) * a.r + x) * a.b + sm.cl[row]) * a.ldx + ch : a.x;
+                    cp_async16_zfill(xs + (uint32_t)row * kRingXRow + (uint32_t)cc * 4u, src, in ? 16u : 0u);
                 }
-                cp_async_mbar_arrive(&s_full[s]);
-                if (++chunk == CB) { chunk = 0; tap = mask_next_g(tm, tap + 1); }
+            });
+            if (++chunk == CB) { chunk = 0; tap = mask_next_g(tm, tap + 1); }
+        }
+    }
+
+    __device__ Unit unit(int unit, int Nt, int row) const {
+        const int NTC = a.Np / Nt;
+        Unit u;
+        u.sp = unit % a.splits;
+        u.col0 = unit / a.splits % NTC * Nt;
+        const long long tile = unit / a.splits / NTC;
+        const int nact = mask_active(a.tapmask + tile * kMaskWords) * (a.c / 64);
+        u.nb = nact * (u.sp + 1) / a.splits - nact * u.sp / a.splits;
+        u.r[0] = tile * 128 + row;
+        u.r[1] = u.r[0] + 8;
+        return u;
+    }
+
+    // a plain read: out-of-grid neighbours and rows past the end were zero-filled
+    __device__ void load(const Unit&, const float* xs, int, int t, float2 (&x)[4][2][2]) const {
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                for (int i = 0; i < 2; ++i) x[s][h][i] = staged_pair(xs, s, h, i, t);
+    }
+
+    // fp16x2 column factor; the whole sum -> scale, shift, ReLU; a split's share -> its partial
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int col = col0 + 8 * jj + 2 * t;
+            const float2 cs = colscale != nullptr ? __ldg(reinterpret_cast<const float2*>(colscale + col)) : make_float2(1.f, 1.f);
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                if (u.r[i] >= a.rows) continue;
+                float2 v = make_float2(acc[4 * jj + 2 * i] * cs.x, acc[4 * jj + 2 * i + 1] * cs.y);
+                if (a.splits > 1) {
+                    *reinterpret_cast<float2*>(a.partial + ((size_t)u.sp * a.rows + u.r[i]) * a.Np + col) = v;
+                } else if (col < a.N) {
+                    const float2 sh = __ldg(reinterpret_cast<const float2*>(a.shift + col));
+                    if (a.scale != nullptr) {
+                        const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + col));
+                        v = make_float2(fmaf(v.x, sc.x, sh.x), fmaf(v.y, sc.y, sh.y));
+                    } else {
+                        v = make_float2(v.x + sh.x, v.y + sh.y);
+                    }
+                    if (a.relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
+                    *reinterpret_cast<float2*>(a.out + (size_t)u.r[i] * a.ldo + col) = v;
+                }
             }
         }
-        return;
     }
 
-    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-    const int g = lane >> 2, t = lane & 3;
-    uint32_t ovf = 0u;
-    uint32_t q = 0;                                                 // ring uses
-    for (long long unit = blockIdx.x; unit < nunits; unit += gridDim.x) {
-        const int sp = (int)(unit % a.splits), nt = (int)(unit / a.splits % NTC);
-        const long long tile = unit / a.splits / NTC, row0 = tile * 128;
-        const uint32_t* tm = a.tapmask + tile * kMaskWords;
-        const int nact = (__popc(__ldg(tm)) + __popc(__ldg(tm + 1)) + __popc(__ldg(tm + 2)) + __popc(__ldg(tm + 3))) * CB;
-        const int nb = nact * (sp + 1) / a.splits - nact * sp / a.splits;
-        const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
-
-        // staged block of ring use u -> A fragments (out-of-grid neighbours and rows past the end were zero-filled)
-        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t u) {
-            const float* xs = reinterpret_cast<const float*>(base + (u % S) * SB + bb);
-#pragma unroll
-            for (int s = 0; s < 4; ++s)
-#pragma unroll
-                for (int hh = 0; hh < 2; ++hh) {
-                    const int kl = 16 * s + 8 * hh + 2 * t;
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const float2 x = *reinterpret_cast<const float2*>(xs + (warp * 16 + g + 8 * i) * (int)(kConvXRow / 4) + kl);
-                        uint32_t pc[NP];
-                        split_pair<NP>(x.x, x.y, pc, ovf);
-#pragma unroll
-                        for (int e = 0; e < NP; ++e) A[e][s][i + 2 * hh] = pc[e];
-                    }
-                }
-        };
-        float acc[NC][32];
-        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
-        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t u, int kb) {
-            const uint32_t wb = smem_u32(base + (u % S) * SB);
-#pragma unroll
-            for (int c0 = 0; c0 < NC; c0 += CG) {
-                float d[CG][32];
-                wg_fence();
-#pragma unroll
-                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
-#pragma unroll
-                    for (int s = 0; s < 4; ++s)
-#pragma unroll
-                        for (int c = 0; c < CG; ++c)
-                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
-                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
-                wg_commit();
-                if (c0 + CG == NC && kb + 1 < nb) {
-                    mbar_wait(&s_full[(u + 1) % S], ((u + 1) / S) & 1u);
-                    prep(An, u + 1);
-                }
-                wg_wait_all();
-                if (c0 + CG == NC) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive1(&s_empty[u % S]);
-                }
-#pragma unroll
-                for (int c = 0; c < CG; ++c) {
-                    wg_fence_acc(d[c]);
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
-                }
-            }
-        };
-        if (nb > 0) {
-            uint32_t A0[NP][4][4], A1[NP][4][4];
-            mbar_wait(&s_full[q % S], (q / S) & 1u);
-            prep(A0, q);
-            for (int kb = 0;; kb += 2) {
-                step(A0, A1, q + kb, kb);
-                if (kb + 1 == nb) break;
-                step(A1, A0, q + kb + 1, kb + 1);
-                if (kb + 2 == nb) break;
-            }
-            q += nb;
-        } else {
-#pragma unroll
-            for (int c = 0; c < NC; ++c)
-#pragma unroll
-                for (int e = 0; e < 32; ++e) acc[c][e] = 0.f;
-        }
-
-        // ---- epilogue: fp16x2 column factor; the whole sum -> scale, shift, ReLU; a split's share -> its partial ----
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                const int col = nt * Nt + c * 64 + 8 * jj + 2 * t;
-                const float2 cs = NP == 2 ? __ldg(reinterpret_cast<const float2*>(a.colscale + col)) : make_float2(1.f, 1.f);
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    if (r[i] >= a.rows) continue;
-                    float2 v = make_float2(acc[c][4 * jj + 2 * i] * cs.x, acc[c][4 * jj + 2 * i + 1] * cs.y);
-                    if (a.splits > 1) {
-                        *reinterpret_cast<float2*>(a.partial + ((size_t)sp * a.rows + r[i]) * a.Np + col) = v;
-                    } else if (col < a.N) {
-                        const float2 sh = __ldg(reinterpret_cast<const float2*>(a.shift + col));
-                        if (a.scale != nullptr) {
-                            const float2 sc = __ldg(reinterpret_cast<const float2*>(a.scale + col));
-                            v = make_float2(fmaf(v.x, sc.x, sh.x), fmaf(v.y, sc.y, sh.y));
-                        } else {
-                            v = make_float2(v.x + sh.x, v.y + sh.y);
-                        }
-                        if (a.relu) v = make_float2(fmaxf(v.x, 0.f), fmaxf(v.y, 0.f));
-                        *reinterpret_cast<float2*>(a.out + (size_t)r[i] * a.ldo + col) = v;
-                    }
-                }
-            }
+    // the FMA fallback's A, every tap
+    __device__ float load_a(long long R, int kk) const {
+        const int h = a.k / 2, tap = kk / a.c, ch = kk - tap * a.c;
+        const long long v = R / a.b;
+        const int cl = (int)(R - v * a.b);
+        const int z = (int)(v / (a.r * a.r)) + tap / (a.k * a.k) - h, y = (int)(v / a.r % a.r) + tap / a.k % a.k - h,
+                  x = (int)(v % a.r) + tap % a.k - h;
+        if (z >= 0 && z < a.r && y >= 0 && y < a.r && x >= 0 && x < a.r)
+            return __ldg(a.x + ((long long)((z * a.r + y) * a.r + x) * a.b + cl) * a.ldx + ch);
+        return 0.f;
     }
-    if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
+    __device__ void store(long long R, int col, float s) const {
+        float v = a.scale != nullptr ? fmaf(s, __ldg(a.scale + col), __ldg(a.shift + col)) : s + __ldg(a.shift + col);
+        if (a.relu) v = fmaxf(v, 0.f);
+        a.out[R * a.ldo + col] = v;
     }
+};
+
+template <int NP, int NC>
+__global__ void __launch_bounds__(kRingThreads, 1) tc_conv3d_kernel(const __grid_constant__ Conv3dArgs a) {
+    ring_gemm<NP, NC>(Conv3dOp{a}, a.ring);
 }
 
 // out = relu(sum_sp partial[sp] * scale + shift), the partials added in split order
@@ -424,8 +350,8 @@ __global__ void conv3d_finalize_kernel(long long rows, int N, int Np, int splits
     }
 }
 
-// W (K, N) -> (K, Np), columns N..Np zero
-__global__ void conv3d_pad_kernel(long long K, int N, int Np, const float* __restrict__ W, float* __restrict__ Wp) {
+// W (K, N) -> Wp (K, Np), columns N .. Np zero
+__global__ void pad_cols_kernel(long long K, int N, int Np, const float* __restrict__ W, float* __restrict__ Wp) {
     const long long total = K * Np;
     for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
         const int col = (int)(e % Np);
@@ -433,68 +359,14 @@ __global__ void conv3d_pad_kernel(long long K, int N, int Np, const float* __res
     }
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// The same layer on the fp32 FMA pipe: 64 x 64 tiles, 256 threads of 4 x 4 outputs, K in steps of 16, every tap, each 64-wide
-// K block summed on its own before it is added to the total (as the tensor path sums).
-// ------------------------------------------------------------------------------------------------------------------
+int pad_cols(long long K, int N, int Np, const float* W, float* Wp, cudaStream_t st) {
+    pad_cols_kernel<<<(unsigned)min((K * Np + 255) / 256, 1024LL), 256, 0, st>>>(K, N, Np, W, Wp);
+    return check_launch("pad_cols_kernel");
+}
+
+// the same layer on the fp32 FMA pipe
 __global__ void __launch_bounds__(256) conv3d_fma_kernel(const __grid_constant__ Conv3dArgs a, const float* __restrict__ W) {
-    __shared__ float As[16][64 + 4], Bs[16][64];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const long long row0 = (long long)blockIdx.x * 64;
-    const int col0 = blockIdx.y * 64, K = a.k * a.k * a.k * a.c, h = a.k / 2;
-    float tot[4][4] = {}, acc[4][4] = {};
-    for (int k0 = 0; k0 < K; k0 += 16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int e = tid + 256 * i, kr = e >> 6, rr = e & 63;
-            const int kk = k0 + kr;
-            const long long R = row0 + rr;
-            float val = 0.f;
-            if (kk < K && R < a.rows) {
-                const int tap = kk / a.c, ch = kk - tap * a.c;
-                const long long v = R / a.b;
-                const int cl = (int)(R - v * a.b);
-                const int z = (int)(v / (a.r * a.r)) + tap / (a.k * a.k) - h, y = (int)(v / a.r % a.r) + tap / a.k % a.k - h,
-                          x = (int)(v % a.r) + tap % a.k - h;
-                if (z >= 0 && z < a.r && y >= 0 && y < a.r && x >= 0 && x < a.r)
-                    val = __ldg(a.x + ((long long)((z * a.r + y) * a.r + x) * a.b + cl) * a.ldx + ch);
-            }
-            As[kr][rr] = val;
-            const int col = col0 + rr;
-            Bs[kr][rr] = (kk < K && col < a.N) ? __ldg(W + (size_t)kk * a.N + col) : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kr = 0; kr < 16; ++kr) {
-            float av[4], bv[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { av[i] = As[kr][ty * 4 + i]; bv[i] = Bs[kr][tx * 4 + i]; }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) acc[i][jj] = fmaf(av[i], bv[jj], acc[i][jj]);
-        }
-        __syncthreads();
-        if ((k0 & 63) == 48 || k0 + 16 >= K) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) { tot[i][jj] += acc[i][jj]; acc[i][jj] = 0.f; }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long long R = row0 + ty * 4 + i;
-        if (R >= a.rows) continue;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int col = col0 + tx * 4 + jj;
-            if (col >= a.N) continue;
-            float v = a.scale != nullptr ? fmaf(tot[i][jj], __ldg(a.scale + col), __ldg(a.shift + col)) : tot[i][jj] + __ldg(a.shift + col);
-            if (a.relu) v = fmaxf(v, 0.f);
-            a.out[R * a.ldo + col] = v;
-        }
-    }
+    fma_gemm(Conv3dOp{a}, a.rows, a.k * a.k * a.k * a.c, a.N, W);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -557,7 +429,6 @@ struct ConvPlan {
     long long tiles;
     size_t mask, wpad, img, partial, total;
 };
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 // Tile width: 128 when Np allows it and the 128-wide tiles alone fill more than half of the SMs.  Splits: as many as keep
 // tiles * column tiles * splits within one wave, at most 16, and at most half the K blocks a tile can have active.
 // Workspace for np weight pieces (tc_np()): np = 3 holds the bf16x3 image; np = 2 holds the fp16x2 image, and the bf16x3 image of
@@ -586,21 +457,9 @@ static ConvPlan conv_plan(int b, int r, int k, int c, int N, int np) {
     return p;
 }
 
-template <int NP, int NC>
-static int launch_conv_shape(const Conv3dArgs& a, cudaStream_t st) {
-    const size_t smem = (size_t)conv_stages(NP, NC) * conv_stage_bytes(NP, NC) + 1024;
-    PSA_CUDA(cudaFuncSetAttribute(tc_conv3d_kernel<NP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, sms = 0;
-    PSA_CUDA(cudaGetDevice(&dev));
-    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const long long units = (a.rows + 127) / 128 * (a.Np / (64 * NC)) * a.splits;
-    tc_conv3d_kernel<NP, NC><<<(unsigned)(units < sms ? units : sms), kConvThreads, smem, st>>>(a);
-    return check_launch("tc_conv3d_kernel");
-}
-template <int NP>
-static int launch_conv_np(const Conv3dArgs& a, int Nt, cudaStream_t st) {
-    return Nt == 128 ? launch_conv_shape<NP, 2>(a, st) : launch_conv_shape<NP, 1>(a, st);
-}
+static const RingKernels kConvRing = {{{(const void*)tc_conv3d_kernel<2, 1>, (const void*)tc_conv3d_kernel<2, 2>},
+                                       {(const void*)tc_conv3d_kernel<3, 1>, (const void*)tc_conv3d_kernel<3, 2>}},
+                                      "tc_conv3d_kernel"};
 
 }  // namespace psa
 
@@ -637,7 +496,7 @@ extern "C" int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const flo
     cudaStream_t st = as_stream(stream);
     Conv3dArgs a;
     a.rows = (long long)b * r * r * r; a.b = b; a.r = r; a.k = k; a.c = c; a.N = c_out; a.Np = c_out; a.splits = 1;
-    a.KC = k * k * k * c / 64; a.x = x; a.ldx = ldx; a.tapmask = nullptr; a.image = nullptr; a.scale = scale; a.shift = shift;
+    a.KC = k * k * k * c / 64; a.x = x; a.ldx = ldx; a.tapmask = nullptr; a.scale = scale; a.shift = shift;
     a.relu = relu ? 1 : 0; a.out = out; a.ldo = ldo; a.partial = nullptr;
     if (mlp_mode() == 1 || !conv_tc_shape(c, c_out) || !conv_tc_aligned(x, ldx, scale, shift, out, ldo)) {
         const dim3 grid((unsigned)((a.rows + 63) / 64), (unsigned)((c_out + 63) / 64));
@@ -658,36 +517,15 @@ extern "C" int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const flo
     const float* wsrc = W;
     if (pl.Np != c_out) {
         float* wp = reinterpret_cast<float*>(wsb + pl.wpad);
-        conv3d_pad_kernel<<<1024, 256, 0, st>>>(K, c_out, pl.Np, W, wp);
-        rc = check_launch("conv3d_pad_kernel");
+        rc = pad_cols(K, c_out, pl.Np, W, wp, st);
         if (rc != PSA_OK) return rc;
         wsrc = wp;
     }
     a.tapmask = mask;
     a.splits = pl.splits;
     a.partial = pl.splits > 1 ? reinterpret_cast<float*>(wsb + pl.partial) : nullptr;
-    const int Nt = pl.Nt | image_flag(tc_np());
-    uint8_t* img3 = wsb + pl.img;
-    if (tc_np() == 3) {
-        rc = build_image(K, K, pl.Np, Nt, wsrc, img3, st);
-        if (rc != PSA_OK) return rc;
-        a.image = img3;
-        rc = launch_conv_np<3>(a, pl.Nt, st);
-    } else {
-        unsigned int* flag = reinterpret_cast<unsigned int*>(wsb);
-        PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
-        uint8_t* img2 = wsb + pl.img;
-        rc = build_image(K, K, pl.Np, Nt, wsrc, img2, st);
-        if (rc != PSA_OK) return rc;
-        a.image = img2; a.ovf = flag; a.wflag = image_trailer(img2, K, pl.Np); a.colscale = image_colscale(img2, K, pl.Np);
-        rc = launch_conv_np<2>(a, pl.Nt, st);
-        if (rc != PSA_OK) return rc;
-        // guarded rerun on bf16x3 operands: its image and its launch are no-ops unless the fp16x2 pass raised the flag
-        rc = build_image(K, K, pl.Np, pl.Nt | kImageBf16x3, wsrc, img3, st, flag);
-        if (rc != PSA_OK) return rc;
-        a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = flag;
-        rc = launch_conv_np<3>(a, pl.Nt, st);
-    }
+    rc = ring_run(kConvRing, a, pl.tiles * (pl.Np / pl.Nt) * pl.splits, K, K, pl.Np, pl.Nt, wsrc, wsb + pl.img, wsb + pl.img,
+                  reinterpret_cast<unsigned int*>(wsb), st);
     if (rc != PSA_OK || pl.splits == 1) return rc;
     const long long total = a.rows * c_out;
     conv3d_finalize_kernel<<<(unsigned)min((total + 255) / 256, 8192LL), 256, 0, st>>>(a.rows, c_out, pl.Np, pl.splits, a.partial, scale, shift,

@@ -9,15 +9,13 @@
 //                          canonical fp32 evaluation of oracle/psa_oracle.c:orc_dgcnn_knn, and writes every D-th entry
 //   xconv_core_kernel      per tile of queries, everything up to the depthwise stage of the separable conv in shared memory and
 //                          registers: only the (B*P, C_in*dm) depthwise output reaches global memory
-//   tc_pcnn_dense_kernel   out = elu(x . W [+ bias]) * scale + shift through row strides, on the tensor cores: tc_spider_kernel's
-//                          ring (a producer warpgroup stages x rows by cp.async, two consumer warpgroups split them into Split<NP>
-//                          operands), K padded to 64 by zero operand columns, W padded to a 64- or 128-wide image
+//   tc_pcnn_dense_kernel   out = elu(x . W [+ bias]) * scale + shift through row strides, on the tensor cores: the shared ring
+//                          (ring_gemm.cuh) staging x rows, K padded to 64 by zero operand columns, W padded to a 64- or 128-wide image
 //   pcnn_dense_fma_kernel  the same on the fp32 FMA pipe (mode 1, K % 4 != 0, rows < 128, unaligned x)
 #include <float.h>
 
 #include "common.cuh"
-#include "mlp_internal.cuh"
-#include "tc_common.cuh"
+#include "ring_gemm.cuh"
 
 namespace psa {
 
@@ -205,267 +203,113 @@ __global__ void __launch_bounds__(kXconvThreads) xconv_core_kernel(const __grid_
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// tc_pcnn_dense_kernel<NP, NC>: out (rows, N) = elu(x . W + bias) * scale + shift over 128-row x 64 NC-channel tiles, persistent.
-// tc_spider_kernel's CTA and ring: two consumer warpgroups (rows 0-63 / 64-127) and a producer warpgroup whose four warps each
-// stage 32 rows of every 64-wide K block by cp.async (16 bytes per copy, chunks past K not copied) while warp 0 drops the block's
-// weights in by TMA.  The consumers read the columns past K as zero.
+// tc_pcnn_dense_kernel<NP, NC>: out (rows, N) = elu(x . W + bias) * scale + shift on the ring (ring_gemm.cuh), unit = 128-row tile x
+// 64 NC-column tile, all Kp / 64 K blocks.  The producers stage x rows (16 bytes per copy, chunks past K not copied); the consumers
+// read the columns past K as zero.
 // ------------------------------------------------------------------------------------------------------------------
 struct PcnnDenseArgs {
     long long rows, ldx, ldo;
     int K, Kp, N, Np;
     const float* x;            // 16-byte aligned, ldx % 4 == 0 on the tensor path
-    const uint8_t* image;      // W padded to (Kp, Np), format of NP, tile width 64 NC
     const float* bias;         // (N) or null
     const float* scale;        // (N)
     const float* shift;        // (N)
     float* out;
-    unsigned int* ovf = nullptr;            // np = 2: raised when an operand left the fp16 range or a weight is not finite
-    const unsigned int* run_if = nullptr;   // non-null: no-op unless *run_if != 0
-    const unsigned int* wflag = nullptr;
-    const float* colscale = nullptr;
+    RingArgs ring;             // W padded to (Kp, Np), format of NP, tile width 64 NC
 };
 
-constexpr int kPdThreads = 384, kPdConsumers = 256;
-constexpr uint32_t kPdXRow = 64u * 4u + 32u;               // as tc_dense_kernel: conflict-free fragment reads
-constexpr uint32_t kPdXBytes = 128u * kPdXRow;
-constexpr uint32_t kPdRingBudget = 206u * 1024u;
-__host__ __device__ constexpr uint32_t pd_stage_bytes(int NP, int NC) { return tc_block_bytes(64 * NC, NP) + kPdXBytes; }
-__host__ __device__ constexpr int pd_stages(int NP, int NC) {
-    return kPdRingBudget / pd_stage_bytes(NP, NC) < 4u ? (int)(kPdRingBudget / pd_stage_bytes(NP, NC)) : 4;
-}
+struct PcnnDenseOp {
+    const PcnnDenseArgs& a;
+    struct Smem {};
+    struct Unit {
+        int nb, col0;
+        long long r[2];
+        bool v[2];
+    };
+
+    __device__ int units(int Nt) const { return (int)((a.rows + 127) / 128 * (a.Np / Nt)); }
+
+    template <class Put>
+    __device__ void produce(int unit, int Nt, int pw, int lane, Smem&, Put&& put) const {
+        const int NTC = a.Np / Nt, KC = a.Kp / 64;
+        const long long row0 = (long long)(unit / NTC) * 128;
+        const int nt = unit % NTC, r0 = 32 * pw, nr = (int)max(0LL, min(32LL, a.rows - row0 - r0));
+        for (int kb = 0; kb < KC; ++kb)
+            put((size_t)nt * KC + kb, [&](uint32_t xs) {
+                const int cc = (lane & 15) * 4, kk = kb * 64 + cc;
+                if (kk >= a.K) return;
+                for (int r = lane >> 4; r < nr; r += 2) {
+                    const int row = r0 + r;
+                    cp_async16(xs + (uint32_t)row * kRingXRow + (uint32_t)cc * 4u, a.x + (size_t)(row0 + row) * a.ldx + kk);
+                }
+            });
+    }
+
+    __device__ Unit unit(int unit, int Nt, int row) const {
+        const int NTC = a.Np / Nt;
+        Unit u;
+        u.nb = a.Kp / 64;
+        u.col0 = unit % NTC * Nt;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            u.r[i] = (long long)(unit / NTC) * 128 + row + 8 * i;
+            u.v[i] = u.r[i] < a.rows;
+        }
+        return u;
+    }
+
+    // rows past `rows` and columns past K read as zero (their staged bytes are stale)
+    __device__ void load(const Unit& u, const float* xs, int kb, int t, float2 (&x)[4][2][2]) const {
+#pragma unroll
+        for (int s = 0; s < 4; ++s)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const bool kin = kb * 64 + 16 * s + 8 * h + 2 * t < a.K;     // K % 4 == 0: both columns of the pair or neither
+#pragma unroll
+                for (int i = 0; i < 2; ++i) x[s][h][i] = u.v[i] && kin ? staged_pair(xs, s, h, i, t) : make_float2(0.f, 0.f);
+            }
+    }
+
+    // fp16x2 column factor, bias, ELU, the batch-norm affine; only the N real columns are written
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int col = col0 + 8 * jj + 2 * t;
+            float cs[2] = {1.f, 1.f}, bi[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f}, sh[2] = {0.f, 0.f};
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+                if (col + h < a.N) {
+                    if (colscale != nullptr) cs[h] = __ldg(colscale + col + h);
+                    if (a.bias != nullptr) bi[h] = __ldg(a.bias + col + h);
+                    sc[h] = __ldg(a.scale + col + h);
+                    sh[h] = __ldg(a.shift + col + h);
+                }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                float* o = a.out + (size_t)u.r[i] * a.ldo + col;
+                const float y0 = fmaf(elu(fmaf(acc[4 * jj + 2 * i], cs[0], bi[0])), sc[0], sh[0]);
+                const float y1 = fmaf(elu(fmaf(acc[4 * jj + 2 * i + 1], cs[1], bi[1])), sc[1], sh[1]);
+                if (u.v[i] && col < a.N) o[0] = y0;
+                if (u.v[i] && col + 1 < a.N) o[1] = y1;
+            }
+        }
+    }
+
+    __device__ float load_a(long long p, int kk) const { return __ldg(a.x + p * a.ldx + kk); }
+    __device__ void store(long long p, int col, float s) const {
+        const float bi = a.bias != nullptr ? __ldg(a.bias + col) : 0.f;
+        a.out[(size_t)p * a.ldo + col] = fmaf(elu(s + bi), __ldg(a.scale + col), __ldg(a.shift + col));
+    }
+};
 
 template <int NP, int NC>
-__global__ void __launch_bounds__(kPdThreads, 1)
-tc_pcnn_dense_kernel(const __grid_constant__ PcnnDenseArgs a) {
-    if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr int Nt = 64 * NC, S = pd_stages(NP, NC);
-    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = pd_stage_bytes(NP, NC);
-    static_assert(S >= 2, "the ring needs two stages");
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
-    __shared__ int s_tile[S];
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int KC = a.Kp / 64, NTC = a.Np / Nt;
-    const long long ntiles = (a.rows + 127) / 128 * NTC;
-    if (tid == 0) {
-        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 128); mbar_init(&s_empty[i], kPdConsumers / 32); }
-        fence_mbar_init();
-    }
-    __syncthreads();
-
-    if (warp >= kPdConsumers / 32) {
-        // ---- producers: warp pw stages tile rows [32 pw, 32 pw + 32) ----
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        const int pw = warp - kPdConsumers / 32;
-        uint32_t q = 0;
-        for (long long tile = blockIdx.x;; tile += gridDim.x) {
-            const bool done = tile >= ntiles;
-            const long long row0 = tile / NTC * 128;
-            const int nt = (int)(tile % NTC);
-            const int r0 = 32 * pw, nr = done ? 0 : (int)max(0LL, min(32LL, a.rows - row0 - r0));
-            for (int kb = 0; kb < KC; ++kb, ++q) {
-                const int s = (int)(q % S);
-                if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
-                if (pw == 0 && lane == 0) {
-                    s_tile[s] = done ? -1 : (int)tile;
-                    if (done) {
-                        mbar_arrive1(&s_full[s]);
-                    } else {
-                        mbar_expect_tx(&s_full[s], bb);
-                        const uint8_t* src = a.image + ((size_t)nt * KC + kb) * bb;
-                        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
-                    }
-                }
-                if (!done) {
-                    const int cc = (lane & 15) * 4, kk = kb * 64 + cc;
-                    if (kk < a.K) {
-                        const uint32_t xs = smem_u32(base + (uint32_t)s * SB + bb);
-                        for (int r = lane >> 4; r < nr; r += 2) {
-                            const int row = r0 + r;
-                            cp_async16(xs + (uint32_t)row * kPdXRow + (uint32_t)cc * 4u, a.x + (size_t)(row0 + row) * a.ldx + kk);
-                        }
-                    }
-                }
-                cp_async_mbar_arrive(&s_full[s]);
-                if (done) break;
-            }
-            if (done) return;
-        }
-    }
-
-    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-    const int g = lane >> 2, t = lane & 3;
-    uint32_t ovf = 0u;
-    uint32_t q = 0;
-    for (;;) {
-        mbar_wait(&s_full[q % S], (q / S) & 1u);
-        const int tile = s_tile[q % S];
-        if (tile < 0) break;
-        const long long row0 = (long long)(tile / NTC) * 128;
-        const int nt = tile % NTC;
-        const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
-        const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
-
-        // staged block of ring use u -> A fragments; rows past `rows` and columns past K read as zero (their bytes are stale)
-        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t u, int kb) {
-            const float* xs = reinterpret_cast<const float*>(base + (u % S) * SB + bb);
-#pragma unroll
-            for (int s = 0; s < 4; ++s)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int kl = 16 * s + 8 * h + 2 * t;
-                    const bool kin = kb * 64 + kl < a.K;          // K % 4 == 0: both columns of the pair or neither
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        float2 x = make_float2(0.f, 0.f);
-                        if (v[i] && kin) x = *reinterpret_cast<const float2*>(xs + (warp * 16 + g + 8 * i) * (int)(kPdXRow / 4) + kl);
-                        uint32_t pc[NP];
-                        split_pair<NP>(x.x, x.y, pc, ovf);
-#pragma unroll
-                        for (int e = 0; e < NP; ++e) A[e][s][i + 2 * h] = pc[e];
-                    }
-                }
-        };
-        float acc[NC][32];
-        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
-        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t u, int kb) {
-            const uint32_t wb = smem_u32(base + (u % S) * SB);
-#pragma unroll
-            for (int c0 = 0; c0 < NC; c0 += CG) {
-                float d[CG][32];
-                wg_fence();
-#pragma unroll
-                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
-#pragma unroll
-                    for (int s = 0; s < 4; ++s)
-#pragma unroll
-                        for (int c = 0; c < CG; ++c)
-                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
-                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
-                wg_commit();
-                if (c0 + CG == NC && kb + 1 < KC) {
-                    mbar_wait(&s_full[(u + 1) % S], ((u + 1) / S) & 1u);
-                    prep(An, u + 1, kb + 1);
-                }
-                wg_wait_all();
-                if (c0 + CG == NC) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive1(&s_empty[u % S]);
-                }
-#pragma unroll
-                for (int c = 0; c < CG; ++c) {
-                    wg_fence_acc(d[c]);
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
-                }
-            }
-        };
-        {
-            uint32_t A0[NP][4][4], A1[NP][4][4];
-            prep(A0, q, 0);
-            for (int kb = 0;; kb += 2) {
-                step(A0, A1, q + kb, kb);
-                if (kb + 1 == KC) break;
-                step(A1, A0, q + kb + 1, kb + 1);
-                if (kb + 2 == KC) break;
-            }
-        }
-        q += KC;
-
-        // ---- epilogue: fp16x2 column factor, bias, ELU, the batch-norm affine; only the N real columns are written ----
-        // one 64-column chunk at a time, the chunk's accumulators passed by reference (a loop over chunks indexes acc through the stack)
-        auto epilogue = [&](const float (&ac)[32], int c) {
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                const int col = nt * Nt + c * 64 + 8 * jj + 2 * t;
-                float cs[2] = {1.f, 1.f}, bi[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f}, sh[2] = {0.f, 0.f};
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-                    if (col + h < a.N) {
-                        if (NP == 2) cs[h] = __ldg(a.colscale + col + h);
-                        if (a.bias != nullptr) bi[h] = __ldg(a.bias + col + h);
-                        sc[h] = __ldg(a.scale + col + h);
-                        sh[h] = __ldg(a.shift + col + h);
-                    }
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    float* o = a.out + (size_t)r[i] * a.ldo + col;
-                    const float y0 = fmaf(elu(fmaf(ac[4 * jj + 2 * i], cs[0], bi[0])), sc[0], sh[0]);
-                    const float y1 = fmaf(elu(fmaf(ac[4 * jj + 2 * i + 1], cs[1], bi[1])), sc[1], sh[1]);
-                    if (v[i] && col < a.N) o[0] = y0;
-                    if (v[i] && col + 1 < a.N) o[1] = y1;
-                }
-            }
-        };
-        epilogue(acc[0], 0);
-        if constexpr (NC == 2) epilogue(acc[1], 1);
-    }
-    if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
-    }
+__global__ void __launch_bounds__(kRingThreads, 1) tc_pcnn_dense_kernel(const __grid_constant__ PcnnDenseArgs a) {
+    ring_gemm<NP, NC>(PcnnDenseOp{a}, a.ring);
 }
 
-// The same on the fp32 FMA pipe: 64 x 64 tiles, 256 threads of 4 x 4 outputs, K in steps of 16, each 64-wide K block summed on
-// its own before it is added to the total (as the tensor path sums).
+// the same on the fp32 FMA pipe
 __global__ void __launch_bounds__(256) pcnn_dense_fma_kernel(const __grid_constant__ PcnnDenseArgs a, const float* __restrict__ W) {
-    __shared__ float As[16][64 + 4], Bs[16][64];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const long long row0 = (long long)blockIdx.x * 64;
-    const int col0 = blockIdx.y * 64;
-    float tot[4][4] = {}, part[4][4] = {};
-    for (int k0 = 0; k0 < a.K; k0 += 16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int e = tid + 256 * i, kr = e >> 6, rr = e & 63;
-            const int kk = k0 + kr;
-            const long long p = row0 + rr;
-            As[kr][rr] = (kk < a.K && p < a.rows) ? __ldg(a.x + p * a.ldx + kk) : 0.f;
-            const int col = col0 + rr;
-            Bs[kr][rr] = (kk < a.K && col < a.N) ? __ldg(W + (size_t)kk * a.N + col) : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kr = 0; kr < 16; ++kr) {
-            float av[4], bv[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { av[i] = As[kr][ty * 4 + i]; bv[i] = Bs[kr][tx * 4 + i]; }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) part[i][jj] = fmaf(av[i], bv[jj], part[i][jj]);
-        }
-        __syncthreads();
-        if ((k0 & 63) == 48 || k0 + 16 >= a.K) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) { tot[i][jj] += part[i][jj]; part[i][jj] = 0.f; }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long long p = row0 + ty * 4 + i;
-        if (p >= a.rows) continue;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int col = col0 + tx * 4 + jj;
-            if (col < a.N) {
-                const float bi = a.bias != nullptr ? __ldg(a.bias + col) : 0.f;
-                a.out[(size_t)p * a.ldo + col] = fmaf(elu(tot[i][jj] + bi), __ldg(a.scale + col), __ldg(a.shift + col));
-            }
-        }
-    }
-}
-
-// W (K, N) -> Wp (K, Np), columns N .. Np zero
-__global__ void pcnn_pad_cols_kernel(int K, int N, int Np, const float* __restrict__ W, float* __restrict__ Wp) {
-    const long long total = (long long)K * Np;
-    for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        const int col = (int)(e % Np);
-        Wp[e] = col < N ? __ldg(W + e / Np * N + col) : 0.f;
-    }
+    fma_gemm(PcnnDenseOp{a}, a.rows, a.K, a.N, W);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -481,7 +325,6 @@ struct PdPlan {
     int Kp, Np, Nt;
     size_t wp, img2, img3, total;
 };
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 static PdPlan pd_plan(int K, int N, int np) {
     PdPlan p{};
     p.Kp = (K + 63) / 64 * 64;
@@ -496,21 +339,9 @@ static PdPlan pd_plan(int K, int N, int np) {
     return p;
 }
 
-template <int NP, int NC>
-static int launch_pd_shape(const PcnnDenseArgs& a, cudaStream_t st) {
-    const size_t smem = (size_t)pd_stages(NP, NC) * pd_stage_bytes(NP, NC) + 1024;
-    PSA_CUDA(cudaFuncSetAttribute(tc_pcnn_dense_kernel<NP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, sms = 0;
-    PSA_CUDA(cudaGetDevice(&dev));
-    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const long long tiles = (a.rows + 127) / 128 * (a.Np / (64 * NC));
-    tc_pcnn_dense_kernel<NP, NC><<<(unsigned)(tiles < sms ? tiles : sms), kPdThreads, smem, st>>>(a);
-    return check_launch("tc_pcnn_dense_kernel");
-}
-template <int NP>
-static int launch_pd_np(const PcnnDenseArgs& a, int Nt, cudaStream_t st) {
-    return Nt == 128 ? launch_pd_shape<NP, 2>(a, st) : launch_pd_shape<NP, 1>(a, st);
-}
+static const RingKernels kPdRing = {{{(const void*)tc_pcnn_dense_kernel<2, 1>, (const void*)tc_pcnn_dense_kernel<2, 2>},
+                                     {(const void*)tc_pcnn_dense_kernel<3, 1>, (const void*)tc_pcnn_dense_kernel<3, 2>}},
+                                    "tc_pcnn_dense_kernel"};
 
 static int xconv_qt(int K, int Cf, int Cin) {
     const int q = kXconvSmemBudget / (xconv_query_floats(K, Cf, Cin) * (int)sizeof(float));
@@ -578,7 +409,6 @@ extern "C" int psa_dense_elu_affine(long long rows, int K, int N, const float* x
     cudaStream_t st = as_stream(stream);
     PcnnDenseArgs a;
     a.rows = rows; a.ldx = ldx; a.ldo = ldo; a.K = K; a.N = N; a.x = x; a.bias = bias; a.scale = scale; a.shift = shift; a.out = out;
-    a.image = nullptr;
     if (mlp_mode() == 1 || !pd_tc_eligible(rows, K, ldx, x)) {
         a.Kp = K; a.Np = N;
         const dim3 grid((unsigned)((rows + 63) / 64), (unsigned)((N + 63) / 64));
@@ -592,27 +422,8 @@ extern "C" int psa_dense_elu_affine(long long rows, int K, int N, const float* x
     uint8_t* wsb = reinterpret_cast<uint8_t*>(workspace);
     a.Kp = pl.Kp; a.Np = pl.Np;
     float* wp = reinterpret_cast<float*>(wsb + pl.wp);
-    pcnn_pad_cols_kernel<<<256, 256, 0, st>>>(K, N, pl.Np, W, wp);
-    int rc = check_launch("pcnn_pad_cols_kernel");
+    const int rc = pad_cols(K, N, pl.Np, W, wp, st);
     if (rc != PSA_OK) return rc;
-    uint8_t* img3 = wsb + pl.img3;
-    if (tc_np() == 3) {
-        rc = build_image(K, pl.Kp, pl.Np, pl.Nt | kImageBf16x3, wp, img3, st);
-        if (rc != PSA_OK) return rc;
-        a.image = img3;
-        return launch_pd_np<3>(a, pl.Nt, st);
-    }
-    unsigned int* flag = reinterpret_cast<unsigned int*>(wsb);
-    PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
-    uint8_t* img2 = wsb + pl.img2;
-    rc = build_image(K, pl.Kp, pl.Np, pl.Nt | kImageF16x2, wp, img2, st);
-    if (rc != PSA_OK) return rc;
-    a.image = img2; a.ovf = flag; a.wflag = image_trailer(img2, pl.Kp, pl.Np); a.colscale = image_colscale(img2, pl.Kp, pl.Np);
-    rc = launch_pd_np<2>(a, pl.Nt, st);
-    if (rc != PSA_OK) return rc;
-    // guarded rerun on bf16x3 operands: its image and its launch are no-ops unless the fp16x2 pass raised the flag
-    rc = build_image(K, pl.Kp, pl.Np, pl.Nt | kImageBf16x3, wp, img3, st, flag);
-    if (rc != PSA_OK) return rc;
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = flag;
-    return launch_pd_np<3>(a, pl.Nt, st);
+    return ring_run(kPdRing, a, (rows + 127) / 128 * (pl.Np / pl.Nt), K, pl.Kp, pl.Np, pl.Nt, wp, wsb + pl.img2, wsb + pl.img3,
+                    reinterpret_cast<unsigned int*>(wsb), st);
 }

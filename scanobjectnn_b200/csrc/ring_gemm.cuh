@@ -1,0 +1,268 @@
+// ring_gemm.cuh -- the warp-specialised tensor-core GEMM shared by spiderConv (spider.cu), conv3d (mfv.cu) and PointCNN's dense
+// layers (pointcnn.cu), its fp32-FMA fallback, and the host sequence that runs it under the fp16x2 range guard.
+//
+// ring_gemm<NP, NC>(op, ring): per work unit, a 128-row x 64 NC-column tile of A . W, with A staged by the op.  Persistent: producers
+// and consumers both walk units blockIdx.x, blockIdx.x + gridDim.x, ..., and a unit may have no K blocks.
+// CTA = two consumer warpgroups (rows 0-63 / 64-127) + a producer warpgroup whose four warps each stage 32 rows of every 64-wide K
+// block by cp.async while warp 0 also drops the block's weights in by TMA.  The consumers' K loop is tc_dense_kernel's (tc_mlp.cu):
+// per block one wgmma group on the registers prepared under the previous one, the block's sum added to fp32 accumulators (no
+// tensor-core accumulation over more than 64 K).  168 registers per thread at launch: the 128 x 128 the producers release
+// (setmaxnreg 40) are exactly the 256 x 64 the consumers take (232).
+//
+// The op supplies what differs (Op::Smem is its per-unit shared table, Unit its per-unit consumer state):
+//   int units(int Nt)                                         work units for Nt-wide column tiles
+//   produce(unit, Nt, pw, lane, Smem&, put)                   producer warp pw's share of a unit: for each K block in order,
+//                                                             put(image block, stage) with stage(xs) issuing the cp.async copies
+//                                                             of the warp's 32 rows into the staged block at shared address xs
+//   Unit unit(unit, Nt, row)                                  .nb K blocks, .col0 first column; the thread's rows are row, row + 8
+//   load(u, xs, kb, t, x)                                     staged block kb -> the A operand's values x[s][h][i] of the thread:
+//                                                             row + 8 i, block columns 16 s + 8 h + 2 t, + 1 (staged_pair)
+//   epilogue(u, acc, col, t, colscale)                        a 64-column chunk of sums from column col (colscale: fp16x2 only)
+// and for the FMA fallback, fma_gemm(op, ...): float load_a(row, k) and store(row, col, sum).
+#pragma once
+#include "common.cuh"
+#include "mlp_internal.cuh"
+#include "tc_common.cuh"
+
+namespace psa {
+
+// the fields every ring launch carries: the weight image and the fp16x2 range guard (Split<NP>, tc_common.cuh)
+struct RingArgs {
+    const uint8_t* image = nullptr;         // W in the format of NP, tile width 64 NC
+    unsigned int* ovf = nullptr;            // np = 2: raised when an operand left the fp16 range or a weight is not finite
+    const unsigned int* run_if = nullptr;   // non-null: no-op unless *run_if != 0
+    const unsigned int* wflag = nullptr;    // np = 2: the image's non-finite-weight word
+    const float* colscale = nullptr;        // np = 2: the image's column factors
+};
+
+constexpr int kRingThreads = 384, kRingConsumers = 256;
+constexpr uint32_t kRingXRow = 64u * 4u + 32u;            // as tc_dense_kernel: conflict-free fragment reads
+constexpr uint32_t kRingXBytes = 128u * kRingXRow;
+constexpr uint32_t kRingBudget = 206u * 1024u;
+__host__ __device__ constexpr uint32_t ring_stage_bytes(int NP, int NC) { return tc::tc_block_bytes(64 * NC, NP) + kRingXBytes; }
+__host__ __device__ constexpr int ring_stages(int NP, int NC) {
+    return kRingBudget / ring_stage_bytes(NP, NC) < 4u ? (int)(kRingBudget / ring_stage_bytes(NP, NC)) : 4;
+}
+
+// the staged pair of row + 8 i, block columns 16 s + 8 h + 2 t, + 1; xs = the staged block's row `row`
+__device__ __forceinline__ float2 staged_pair(const float* xs, int s, int h, int i, int t) {
+    return *reinterpret_cast<const float2*>(xs + 8 * i * (int)(kRingXRow / 4) + 16 * s + 8 * h + 2 * t);
+}
+
+template <int NP, int NC, class Op>
+__device__ __forceinline__ void ring_gemm(const Op& op, const RingArgs& ra) {
+    using namespace tc;
+    if (ra.run_if != nullptr && *ra.run_if == 0u) return;
+    constexpr int Nt = 64 * NC, S = ring_stages(NP, NC);
+    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = ring_stage_bytes(NP, NC);
+    static_assert(S >= 2, "the ring needs two stages");
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
+    __shared__ typename Op::Smem s_op;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+    const int units = op.units(Nt);
+    if (tid == 0) {
+        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 128); mbar_init(&s_empty[i], kRingConsumers / 32); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp >= kRingConsumers / 32) {
+        // ---- producers: warp pw stages tile rows [32 pw, 32 pw + 32) ----
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
+        const int pw = warp - kRingConsumers / 32;
+        uint32_t q = 0;                                             // ring uses
+        auto put = [&](size_t block, auto&& stage) {
+            const int s = (int)(q % S);
+            if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
+            if (pw == 0 && lane == 0) {
+                mbar_expect_tx(&s_full[s], bb);
+                const uint8_t* src = ra.image + block * bb;
+                for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
+            }
+            stage(smem_u32(base + (uint32_t)s * SB + bb));
+            cp_async_mbar_arrive(&s_full[s]);
+            ++q;
+        };
+        for (int unit = blockIdx.x; unit < units; unit += gridDim.x) op.produce(unit, Nt, pw, lane, s_op, put);
+        return;
+    }
+
+    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
+    const int g = lane >> 2, t = lane & 3, row = warp * 16 + g;
+    uint32_t ovf = 0u;
+    uint32_t q = 0;                                                 // ring uses
+    for (int unit = blockIdx.x; unit < units; unit += gridDim.x) {
+        const auto u = op.unit(unit, Nt, row);
+
+        // staged block of ring use `use` -> the op's values -> A fragments
+        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t use, int kb) {
+            const float* xs = reinterpret_cast<const float*>(base + (use % S) * SB + bb) + row * (int)(kRingXRow / 4);
+            float2 x[4][2][2];
+            op.load(u, xs, kb, t, x);
+#pragma unroll
+            for (int s = 0; s < 4; ++s)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        uint32_t pc[NP];
+                        split_pair<NP>(x[s][h][i].x, x[s][h][i].y, pc, ovf);
+#pragma unroll
+                        for (int e = 0; e < NP; ++e) A[e][s][i + 2 * h] = pc[e];
+                    }
+        };
+        float acc[NC][32];
+        // tc_dense_kernel's step: issue block kb's group on A, prepare block kb + 1 into An while it runs, wait, release, add
+        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
+        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t use, int kb) {
+            const uint32_t wb = smem_u32(base + (use % S) * SB);
+#pragma unroll
+            for (int c0 = 0; c0 < NC; c0 += CG) {
+                float d[CG][32];
+                wg_fence();
+#pragma unroll
+                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
+#pragma unroll
+                    for (int s = 0; s < 4; ++s)
+#pragma unroll
+                        for (int c = 0; c < CG; ++c)
+                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
+                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
+                wg_commit();
+                if (c0 + CG == NC && kb + 1 < u.nb) {
+                    mbar_wait(&s_full[(use + 1) % S], ((use + 1) / S) & 1u);
+                    prep(An, use + 1, kb + 1);
+                }
+                wg_wait_all();
+                if (c0 + CG == NC) {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive1(&s_empty[use % S]);
+                }
+#pragma unroll
+                for (int c = 0; c < CG; ++c) {
+                    wg_fence_acc(d[c]);
+#pragma unroll
+                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
+                }
+            }
+        };
+        if (u.nb > 0) {
+            uint32_t A0[NP][4][4], A1[NP][4][4];
+            mbar_wait(&s_full[q % S], (q / S) & 1u);
+            prep(A0, q, 0);
+            for (int kb = 0;; kb += 2) {
+                step(A0, A1, q + kb, kb);
+                if (kb + 1 == u.nb) break;
+                step(A1, A0, q + kb + 1, kb + 1);
+                if (kb + 2 == u.nb) break;
+            }
+            q += u.nb;
+        } else {
+#pragma unroll
+            for (int c = 0; c < NC; ++c)
+#pragma unroll
+                for (int e = 0; e < 32; ++e) acc[c][e] = 0.f;
+        }
+        // one 64-column chunk at a time, its accumulators passed by reference (a loop over chunks indexes acc through the stack)
+        const float* cs = NP == 2 ? ra.colscale : nullptr;
+        op.epilogue(u, acc[0], u.col0, t, cs);
+        if constexpr (NC == 2) op.epilogue(u, acc[1], u.col0 + 64, t, cs);
+    }
+    if constexpr (NP == 2) {
+        if (f16x2_overflowed(ovf) || (tid == 0 && ra.wflag != nullptr && *ra.wflag != 0u)) atomicOr(ra.ovf, 1u);
+    }
+}
+
+// C (rows, N) = A (rows, K) . W (K, N) on the fp32 FMA pipe: 64 x 64 tiles, 256 threads of 4 x 4 outputs, K in steps of 16, each
+// 64-wide K block summed on its own before it is added to the total (as the ring sums).  op.load_a(row, k) is called inside the
+// matrix only; op.store(row, col, sum) writes an output.
+template <class Op>
+__device__ __forceinline__ void fma_gemm(const Op& op, long long rows, int K, int N, const float* __restrict__ W) {
+    __shared__ float As[16][64 + 4], Bs[16][64];
+    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+    const long long row0 = (long long)blockIdx.x * 64;
+    const int col0 = blockIdx.y * 64;
+    float tot[4][4] = {}, part[4][4] = {};
+    for (int k0 = 0; k0 < K; k0 += 16) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int e = tid + 256 * i, kr = e >> 6, rr = e & 63;
+            const int kk = k0 + kr;
+            const long long p = row0 + rr;
+            As[kr][rr] = (kk < K && p < rows) ? op.load_a(p, kk) : 0.f;
+            const int col = col0 + rr;
+            Bs[kr][rr] = (kk < K && col < N) ? __ldg(W + (size_t)kk * N + col) : 0.f;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int kr = 0; kr < 16; ++kr) {
+            float av[4], bv[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) { av[i] = As[kr][ty * 4 + i]; bv[i] = Bs[kr][tx * 4 + i]; }
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) part[i][jj] = fmaf(av[i], bv[jj], part[i][jj]);
+        }
+        __syncthreads();
+        if ((k0 & 63) == 48 || k0 + 16 >= K) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int jj = 0; jj < 4; ++jj) { tot[i][jj] += part[i][jj]; part[i][jj] = 0.f; }
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        const long long p = row0 + ty * 4 + i;
+        if (p >= rows) continue;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const int col = col0 + tx * 4 + jj;
+            if (col < N) op.store(p, col, tot[i][jj]);
+        }
+    }
+}
+
+// ---- host side ----
+static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+// an op's four ring kernels, fn[NP - 2][NC - 1]
+struct RingKernels {
+    const void* fn[2][2];
+    const char* name;
+};
+// one launch of the (np, Nt / 64) kernel on min(units, SMs) CTAs; args points at the kernel's argument struct (ring_gemm.cu)
+int ring_launch(const RingKernels& k, int np, int Nt, const void* args, long long units, cudaStream_t st);
+// W (K, N) -> Wp (K, Np), columns N .. Np zero (mfv.cu)
+int pad_cols(long long K, int N, int Np, const float* W, float* Wp, cudaStream_t st);
+
+// The op's ring GEMM in the current arithmetic mode, on the image of W (K rows, zero rows up to Kp; N columns) in Nt-wide tiles.
+// Mode 2: bf16x3 only.  Otherwise the fp16x2 launch, then a bf16x3 rerun whose image and launch are no-ops unless the first launch
+// raised the word at `flag` (256 bytes).  img2 and img3 may alias: the rerun builds its image after the fp16x2 launch, that
+// image's last reader, has run.  `a.ring` is filled in here.
+template <class Args>
+int ring_run(const RingKernels& k, Args a, long long units, int K, int Kp, int N, int Nt, const float* W, uint8_t* img2, uint8_t* img3,
+             unsigned int* flag, cudaStream_t st) {
+    int rc;
+    if (tc_np() == 3) {
+        if ((rc = build_image(K, Kp, N, Nt | tc::kImageBf16x3, W, img3, st)) != PSA_OK) return rc;
+        a.ring = RingArgs{};
+        a.ring.image = img3;
+        return ring_launch(k, 3, Nt, &a, units, st);
+    }
+    PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
+    if ((rc = build_image(K, Kp, N, Nt | tc::kImageF16x2, W, img2, st)) != PSA_OK) return rc;
+    a.ring = RingArgs{};
+    a.ring.image = img2; a.ring.ovf = flag; a.ring.wflag = image_trailer(img2, Kp, N); a.ring.colscale = image_colscale(img2, Kp, N);
+    if ((rc = ring_launch(k, 2, Nt, &a, units, st)) != PSA_OK) return rc;
+    if ((rc = build_image(K, Kp, N, Nt | tc::kImageBf16x3, W, img3, st, flag)) != PSA_OK) return rc;
+    a.ring = RingArgs{};
+    a.ring.image = img3; a.ring.run_if = flag;
+    return ring_launch(k, 3, Nt, &a, units, st);
+}
+
+}  // namespace psa

@@ -10,15 +10,14 @@
 //                          of a 64-wide K block into shared memory, the consumers apply the previous layer's group norm (a per-cloud
 //                          affine) + ReLU and the factor g while they split the block into tensor-core operands.  The weight rows
 //                          are permuted to (j, t, c) order when the image is built, so a K block is one (j, t) slice of a
-//                          gathered row (two for c = 32).  Same ring, operand split and range guard as tc_dense_kernel (tc_mlp.cu).
+//                          gathered row (two for c = 32).  Runs on the shared ring (ring_gemm.cuh).
 //   spider_fma_kernel      the same product on the fp32 FMA pipe (mode 1, and shapes the tensor path does not take: layer 1, c = 3)
 //   group_norm_*           per (cloud, group) mean and centred variance in fp64 -> the per-cloud affine (scale, shift)
 //   topk_pool_kernel       the two largest values of relu(y * scale + shift) per (cloud, channel)
 #include <float.h>
 
 #include "common.cuh"
-#include "mlp_internal.cuh"
-#include "tc_common.cuh"
+#include "ring_gemm.cuh"
 
 namespace psa {
 
@@ -64,286 +63,144 @@ __global__ void spider_permute_kernel(int k, int c, int T, int N, const float* _
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// tc_spider_kernel<NP, NC>: y (rows, N) = A . Wp + bias over 128-row x 64 NC-channel tiles, persistent (static tile order).
-// CTA = two consumer warpgroups (rows 0-63 / 64-127) + a producer warpgroup whose four warps each gather 32 rows of every K
-// block (cp.async, 16 bytes per copy) while warp 0 also drops the block's weights in by TMA.  Per tile a producer warp first
-// copies its rows' k neighbour indices to shared memory, so the gathers of a block only wait on shared-memory reads.
-// The consumers' K loop is tc_dense_kernel's: per block one wgmma group on the registers prepared under the previous one, the
-// block's sum added to fp32 accumulators (no tensor-core accumulation over more than 64 K).
+// tc_spider_kernel<NP, NC>: y (rows, N) = A . Wp + bias on the ring (ring_gemm.cuh), unit = 128-row tile x 64 NC-column tile, all
+// K blocks.  Per unit a producer warp first copies its rows' k neighbour indices to shared memory, so the gathers of a block only
+// wait on shared-memory reads.
 // ------------------------------------------------------------------------------------------------------------------
 struct SpiderArgs {
     long long rows;            // b * n
-    int n, c, k, T, K, N;      // K = k * T * c, a multiple of 64
-    const float* feat;         // (rows, c), 16-byte aligned
+    int n, c, k, T, K, N;      // K = k * T * c, a multiple of 64 on the tensor path
+    const float* feat;         // (rows, c), 16-byte aligned on the tensor path
     const int* idx;            // (rows, k)
     const float* g;            // (rows * k, T)
     const float* fs;           // (b, c) or null, 8-byte aligned on the tensor path
     const float* fu;
-    const uint8_t* image;      // Wp in the format of NP, tile width 64 NC
     const float* bias;         // (N), 8-byte aligned on the tensor path
     float* y;                  // (rows, N), 8-byte aligned on the tensor path
-    unsigned int* ovf = nullptr;            // np = 2: raised when an operand left the fp16 range or a weight is not finite
-    const unsigned int* run_if = nullptr;   // non-null: no-op unless *run_if != 0
-    const unsigned int* wflag = nullptr;
-    const float* colscale = nullptr;
+    RingArgs ring;             // Wp in the format of NP, tile width 64 NC
 };
 
-constexpr int kSpiderThreads = 384, kSpiderConsumers = 256;
-constexpr uint32_t kSpiderXRow = 64u * 4u + 32u;          // as tc_dense_kernel: conflict-free fragment reads
-constexpr uint32_t kSpiderXBytes = 128u * kSpiderXRow;
-constexpr uint32_t kSpiderRingBudget = 206u * 1024u;
-__host__ __device__ constexpr uint32_t spider_stage_bytes(int NP, int NC) { return tc_block_bytes(64 * NC, NP) + kSpiderXBytes; }
-__host__ __device__ constexpr int spider_stages(int NP, int NC) {
-    return kSpiderRingBudget / spider_stage_bytes(NP, NC) < 4u ? (int)(kSpiderRingBudget / spider_stage_bytes(NP, NC)) : 4;
-}
+struct SpiderOp {
+    const SpiderArgs& a;
+    struct Smem {
+        int nbr[128 * kSpiderMaxK];                        // the unit's neighbour rows (global row index)
+    };
+    struct Unit {
+        int nb, col0;
+        long long r[2];
+        bool v[2];
+        int cb[2];                                         // the rows' clouds
+    };
+
+    __device__ int units(int Nt) const { return (int)((a.rows + 127) / 128 * (a.N / Nt)); }
+
+    template <class Put>
+    __device__ void produce(int unit, int Nt, int pw, int lane, Smem& sm, Put&& put) const {
+        const int NTC = a.N / Nt, KC = a.K / 64, seg = a.T * a.c;
+        const long long row0 = (long long)(unit / NTC) * 128;
+        const int nt = unit % NTC, r0 = 32 * pw, nr = (int)max(0LL, min(32LL, a.rows - row0 - r0));
+        __syncwarp();                                      // the previous unit's reads of nbr are done
+        for (int e = lane; e < nr * a.k; e += 32) {
+            const int r = e / a.k;
+            const long long p = row0 + r0 + r;
+            sm.nbr[(r0 + r) * kSpiderMaxK + (e - r * a.k)] = (int)(p / a.n * a.n) + __ldg(a.idx + p * a.k + (e - r * a.k));
+        }
+        __syncwarp();
+        for (int kb = 0; kb < KC; ++kb)
+            put((size_t)nt * KC + kb, [&](uint32_t xs) {
+                // lane (row half, 16-byte chunk): the chunk's column of the block is fixed per lane, so is its (j, t, c)
+                const int cc = (lane & 15) * 4, kk = kb * 64 + cc;
+                const int j = kk / seg, rem = kk - j * seg, ch = rem - rem / a.c * a.c;
+                for (int r = lane >> 4; r < nr; r += 2) {
+                    const int row = r0 + r;
+                    cp_async16(xs + (uint32_t)row * kRingXRow + (uint32_t)cc * 4u, a.feat + (size_t)sm.nbr[row * kSpiderMaxK + j] * a.c + ch);
+                }
+            });
+    }
+
+    __device__ Unit unit(int unit, int Nt, int row) const {
+        const int NTC = a.N / Nt;
+        Unit u;
+        u.nb = a.K / 64;
+        u.col0 = unit % NTC * Nt;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            u.r[i] = (long long)(unit / NTC) * 128 + row + 8 * i;
+            u.v[i] = u.r[i] < a.rows;
+            u.cb[i] = u.v[i] ? (int)(u.r[i] / a.n) * a.c : 0;
+        }
+        return u;
+    }
+
+    // the previous layer's group norm + ReLU, times g_t(delta_pj); rows past `rows` read as zero (their staged bytes are stale)
+    __device__ void load(const Unit& u, const float* xs, int kb, int t, float2 (&x)[4][2][2]) const {
+        const int seg = a.T * a.c;
+        // c % 32 == 0: each 32-column half of the block lies in one (j, t) slice, channels ch0 ..
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) {
+            const int kk = kb * 64 + 32 * hf, j = kk / seg, rem = kk - j * seg, tt = rem / a.c, ch0 = rem - tt * a.c;
+            float gv[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) gv[i] = u.v[i] ? __ldg(a.g + (u.r[i] * a.k + j) * a.T + tt) : 0.f;
+#pragma unroll
+            for (int s = 2 * hf; s < 2 * hf + 2; ++s)
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int ch = ch0 + 16 * s + 8 * h + 2 * t - 32 * hf;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        float2 v = make_float2(0.f, 0.f);
+                        if (u.v[i]) {
+                            v = staged_pair(xs, s, h, i, t);
+                            if (a.fs != nullptr) {
+                                const float2 sc = __ldg(reinterpret_cast<const float2*>(a.fs + u.cb[i] + ch));
+                                const float2 sh = __ldg(reinterpret_cast<const float2*>(a.fu + u.cb[i] + ch));
+                                v.x = fmaxf(fmaf(v.x, sc.x, sh.x), 0.f);
+                                v.y = fmaxf(fmaf(v.y, sc.y, sh.y), 0.f);
+                            }
+                            v.x *= gv[i];
+                            v.y *= gv[i];
+                        }
+                        x[s][h][i] = v;
+                    }
+                }
+        }
+    }
+
+    // fp16x2 column factor, bias; pre-group-norm y
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+            const int col = col0 + 8 * jj + 2 * t;
+            const float2 cs = colscale != nullptr ? __ldg(reinterpret_cast<const float2*>(colscale + col)) : make_float2(1.f, 1.f);
+            const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + col));
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+                if (u.v[i])
+                    *reinterpret_cast<float2*>(a.y + (size_t)u.r[i] * a.N + col) =
+                        make_float2(fmaf(acc[4 * jj + 2 * i], cs.x, bi.x), fmaf(acc[4 * jj + 2 * i + 1], cs.y, bi.y));
+        }
+    }
+
+    // the FMA fallback's A, in the reference's K order (j, c, t)
+    __device__ float load_a(long long p, int kk) const {
+        const int ct = a.c * a.T, j = kk / ct, rem = kk - j * ct, ch = rem / a.T, tt = rem - ch * a.T;
+        const int b = (int)(p / a.n);
+        float x = __ldg(a.feat + ((long long)b * a.n + __ldg(a.idx + p * a.k + j)) * a.c + ch);
+        if (a.fs != nullptr) x = fmaxf(fmaf(x, __ldg(a.fs + b * a.c + ch), __ldg(a.fu + b * a.c + ch)), 0.f);
+        return x * __ldg(a.g + (p * a.k + j) * a.T + tt);
+    }
+    __device__ void store(long long p, int col, float s) const { a.y[(size_t)p * a.N + col] = s + __ldg(a.bias + col); }
+};
 
 template <int NP, int NC>
-__global__ void __launch_bounds__(kSpiderThreads, 1)
-tc_spider_kernel(const __grid_constant__ SpiderArgs a) {
-    if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr int Nt = 64 * NC, S = spider_stages(NP, NC);
-    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = spider_stage_bytes(NP, NC);
-    static_assert(S >= 2, "the ring needs two stages");
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
-    __shared__ int s_tile[S];
-    __shared__ int s_nbr[128 * kSpiderMaxK];                        // the tile's neighbour rows (global row index)
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int KC = a.K / 64, NTC = a.N / Nt, seg = a.T * a.c;
-    const long long ntiles = (a.rows + 127) / 128 * NTC;
-    if (tid == 0) {
-        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 128); mbar_init(&s_empty[i], kSpiderConsumers / 32); }
-        fence_mbar_init();
-    }
-    __syncthreads();
-
-    if (warp >= kSpiderConsumers / 32) {
-        // ---- producers: warp pw gathers tile rows [32 pw, 32 pw + 32) ----
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        const int pw = warp - kSpiderConsumers / 32;
-        uint32_t q = 0;
-        for (long long tile = blockIdx.x;; tile += gridDim.x) {
-            const bool done = tile >= ntiles;
-            const long long row0 = tile / NTC * 128;
-            const int nt = (int)(tile % NTC);
-            const int r0 = 32 * pw, nr = done ? 0 : (int)max(0LL, min(32LL, a.rows - row0 - r0));
-            if (!done) {
-                __syncwarp();                                        // the previous tile's reads of s_nbr are done
-                for (int e = lane; e < nr * a.k; e += 32) {
-                    const int r = e / a.k;
-                    const long long p = row0 + r0 + r;
-                    s_nbr[(r0 + r) * kSpiderMaxK + (e - r * a.k)] = (int)(p / a.n * a.n) + __ldg(a.idx + p * a.k + (e - r * a.k));
-                }
-                __syncwarp();
-            }
-            for (int kb = 0; kb < KC; ++kb, ++q) {
-                const int s = (int)(q % S);
-                if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
-                if (pw == 0 && lane == 0) {
-                    s_tile[s] = done ? -1 : (int)tile;
-                    if (done) {
-                        mbar_arrive1(&s_full[s]);
-                    } else {
-                        mbar_expect_tx(&s_full[s], bb);
-                        const uint8_t* src = a.image + ((size_t)nt * KC + kb) * bb;
-                        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
-                    }
-                }
-                if (!done) {
-                    // lane (row half, 16-byte chunk): the chunk's column of the block is fixed per lane, so is its (j, t, c)
-                    const int cc = (lane & 15) * 4, kk = kb * 64 + cc;
-                    const int j = kk / seg, rem = kk - j * seg, ch = rem - rem / a.c * a.c;
-                    const uint32_t xs = smem_u32(base + (uint32_t)s * SB + bb);
-                    for (int r = lane >> 4; r < nr; r += 2) {
-                        const int row = r0 + r;
-                        cp_async16(xs + (uint32_t)row * kSpiderXRow + (uint32_t)cc * 4u, a.feat + (size_t)s_nbr[row * kSpiderMaxK + j] * a.c + ch);
-                    }
-                }
-                cp_async_mbar_arrive(&s_full[s]);
-                if (done) break;
-            }
-            if (done) return;
-        }
-    }
-
-    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-    const int g = lane >> 2, t = lane & 3;
-    uint32_t ovf = 0u;
-    uint32_t q = 0;                                                 // ring uses
-    for (;;) {
-        mbar_wait(&s_full[q % S], (q / S) & 1u);
-        const int tile = s_tile[q % S];
-        if (tile < 0) break;
-        const long long row0 = (long long)(tile / NTC) * 128;
-        const int nt = tile % NTC;
-        const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
-        const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
-        const int cb[2] = {v[0] ? (int)(r[0] / a.n) * a.c : 0, v[1] ? (int)(r[1] / a.n) * a.c : 0};   // the rows' clouds
-
-        // gathered block of ring use u -> A fragments: the previous layer's group norm + ReLU, times g_t(delta_pj); rows past
-        // `rows` read as zero (their staged bytes are stale)
-        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t u, int kb) {
-            const float* xs = reinterpret_cast<const float*>(base + (u % S) * SB + bb);
-            // c % 32 == 0: each 32-column half of the block lies in one (j, t) slice, channels ch0 ..
-#pragma unroll
-            for (int hf = 0; hf < 2; ++hf) {
-                const int kk = kb * 64 + 32 * hf, j = kk / seg, rem = kk - j * seg, tt = rem / a.c, ch0 = rem - tt * a.c;
-                float gv[2];
-#pragma unroll
-                for (int i = 0; i < 2; ++i) gv[i] = v[i] ? __ldg(a.g + (r[i] * a.k + j) * a.T + tt) : 0.f;
-#pragma unroll
-                for (int s = 2 * hf; s < 2 * hf + 2; ++s)
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int kl = 16 * s + 8 * h + 2 * t, ch = ch0 + kl - 32 * hf;
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            float2 x = make_float2(0.f, 0.f);
-                            if (v[i]) {
-                                x = *reinterpret_cast<const float2*>(xs + (warp * 16 + g + 8 * i) * (int)(kSpiderXRow / 4) + kl);
-                                if (a.fs != nullptr) {
-                                    const float2 sc = __ldg(reinterpret_cast<const float2*>(a.fs + cb[i] + ch));
-                                    const float2 sh = __ldg(reinterpret_cast<const float2*>(a.fu + cb[i] + ch));
-                                    x.x = fmaxf(fmaf(x.x, sc.x, sh.x), 0.f);
-                                    x.y = fmaxf(fmaf(x.y, sc.y, sh.y), 0.f);
-                                }
-                                x.x *= gv[i];
-                                x.y *= gv[i];
-                            }
-                            uint32_t pc[NP];
-                            split_pair<NP>(x.x, x.y, pc, ovf);
-#pragma unroll
-                            for (int e = 0; e < NP; ++e) A[e][s][i + 2 * h] = pc[e];
-                        }
-                    }
-            }
-        };
-        float acc[NC][32];
-        // tc_dense_kernel's step: issue block kb's group on A, prepare block kb + 1 into An while it runs, wait, release, add
-        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
-        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t u, int kb) {
-            const uint32_t wb = smem_u32(base + (u % S) * SB);
-#pragma unroll
-            for (int c0 = 0; c0 < NC; c0 += CG) {
-                float d[CG][32];
-                wg_fence();
-#pragma unroll
-                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
-#pragma unroll
-                    for (int s = 0; s < 4; ++s)
-#pragma unroll
-                        for (int c = 0; c < CG; ++c)
-                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
-                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
-                wg_commit();
-                if (c0 + CG == NC && kb + 1 < KC) {
-                    mbar_wait(&s_full[(u + 1) % S], ((u + 1) / S) & 1u);
-                    prep(An, u + 1, kb + 1);
-                }
-                wg_wait_all();
-                if (c0 + CG == NC) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive1(&s_empty[u % S]);
-                }
-#pragma unroll
-                for (int c = 0; c < CG; ++c) {
-                    wg_fence_acc(d[c]);
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
-                }
-            }
-        };
-        {
-            uint32_t A0[NP][4][4], A1[NP][4][4];
-            prep(A0, q, 0);
-            for (int kb = 0;; kb += 2) {
-                step(A0, A1, q + kb, kb);
-                if (kb + 1 == KC) break;
-                step(A1, A0, q + kb + 1, kb + 1);
-                if (kb + 2 == KC) break;
-            }
-        }
-        q += KC;
-
-        // ---- epilogue: fp16x2 column factor, bias; pre-group-norm y ----
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-                const int col = nt * Nt + c * 64 + 8 * jj + 2 * t;
-                const float2 cs = NP == 2 ? __ldg(reinterpret_cast<const float2*>(a.colscale + col)) : make_float2(1.f, 1.f);
-                const float2 bi = __ldg(reinterpret_cast<const float2*>(a.bias + col));
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-                    if (v[i])
-                        *reinterpret_cast<float2*>(a.y + (size_t)r[i] * a.N + col) =
-                            make_float2(fmaf(acc[c][4 * jj + 2 * i], cs.x, bi.x), fmaf(acc[c][4 * jj + 2 * i + 1], cs.y, bi.y));
-            }
-    }
-    if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
-    }
+__global__ void __launch_bounds__(kRingThreads, 1) tc_spider_kernel(const __grid_constant__ SpiderArgs a) {
+    ring_gemm<NP, NC>(SpiderOp{a}, a.ring);
 }
 
-// ------------------------------------------------------------------------------------------------------------------
-// The same product on the fp32 FMA pipe, in the reference's K order (j, c, t): 64 x 64 tiles, 256 threads of 4 x 4 outputs,
-// K in steps of 16, each 64-wide K block summed on its own before it is added to the total (as the tensor path sums).
-// ------------------------------------------------------------------------------------------------------------------
+// the same product on the fp32 FMA pipe, with the unpermuted W
 __global__ void __launch_bounds__(256) spider_fma_kernel(const __grid_constant__ SpiderArgs a, const float* __restrict__ W) {
-    __shared__ float As[16][64 + 4], Bs[16][64];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const long long row0 = (long long)blockIdx.x * 64;
-    const int col0 = blockIdx.y * 64, ct = a.c * a.T;
-    float tot[4][4] = {}, part[4][4] = {};
-    for (int k0 = 0; k0 < a.K; k0 += 16) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const int e = tid + 256 * i, kr = e >> 6, rr = e & 63;
-            const int kk = k0 + kr;
-            const long long p = row0 + rr;
-            float val = 0.f;
-            if (kk < a.K && p < a.rows) {
-                const int j = kk / ct, rem = kk - j * ct, ch = rem / a.T, tt = rem - ch * a.T;
-                const int b = (int)(p / a.n);
-                float x = __ldg(a.feat + ((long long)b * a.n + __ldg(a.idx + p * a.k + j)) * a.c + ch);
-                if (a.fs != nullptr) x = fmaxf(fmaf(x, __ldg(a.fs + b * a.c + ch), __ldg(a.fu + b * a.c + ch)), 0.f);
-                val = x * __ldg(a.g + (p * a.k + j) * a.T + tt);
-            }
-            As[kr][rr] = val;
-            const int col = col0 + rr;
-            Bs[kr][rr] = (kk < a.K && col < a.N) ? __ldg(W + (size_t)kk * a.N + col) : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kr = 0; kr < 16; ++kr) {
-            float av[4], bv[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { av[i] = As[kr][ty * 4 + i]; bv[i] = Bs[kr][tx * 4 + i]; }
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) part[i][jj] = fmaf(av[i], bv[jj], part[i][jj]);
-        }
-        __syncthreads();
-        if ((k0 & 63) == 48 || k0 + 16 >= a.K) {
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int jj = 0; jj < 4; ++jj) { tot[i][jj] += part[i][jj]; part[i][jj] = 0.f; }
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const long long p = row0 + ty * 4 + i;
-        if (p >= a.rows) continue;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-            const int col = col0 + tx * 4 + jj;
-            if (col < a.N) a.y[(size_t)p * a.N + col] = tot[i][jj] + __ldg(a.bias + col);
-        }
-    }
+    fma_gemm(SpiderOp{a}, a.rows, a.K, a.N, W);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -449,7 +306,6 @@ static bool spider_tc_eligible(long long rows, int c, int k, int T, int N, const
 struct SpiderWs {
     size_t g, wp, img2, img3, total;
 };
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 static SpiderWs spider_ws(int b, int n, int c, int k, int T, int N) {
     SpiderWs w{};
     const long long rows = (long long)b * n;
@@ -465,21 +321,9 @@ static SpiderWs spider_ws(int b, int n, int c, int k, int T, int N) {
     return w;
 }
 
-template <int NP, int NC>
-static int launch_spider_shape(const SpiderArgs& a, cudaStream_t st) {
-    const size_t smem = (size_t)spider_stages(NP, NC) * spider_stage_bytes(NP, NC) + 1024;
-    PSA_CUDA(cudaFuncSetAttribute(tc_spider_kernel<NP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int dev = 0, sms = 0;
-    PSA_CUDA(cudaGetDevice(&dev));
-    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    const long long tiles = (a.rows + 127) / 128 * (a.N / (64 * NC));
-    tc_spider_kernel<NP, NC><<<(unsigned)(tiles < sms ? tiles : sms), kSpiderThreads, smem, st>>>(a);
-    return check_launch("tc_spider_kernel");
-}
-template <int NP>
-static int launch_spider_np(const SpiderArgs& a, int Nt, cudaStream_t st) {
-    return Nt == 128 ? launch_spider_shape<NP, 2>(a, st) : launch_spider_shape<NP, 1>(a, st);
-}
+static const RingKernels kSpiderRing = {{{(const void*)tc_spider_kernel<2, 1>, (const void*)tc_spider_kernel<2, 2>},
+                                         {(const void*)tc_spider_kernel<3, 1>, (const void*)tc_spider_kernel<3, 2>}},
+                                        "tc_spider_kernel"};
 
 }  // namespace psa
 
@@ -510,7 +354,7 @@ extern "C" int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_ou
     SpiderArgs a;
     a.rows = rows; a.n = n; a.c = c; a.k = k; a.T = T; a.K = k * T * c; a.N = c_out;
     a.feat = feat; a.idx = nn_idx; a.g = reinterpret_cast<float*>(wsb + ws.g); a.fs = feat_scale; a.fu = feat_shift;
-    a.bias = bias; a.y = y; a.image = nullptr;
+    a.bias = bias; a.y = y;
     spider_taylor_kernel<<<(unsigned)((pairs * T + 255) / 256), 256, 0, st>>>(pairs, T, delta, taylor, const_cast<float*>(a.g));
     int rc = check_launch("spider_taylor_kernel");
     if (rc != PSA_OK) return rc;
@@ -524,26 +368,8 @@ extern "C" int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_ou
     spider_permute_kernel<<<1024, 256, 0, st>>>(k, c, T, c_out, W, wp);
     rc = check_launch("spider_permute_kernel");
     if (rc != PSA_OK) return rc;
-    uint8_t* img3 = wsb + ws.img3;
-    if (tc_np() == 3) {
-        rc = build_image(K, K, c_out, Nt | kImageBf16x3, wp, img3, st);
-        if (rc != PSA_OK) return rc;
-        a.image = img3;
-        return launch_spider_np<3>(a, Nt, st);
-    }
-    unsigned int* flag = reinterpret_cast<unsigned int*>(wsb);
-    PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
-    uint8_t* img2 = wsb + ws.img2;
-    rc = build_image(K, K, c_out, Nt | kImageF16x2, wp, img2, st);
-    if (rc != PSA_OK) return rc;
-    a.image = img2; a.ovf = flag; a.wflag = image_trailer(img2, K, c_out); a.colscale = image_colscale(img2, K, c_out);
-    rc = launch_spider_np<2>(a, Nt, st);
-    if (rc != PSA_OK) return rc;
-    // guarded rerun on bf16x3 operands: its image and its launch are no-ops unless the fp16x2 pass raised the flag
-    rc = build_image(K, K, c_out, Nt | kImageBf16x3, wp, img3, st, flag);
-    if (rc != PSA_OK) return rc;
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = flag;
-    return launch_spider_np<3>(a, Nt, st);
+    return ring_run(kSpiderRing, a, (rows + 127) / 128 * (c_out / Nt), K, K, c_out, Nt, wp, wsb + ws.img2, wsb + ws.img3,
+                    reinterpret_cast<unsigned int*>(wsb), st);
 }
 
 extern "C" int psa_group_norm_affine(int b, int n, int c, int groups, float eps, const float* y, const float* gamma,

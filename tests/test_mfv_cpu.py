@@ -185,14 +185,13 @@ def test_invalid_arguments_are_rejected_without_a_gpu():
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_conv3d_kernel_code_shape():
-    """tc_conv3d_kernel: wgmma, bulk copies and mbarriers in every instantiation, wgmma issued in straight-line groups, the
-    producers' registers handed to the consumers; no local memory in any kernel of mfv.cu."""
+def test_mfv_kernels_use_no_local_memory():
+    """no local memory in any kernel of mfv.cu (tc_conv3d_kernel's wgmma, copies and register hand-off: test_sass_ring.py)"""
     from scanobjectnn_b200.build import build_library
     build_library()
     out = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True, check=True).stdout
     funcs, name = {}, None
-    kernels = ("tc_conv3d_kernel", "conv3d_fma_kernel", "fisher_vector_kernel", "pool3d_", "conv3d_tapmask", "conv3d_finalize", "conv3d_pad")
+    kernels = ("tc_conv3d_kernel", "conv3d_fma_kernel", "fisher_vector_kernel", "pool3d_", "conv3d_tapmask", "conv3d_finalize", "pad_cols")
     for line in out.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
@@ -201,17 +200,7 @@ def test_conv3d_kernel_code_shape():
                 funcs[name] = []
         elif name is not None:
             funcs[name].append(line)
-    tc = {k: v for k, v in funcs.items() if "tc_conv3d_kernel" in k}
-    assert len(tc) == 4, sorted(tc)                  # NP in {2, 3} x NC in {1, 2}
-    assert len(funcs) == 11, sorted(funcs)
-    for name, lines in tc.items():
-        text = "\n".join(lines)
-        for mn in ("HGMMA", "UBLKCP", "SYNCS", "LDGSTS"):
-            assert re.search(r"\b" + mn, text), f"{name}: no {mn}"
-        hgmma = sum(1 for l in lines if re.search(r"\bHGMMA(\.\w+)*", l))
-        arrive = sum(1 for l in lines if "WARPGROUP.ARRIVE" in l)
-        assert arrive >= 1 and 4 * arrive <= hgmma, f"{name}: {arrive} WARPGROUP.ARRIVE for {hgmma} HGMMA -- serialized"
-        assert sum(1 for l in lines if "USETMAXREG" in l) >= 2, f"{name}: no setmaxnreg"
+    assert len(funcs) == 11, sorted(funcs)          # four tc_conv3d_kernel instantiations and seven other kernels
     for name, lines in funcs.items():
         assert not any(re.search(r"\b(STL|LDL)\b", l) for l in lines), f"{name}: local memory (spills)"
 

@@ -1,6 +1,7 @@
 """PointCNN without a GPU: the reference's variable names and TF shapes and a TF checkpoint round trip, the float64 restatement
 (oracle/pointcnn_oracle.py) against an independent float64 torch composition (F.conv2d with groups, F.elu, F.batch_norm), the C kNN
-oracle against DGCNN's, the refusals that need no device, the C ABI's argument checks, and the code shape of the new kernels."""
+oracle against DGCNN's, the refusals that need no device, the C ABI's argument checks, and the new kernels' spills and atomics (the
+dense kernel's code shape: test_sass_ring.py)."""
 import ctypes as C
 import os
 import re
@@ -194,7 +195,7 @@ def test_c_abi_rejects_bad_arguments_without_a_gpu():
 
 
 @pytest.mark.skipif(shutil.which("cuobjdump") is None and not os.path.exists("/usr/local/cuda/bin/cuobjdump"), reason="no cuobjdump")
-def test_new_kernels_do_not_spill_use_wgmma_and_no_float_atomics(tmp_path):
+def test_new_kernels_do_not_spill_and_use_no_float_atomics(tmp_path):
     nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     src = os.path.join(ROOT, "scanobjectnn_b200", "csrc", "pointcnn.cu")
@@ -203,9 +204,6 @@ def test_new_kernels_do_not_spill_use_wgmma_and_no_float_atomics(tmp_path):
                        capture_output=True, text=True, check=True)
     log = r.stdout + r.stderr
     frames = re.findall(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", log)
-    assert len(frames) >= 8 and all(f == ("0", "0", "0") for f in frames), log
+    assert len(frames) >= 7 and all(f == ("0", "0", "0") for f in frames), log
     sass = subprocess.run([cuobjdump, "-sass", obj], capture_output=True, text=True, check=True).stdout
-    funcs = re.split(r"\n\s*Function : ", sass)
-    dense = [f for f in funcs if f.startswith("_ZN3psa20tc_pcnn_dense_kernel")]
-    assert len(dense) == 4 and all("HGMMA" in f for f in dense)
     assert not re.search(r"\b(RED|ATOM|ATOMG)\.[A-Z.]*F32", sass)

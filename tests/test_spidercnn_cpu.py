@@ -1,11 +1,7 @@
 """SpiderCNN without a GPU: the float64 restatement (oracle/spidercnn_oracle.py) against a plain-loop transcription of the
 reference at a tiny size with the real channel widths, the reference's variable names and shapes and a TF checkpoint round trip,
-the refusal of training mode, the C ABI's argument checks, and the code shape of the fused kernel (cuobjdump)."""
+the refusal of training mode and the C ABI's argument checks (the fused kernel's code shape: test_sass_ring.py)."""
 import ctypes as C
-import os
-import re
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,10 +10,6 @@ import torch
 from oracle import spidercnn_oracle as so
 from scanobjectnn_b200 import checkpoint as ck
 from scanobjectnn_b200 import spidercnn_cls_xyz as M
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-LIB = os.path.join(ROOT, "scanobjectnn_b200", "libpsa.so")
-
 
 def _reference_shapes(num_class=15):
     want = {}
@@ -168,31 +160,3 @@ def test_invalid_arguments_are_rejected_without_a_gpu():
     assert lib.psa_topk_pool(1, 16, 32, 3, null, null, null, 1, null, 32, 0, null) == -2           # only k = 2
     assert lib.psa_topk_pool(1, 1, 32, 2, null, null, null, 1, null, 32, 0, null) == -1            # fewer points than k
     assert lib.psa_topk_pool(1, 16, 32, 2, null, null, null, 1, null, 48, 20, null) == -1          # channels past out_channels
-
-
-@pytest.mark.skipif(shutil.which("cuobjdump") is None, reason="cuobjdump not on PATH")
-def test_spider_kernel_code_shape():
-    """tc_spider_kernel: wgmma, bulk copies and mbarriers in every instantiation, the wgmma issued in straight-line groups (one
-    WARPGROUP.ARRIVE per group, not per HGMMA), the producers' registers handed to the consumers, and no local-memory spills."""
-    from scanobjectnn_b200.build import build_library
-    build_library()
-    out = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True, check=True).stdout
-    funcs, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1) if "tc_spider_kernel" in m.group(1) else None
-            if name:
-                funcs[name] = []
-        elif name is not None:
-            funcs[name].append(line)
-    assert len(funcs) == 4, sorted(funcs)           # NP in {2, 3} x NC in {1, 2}
-    for name, lines in funcs.items():
-        text = "\n".join(lines)
-        for mn in ("HGMMA", "UBLKCP", "SYNCS"):
-            assert re.search(r"\b" + mn, text), f"{name}: no {mn}"
-        hgmma = sum(1 for l in lines if re.search(r"\bHGMMA(\.\w+)*", l))
-        arrive = sum(1 for l in lines if "WARPGROUP.ARRIVE" in l)
-        assert arrive >= 1 and 4 * arrive <= hgmma, f"{name}: {arrive} WARPGROUP.ARRIVE for {hgmma} HGMMA -- serialized"
-        assert sum(1 for l in lines if "USETMAXREG" in l) >= 2, f"{name}: no setmaxnreg"
-        assert not any(re.search(r"\b(STL|LDL)\b", l) for l in lines), f"{name}: register spills"
