@@ -514,6 +514,88 @@ def pointnet2_bga(x, P, frozen, masks, idx, run=None, drops=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# plans of the shared ring GEMM's three ops (csrc/mfv.cu conv_plan, csrc/pointcnn.cu pd_plan, csrc/spider.cu spider_ws with
+# csrc/tc_mlp.cu tc_dense_nt): the tile widths, splits and workspace bytes the launchers pick, so that a test can name the path a
+# shape takes.  tests/test_ring_gemm_plan_cpu.py checks the byte counts against the library's workspace queries.
+# ---------------------------------------------------------------------------------------------------------------------
+PLAN_SMS = 132                    # kNumSMs (csrc/common.cuh): what the plans assume, whatever the device has
+
+
+def _al256(x):
+    return (x + 255) & ~255
+
+
+def image_bytes(K, N, np_):
+    """tc_image_alloc_bytes (csrc/tc_common.cuh): the blocks, np = 2's column factors, the 256-byte trailer"""
+    blocks = _al256(K * N * 2 * np_)
+    return blocks + (_al256(N * 4) if np_ == 2 else 0) + 256
+
+
+def wide_tiles(tiles, Np):
+    """the 128-wide column tile of tc_dense_nt and conv_plan: when Np allows it and those tiles alone fill more than half the SMs"""
+    return Np % 128 == 0 and 2 * tiles * (Np // 128) > PLAN_SMS
+
+
+def conv_active_taps(b, r, k, tile, rows):
+    """conv3d_tapmask_kernel: the taps of a k^3 kernel that reach inside the r^3 grid for some row of 128-row tile `tile`"""
+    h, r0, r1 = k // 2, tile * 128, min(rows, tile * 128 + 128) - 1
+    vox = [(v // (r * r), v // r % r, v % r) for v in range(r0 // b, r1 // b + 1)]
+    offs = [(t // (k * k) - h, t // k % k - h, t % k - h) for t in range(k ** 3)]
+    return sum(any(all(0 <= p + o < r for p, o in zip(v, off)) for v in vox) for off in offs)
+
+
+def conv_plan(b, r, k, c, n, np_):
+    """conv_plan (csrc/mfv.cu) -> dict: tiles, Np, Nt, splits, units (all column tiles and splits) and the workspace `total` for
+    np_ = 2 (mode 0) or 3 (mode 2)"""
+    rows, K, CB = b * r ** 3, k ** 3 * c, c // 64
+    tiles, Np = -(-rows // 128), -(-n // 64) * 64
+    Nt = 128 if wide_tiles(tiles, Np) else 64
+    units = tiles * (Np // Nt)
+    reach = min(k, 2 * r - 1)
+    maxk = reach ** 3 * CB
+    s = min(1 if units >= PLAN_SMS else PLAN_SMS // units, 16)
+    s = s if s < maxk // 2 else max(maxk // 2, 1)
+    total = 256 + _al256(tiles * 16)
+    if Np != n:
+        total += _al256(K * Np * 4)
+    total += image_bytes(K, Np, 2) if np_ == 2 and image_bytes(K, Np, 2) > image_bytes(K, Np, 3) else image_bytes(K, Np, 3)
+    if s > 1:
+        total += _al256(s * rows * Np * 4)
+    return dict(rows=rows, tiles=tiles, Np=Np, Nt=Nt, splits=s, units=units * s, total=total)
+
+
+def conv_unit_blocks(b, r, k, c, splits):
+    """per 128-row tile, the K blocks of each of its split units (Conv3dOp::unit): the tile's active blocks divided in order"""
+    rows = b * r ** 3
+    nact = [conv_active_taps(b, r, k, t, rows) * (c // 64) for t in range(-(-rows // 128))]
+    return [[a * (sp + 1) // splits - a * sp // splits for sp in range(splits)] for a in nact]
+
+
+def pd_plan(rows, K, N, np_):
+    """pd_plan (csrc/pointcnn.cu): K padded to 64, N to 64-wide blocks taken two at a time when their count is even"""
+    Kp, nblk = -(-K // 64) * 64, -(-N // 64)
+    Nt, Np = (128 if nblk % 2 == 0 else 64), nblk * 64
+    total = 256 + _al256(K * Np * 4) + (image_bytes(Kp, Np, 2) if np_ == 2 else 0) + image_bytes(Kp, Np, 3)
+    return dict(Kp=Kp, Np=Np, Nt=Nt, units=-(-rows // 128) * (Np // Nt), total=total)
+
+
+def spider_tensor_shape(rows, c, k, t, n):
+    """spider_tc_eligible (csrc/spider.cu) for aligned pointers"""
+    return rows >= 128 and c % 32 == 0 and k * t * c % 64 == 0 and n % 64 == 0 and (n == 64 or n % 128 == 0)
+
+
+def spider_plan(b, npts, c, k, t, n):
+    """spider_ws (csrc/spider.cu) and the tile width of tc_dense_nt; the workspace holds both images in every mode"""
+    rows, K = b * npts, k * t * c
+    tiles = -(-rows // 128)
+    Nt = 128 if wide_tiles(tiles, n) else 64
+    total = 256 + _al256(rows * k * t * 4)
+    if spider_tensor_shape(rows, c, k, t, n):
+        total += _al256(K * n * 4) + image_bytes(K, n, 2) + image_bytes(K, n, 3)
+    return dict(rows=rows, Nt=Nt, units=tiles * (n // Nt), total=total)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # metrics
 # ---------------------------------------------------------------------------------------------------------------------
 def rel(got, want):
