@@ -210,6 +210,8 @@ __device__ __forceinline__ int mask_active(const uint32_t* tm) {
 
 struct Conv3dOp {
     const Conv3dArgs& a;
+    static constexpr bool kClaim = false;
+    static constexpr uint32_t kBudget = kRingBudget;
     struct Smem {
         int zyx[128], cl[128];                             // the unit's rows: packed voxel coordinates (-1: past the end), cloud
     };
@@ -261,7 +263,7 @@ struct Conv3dOp {
         }
     }
 
-    __device__ Unit unit(int unit, int Nt, int row) const {
+    __device__ Unit unit(int unit, int Nt, int row, Smem&, int) const {
         const int NTC = a.Np / Nt;
         Unit u;
         u.sp = unit % a.splits;
@@ -285,7 +287,7 @@ struct Conv3dOp {
     }
 
     // fp16x2 column factor; the whole sum -> scale, shift, ReLU; a split's share -> its partial
-    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale, Smem&) const {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
             const int col = col0 + 8 * jj + 2 * t;
@@ -459,7 +461,7 @@ static ConvPlan conv_plan(int b, int r, int k, int c, int N, int np) {
 
 static const RingKernels kConvRing = {{{(const void*)tc_conv3d_kernel<2, 1>, (const void*)tc_conv3d_kernel<2, 2>},
                                        {(const void*)tc_conv3d_kernel<3, 1>, (const void*)tc_conv3d_kernel<3, 2>}},
-                                      "tc_conv3d_kernel"};
+                                      "tc_conv3d_kernel", Conv3dOp::kBudget};
 
 }  // namespace psa
 
@@ -524,8 +526,9 @@ extern "C" int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const flo
     a.tapmask = mask;
     a.splits = pl.splits;
     a.partial = pl.splits > 1 ? reinterpret_cast<float*>(wsb + pl.partial) : nullptr;
-    rc = ring_run(kConvRing, a, pl.tiles * (pl.Np / pl.Nt) * pl.splits, K, K, pl.Np, pl.Nt, wsrc, wsb + pl.img, wsb + pl.img,
-                  reinterpret_cast<unsigned int*>(wsb), st);
+    PSA_CUDA(cudaMemsetAsync(wsb, 0, 256, st));
+    rc = ring_run(kConvRing, a, pl.tiles * (pl.Np / pl.Nt) * pl.splits, RingWeights{K, K, pl.Np, pl.Nt, wsrc, wsb + pl.img, wsb + pl.img},
+                  reinterpret_cast<unsigned int*>(wsb), nullptr, st);
     if (rc != PSA_OK || pl.splits == 1) return rc;
     const long long total = a.rows * c_out;
     conv3d_finalize_kernel<<<(unsigned)min((total + 255) / 256, 8192LL), 256, 0, st>>>(a.rows, c_out, pl.Np, pl.splits, a.partial, scale, shift,

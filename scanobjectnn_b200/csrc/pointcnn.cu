@@ -220,6 +220,8 @@ struct PcnnDenseArgs {
 
 struct PcnnDenseOp {
     const PcnnDenseArgs& a;
+    static constexpr bool kClaim = false;
+    static constexpr uint32_t kBudget = kRingBudget;
     struct Smem {};
     struct Unit {
         int nb, col0;
@@ -234,18 +236,10 @@ struct PcnnDenseOp {
         const int NTC = a.Np / Nt, KC = a.Kp / 64;
         const long long row0 = (long long)(unit / NTC) * 128;
         const int nt = unit % NTC, r0 = 32 * pw, nr = (int)max(0LL, min(32LL, a.rows - row0 - r0));
-        for (int kb = 0; kb < KC; ++kb)
-            put((size_t)nt * KC + kb, [&](uint32_t xs) {
-                const int cc = (lane & 15) * 4, kk = kb * 64 + cc;
-                if (kk >= a.K) return;
-                for (int r = lane >> 4; r < nr; r += 2) {
-                    const int row = r0 + r;
-                    cp_async16(xs + (uint32_t)row * kRingXRow + (uint32_t)cc * 4u, a.x + (size_t)(row0 + row) * a.ldx + kk);
-                }
-            });
+        for (int kb = 0; kb < KC; ++kb) put((size_t)nt * KC + kb, [&](uint32_t xs) { stage_rows16(xs, a.x, a.ldx, row0, r0, nr, kb, a.K, lane); });
     }
 
-    __device__ Unit unit(int unit, int Nt, int row) const {
+    __device__ Unit unit(int unit, int Nt, int row, Smem&, int) const {
         const int NTC = a.Np / Nt;
         Unit u;
         u.nb = a.Kp / 64;
@@ -271,7 +265,7 @@ struct PcnnDenseOp {
     }
 
     // fp16x2 column factor, bias, ELU, the batch-norm affine; only the N real columns are written
-    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale, Smem&) const {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
             const int col = col0 + 8 * jj + 2 * t;
@@ -341,7 +335,7 @@ static PdPlan pd_plan(int K, int N, int np) {
 
 static const RingKernels kPdRing = {{{(const void*)tc_pcnn_dense_kernel<2, 1>, (const void*)tc_pcnn_dense_kernel<2, 2>},
                                      {(const void*)tc_pcnn_dense_kernel<3, 1>, (const void*)tc_pcnn_dense_kernel<3, 2>}},
-                                    "tc_pcnn_dense_kernel"};
+                                    "tc_pcnn_dense_kernel", PcnnDenseOp::kBudget};
 
 static int xconv_qt(int K, int Cf, int Cin) {
     const int q = kXconvSmemBudget / (xconv_query_floats(K, Cf, Cin) * (int)sizeof(float));
@@ -424,6 +418,7 @@ extern "C" int psa_dense_elu_affine(long long rows, int K, int N, const float* x
     float* wp = reinterpret_cast<float*>(wsb + pl.wp);
     const int rc = pad_cols(K, N, pl.Np, W, wp, st);
     if (rc != PSA_OK) return rc;
-    return ring_run(kPdRing, a, (rows + 127) / 128 * (pl.Np / pl.Nt), K, pl.Kp, pl.Np, pl.Nt, wp, wsb + pl.img2, wsb + pl.img3,
-                    reinterpret_cast<unsigned int*>(wsb), st);
+    PSA_CUDA(cudaMemsetAsync(wsb, 0, 256, st));
+    return ring_run(kPdRing, a, (rows + 127) / 128 * (pl.Np / pl.Nt), RingWeights{K, pl.Kp, pl.Np, pl.Nt, wp, wsb + pl.img2, wsb + pl.img3},
+                    reinterpret_cast<unsigned int*>(wsb), nullptr, st);
 }

@@ -82,6 +82,8 @@ struct SpiderArgs {
 
 struct SpiderOp {
     const SpiderArgs& a;
+    static constexpr bool kClaim = false;
+    static constexpr uint32_t kBudget = kRingBudget;
     struct Smem {
         int nbr[128 * kSpiderMaxK];                        // the unit's neighbour rows (global row index)
     };
@@ -118,7 +120,7 @@ struct SpiderOp {
             });
     }
 
-    __device__ Unit unit(int unit, int Nt, int row) const {
+    __device__ Unit unit(int unit, int Nt, int row, Smem&, int) const {
         const int NTC = a.N / Nt;
         Unit u;
         u.nb = a.K / 64;
@@ -168,7 +170,7 @@ struct SpiderOp {
     }
 
     // fp16x2 column factor, bias; pre-group-norm y
-    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale) const {
+    __device__ void epilogue(const Unit& u, const float (&acc)[32], int col0, int t, const float* colscale, Smem&) const {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
             const int col = col0 + 8 * jj + 2 * t;
@@ -323,7 +325,7 @@ static SpiderWs spider_ws(int b, int n, int c, int k, int T, int N) {
 
 static const RingKernels kSpiderRing = {{{(const void*)tc_spider_kernel<2, 1>, (const void*)tc_spider_kernel<2, 2>},
                                          {(const void*)tc_spider_kernel<3, 1>, (const void*)tc_spider_kernel<3, 2>}},
-                                        "tc_spider_kernel"};
+                                        "tc_spider_kernel", SpiderOp::kBudget};
 
 }  // namespace psa
 
@@ -368,8 +370,9 @@ extern "C" int psa_spider_conv_infer(int b, int n, int c, int k, int T, int c_ou
     spider_permute_kernel<<<1024, 256, 0, st>>>(k, c, T, c_out, W, wp);
     rc = check_launch("spider_permute_kernel");
     if (rc != PSA_OK) return rc;
-    return ring_run(kSpiderRing, a, (rows + 127) / 128 * (c_out / Nt), K, K, c_out, Nt, wp, wsb + ws.img2, wsb + ws.img3,
-                    reinterpret_cast<unsigned int*>(wsb), st);
+    PSA_CUDA(cudaMemsetAsync(wsb, 0, 256, st));
+    return ring_run(kSpiderRing, a, (rows + 127) / 128 * (c_out / Nt), RingWeights{K, K, c_out, Nt, wp, wsb + ws.img2, wsb + ws.img3},
+                    reinterpret_cast<unsigned int*>(wsb), nullptr, st);
 }
 
 extern "C" int psa_group_norm_affine(int b, int n, int c, int groups, float eps, const float* y, const float* gamma,

@@ -44,6 +44,8 @@ __device__ __forceinline__ void mbar_arrive1(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];\n" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __shfl_sync(0xffffffffu, v, 0); }
+// named barrier `id` of `count` threads
+__device__ __forceinline__ void unit_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
 // ---- bulk async copy global -> shared (TMA engine, 1-D, no tensor map), completion on an mbarrier ----
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {

@@ -16,9 +16,9 @@
 //
 // Kernels (both templated on NP, the pieces per operand -- Split<NP> in tc_common.cuh):
 //   tc_sa_kernel<NP,..>       SA level (specialised on its shape); optional centre weights = multi-layer EdgeConv over 3-D points
-//   tc_dense_kernel<NP,NC>    dense layer, persistent over 128-row x 64 NC-channel tiles, a producer warp feeding two consumer
-//                             warpgroups; also the training-mode forward (previous batch norm applied on load, column
-//                             statistics in the epilogue)
+//   tc_dense_kernel<NP,NC>    dense layer on the shared ring (ring_gemm.cuh), units of 128 rows x 64 NC channels claimed from a
+//                             counter; also the training-mode forward (previous batch norm applied on load, column statistics
+//                             in the epilogue)
 //   tc_group_all_kernel<..>   a three-layer group-all level with 128 points per cloud, fp16x2: one four-CTA cluster per cloud,
 //                             the activations between the layers kept in the cluster's shared memory
 // fp32 parity: operands are quantised by this code, so the tensor core only ever sees exactly representable values; fp32
@@ -37,6 +37,7 @@
 
 #include "common.cuh"
 #include "mlp_internal.cuh"
+#include "ring_gemm.cuh"
 #include "tc_common.cuh"
 
 namespace psa {
@@ -273,9 +274,6 @@ __device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[
 #pragma unroll
     for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
 }
-
-// named barrier `id` (1..15) over `count` threads: synchronises one unit of tc_sa_kernel without holding up the other
-__device__ __forceinline__ void unit_bar_sync(int id, int count) { asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory"); }
 
 // Specialised on the level shape: C1 = width of layer 1 (64 | 128), NL = tensor layers (1 | 2), N0 = width of the inner tensor
 // layer when NL = 2 (64 | 128).  The last layer's width is a runtime multiple of 64.
@@ -679,10 +677,9 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
 struct TcDenseArgs {
     long long rows;
     int K, Kp, N;          // Kp = K rounded up to 64
-    int pool_k;            // 1, 32, 64 or 128
+    int pool_k;            // 1, 32, 64 or a multiple of 128
     int relu;
     const float* x;        // (rows, K)
-    const uint8_t* image;  // weight image for (Kp, N)
     const float* scale;    // (N) or null
     const float* shift;    // (N) or null
     const float* xyz3;     // optional side input (rows, 3): out += xyz3 . w3 before scale/shift (the xyz rows of a
@@ -694,222 +691,117 @@ struct TcDenseArgs {
     const float* in_shift = nullptr;
     int in_relu = 0;
     float* stat_partial = nullptr;     // (row tiles, 2, N) or null
-    // operand split (see TcArgs): np = 2 launches raise *ovf, the np = 3 rerun is skipped unless *run_if != 0
-    unsigned int* ovf = nullptr;
-    const unsigned int* run_if = nullptr;
-    const unsigned int* wflag = nullptr;
-    const float* colscale = nullptr;   // np = 2: column factors 2^-e_n of the weight image (folded into the epilogue's scale)
-    // zeroed before the launch: tiles are claimed from it (a CTA that starts late or shares its SM with another stream's
-    // kernels simply takes fewer); null: CTA i takes tiles i, i + grid, ...
-    unsigned int* tile_counter = nullptr;
     // optional per-row-group input (pool_k == 1): row r adds group_add[r / group_rows] (N) before scale/shift, e.g. the
     // per-cloud product of a global feature tiled over the cloud's points
     const float* group_add = nullptr;
     long long group_rows = 0;
+    RingArgs ring;                     // W (Kp, N) in the format of NP, tile width 64 NC
 };
 
-// Persistent, warp-specialised.  CTA = two consumer warpgroups (rows 0-63 / 64-127 of a 128-row x Nt = 64 NC tile) + a
-// producer warpgroup, of which one warp works; setmaxnreg moves the registers to the consumers.  The producer claims tiles and
-// streams their 64-wide K blocks through a ring of stages, each holding the block's x rows (fp32, padded rows: conflict-free
-// fragment reads) and its weight block, one full mbarrier per stage; consumers release a stage through its empty mbarrier
-// (one arrival per warp).  The ring runs across tiles, so the next tile's first blocks land during this tile's epilogue.
-//   Per block the consumers issue the wgmma group, split the NEXT block's x (shared memory -> A fragments, batch norm + ReLU
-// of training mode, fp16 range tracking) while it runs, then wait and add the block's sum to the fp32 accumulators: the tensor
-// core's accumulation never runs over more than 64 K however long the dot product is, and every output sees the same sums
-// in the same order whatever the schedule.  One group in flight at a time, so every wait retires the same group on every path.
-//   Epilogue in the fragment layout: xyz side input, per-group input, affine, ReLU, then either float2 stores (+ per-tile column statistics) or
-// the max over pool_k rows; the cross-warp part synchronises the consumers on a named barrier.
-constexpr int kDenseThreads = 384, kDenseConsumers = 256;
-constexpr uint32_t kDenseXRow = 64u * 4u + 32u;           // bytes per staged x row: 8-bank offset between rows g and g + 1
-constexpr uint32_t kDenseXBytes = 128u * kDenseXRow;
-constexpr uint32_t kDenseRingBudget = 210u * 1024u;       // the ring's shared memory (next to s_red and the barriers)
-__host__ __device__ constexpr uint32_t dense_stage_bytes(int NP, int NC) { return tc_block_bytes(64 * NC, NP) + kDenseXBytes; }
-__host__ __device__ constexpr int dense_stages(int NP, int NC) {
-    return kDenseRingBudget / dense_stage_bytes(NP, NC) < 4u ? (int)(kDenseRingBudget / dense_stage_bytes(NP, NC)) : 4;
-}
-
+// The dense layer on the ring (ring_gemm.cuh), unit = 128-row tile x Nt = 64 NC-column tile, all Kp / 64 K blocks, claimed from
+// the launch's counter.  The producers stage x rows, 16 bytes per copy, or 4 for K % 4 != 0 / unaligned x; the consumers read rows
+// past `rows` and columns past K as zero.  Each unit's affine goes through shared memory, loaded once per column under the K loop:
+// fp16x2 folds the column factor 2^-e_n into the scale, and its inverse brings what the epilogue adds to the accumulators into their
+// units.  Epilogue in the fragment layout: xyz side input, per-group input, affine, ReLU, then either float2 stores (+ per-tile
+// column statistics) or the max over pool_k rows; the cross-warp part synchronises the consumers on named barrier 1.
 template <int NP, int NC>
-__global__ void __launch_bounds__(kDenseThreads, 1)
-tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
-    if (a.run_if != nullptr && *a.run_if == 0u) return;
-    constexpr int Nt = 64 * NC, S = dense_stages(NP, NC);
-    constexpr uint32_t bb = tc_block_bytes(Nt, NP), piece = Nt * 128u, SB = dense_stage_bytes(NP, NC);
-    static_assert(S >= 2, "the ring needs two stages");
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t s_full[S], s_empty[S];
-    __shared__ int s_tile[S];                                       // the tile a stage belongs to, -1: no more tiles
-    __shared__ float s_red[2][8][Nt];
-    __shared__ __align__(16) float s_aff[2][3][Nt];                 // [tile parity]: scale x column factor, shift, 1 / column factor
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    const int KC = a.Kp / 64, NTC = a.N / Nt;
-    const long long ntiles = (a.rows + 127) / 128 * NTC;
-    if (tid == 0) {
-        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1 + 32); mbar_init(&s_empty[i], kDenseConsumers / 32); }
-        fence_mbar_init();
-    }
-    __syncthreads();
+struct DenseOp {
+    static constexpr int Nt = 64 * NC;
+    const TcDenseArgs& a;
+    static constexpr bool kClaim = true;
+    static constexpr uint32_t kBudget = 210u * 1024u;         // four stages at NP = 2, NC = 1, next to Smem
+    struct Smem {
+        float red[2][8][Nt];                                  // per warp: column sums and sums of squares, or column maxima
+        __align__(16) float aff[2][3][Nt];                    // [unit parity]: scale x column factor, shift, 1 / column factor
+    };
+    struct Unit {
+        int nb, col0, par;
+        long long tile;                                       // row tile
+        long long r[2];
+        bool v[2];
+    };
 
-    if (warp >= kDenseConsumers / 32) {
-        // ---- producer ----
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        if (warp != kDenseConsumers / 32) return;
-        const bool vec = (a.K & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0;    // rows of x are 16-byte aligned
-        uint32_t q = 0;                                             // ring uses
-        for (long long i = 0;; ++i) {
-            long long tile = 0;
-            if (lane == 0) tile = a.tile_counter != nullptr ? (long long)atomicAdd(a.tile_counter, 1u) : (long long)blockIdx.x + i * gridDim.x;
-            tile = __shfl_sync(0xffffffffu, tile, 0);
-            const bool done = tile >= ntiles;
-            const long long row0 = tile / NTC * 128;
-            const int nt = (int)(tile % NTC), nrows = done ? 0 : (int)min(128LL, a.rows - row0);
-            for (int kb = 0; kb < KC; ++kb, ++q) {
-                const int s = (int)(q % S);
-                if (q >= (uint32_t)S) mbar_wait(&s_empty[s], ((q / S) - 1u) & 1u);
-                if (lane == 0) {
-                    s_tile[s] = done ? -1 : (int)tile;
-                    if (done) {
-                        mbar_arrive1(&s_full[s]);
-                    } else {
-                        mbar_expect_tx(&s_full[s], bb);
-                        const uint8_t* src = a.image + ((size_t)nt * KC + kb) * bb;
-                        for (uint32_t o = 0; o < bb; o += 16384u) bulk_g2s(base + (uint32_t)s * SB + o, src + o, min(16384u, bb - o), &s_full[s]);
-                    }
-                }
-                if (!done) {
-                    // x rows [row0, row0 + nrows) x columns [64 kb, 64 kb + kw): 16-byte async copies, a warp covering two rows per
-                    // instruction, or 4-byte ones for odd K / unaligned x.  Rows past `rows` and columns past K are left stale: the
-                    // consumers read them as zero.
-                    const uint32_t xs = smem_u32(base + (uint32_t)s * SB + bb);
-                    const float* xb = a.x + (size_t)row0 * a.K + kb * 64;
-                    const int kw = min(64, a.K - kb * 64);
-                    if (vec) {
-                        for (int e = lane; e < nrows * 16; e += 32) {
-                            const int r = e >> 4, c = (e & 15) * 4;
-                            if (c < kw) cp_async16(xs + (uint32_t)r * kDenseXRow + (uint32_t)c * 4u, xb + (size_t)r * a.K + c);
-                        }
-                    } else {
-                        for (int e = lane; e < nrows * 64; e += 32) {
-                            const int r = e >> 6, c = e & 63;
-                            if (c < kw) cp_async4(xs + (uint32_t)r * kDenseXRow + (uint32_t)c * 4u, xb + (size_t)r * a.K + c);
-                        }
-                    }
-                }
-                cp_async_mbar_arrive(&s_full[s]);                  // one arrival per lane, once its copies have landed
-                if (done) break;
-            }
-            if (done) return;
+    __device__ int units(int) const { return (int)((a.rows + 127) / 128 * (a.N / Nt)); }
+
+    template <class Put>
+    __device__ void produce(int unit, int, int pw, int lane, Smem&, Put&& put) const {
+        const int NTC = a.N / Nt, KC = a.Kp / 64;
+        const long long row0 = (long long)(unit / NTC) * 128;
+        const int nt = unit % NTC, r0 = 32 * pw, nr = (int)max(0LL, min(32LL, a.rows - row0 - r0));
+        if ((a.K & 3) == 0 && (reinterpret_cast<uintptr_t>(a.x) & 15) == 0) {     // rows of x are 16-byte aligned
+            for (int kb = 0; kb < KC; ++kb) put((size_t)nt * KC + kb, [&](uint32_t xs) { stage_rows16(xs, a.x, a.K, row0, r0, nr, kb, a.K, lane); });
+            return;
         }
+        for (int kb = 0; kb < KC; ++kb)
+            put((size_t)nt * KC + kb, [&](uint32_t xs) {
+#pragma unroll 1
+                for (int e = lane; e < nr * 64; e += 32) {
+                    const int row = r0 + (e >> 6), c = e & 63;
+                    if (kb * 64 + c < a.K) cp_async4(xs + (uint32_t)row * kRingXRow + (uint32_t)c * 4u, a.x + (size_t)(row0 + row) * a.K + kb * 64 + c);
+                }
+            });
     }
 
-    // ---- consumers: warp w holds tile rows 16w + g and 16w + g + 8 ----
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n");
-    const int g = lane >> 2, t = lane & 3;
-    uint32_t ovf = 0u;
-    uint32_t q = 0;                                                 // ring uses
-    for (uint32_t par = 0;; par ^= 1u) {
-        mbar_wait(&s_full[q % S], (q / S) & 1u);
-        const int tile = s_tile[q % S];
-        if (tile < 0) break;
-        const long long row0 = (long long)(tile / NTC) * 128;
-        const int nt = tile % NTC;
-        // the tile's affine through shared memory, loaded once per column under the K loop and read by the epilogue after the
-        // barrier in front of it; fp16x2: the column factor 2^-e_n joins the scale, its inverse brings what the epilogue adds to
-        // the accumulators into their units.  Two buffers by tile parity: the write for this tile follows the barrier of the last
-        // one, so it cannot overtake the epilogue of the tile before.
-        float (&aff)[3][Nt] = s_aff[par];
+    // the unit's affine into aff[n & 1]: the write for this unit follows the barrier of the last one, so it cannot overtake the
+    // epilogue of the unit before
+    __device__ Unit unit(int unit, int, int row, Smem& sm, int n) const {
+        const int NTC = a.N / Nt, tid = threadIdx.x;
+        Unit u;
+        u.nb = a.Kp / 64;
+        u.tile = unit / NTC;
+        u.col0 = unit % NTC * Nt;
+        u.par = n & 1;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            u.r[i] = u.tile * 128 + row + 8 * i;
+            u.v[i] = u.r[i] < a.rows;
+        }
         if (tid < Nt) {
-            const int col = nt * Nt + tid;
-            const float cs = NP == 2 ? __ldg(a.colscale + col) : 1.f;
-            aff[0][tid] = (a.scale ? __ldg(a.scale + col) : 1.f) * cs;
-            aff[1][tid] = a.shift ? __ldg(a.shift + col) : 0.f;
-            aff[2][tid] = NP == 2 ? pow2_rcp(cs) : 1.f;
+            const int col = u.col0 + tid;
+            const float cs = NP == 2 ? __ldg(a.ring.colscale + col) : 1.f;
+            sm.aff[u.par][0][tid] = (a.scale ? __ldg(a.scale + col) : 1.f) * cs;
+            sm.aff[u.par][1][tid] = a.shift ? __ldg(a.shift + col) : 0.f;
+            sm.aff[u.par][2][tid] = NP == 2 ? pow2_rcp(cs) : 1.f;
         }
-        const long long r[2] = {row0 + warp * 16 + g, row0 + warp * 16 + g + 8};
-        const bool v[2] = {r[0] < a.rows, r[1] < a.rows};
+        return u;
+    }
 
-        // x block of ring use u -> A fragments: rows past `rows` and columns past K read as zero (as the staged bytes there
-        // are stale), then the previous layer's batch norm + ReLU of training mode
-        auto prep = [&](uint32_t (&A)[NP][4][4], uint32_t u, int kb) {
-            const float* xs = reinterpret_cast<const float*>(base + (u % S) * SB + bb);
+    // the row and K masks, then the previous layer's batch norm + ReLU of training mode
+    __device__ void load(const Unit& u, const float* xs, int kb, int t, float2 (&x)[4][2][2]) const {
 #pragma unroll
-            for (int s = 0; s < 4; ++s)
+        for (int s = 0; s < 4; ++s)
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int kl = 16 * s + 8 * h + 2 * t, k = kb * 64 + kl;
-                        float2 x = make_float2(0.f, 0.f);
-                        if (v[i]) {
-                            const float2 y = *reinterpret_cast<const float2*>(xs + (warp * 16 + g + 8 * i) * (int)(kDenseXRow / 4) + kl);
-                            if (k < a.K) x.x = y.x;
-                            if (k + 1 < a.K) x.y = y.y;
-                            if (a.in_scale != nullptr) {
-                                if (k < a.K) { x.x = fmaf(x.x, __ldg(a.in_scale + k), __ldg(a.in_shift + k)); if (a.in_relu) x.x = fmaxf(x.x, 0.f); }
-                                if (k + 1 < a.K) { x.y = fmaf(x.y, __ldg(a.in_scale + k + 1), __ldg(a.in_shift + k + 1)); if (a.in_relu) x.y = fmaxf(x.y, 0.f); }
-                            }
+                for (int i = 0; i < 2; ++i) {
+                    const int k = kb * 64 + 16 * s + 8 * h + 2 * t;
+                    float2 v = make_float2(0.f, 0.f);
+                    if (u.v[i]) {
+                        const float2 y = staged_pair(xs, s, h, i, t);
+                        if (k < a.K) v.x = y.x;
+                        if (k + 1 < a.K) v.y = y.y;
+                        if (a.in_scale != nullptr) {
+                            if (k < a.K) { v.x = fmaf(v.x, __ldg(a.in_scale + k), __ldg(a.in_shift + k)); if (a.in_relu) v.x = fmaxf(v.x, 0.f); }
+                            if (k + 1 < a.K) { v.y = fmaf(v.y, __ldg(a.in_scale + k + 1), __ldg(a.in_shift + k + 1)); if (a.in_relu) v.y = fmaxf(v.y, 0.f); }
                         }
-                        put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
                     }
-        };
-        float acc[NC][32];
-        // block kb (ring use u): issue its group on A, prepare block kb + 1 into An while it runs, wait, release the stage, add.
-        // bf16x3 128-wide tiles issue one 64-channel chunk per group (the next block is prepared under the second), so that
-        // two A buffers, the accumulators and one chunk's sum fit the consumers' 232 registers.
-        constexpr int CG = NP == 3 && NC == 2 ? 1 : NC;            // 64-channel chunks per group
-        auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], uint32_t u, int kb) {
-            const uint32_t wb = smem_u32(base + (u % S) * SB);
-#pragma unroll
-            for (int c0 = 0; c0 < NC; c0 += CG) {
-                float d[CG][32];
-                wg_fence();
-#pragma unroll
-                for (int tt = 0; tt < Split<NP>::kTerms; ++tt)
-#pragma unroll
-                    for (int s = 0; s < 4; ++s)
-#pragma unroll
-                        for (int c = 0; c < CG; ++c)
-                            wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][s][0], A[Split<NP>::a(tt)][s][1], A[Split<NP>::a(tt)][s][2], A[Split<NP>::a(tt)][s][3],
-                                          wg_desc(wb + Split<NP>::w(tt) * piece + (uint32_t)(c0 + c) * 8192u + (uint32_t)s * 32u), (tt | s) ? 1u : 0u);
-                wg_commit();
-                if (c0 + CG == NC && kb + 1 < KC) {
-                    mbar_wait(&s_full[(u + 1) % S], ((u + 1) / S) & 1u);
-                    prep(An, u + 1, kb + 1);
+                    x[s][h][i] = v;
                 }
-                wg_wait_all();
-                if (c0 + CG == NC) {
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive1(&s_empty[u % S]);           // x read, weights consumed: the stage may be refilled
-                }
-#pragma unroll
-                for (int c = 0; c < CG; ++c) {
-                    wg_fence_acc(d[c]);
-#pragma unroll
-                    for (int e = 0; e < 32; ++e) acc[c0 + c][e] = kb ? acc[c0 + c][e] + d[c][e] : d[c][e];
-                }
-            }
-        };
-        {
-            uint32_t A0[NP][4][4], A1[NP][4][4];
-            prep(A0, q, 0);
-            for (int kb = 0;; kb += 2) {
-                step(A0, A1, q + kb, kb);
-                if (kb + 1 == KC) break;
-                step(A1, A0, q + kb + 1, kb + 1);
-                if (kb + 2 == KC) break;
-            }
-        }
-        q += KC;
+    }
 
-        // ---- epilogue ----
-        unit_bar_sync(1, kDenseConsumers);                          // the tile's affine is in `aff`
+    // One 64-column chunk.  Its cross-warp fold reads the chunk's own columns of `red`, so the next chunk's writes need no barrier;
+    // the next unit's writes follow the barrier in front of its first chunk.
+    __device__ void epilogue(const Unit& u, float (&acc)[32], int col0, int t, const float*, Smem& sm) const {
+        const int tid = threadIdx.x, warp = tid >> 5, g = (tid & 31) >> 2, cl0 = col0 - u.col0;
+        const float (&aff)[3][Nt] = sm.aff[u.par];
+        if (cl0 == 0) unit_bar_sync(1, kRingConsumers);        // the unit's affine is in `aff`
         float xs[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
         if (a.xyz3 != nullptr)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
-                if (v[i])
+                if (u.v[i])
 #pragma unroll
-                    for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz3 + (size_t)r[i] * 3 + k);
+                    for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz3 + (size_t)u.r[i] * 3 + k);
         // the per-group input, added to the accumulators in a pass of its own so that the loop below is the same code with or
         // without it.  Rows g and g + 8 may lie in different groups, and groups need not align with the 128-row tiles.  fp16x2:
         // the accumulators hold the product times 2^e_n, and so must what is added to them (exact, the rounding of the sum is
@@ -917,105 +809,108 @@ tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
         if (a.group_add != nullptr)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
-                if (v[i]) {
-                    const float* ga = a.group_add + (size_t)(r[i] / a.group_rows) * a.N + nt * Nt + 2 * t;
+                if (u.v[i]) {
+                    const float* ga = a.group_add + (size_t)(u.r[i] / a.group_rows) * a.N + col0 + 2 * t;
 #pragma unroll
-                    for (int c = 0; c < NC; ++c)
-#pragma unroll
-                        for (int j = 0; j < 8; ++j) {
-                            const float2 u = __ldg(reinterpret_cast<const float2*>(ga + c * 64 + 8 * j));
-                            const float2 f = *reinterpret_cast<const float2*>(&aff[2][c * 64 + 8 * j + 2 * t]);
-                            acc[c][4 * j + 2 * i] = fmaf(u.x, f.x, acc[c][4 * j + 2 * i]);
-                            acc[c][4 * j + 2 * i + 1] = fmaf(u.y, f.y, acc[c][4 * j + 2 * i + 1]);
-                        }
-                }
-#pragma unroll
-        for (int c = 0; c < NC; ++c)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                const int cl = c * 64 + 8 * j + 2 * t;
-                float y[2][2];
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int col = nt * Nt + cl + e;
-                    const float sc = aff[0][cl + e], sh = aff[1][cl + e];
-                    float w0 = 0.f, w1 = 0.f, w2 = 0.f;
-                    if (a.xyz3 != nullptr) {
-                        const float f = aff[2][cl + e];
-                        w0 = __ldg(a.w3 + col) * f; w1 = __ldg(a.w3 + a.N + col) * f; w2 = __ldg(a.w3 + 2 * a.N + col) * f;
-                    }
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        float x = acc[c][4 * j + 2 * i + e];
-                        if (a.xyz3 != nullptr) x = fmaf(xs[i][2], w2, fmaf(xs[i][1], w1, fmaf(xs[i][0], w0, x)));
-                        x = fmaf(x, sc, sh);
-                        if (a.relu) x = fmaxf(x, 0.f);
-                        y[i][e] = x;
+                    for (int j = 0; j < 8; ++j) {
+                        const float2 gv = __ldg(reinterpret_cast<const float2*>(ga + 8 * j));
+                        const float2 f = *reinterpret_cast<const float2*>(&aff[2][cl0 + 8 * j + 2 * t]);
+                        acc[4 * j + 2 * i] = fmaf(gv.x, f.x, acc[4 * j + 2 * i]);
+                        acc[4 * j + 2 * i + 1] = fmaf(gv.y, f.y, acc[4 * j + 2 * i + 1]);
                     }
                 }
-                if (a.pool_k == 1) {
 #pragma unroll
-                    for (int i = 0; i < 2; ++i)
-                        if (v[i]) *reinterpret_cast<float2*>(a.out + (size_t)r[i] * a.N + nt * Nt + cl) = make_float2(y[i][0], y[i][1]);
-                    if (a.stat_partial != nullptr) {
+        for (int j = 0; j < 8; ++j) {
+            const int cl = cl0 + 8 * j + 2 * t;
+            float y[2][2];
 #pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            float ssum = 0.f, ssq = 0.f;
+            for (int e = 0; e < 2; ++e) {
+                const int col = u.col0 + cl + e;
+                const float sc = aff[0][cl + e], sh = aff[1][cl + e];
+                float w0 = 0.f, w1 = 0.f, w2 = 0.f;
+                if (a.xyz3 != nullptr) {
+                    const float f = aff[2][cl + e];
+                    w0 = __ldg(a.w3 + col) * f; w1 = __ldg(a.w3 + a.N + col) * f; w2 = __ldg(a.w3 + 2 * a.N + col) * f;
+                }
 #pragma unroll
-                            for (int i = 0; i < 2; ++i)
-                                if (v[i]) { ssum += y[i][e]; ssq = fmaf(y[i][e], y[i][e], ssq); }
-                            ssum = warp_rowsum16(ssum);
-                            ssq = warp_rowsum16(ssq);
-                            if (g == 0) { s_red[0][warp][cl + e] = ssum; s_red[1][warp][cl + e] = ssq; }
-                        }
-                    }
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const float m = warp_rowmax16(v[0] ? y[0][e] : -FLT_MAX, v[1] ? y[1][e] : -FLT_MAX);
-                        if (g == 0) s_red[0][warp][cl + e] = m;
-                    }
+                for (int i = 0; i < 2; ++i) {
+                    float x = acc[4 * j + 2 * i + e];
+                    if (a.xyz3 != nullptr) x = fmaf(xs[i][2], w2, fmaf(xs[i][1], w1, fmaf(xs[i][0], w0, x)));
+                    x = fmaf(x, sc, sh);
+                    if (a.relu) x = fmaxf(x, 0.f);
+                    y[i][e] = x;
                 }
             }
+            if (a.pool_k == 1) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (u.v[i]) *reinterpret_cast<float2*>(a.out + (size_t)u.r[i] * a.N + u.col0 + cl) = make_float2(y[i][0], y[i][1]);
+                if (a.stat_partial != nullptr) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        float ssum = 0.f, ssq = 0.f;
+#pragma unroll
+                        for (int i = 0; i < 2; ++i)
+                            if (u.v[i]) { ssum += y[i][e]; ssq = fmaf(y[i][e], y[i][e], ssq); }
+                        ssum = warp_rowsum16(ssum);
+                        ssq = warp_rowsum16(ssq);
+                        if (g == 0) { sm.red[0][warp][cl + e] = ssum; sm.red[1][warp][cl + e] = ssq; }
+                    }
+                }
+            } else {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float m = warp_rowmax16(u.v[0] ? y[0][e] : -FLT_MAX, u.v[1] ? y[1][e] : -FLT_MAX);
+                    if (g == 0) sm.red[0][warp][cl + e] = m;
+                }
+            }
+        }
         if (a.pool_k == 1) {
             if (a.stat_partial != nullptr) {
                 // per-tile column statistics, the eight warps' 16-row partials folded in warp order (deterministic)
-                unit_bar_sync(1, kDenseConsumers);
-                for (int cl = tid; cl < Nt; cl += kDenseConsumers) {
+                unit_bar_sync(1, kRingConsumers);
+                if (tid < 64) {
+                    const int cl = cl0 + tid;
                     float t0 = 0.f, t1 = 0.f;
-                    for (int w = 0; w < 8; ++w) { t0 += s_red[0][w][cl]; t1 += s_red[1][w][cl]; }
-                    float* dst = a.stat_partial + (size_t)(tile / NTC) * 2 * a.N;
-                    dst[nt * Nt + cl] = t0;
-                    dst[a.N + nt * Nt + cl] = t1;
+                    for (int w = 0; w < 8; ++w) { t0 += sm.red[0][w][cl]; t1 += sm.red[1][w][cl]; }
+                    float* dst = a.stat_partial + (size_t)u.tile * 2 * a.N;
+                    dst[u.col0 + cl] = t0;
+                    dst[a.N + u.col0 + cl] = t1;
                 }
-                unit_bar_sync(1, kDenseConsumers);                         // s_red is rewritten by the next tile
             }
         } else {
-            unit_bar_sync(1, kDenseConsumers);
+            unit_bar_sync(1, kRingConsumers);
             const bool big = a.pool_k > 128;                             // the whole 128-row tile lies inside one group
             const int wpg = big ? 8 : a.pool_k / 16;                     // warps per pooling group
-            for (int e = tid; e < (8 / wpg) * Nt; e += kDenseConsumers) {
-                const int grp = e / Nt, cl = e % Nt;
-                const long long rs = row0 + grp * wpg * 16;
+            for (int e = tid; e < (8 / wpg) * 64; e += kRingConsumers) {
+                const int grp = e / 64, cl = cl0 + e % 64;
+                const long long rs = u.tile * 128 + grp * wpg * 16;
                 if (rs >= a.rows) continue;
-                float mx = s_red[0][grp * wpg][cl];
-                for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, s_red[0][grp * wpg + w][cl]);
+                float mx = sm.red[0][grp * wpg][cl];
+                for (int w = 1; w < wpg; ++w) mx = fmaxf(mx, sm.red[0][grp * wpg + w][cl]);
                 const long long wg = rs / a.pool_k;
                 if (!big) {
-                    a.out[(size_t)wg * a.N + nt * Nt + cl] = mx;
+                    a.out[(size_t)wg * a.N + u.col0 + cl] = mx;
                 } else {
                     int code = __float_as_int(mx);
                     code = code >= 0 ? code : code ^ 0x7fffffff;
-                    atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + nt * Nt + cl, code);
+                    atomicMax(reinterpret_cast<int*>(a.out) + (size_t)wg * a.N + u.col0 + cl, code);
                 }
             }
-            unit_bar_sync(1, kDenseConsumers);
         }
     }
-    if constexpr (NP == 2) {
-        if (f16x2_overflowed(ovf) || (tid == 0 && a.wflag != nullptr && *a.wflag != 0u)) atomicOr(a.ovf, 1u);
-    }
+};
+
+template <int NP, int NC>
+__global__ void __launch_bounds__(kRingThreads, 1) tc_dense_kernel(const __grid_constant__ TcDenseArgs a) {
+    ring_gemm<NP, NC>(DenseOp<NP, NC>{a}, a.ring);
 }
+
+static_assert(ring_stages(2, 1, DenseOp<2, 1>::kBudget) == 4 && ring_stages(3, 1, DenseOp<3, 1>::kBudget) == 3 &&
+              ring_stages(2, 2, DenseOp<2, 2>::kBudget) == 3 && ring_stages(3, 2, DenseOp<3, 2>::kBudget) == 2, "stages of the dense ring");
+static const RingKernels kDenseRing = {{{(const void*)tc_dense_kernel<2, 1>, (const void*)tc_dense_kernel<2, 2>},
+                                        {(const void*)tc_dense_kernel<3, 1>, (const void*)tc_dense_kernel<3, 2>}},
+                                       "tc_dense_kernel", DenseOp<2, 1>::kBudget};
 
 bool tc_dense_eligible(long long rows, int K, int N, int pool_k) {
     if (rows < 128 || K < 32 || N < 64 || (N % 64) != 0) return false;
@@ -1068,50 +963,11 @@ const float* image_colscale(const uint8_t* image, int Kp, int N) {
     return reinterpret_cast<const float*>(image + tc_image_colscale_off(Kp, N, 2));
 }
 
-template <int NP, int NC>
-static int launch_tc_dense_shape(const TcDenseArgs& a, cudaStream_t st) {
-    const size_t smem = (size_t)dense_stages(NP, NC) * dense_stage_bytes(NP, NC) + 1024;
-    PSA_CUDA(cudaFuncSetAttribute(tc_dense_kernel<NP, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    // persistent CTAs: as many as are resident at once, never more than there are tiles
-    int dev = 0, sms = 0, per_sm = 0;
-    PSA_CUDA(cudaGetDevice(&dev));
-    PSA_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PSA_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, tc_dense_kernel<NP, NC>, kDenseThreads, smem));
-    const long long tiles = (a.rows + 127) / 128 * (a.N / (64 * NC)), resident = (long long)sms * (per_sm > 0 ? per_sm : 1);
-    tc_dense_kernel<NP, NC><<<(unsigned)(tiles < resident ? tiles : resident), kDenseThreads, smem, st>>>(a);
-    return check_launch("tc_dense_kernel");
-}
-
-// one launch of a dense layer with NP pieces; `image` holds the weights in that format
-template <int NP>
-static int launch_tc_dense_np(TcDenseArgs& a, int Nt, cudaStream_t st) {
-    const bool big = a.pool_k > 128;
-    if (big) { int rc0 = launch_fill_ord_neg_inf(a.rows / a.pool_k * a.N, a.out, st, a.run_if); if (rc0 != PSA_OK) return rc0; }
-    const int rc = Nt == 128 ? launch_tc_dense_shape<NP, 2>(a, st) : launch_tc_dense_shape<NP, 1>(a, st);
-    if (rc != PSA_OK) return rc;
-    if (big) return launch_decode_ord(a.rows / a.pool_k * a.N, a.out, st, a.run_if);
-    return PSA_OK;
-}
-
 // the zeroed 256-byte word region of psa_shared_mlp / psa_sa_group_all_infer: range flag of layer l at [l], the tile counters
 // of layer l and of its rerun at [kTileCounterWords + 2 l, + 1]
 constexpr int kTileCounterWords = PSA_MAX_MLP_LAYERS;
 
-// the guarded bf16x3 rerun of a dense layer (`a`: the layer's arguments; its np = 2 fields are reset), a no-op unless *run_if != 0.
-// A prebuilt image carries its bf16x3 twin behind the fp16x2 blocks (psa_prepare_weight_image); otherwise the twin is built into
-// ws_img (tc_dense_image_bytes(K, N)), conditionally too.
-static int launch_tc_dense_rerun(TcDenseArgs a, int Nt, const float* W, const uint8_t* prebuilt, uint8_t* ws_img, const unsigned int* run_if,
-                                 unsigned int* counter, cudaStream_t st) {
-    uint8_t* img3 = ws_img + tc_dense_image_off3(a.K, a.N);
-    if (prebuilt != nullptr) {
-        img3 = const_cast<uint8_t*>(prebuilt) + tc_image_alloc_bytes(a.Kp, a.N, 2);
-    } else {
-        const int rc = build_image(a.K, a.Kp, a.N, Nt | kImageBf16x3, W, img3, st, run_if);
-        if (rc != PSA_OK) return rc;
-    }
-    a.image = img3; a.ovf = nullptr; a.wflag = nullptr; a.colscale = nullptr; a.run_if = run_if; a.tile_counter = counter;
-    return launch_tc_dense_np<3>(a, Nt, st);
-}
+static long long tc_dense_units(long long rows, int N, int Nt) { return (rows + 127) / 128 * (N / Nt); }
 
 // out = relu?((x . W [+ xyz3 . w3] [+ group_add[r / group_rows]]) * scale + shift) on the tensor cores, optional max over runs of
 // pool_k rows (not with group_add).
@@ -1129,20 +985,10 @@ int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const fl
     a.rows = rows; a.K = K; a.Kp = Kp; a.N = N; a.pool_k = pool_k; a.relu = relu;
     a.x = x; a.scale = scale; a.shift = shift; a.out = out; a.xyz3 = xyz3; a.w3 = w3;
     a.group_add = group_add; a.group_rows = group_rows;
-    a.tile_counter = counters;
-    uint8_t* img3 = ws_img + tc_dense_image_off3(K, N);
-    int rc;
-    if (g_tc_np == 3) {
-        if (prebuilt == nullptr) { rc = build_image(K, Kp, N, Nt | kImageBf16x3, W, img3, st); if (rc != PSA_OK) return rc; }
-        a.image = prebuilt ? prebuilt : img3;
-        return launch_tc_dense_np<3>(a, Nt, st);
-    }
-    if (prebuilt == nullptr) { rc = build_image(K, Kp, N, Nt | kImageF16x2, W, ws_img, st); if (rc != PSA_OK) return rc; }
-    a.image = prebuilt ? prebuilt : ws_img;
-    a.ovf = flag; a.wflag = image_trailer(a.image, Kp, N); a.colscale = image_colscale(a.image, Kp, N);
-    rc = launch_tc_dense_np<2>(a, Nt, st);
-    if (rc != PSA_OK) return rc;
-    return launch_tc_dense_rerun(a, Nt, W, prebuilt, ws_img, flag, counters + 1, st);   // a no-op unless the fp16x2 pass raised the flag
+    RingPool pool;
+    if (pool_k > 128) { pool.out = out; pool.count = rows / pool_k * N; }
+    return ring_run(kDenseRing, a, tc_dense_units(rows, N, Nt), RingWeights{K, Kp, N, Nt, W, ws_img, ws_img + tc_dense_image_off3(K, N), prebuilt},
+                    flag, counters, st, pool);
 }
 
 // Training-mode forward of one layer on tc_dense_kernel: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
@@ -1160,9 +1006,10 @@ int launch_tc_dense_train(long long rows, int K, int N, const float* x, const fl
     if (rc != PSA_OK) return rc;
     TcDenseArgs a;
     a.rows = rows; a.K = K; a.Kp = Kp; a.N = N; a.pool_k = 1; a.relu = 0;
-    a.x = x; a.image = image_ws; a.scale = nullptr; a.shift = bias; a.out = y; a.xyz3 = nullptr; a.w3 = nullptr;
+    a.x = x; a.scale = nullptr; a.shift = bias; a.out = y; a.xyz3 = nullptr; a.w3 = nullptr;
     a.in_scale = in_scale; a.in_shift = in_shift; a.in_relu = in_relu; a.stat_partial = stat_partial;
-    return launch_tc_dense_np<3>(a, 128, st);
+    a.ring.image = image_ws;
+    return ring_launch(kDenseRing, 3, 128, &a, tc_dense_units(rows, N, 128), st);
 }
 
 // A prebuilt image (psa_prepare_weight_image) is used when its format, tile width and first row match; otherwise null (the
@@ -1342,7 +1189,7 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
 //     W1 as the epilogue side input) and layer 1 in one 64- or 128-column pass each, the last layer in 128-column passes, each
 //     followed by the max over the 128 rows -- a plain store of out[cloud, col];
 //   * the slices of layers 0 and 1 stay in the CTA's own shared memory as fp32 after the affine and ReLU, in the padded rows of
-//     tc_dense_kernel's x stages (kDenseXRow), one 128 x 64 block per 64 columns.  K block kb of layer l + 1 lives in the CTA
+//     tc_dense_kernel's x stages (kRingXRow), one 128 x 64 block per 64 columns.  K block kb of layer l + 1 lives in the CTA
 //     that owns those columns of layer l: the consumers read it with ld.shared::cluster and split it into A fragments while
 //     block kb - 1's wgmma group runs, as tc_dense_kernel does with its staged x.  Layer 0's input rows are read from global
 //     memory the same way (4 KB of 32-byte sectors per block and warp, from L2: the four CTAs of a cloud read the same rows);
@@ -1383,7 +1230,7 @@ constexpr uint32_t kGaStageBytes = 32768u;      // one K block of 128 weight col
 constexpr uint32_t kGaSmemBudget = 222u * 1024u;
 // dynamic shared memory: 1 KB alignment, the ring, the slices of layers 0 and 1 (W0 + W1 columns), the affine of every layer
 __host__ __device__ inline uint32_t group_all_smem(int W0, int W1, int W2) {
-    return 1024u + kGaStages * kGaStageBytes + (uint32_t)(W0 + W1) / 64u * kDenseXBytes + 12u * (uint32_t)(W0 + W1 + W2);
+    return 1024u + kGaStages * kGaStageBytes + (uint32_t)(W0 + W1) / 64u * kRingXBytes + 12u * (uint32_t)(W0 + W1 + W2);
 }
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -1426,7 +1273,7 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
 
 // NC0, NC1: 64-column chunks of the layer-0 and layer-1 slices (one pass each); the last layer runs in 128-column passes
 template <int NC0, int NC1>
-__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kDenseThreads, 1)
+__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kRingThreads, 1)
 tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
     constexpr int NP = 2, S = kGaStages;
     constexpr uint32_t piece = 8192u, chunk = 16384u;               // a 64-column chunk of a stage: its two pieces
@@ -1440,8 +1287,8 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
     constexpr int W0 = 64 * NC0, W1 = 64 * NC1;                     // slice widths
     const int W2 = a.N[2] / 4;
     uint8_t* slice0 = base + S * kGaStageBytes;
-    uint8_t* slice1 = slice0 + NC0 * kDenseXBytes;
-    float* aff0 = reinterpret_cast<float*>(slice1 + NC1 * kDenseXBytes);   // per layer: scale x column factor, shift, 1 / column factor
+    uint8_t* slice1 = slice0 + NC0 * kRingXBytes;
+    float* aff0 = reinterpret_cast<float*>(slice1 + NC1 * kRingXBytes);   // per layer: scale x column factor, shift, 1 / column factor
     float* aff1 = aff0 + 3 * W0;
     float* aff2 = aff1 + 3 * W1;
     {
@@ -1449,7 +1296,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
         const int W[3] = {W0, W1, W2};
 #pragma unroll
         for (int l = 0; l < 3; ++l)
-            for (int i = tid; i < W[l]; i += kDenseThreads) {
+            for (int i = tid; i < W[l]; i += kRingThreads) {
                 const int col = (int)rank * W[l] + i;
                 const float cs = __ldg(a.colscale[l] + col);
                 aff[l][i] = (a.scale[l] ? __ldg(a.scale[l] + col) : 1.f) * cs;
@@ -1458,7 +1305,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
             }
     }
     if (tid == 0) {
-        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], kDenseConsumers / 32); }
+        for (int i = 0; i < S; ++i) { mbar_init(&s_full[i], 1); mbar_init(&s_empty[i], kRingConsumers / 32); }
         mbar_init(&s_ready[0], 4); mbar_init(&s_ready[1], 4); mbar_init(&s_done, 4);
         fence_mbar_init();
     }
@@ -1466,10 +1313,10 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
     cluster_sync_all();                                             // hazard 1: the peers' barriers are initialised
     const int KC[3] = {a.c / 64, 4 * W0 / 64, 4 * W1 / 64};
 
-    if (warp >= kDenseConsumers / 32) {
+    if (warp >= kRingConsumers / 32) {
         // ---- producer: the weight blocks of every pass, in the consumers' order ----
         asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        if (warp != kDenseConsumers / 32) return;
+        if (warp != kRingConsumers / 32) return;
         uint32_t u = 0;                                             // ring uses
 #pragma unroll
         for (int l = 0; l < 3; ++l) {
@@ -1525,7 +1372,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                         }
             } else {
                 constexpr int Wp = L == 1 ? W0 : W1;                // the input's slice width: block kb is in CTA kb * 64 / Wp
-                const uint32_t src = mapa_shared(smem_u32(L == 1 ? slice0 : slice1) + (uint32_t)((kb * 64) % Wp / 64) * kDenseXBytes,
+                const uint32_t src = mapa_shared(smem_u32(L == 1 ? slice0 : slice1) + (uint32_t)((kb * 64) % Wp / 64) * kRingXBytes,
                                                  (uint32_t)(kb * 64 / Wp));
 #pragma unroll
                 for (int s = 0; s < 4; ++s)
@@ -1533,7 +1380,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                     for (int h = 0; h < 2; ++h)
 #pragma unroll
                         for (int i = 0; i < 2; ++i) {
-                            const float2 x = ld_cluster_f32x2(src + (uint32_t)rl[i] * kDenseXRow + (uint32_t)(16 * s + 8 * h + 2 * t) * 4u);
+                            const float2 x = ld_cluster_f32x2(src + (uint32_t)rl[i] * kRingXRow + (uint32_t)(16 * s + 8 * h + 2 * t) * 4u);
                             put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
                         }
             }
@@ -1613,9 +1460,9 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                     }
                 }
                 if constexpr (L < 2) {
-                    uint8_t* sl = (L == 0 ? slice0 : slice1) + (ls >> 6) * kDenseXBytes + (ls & 63) * 4;
+                    uint8_t* sl = (L == 0 ? slice0 : slice1) + (ls >> 6) * kRingXBytes + (ls & 63) * 4;
 #pragma unroll
-                    for (int i = 0; i < 2; ++i) *reinterpret_cast<float2*>(sl + rl[i] * kDenseXRow) = make_float2(y[i][0], y[i][1]);
+                    for (int i = 0; i < 2; ++i) *reinterpret_cast<float2*>(sl + rl[i] * kRingXRow) = make_float2(y[i][0], y[i][1]);
                 } else {
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -1624,18 +1471,18 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                     }
                 }
             }
-        unit_bar_sync(1, kDenseConsumers);
+        unit_bar_sync(1, kRingConsumers);
         if constexpr (L < 2) {
             // hazard 2: the slice is complete in this CTA -> tell every CTA of the cluster, then wait until all four are
             if (tid < 4) mbar_arrive_cluster(mapa_shared(smem_u32(&s_ready[L]), (uint32_t)tid));
             mbar_wait_cluster(&s_ready[L], 0);
         } else {
-            for (int cl = tid; cl < 64 * NC; cl += kDenseConsumers) {
+            for (int cl = tid; cl < 64 * NC; cl += kRingConsumers) {
                 float mx = s_red[0][cl];
                 for (int w = 1; w < 8; ++w) mx = fmaxf(mx, s_red[w][cl]);
                 a.out[(size_t)cloud * a.N[2] + (size_t)rank * W2 + lc + cl] = mx;
             }
-            unit_bar_sync(1, kDenseConsumers);                      // s_red is rewritten by the next pass
+            unit_bar_sync(1, kRingConsumers);                      // s_red is rewritten by the next pass
         }
     };
     pass(std::integral_constant<int, 0>{}, std::integral_constant<int, NC0>{}, 0);
@@ -1659,7 +1506,7 @@ static size_t group_all_fits(const psa_mlp* mlp) {
     if (cudaFuncSetAttribute(tc_group_all_kernel<NC0, NC1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return 0;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(4, 1, 1);
-    cfg.blockDim = dim3(kDenseThreads, 1, 1);
+    cfg.blockDim = dim3(kRingThreads, 1, 1);
     cfg.dynamicSmemBytes = smem;
     int clusters = 0;
     if (cudaOccupancyMaxActiveClusters(&clusters, tc_group_all_kernel<NC0, NC1>, &cfg) != cudaSuccess) { (void)cudaGetLastError(); return 0; }
@@ -1701,9 +1548,9 @@ static int sa_group_all_cluster(int b, int c, const float* xyz, const float* poi
         g.scale[l] = mlp->scale[l]; g.shift[l] = mlp->shift[l]; g.relu[l] = mlp->relu[l];
     }
     const int N0 = mlp->channels[1], N1 = mlp->channels[2];
-    if (N0 == 256 && N1 == 256) tc_group_all_kernel<1, 1><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
-    else if (N0 == 256) tc_group_all_kernel<1, 2><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
-    else tc_group_all_kernel<2, 1><<<4u * (unsigned)b, kDenseThreads, smem, st>>>(g);
+    if (N0 == 256 && N1 == 256) tc_group_all_kernel<1, 1><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
+    else if (N0 == 256) tc_group_all_kernel<1, 2><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
+    else tc_group_all_kernel<2, 1><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
     rc = check_launch("tc_group_all_kernel");
     if (rc != PSA_OK) return rc;
     const float* cur = points;
@@ -1713,8 +1560,9 @@ static int sa_group_all_cluster(int b, int c, const float* xyz, const float* poi
         a.rows = rows; a.K = K; a.Kp = K; a.N = N; a.pool_k = l == 2 ? 128 : 1; a.relu = mlp->relu[l];
         a.x = cur; a.scale = mlp->scale[l]; a.shift = mlp->shift[l]; a.out = l == 2 ? out : (l & 1) ? ws1 : ws0;
         a.xyz3 = l == 0 ? xyz : nullptr; a.w3 = l == 0 ? mlp->weight[0] : nullptr;
-        rc = launch_tc_dense_rerun(a, g.Nt[l], l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l], pre[l], ws_img[l], flag,
-                                   words + kTileCounterWords + 2 * l + 1, st);
+        const RingWeights w{K, K, N, g.Nt[l], l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l], ws_img[l],
+                            ws_img[l] + tc_dense_image_off3(K, N), pre[l]};
+        rc = ring_rerun(kDenseRing, a, tc_dense_units(rows, N, g.Nt[l]), w, flag, words + kTileCounterWords + 2 * l + 1, st);
         if (rc != PSA_OK) return rc;
         cur = a.out;
     }

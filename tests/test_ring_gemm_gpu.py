@@ -1,5 +1,5 @@
-"""The shared ring GEMM (csrc/ring_gemm.cuh) and its FMA fallback through all three of its ops -- conv3d, PointCNN's dense layer and
-spiderConv -- called through the C ABI so that the test owns every buffer, against float64 at the plan's edges:
+"""The shared ring GEMM (csrc/ring_gemm.cuh) and its FMA fallback through its ops -- conv3d, PointCNN's dense layer, spiderConv and
+the dense layer of psa_shared_mlp -- called through the C ABI so that the test owns every buffer, against float64 at the plan's edges:
 
 * every call is poisoned around: inputs are slices of NaN-filled buffers (NaN columns on both sides, NaN rows past the end), the
   output is a slice of a NaN-filled wider buffer, the workspace is NaN-filled and has NaN bytes past what it asked for.  Only the
@@ -66,17 +66,18 @@ def _owned(view, buf, what):
 
 
 class _Ws:
-    """a NaN-filled workspace of the bytes the current mode asks for, and 4 KB more that must stay NaN; word 0 is the range flag"""
+    """a NaN-filled workspace of the bytes the current mode asks for, and 4 KB more that must stay NaN; word `flag_word` is the range
+    flag"""
 
-    def __init__(self, need):
-        self.need = int(need)
+    def __init__(self, need, flag_word=0):
+        self.need, self.flag_word = int(need), flag_word
         self.buf = torch.full((self.need // 4 + 1024,), NAN, device="cuda")
 
     def args(self):
         return P(self.buf), C.c_size_t(self.need)
 
     def flag(self):
-        return int(self.buf[:1].view(torch.int32))
+        return int(self.buf[self.flag_word:self.flag_word + 1].view(torch.int32))
 
     def check_tail(self, what):
         assert bool((self.buf[self.need // 4:].view(torch.int32) == NAN_BITS).all()), f"{what}: wrote past its workspace"
@@ -213,6 +214,62 @@ class Spider:
         return R.spider_plan(self.b, self.npts, self.c, self.k, self.t, self.n)
 
 
+class Mlp:
+    """a one-layer psa_shared_mlp (psa_shared_mlp_grouped with group_rows): (x . W [+ group_add[r / group_rows]]) * scale + shift,
+    no ReLU, then the max over runs of pool_k rows; x starts `offset` floats past a 16-byte boundary"""
+    name = "mlp"
+
+    def __init__(self, rows, K, N, pool_k, offset=0, group_rows=0, seed=0):
+        self.rows, self.K, self.n, self.pool_k, self.offset, self.group_rows = rows, K, N, pool_k, offset, group_rows
+        g = torch.Generator().manual_seed(seed)
+        self.x = torch.randn((rows, K), generator=g).cuda()
+        self.W = (torch.randn((K, N), generator=g) / np.sqrt(K)).cuda()
+        self.scale = (torch.rand(N, generator=g) * 2 + 0.5).cuda()
+        self.shift = (torch.randn(N, generator=g) * 0.1).cuda()
+        self.gadd = torch.randn((rows // group_rows, N), generator=g).cuda() if group_rows else None
+
+    def want(self, x=None):
+        y = G.npy(self.x if x is None else x).astype(np.float64) @ G.npy(self.W).astype(np.float64)
+        if self.gadd is not None:
+            y += np.repeat(G.npy(self.gadd).astype(np.float64), self.group_rows, axis=0)
+        y = y * G.npy(self.scale) + G.npy(self.shift)
+        return torch.from_numpy(y.reshape(self.rows // self.pool_k, self.pool_k, self.n).max(1))
+
+    def mlp(self, W=None):
+        return ops.MlpParams([(_inside(self.W if W is None else W), _inside(self.scale), _inside(self.shift), False)])
+
+    def need(self):
+        return _lib.load().psa_shared_mlp_workspace_bytes(self.rows, self.mlp().ref)
+
+    def flag_word(self):
+        return (self.need() - 256) // 4                                       # the word region sits at the workspace's end
+
+    def call(self, ws, x=None, W=None):
+        x = self.x if x is None else x
+        xbuf = torch.full((x.numel() + 128,), NAN, device="cuda")
+        xi = xbuf[64 + self.offset:64 + self.offset + x.numel()].view(x.shape)
+        xi.copy_(x)
+        obuf = torch.full(((self.rows // self.pool_k) * self.n + 128,), NAN, device="cuda")
+        out = obuf[64:64 + (self.rows // self.pool_k) * self.n]
+        mlp, lib = self.mlp(W), _lib.load()
+        if self.gadd is None:
+            rc = lib.psa_shared_mlp(self.rows, self.pool_k, P(xi), mlp.ref, P(out), *ws.args(), _lib.stream())
+        else:
+            rc = lib.psa_shared_mlp_grouped(self.rows, self.group_rows, P(xi), mlp.ref, P(_inside(self.gadd)), P(out), *ws.args(),
+                                            _lib.stream())
+        assert rc == 0, lib.psa_last_error()
+        return _owned(out, obuf, self.label()).view(self.rows // self.pool_k, self.n)
+
+    def label(self):
+        ga = f" group_rows={self.group_rows}" if self.group_rows else ""
+        return f"shared_mlp {self.rows}x{self.K}x{self.n} pool {self.pool_k} offset {self.offset}{ga}"
+
+    def plan(self):
+        tiles = (self.rows + 127) // 128
+        Nt = 128 if R.wide_tiles(tiles, self.n) else 64
+        return dict(Nt=Nt, units=tiles * (self.n // Nt))
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # stale shared memory
 # ---------------------------------------------------------------------------------------------------------------------
@@ -228,6 +285,12 @@ def _stale_inf(op, nc):
         out = torch.empty((rows, N), device="cuda")
         ws = _Ws(lib.psa_dense_elu_affine_workspace_bytes(rows, K, N))
         rc = lib.psa_dense_elu_affine(rows, K, N, P(x), K, P(W), P(None), P(ones), P(ones), P(out), N, *ws.args(), _lib.stream())
+    elif op.name == "mlp":
+        x, W = torch.full((rows, K), INF, device="cuda"), torch.full((K, N), INF, device="cuda")
+        out = torch.empty((rows, N), device="cuda")
+        mlp = ops.MlpParams([(W, ones, ones, False)])
+        ws = _Ws(lib.psa_shared_mlp_workspace_bytes(rows, mlp.ref))
+        rc = lib.psa_shared_mlp(rows, 1, P(x), mlp.ref, P(out), *ws.args(), _lib.stream())
     else:                                                                     # spider: c = 64, k = 1, T = 4, g = 1
         c, t = 64, 4
         feat, W = torch.full((rows, c), INF, device="cuda"), torch.full((t * c, N), INF, device="cuda")
@@ -245,7 +308,7 @@ def _run(op, mode, **inputs):
     """op's call in `mode` on a fresh poisoned workspace, after _stale_inf for the ring ops that mask stale bytes; in mode 0 a
     clean call must leave the range flag down (the fp16x2 result stands).  -> (output, workspace)"""
     with _mode(mode):
-        ws = _Ws(op.need())
+        ws = _Ws(op.need(), op.flag_word() if op.name == "mlp" else 0)
         if mode != 1 and op.name != "conv3d":                                # conv3d zero-fills every staged byte itself
             _stale_inf(op, op.plan()["Nt"] // 64)
         y = op.call(ws, **inputs)
@@ -416,3 +479,29 @@ def test_dense_rows_are_independent(mode):
     a = _check(long, mode, want)
     b = _check(short, mode, want[:R_])
     assert _bits_equal(a[:R_], b)
+
+
+MLP = [
+    # rows % 128 in {1, 127}; K in {32, 99, 131} (99, 131: 4-byte staging); x off its 16-byte boundary; N in {64, 128, 256}
+    (129, 32, 64, 1, 0), (255, 99, 128, 1, 0), (4223, 131, 256, 1, 0), (4223, 32, 128, 1, 1),
+    # pool_k in {32, 64, 128, 256} (256: the ordered-int atomicMax between its fill and decode)
+    (4096, 99, 128, 32, 0), (8192, 32, 256, 64, 1), (16896, 131, 64, 128, 0), (33792, 64, 128, 256, 0),
+    # more units than SMs on 64- and 128-wide tiles
+    (17025, 32, 64, 1, 1), (17023, 131, 128, 1, 0),
+]
+MLP_GROUPED = (4223, 99, 128, 1, 0, 103)                                       # 41 groups of 103 rows, across the tiles
+
+
+def test_mlp_cases_cover_both_tile_widths_past_one_wave():
+    seen = {Mlp(*c[:4]).plan()["Nt"] for c in MLP if Mlp(*c[:4]).plan()["units"] > R.PLAN_SMS}
+    assert seen == {64, 128}
+
+
+@pytest.mark.parametrize("case", MLP + [MLP_GROUPED], ids=lambda c: "x".join(map(str, c)))
+@pytest.mark.parametrize("mode", (0, 2))
+def test_shared_mlp_dense_layer_matches_float64(case, mode):
+    """the dense op on the ring: its producer stages rows by 16- or 4-byte copies into stale shared memory, its consumers mask the
+    rows past the end and the columns past K, and its epilogue stores, pools or takes the ordered-int max"""
+    rows, K, N, pool_k, offset = case[:5]
+    op = Mlp(rows, K, N, pool_k, offset, group_rows=case[5] if len(case) > 5 else 0, seed=rows + K)
+    _check(op, mode)
