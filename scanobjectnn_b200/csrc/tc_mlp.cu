@@ -1188,11 +1188,12 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
 //   * CTA rank r computes columns [r N_l / 4, (r + 1) N_l / 4) of each layer for all 128 rows: layer 0 (K = c, the xyz rows of
 //     W1 as the epilogue side input) and layer 1 in one 64- or 128-column pass each, the last layer in 128-column passes, each
 //     followed by the max over the 128 rows -- a plain store of out[cloud, col];
-//   * the slices of layers 0 and 1 stay in the CTA's own shared memory as fp32 after the affine and ReLU, in the padded rows of
-//     tc_dense_kernel's x stages (kRingXRow), one 128 x 64 block per 64 columns.  K block kb of layer l + 1 lives in the CTA
-//     that owns those columns of layer l: the consumers read it with ld.shared::cluster and split it into A fragments while
-//     block kb - 1's wgmma group runs, as tc_dense_kernel does with its staged x.  Layer 0's input rows are read from global
-//     memory the same way (4 KB of 32-byte sectors per block and warp, from L2: the four CTAs of a cloud read the same rows);
+//   * the slices of layers 0 and 1 stay in the CTA's own shared memory, written once after the affine and ReLU as the Split<2>
+//     pieces the next layer's wgmma takes, in A-fragment order (ga_frag_off), 32 KB per 64 columns.  K block kb of layer l + 1
+//     lives in the CTA that owns those columns of layer l: every consumer thread loads its fragments of it with eight 16-byte
+//     loads (ld.shared::cluster when a peer owns it) while block kb - 1's wgmma group runs -- nothing to split, and the loads
+//     are not waited for until block kb's group is issued.  Layer 0's input rows are read from global memory and split by the
+//     consumers (4 KB of 32-byte sectors per block and warp, from L2: the four CTAs of a cloud read the same rows);
 //   * one producer warp streams the weight blocks of all three layers through one ring of 32 KB stages (cp.async.bulk from
 //     the layers' fp16x2 images, whatever their tile width), so the next layer's first blocks land during this layer's epilogue.
 // Arithmetic is tc_dense_kernel's: per 64-wide K block a fresh wgmma sum over the Split<2> pieces in the same order, added into
@@ -1228,9 +1229,14 @@ struct TcGroupAllArgs {
 constexpr int kGaStages = 3;
 constexpr uint32_t kGaStageBytes = 32768u;      // one K block of 128 weight columns, two fp16 pieces
 constexpr uint32_t kGaSmemBudget = 222u * 1024u;
+// A 64-column block of a slice holds the next layer's A fragments of all 128 rows, already split: for consumer warp w, piece
+// pc and K step ks (q = 4 pc + ks), lane l's four registers A[pc][ks][0..3] are 16 bytes at ga_frag_off(w, l, q) -- a warp's
+// 16-byte loads of one q are 512 contiguous bytes.  Two fp16 pieces of 128 x 64 values: 32 KB.
+constexpr uint32_t kGaSliceBytes = 32768u;
+__device__ __forceinline__ uint32_t ga_frag_off(int warp, int lane, int q) { return (uint32_t)(((warp * 8 + q) * 32 + lane) * 16); }
 // dynamic shared memory: 1 KB alignment, the ring, the slices of layers 0 and 1 (W0 + W1 columns), the affine of every layer
 __host__ __device__ inline uint32_t group_all_smem(int W0, int W1, int W2) {
-    return 1024u + kGaStages * kGaStageBytes + (uint32_t)(W0 + W1) / 64u * kRingXBytes + 12u * (uint32_t)(W0 + W1 + W2);
+    return 1024u + kGaStages * kGaStageBytes + (uint32_t)(W0 + W1) / 64u * kGaSliceBytes + 12u * (uint32_t)(W0 + W1 + W2);
 }
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
@@ -1244,10 +1250,14 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t addr, uint32_t rank) {
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(addr), "r"(rank));
     return r;
 }
-__device__ __forceinline__ float2 ld_cluster_f32x2(uint32_t addr) {
-    float2 v;
-    asm volatile("ld.shared::cluster.v2.f32 {%0, %1}, [%2];\n" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
-    return v;
+__device__ __forceinline__ void ld_cluster_v4(uint32_t addr, uint32_t (&v)[4]) {
+    asm volatile("ld.shared::cluster.v4.u32 {%0, %1, %2, %3}, [%4];\n" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void ld_shared_v4(uint32_t addr, uint32_t (&v)[4]) {
+    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];\n" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr) : "memory");
+}
+__device__ __forceinline__ void st_shared_v4(uint32_t addr, const uint32_t (&v)[4]) {
+    asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;\n" ::: "memory");
@@ -1271,6 +1281,40 @@ __device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity
     } while (!done);
 }
 
+#ifdef PSA_GA_STAMPS
+// K-block timeline (tools/group_all_timing.py builds a separate library with -DPSA_GA_STAMPS; libpsa.so has none of this):
+// thread 0 of each consumer warpgroup of CTA i < kGaStampCtas writes clock64() at ring use u < kGaStampUses: [0] weight block
+// ready, [1] wgmma group issued, [2] the next K block's A operand in registers, [3] group retired; [kGaStampUses - 1][0] is the
+// warpgroup's start.
+constexpr int kGaStampCtas = 256, kGaStampUses = 64;
+__device__ long long g_ga_stamps[kGaStampCtas][2][kGaStampUses][4];
+extern "C" PSA_API int psa_group_all_stamps(long long* dst) {
+    return cudaMemcpyFromSymbol(dst, g_ga_stamps, sizeof(g_ga_stamps)) == cudaSuccess ? 0 : 1;
+}
+#define GA_STAMP(u, k)                                                                                              \
+    do {                                                                                                            \
+        if ((threadIdx.x & 127) == 0 && blockIdx.x < kGaStampCtas && (u) < kGaStampUses)                            \
+            g_ga_stamps[blockIdx.x][threadIdx.x >> 7][(u)][(k)] = clock64();                                        \
+    } while (0)
+// the stamp after a volatile store of a value computed from register r, so the load that wrote r has landed (x * 0 cannot
+// be folded away in IEEE arithmetic)
+#define GA_STAMP_AFTER(u, k, r)                                                                                     \
+    do {                                                                                                            \
+        if ((threadIdx.x & 127) == 0 && blockIdx.x < kGaStampCtas && (u) < kGaStampUses) {                          \
+            volatile long long* p_ = &g_ga_stamps[blockIdx.x][threadIdx.x >> 7][(u)][(k)];                          \
+            *p_ = (long long)__float_as_uint(__fmul_rn(__uint_as_float(r), 0.f));                                   \
+            *p_ = clock64();                                                                                        \
+        }                                                                                                           \
+    } while (0)
+#else
+#define GA_STAMP(u, k) \
+    do {               \
+    } while (0)
+#define GA_STAMP_AFTER(u, k, r) \
+    do {                        \
+    } while (0)
+#endif
+
 // NC0, NC1: 64-column chunks of the layer-0 and layer-1 slices (one pass each); the last layer runs in 128-column passes
 template <int NC0, int NC1>
 __global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(kRingThreads, 1)
@@ -1287,8 +1331,8 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
     constexpr int W0 = 64 * NC0, W1 = 64 * NC1;                     // slice widths
     const int W2 = a.N[2] / 4;
     uint8_t* slice0 = base + S * kGaStageBytes;
-    uint8_t* slice1 = slice0 + NC0 * kRingXBytes;
-    float* aff0 = reinterpret_cast<float*>(slice1 + NC1 * kRingXBytes);   // per layer: scale x column factor, shift, 1 / column factor
+    uint8_t* slice1 = slice0 + NC0 * kGaSliceBytes;
+    float* aff0 = reinterpret_cast<float*>(slice1 + NC1 * kGaSliceBytes);   // per layer: scale x column factor, shift, 1 / column factor
     float* aff1 = aff0 + 3 * W0;
     float* aff2 = aff1 + 3 * W1;
     {
@@ -1352,12 +1396,14 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
     const int rl[2] = {warp * 16 + g, warp * 16 + g + 8};
     uint32_t ovf = 0u;
     uint32_t u = 0;                                                 // ring uses
+    GA_STAMP(kGaStampUses - 1, 0);
 
     // one pass of layer L: 64 NC columns starting at column `lc` of this CTA's slice
     auto pass = [&](auto Ltag, auto NCtag, int lc) {
         constexpr int L = decltype(Ltag)::value, NC = decltype(NCtag)::value;
         const int nkb = KC[L];
-        // K block kb of the layer's input -> A fragments (16 float2 loads in flight per thread)
+        // K block kb of the layer's input -> A fragments: layer 0 splits 16 float2 loads from global memory, layers 1 and 2 load
+        // the pieces the owner of the block stored (8 16-byte loads, nothing to wait for until the block's wgmma group)
         auto prep = [&](uint32_t (&A)[NP][4][4], int kb) {
             if constexpr (L == 0) {
                 const float* xb = a.points + (size_t)cloud * 128 * a.c + kb * 64;
@@ -1372,17 +1418,16 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                         }
             } else {
                 constexpr int Wp = L == 1 ? W0 : W1;                // the input's slice width: block kb is in CTA kb * 64 / Wp
-                const uint32_t src = mapa_shared(smem_u32(L == 1 ? slice0 : slice1) + (uint32_t)((kb * 64) % Wp / 64) * kRingXBytes,
-                                                 (uint32_t)(kb * 64 / Wp));
+                const uint32_t owner = (uint32_t)(kb * 64 / Wp);
+                const uint32_t src = smem_u32(L == 1 ? slice0 : slice1) + (uint32_t)((kb * 64) % Wp / 64) * kGaSliceBytes + ga_frag_off(warp, lane, 0);
+                if (owner == rank) {
 #pragma unroll
-                for (int s = 0; s < 4; ++s)
+                    for (int q = 0; q < NP * 4; ++q) ld_shared_v4(src + (uint32_t)q * 512u, A[q >> 2][q & 3]);
+                } else {
+                    const uint32_t rsrc = mapa_shared(src, owner);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h)
-#pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            const float2 x = ld_cluster_f32x2(src + (uint32_t)rl[i] * kRingXRow + (uint32_t)(16 * s + 8 * h + 2 * t) * 4u);
-                            put_a<NP, 4>(A, s, i + 2 * h, x.x, x.y, ovf);
-                        }
+                    for (int q = 0; q < NP * 4; ++q) ld_cluster_v4(rsrc + (uint32_t)q * 512u, A[q >> 2][q & 3]);
+                }
             }
         };
         float acc[NC][32];
@@ -1390,6 +1435,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
         auto step = [&](const uint32_t (&A)[NP][4][4], uint32_t (&An)[NP][4][4], int kb) {
             const int s = (int)(u % S);
             mbar_wait(&s_full[s], (u / S) & 1u);
+            GA_STAMP(u, 0);
             const uint32_t wb = smem_u32(base) + (uint32_t)s * kGaStageBytes;
             float d[NC][32];
             wg_fence();
@@ -1402,8 +1448,11 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                         wg_mma_rs<NP>(d[c], A[Split<NP>::a(tt)][ks][0], A[Split<NP>::a(tt)][ks][1], A[Split<NP>::a(tt)][ks][2], A[Split<NP>::a(tt)][ks][3],
                                       wg_desc(wb + (uint32_t)c * chunk + Split<NP>::w(tt) * piece + (uint32_t)ks * 32u), (tt | ks) ? 1u : 0u);
             wg_commit();
+            GA_STAMP(u, 1);
             if (kb + 1 < nkb) prep(An, kb + 1);
+            GA_STAMP_AFTER(u, 2, An[1][3][3]);
             wg_wait_all();
+            GA_STAMP(u, 3);
             __syncwarp();
             if (lane == 0) mbar_arrive1(&s_empty[s]);               // weights consumed: the stage may be refilled
             ++u;
@@ -1436,7 +1485,8 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
 #pragma unroll
                 for (int k = 0; k < 3; ++k) xs[i][k] = __ldg(a.xyz + ((size_t)cloud * 128 + rl[i]) * 3 + k);
 #pragma unroll
-        for (int c = 0; c < NC; ++c)
+        for (int c = 0; c < NC; ++c) {
+            uint32_t fr[NP][4];                                     // L < 2: the A fragments of K step j / 2 of the next layer
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int cl = c * 64 + 8 * j + 2 * t, ls = lc + cl;   // column in the pass, in the slice
@@ -1460,9 +1510,19 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                     }
                 }
                 if constexpr (L < 2) {
-                    uint8_t* sl = (L == 0 ? slice0 : slice1) + (ls >> 6) * kRingXBytes + (ls & 63) * 4;
+                    // the pieces the next layer's wgmma takes (the split its readers did before, once here, range tracked)
 #pragma unroll
-                    for (int i = 0; i < 2; ++i) *reinterpret_cast<float2*>(sl + rl[i] * kRingXRow) = make_float2(y[i][0], y[i][1]);
+                    for (int i = 0; i < 2; ++i) {
+                        uint32_t p[NP];
+                        split_pair<NP>(y[i][0], y[i][1], p, ovf);
+#pragma unroll
+                        for (int pc = 0; pc < NP; ++pc) fr[pc][i + 2 * (j & 1)] = p[pc];
+                    }
+                    if (j & 1) {
+                        const uint32_t sl = smem_u32(L == 0 ? slice0 : slice1) + (uint32_t)c * kGaSliceBytes;
+#pragma unroll
+                        for (int pc = 0; pc < NP; ++pc) st_shared_v4(sl + ga_frag_off(warp, lane, 4 * pc + (j >> 1)), fr[pc]);
+                    }
                 } else {
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
@@ -1471,6 +1531,7 @@ tc_group_all_kernel(const __grid_constant__ TcGroupAllArgs a) {
                     }
                 }
             }
+        }
         unit_bar_sync(1, kRingConsumers);
         if constexpr (L < 2) {
             // hazard 2: the slice is complete in this CTA -> tell every CTA of the cluster, then wait until all four are
