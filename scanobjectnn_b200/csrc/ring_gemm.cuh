@@ -301,6 +301,18 @@ struct RingWeights {
     uint8_t* img3;
     const uint8_t* prebuilt = nullptr;
 };
+// The image of a launch with np pieces: the prebuilt one, or built from W into the workspace (img2 / img3).  A rerun (`run_if`, its
+// flag, non-null) takes bf16x3 from the twin behind a prebuilt fp16x2 image, or builds it into img3 only if *run_if != 0.
+inline int ring_image(const RingWeights& w, int np, const unsigned int* run_if, cudaStream_t st, const uint8_t*& image) {
+    if (w.prebuilt != nullptr) {
+        image = run_if != nullptr ? w.prebuilt + tc::tc_image_alloc_bytes(w.Kp, w.N, 2) : w.prebuilt;
+        return PSA_OK;
+    }
+    uint8_t* own = np == 2 ? w.img2 : w.img3;
+    image = own;
+    return build_image(w.K, w.Kp, w.N, w.Nt | tc::image_flag(np), w.W, own, st, run_if);
+}
+
 // an output the kernel max-pools by ordered-int atomicMax: filled with the code of -inf before every launch, decoded after it
 struct RingPool {
     float* out = nullptr;
@@ -320,13 +332,9 @@ int ring_launch_pooled(const RingKernels& k, int np, const Args& a, long long un
 template <class Args>
 int ring_rerun(const RingKernels& k, Args a, long long units, const RingWeights& w, const unsigned int* flag, unsigned int* counter,
                cudaStream_t st, const RingPool& pool = {}) {
-    const uint8_t* img3 = w.img3;
-    if (w.prebuilt != nullptr) {
-        img3 = w.prebuilt + tc::tc_image_alloc_bytes(w.Kp, w.N, 2);
-    } else {
-        const int rc = build_image(w.K, w.Kp, w.N, w.Nt | tc::kImageBf16x3, w.W, w.img3, st, flag);
-        if (rc != PSA_OK) return rc;
-    }
+    const uint8_t* img3;
+    const int rc = ring_image(w, 3, flag, st, img3);
+    if (rc != PSA_OK) return rc;
     a.ring = RingArgs{};
     a.ring.image = img3; a.ring.run_if = flag; a.ring.counter = counter;
     return ring_launch_pooled(k, 3, a, units, w.Nt, pool, st);
@@ -339,19 +347,14 @@ template <class Args>
 int ring_run(const RingKernels& k, Args a, long long units, const RingWeights& w, unsigned int* flag, unsigned int* counters,
              cudaStream_t st, const RingPool& pool = {}) {
     const int np = tc_np();
-    const uint8_t* image = w.prebuilt;
-    if (image == nullptr) {
-        uint8_t* own = np == 2 ? w.img2 : w.img3;
-        const int rc = build_image(w.K, w.Kp, w.N, w.Nt | tc::image_flag(np), w.W, own, st);
-        if (rc != PSA_OK) return rc;
-        image = own;
-    }
+    const uint8_t* image;
+    int rc = ring_image(w, np, nullptr, st, image);
+    if (rc != PSA_OK) return rc;
     a.ring = RingArgs{};
     a.ring.image = image; a.ring.counter = counters;
     if (np == 3) return ring_launch_pooled(k, 3, a, units, w.Nt, pool, st);
     a.ring.ovf = flag; a.ring.wflag = image_trailer(image, w.Kp, w.N); a.ring.colscale = image_colscale(image, w.Kp, w.N);
-    const int rc = ring_launch_pooled(k, 2, a, units, w.Nt, pool, st);
-    if (rc != PSA_OK) return rc;
+    if ((rc = ring_launch_pooled(k, 2, a, units, w.Nt, pool, st)) != PSA_OK) return rc;
     return ring_rerun(k, a, units, w, flag, counters != nullptr ? counters + 1 : nullptr, st, pool);
 }
 

@@ -32,6 +32,7 @@
 #include <float.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <atomic>
 #include <type_traits>
 
@@ -912,7 +913,7 @@ static const RingKernels kDenseRing = {{{(const void*)tc_dense_kernel<2, 1>, (co
                                         {(const void*)tc_dense_kernel<3, 1>, (const void*)tc_dense_kernel<3, 2>}},
                                        "tc_dense_kernel", DenseOp<2, 1>::kBudget};
 
-bool tc_dense_eligible(long long rows, int K, int N, int pool_k) {
+static bool tc_dense_eligible(long long rows, int K, int N, int pool_k) {
     if (rows < 128 || K < 32 || N < 64 || (N % 64) != 0) return false;
     if (N > 64 && (N % 128) != 0) return false;
     if (!(pool_k == 1 || pool_k == 32 || pool_k == 64 || (pool_k >= 128 && pool_k % 128 == 0))) return false;
@@ -922,7 +923,9 @@ bool tc_dense_eligible(long long rows, int K, int N, int pool_k) {
 
 // Operand split of the inference launches: 2 = fp16x2 with the np = 3 rerun guard (default), 3 = bf16x3 only (psa_set_mlp_mode(2)).
 static std::atomic<int> g_tc_np{2};        // process-wide settings: atomics, so that a concurrent psa_set_mlp_mode is a race-free (if unordered) switch
+static std::atomic<int> g_mlp_mode{0};
 int tc_np() { return g_tc_np; }
+int mlp_mode() { return g_mlp_mode; }
 
 // Workspace reservation for one dense layer's images: an fp16x2 image (used when the caller brought no prebuilt one) followed by
 // the bf16x3 image of the guarded rerun / of mode 2 / of the training forward.
@@ -963,32 +966,67 @@ const float* image_colscale(const uint8_t* image, int Kp, int N) {
     return reinterpret_cast<const float*>(image + tc_image_colscale_off(Kp, N, 2));
 }
 
-// the zeroed 256-byte word region of psa_shared_mlp / psa_sa_group_all_infer: range flag of layer l at [l], the tile counters
-// of layer l and of its rerun at [kTileCounterWords + 2 l, + 1]
-constexpr int kTileCounterWords = PSA_MAX_MLP_LAYERS;
-
 static long long tc_dense_units(long long rows, int N, int Nt) { return (rows + 127) / 128 * (N / Nt); }
 
-// out = relu?((x . W [+ xyz3 . w3] [+ group_add[r / group_rows]]) * scale + shift) on the tensor cores, optional max over runs of
-// pool_k rows (not with group_add).
-//   prebuilt : image of W in the CURRENT split's format (psa_prepare_weight_image), or null
-//   ws_img   : tc_dense_image_bytes(K, N) of scratch (missing images are built here)
-//   flag     : one zeroed device word (np = 2: raised when a value left the fp16 range; the bf16x3 rerun is conditional on it)
-//   counters : two zeroed device words, the tile counters of the launch and of its rerun
-int launch_tc_dense(long long rows, int K, int N, int pool_k, int relu, const float* x, const float* W, const float* scale,
-                    const float* shift, float* out, const uint8_t* prebuilt, uint8_t* ws_img, unsigned int* flag, unsigned int* counters,
-                    cudaStream_t st, const float* xyz3 = nullptr, const float* w3 = nullptr, const float* group_add = nullptr,
-                    long long group_rows = 0) {
-    const int Kp = (K + 63) & ~63;
-    const int Nt = tc_dense_nt(rows, N) & ~kImageFlags;
+// The zeroed 256-byte word region of an inference entry point.  Its dense step l -- layer l of a chain, the U GEMM (0) and the
+// level (1) of tc_sa_run, EdgeConv's GEMM (0) -- has its range flag at [l] (np = 2: raised when a value left the fp16 range; the
+// bf16x3 rerun is conditional on it) and the tile counters of its launch and of its rerun at [PSA_MAX_MLP_LAYERS + 2 l, + 1].
+struct StepWords {
+    unsigned int* flag;
+    unsigned int* counters;
+};
+static StepWords step_words(unsigned int* region, int l) { return {region + l, region + PSA_MAX_MLP_LAYERS + 2 * l}; }
+constexpr int kClusterFlagStep = 3;        // the group-all cluster kernel's flag: a step its three-layer chain leaves free
+
+// One inference dense layer: out = relu?((x . W [+ xyz3 . w3] [+ group_add[r / group_rows]]) * scale + shift), optional max over
+// runs of pool_k rows (not with group_add).
+struct DenseStep {
+    long long rows;
+    int K, N, pool_k, relu;
+    const float* x;
+    const float* W;
+    const float* scale;                  // or null
+    const float* shift;                  // or null
+    float* out;
+    const float* xyz3 = nullptr;         // (rows, 3) side input with w3 (3, N): the tensor-core path only
+    const float* w3 = nullptr;
+    const float* group_add = nullptr;
+    long long group_rows = 0;
+    const uint8_t* prebuilt = nullptr;   // image of W in the current split's format (psa_prepare_weight_image), or null
+    uint8_t* img = nullptr;              // tc_dense_image_bytes(K, N) of scratch: the images not prebuilt are built here
+    StepWords words{};                   // in a zeroed word region
+    float* fc_partial = nullptr;         // non-null: fc_small's partial sums, for an FMA layer of rows <= 32
+};
+
+// The one choice between the tensor cores and the FMA kernels of an inference dense layer: mode 1 never takes the tensor cores.
+static bool dense_on_tc(long long rows, int K, int N, int pool_k) { return g_mlp_mode != 1 && tc_dense_eligible(rows, K, N, pool_k); }
+
+// a tensor-core step's kernel arguments (`ring` is filled by ring_run / ring_rerun) and weights
+static TcDenseArgs tc_dense_args(const DenseStep& s) {
     TcDenseArgs a;
-    a.rows = rows; a.K = K; a.Kp = Kp; a.N = N; a.pool_k = pool_k; a.relu = relu;
-    a.x = x; a.scale = scale; a.shift = shift; a.out = out; a.xyz3 = xyz3; a.w3 = w3;
-    a.group_add = group_add; a.group_rows = group_rows;
-    RingPool pool;
-    if (pool_k > 128) { pool.out = out; pool.count = rows / pool_k * N; }
-    return ring_run(kDenseRing, a, tc_dense_units(rows, N, Nt), RingWeights{K, Kp, N, Nt, W, ws_img, ws_img + tc_dense_image_off3(K, N), prebuilt},
-                    flag, counters, st, pool);
+    a.rows = s.rows; a.K = s.K; a.Kp = (s.K + 63) & ~63; a.N = s.N; a.pool_k = s.pool_k; a.relu = s.relu;
+    a.x = s.x; a.scale = s.scale; a.shift = s.shift; a.out = s.out; a.xyz3 = s.xyz3; a.w3 = s.w3;
+    a.group_add = s.group_add; a.group_rows = s.group_rows;
+    return a;
+}
+static RingWeights tc_dense_weights(const DenseStep& s) {
+    return RingWeights{s.K, (s.K + 63) & ~63, s.N, tc_dense_nt(s.rows, s.N) & ~kImageFlags, s.W, s.img, s.img + tc_dense_image_off3(s.K, s.N), s.prebuilt};
+}
+
+static int run_dense(const DenseStep& s, cudaStream_t st) {
+    if (dense_on_tc(s.rows, s.K, s.N, s.pool_k)) {
+        RingPool pool;
+        if (s.pool_k > 128) { pool.out = s.out; pool.count = s.rows / s.pool_k * s.N; }
+        const RingWeights w = tc_dense_weights(s);
+        return ring_run(kDenseRing, tc_dense_args(s), tc_dense_units(s.rows, s.N, w.Nt), w, s.words.flag, s.words.counters, st, pool);
+    }
+    PSA_SUPPORTED(s.xyz3 == nullptr, "sa_group_all: layer 0 must run on the tensor-core path");
+    DenseArgs d;
+    d.rows = s.rows; d.K = s.K; d.N = s.N; d.pool_k = s.pool_k; d.relu = s.relu;
+    d.x = s.x; d.W = s.W; d.scale = s.scale; d.shift = s.shift; d.out = s.out;
+    d.group_add = s.group_add; d.group_rows = s.group_rows;
+    if (s.fc_partial != nullptr && s.rows <= 32 && s.pool_k == 1 && s.group_add == nullptr) return launch_fc_small(d, s.fc_partial, st);
+    return launch_dense(d, st);
 }
 
 // Training-mode forward of one layer on tc_dense_kernel: y = relu(bn_prev(x)) . W + bias (pre-BN output), per-row-tile column
@@ -1111,32 +1149,26 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
                      const int* idx, const psa_mlp* mlp, const float* w1c, float* out, void* workspace, cudaStream_t st) {
     int rc = PSA_OK;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    unsigned int* words = reinterpret_cast<unsigned int*>(ws);     // [0] tile counter, [1] tile counter of the rerun, [2] range flag of
-    PSA_CUDA(cudaMemsetAsync(ws, 0, 256, st));                     // the level, [3] range flag of the U GEMM, [4, 5] its tile counters
+    unsigned int* region = reinterpret_cast<unsigned int*>(ws);
+    const StepWords words = step_words(region, 1);
+    PSA_CUDA(cudaMemsetAsync(ws, 0, 256, st));
     ws += 256;
-    uint8_t* img2[kMaxTcLayers];
-    uint8_t* img3[kMaxTcLayers];
+    RingWeights w[kMaxTcLayers];
     for (int l = 0; l < a.nl; ++l) {
-        img2[l] = ws; ws += tc_image_alloc_bytes(a.Kd[l], a.Ntot[l], 2);
-        img3[l] = ws; ws += tc_image_alloc_bytes(a.Kd[l], a.Ntot[l], 3);
+        const int K = a.Kd[l], N = a.Ntot[l];
+        w[l] = RingWeights{K, K, N, kSaNt, mlp->weight[1 + l], ws, ws + tc_image_alloc_bytes(K, N, 2), prebuilt_image(mlp, 1 + l, 0, tc_sa_image_nt())};
+        ws += tc_image_alloc_bytes(K, N, 2) + tc_image_alloc_bytes(K, N, 3);
     }
     const float* uf = nullptr;
     if (c > 0) {
         // U = points . W1[3:,:]  once per source point (rows b*n), raw (affine + ReLU are applied after the xyz part)
-        float* ufw = reinterpret_cast<float*>(ws);
-        uint8_t* uimg = ws + (((size_t)b * n * a.C1 * sizeof(float) + 255) & ~(size_t)255);
-        const float* w1f = mlp->weight[0] + (size_t)3 * a.C1;
-        if (tc_dense_eligible((long long)b * n, c, a.C1, 1)) {
-            rc = launch_tc_dense((long long)b * n, c, a.C1, 1, 0, points, w1f, nullptr, nullptr, ufw, prebuilt_image(mlp, 0, 3, tc_dense_nt((long long)b * n, a.C1)),
-                                 uimg, words + 3, words + 4, st);
-        } else {
-            DenseArgs d;
-            d.rows = (long long)b * n; d.K = c; d.N = a.C1; d.pool_k = 1; d.relu = 0;
-            d.x = points; d.W = w1f; d.scale = nullptr; d.shift = nullptr; d.out = ufw;
-            rc = launch_dense(d, st);
-        }
-        if (rc != PSA_OK) return rc;
-        uf = ufw;
+        const long long rows = (long long)b * n;
+        DenseStep u{rows, c, a.C1, 1, 0, points, mlp->weight[0] + (size_t)3 * a.C1, nullptr, nullptr, reinterpret_cast<float*>(ws)};
+        u.prebuilt = prebuilt_image(mlp, 0, 3, tc_dense_nt(rows, a.C1));
+        u.img = ws + (((size_t)rows * a.C1 * sizeof(float) + 255) & ~(size_t)255);
+        u.words = step_words(region, 0);
+        if ((rc = run_dense(u, st)) != PSA_OK) return rc;
+        uf = u.out;
     }
     auto fill = [&](TcArgs& t) {
         t.groups = (long long)b * m; t.K = nsample; t.n = n; t.m = m;
@@ -1149,35 +1181,22 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     };
     fill(a);
     for (int l = 0; l < a.nl; ++l) {
-        const int nt_img = tc_sa_image_nt();
-        const uint8_t* pre = prebuilt_image(mlp, 1 + l, 0, nt_img);
-        uint8_t* own = a.np == 2 ? img2[l] : img3[l];
-        if (pre == nullptr) { rc = build_image(a.Kd[l], a.Kd[l], a.Ntot[l], nt_img, mlp->weight[1 + l], own, st); if (rc != PSA_OK) return rc; }
-        a.image[l] = pre ? pre : own;
-        if (a.np == 2) { a.wflag[l] = image_trailer(a.image[l], a.Kd[l], a.Ntot[l]); a.colscale[l] = image_colscale(a.image[l], a.Kd[l], a.Ntot[l]); }
+        if ((rc = ring_image(w[l], a.np, nullptr, st, a.image[l])) != PSA_OK) return rc;
+        if (a.np == 2) { a.wflag[l] = image_trailer(a.image[l], w[l].Kp, w[l].N); a.colscale[l] = image_colscale(a.image[l], w[l].Kp, w[l].N); }
     }
-    a.tile_counter = words;
+    a.tile_counter = words.counters;
     if (a.np == 3) return launch_tc_sa_np<3>(a, st);
-    a.ovf = words + 2;
+    a.ovf = words.flag;
     rc = launch_tc_sa_np<2>(a, st);
     if (rc != PSA_OK) return rc;
     // guarded rerun with bf16x3 operands: image builds and the level itself are no-ops unless the fp16x2 pass raised the flag
     TcArgs a3;
     PSA_REQUIRE(tc_sa_eligible(mlp, c, nsample, &a3, 3), "sa_module: internal error (bf16x3 eligibility)");
     fill(a3);
-    for (int l = 0; l < a3.nl; ++l) {
-        // a prebuilt fp16x2 image carries its bf16x3 twin behind it
-        const uint8_t* pre = prebuilt_image(mlp, 1 + l, 0, kSaNt | kImageF16x2);
-        if (pre != nullptr) {
-            a3.image[l] = pre + tc_image_alloc_bytes(a3.Kd[l], a3.Ntot[l], 2);
-        } else {
-            rc = build_image(a3.Kd[l], a3.Kd[l], a3.Ntot[l], kSaNt | kImageBf16x3, mlp->weight[1 + l], img3[l], st, words + 2);
-            if (rc != PSA_OK) return rc;
-            a3.image[l] = img3[l];
-        }
-    }
-    a3.tile_counter = words + 1;
-    a3.run_if = words + 2;
+    for (int l = 0; l < a3.nl; ++l)
+        if ((rc = ring_image(w[l], 3, words.flag, st, a3.image[l])) != PSA_OK) return rc;
+    a3.tile_counter = words.counters + 1;
+    a3.run_if = words.flag;
     return launch_tc_sa_np<3>(a3, st);
 }
 
@@ -1583,49 +1602,92 @@ static size_t group_all_eligible(int n, int c, const float* points, const psa_ml
     return 0;
 }
 
-// The group-all level of psa_sa_group_all_infer on tc_group_all_kernel (group_all_eligible said yes, `smem`), then the chain's
-// three bf16x3 layer launches, conditional on the kernel's range flag: the output is then what psa_set_mlp_mode(2) gives.
-// Workspace as the chain's: intermediate rows ws0 / ws1 (used by the reruns only), per-layer images from `img`, the zeroed word
-// region `words` (the flag is its free word [kTileCounterWords - 1], the reruns' tile counters those of the chain).
-static int sa_group_all_cluster(int b, int c, const float* xyz, const float* points, const psa_mlp* mlp, float* out, float* ws0, float* ws1,
-                                uint8_t* img, unsigned int* words, size_t smem, cudaStream_t st) {
-    const long long rows = (long long)b * 128;
-    unsigned int* flag = words + kTileCounterWords - 1;
+// A chain of inference dense layers (psa_shared_mlp, psa_shared_mlp_grouped, psa_sa_group_all_infer) and its workspace, the one
+// layout both the size queries and the launchers read: activations ping-pong between two halves, one image slot per layer,
+// fc_small's partial sums when rows <= 32, the zeroed word region last.  Group-all's first layer (row0 = 3) is the K0 = c
+// feature rows of its W, the xyz rows the side input.
+struct ChainPlan {
+    long long rows;
+    int L, row0;
+    int K[PSA_MAX_MLP_LAYERS], N[PSA_MAX_MLP_LAYERS];
+    size_t half, img[PSA_MAX_MLP_LAYERS], fc, words, bytes;   // byte offsets into the workspace; its size
+};
+static ChainPlan chain_plan(long long rows, const psa_mlp* mlp, int K0, int row0) {
+    ChainPlan p{};
+    p.rows = rows; p.L = mlp->n_layers; p.row0 = row0;
+    int cmax = 0;
+    for (int l = 0; l < p.L; ++l) {
+        p.K[l] = l == 0 ? K0 : mlp->channels[l];
+        p.N[l] = mlp->channels[l + 1];
+        if (l > 0) cmax = std::max(cmax, p.K[l]);
+    }
+    p.half = p.L > 1 ? al256((size_t)rows * cmax * sizeof(float)) : 0;
+    size_t off = 2 * p.half, fc = 0;
+    for (int l = 0; l < p.L; ++l) {
+        p.img[l] = off;
+        off += tc_dense_image_bytes(p.K[l], std::max(p.N[l], 64));
+        if (rows <= 32) fc = std::max(fc, fc_small_workspace_bytes(p.K[l], p.N[l]));
+    }
+    p.fc = off;
+    p.words = off + al256(fc);
+    p.bytes = p.words + 256;
+    return p;
+}
+
+// layer l of chain p in the workspace ws: x is the first layer's input, xyz group-all's side input, out the last layer's output,
+// pool_k the last layer's
+static DenseStep chain_step(const ChainPlan& p, int l, int pool_k, const psa_mlp* mlp, const float* x, const float* xyz, float* out, uint8_t* ws) {
+    float* half[2] = {reinterpret_cast<float*>(ws), reinterpret_cast<float*>(ws + p.half)};
+    const int row0 = l == 0 ? p.row0 : 0;
+    DenseStep s{p.rows, p.K[l], p.N[l], l == p.L - 1 ? pool_k : 1, mlp->relu[l], l == 0 ? x : half[(l - 1) & 1],
+                mlp->weight[l] + (size_t)row0 * p.N[l], mlp->scale[l], mlp->shift[l], l == p.L - 1 ? out : half[l & 1]};
+    if (row0 != 0) { s.xyz3 = xyz; s.w3 = mlp->weight[0]; }
+    s.prebuilt = prebuilt_image(mlp, l, row0, tc_dense_nt(p.rows, s.N));
+    s.img = ws + p.img[l];
+    s.words = step_words(reinterpret_cast<unsigned int*>(ws + p.words), l);
+    if (p.rows <= 32) s.fc_partial = reinterpret_cast<float*>(ws + p.fc);
+    return s;
+}
+
+static int run_chain(const ChainPlan& p, int pool_k, const psa_mlp* mlp, const float* x, const float* xyz, const float* group_add,
+                     long long group_rows, float* out, uint8_t* ws, cudaStream_t st) {
+    for (int l = 0; l < p.L; ++l) {
+        DenseStep s = chain_step(p, l, pool_k, mlp, x, xyz, out, ws);
+        s.group_add = l == 0 ? group_add : nullptr;
+        s.group_rows = group_rows;
+        const int rc = run_dense(s, st);
+        if (rc != PSA_OK) return rc;
+    }
+    return PSA_OK;
+}
+
+// The group-all level of psa_sa_group_all_infer on tc_group_all_kernel (group_all_eligible said yes, `smem`), then the bf16x3
+// reruns of chain p's three layers, conditional on the kernel's range flag: the output is then what psa_set_mlp_mode(2) gives.
+// The layers, their images and the reruns' workspace and tile counters are those of the chain.
+static int sa_group_all_cluster(const ChainPlan& p, const float* xyz, const float* points, const psa_mlp* mlp, float* out, uint8_t* ws,
+                                size_t smem, cudaStream_t st) {
+    unsigned int* flag = step_words(reinterpret_cast<unsigned int*>(ws + p.words), kClusterFlagStep).flag;
     TcGroupAllArgs g{};
-    g.c = c; g.points = points; g.xyz = xyz; g.w3 = mlp->weight[0]; g.out = out; g.ovf = flag;
-    const uint8_t* pre[3];
-    uint8_t* ws_img[3];
+    g.c = p.K[0]; g.points = points; g.xyz = xyz; g.w3 = mlp->weight[0]; g.out = out; g.ovf = flag;
+    DenseStep s[3];
     int rc;
     for (int l = 0; l < 3; ++l) {
-        const int K = l == 0 ? c : mlp->channels[l], N = mlp->channels[l + 1], Nt = tc_dense_nt(rows, N);
-        const float* W = l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l];
-        pre[l] = prebuilt_image(mlp, l, l == 0 ? 3 : 0, Nt);
-        ws_img[l] = img;
-        img += tc_dense_image_bytes(K, N);
-        if (pre[l] == nullptr) { rc = build_image(K, K, N, Nt, W, ws_img[l], st); if (rc != PSA_OK) return rc; }
-        const uint8_t* image = pre[l] ? pre[l] : ws_img[l];
-        g.N[l] = N; g.Nt[l] = Nt & ~kImageFlags; g.image[l] = image;
-        g.colscale[l] = image_colscale(image, K, N); g.wflag[l] = image_trailer(image, K, N);
-        g.scale[l] = mlp->scale[l]; g.shift[l] = mlp->shift[l]; g.relu[l] = mlp->relu[l];
+        s[l] = chain_step(p, l, 128, mlp, points, xyz, out, ws);
+        const RingWeights w = tc_dense_weights(s[l]);
+        if ((rc = ring_image(w, 2, nullptr, st, g.image[l])) != PSA_OK) return rc;
+        g.N[l] = w.N; g.Nt[l] = w.Nt;
+        g.colscale[l] = image_colscale(g.image[l], w.Kp, w.N); g.wflag[l] = image_trailer(g.image[l], w.Kp, w.N);
+        g.scale[l] = s[l].scale; g.shift[l] = s[l].shift; g.relu[l] = s[l].relu;
     }
-    const int N0 = mlp->channels[1], N1 = mlp->channels[2];
-    if (N0 == 256 && N1 == 256) tc_group_all_kernel<1, 1><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
-    else if (N0 == 256) tc_group_all_kernel<1, 2><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
-    else tc_group_all_kernel<2, 1><<<4u * (unsigned)b, kRingThreads, smem, st>>>(g);
-    rc = check_launch("tc_group_all_kernel");
-    if (rc != PSA_OK) return rc;
-    const float* cur = points;
+    const unsigned grid = 4u * (unsigned)(p.rows / 128);
+    if (g.N[0] == 256 && g.N[1] == 256) tc_group_all_kernel<1, 1><<<grid, kRingThreads, smem, st>>>(g);
+    else if (g.N[0] == 256) tc_group_all_kernel<1, 2><<<grid, kRingThreads, smem, st>>>(g);
+    else tc_group_all_kernel<2, 1><<<grid, kRingThreads, smem, st>>>(g);
+    if ((rc = check_launch("tc_group_all_kernel")) != PSA_OK) return rc;
     for (int l = 0; l < 3; ++l) {
-        const int K = l == 0 ? c : mlp->channels[l], N = mlp->channels[l + 1];
-        TcDenseArgs a;
-        a.rows = rows; a.K = K; a.Kp = K; a.N = N; a.pool_k = l == 2 ? 128 : 1; a.relu = mlp->relu[l];
-        a.x = cur; a.scale = mlp->scale[l]; a.shift = mlp->shift[l]; a.out = l == 2 ? out : (l & 1) ? ws1 : ws0;
-        a.xyz3 = l == 0 ? xyz : nullptr; a.w3 = l == 0 ? mlp->weight[0] : nullptr;
-        const RingWeights w{K, K, N, g.Nt[l], l == 0 ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l], ws_img[l],
-                            ws_img[l] + tc_dense_image_off3(K, N), pre[l]};
-        rc = ring_rerun(kDenseRing, a, tc_dense_units(rows, N, g.Nt[l]), w, flag, words + kTileCounterWords + 2 * l + 1, st);
+        const RingWeights w = tc_dense_weights(s[l]);
+        rc = ring_rerun(kDenseRing, tc_dense_args(s[l]), tc_dense_units(p.rows, w.N, w.Nt), w, flag, s[l].words.counters + 1, st);
         if (rc != PSA_OK) return rc;
-        cur = a.out;
     }
     return PSA_OK;
 }
@@ -1634,8 +1696,6 @@ static int sa_group_all_cluster(int b, int c, const float* xyz, const float* poi
 
 using namespace psa;
 
-static std::atomic<int> g_mlp_mode{0};
-int psa::mlp_mode() { return g_mlp_mode; }
 extern "C" PSA_API int psa_set_mlp_mode(int mode) {
     PSA_REQUIRE(mode == 0 || mode == 1 || mode == 2,
                 "set_mlp_mode: mode must be 0 (tensor cores, fp16x2 operands with the range guard), 1 (fp32 FMA kernels only) or 2 (tensor cores, bf16x3)");
@@ -1682,66 +1742,21 @@ extern "C" int psa_sa_module_infer(int b, int n, int m, int c, float radius, int
 }
 
 extern "C" size_t psa_shared_mlp_workspace_bytes(long long rows, const psa_mlp* mlp) {
-    if (mlp == nullptr || mlp->n_layers < 1) return 0;
-    size_t bytes = 0;
-    int cmax = 0;
-    for (int l = 1; l < mlp->n_layers; ++l) cmax = cmax > mlp->channels[l] ? cmax : mlp->channels[l];
-    if (mlp->n_layers > 1) bytes += 2 * (((size_t)rows * cmax * sizeof(float) + 255) & ~(size_t)255);
-    for (int l = 0; l < mlp->n_layers; ++l) bytes += tc_dense_image_bytes(mlp->channels[l], mlp->channels[l + 1] < 64 ? 64 : mlp->channels[l + 1]);
-    if (rows <= 32) {
-        size_t fc = 0;
-        for (int l = 0; l < mlp->n_layers; ++l) { size_t f = fc_small_workspace_bytes(mlp->channels[l], mlp->channels[l + 1]); fc = f > fc ? f : fc; }
-        bytes += (fc + 255) & ~(size_t)255;
-    }
-    return bytes + 256;       // range flags of the tensor-core layers (one word per layer) and their tile counters, last
+    if (mlp == nullptr || mlp->n_layers < 1 || mlp->n_layers > PSA_MAX_MLP_LAYERS) return 0;
+    return chain_plan(rows, mlp, mlp->channels[0], 0).bytes;
 }
 
 // The layer chain of psa_shared_mlp and psa_shared_mlp_grouped (arguments validated by the caller; group_add: layer 0's per-group input,
 // or null).
 static int shared_mlp_chain(long long rows, int pool_k, const float* x, const psa_mlp* mlp, const float* group_add, long long group_rows,
                             float* out, void* workspace, size_t workspace_bytes, psa_stream_t stream) {
-    int rc;
-    const int L = mlp->n_layers;
-    const size_t need = psa_shared_mlp_workspace_bytes(rows, mlp);
-    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= need, "shared_mlp: workspace of %zu bytes required (got %zu)", need, workspace_bytes);
+    const ChainPlan p = chain_plan(rows, mlp, mlp->channels[0], 0);
+    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= p.bytes, "shared_mlp: workspace of %zu bytes required (got %zu)", p.bytes, workspace_bytes);
     PSA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "shared_mlp: workspace must be 256-byte aligned");
-    int cmax = 0;
-    for (int l = 1; l < L; ++l) cmax = cmax > mlp->channels[l] ? cmax : mlp->channels[l];
-    const size_t half = L > 1 ? (((size_t)rows * cmax * sizeof(float) + 255) & ~(size_t)255) : 0;
-    uint8_t* wsb = reinterpret_cast<uint8_t*>(workspace);
-    float* ws0 = reinterpret_cast<float*>(wsb);
-    float* ws1 = reinterpret_cast<float*>(wsb + half);
-    uint8_t* img = wsb + 2 * half;
-    float* fc_partial = nullptr;
-    if (rows <= 32) {   // the K-split partial sums of the small-M kernel sit at the end of the workspace
-        size_t imgs = 0;
-        for (int l = 0; l < L; ++l) imgs += tc_dense_image_bytes(mlp->channels[l], mlp->channels[l + 1] < 64 ? 64 : mlp->channels[l + 1]);
-        fc_partial = reinterpret_cast<float*>(img + imgs);
-    }
-    const float* cur = x;
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     cudaStream_t st = as_stream(stream);
-    unsigned int* flags = reinterpret_cast<unsigned int*>(wsb + need - 256);
-    PSA_CUDA(cudaMemsetAsync(flags, 0, 256, st));
-    for (int l = 0; l < L; ++l) {
-        const int K = mlp->channels[l], N = mlp->channels[l + 1];
-        const int pk = (l == L - 1) ? pool_k : 1;
-        float* dst = (l == L - 1) ? out : ((l & 1) ? ws1 : ws0);
-        const float* gadd = l == 0 ? group_add : nullptr;
-        if (g_mlp_mode != 1 && tc_dense_eligible(rows, K, N, pk)) {
-            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, mlp->weight[l], mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, 0, tc_dense_nt(rows, N)),
-                                 img, flags + l, flags + kTileCounterWords + 2 * l, st, nullptr, nullptr, gadd, group_rows);
-        } else {
-            DenseArgs d;
-            d.rows = rows; d.K = K; d.N = N; d.pool_k = pk; d.relu = mlp->relu[l];
-            d.x = cur; d.W = mlp->weight[l]; d.scale = mlp->scale[l]; d.shift = mlp->shift[l]; d.out = dst;
-            d.group_add = gadd; d.group_rows = group_rows;
-            rc = (rows <= 32 && pk == 1 && gadd == nullptr) ? launch_fc_small(d, fc_partial, st) : launch_dense(d, st);
-        }
-        if (rc != PSA_OK) return rc;
-        img += tc_dense_image_bytes(K, N < 64 ? 64 : N);
-        cur = dst;
-    }
-    return PSA_OK;
+    PSA_CUDA(cudaMemsetAsync(ws + p.words, 0, 256, st));
+    return run_chain(p, pool_k, mlp, x, nullptr, group_add, group_rows, out, ws, st);
 }
 
 extern "C" int psa_shared_mlp(long long rows, int pool_k, const float* x, const psa_mlp* mlp, float* out,
@@ -1770,10 +1785,8 @@ extern "C" int psa_shared_mlp_grouped(long long rows, long long group_rows, cons
 // n points of each cloud -- without building the (b,n,3+c) concatenation: the feature part [3:,:] of the first layer runs
 // as an aligned K = c GEMM on the tensor cores, the three xyz rows of W1 are folded into its epilogue.
 extern "C" size_t psa_sa_group_all_workspace_bytes(int b, int n, int c, const psa_mlp* mlp) {
-    if (mlp == nullptr || mlp->n_layers < 1) return 0;
-    psa_mlp m2 = *mlp;
-    m2.channels[0] = c;
-    return psa_shared_mlp_workspace_bytes((long long)b * n, &m2);
+    if (mlp == nullptr || mlp->n_layers < 1 || mlp->n_layers > PSA_MAX_MLP_LAYERS) return 0;
+    return chain_plan((long long)b * n, mlp, c, 3).bytes;
 }
 
 extern "C" int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, const float* points, const psa_mlp* mlp,
@@ -1784,51 +1797,20 @@ extern "C" int psa_sa_group_all_infer(int b, int n, int c, const float* xyz, con
     PSA_REQUIRE(mlp->channels[0] == 3 + c, "sa_group_all: mlp input width %d != 3 + c (%d)", mlp->channels[0], 3 + c);
     if (b == 0) return PSA_OK;
     PSA_REQUIRE(xyz && points && out, "sa_group_all: null buffer");
-    const long long rows = (long long)b * n;
-    const int L = mlp->n_layers;
-    const int N0 = mlp->channels[1];
-    const int pk0 = (L == 1) ? n : 1;
-    PSA_SUPPORTED(g_mlp_mode != 1 && tc_dense_eligible(rows, c, N0, pk0),
-                  "sa_group_all: first layer (%d -> %d over %lld rows) is not eligible for the tensor-core path; concatenate and use shared_mlp", c, N0, rows);
-    const size_t need = psa_sa_group_all_workspace_bytes(b, n, c, mlp);
-    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= need, "sa_group_all: workspace of %zu bytes required (got %zu)", need, workspace_bytes);
+    const ChainPlan p = chain_plan((long long)b * n, mlp, c, 3);
+    PSA_SUPPORTED(dense_on_tc(p.rows, c, p.N[0], p.L == 1 ? n : 1),
+                  "sa_group_all: first layer (%d -> %d over %lld rows) is not eligible for the tensor-core path; concatenate and use shared_mlp", c, p.N[0], p.rows);
+    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= p.bytes, "sa_group_all: workspace of %zu bytes required (got %zu)", p.bytes, workspace_bytes);
     PSA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "sa_group_all: workspace must be 256-byte aligned");
-    int cmax = 0;
-    for (int l = 1; l < L; ++l) cmax = cmax > mlp->channels[l] ? cmax : mlp->channels[l];
-    const size_t half = L > 1 ? (((size_t)rows * cmax * sizeof(float) + 255) & ~(size_t)255) : 0;
-    uint8_t* wsb = reinterpret_cast<uint8_t*>(workspace);
-    float* ws0 = reinterpret_cast<float*>(wsb);
-    float* ws1 = reinterpret_cast<float*>(wsb + half);
-    uint8_t* img = wsb + 2 * half;
+    uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     cudaStream_t st = as_stream(stream);
-    unsigned int* flags = reinterpret_cast<unsigned int*>(wsb + need - 256);
-    PSA_CUDA(cudaMemsetAsync(flags, 0, 256, st));
+    PSA_CUDA(cudaMemsetAsync(ws + p.words, 0, 256, st));
     // one cluster of four CTAs per cloud when the level allows it; otherwise one launch per layer
     if (g_mlp_mode == 0) {
         const size_t smem = group_all_eligible(n, c, points, mlp);
-        if (smem != 0) return sa_group_all_cluster(b, c, xyz, points, mlp, out, ws0, ws1, img, flags, smem, st);
+        if (smem != 0) return sa_group_all_cluster(p, xyz, points, mlp, out, ws, smem, st);
     }
-    const float* cur = points;
-    for (int l = 0; l < L; ++l) {
-        const int K = (l == 0) ? c : mlp->channels[l], N = mlp->channels[l + 1];
-        const int pk = (l == L - 1) ? n : 1;
-        float* dst = (l == L - 1) ? out : ((l & 1) ? ws1 : ws0);
-        const float* W = (l == 0) ? mlp->weight[0] + (size_t)3 * N : mlp->weight[l];
-        if (tc_dense_eligible(rows, K, N, pk)) {
-            rc = launch_tc_dense(rows, K, N, pk, mlp->relu[l], cur, W, mlp->scale[l], mlp->shift[l], dst, prebuilt_image(mlp, l, l == 0 ? 3 : 0, tc_dense_nt(rows, N)),
-                                 img, flags + l, flags + kTileCounterWords + 2 * l, st, l == 0 ? xyz : nullptr, l == 0 ? mlp->weight[0] : nullptr);
-        } else {
-            PSA_SUPPORTED(l > 0, "sa_group_all: layer 0 must run on the tensor-core path");
-            DenseArgs d;
-            d.rows = rows; d.K = K; d.N = N; d.pool_k = pk; d.relu = mlp->relu[l];
-            d.x = cur; d.W = W; d.scale = mlp->scale[l]; d.shift = mlp->shift[l]; d.out = dst;
-            rc = launch_dense(d, st);
-        }
-        if (rc != PSA_OK) return rc;
-        img += tc_dense_image_bytes(K, N < 64 ? 64 : N);
-        cur = dst;
-    }
-    return PSA_OK;
+    return run_chain(p, n, mlp, points, xyz, nullptr, 0, out, ws, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1905,17 +1887,35 @@ static bool edgeconv_dual_ok(int c, int k, const psa_mlp* mlp, psa_mlp* m2, TcAr
     return tc_sa_eligible(m2, 0, 32, a);
 }
 
-extern "C" size_t psa_edgeconv_workspace_bytes(int b, int n, int c, int k, const psa_mlp* mlp) {
-    if (mlp == nullptr) return 0;
+// The path of a single-layer EdgeConv call and its workspace, read by both psa_edgeconv_workspace_bytes and psa_edgeconv_infer.
+// Dual: the padded neighbour indices, then tc_sa_run's workspace at `off`.  Algebra: Wc, AB at `off`, the GEMM's image slot at
+// `img`, the zeroed word region at `words`.  FMA (the fused kernel): none.
+struct EdgePlan {
+    enum Path { kFma, kDual, kAlgebra } path = kFma;
+    psa_mlp m2;                       // dual: the level's MLP and its eligibility result
+    TcArgs a;
+    size_t off = 0, img = 0, words = 0, bytes = 0;
+};
+static EdgePlan edgeconv_plan(int b, int n, int c, int k, const psa_mlp* mlp) {
+    EdgePlan p;
     const long long rows = (long long)b * n;
-    {
-        psa_mlp m2;
-        TcArgs a;
-        if (edgeconv_dual_ok(c, k, mlp, &m2, &a)) return (((size_t)rows * 32 * 4 + 255) & ~(size_t)255) + tc_sa_workspace_bytes(a, b, n, 0);
+    if (edgeconv_dual_ok(c, k, mlp, &p.m2, &p.a)) {
+        p.path = EdgePlan::kDual;
+        p.off = al256((size_t)rows * 32 * 4);
+        p.bytes = p.off + tc_sa_workspace_bytes(p.a, b, n, 0);
+    } else if (edgeconv_algebra_ok(rows, c, k, mlp)) {
+        const int N = mlp->channels[1];
+        p.path = EdgePlan::kAlgebra;
+        p.off = al256((size_t)c * 2 * N * 4);
+        p.img = p.off + al256((size_t)rows * 2 * N * 4);
+        p.words = p.img + tc_dense_image_bytes(c, 2 * N);
+        p.bytes = p.words + 256;
     }
-    if (!edgeconv_algebra_ok(rows, c, k, mlp)) return 0;
-    const int N = mlp->channels[1];
-    return (((size_t)c * 2 * N * 4 + 255) & ~(size_t)255) + (((size_t)rows * 2 * N * 4 + 255) & ~(size_t)255) + tc_dense_image_bytes(c, 2 * N) + 256;
+    return p;
+}
+
+extern "C" size_t psa_edgeconv_workspace_bytes(int b, int n, int c, int k, const psa_mlp* mlp) {
+    return mlp == nullptr ? 0 : edgeconv_plan(b, n, c, k, mlp).bytes;
 }
 
 extern "C" int psa_edgeconv_infer(int b, int n, int c, int k, const float* x, const int* nn_idx, const psa_mlp* mlp,
@@ -1928,46 +1928,29 @@ extern "C" int psa_edgeconv_infer(int b, int n, int c, int k, const float* x, co
     PSA_REQUIRE(x && nn_idx && out, "edgeconv: null buffer");
     cudaStream_t st = as_stream(stream);
     const long long rows = (long long)b * n;
-    {
-        psa_mlp m2;
-        TcArgs a;
-        if (edgeconv_dual_ok(c, k, mlp, &m2, &a)) {
-            const size_t need = psa_edgeconv_workspace_bytes(b, n, c, k, mlp);
-            PSA_REQUIRE(workspace != nullptr && workspace_bytes >= need, "edgeconv: workspace of %zu bytes required (got %zu)", need, workspace_bytes);
-            PSA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "edgeconv: workspace must be 256-byte aligned");
-            int* idx32 = reinterpret_cast<int*>(workspace);
-            edge_pad_idx_kernel<<<(unsigned)((rows * 32 + 255) / 256 < 65535 * 4 ? (rows * 32 + 255) / 256 : 65535 * 4), 256, 0, st>>>(rows, k, nn_idx, idx32);
-            rc = check_launch("edge_pad_idx_kernel");
-            if (rc != PSA_OK) return rc;
-            return tc_sa_run(a, b, n, n, 0, 32, x, x, nullptr, idx32, &m2, mlp->weight[0], out,
-                             reinterpret_cast<uint8_t*>(workspace) + (((size_t)rows * 32 * 4 + 255) & ~(size_t)255), st);
-        }
-    }
-    if (!edgeconv_algebra_ok(rows, c, k, mlp)) return edgeconv_simt(b, n, c, k, x, nn_idx, mlp, out, st);
-    const int N = mlp->channels[1];
-    const size_t need = psa_edgeconv_workspace_bytes(b, n, c, k, mlp);
-    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= need, "edgeconv: workspace of %zu bytes required (got %zu)", need, workspace_bytes);
+    EdgePlan p = edgeconv_plan(b, n, c, k, mlp);
+    if (p.path == EdgePlan::kFma) return edgeconv_simt(b, n, c, k, x, nn_idx, mlp, out, st);
+    PSA_REQUIRE(workspace != nullptr && workspace_bytes >= p.bytes, "edgeconv: workspace of %zu bytes required (got %zu)", p.bytes, workspace_bytes);
     PSA_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 255) == 0, "edgeconv: workspace must be 256-byte aligned");
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
-    float* Wc = reinterpret_cast<float*>(ws);
-    ws += ((size_t)c * 2 * N * 4 + 255) & ~(size_t)255;
-    float* AB = reinterpret_cast<float*>(ws);
-    ws += ((size_t)rows * 2 * N * 4 + 255) & ~(size_t)255;
-    edge_wc_kernel<<<(c * 2 * N + 255) / 256, 256, 0, st>>>(c, N, mlp->weight[0], Wc);
-    if (tc_dense_eligible(rows, c, 2 * N, 1)) {
-        unsigned int* flag = reinterpret_cast<unsigned int*>(reinterpret_cast<uint8_t*>(workspace) + need - 256);
-        PSA_CUDA(cudaMemsetAsync(flag, 0, 256, st));
-        rc = launch_tc_dense(rows, c, 2 * N, 1, 0, x, Wc, nullptr, nullptr, AB, nullptr, ws, flag, flag + 1, st);
-    } else {
-        DenseArgs d;
-        d.rows = rows; d.K = c; d.N = 2 * N; d.pool_k = 1; d.relu = 0;
-        d.x = x; d.W = Wc; d.scale = nullptr; d.shift = nullptr; d.out = AB;
-        rc = launch_dense(d, st);
+    if (p.path == EdgePlan::kDual) {
+        int* idx32 = reinterpret_cast<int*>(ws);
+        edge_pad_idx_kernel<<<(unsigned)((rows * 32 + 255) / 256 < 65535 * 4 ? (rows * 32 + 255) / 256 : 65535 * 4), 256, 0, st>>>(rows, k, nn_idx, idx32);
+        rc = check_launch("edge_pad_idx_kernel");
+        if (rc != PSA_OK) return rc;
+        return tc_sa_run(p.a, b, n, n, 0, 32, x, x, nullptr, idx32, &p.m2, mlp->weight[0], out, ws + p.off, st);
     }
-    if (rc != PSA_OK) return rc;
+    const int N = mlp->channels[1];
+    float* Wc = reinterpret_cast<float*>(ws);
+    edge_wc_kernel<<<(c * 2 * N + 255) / 256, 256, 0, st>>>(c, N, mlp->weight[0], Wc);
+    DenseStep ab{rows, c, 2 * N, 1, 0, x, Wc, nullptr, nullptr, reinterpret_cast<float*>(ws + p.off)};
+    ab.img = ws + p.img;
+    ab.words = step_words(reinterpret_cast<unsigned int*>(ws + p.words), 0);
+    if (dense_on_tc(rows, c, 2 * N, 1)) PSA_CUDA(cudaMemsetAsync(ws + p.words, 0, 256, st));
+    if ((rc = run_dense(ab, st)) != PSA_OK) return rc;
     const int grid = (int)((rows + 7) / 8 < (long long)kNumSMs * 8 ? (rows + 7) / 8 : (long long)kNumSMs * 8);
     const int vec = N / 32;
-#define PSA_EDGE_LAUNCH(V) edge_gather_max_kernel<V><<<grid, 256, 0, st>>>(rows, n, k, N, AB, nn_idx, mlp->scale[0], mlp->shift[0], mlp->relu[0], out)
+#define PSA_EDGE_LAUNCH(V) edge_gather_max_kernel<V><<<grid, 256, 0, st>>>(rows, n, k, N, ab.out, nn_idx, mlp->scale[0], mlp->shift[0], mlp->relu[0], out)
     if (vec == 1) PSA_EDGE_LAUNCH(1); else if (vec == 2) PSA_EDGE_LAUNCH(2); else if (vec == 4) PSA_EDGE_LAUNCH(4); else PSA_EDGE_LAUNCH(8);
 #undef PSA_EDGE_LAUNCH
     return check_launch("edge_gather_max_kernel");
@@ -1992,20 +1975,19 @@ extern "C" int psa_mlp_image_plan(int usage, long long rows, int pool_k, int c, 
     if (rc != PSA_OK) return rc;
     for (int l = 0; l < PSA_MAX_MLP_LAYERS; ++l) { nt[l] = 0; row0[l] = 0; bytes[l] = 0; }
     if (g_mlp_mode == 1) return PSA_OK;
-    const int L = mlp->n_layers;
     if (usage == PSA_USAGE_SHARED_MLP || usage == PSA_USAGE_SA_GROUP_ALL) {
-        for (int l = 0; l < L; ++l) {
-            const int r0 = (usage == PSA_USAGE_SA_GROUP_ALL && l == 0) ? 3 : 0;
-            const int K = mlp->channels[l] - r0, N = mlp->channels[l + 1];
-            const int pk = (l == L - 1) ? pool_k : 1;
-            if (K >= 1 && tc_dense_eligible(rows, K, N, pk)) { nt[l] = tc_dense_nt(rows, N); row0[l] = r0; bytes[l] = tc_plan_image_bytes((K + 63) & ~63, N); }
+        const int r0 = usage == PSA_USAGE_SA_GROUP_ALL ? 3 : 0;
+        const ChainPlan p = chain_plan(rows, mlp, mlp->channels[0] - r0, r0);
+        for (int l = 0; l < p.L; ++l) {
+            const int K = p.K[l], N = p.N[l];
+            if (dense_on_tc(rows, K, N, l == p.L - 1 ? pool_k : 1)) { nt[l] = tc_dense_nt(rows, N); row0[l] = l == 0 ? r0 : 0; bytes[l] = tc_plan_image_bytes((K + 63) & ~63, N); }
         }
         return PSA_OK;
     }
     PSA_REQUIRE(usage == PSA_USAGE_SA_MODULE, "mlp_image_plan: unknown usage %d", usage);
     TcArgs a;
     if (!tc_sa_eligible(mlp, c, nsample, &a)) return PSA_OK;
-    if (c > 0 && tc_dense_eligible(rows, c, a.C1, 1)) { nt[0] = tc_dense_nt(rows, a.C1); row0[0] = 3; bytes[0] = tc_plan_image_bytes((c + 63) & ~63, a.C1); }
+    if (c > 0 && dense_on_tc(rows, c, a.C1, 1)) { nt[0] = tc_dense_nt(rows, a.C1); row0[0] = 3; bytes[0] = tc_plan_image_bytes((c + 63) & ~63, a.C1); }
     for (int l = 0; l < a.nl; ++l) { nt[1 + l] = tc_sa_image_nt(); row0[1 + l] = 0; bytes[1 + l] = tc_plan_image_bytes(a.Kd[l], a.Ntot[l]); }
     return PSA_OK;
 }

@@ -596,6 +596,109 @@ def spider_plan(b, npts, c, k, t, n):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# plans of the inference dense layers (csrc/tc_mlp.cu): the chain of psa_shared_mlp / psa_sa_group_all_infer, the
+# set-abstraction level and EdgeConv.  `mode` is psa_set_mlp_mode's.  tests/test_dense_chain_plan_cpu.py checks them against
+# the library's workspace queries and psa_mlp_image_plan.
+# ---------------------------------------------------------------------------------------------------------------------
+FC_KS = 64                        # kFcKs (csrc/mlp.cu): the K slice of one fc_small partial
+
+
+def dense_image_bytes(K, N):
+    """tc_dense_image_bytes: an fp16x2 image and the bf16x3 image of its rerun, K padded to 64"""
+    Kp = -(-K // 64) * 64
+    return image_bytes(Kp, N, 2) + image_bytes(Kp, N, 3)
+
+
+def dense_on_tc(rows, K, N, pool_k, mode):
+    """dense_on_tc / tc_dense_eligible: the tensor-core path of one dense layer"""
+    pool_ok = pool_k in (1, 32, 64) or (pool_k >= 128 and pool_k % 128 == 0)
+    return (mode != 1 and rows >= 128 and K >= 32 and N >= 64 and N % 64 == 0 and (N == 64 or N % 128 == 0) and pool_ok
+            and (pool_k == 1 or rows % pool_k == 0))
+
+
+def dense_nt(rows, N, mode):
+    """tc_dense_nt: the tile width with the image format flag of the mode"""
+    return (128 if wide_tiles(-(-rows // 128), N) else 64) | (0x100 if mode == 2 else 0x200)
+
+
+def plan_image_bytes(Kp, N, mode):
+    """tc_plan_image_bytes: a prebuilt image, fp16x2 blocks followed by their bf16x3 twin in mode 0"""
+    return image_bytes(Kp, N, 3) + (image_bytes(Kp, N, 2) if mode == 0 else 0)
+
+
+def chain_plan(rows, channels, K0):
+    """chain_plan: (K, N) per layer and the workspace bytes -- two ping-pong halves of the widest inner activation, an image
+    slot per layer, fc_small's partials when rows <= 32, the 256-byte word region"""
+    KN = [(K0 if l == 0 else channels[l], channels[l + 1]) for l in range(len(channels) - 1)]
+    inner = [K for K, _ in KN[1:]]
+    total = 2 * _al256(rows * max(inner) * 4) if inner else 0
+    total += sum(dense_image_bytes(K, max(N, 64)) for K, N in KN)
+    if rows <= 32:
+        total += _al256(max(-(-K // FC_KS) * 32 * N * 4 for K, N in KN))
+    return dict(layers=KN, total=total + 256)
+
+
+def chain_images(rows, pool_k, channels, row0, mode):
+    """psa_mlp_image_plan for a chain: (nt, row0, bytes) of each layer on the tensor cores, zeros for the others"""
+    out = []
+    KN = chain_plan(rows, channels, channels[0] - row0)["layers"]
+    for l, (K, N) in enumerate(KN):
+        pk = pool_k if l == len(KN) - 1 else 1
+        on = dense_on_tc(rows, K, N, pk, mode)
+        out.append((dense_nt(rows, N, mode), row0 if l == 0 else 0, plan_image_bytes(-(-K // 64) * 64, N, mode)) if on else (0, 0, 0))
+    return out
+
+
+def sa_tc_layers(channels, c, nsample, mode):
+    """tc_sa_eligible for both splits: [(Kd, Ntot)] of the level's tensor layers, or None for the FMA fused kernel"""
+    L = len(channels) - 1
+    if mode == 1 or not 2 <= L <= 3 or nsample not in (32, 64, 128) or channels[0] != 3 + c or channels[1] not in (64, 128):
+        return None
+    layers = [(channels[1 + l], channels[2 + l]) for l in range(L - 1)]
+    for l, (K, N) in enumerate(layers):
+        if K not in (64, 128) or (l < len(layers) - 1 and N not in (64, 128)) or (l == len(layers) - 1 and N != 64 and N % 128):
+            return None
+    # tc_sa_layout at np = 3, which the fp16x2 layout never exceeds: every layer resident, or the last one streamed through two
+    # slots of one 64-channel chunk
+    fixed = 8 * channels[1] * 4 + sum(2 * N * 4 for _, N in layers)
+    resident = sum(K * N * 2 * 3 for K, N in layers)
+    streamed = resident - layers[-1][0] * layers[-1][1] * 2 * 3 + 2 * (layers[-1][0] // 64) * 64 * 128 * 3
+    return layers if min(resident, streamed) + fixed + 1024 <= 220 * 1024 else None
+
+
+def sa_workspace(b, n, c, channels, layers):
+    """tc_sa_workspace_bytes: the word region, both images of every tensor layer, the U rows and the U GEMM's image slot"""
+    total = 256 + sum(image_bytes(K, N, 2) + image_bytes(K, N, 3) for K, N in layers)
+    return total + (_al256(b * n * channels[1] * 4) + dense_image_bytes(c, channels[1]) if c > 0 else 0)
+
+
+def sa_images(rows, c, nsample, channels, mode):
+    """psa_mlp_image_plan for a set-abstraction level: the U GEMM (row0 = 3) and the level's 64-wide tensor layers"""
+    out = [(0, 0, 0)] * 4
+    layers = sa_tc_layers(channels, c, nsample, mode)
+    if layers is None:
+        return out
+    if c > 0 and dense_on_tc(rows, c, channels[1], 1, mode):
+        out[0] = (dense_nt(rows, channels[1], mode), 3, plan_image_bytes(-(-c // 64) * 64, channels[1], mode))
+    for l, (K, N) in enumerate(layers):
+        out[1 + l] = (64 | (0x100 if mode == 2 else 0x200), 0, plan_image_bytes(K, N, mode))
+    return out
+
+
+def edgeconv_workspace(b, n, c, k, channels, mode):
+    """psa_edgeconv_workspace_bytes: the dual-SA path (c = 3, two layers or more), the algebra path (one layer), else none"""
+    rows = b * n
+    if mode != 1 and c == 3 and 1 <= k <= 32 and len(channels) >= 3:
+        layers = sa_tc_layers([3] + list(channels[1:]), 0, 32, mode)
+        if layers is not None:
+            return _al256(rows * 32 * 4) + sa_workspace(b, n, 0, channels, layers)
+    N = channels[1]
+    if mode == 1 or len(channels) != 2 or rows < 128 or k > 32 or N not in (32, 64, 128, 256):
+        return 0
+    return _al256(c * 2 * N * 4) + _al256(rows * 2 * N * 4) + dense_image_bytes(c, 2 * N) + 256
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # metrics
 # ---------------------------------------------------------------------------------------------------------------------
 def rel(got, want):
