@@ -360,7 +360,8 @@ fused_group_mlp_kernel(const __grid_constant__ FusedArgs a) {
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Dense single layer: out = relu?((x . W [+ group_add[r / group_rows]]) * scale + shift) with optional max over runs of pool_k rows.
+// Dense single layer: out = relu?((x . W [+ group_add[r / group_rows]] [+ xyz3[r] . w3]) * scale + shift) with optional max over
+// runs of pool_k rows.
 // A streamed from global in [BM][BK] chunks (cp.async when the row pitch allows 16-byte copies).
 // ------------------------------------------------------------------------------------------------------------
 constexpr int LDA_D = BK + 4;   // 20 floats = 80 B rows: 16-byte aligned, conflict-light
@@ -439,6 +440,23 @@ dense_layer_kernel(const __grid_constant__ DenseArgs a) {
                 for (int j = 0; j < 4; ++j) {
                     const int col = n0 + h * 64 + tx * 4 + j;
                     if (col < a.N) acc[i][h * 4 + j] += __ldg(ga + col);
+                }
+        }
+    }
+    if (a.xyz3 != nullptr) {           // the side input (pool_k == 1), in the same order as tc_dense_kernel's epilogue
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+            const int row = ty * 8 + i;
+            if (row >= tile_rows) break;
+            const float* q = a.xyz3 + (row0 + row) * 3;
+            const float x0 = __ldg(q), x1 = __ldg(q + 1), x2 = __ldg(q + 2);
+#pragma unroll
+            for (int h = 0; h < TN / 4; ++h)
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const int col = n0 + h * 64 + tx * 4 + j;
+                    if (col < a.N)
+                        acc[i][h * 4 + j] = fmaf(x2, __ldg(a.w3 + 2 * a.N + col), fmaf(x1, __ldg(a.w3 + a.N + col), fmaf(x0, __ldg(a.w3 + col), acc[i][h * 4 + j])));
                 }
         }
     }

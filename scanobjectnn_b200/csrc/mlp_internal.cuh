@@ -17,6 +17,9 @@ struct DenseArgs {
     // optional per-row-group input, pool_k == 1 only: row r adds group_add[r / group_rows] (N) to x . W before the affine
     const float* group_add = nullptr;
     long long group_rows = 0;
+    // optional side input, pool_k == 1 only: row r adds xyz3[r] (3) . w3 (3, N) to x . W before the affine
+    const float* xyz3 = nullptr;
+    const float* w3 = nullptr;
 };
 
 

@@ -4,11 +4,12 @@
 // What the reference does (pointnet2/utils/pointnet_util.py:113-127): group_point -> (B,m,K,3+C) tensor -> three
 // cuDNN 1x1 convs over B*m*K rows -> reduce_max.  What the kernels here do per tile (64 or 128 rows):
 //
-//   layer 1   is never a GEMM over grouped rows.  (x_j - c) . Wx + f_j . Wf  =  U[j] + (x_j - c) . Wx   with
-//             U = points . W1[3:,:] computed ONCE per source point (K-fold fewer rows, a dense-layer launch); each
-//             thread gathers its part of the U rows, adds the 3-term xyz part in FMAs, applies the folded BN affine + ReLU
-//             and keeps the result in registers as the A operand of layer 2 -- the (B,m,K,C) tensors of the reference
-//             never exist, not even in shared memory.
+//   layer 1   is never a GEMM over grouped rows.  s ((x_j - c) . Wx + f_j . Wf) + t  =  V[j] - c . (s Wx)   with
+//             V = s (points . W1[3:,:] + xyz . W1[:3,:]) + t computed ONCE per source point (K-fold fewer rows, a dense-layer
+//             launch); each thread gathers its part of the V rows, subtracts the centre term of its columns (3 FMAs per column
+//             and neighbourhood, shared by its rows), applies the ReLU and keeps the result in registers as the A operand of
+//             layer 2 -- the (B,m,K,C) tensors of the reference never exist, not even in shared memory.  Levels without
+//             input features evaluate t + (x_j - c) . (s Wx) per row.
 //   layers 2+ wgmma, A from registers, B = weights in shared memory in the canonical K-major SWIZZLE_128B layout, dropped
 //             there by cp.async.bulk from pre-arranged images; D in registers, whose layout is that of the next A operand.
 //   max-pool  the last epilogue reduces each neighbourhood's rows in-thread, across the warp with shuffles and across warps in
@@ -67,7 +68,7 @@ struct TcArgs {
     int n, m;              // dataset points / queries per cloud
     const float* xyz;      // (b,n,3)
     const float* new_xyz;  // (b,m,3)
-    const float* uf;       // (b*n, C1) = points . W1[3:,:], or null when the level has no input features
+    const float* uf;       // (b*n, C1) = V = s (points . W1[3:,:] + xyz . W1[:3,:]) + t, or null when the level has no input features
     const int* idx;        // (groups, K)
     float* out;            // (groups, Ntot[last])
     // layer 1 (FMA path)
@@ -193,8 +194,9 @@ __global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float
 //   the rows of each neighbourhood before its ball-query padding (16-row slots packed back to back); K = 128 or a streamed
 //   last layer: the two work together on 128-row passes of whole neighbourhoods.  NL = 2: layer 1's gathers are issued one
 //   pass ahead.
-//   * layer 1 on the FMA pipe: each thread evaluates U[j] + (x_j - c) . Wx (+ c . Wc), the folded affine and ReLU for the
-//     rows and channels of ITS A fragment and splits the result into NP pieces -- straight into registers;
+//   * layer 1 on the FMA pipe: each thread evaluates V[j] + c . s (Wc - Wx) (levels with input features) or
+//     t + (x_j - c) . s Wx (+ c . s Wc), and the ReLU for the rows and channels of ITS A fragment and splits the result into
+//     NP pieces -- straight into registers;
 //   * inner tensor layers: wgmma with A from registers, B = weight image in shared memory; the D fragment goes through
 //     affine + ReLU + split and is the next layer's A fragment (same register layout), nothing is staged;
 //   * last layer in 64-channel chunks: wgmma, affine + ReLU, max over each neighbourhood's rows (in-thread, shuffles across
@@ -225,7 +227,7 @@ __host__ __device__ inline TcSaLayout tc_sa_layout(const TcArgs& a) {
     L.ring[0] = off; off += L.ring_bytes;
     L.ring[1] = off; off += L.ring_bytes;
     L.vec = off;
-    off += 8u * a.C1 * 4u;       // w1x (3 C1), w1c (3 C1), s1, t1
+    off += 7u * a.C1 * 4u;       // w1x (3 C1), w1c (3 C1), t1
 #pragma unroll
     for (int l = 0; l < kMaxTcLayers; ++l) off += l < a.nl ? 2u * a.Ntot[l] * 4u : 0u;
     L.total = off;
@@ -276,6 +278,45 @@ __device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[
     for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
 }
 
+#ifdef PSA_SA_STAMPS
+// Pass timeline (tools/sa_timing.py builds a separate library with -DPSA_SA_STAMPS; libpsa.so has none of this): lane 0 of the
+// first warp of each warpgroup of CTA i < kSaStampCtas writes clock64() at phase k of the unit's pass p < kSaStampPasses
+// (SaStamp below; chunk nc of the last layer at kSaChunk0 + 3 nc + {issued, retired, epilogue done}).  psa_sa_stamps_clear zeroes
+// the table, so that a slot a launch did not reach reads 0.
+enum SaStamp { kSaTop, kSaInputs, kSaLayer1, kSaL2Issued, kSaL2Retired, kSaL2Epi, kSaPool1, kSaPool2, kSaNextA, kSaNextB, kSaChunk0 };
+constexpr int kSaStampCtas = 264, kSaStampPasses = 64, kSaStampPhases = kSaChunk0 + 3 * 4;
+__device__ long long g_sa_stamps[kSaStampCtas][2][kSaStampPasses][kSaStampPhases];
+extern "C" PSA_API int psa_sa_stamps(long long* dst) {
+    return cudaMemcpyFromSymbol(dst, g_sa_stamps, sizeof(g_sa_stamps)) == cudaSuccess ? 0 : 1;
+}
+extern "C" PSA_API int psa_sa_stamps_clear(void) {
+    void* p = nullptr;
+    if (cudaGetSymbolAddress(&p, g_sa_stamps) != cudaSuccess) return 1;
+    return cudaMemset(p, 0, sizeof(g_sa_stamps)) == cudaSuccess ? 0 : 1;
+}
+#define SA_STAMP(p, k)                                                                                              \
+    do {                                                                                                            \
+        if ((threadIdx.x & 127) == 0 && blockIdx.x < kSaStampCtas && (p) < kSaStampPasses && (k) < kSaStampPhases) \
+            g_sa_stamps[blockIdx.x][threadIdx.x >> 7][(p)][(k)] = clock64();                                        \
+    } while (0)
+// the stamp after a volatile store of a value computed from the float r, so the load that wrote r has landed
+#define SA_STAMP_AFTER(p, k, r)                                                                                     \
+    do {                                                                                                            \
+        if ((threadIdx.x & 127) == 0 && blockIdx.x < kSaStampCtas && (p) < kSaStampPasses) {                        \
+            volatile long long* p_ = &g_sa_stamps[blockIdx.x][threadIdx.x >> 7][(p)][(k)];                          \
+            *p_ = (long long)__float_as_uint(__fmul_rn((r), 0.f));                                                  \
+            *p_ = clock64();                                                                                        \
+        }                                                                                                           \
+    } while (0)
+#else
+#define SA_STAMP(p, k) \
+    do {               \
+    } while (0)
+#define SA_STAMP_AFTER(p, k, r) \
+    do {                        \
+    } while (0)
+#endif
+
 // Specialised on the level shape: C1 = width of layer 1 (64 | 128), NL = tensor layers (1 | 2), N0 = width of the inner tensor
 // layer when NL = 2 (64 | 128).  The last layer's width is a runtime multiple of 64.
 template <int NP, int C1, int NL, int N0>
@@ -306,19 +347,19 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     float* vec = reinterpret_cast<float*>(base + L.vec);
     float* w1x = vec;
     float* w1c = vec + 3 * C1;
-    float* s1 = vec + 6 * C1;
-    float* t1 = s1 + C1;
+    float* t1 = vec + 6 * C1;
     float* sl0 = t1 + C1;                                     // scale / shift of tensor layer 0 ..
     float* tl0 = sl0 + a.Ntot[0];
     float* slL = NL == 2 ? tl0 + a.Ntot[0] : sl0;             // .. and of the last one
     float* tlL = slL + a.Ntot[last];
-    // the BN scale of layer 1 is folded into its xyz / centre weights: s (U + d.W) + t = (s U + t) + d.(s W)
+    // the BN scale of layer 1 is folded into its xyz / centre weights: s (d.Wx + c.Wc) + t = t + d.(s Wx) + c.(s Wc).  With
+    // input features the xyz part of the neighbour is in V (x_j.Wx, the affine), and w1c holds s (Wc - Wx): V[j] + c.w1c
     for (int i = tid; i < 3 * C1; i += kSaThreads) {
         const float sc = a.s1 ? __ldg(a.s1 + i % C1) : 1.f;
         w1x[i] = __ldg(a.w1x + i) * sc;
-        w1c[i] = a.w1c ? __ldg(a.w1c + i) * sc : 0.f;
+        w1c[i] = (a.w1c ? __ldg(a.w1c + i) : 0.f) * sc - (a.uf ? w1x[i] : 0.f);
     }
-    for (int i = tid; i < C1; i += kSaThreads) { s1[i] = a.s1 ? __ldg(a.s1 + i) : 1.f; t1[i] = __ldg(a.t1 + i); }
+    for (int i = tid; i < C1; i += kSaThreads) t1[i] = __ldg(a.t1 + i);
     // the column factors of the fp16x2 weight images are folded into the tensor layers' scales
 #pragma unroll
     for (int l = 0; l < NL; ++l)
@@ -406,14 +447,15 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     };
 
     // Layer 1's inputs for this thread's two rows are gathered one pass ahead (NL = 2), while the previous pass's last-layer
-    // wgmma run: stage A (neighbour index, centre) once the first chunk is issued, stage B (neighbour coordinates, U row) once
-    // the last one is.  The next pass's slot table must be filled by then; it is not when the next pass opens a chunk claimed
-    // in this very pass (the table is filled between the pooling barriers), and both stages then follow the first pooling.
-    // The 64-float U rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM); other levels
-    // load them in layer 1.
-    constexpr bool kHoldU = NP == 2 && C1 == 128;
+    // wgmma run: stage A (neighbour index, centre) once the first chunk is issued, stage B (the V row, or the neighbour
+    // coordinates of a level without input features) once the last one is.  The next pass's slot table must be filled by
+    // then; it is not when the next pass opens a chunk claimed in this very pass (the table is filled between the pooling
+    // barriers), and both stages then follow the first pooling.
+    // The 64-float V rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM); other levels
+    // load them in layer 1, as do the levels that gather at the top of the pass (nothing to hide the loads behind there).
     constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the pass:
                                                               // measured faster there, the pass is too short to hide the loads
+    constexpr bool kHoldU = NP == 2 && C1 == 128 && kAhead;
     constexpr int kUH = kHoldU ? C1 / 8 : 1;                  // float2 per row held
     int incl = 0;                                             // slots of the chunk gather_a last read, prefix (lane i: neighbourhoods
                                                               // 0..i); the chunk's total is lane C - 1's, one shuffle away
@@ -458,8 +500,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         const long long bi = gn / a.m;
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
-            const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
-            px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
+            if (a.uf == nullptr) {                            // with input features the neighbour's coordinates are in V
+                const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
+                px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
+            }
             urow[i] = a.uf ? a.uf + ((size_t)bi * a.n + jn[i]) * C1 : nullptr;
             if constexpr (kHoldU) {
                 if (a.uf != nullptr) {
@@ -483,48 +527,73 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     uint32_t it = 0;                                          // passes of this unit
     for (; ch < nchunks; ++it) {
         if (p == 0 && ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
+        SA_STAMP(it, kSaTop);
         if (!kAhead) { gather_a(ch, buf, p, it & 1); gather_b(); }
+        SA_STAMP_AFTER(it, kSaInputs, a.uf == nullptr ? px[0] : kHoldU ? uh[0][0].x : __ldg(urow[0] + 2 * t));
 
         // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
         uint32_t A[NP][8][4];
-        {
+        if (a.uf != nullptr) {
+            // V[j] + c . w1c: the centre term of a column is shared by this thread's two rows (one neighbourhood per warp)
+#pragma unroll
+            for (int s = 0; s < C1 / 16; ++s) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int k = 16 * s + 8 * h + 2 * t;
+                    const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
+                                 cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
+                    const float2 ct = ffma2_rn(make_float2(cz, cz), cwz, ffma2_rn(make_float2(cy, cy), cwy, fmul2_rn(make_float2(cx, cx), cwx)));
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        float2 v;
+                        if constexpr (kHoldU) v = uh[i][2 * s + h];
+                        else v = __ldg(reinterpret_cast<const float2*>(urow[i] + k));
+                        v = fadd2_rn(v, ct);
+                        if (a.relu1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+                        put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);
+                    }
+                }
+            }
+        } else {
+            // t + (x_j - c) . w1x (+ c . w1c)
             float dx[2], dy[2], dz[2];
 #pragma unroll
             for (int i = 0; i < 2; ++i) { dx[i] = px[i] - cx; dy[i] = py[i] - cy; dz[i] = pz[i] - cz; }
 #pragma unroll
             for (int s = 0; s < C1 / 16; ++s) {
-                {
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int k = 16 * s + 8 * h + 2 * t;
-                        const float2 sc = *reinterpret_cast<const float2*>(s1 + k), sh = *reinterpret_cast<const float2*>(t1 + k);
-                        const float2 wx = *reinterpret_cast<const float2*>(w1x + k), wy = *reinterpret_cast<const float2*>(w1x + C1 + k),
-                                     wz = *reinterpret_cast<const float2*>(w1x + 2 * C1 + k);
+                for (int h = 0; h < 2; ++h) {
+                    const int k = 16 * s + 8 * h + 2 * t;
+                    const float2 sh = *reinterpret_cast<const float2*>(t1 + k);
+                    const float2 wx = *reinterpret_cast<const float2*>(w1x + k), wy = *reinterpret_cast<const float2*>(w1x + C1 + k),
+                                 wz = *reinterpret_cast<const float2*>(w1x + 2 * C1 + k);
 #pragma unroll
-                        for (int i = 0; i < 2; ++i) {
-                            float2 uv;
-                            if constexpr (kHoldU) uv = uh[i][2 * s + h];
-                            else uv = urow[i] ? __ldg(reinterpret_cast<const float2*>(urow[i] + k)) : sh;
-                            float2 v = a.uf ? ffma2_rn(uv, sc, sh) : sh;
-                            if (a.w1c != nullptr) {        // EdgeConv: the part of the first layer that acts on the centre x_i
-                                const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
-                                             cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
-                                v = ffma2_rn(make_float2(cz, cz), cwz, ffma2_rn(make_float2(cy, cy), cwy, ffma2_rn(make_float2(cx, cx), cwx, v)));
-                            }
-                            v = ffma2_rn(make_float2(dz[i], dz[i]), wz, ffma2_rn(make_float2(dy[i], dy[i]), wy, ffma2_rn(make_float2(dx[i], dx[i]), wx, v)));
-                            if (a.relu1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
-                            put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);
+                    for (int i = 0; i < 2; ++i) {
+                        float2 v = sh;
+                        if (a.w1c != nullptr) {            // EdgeConv: the part of the first layer that acts on the centre x_i
+                            const float2 cwx = *reinterpret_cast<const float2*>(w1c + k), cwy = *reinterpret_cast<const float2*>(w1c + C1 + k),
+                                         cwz = *reinterpret_cast<const float2*>(w1c + 2 * C1 + k);
+                            v = ffma2_rn(make_float2(cz, cz), cwz, ffma2_rn(make_float2(cy, cy), cwy, ffma2_rn(make_float2(cx, cx), cwx, v)));
                         }
+                        v = ffma2_rn(make_float2(dz[i], dz[i]), wz, ffma2_rn(make_float2(dy[i], dy[i]), wy, ffma2_rn(make_float2(dx[i], dx[i]), wx, v)));
+                        if (a.relu1) { v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); }
+                        put_a<NP, 8>(A, s, i + 2 * h, v.x, v.y, ovf);
                     }
                 }
             }
         }
+        SA_STAMP(it, kSaLayer1);
 
         if constexpr (NL == 2) {
             // ---- inner layer (N0 wide): D fragments -> affine + ReLU -> A fragments of the last layer ----
             constexpr int NCH = N0 / 64;
             float d[NCH][32];
-            sa_mma<NP, C1 / 16, NCH>(d, A, smem_u32(base + L.w[0]), (uint32_t)(C1 / 64) * bb);
+            sa_mma_issue<NP, C1 / 16, NCH>(d, A, smem_u32(base + L.w[0]), (uint32_t)(C1 / 64) * bb);
+            SA_STAMP(it, kSaL2Issued);
+            wg_wait_all();
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) wg_fence_acc(d[c]);
+            SA_STAMP(it, kSaL2Retired);
 #pragma unroll
             for (int c = 0; c < NCH; ++c) {
 #pragma unroll
@@ -542,6 +611,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                     }
                 }
             }
+            SA_STAMP(it, kSaL2Epi);
         }
         if constexpr (NP == 2) { ovf_seen = ovf_seen || f16x2_overflowed(ovf); ovf = 0u; }   // every leading piece is stored
         {
@@ -565,10 +635,12 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                     wb = smem_u32(base + L.w[last]) + (uint32_t)(nc * (KSL / 4)) * bb;
                 }
                 sa_mma_issue<NP, KSL, 1>(acc, A, wb, 0u);
+                SA_STAMP(it, kSaChunk0 + 3 * nc);
             };
             // affine + ReLU of chunk nc, this warp's 16-row column maxima (and warp 0's carried run max) into its row of `red`
             auto epilogue = [&](float (&acc)[1][32], int nc) {
                 wg_fence_acc(acc[0]);
+                SA_STAMP(it, kSaChunk0 + 3 * nc + 1);
                 auto rowmax = [&](int j) {                        // columns 8j + 2t, + 1: max over rows g, g + 8
                     const int col = nc * 64 + 8 * j + 2 * t;
                     const float2 sc = *reinterpret_cast<const float2*>(slL + col), sh = *reinterpret_cast<const float2*>(tlL + col);
@@ -597,10 +669,12 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                     m.y = carry_in ? fmaxf(m.y, c.y) : m.y;
                 }
                 *reinterpret_cast<float2*>(dst) = m;
+                SA_STAMP(it, kSaChunk0 + 3 * nc + 2);
             };
             // chunks [gi NG, gi NG + NG) are in `red`: combine the run starting at each warp's slot, two columns per lane
             auto pool = [&](int gi) {
                 unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in red; ring slot consumed
+                SA_STAMP(it, kSaPool1);
                 if (gi == 0 && p == 0) {                          // the chunk claimed at the top of this pass
                     claimed = s_claim[unit];
                     if (claimed < nchunks) fill_table(claimed, buf ^ 1);
@@ -622,7 +696,13 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                     }
                 }
                 unit_bar_sync(ubar, uthreads);                    // red is reused by the next group; the slot table is filled
-                if (gi == 0 && after_pool && claimed < nchunks) { gather_a(claimed, buf ^ 1, 0, (it + 1) & 1); gather_b(); }
+                SA_STAMP(it, kSaPool2);
+                if (gi == 0 && after_pool && claimed < nchunks) {
+                    gather_a(claimed, buf ^ 1, 0, (it + 1) & 1);
+                    SA_STAMP(it, kSaNextA);
+                    gather_b();
+                    SA_STAMP(it, kSaNextB);
+                }
             };
             // Every path below issues and waits in straight lines, and every group ends in wait_group 0 before pooling: ptxas
             // keeps the wgmma asynchronous only when it can see which group a wait retires on every path.  Stage B of the
@@ -632,7 +712,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
             for (int c0 = 0; c0 < NCL; c0 += NG) {
                 const int end = c0 + NG;
                 issue(d0, c0);
-                if (ahead && c0 == 0) gather_a(same ? ch : claimed, same ? buf : buf ^ 1, same ? p + 1 : 0, (it + 1) & 1);
+                if (ahead && c0 == 0) {
+                    gather_a(same ? ch : claimed, same ? buf : buf ^ 1, same ? p + 1 : 0, (it + 1) & 1);
+                    SA_STAMP(it, kSaNextA);
+                }
                 if constexpr (kDouble) {
                     float d1[1][32];
                     int nc = c0;
@@ -642,15 +725,15 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                     }
                     if (nc + 1 < end) {
                         issue(d1, nc + 1); wg_wait<1>(); epilogue(d0, nc);
-                        if (ahead && nc + 2 == NCL) gather_b();
+                        if (ahead && nc + 2 == NCL) { gather_b(); SA_STAMP(it, kSaNextB); }
                         wg_wait<0>(); epilogue(d1, nc + 1);
                     } else {
-                        if (ahead && nc + 1 == NCL) gather_b();
+                        if (ahead && nc + 1 == NCL) { gather_b(); SA_STAMP(it, kSaNextB); }
                         wg_wait<0>(); epilogue(d0, nc);
                     }
                 } else {
                     for (int nc = c0;;) {
-                        if (ahead && nc + 1 == NCL) gather_b();
+                        if (ahead && nc + 1 == NCL) { gather_b(); SA_STAMP(it, kSaNextB); }
                         wg_wait<0>(); epilogue(d0, nc);
                         if (++nc == end) break;
                         issue(d0, nc);
@@ -988,7 +1071,7 @@ struct DenseStep {
     const float* scale;                  // or null
     const float* shift;                  // or null
     float* out;
-    const float* xyz3 = nullptr;         // (rows, 3) side input with w3 (3, N): the tensor-core path only
+    const float* xyz3 = nullptr;         // (rows, 3) side input with w3 (3, N)
     const float* w3 = nullptr;
     const float* group_add = nullptr;
     long long group_rows = 0;
@@ -1020,12 +1103,11 @@ static int run_dense(const DenseStep& s, cudaStream_t st) {
         const RingWeights w = tc_dense_weights(s);
         return ring_run(kDenseRing, tc_dense_args(s), tc_dense_units(s.rows, s.N, w.Nt), w, s.words.flag, s.words.counters, st, pool);
     }
-    PSA_SUPPORTED(s.xyz3 == nullptr, "sa_group_all: layer 0 must run on the tensor-core path");
     DenseArgs d;
     d.rows = s.rows; d.K = s.K; d.N = s.N; d.pool_k = s.pool_k; d.relu = s.relu;
     d.x = s.x; d.W = s.W; d.scale = s.scale; d.shift = s.shift; d.out = s.out;
-    d.group_add = s.group_add; d.group_rows = s.group_rows;
-    if (s.fc_partial != nullptr && s.rows <= 32 && s.pool_k == 1 && s.group_add == nullptr) return launch_fc_small(d, s.fc_partial, st);
+    d.group_add = s.group_add; d.group_rows = s.group_rows; d.xyz3 = s.xyz3; d.w3 = s.w3;
+    if (s.fc_partial != nullptr && s.rows <= 32 && s.pool_k == 1 && s.group_add == nullptr && s.xyz3 == nullptr) return launch_fc_small(d, s.fc_partial, st);
     return launch_dense(d, st);
 }
 
@@ -1161,9 +1243,12 @@ static int tc_sa_run(TcArgs& a, int b, int n, int m, int c, int nsample, const f
     }
     const float* uf = nullptr;
     if (c > 0) {
-        // U = points . W1[3:,:]  once per source point (rows b*n), raw (affine + ReLU are applied after the xyz part)
+        // V = s (points . W1[3:,:] + xyz . W1[:3,:]) + t  once per source point (rows b*n), no ReLU: the level subtracts the
+        // centre's part before it
         const long long rows = (long long)b * n;
-        DenseStep u{rows, c, a.C1, 1, 0, points, mlp->weight[0] + (size_t)3 * a.C1, nullptr, nullptr, reinterpret_cast<float*>(ws)};
+        DenseStep u{rows, c, a.C1, 1, 0, points, mlp->weight[0] + (size_t)3 * a.C1, mlp->scale[0], mlp->shift[0], reinterpret_cast<float*>(ws)};
+        u.xyz3 = xyz;
+        u.w3 = mlp->weight[0];
         u.prebuilt = prebuilt_image(mlp, 0, 3, tc_dense_nt(rows, a.C1));
         u.img = ws + (((size_t)rows * a.C1 * sizeof(float) + 255) & ~(size_t)255);
         u.words = step_words(region, 0);
