@@ -561,6 +561,48 @@ PSA_API int psa_topk_pool(int b, int n, int c, int k, const float* y, const floa
                           float* out, int out_channels, int offset, psa_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * SpiderCNN, training backward (fp32 FMA, no float atomics: every sum in a fixed order).  Notation of
+ * psa_spider_conv_infer; dy (b,n,c_out) = the gradient of a layer's pre-group-norm output y.  T == 5 only
+ * (SpiderCNN's taylor_channel), else PSA_ERR_UNSUPPORTED.  No (b,n,k,c*T) tensor is formed.
+ * ------------------------------------------------------------------------------------------- */
+
+/* g (b,n,k,T) = the Taylor filter values g_t(delta[p][j]) of psa_spider_conv_infer, bit-identical to its own. */
+PSA_API int psa_spider_taylor_filter(int b, int n, int k, int T, const float* delta, const float* taylor, float* g,
+                                     psa_stream_t stream);
+
+/* Scratch of psa_spider_conv_bwd_weight, psa_spider_taylor_grad and psa_spider_gn_bwd for these dims (one buffer serves all
+ * three); 256-byte aligned.  0 for dims none of them takes. */
+PSA_API size_t psa_spider_conv_bwd_workspace_bytes(int b, int n, int c, int k, int T, int c_out);
+
+/* dW (k, c*T, c_out) = A^T . dy with A[p][j*c*T + ch*T + t] = h[nn(p,j)][ch] * g[p][j][t] (the reference's conv-input row
+ * order, so dW is the variable's gradient as it is laid out); h as in psa_spider_conv_infer. */
+PSA_API int psa_spider_conv_bwd_weight(int b, int n, int c, int k, int T, int c_out, const int* nn_idx, const float* feat,
+                                       const float* feat_scale, const float* feat_shift, const float* g, const float* dy, float* dW,
+                                       void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* With Q[p][j][ch][t] = sum_o dy[p][o] * W[j][ch*T + t][o] (never stored):
+ *   D (b,n,k,c)  D[p][j][ch] = sum_t g[p][j][t] * Q     (NULL: skipped; psa_group_point_grad(D, nn_idx) is then dh of feat)
+ *   dg (b,n,k,T) dg[p][j][t] = sum_ch h[nn(p,j)][ch] * Q */
+PSA_API int psa_spider_conv_bwd_data(int b, int n, int c, int k, int T, int c_out, const int* nn_idx, const float* feat,
+                                     const float* feat_scale, const float* feat_shift, const float* g, const float* W, const float* dy,
+                                     float* D, float* dg, psa_stream_t stream);
+
+/* dtaylor[m * ld_taylor + t] = sum_{p,j} dg[p][j][t] * mono_m(delta[p][j]), m in psa_spider_conv_infer's monomial order,
+ * accumulated in fp64. */
+PSA_API int psa_spider_taylor_grad(int b, int n, int k, int T, const float* delta, const float* dg, float* dtaylor, int ld_taylor,
+                                   void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* Backward of h = relu(group_norm(y)) and of its top-2 pooling: per (cloud, group) the forward's fp64 mean and variance
+ * (psa_group_norm_affine), the winners of psa_topk_pool on relu(y * scale + shift) with tf.nn.top_k's tie order (lower point
+ * first), dh = dpool routed to the winners (dpool (b, pool_channels, 2), this layer's channels at offset) + dh_next (b,n,c) or
+ * NULL, dz = dh where y * scale + shift > 0, and
+ *   dy = rstd * (gamma dz - mean_group(gamma dz) - xhat * mean_group(gamma dz xhat)),  dgamma = sum dz xhat,  dbeta = sum dz.
+ * c / groups must divide 256; n >= 2. */
+PSA_API int psa_spider_gn_bwd(int b, int n, int c, int groups, float eps, const float* y, const float* scale, const float* shift,
+                              const float* gamma, const float* dpool, int pool_channels, int offset, const float* dh_next, float* dy,
+                              float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * 3DmFV-Net, inference mode (3DmFV-Net/utils/tf_util.py:578-652 get_3dmfv, :254-311 conv3d, :406-429 pools)
  * Grid activations are (b * r^3, c) in voxel-major row order: row = voxel * b + cloud, voxel = (d * r + h) * r + w.
  * ------------------------------------------------------------------------------------------- */

@@ -114,6 +114,12 @@ SIGNATURES = {
     "psa_spider_conv_infer": [_i, _i, _i, _i, _i, _i] + [_p] * 9 + [_p, _sz, _p],
     "psa_group_norm_affine": [_i, _i, _i, _i, _f, _p, _p, _p, _p, _p, _p, _i, _p],
     "psa_topk_pool": [_i, _i, _i, _i, _p, _p, _p, _i, _p, _i, _i, _p],
+    # SpiderCNN (training backward)
+    "psa_spider_taylor_filter": [_i, _i, _i, _i, _p, _p, _p, _p],
+    "psa_spider_conv_bwd_weight": [_i] * 6 + [_p] * 7 + [_p, _sz, _p],
+    "psa_spider_conv_bwd_data": [_i] * 6 + [_p] * 9 + [_p],
+    "psa_spider_taylor_grad": [_i, _i, _i, _i, _p, _p, _p, _i, _p, _sz, _p],
+    "psa_spider_gn_bwd": [_i, _i, _i, _i, _f, _p, _p, _p, _p, _p, _i, _i, _p, _p, _p, _p, _p, _sz, _p],
     # 3DmFV-Net (inference)
     "psa_fisher_vector": [_i, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_conv3d_infer": [_i, _i, _i, _i, _i, _p, _ll, _p, _p, _p, _i, _p, _ll, _p, _sz, _p],
@@ -131,7 +137,7 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_train_dense_workspace_bytes", "psa_bn_bwd_workspace_bytes", "psa_sa_conv1_bwd_workspace_bytes", "psa_knn_graph_workspace_bytes",
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
                 "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes", "psa_spider_conv_workspace_bytes",
-                "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes")
+                "psa_spider_conv_bwd_workspace_bytes", "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes")
 
 _lib = None
 
@@ -178,6 +184,8 @@ def load() -> C.CDLL:
     lib.psa_edgeconv2_train_workspace_bytes.restype = C.c_size_t
     lib.psa_spider_conv_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
     lib.psa_spider_conv_workspace_bytes.restype = C.c_size_t
+    lib.psa_spider_conv_bwd_workspace_bytes.argtypes = [_i, _i, _i, _i, _i, _i]
+    lib.psa_spider_conv_bwd_workspace_bytes.restype = C.c_size_t
     lib.psa_conv3d_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
     lib.psa_conv3d_workspace_bytes.restype = C.c_size_t
     lib.psa_dense_elu_affine_workspace_bytes.argtypes = [_ll, _i, _i]

@@ -21,6 +21,8 @@ int launch_group_csr(int b, int n, int mk, const int* idx, int* offsets, int* li
 
 // train.cu: out[e] = sum_p partial[p * len + e] in a fixed order (fp64)
 int reduce_partials(int nparts, int len, const float* partial, float* out, cudaStream_t st);
+// train.cu: the contraction split of a weight gradient over `rows` rows with `tiles` output tiles (splits, rows per split)
+int weight_grad_splits(long long rows, int tiles, long long* k_per_split);
 // train.cu: batch-norm backward from (nparts, 2, C) partials [sum dz | sum dz * xhat] over `rows` rows -> dgamma, dbeta and the
 // coefficients of dy = ca * dz + cb * y + cc (psa_bn_bwd_coeffs)
 int launch_bn_bwd_final(int nparts, int C, long long rows, const float* partial, const float* gamma, const float* mean_inv, float* dgamma,

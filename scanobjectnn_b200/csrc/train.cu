@@ -513,7 +513,7 @@ static int small_m_splits(long long contraction) {
     return (int)(s < 1 ? 1 : (s > 16 ? 16 : s));
 }
 
-static int weight_grad_splits(long long rows, int tiles, long long* k_per_split) {
+int weight_grad_splits(long long rows, int tiles, long long* k_per_split) {
     long long want = (2LL * kNumSMs + tiles - 1) / tiles;
     long long maxs = (rows + 255) / 256;                       // at least 256 rows of contraction per split
     if (want > maxs) want = maxs;

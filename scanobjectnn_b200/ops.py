@@ -697,6 +697,116 @@ def topk_pool(y, k: int = 2, scale=None, shift=None, relu: bool = False, out=Non
     return out
 
 
+# --- SpiderCNN training backward (psa_spider_*: fp32 FMA, fixed-order sums) ---
+def _spider_ws(b, n, c, k, t, c_out, device):
+    need = int(_lib.load().psa_spider_conv_bwd_workspace_bytes(b, n, c, k, t, c_out))
+    return torch.empty((max(need, 4) + 3) // 4, dtype=torch.float32, device=device), C.c_size_t(need)
+
+
+def spider_taylor_filter(delta, taylor) -> torch.Tensor:
+    """The Taylor filter values of spider_conv: delta (B,N,k,3), taylor (20,T) -> g (B,N,k,T)."""
+    delta = _dev(delta, torch.float32, "delta", 4)
+    taylor = _dev(taylor, torch.float32, "taylor", 2)
+    b, n, k, three = delta.shape
+    if three != 3 or taylor.shape[0] != 20:
+        raise ValueError(f"spider_taylor_filter: delta {tuple(delta.shape)} / taylor {tuple(taylor.shape)}: want (B,N,k,3) / (20,T)")
+    g = torch.empty((b, n, k, taylor.shape[1]), dtype=torch.float32, device=delta.device)
+    check(_lib.load().psa_spider_taylor_filter(b, n, k, taylor.shape[1], _ptr(delta), _ptr(taylor), _ptr(g), _stream()), "spider_taylor_filter")
+    return g
+
+
+def _spider_bwd_inputs(nn_idx, feat, g, dy, feat_scale, feat_shift, what):
+    nn_idx = _dev(nn_idx, torch.int32, "nn_idx", 3)
+    feat = _dev(feat, torch.float32, "feat", 3)
+    g = _dev(g, torch.float32, "g", 4)
+    dy = _dev(dy, torch.float32, "dy", 3)
+    b, n, c = feat.shape
+    k = nn_idx.shape[2]
+    if tuple(nn_idx.shape[:2]) != (b, n) or tuple(g.shape[:3]) != (b, n, k) or tuple(dy.shape[:2]) != (b, n):
+        raise ValueError(f"{what}: nn_idx {tuple(nn_idx.shape)} / g {tuple(g.shape)} / dy {tuple(dy.shape)} do not match feat {tuple(feat.shape)}")
+    if (feat_scale is None) != (feat_shift is None):
+        raise ValueError(f"{what}: feat_scale and feat_shift go together")
+    if feat_scale is not None:
+        feat_scale = _dev(feat_scale, torch.float32, "feat_scale", 2)
+        feat_shift = _dev(feat_shift, torch.float32, "feat_shift", 2)
+        if tuple(feat_scale.shape) != (b, c) or tuple(feat_shift.shape) != (b, c):
+            raise ValueError(f"{what}: feat_scale / feat_shift must be ({b}, {c})")
+    return nn_idx, feat, g, dy, feat_scale, feat_shift
+
+
+def spider_conv_bwd_weight(nn_idx, feat, g, dy, feat_scale=None, feat_shift=None) -> torch.Tensor:
+    """The gradient of spider_conv's weights: nn_idx (B,N,k), feat (B,N,C), g (B,N,k,T) (spider_taylor_filter), dy (B,N,C_out) the
+    gradient of y -> dW (k, C*T, C_out), the reference's row order (j, c, t)."""
+    nn_idx, feat, g, dy, feat_scale, feat_shift = _spider_bwd_inputs(nn_idx, feat, g, dy, feat_scale, feat_shift, "spider_conv_bwd_weight")
+    b, n, c = feat.shape
+    k, t, c_out = nn_idx.shape[2], g.shape[3], dy.shape[2]
+    dW = torch.empty((k, c * t, c_out), dtype=torch.float32, device=feat.device)
+    ws, nbytes = _spider_ws(b, n, c, k, t, c_out, feat.device)
+    check(_lib.load().psa_spider_conv_bwd_weight(b, n, c, k, t, c_out, _ptr(nn_idx), _ptr(feat), _ptr(feat_scale), _ptr(feat_shift), _ptr(g),
+                                                 _ptr(dy), _ptr(dW), _ptr(ws), nbytes, _stream()), "spider_conv_bwd_weight")
+    return dW
+
+
+def spider_conv_bwd_data(nn_idx, feat, g, weights, dy, feat_scale=None, feat_shift=None, want_D: bool = True):
+    """The data side of spider_conv's backward -> (D (B,N,k,C) or None, dg (B,N,k,T)): D[p,j,c] = sum_t g Q, dg[p,j,t] = sum_c h Q with
+    Q[p,j,c,t] = sum_o dy[p,o] W[j,c*T+t,o].  group_point_grad(D, nn_idx) is the gradient of the layer's input activation."""
+    nn_idx, feat, g, dy, feat_scale, feat_shift = _spider_bwd_inputs(nn_idx, feat, g, dy, feat_scale, feat_shift, "spider_conv_bwd_data")
+    weights = _dev(weights, torch.float32, "weights")
+    b, n, c = feat.shape
+    k, t, c_out = nn_idx.shape[2], g.shape[3], dy.shape[2]
+    if weights.numel() != k * c * t * c_out or weights.shape[-1] != c_out:
+        raise ValueError(f"spider_conv_bwd_data: weights {tuple(weights.shape)} do not match k={k} C={c} T={t} C_out={c_out}")
+    D = torch.empty((b, n, k, c), dtype=torch.float32, device=feat.device) if want_D else None
+    dg = torch.empty((b, n, k, t), dtype=torch.float32, device=feat.device)
+    check(_lib.load().psa_spider_conv_bwd_data(b, n, c, k, t, c_out, _ptr(nn_idx), _ptr(feat), _ptr(feat_scale), _ptr(feat_shift), _ptr(g),
+                                               _ptr(weights), _ptr(dy), _ptr(D), _ptr(dg), _stream()), "spider_conv_bwd_data")
+    return D, dg
+
+
+def spider_taylor_grad(delta, dg) -> torch.Tensor:
+    """The gradient of the (20,T) Taylor coefficients: delta (B,N,k,3), dg (B,N,k,T) -> (20,T), sums in fp64."""
+    delta = _dev(delta, torch.float32, "delta", 4)
+    dg = _dev(dg, torch.float32, "dg", 4)
+    b, n, k, _ = delta.shape
+    if delta.shape[3] != 3 or tuple(dg.shape[:3]) != (b, n, k):
+        raise ValueError(f"spider_taylor_grad: delta {tuple(delta.shape)} / dg {tuple(dg.shape)} do not match")
+    t = dg.shape[3]
+    out = torch.empty((20, t), dtype=torch.float32, device=dg.device)
+    ws, nbytes = _spider_ws(b, n, 1, k, t, 1, dg.device)
+    check(_lib.load().psa_spider_taylor_grad(b, n, k, t, _ptr(delta), _ptr(dg), _ptr(out), t, _ptr(ws), nbytes, _stream()), "spider_taylor_grad")
+    return out
+
+
+def spider_gn_bwd(y, scale, shift, gamma, groups: int, dpool, offset: int = 0, dh_next=None, eps: float = 1e-6):
+    """Backward of topk_pool(relu(group_norm(y))) plus a gradient dh_next (B,N,C) of the activation itself: y (B,N,C), scale / shift (B,C)
+    (group_norm_affine), dpool (B,C_total,2) the pooled gradient whose channels [offset, offset + C) are this layer's ->
+    (dy (B,N,C), dgamma (C), dbeta (C))."""
+    y = _dev(y, torch.float32, "y", 3)
+    scale = _dev(scale, torch.float32, "scale", 2)
+    shift = _dev(shift, torch.float32, "shift", 2)
+    gamma = _dev(gamma, torch.float32, "gamma", 1)
+    dpool = _dev(dpool, torch.float32, "dpool", 3)
+    b, n, c = y.shape
+    if tuple(scale.shape) != (b, c) or tuple(shift.shape) != (b, c) or gamma.numel() != c:
+        raise ValueError(f"spider_gn_bwd: scale / shift must be ({b}, {c}) and gamma ({c})")
+    if dpool.shape[0] != b or dpool.shape[2] != 2 or not 0 <= offset <= dpool.shape[1] - c:
+        raise ValueError(f"spider_gn_bwd: dpool {tuple(dpool.shape)} does not hold {c} channels at offset {offset}")
+    if groups < 1 or c % groups:
+        raise ValueError(f"spider_gn_bwd: {groups} groups do not divide {c} channels")
+    if dh_next is not None:
+        dh_next = _dev(dh_next, torch.float32, "dh_next", 3)
+        if tuple(dh_next.shape) != (b, n, c):
+            raise ValueError(f"spider_gn_bwd: dh_next must be ({b}, {n}, {c})")
+    dy = torch.empty_like(y)
+    dgamma = torch.empty(c, dtype=torch.float32, device=y.device)
+    dbeta = torch.empty(c, dtype=torch.float32, device=y.device)
+    ws = torch.empty(max(b * 2 * c * 2, 1), dtype=torch.float32, device=y.device)
+    check(_lib.load().psa_spider_gn_bwd(b, n, c, groups, C.c_float(eps), _ptr(y), _ptr(scale), _ptr(shift), _ptr(gamma), _ptr(dpool),
+                                        dpool.shape[1], offset, _ptr(dh_next), _ptr(dy), _ptr(dgamma), _ptr(dbeta), _ptr(ws),
+                                        C.c_size_t(ws.numel() * 4), _stream()), "spider_gn_bwd")
+    return dy, dgamma, dbeta
+
+
 # ------------------------------------------------------------------------------------------------
 # 3DmFV-Net
 # ------------------------------------------------------------------------------------------------
