@@ -635,6 +635,50 @@ PSA_API int psa_conv3d_infer(int b, int r, int k, int c, int c_out, const float*
 PSA_API int psa_pool3d(int b, int r, int c, int kind, const float* x, float* out, psa_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * 3DmFV-Net, training (3DmFV-Net/train.py:163-173: the Fisher vector takes fed placeholders, so the backward stops at the
+ * grid).  fp32 FMA in every arithmetic mode, no float atomics: every sum runs in a fixed order and a step is bit-reproducible.
+ * Notation of psa_conv3d_infer; K = k^3 * c; dy (b*r^3, c_out) contiguous = the gradient of a conv's pre-batch-norm output.
+ * Neither product forms the (b*r^3, K) im2col operand, and both skip every 16-wide contraction block for which each kernel tap
+ * it touches lies outside the grid for all the rows it touches.
+ * ------------------------------------------------------------------------------------------- */
+
+/* Scratch of psa_conv3d_bwd_weight and psa_conv3d_bwd_data (split-contraction partials), 256-byte aligned; 0 for bad dims. */
+PSA_API size_t psa_conv3d_bwd_workspace_bytes(int b, int r, int k, int c, int c_out);
+
+/* dW (K, c_out) = A^T . dy, A[row][(tap, ch)] = x[neighbour(row, tap)][ch] or 0 outside the grid: the gradient of the TF kernel
+ * (k,k,k,c,c_out) in its own layout.  Split over the rows, partials added in split order.  x rows of stride ldx. */
+PSA_API int psa_conv3d_bwd_weight(int b, int r, int k, int c, int c_out, const float* x, long long ldx, const float* dy, float* dW,
+                                  void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* dx[u][ch] (+)= sum_tap sum_o dy[u - offset(tap)][o] * W[tap][ch][o] (terms outside the grid are 0): the gradient of the conv's
+ * input, written at row stride ld_dx; accumulate != 0 adds it to what dx holds.  Split over the taps, partials added in split
+ * order. */
+PSA_API int psa_conv3d_bwd_data(int b, int r, int k, int c, int c_out, const float* dy, const float* W, float* dx, long long ld_dx,
+                                int accumulate, void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* The multiply-adds the two products issue at these dims (their tiles and skip rule, no GPU needed) and the multiply-adds whose
+ * tap lies inside the grid: issued_weight, issued_data, in_grid (each may be NULL). */
+PSA_API int psa_conv3d_bwd_macs(int b, int r, int k, int c, int c_out, long long* issued_weight, long long* issued_data,
+                                long long* in_grid);
+
+/* out[row * ldo + ch] = relu(y[row][ch] * scale[ch] + shift[ch]) (one fmaf, the gate psa_grad_in tests): y (rows, C). */
+PSA_API int psa_mfv_bn_relu(long long rows, int C, const float* y, const float* scale, const float* shift, float* out, long long ldo,
+                            psa_stream_t stream);
+
+/* dy (rows, C) = the psa_grad_in g evaluated at every element (mode 0), materialised for the conv3d products' gathers. */
+PSA_API int psa_mfv_bn_dy(long long rows, int C, const psa_grad_in* g, float* dy, psa_stream_t stream);
+
+/* psa_pool3d's SAME 2^3 stride-2 max that also records its winner: winner[v][ch] = the first maximum in window order
+ * (dz, dy, dx) as dz * 4 + dy * 2 + dx; cells of the far-end padding never win.  out, winner (b*ceil(r/2)^3, c). */
+PSA_API int psa_pool3d_max_train(int b, int r, int c, const float* x, float* out, unsigned char* winner, psa_stream_t stream);
+
+/* Backward of psa_pool3d: dout (b*ro^3, c) -> dx (b*r^3, c), every element written.  kind 0 (3^3 average): dx[u] = sum over the
+ * windows v holding u, in (dz, dy, dx) order, of dout[v] / count(v).  kind 1 (2^3 max): dx[u] = dout[v] where u is v's recorded
+ * winner, else 0. */
+PSA_API int psa_pool3d_bwd(int b, int r, int c, int kind, const float* dout, const unsigned char* winner, float* dx,
+                           psa_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------
  * PointCNN, inference mode (PointCNN/pointcnn.py:10-52 xconv, pointfly.py:122-128, 163-176 knn_indices_general,
  * :298-347 dense / conv2d / depthwise_conv2d / separable_conv2d).  Every layer with batch norm has no bias and applies
  * ELU before the batch norm: a = elu(x . W) * s + t, s = gamma / sqrt(moving_variance + 1e-3), t = beta - moving_mean * s.

@@ -124,6 +124,14 @@ SIGNATURES = {
     "psa_fisher_vector": [_i, _i, _i, _p, _p, _p, _p, _p, _p],
     "psa_conv3d_infer": [_i, _i, _i, _i, _i, _p, _ll, _p, _p, _p, _i, _p, _ll, _p, _sz, _p],
     "psa_pool3d": [_i, _i, _i, _i, _p, _p, _p],
+    # 3DmFV-Net (training)
+    "psa_conv3d_bwd_weight": [_i, _i, _i, _i, _i, _p, _ll, _p, _p, _p, _sz, _p],
+    "psa_conv3d_bwd_data": [_i, _i, _i, _i, _i, _p, _p, _p, _ll, _i, _p, _sz, _p],
+    "psa_conv3d_bwd_macs": [_i, _i, _i, _i, _i, _p, _p, _p],
+    "psa_mfv_bn_relu": [_ll, _i, _p, _p, _p, _p, _ll, _p],
+    "psa_mfv_bn_dy": [_ll, _i, _gin, _p, _p],
+    "psa_pool3d_max_train": [_i, _i, _i, _p, _p, _p, _p],
+    "psa_pool3d_bwd": [_i, _i, _i, _i, _p, _p, _p, _p],
     # PointCNN (inference)
     "psa_knn_dilated": [_i, _i, _i, _i, _i, _p, _p, _p, _p],
     "psa_xconv_core": [_i, _i, _i, _p, _p, _p, _p, C.POINTER(PsaXconv), _p, _p],
@@ -137,7 +145,8 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_train_dense_workspace_bytes", "psa_bn_bwd_workspace_bytes", "psa_sa_conv1_bwd_workspace_bytes", "psa_knn_graph_workspace_bytes",
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
                 "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes", "psa_spider_conv_workspace_bytes",
-                "psa_spider_conv_bwd_workspace_bytes", "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes")
+                "psa_spider_conv_bwd_workspace_bytes", "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes",
+                "psa_conv3d_bwd_workspace_bytes")
 
 _lib = None
 
@@ -189,6 +198,8 @@ def load() -> C.CDLL:
     lib.psa_conv3d_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
     lib.psa_conv3d_workspace_bytes.restype = C.c_size_t
     lib.psa_dense_elu_affine_workspace_bytes.argtypes = [_ll, _i, _i]
+    lib.psa_conv3d_bwd_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
+    lib.psa_conv3d_bwd_workspace_bytes.restype = C.c_size_t
     lib.psa_dense_elu_affine_workspace_bytes.restype = C.c_size_t
     lib.psa_version.restype = C.c_int
     lib.psa_sm_arch.restype = C.c_int

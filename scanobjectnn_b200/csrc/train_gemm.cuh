@@ -134,6 +134,15 @@ struct MatIn {
 constexpr int kGemmThreads = 256;
 constexpr int kGemmBK = 16;
 
+// Optional contraction skipping: an A functor that declares `static constexpr bool kSkipK = true` provides
+//   long long next_k(long long k, long long k_end, long long m0, int bm)
+// = the first contraction block start >= k (k is one; the result is k plus a multiple of kGemmBK, or k_end) whose block can hold a
+// non-zero product for the tile's rows [m0, m0 + bm).  Every other functor runs every block, as before.
+template <class F, class = void>
+struct GemmSkipK { static constexpr bool value = false; };
+template <class F>
+struct GemmSkipK<F, decltype((void)F::kSkipK)> { static constexpr bool value = F::kSkipK; };
+
 struct GemmOut {
     float* out;            // (M, ld_out) -- or split-K partials (splits, M, N) when splits > 1
     long long ld_out;
@@ -250,14 +259,22 @@ train_gemm_kernel(const FA fa, const FB fb, const GemmOut o, long long M, int N,
 #pragma unroll
         for (int j = 0; j < TN / 2; ++j) acc[i][j] = make_float2(0.f, 0.f);
 
-    if (k_begin < k_end) {
-        fetch(k_begin);
+    long long k_first = k_begin;
+    if constexpr (GemmSkipK<FA>::value) {
+        if (k_begin < k_end) k_first = fa.next_k(k_begin, k_end, m0, BM);
+    }
+    if (k_first < k_end) {
+        fetch(k_first);
         stash(0);
         __syncthreads();
         int buf = 0;
-        for (long long k0 = k_begin; k0 < k_end; k0 += kGemmBK) {
-            const bool more = k0 + kGemmBK < k_end;
-            if (more) fetch(k0 + kGemmBK);
+        for (long long k0 = k_first, kn; k0 < k_end; k0 = kn) {
+            kn = k0 + kGemmBK;
+            if constexpr (GemmSkipK<FA>::value) {
+                if (kn < k_end) kn = fa.next_k(kn, k_end, m0, BM);
+            }
+            const bool more = kn < k_end;
+            if (more) fetch(kn);
 #pragma unroll
             for (int kk = 0; kk < kGemmBK; ++kk) {
                 float a[TM];

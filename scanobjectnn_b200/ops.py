@@ -23,7 +23,7 @@ __all__ = [
     "get_edge_feature", "farthest_point_sample_and_gather", "MlpParams", "shared_mlp", "shared_mlp_grouped", "sa_module_infer",
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
     "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d", "knn_dilated", "xconv_core",
-    "dense_elu_affine",
+    "dense_elu_affine", "conv3d_bwd_weight", "conv3d_bwd_data", "conv3d_bwd_macs", "pool3d_max_train", "pool3d_bwd",
 ]
 
 
@@ -876,6 +876,98 @@ def conv3d(x, r: int, weights, scale, shift, relu: bool = True, out=None, offset
     check(lib.psa_conv3d_infer(b, r, k, c, c_out, _ptr(x), x.stride(0), _ptr(weights), _ptr(scale), _ptr(shift), 1 if relu else 0,
                                _ptr(view), out.stride(0), _ptr(ws), C.c_size_t(need), _stream()), "conv3d")
     return out
+
+
+def _conv3d_bwd_ws(b, r, k, c, c_out, device) -> tuple[torch.Tensor, C.c_size_t]:
+    need = int(_lib.load().psa_conv3d_bwd_workspace_bytes(b, r, k, c, c_out))
+    return torch.empty((need + 3) // 4 + 64, dtype=torch.float32, device=device), C.c_size_t(need)
+
+
+def _conv3d_k(kk: int) -> int:
+    k = {1: 1, 27: 3, 125: 5}.get(kk)
+    if k is None:
+        raise ValueError(f"conv3d: {kk} taps, expected k^3 with k in (1, 3, 5)")
+    return k
+
+
+def conv3d_bwd_weight(x, r: int, dy, k: int) -> torch.Tensor:
+    """The gradient of conv3d's weights (psa_conv3d_bwd_weight, fp32): x (B*r^3, C) voxel-major rows (a column slice is read in
+    place), dy (B*r^3, C_out) the gradient of the conv's pre-batch-norm output -> dW (k,k,k,C,C_out), TF's kernel layout."""
+    if not (isinstance(x, torch.Tensor) and x.is_cuda and x.dtype == torch.float32 and x.dim() == 2 and x.stride(1) == 1):
+        x = _dev(x, torch.float32, "x", 2)
+    dy = _dev(dy, torch.float32, "dy", 2)
+    rows, c = x.shape
+    if rows % r ** 3 or dy.shape[0] != rows:
+        raise ValueError(f"conv3d_bwd_weight: x has {rows} rows, dy {dy.shape[0]}; both must be B*r^3 with r = {r}")
+    b, c_out = rows // r ** 3, dy.shape[1]
+    dW = torch.empty((k, k, k, c, c_out), dtype=torch.float32, device=x.device)
+    ws, wsn = _conv3d_bwd_ws(b, r, k, c, c_out, x.device)
+    check(_lib.load().psa_conv3d_bwd_weight(b, r, k, c, c_out, _ptr(x), x.stride(0), _ptr(dy), _ptr(dW), _ptr(ws), wsn, _stream()),
+          "conv3d_bwd_weight")
+    return dW
+
+
+def conv3d_bwd_data(dy, r: int, weights, out=None, accumulate: bool = False) -> torch.Tensor:
+    """The gradient of conv3d's input (psa_conv3d_bwd_data, fp32): dy (B*r^3, C_out), weights (k,k,k,C,C_out) -> dx (B*r^3, C).
+    out (B*r^3, >= C), possibly a column slice of a wider buffer: written in place, or added to with accumulate=True."""
+    dy = _dev(dy, torch.float32, "dy", 2)
+    weights = _dev(weights, torch.float32, "weights")
+    rows, c_out = dy.shape
+    c = weights.shape[-2] if weights.dim() == 5 else None
+    if c is None or weights.shape[-1] != c_out or rows % r ** 3:
+        raise ValueError(f"conv3d_bwd_data: weights {tuple(weights.shape)} are not (k,k,k,C,{c_out}), or {rows} rows are not B*r^3")
+    k = _conv3d_k(weights.numel() // (c * c_out))
+    if out is None:
+        out = torch.empty((rows, c), dtype=torch.float32, device=dy.device)
+    elif not (out.is_cuda and out.dtype == torch.float32 and out.dim() == 2 and out.shape[0] == rows and out.shape[1] >= c and out.stride(1) == 1):
+        raise ValueError(f"conv3d_bwd_data: out must be a float32 CUDA tensor ({rows}, >= {c}) with unit column stride")
+    b = rows // r ** 3
+    ws, wsn = _conv3d_bwd_ws(b, r, k, c, c_out, dy.device)
+    check(_lib.load().psa_conv3d_bwd_data(b, r, k, c, c_out, _ptr(dy), _ptr(weights), _ptr(out), out.stride(0), 1 if accumulate else 0,
+                                          _ptr(ws), wsn, _stream()), "conv3d_bwd_data")
+    return out
+
+
+def conv3d_bwd_macs(b: int, r: int, k: int, c: int, c_out: int) -> tuple[int, int, int]:
+    """(multiply-adds issued by the weight gradient, by the data gradient, multiply-adds with the tap inside the grid) at these dims"""
+    v = [C.c_longlong(0) for _ in range(3)]
+    check(_lib.load().psa_conv3d_bwd_macs(b, r, k, c, c_out, *(C.byref(t) for t in v)), "conv3d_bwd_macs")
+    return tuple(int(t.value) for t in v)
+
+
+def pool3d_max_train(x, r: int) -> tuple[torch.Tensor, torch.Tensor]:
+    """pool3d(x, r, 'max') and its winners (psa_pool3d_max_train): -> (out, winner) (B*ceil(r/2)^3, C), winner uint8 = the first
+    maximum's window position dz * 4 + dy * 2 + dx."""
+    x = _dev(x, torch.float32, "x", 2)
+    rows, c = x.shape
+    if rows % r ** 3:
+        raise ValueError(f"pool3d_max_train: {rows} rows are not a multiple of r^3 = {r ** 3}")
+    b, ro = rows // r ** 3, (r + 1) // 2
+    out = torch.empty((b * ro ** 3, c), dtype=torch.float32, device=x.device)
+    win = torch.empty((b * ro ** 3, c), dtype=torch.uint8, device=x.device)
+    check(_lib.load().psa_pool3d_max_train(b, r, c, _ptr(x), _ptr(out), _ptr(win), _stream()), "pool3d_max_train")
+    return out, win
+
+
+def pool3d_bwd(dout, r: int, kind: str, winner=None) -> torch.Tensor:
+    """The backward of pool3d on an r^3 grid (psa_pool3d_bwd): 'avg' -> dx (B*r^3, C) from dout (B*r^3, C); 'max' -> dx from dout
+    (B*ceil(r/2)^3, C) and pool3d_max_train's winners."""
+    dout = _dev(dout, torch.float32, "dout", 2)
+    if kind not in ("avg", "max"):
+        raise ValueError(f"pool3d_bwd: kind must be 'avg' or 'max', got {kind!r}")
+    ro = r if kind == "avg" else (r + 1) // 2
+    rows, c = dout.shape
+    if rows % ro ** 3:
+        raise ValueError(f"pool3d_bwd: {rows} rows are not a multiple of {ro ** 3}")
+    if kind == "max":
+        if winner is None or winner.dtype != torch.uint8 or tuple(winner.shape) != tuple(dout.shape):
+            raise ValueError("pool3d_bwd: 'max' needs pool3d_max_train's uint8 winners of dout's shape")
+        winner = winner.contiguous()
+    b = rows // ro ** 3
+    dx = torch.empty((b * r ** 3, c), dtype=torch.float32, device=dout.device)
+    check(_lib.load().psa_pool3d_bwd(b, r, c, 0 if kind == "avg" else 1, _ptr(dout), _ptr(winner if kind == "max" else None), _ptr(dx),
+                                     _stream()), "pool3d_bwd")
+    return dx
 
 
 def pool3d(x, r: int, kind: str) -> torch.Tensor:
