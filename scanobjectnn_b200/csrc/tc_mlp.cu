@@ -12,8 +12,8 @@
 //             input features evaluate t + (x_j - c) . (s Wx) per row.
 //   layers 2+ wgmma, A from registers, B = weights in shared memory in the canonical K-major SWIZZLE_128B layout, dropped
 //             there by cp.async.bulk from pre-arranged images; D in registers, whose layout is that of the next A operand.
-//   max-pool  the last epilogue reduces each neighbourhood's rows in-thread, across the warp with shuffles and across warps in
-//             shared memory, and writes (B,m,C_out) coalesced.
+//   max-pool  the last epilogue reduces each neighbourhood's rows in-thread and across the warp with shuffles, folds them into
+//             a shared-memory row per neighbourhood with atomicMax, and writes (B,m,C_out) coalesced once per chunk.
 //
 // Kernels (both templated on NP, the pieces per operand -- Split<NP> in tc_common.cuh):
 //   tc_sa_kernel<NP,..>       SA level (specialised on its shape); optional centre weights = multi-layer EdgeConv over 3-D points
@@ -86,7 +86,6 @@ struct TcArgs {
     int Kd[kMaxTcLayers], Ntot[kMaxTcLayers];
     int stream_last;       // 1: the last layer's weights do not fit next to the others -> one 64-channel chunk at a time
     int joint;             // tc_sa_kernel: both warpgroups on one 128-row pass, every row computed (set by the launcher)
-    int pool_chunks;       // tc_sa_kernel: 64-channel chunks of the last layer pooled together (set by the launcher)
     unsigned int* tile_counter;   // zeroed before the launch: tiles are handed out dynamically (CTAs that start late or
                                   // share their SM with another stream's kernels simply take fewer)
     int np;                       // operand pieces: 2 (fp16x2) or 3 (bf16x3)
@@ -200,7 +199,8 @@ __global__ void tc_prep_weights_kernel(int K, int Kp, int N, int Nt, const float
 //   * inner tensor layers: wgmma with A from registers, B = weight image in shared memory; the D fragment goes through
 //     affine + ReLU + split and is the next layer's A fragment (same register layout), nothing is staged;
 //   * last layer in 64-channel chunks: wgmma, affine + ReLU, max over each neighbourhood's rows (in-thread, shuffles across
-//     the warp, shared memory across warps), coalesced (B,m,C_out) stores.
+//     the warp, shared atomicMax across warps and passes), coalesced (B,m,C_out) stores at the end of each chunk of
+//     neighbourhoods.
 //   Weights of every layer are resident in shared memory (one TMA bulk load per CTA); a last layer that does not fit next to
 //   the others is streamed one 64-channel chunk at a time through a two-slot ring, one chunk ahead.
 // ------------------------------------------------------------------------------------------------------------------
@@ -239,10 +239,21 @@ __host__ __device__ inline TcSaLayout tc_sa_layout(const TcArgs& a) {
 // end of the grid is balanced (PointNet++ SA2: 512 chunks for 264 units), enough neighbourhoods per chunk that its last pass
 // is mostly full
 __host__ __device__ inline int sa_chunk(int K, bool joint) { return (joint ? 128 : 512) / K; }
-// shared memory of the pooling carry (a warpgroup unit's running max of a neighbourhood that spans two passes), after the layout
-__host__ __device__ inline uint32_t sa_carry_bytes(const TcArgs& a) { return a.joint ? 0u : 2u * a.Ntot[a.nl - 1] * 4u; }
-// shared memory of the pooling buffer, after the carry: each warp's column maxima of `chunks` 64-channel chunks
-__host__ __device__ inline uint32_t sa_red_bytes(int chunks) { return 8u * 64u * 4u * (uint32_t)chunks; }
+// columns of a unit's pooling buffer: every column of the last layer, or the 64 of the ring slot being consumed when it streams
+__host__ __device__ inline int sa_pool_cols(const TcArgs& a) { return a.stream_last ? 64 : a.Ntot[a.nl - 1]; }
+// shared memory of the pooling buffers, after the layout: per unit, one row of sa_pool_cols words per neighbourhood of its chunk
+__host__ __device__ inline uint32_t sa_pool_bytes(const TcArgs& a) {
+    return (a.joint ? 1u : 2u) * (uint32_t)sa_chunk(a.K, a.joint) * (uint32_t)sa_pool_cols(a) * 4u;
+}
+// a float as an int that orders like it (shared atomicMax has no float form): the bits of a value >= +0, the magnitude bits
+// flipped below it.  The map is its own inverse; -inf maps to kSaPoolEmpty, below every finite value.
+__device__ __forceinline__ int sa_pool_code(float x) {
+    const int b = __float_as_int(x);
+    return b >= 0 ? b : b ^ 0x7fffffff;
+}
+__device__ __forceinline__ float sa_pool_value(int c) { return __int_as_float(c >= 0 ? c : c ^ 0x7fffffff); }
+__device__ __forceinline__ void red_smem_max(uint32_t addr, int v) { asm volatile("red.shared.max.s32 [%0], %1;\n" ::"r"(addr), "r"(v) : "memory"); }
+constexpr int kSaPoolEmpty = (int)0x807fffff;
 
 // thread 0: use q of the streamed last layer's ring = 64-channel chunk q % ncl into slot q & 1
 __device__ __forceinline__ void sa_fill_ring(uint32_t q, const uint8_t* image, int ncl, const TcSaLayout& L, uint8_t* base, uint64_t* bars) {
@@ -281,9 +292,10 @@ __device__ __forceinline__ void sa_mma(float (&d)[NCH][32], const uint32_t (&A)[
 #ifdef PSA_SA_STAMPS
 // Pass timeline (tools/sa_timing.py builds a separate library with -DPSA_SA_STAMPS; libpsa.so has none of this): lane 0 of the
 // first warp of each warpgroup of CTA i < kSaStampCtas writes clock64() at phase k of the unit's pass p < kSaStampPasses
-// (SaStamp below; chunk nc of the last layer at kSaChunk0 + 3 nc + {issued, retired, epilogue done}).  psa_sa_stamps_clear zeroes
-// the table, so that a slot a launch did not reach reads 0.
-enum SaStamp { kSaTop, kSaInputs, kSaLayer1, kSaL2Issued, kSaL2Retired, kSaL2Epi, kSaPool1, kSaPool2, kSaNextA, kSaNextB, kSaChunk0 };
+// (SaStamp below; chunk nc of the last layer at kSaChunk0 + 3 nc + {issued, retired, epilogue done}; the two barriers of the
+// store at the end of a chunk of neighbourhoods only in the passes that end one).  psa_sa_stamps_clear zeroes the table, so
+// that a slot a launch did not reach reads 0.
+enum SaStamp { kSaTop, kSaInputs, kSaLayer1, kSaL2Issued, kSaL2Retired, kSaL2Epi, kSaEnd1, kSaEnd2, kSaNextA, kSaNextB, kSaChunk0 };
 constexpr int kSaStampCtas = 264, kSaStampPasses = 64, kSaStampPhases = kSaChunk0 + 3 * 4;
 __device__ long long g_sa_stamps[kSaStampCtas][2][kSaStampPasses][kSaStampPhases];
 extern "C" PSA_API int psa_sa_stamps(long long* dst) {
@@ -330,14 +342,13 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     constexpr bool kDouble = !(C1 == 64 && (NL == 1 || N0 == 64));
     if (a.run_if != nullptr && *a.run_if == 0u) return;      // np = 3 rerun of a launch that stayed inside the fp16 range: nothing to do
     constexpr uint32_t bb = tc_block_bytes(kSaNt, NP);
-    uint32_t ovf = 0u;                                        // np = 2: packed |max| of every leading piece this thread stores ..
-    bool ovf_seen = false;                                    // .. folded in once per pass, so that `ovf` lives only in layers 1..L-1
+    uint32_t ovf = 0u;                                        // np = 2: packed |max| of every leading piece this thread stores,
+                                                              // checked once per pass so that it lives only in layers 1..L-1
     extern __shared__ uint8_t smem_raw[];
     __shared__ __align__(8) uint64_t s_rbar;                 // resident weights landed
     __shared__ __align__(8) uint64_t s_wbar[2];              // ring slot landed
-    __shared__ unsigned int s_claim[2];                      // [unit]: the chunk claimed after the current one
+    __shared__ unsigned int s_chunk[2][2];                   // [unit][table]: the chunk whose slot counts are in s_slots
     __shared__ int s_slots[2][2][16];                        // [unit][table]: 16-row slots of each neighbourhood of a chunk
-    __shared__ long long s_desc[2][2][8];                    // [unit][pass parity][warp]: pooling run that starts at the warp
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int g = lane >> 2, t = lane & 3;
@@ -367,6 +378,7 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
             (l == 0 ? sl0 : slL)[i] = (a.s[l] ? __ldg(a.s[l] + i) : 1.f) * (NP == 2 ? __ldg(a.colscale[l] + i) : 1.f);
             (l == 0 ? tl0 : tlL)[i] = __ldg(a.t[l] + i);
         }
+    for (uint32_t i = tid; i < sa_pool_bytes(a) / 4u; i += kSaThreads) reinterpret_cast<int*>(base + L.total)[i] = kSaPoolEmpty;
     if (tid == 0) {
         mbar_init(&s_rbar, 1); mbar_init(&s_wbar[0], 1); mbar_init(&s_wbar[1], 1);
         fence_mbar_init();
@@ -399,9 +411,11 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     //   A unit claims a chunk of C consecutive neighbourhoods at a time and computes it in passes of one 16-row slot per warp.
     // The ball query pads a neighbourhood by repeating its first index, and a max does not change when a row is repeated: a
     // neighbourhood whose entries from L on all equal idx[0] only needs its first L rows, ceil(L / 16) slots.  The slots of a
-    // chunk are packed back to back, so a neighbourhood may start in one pass and end in the next; its running max is carried
-    // in the unit's shared memory.  Warps past the chunk's last slot recompute that slot and store nothing.  Joint units keep
-    // every row: a chunk is then one 128-row pass, as before.
+    // chunk are packed back to back, so a neighbourhood may start in one pass and end in a later one.  Each warp folds its
+    // slot's column maxima into its neighbourhood's row of the unit's pooling buffer with atomicMax, whichever pass it is in;
+    // only the chunk's end synchronises the unit, to store the rows and reset them.  Warps past the chunk's last slot
+    // recompute that slot and fold it in again (a max is idempotent).  Joint units keep every row: a chunk is then one
+    // 128-row pass, as before.
     const int K = a.K;
     const bool joint = a.joint;
     const int W = joint ? 8 : 4;                             // warps of the unit = slots per pass
@@ -411,9 +425,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     const int ut = joint ? tid : tid & 127, uw0 = joint ? 0 : 4 * unit;   // thread index in the unit, first warp of the unit
     const int wl = warp - uw0;                                // warp index in the unit
     const unsigned nchunks = (unsigned)((a.groups + C - 1) / C);
-    float* carry = reinterpret_cast<float*>(base + L.total) + (size_t)unit * a.Ntot[last];   // warpgroup units: Ntot[last] floats
-    const int NG = a.pool_chunks, rs = 64 * NG;               // chunks pooled together, floats per warp row of `red`
-    float* red = reinterpret_cast<float*>(base + L.total + sa_carry_bytes(a)) + (size_t)warp * rs;   // this warp's row
+    const int PC = sa_pool_cols(a);
+    // the unit's pooling buffer [C][PC]: ordered codes (sa_pool_code), kSaPoolEmpty between chunks; an offset from `base`, so
+    // that no pointer of its own is held through the pass
+    const uint32_t pool = L.total + (uint32_t)(unit * C * PC) * 4u;
 
     // slot counts of chunk ch into table b, by the whole unit (read after a unit barrier).  L = 1 + the last j with
     // idx[j] != idx[0] (1 when all are equal), from a ballot per 32 entries; a warp covers 128 entries = 4 neighbourhoods of 32
@@ -449,8 +464,8 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
     // Layer 1's inputs for this thread's two rows are gathered one pass ahead (NL = 2), while the previous pass's last-layer
     // wgmma run: stage A (neighbour index, centre) once the first chunk is issued, stage B (the V row, or the neighbour
     // coordinates of a level without input features) once the last one is.  The next pass's slot table must be filled by
-    // then; it is not when the next pass opens a chunk claimed in this very pass (the table is filled between the pooling
-    // barriers), and both stages then follow the first pooling.
+    // then; it is not when the next pass opens a new chunk (its table is filled at the end of the current one), and both
+    // stages then follow that chunk-end store.
     // The 64-float V rows of C1 = 128 levels are held in registers (fp16x2: those levels keep one CTA per SM); other levels
     // load them in layer 1, as do the levels that gather at the top of the pass (nothing to hide the loads behind there).
     constexpr bool kAhead = NL == 2;                          // one-tensor-layer levels (EdgeConv) gather at the top of the pass:
@@ -461,12 +476,16 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                                                               // 0..i); the chunk's total is lane C - 1's, one shuffle away
     int jn[2];
     long long gn = 0;                                         // the neighbourhood of this warp's slot
-    bool carry_next = false;                                  // warp 0: the gathered pass continues a run of the pass before
     float cx = 0.f, cy = 0.f, cz = 0.f, px[2], py[2], pz[2];
     const float* urow[2];
-    float2 uh[2][kUH];
-    // stage A of pass p of chunk ch (slot table b); lane 0 records the warp's pooling run in s_desc[unit][d]
-    auto gather_a = [&](unsigned ch, int b, int p, int d) {
+    float2 uh[2][kUH];                                        // kHoldU: the V row, or the neighbour's coordinates of a level
+                                                              // without input features (not px .. pz: six registers SA2 lacks)
+    // the chunk's slot total, and the neighbourhood (index in the chunk) of this warp's slot in pass p, both from the prefix.
+    // Warps past the chunk's last slot take that slot's.
+    auto slot_total = [&]() { return __shfl_sync(0xffffffffu, incl, C - 1); };
+    auto slot_nb = [&](int p) { return __popc(__ballot_sync(0xffffffffu, incl <= min(p * W + wl, slot_total() - 1)) & ((1u << C) - 1u)); };
+    // stage A of pass p of chunk ch (slot table b)
+    auto gather_a = [&](unsigned ch, int b, int p) {
         if (p == 0) {                                         // a new chunk: prefix of its slot table
             incl = lane < C ? s_slots[unit][b][lane] : 0;
 #pragma unroll
@@ -475,26 +494,14 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                 if (lane >= o) incl += y;
             }
         }
-        const int T = __shfl_sync(0xffffffffu, incl, C - 1);
-        const int s = p * W + wl, ss = min(s, T - 1);
-        const int nb = __popc(__ballot_sync(0xffffffffu, incl <= ss) & ((1u << C) - 1u));
-        const int end = __shfl_sync(0xffffffffu, incl, nb), start = nb ? __shfl_sync(0xffffffffu, incl, nb - 1) : 0;
+        const int ss = min(p * W + wl, slot_total() - 1), nb = slot_nb(p);
+        const int start = nb ? __shfl_sync(0xffffffffu, incl, nb - 1) : 0;
         gn = (long long)ch * C + nb;
         const int row = 16 * (ss - start) + g;
 #pragma unroll
         for (int i = 0; i < 2; ++i) jn[i] = __ldg(a.idx + gn * K + row + 8 * i);
         const float* c = a.new_xyz + (size_t)gn * 3;
         cx = __ldg(c); cy = __ldg(c + 1); cz = __ldg(c + 2);
-        carry_next = wl == 0 && s < T && s > start;
-        if (lane == 0) {
-            // a run = the warps of one neighbourhood in this pass: [len, carried in from the last pass, carried out to the next]
-            long long run = 0;
-            if (s < T && (wl == 0 || s == start)) {
-                const int pe = (p + 1) * W;
-                run = gn << 8 | (long long)(min(end, pe) - s) | (s > start ? 16 : 0) | (end > pe ? 32 : 0);
-            }
-            s_desc[unit][d][wl] = run;
-        }
     };
     auto gather_b = [&]() {
         const long long bi = gn / a.m;
@@ -502,7 +509,8 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         for (int i = 0; i < 2; ++i) {
             if (a.uf == nullptr) {                            // with input features the neighbour's coordinates are in V
                 const float* p = a.xyz + ((size_t)bi * a.n + jn[i]) * 3;
-                px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2);
+                if constexpr (kHoldU) { uh[i][0] = make_float2(__ldg(p), __ldg(p + 1)); uh[i][1].x = __ldg(p + 2); }
+                else { px[i] = __ldg(p); py[i] = __ldg(p + 1); pz[i] = __ldg(p + 2); }
             }
             urow[i] = a.uf ? a.uf + ((size_t)bi * a.n + jn[i]) * C1 : nullptr;
             if constexpr (kHoldU) {
@@ -514,22 +522,22 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
         }
     };
 
-    // The chunk after the current one is claimed at the top of the current one's first pass, read after the first pooling
-    // barrier of that pass and its slot table filled before the second; the barriers order the read before the next claim
-    // and the table before the gather that reads it.
-    if (ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
+    // The chunk after the current one is claimed at the top of the current one's first pass into the other table, read after
+    // the first barrier of the current one's end and its slot counts filled before the second; the barriers order the read
+    // before the next claim and the table before the gather that reads it.  The current chunk is read from its table where
+    // it is needed rather than held in a register through the pass (a spilled word in SA1 and SA2).
+    if (ut == 0) s_chunk[unit][0] = atomicAdd(a.tile_counter, 1u);
     unit_bar_sync(ubar, uthreads);
-    unsigned ch = s_claim[unit], claimed = 0;
-    if (ch < nchunks) fill_table(ch, 0);
+    if (s_chunk[unit][0] < nchunks) fill_table(s_chunk[unit][0], 0);
     unit_bar_sync(ubar, uthreads);
-    int buf = 0, p = 0;                                       // slot table and pass index of the current chunk
-    if (kAhead && ch < nchunks) { gather_a(ch, 0, 0, 0); gather_b(); }
+    int buf = 0, p = 0;                                       // table and pass index of the current chunk
+    if (kAhead && s_chunk[unit][0] < nchunks) { gather_a(s_chunk[unit][0], 0, 0); gather_b(); }
     uint32_t it = 0;                                          // passes of this unit
-    for (; ch < nchunks; ++it) {
-        if (p == 0 && ut == 0) s_claim[unit] = atomicAdd(a.tile_counter, 1u);
+    for (; s_chunk[unit][buf] < nchunks; ++it) {
+        if (p == 0 && ut == 0) s_chunk[unit][buf ^ 1] = atomicAdd(a.tile_counter, 1u);
         SA_STAMP(it, kSaTop);
-        if (!kAhead) { gather_a(ch, buf, p, it & 1); gather_b(); }
-        SA_STAMP_AFTER(it, kSaInputs, a.uf == nullptr ? px[0] : kHoldU ? uh[0][0].x : __ldg(urow[0] + 2 * t));
+        if (!kAhead) { gather_a(s_chunk[unit][buf], buf, p); gather_b(); }
+        SA_STAMP_AFTER(it, kSaInputs, kHoldU ? uh[0][0].x : a.uf == nullptr ? px[0] : __ldg(urow[0] + 2 * t));
 
         // ---- layer 1 on the FMA pipe, straight into the A fragments (K = C1) ----
         uint32_t A[NP][8][4];
@@ -558,7 +566,10 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
             // t + (x_j - c) . w1x (+ c . w1c)
             float dx[2], dy[2], dz[2];
 #pragma unroll
-            for (int i = 0; i < 2; ++i) { dx[i] = px[i] - cx; dy[i] = py[i] - cy; dz[i] = pz[i] - cz; }
+            for (int i = 0; i < 2; ++i) {
+                if constexpr (kHoldU) { dx[i] = uh[i][0].x - cx; dy[i] = uh[i][0].y - cy; dz[i] = uh[i][1].x - cz; }
+                else { dx[i] = px[i] - cx; dy[i] = py[i] - cy; dz[i] = pz[i] - cz; }
+            }
 #pragma unroll
             for (int s = 0; s < C1 / 16; ++s) {
 #pragma unroll
@@ -613,18 +624,20 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
             }
             SA_STAMP(it, kSaL2Epi);
         }
-        if constexpr (NP == 2) { ovf_seen = ovf_seen || f16x2_overflowed(ovf); ovf = 0u; }   // every leading piece is stored
+        if constexpr (NP == 2) {                              // every leading piece is stored; the flag is raised at once, so
+            if (f16x2_overflowed(ovf)) atomicOr(a.ovf, 1u);   // that no predicate is held through the rest of the pass
+            ovf = 0u;
+        }
         {
-            // ---- last layer, 64 output channels at a time, max-pooled over each neighbourhood once per NG chunks ----
+            // ---- last layer, 64 output channels at a time, max-pooled over each neighbourhood in the unit's pooling buffer ----
             // kDouble: chunk nc + 1's group is issued before chunk nc's epilogue and runs during it (wait_group 1)
             const int N = a.Ntot[last];
-            const bool carry_in = carry_next;                 // warp 0 folds the carried run max into its pooled maxima
-            // the next pass continues this chunk, or opens `claimed`
-            const bool same = (p + 1) * W < __shfl_sync(0xffffffffu, incl, C - 1);
-            // gather the next pass in the shadow of this one's last layer: its slot table is ready unless the chunk was claimed
-            // in this pass, and then the gather follows the first pooling
-            const bool ahead = kAhead && (same || (p > 0 && claimed < nchunks));
-            const bool after_pool = kAhead && !same && p == 0;
+            const int NG = a.stream_last ? 1 : NCL;           // 64-channel chunks per store: a streamed layer's ring slot holds one
+            // the next pass continues this chunk, or opens the one in the other table (a joint chunk is one pass: never `same`)
+            const bool same = (p + 1) * W < slot_total();
+            // gather the next pass of this chunk in the shadow of this one's last layer; the first pass of a chunk gathers after
+            // the store that ends the chunk before, which fills its slot table
+            const bool ahead = kAhead && same;
             auto issue = [&](float (&acc)[1][32], int nc) {
                 uint32_t wb;
                 if (a.stream_last) {                              // ring use q = chunk nc of pass it (every pass runs all NCL)
@@ -637,7 +650,9 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                 sa_mma_issue<NP, KSL, 1>(acc, A, wb, 0u);
                 SA_STAMP(it, kSaChunk0 + 3 * nc);
             };
-            // affine + ReLU of chunk nc, this warp's 16-row column maxima (and warp 0's carried run max) into its row of `red`
+            // affine + ReLU of chunk nc, this warp's 16-row column maxima folded into its neighbourhood's row.  Every warp folds,
+            // those past the chunk's last slot included (they repeat that slot), so that no branch sits inside the wgmma group
+            // in flight
             auto epilogue = [&](float (&acc)[1][32], int nc) {
                 wg_fence_acc(acc[0]);
                 SA_STAMP(it, kSaChunk0 + 3 * nc + 1);
@@ -659,61 +674,54 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                 }
                 colmax_halve<4>(v, (g >> 1) & 1);
                 colmax_halve<2>(v, g & 1);
-                float2 m = make_float2(v[0], v[1]);
-                const int x = 8 * g + 2 * t;
-                float* dst = red + (nc % NG) * 64 + x;
-                {   // written by the last pass; this pass writes it after a pooling barrier.  Every warp loads and selects, so
-                    // that no branch sits inside the wgmma group in flight; without a carry the load reads its own `red` words
-                    const float2 c = *reinterpret_cast<const float2*>(carry_in ? carry + nc * 64 + x : dst);
-                    m.x = carry_in ? fmaxf(m.x, c.x) : m.x;
-                    m.y = carry_in ? fmaxf(m.y, c.y) : m.y;
-                }
-                *reinterpret_cast<float2*>(dst) = m;
+                // this warp's columns 8g + 2t, + 1 of its neighbourhood's row (found again here rather than held through the pass)
+                const uint32_t dst = smem_u32(base + pool) + 4u * (uint32_t)(slot_nb(p) * PC + (a.stream_last ? 0 : nc * 64) + 8 * g + 2 * t);
+                red_smem_max(dst, sa_pool_code(v[0]));
+                red_smem_max(dst + 4u, sa_pool_code(v[1]));
                 SA_STAMP(it, kSaChunk0 + 3 * nc + 2);
             };
-            // chunks [gi NG, gi NG + NG) are in `red`: combine the run starting at each warp's slot, two columns per lane
-            auto pool = [&](int gi) {
-                unit_bar_sync(ubar, uthreads);                    // every warp's maxima are in red; ring slot consumed
-                SA_STAMP(it, kSaPool1);
-                if (gi == 0 && p == 0) {                          // the chunk claimed at the top of this pass
-                    claimed = s_claim[unit];
-                    if (claimed < nchunks) fill_table(claimed, buf ^ 1);
-                }
-                if (a.stream_last && tid == 0)                    // NG = 1: ring use gi of this pass is consumed
-                    sa_fill_ring(it * (uint32_t)NCL + (uint32_t)gi + 2u, a.image[last], NCL, L, base, s_wbar);
-                const long long run = s_desc[unit][it & 1][wl];
-                const int len = (int)(run & 15);
-                if (len != 0) {
-                    for (int c = 0; c < NG; ++c) {
-                        const float2* r = reinterpret_cast<const float2*>(red + c * 64) + lane;
-                        float2 mx = r[0];
-#pragma unroll
-                        for (int w = 1; w < 8; ++w)
-                            if (w < len) { const float2 v = r[w * rs / 2]; mx.x = fmaxf(mx.x, v.x); mx.y = fmaxf(mx.y, v.y); }
-                        const int col = (gi * NG + c) * 64 + 2 * lane;
-                        if (run & 32) *reinterpret_cast<float2*>(carry + col) = mx;
-                        else *reinterpret_cast<float2*>(a.out + (size_t)(run >> 8) * N + col) = mx;
+            // the end of a chunk of neighbourhoods (streamed: of its 64 channels from c0 on): the buffer's rows are stored for the
+            // neighbourhoods before a.groups (each of them has a slot, so its row holds a value) and reset, two columns per thread.
+            // The last store of the pass fills the next chunk's table and gathers its first pass; not an earlier one, whose
+            // gather would move the prefix that the pass's later epilogues find their rows with
+            auto store = [&](int c0) {
+                unit_bar_sync(ubar, uthreads);                    // every warp's atomics have landed; ring slot consumed
+                SA_STAMP(it, kSaEnd1);
+                const unsigned next = s_chunk[unit][buf ^ 1];     // claimed at the top of this chunk's first pass
+                const bool last_store = c0 + NG == NCL;
+                if (last_store && next < nchunks) fill_table(next, buf ^ 1);
+                if (a.stream_last && tid == 0)                    // ring use c0 of this pass is consumed
+                    sa_fill_ring(it * (uint32_t)NCL + (uint32_t)c0 + 2u, a.image[last], NCL, L, base, s_wbar);
+                const long long g0 = (long long)s_chunk[unit][buf] * C;
+                const int rows = (int)min((long long)C, a.groups - g0), half = PC / 2;
+                for (int e = ut; e < C * half; e += uthreads) {
+                    int2* const q = reinterpret_cast<int2*>(base + pool) + e;
+                    const int r = e / half, col = c0 * 64 + 2 * (e - r * half);
+                    if (r < rows) {
+                        const int2 c = *q;
+                        *reinterpret_cast<float2*>(a.out + (size_t)(g0 + r) * N + col) = make_float2(sa_pool_value(c.x), sa_pool_value(c.y));
                     }
+                    *q = make_int2(kSaPoolEmpty, kSaPoolEmpty);
                 }
-                unit_bar_sync(ubar, uthreads);                    // red is reused by the next group; the slot table is filled
-                SA_STAMP(it, kSaPool2);
-                if (gi == 0 && after_pool && claimed < nchunks) {
-                    gather_a(claimed, buf ^ 1, 0, (it + 1) & 1);
+                unit_bar_sync(ubar, uthreads);                    // the rows are reset; the next chunk's slot table is filled
+                SA_STAMP(it, kSaEnd2);
+                if (kAhead && last_store && next < nchunks) {
+                    gather_a(next, buf ^ 1, 0);
                     SA_STAMP(it, kSaNextA);
                     gather_b();
                     SA_STAMP(it, kSaNextB);
                 }
             };
-            // Every path below issues and waits in straight lines, and every group ends in wait_group 0 before pooling: ptxas
+            // Every path below issues and waits in straight lines, and every group ends in wait_group 0 before the store: ptxas
             // keeps the wgmma asynchronous only when it can see which group a wait retires on every path.  Stage B of the
             // gather is issued on every path that waits for the last chunk (NCL - 1), before that wait and after the epilogue
-            // of the chunk before it: whatever the group size, it follows stage A in every pass that gathers ahead.
+            // of the chunk before it, so it follows stage A in every pass that gathers ahead.
             float d0[1][32];
             for (int c0 = 0; c0 < NCL; c0 += NG) {
                 const int end = c0 + NG;
                 issue(d0, c0);
                 if (ahead && c0 == 0) {
-                    gather_a(same ? ch : claimed, same ? buf : buf ^ 1, same ? p + 1 : 0, (it + 1) & 1);
+                    gather_a(s_chunk[unit][buf], buf, p + 1);
                     SA_STAMP(it, kSaNextA);
                 }
                 if constexpr (kDouble) {
@@ -739,14 +747,13 @@ tc_sa_kernel(const __grid_constant__ TcArgs a) {
                         issue(d0, nc);
                     }
                 }
-                pool(c0 / NG);
+                if (!same) store(c0);
             }
-            if (!same) { ch = claimed; buf ^= 1; p = 0; }
+            if (!same) { buf ^= 1; p = 0; }
             else ++p;
         }
     }
     if constexpr (NP == 2) {
-        if (ovf_seen) atomicOr(a.ovf, 1u);
         if (tid == 0)
             for (int l = 0; l < NL; ++l)
                 if (a.wflag[l] != nullptr && *a.wflag[l] != 0u) atomicOr(a.ovf, 1u);
@@ -1202,23 +1209,20 @@ static int launch_tc_sa_shape(const TcArgs& a, long long ctas_needed, size_t sme
 template <int NP>
 static int launch_tc_sa_np(TcArgs& a, cudaStream_t st) {
     // chunks of one unit (see tc_sa_kernel): a unit is a warpgroup, or the whole CTA when K = 128 or the last layer streams.
-    // The pooling carry of warpgroup units and the pooling buffer sit after the layout, in the shared memory the SM has above
-    // the budget tc_sa_eligible checks (4 KB are left for the static arrays).  The buffer holds as many of the last layer's
-    // 64-channel chunks as fit (all of them for the PointNet++ levels: one pooling per pass); a streamed last layer pools each
-    // chunk before its ring slot is refilled.  A level whose carry and one-chunk buffer do not fit keeps joint units.
+    // The units' pooling buffers sit after the layout, in the shared memory the SM has above the budget tc_sa_eligible checks
+    // (4 KB are left for the static arrays).  A level whose warpgroup buffers do not fit keeps joint units, and one whose joint
+    // buffer does not fit next to a resident last layer streams that layer: its buffer then holds 64 columns (at most 1 KB),
+    // and its layout is no larger than the resident one (a last layer of 64 channels never gets here).
     const uint32_t limit = 223u * 1024u;
+    auto fits = [&] { return tc_sa_layout(a).total + 1024u + sa_pool_bytes(a) <= limit; };
     a.joint = a.K == 128 || a.stream_last;
-    if (!a.joint && tc_sa_layout(a).total + 1024 + sa_carry_bytes(a) + sa_red_bytes(1) > limit) a.joint = 1;
-    const size_t used = (size_t)tc_sa_layout(a).total + 1024 + sa_carry_bytes(a);
-    const int ncl = a.Ntot[a.nl - 1] / 64;
-    a.pool_chunks = 1;
-    if (!a.stream_last)
-        for (int ng = ncl; ng > 1; --ng)
-            if (ncl % ng == 0 && used + sa_red_bytes(ng) <= limit) { a.pool_chunks = ng; break; }
+    if (!a.joint && !fits()) a.joint = 1;
+    if (!fits()) a.stream_last = 1;
+    PSA_REQUIRE(fits(), "sa_module: internal error (pooling buffer does not fit)");
     const int C = sa_chunk(a.K, a.joint);
     const long long nchunks = (a.groups + C - 1) / C;
     const long long ctas_needed = a.joint ? nchunks : (nchunks + 1) / 2;   // two units per CTA
-    const size_t smem = used + sa_red_bytes(a.pool_chunks);
+    const size_t smem = (size_t)tc_sa_layout(a).total + 1024 + sa_pool_bytes(a);
     // shapes accepted by tc_sa_eligible: C1 in {64, 128}, one or two tensor layers, an inner layer 64 or 128 wide
     if (a.nl == 1) return a.C1 == 64 ? launch_tc_sa_shape<NP, 64, 1, 0>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 128, 1, 0>(a, ctas_needed, smem, st);
     if (a.C1 == 64) return a.Ntot[0] == 64 ? launch_tc_sa_shape<NP, 64, 2, 64>(a, ctas_needed, smem, st) : launch_tc_sa_shape<NP, 64, 2, 128>(a, ctas_needed, smem, st);

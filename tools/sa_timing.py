@@ -6,10 +6,12 @@ mlp [128, 128, 256] over 128 features (SA1's output).  The ball queries are comp
   stamps   one launch of a separate build of libpsa.so with -DPSA_SA_STAMPS (compiled into a temporary directory; the library
            the package loads has no stamps): lane 0 of the first warp of every warpgroup records clock64() at the phase
            boundaries of each 64-row pass (pass top; layer 1's gathered inputs in registers; layer 1 built; layer 2 issued,
-           retired, epilogue done; each last-layer chunk issued, retired, epilogue done; both pooling barriers passed; the next
-           pass's gather stages A and B issued).  Printed as the mean cycles from one phase to the next, in the order the phases
-           run, over every pass of every warpgroup, in SM cycles.  The stamps add global stores and registers of their own (the
-           stamped build spills a few words), so the table is a breakdown of a pass, not its exact length in libpsa.so.
+           retired, epilogue done; each last-layer chunk issued, retired, epilogue done; in a pass that ends a chunk of
+           neighbourhoods, both barriers of its store passed; the next pass's gather stages A and B issued).  Printed as the
+           mean cycles from one phase to the next, in the order the phases run, over every pass of every warpgroup that
+           reached the phase, in SM cycles; then the same apart for the passes that end a chunk and for those that do not.
+           The stamps add global stores and registers of their own (the stamped build spills a few words), so the table is
+           a breakdown of a pass, not its exact length in libpsa.so.
 
 Prints the card's name, power limit and max SM clock, read in the same run.
 
@@ -34,7 +36,7 @@ sys.path.insert(0, ROOT)
 B, N = 32, 2048
 STAMP_CTAS, STAMP_PASSES = 264, 64        # kSaStampCtas, kSaStampPasses in csrc/tc_mlp.cu
 PHASES = ["top", "inputs landed", "layer 1 built", "layer 2 issued", "layer 2 retired", "layer 2 epilogue",
-          "pool barrier 1", "pool barrier 2", "next stage A issued", "next stage B issued"]
+          "chunk end barrier 1", "chunk end barrier 2", "next stage A issued", "next stage B issued"]
 CHUNKS = 4
 NPHASE = len(PHASES) + 3 * CHUNKS         # kSaStampPhases
 
@@ -95,26 +97,36 @@ def build_stamped(tmp):
     return lib
 
 
+def table(st, top, rel, passes):
+    """the mean cycles from one phase to the next over the passes selected by `passes`, in the order the phases run"""
+    names = phase_names()
+    mean = {}
+    for k in range(1, NPHASE):
+        ok = passes & (st[:, :-1, k] > 0)
+        if ok.sum() > 0:
+            mean[names[k]] = float(rel[:, :, k][ok].mean())
+    rows, prev, prev_t = [], "top", 0.0
+    for n in sorted(mean, key=mean.get):
+        rows.append({"phase": f"{prev} -> {n}", "cycles": round(mean[n] - prev_t, 1)})
+        prev, prev_t = n, mean[n]
+    length = float((top[:, 1:] - top[:, :-1])[passes].mean())
+    rows.append({"phase": f"{prev} -> next top", "cycles": round(length - prev_t, 1)})
+    return {"passes": int(passes.sum()), "pass_cycles": round(length, 1), "phases": rows}
+
+
 def summarise(st):
-    """st: (ctas, 2, passes, phases) clock64 stamps, 0 where a pass did not reach a phase -> per-phase means"""
+    """st: (ctas, 2, passes, phases) clock64 stamps, 0 where a pass did not reach a phase -> per-phase means over every pass,
+    and apart over the passes that end a chunk of neighbourhoods and those that do not"""
     st = st.reshape(-1, STAMP_PASSES, NPHASE).astype(np.float64)
     top = st[:, :, 0]
     done = (top[:, :-1] > 0) & (top[:, 1:] > 0)            # passes followed by another: their length is known
     rel = st[:, :-1, :] - top[:, :-1, None]
-    names = phase_names()
-    mean = {}
-    for k in range(1, NPHASE):
-        ok = done & (st[:, :-1, k] > 0)
-        if ok.sum() > 0:
-            mean[names[k]] = float(rel[:, :, k][ok].mean())
-    order = sorted(mean, key=mean.get)
-    rows, prev, prev_t = [], "top", 0.0
-    for n in order:
-        rows.append({"phase": f"{prev} -> {n}", "cycles": round(mean[n] - prev_t, 1)})
-        prev, prev_t = n, mean[n]
-    length = float((top[:, 1:] - top[:, :-1])[done].mean())
-    rows.append({"phase": f"{prev} -> next top", "cycles": round(length - prev_t, 1)})
-    return {"passes": int(done.sum()), "pass_cycles": round(length, 1), "phases": rows}
+    ends = done & (st[:, :-1, PHASES.index("chunk end barrier 1")] > 0)
+    out = table(st, top, rel, done)
+    for name, m in (("chunk_end", ends), ("inside_chunk", done & ~ends)):
+        if m.any():
+            out[name] = table(st, top, rel, m)
+    return out
 
 
 def stamps_child(lib_path, name):
