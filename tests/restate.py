@@ -660,7 +660,7 @@ def sa_tc_layers(channels, c, nsample, mode):
             return None
     # tc_sa_layout at np = 3, which the fp16x2 layout never exceeds: every layer resident, or the last one streamed through two
     # slots of one 64-channel chunk
-    fixed = 8 * channels[1] * 4 + sum(2 * N * 4 for _, N in layers)
+    fixed = 7 * channels[1] * 4 + sum(2 * N * 4 for _, N in layers)          # w1x, w1c (3 C1 each), t1; scale, shift per layer
     resident = sum(K * N * 2 * 3 for K, N in layers)
     streamed = resident - layers[-1][0] * layers[-1][1] * 2 * 3 + 2 * (layers[-1][0] // 64) * 64 * 128 * 3
     return layers if min(resident, streamed) + fixed + 1024 <= 220 * 1024 else None
