@@ -358,7 +358,10 @@ typedef struct psa_grad_in {
 } psa_grad_in;
 
 /* y (rows, N) = in (rows, K) . W (K, N) + bias; stats (2, N) = per-channel [sum, sum of squares] of y (or NULL).
- * workspace: psa_train_dense_workspace_bytes(rows, K, N). */
+ * workspace: psa_train_dense_workspace_bytes(rows, K, N).  The fp32 GEMM loads psa_act_in / psa_grad_in operands element by
+ * element where they are not 16-byte aligned with strides a multiple of 4.  It takes at most 65535 row tiles of 128, about
+ * 8.4 M rows, in the forward (every shape the tensor-core forward does not take) and the input gradient (else
+ * PSA_ERR_UNSUPPORTED, before anything is launched). */
 PSA_API size_t psa_train_dense_workspace_bytes(long long rows, int K, int N);
 PSA_API int psa_train_dense_fwd(long long rows, int K, int N, const psa_act_in* in, const float* W, const float* bias,
                                 float* y, float* stats, void* workspace, size_t workspace_bytes, psa_stream_t stream);
@@ -390,7 +393,7 @@ PSA_API int psa_train_bias_grad(long long rows, int N, const psa_grad_in* g, flo
  * whose products with W_g give dg and dW_g (psa_train_dense_bwd_input / _bwd_weight over the groups).  Under batch norm the
  * whole-batch sum of dy is zero but the per-group sums are not.  Sums in a fixed order: bit-reproducible.  group_rows must
  * divide rows (else PSA_ERR_INVALID_ARGUMENT); at most 65535 groups (else PSA_ERR_UNSUPPORTED).  psa_train_bias_grad is the
- * group_rows = rows case. */
+ * group_rows = rows case.  The forward takes at most 65535 row tiles of 128 (else PSA_ERR_UNSUPPORTED). */
 PSA_API int psa_train_dense_fwd_grouped(long long rows, long long group_rows, int K, int N, const psa_act_in* in, const float* W,
                                         const float* bias, const float* group_add, float* y, float* stats, void* workspace,
                                         size_t workspace_bytes, psa_stream_t stream);
@@ -411,13 +414,20 @@ PSA_API int psa_bn_finalize_rows(long long rows, int C, const float* y, const fl
                                  float* moving_mean, float* moving_var, float* scale, float* shift, float* mean_inv,
                                  psa_stream_t stream);
 
-/* relu(BN(y)) then max over each run of pool_k rows: pooled (groups, C), argk (groups, C) = first winning row. */
+/* relu(BN(y)) then max over each run of pool_k rows: pooled (groups, C), argk (groups, C) = first winning row.  A group whose
+ * values are all <= 0 after the relu pools 0 with argk 0.  y, scale, shift, pooled and argk 16-byte aligned, C a multiple of 4
+ * (else PSA_ERR_INVALID_ARGUMENT); the same holds for psa_pool_rows' x and out. */
 PSA_API int psa_train_pool_fwd(long long groups, int pool_k, int C, const float* y, const float* scale,
                                const float* shift, float* pooled, int* argk, psa_stream_t stream);
 
 /* Batch-norm backward sums of a layer: dbeta[c] = sum_r dz, dgamma[c] = sum_r dz * xhat (g->ca/cb/cc are ignored),
  * and the coefficients ca = gamma*inv, cb = -gamma*inv^2*dgamma/rows, cc = gamma*inv*(mean*inv*dgamma - dbeta)/rows
- * that make psa_grad_in evaluate dy.  workspace: psa_bn_bwd_workspace_bytes(C). */
+ * that make psa_grad_in evaluate dy.  workspace: psa_bn_bwd_workspace_bytes(C).
+ * The batch-norm sums here and psa_sa_conv1_bwd / _bwd_xyz read g with 16-byte vector loads and take only such operands (else
+ * PSA_ERR_INVALID_ARGUMENT): every non-NULL pointer of g they read (y, s, t, ca, cb, cc; dh and mask in mode 0; dp, pv, argk in
+ * mode 1) 16-byte aligned, ld a multiple of 4 where y is read (always here, with y given), ld_dh a multiple of 4 in mode 0, and
+ * in mode 1 g->C equal to the layer width (C, C1) and pool_k dividing the rows.  mean_inv here, dU of psa_sa_conv1_bwd and the
+ * workspace of psa_sa_conv1_bwd_xyz are 16-byte aligned too. */
 PSA_API size_t psa_bn_bwd_workspace_bytes(int C);
 PSA_API int psa_bn_bwd_coeffs(long long rows, int C, const psa_grad_in* g, const float* gamma, const float* mean_inv,
                               float* dgamma, float* dbeta, float* ca, float* cb, float* cc, void* workspace,

@@ -229,7 +229,8 @@ bn_bwd_partial_kernel(const GradIn g, long long rows, int C, const float* __rest
         const long long r0 = (long long)blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
         if (g.mode == 0) {
             for (long long r = r0 + rl; r < r1; r += RL) {
-                const float4 yv = g.y4(r, c);
+                // y itself, not g.y4: that reads zeros without a relu gate (s == NULL), and xhat needs y in every case
+                const float4 yv = __ldg(reinterpret_cast<const float4*>(g.y + r * g.ld + c));
                 const float4 dz = g.dz4(r, c, yv);
                 sb.x += dz.x; sb.y += dz.y; sb.z += dz.z; sb.w += dz.w;
                 sg.x = fmaf(dz.x, (yv.x - mu.x) * inv.x, sg.x); sg.y = fmaf(dz.y, (yv.y - mu.y) * inv.y, sg.y);
@@ -524,6 +525,34 @@ int weight_grad_splits(long long rows, int tiles, long long* k_per_split) {
     return (int)((rows + kps - 1) / kps);
 }
 
+static bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+// The GEMM launchers put the 128-row tiles of the output on gridDim.y
+constexpr long long kMaxRowTiles = 65535;
+
+// A psa_grad_in read by the training reductions (bn_bwd_partial, conv1_dwxyz_partial, group_grad_csr, conv1_vxyz).  Unlike the
+// GEMM, they load it with GradIn's float4 / int4 accessors and have no scalar fallback, so every vector they read must be 16-byte
+// aligned with rows a multiple of 4 floats, and the pooled routing must cover `rows` rows of `width` channels.  `read_y`: y is read
+// whatever s / ca hold; `coeffs`: ca / cb / cc are read.
+static int check_vec_grad(const char* fn, const psa_grad_in* g, long long rows, int width, bool read_y, bool coeffs) {
+    PSA_REQUIRE(g->mode == 0 || g->mode == 1, "%s: grad_in mode %d (0 or 1)", fn, g->mode);
+    if (read_y || g->s != nullptr || (coeffs && g->ca != nullptr))
+        PSA_REQUIRE(g->y != nullptr && al16(g->y) && g->ld % 4 == 0, "%s: grad_in y must be 16-byte aligned with ld a multiple of 4 (ld=%lld)", fn,
+                    g->ld);
+    PSA_REQUIRE(al16(g->s) && al16(g->t), "%s: grad_in s / t must be 16-byte aligned", fn);
+    if (coeffs) PSA_REQUIRE(al16(g->ca) && al16(g->cb) && al16(g->cc), "%s: grad_in ca / cb / cc must be 16-byte aligned", fn);
+    if (g->mode == 0) {
+        PSA_REQUIRE(g->dh != nullptr && al16(g->dh) && al16(g->mask) && g->ld_dh % 4 == 0,
+                    "%s: grad_in dh / mask must be 16-byte aligned with ld_dh a multiple of 4 (ld_dh=%lld)", fn, g->ld_dh);
+    } else {
+        PSA_REQUIRE(g->C == width && g->pool_k >= 1 && rows % g->pool_k == 0,
+                    "%s: pooled grad_in needs C == %d and pool_k dividing %lld rows (C=%d pool_k=%d)", fn, width, rows, g->C, g->pool_k);
+        PSA_REQUIRE(g->dp != nullptr && g->pv != nullptr && g->argk != nullptr && al16(g->dp) && al16(g->pv) && al16(g->argk),
+                    "%s: grad_in dp / pv / argk must be 16-byte aligned", fn);
+    }
+    return PSA_OK;
+}
+
 }  // namespace psa
 
 using namespace psa;
@@ -569,6 +598,7 @@ extern "C" int psa_train_dense_fwd(long long rows, int K, int N, const psa_act_i
         if (stats != nullptr) return reduce_partials((int)tiles_m, 2 * N, sp, stats, st);
         return PSA_OK;
     }
+    PSA_SUPPORTED(tiles_m <= kMaxRowTiles, "train_dense_fwd: rows=%lld exceeds %lld row tiles of 128 on the fp32 path", rows, kMaxRowTiles);
     const ActIn fa(*in);
     const MatIn fb{W, N};
     int rc;
@@ -607,6 +637,7 @@ extern "C" int psa_train_dense_fwd_grouped(long long rows, long long group_rows,
     PSA_REQUIRE(in && in->x && W && group_add && y, "train_dense_fwd_grouped: null buffer");
     cudaStream_t st = as_stream(stream);
     const long long tiles_m = (rows + 127) / 128;
+    PSA_SUPPORTED(tiles_m <= kMaxRowTiles, "train_dense_fwd_grouped: rows=%lld exceeds %lld row tiles of 128", rows, kMaxRowTiles);
     GemmOut o;
     o.out = y; o.ld_out = N; o.bias = bias; o.col_skip = 0; o.stat_partial = nullptr;
     o.group_add = group_add; o.group_rows = group_rows;
@@ -630,6 +661,7 @@ extern "C" int psa_train_dense_bwd_input(long long rows, int K, int N, const psa
     PSA_REQUIRE(rows >= 0 && K >= 1 && N >= 1 && col_skip >= 0 && col_skip < K, "train_dense_bwd_input: bad dims");
     if (rows == 0) return PSA_OK;
     PSA_REQUIRE(g && W && dx, "train_dense_bwd_input: null buffer");
+    PSA_SUPPORTED((rows + 127) / 128 <= kMaxRowTiles, "train_dense_bwd_input: rows=%lld exceeds %lld row tiles of 128", rows, kMaxRowTiles);
     GemmOut o;
     o.out = dx; o.ld_out = ld_dx; o.bias = nullptr; o.col_skip = col_skip; o.stat_partial = nullptr;
     const GradIn fa(*g);
@@ -703,6 +735,7 @@ extern "C" int psa_train_pool_fwd(long long groups, int pool_k, int C, const flo
     PSA_REQUIRE(groups >= 0 && pool_k >= 1 && C >= 4 && C % 4 == 0, "train_pool_fwd: C=%d must be a multiple of 4", C);
     if (groups == 0) return PSA_OK;
     PSA_REQUIRE(y && scale && shift && pooled && argk, "train_pool_fwd: null buffer");
+    PSA_REQUIRE(al16(y) && al16(scale) && al16(shift) && al16(pooled) && al16(argk), "train_pool_fwd: y, scale, shift, pooled, argk must be 16-byte aligned");
     const long long total = groups * (C / 4);
     train_pool_fwd_kernel<<<(unsigned)((total + 127) / 128), 128, 0, as_stream(stream)>>>(
         groups, pool_k, C / 4, reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(scale), reinterpret_cast<const float4*>(shift),
@@ -715,6 +748,7 @@ extern "C" int psa_pool_rows(long long groups, int pool_k, int C, int mode, cons
     PSA_REQUIRE(mode >= 0 && mode <= 2 && (mode != 2 || dist != nullptr), "pool_rows: mode %d", mode);
     if (groups == 0) return PSA_OK;
     PSA_REQUIRE(x && out, "pool_rows: null buffer");
+    PSA_REQUIRE(al16(x) && al16(out), "pool_rows: x and out must be 16-byte aligned");
     const long long total = groups * (C / 4);
     pool_rows_kernel<<<(unsigned)((total + 127) / 128), 128, 0, as_stream(stream)>>>(groups, pool_k, C / 4, mode, reinterpret_cast<const float4*>(x), dist,
                                                                                        reinterpret_cast<float4*>(out));
@@ -731,13 +765,14 @@ extern "C" int psa_bn_bwd_coeffs(long long rows, int C, const psa_grad_in* g, co
     PSA_SUPPORTED(C % 4 == 0 && C <= 1024, "bn_bwd_coeffs: C=%d must be a multiple of 4, at most 1024", C);
     PSA_REQUIRE(g && gamma && mean_inv && dgamma && dbeta && ca && cb && cc, "bn_bwd_coeffs: null buffer");
     PSA_REQUIRE(workspace && workspace_bytes >= psa_bn_bwd_workspace_bytes(C), "bn_bwd_coeffs: workspace too small");
+    int rc = check_vec_grad("bn_bwd_coeffs", g, rows, C, true, false);
+    if (rc != PSA_OK) return rc;
+    PSA_REQUIRE(al16(mean_inv), "bn_bwd_coeffs: mean_inv must be 16-byte aligned");
     cudaStream_t st = as_stream(stream);
     GradIn gi(*g);
     gi.ca = gi.cb = gi.cc = nullptr;
-    PSA_REQUIRE(gi.y != nullptr && gi.ld % 4 == 0, "bn_bwd_coeffs: y must be given with a row stride that is a multiple of 4");
     // units the blocks iterate over: rows (dense dz) or pooled groups (max-pool routing)
     const long long units = gi.mode == 0 ? rows : rows / gi.pool_k;
-    if (gi.mode == 1) PSA_REQUIRE(gi.pool_k >= 1 && rows % gi.pool_k == 0 && gi.C == C, "bn_bwd_coeffs: pooled routing needs rows %% pool_k == 0");
     const int RL = kBnbThreads / (C / 4);
     long long blocks = (units + (long long)RL * 8 - 1) / ((long long)RL * 8);
     if (blocks > kBnbMaxBlocks) blocks = kBnbMaxBlocks;
@@ -746,7 +781,7 @@ extern "C" int psa_bn_bwd_coeffs(long long rows, int C, const psa_grad_in* g, co
     blocks = (units + upb - 1) / upb;
     float* partial = reinterpret_cast<float*>(workspace);
     bn_bwd_partial_kernel<<<(unsigned)blocks, kBnbThreads, 0, st>>>(gi, units, C, mean_inv, upb, partial);
-    int rc = check_launch("bn_bwd_partial_kernel");
+    rc = check_launch("bn_bwd_partial_kernel");
     if (rc != PSA_OK) return rc;
     return launch_bn_bwd_final((int)blocks, C, rows, partial, gamma, mean_inv, dgamma, dbeta, ca, cb, cc, st);
 }
@@ -764,9 +799,12 @@ extern "C" int psa_sa_conv1_bwd(int b, int n, int m, int nsample, int C1, const 
     PSA_SUPPORTED(C1 % 4 == 0 && C1 <= 1024, "sa_conv1_bwd: C1=%d", C1);
     PSA_REQUIRE(xyz && new_xyz && idx && g && dW_xyz, "sa_conv1_bwd: null buffer");
     PSA_REQUIRE(workspace && workspace_bytes >= psa_sa_conv1_bwd_workspace_bytes(b, n, m, nsample, C1, dU != nullptr), "sa_conv1_bwd: workspace too small");
+    const long long rows = (long long)b * m * nsample;
+    int rc = check_vec_grad("sa_conv1_bwd", g, rows, C1, false, true);
+    if (rc != PSA_OK) return rc;
+    PSA_REQUIRE(al16(dU), "sa_conv1_bwd: dU must be 16-byte aligned");
     cudaStream_t st = as_stream(stream);
     const GradIn gi(*g);
-    const long long rows = (long long)b * m * nsample;
     const int RL = kBnbThreads / (C1 / 4);
     long long blocks = (rows + (long long)RL * 8 - 1) / ((long long)RL * 8);
     if (blocks > kBnbMaxBlocks) blocks = kBnbMaxBlocks;
@@ -775,7 +813,7 @@ extern "C" int psa_sa_conv1_bwd(int b, int n, int m, int nsample, int C1, const 
     float* partial = reinterpret_cast<float*>(workspace);
     conv1_dwxyz_partial_kernel<<<(unsigned)blocks, kBnbThreads, 0, st>>>(gi, rows, nsample, (long long)m * nsample, n, m, C1, xyz, new_xyz, idx,
                                                                          rpb, partial);
-    int rc = check_launch("conv1_dwxyz_partial_kernel");
+    rc = check_launch("conv1_dwxyz_partial_kernel");
     if (rc != PSA_OK) return rc;
     rc = reduce_partials((int)blocks, 3 * C1, partial, dW_xyz, st);
     if (rc != PSA_OK) return rc;
@@ -810,9 +848,12 @@ extern "C" int psa_sa_conv1_bwd_xyz(int b, int n, int m, int nsample, int C1, co
     PSA_REQUIRE((reinterpret_cast<uintptr_t>(W_xyz) & 15) == 0, "sa_conv1_bwd_xyz: W_xyz must be 16-byte aligned");
     const size_t need = psa_sa_conv1_bwd_xyz_workspace_bytes(b, n, m, nsample);
     PSA_REQUIRE(workspace && workspace_bytes >= need, "sa_conv1_bwd_xyz: workspace of %zu bytes required, got %zu", need, workspace_bytes);
+    PSA_REQUIRE(al16(workspace), "sa_conv1_bwd_xyz: workspace must be 16-byte aligned");
+    const long long queries = (long long)b * m, rows = queries * nsample;
+    int rc = check_vec_grad("sa_conv1_bwd_xyz", g, rows, C1, false, true);
+    if (rc != PSA_OK) return rc;
     cudaStream_t st = as_stream(stream);
     const GradIn gi(*g);
-    const long long queries = (long long)b * m, rows = queries * nsample;
     uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
     float4* v = reinterpret_cast<float4*>(ws);
     int* offsets = reinterpret_cast<int*>(ws + align256((size_t)rows * sizeof(float4)));
@@ -821,7 +862,7 @@ extern "C" int psa_sa_conv1_bwd_xyz(int b, int n, int m, int nsample, int C1, co
     if (C1 <= 32) conv1_vxyz_kernel<8><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
     else if (C1 <= 64) conv1_vxyz_kernel<16><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
     else conv1_vxyz_kernel<32><<<qblocks, 256, 0, st>>>(gi, queries, nsample, C1, W_xyz, v, dnew_xyz);
-    int rc = check_launch("conv1_vxyz_kernel");
+    rc = check_launch("conv1_vxyz_kernel");
     if (rc != PSA_OK) return rc;
     rc = launch_group_csr(b, n, m * nsample, idx, offsets, list, st);
     if (rc != PSA_OK) return rc;

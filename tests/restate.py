@@ -699,6 +699,121 @@ def edgeconv_workspace(b, n, c, k, channels, mode):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# routing of the training GEMM's launchers (csrc/train.cu): which kernel path, tile and contraction split each product takes,
+# and psa_train_dense_workspace_bytes.  tests/test_train_gemm_plan_cpu.py checks the workspace against the library, and that
+# the cases of tests/test_train_gemm_gpu.py reach every path.
+# ---------------------------------------------------------------------------------------------------------------------
+TRAIN_SMALL_M = 1024              # kSmallM: rows up to this split the contraction of the forward / input gradient
+TRAIN_BK = 16                     # kGemmBK
+
+
+def tc_train_fwd_eligible(rows, K, N):
+    return rows >= 128 and 128 <= K <= 512 and N >= 128 and N % 128 == 0
+
+
+def small_m_splits(contraction):
+    return max(1, min(16, contraction // 64))
+
+
+def weight_grad_splits(rows, tiles):
+    """(splits, k_per_split) of the weight gradient's contraction over the rows"""
+    want = max(1, min((2 * PLAN_SMS + tiles - 1) // tiles, (rows + 255) // 256))
+    kps = -(-(-(-rows // want)) // TRAIN_BK) * TRAIN_BK
+    return -(-rows // kps), kps
+
+
+def _split_k(contraction):
+    """(nz, k_per_split) of a small-M product: small_m_splits rounded to whole BK blocks"""
+    s = small_m_splits(contraction)
+    kps = -(-(-(-contraction // s)) // TRAIN_BK) * TRAIN_BK
+    return -(-contraction // kps), kps
+
+
+def train_fwd_plan(rows, K, N, ld=None, mask=False):
+    """psa_train_dense_fwd: path "tc" (the tensor-core forward), "split" (small M, contraction split over CTAs, statistics from
+    col_stats_kernel) or "fp32" (one pass, statistics from the epilogue); the tile width bn of the fp32 paths"""
+    if tc_train_fwd_eligible(rows, K, N) and (ld is None or ld == K) and not mask:
+        return dict(path="tc")
+    bn = 64 if N <= 64 else 128
+    if rows <= TRAIN_SMALL_M and small_m_splits(K) > 1:
+        nz, kps = _split_k(K)
+        return dict(path="split", bn=bn, splits=nz, kps=kps)
+    return dict(path="fp32", bn=bn, splits=1)
+
+
+def train_bwd_input_plan(rows, K, N, workspace_bytes):
+    """psa_train_dense_bwd_input: "split" when small M and the workspace holds the partials, else "fp32" (one split)"""
+    bn = 64 if K <= 64 else 128
+    if rows <= TRAIN_SMALL_M and small_m_splits(N) > 1 and workspace_bytes >= small_m_splits(N) * rows * K * 4:
+        nz, kps = _split_k(N)
+        return dict(path="split", bn=bn, splits=nz, kps=kps)
+    return dict(path="fp32", bn=bn, splits=1)
+
+
+def train_bwd_weight_plan(rows, K, N):
+    """psa_train_dense_bwd_weight: the (bm, bn) tiling over (K, N) and the split of the rows"""
+    bm, bn = (64 if K <= 64 else 128), (64 if N <= 64 else 128)
+    splits, kps = weight_grad_splits(rows, -(-K // bm) * -(-N // bn))
+    return dict(bm=bm, bn=bn, splits=splits, kps=kps)
+
+
+def train_dense_workspace(rows, K, N):
+    """psa_train_dense_workspace_bytes"""
+    fwd = -(-rows // 128) * 2 * N * 4
+    w = train_bwd_weight_plan(rows, K, N)
+    need = max(fwd, w["splits"] * K * N * 4 if w["splits"] > 1 else 0, 16 * rows * max(K, N) * 4 if rows <= TRAIN_SMALL_M else 0)
+    if tc_train_fwd_eligible(rows, K, N):
+        need = max(need, _al256(fwd) + dense_image_bytes(K, N))
+    return need + 256
+
+
+# The dense cases of tests/test_train_gemm_gpu.py.  act: "raw" (x as is), "bn" (relu(x * scale + shift)), "bn_mask" (and a dropout
+# mask); x layout: "dense" (ld = K), "slice" (a column slice, ld = K + 8), "ld_odd" (ld = K + 3), "offset" (x, mask, scale and
+# shift 4 bytes past a 16-byte boundary).  src: the psa_grad_in flags joined by "+": mask, gate (the relu gate from s / t),
+# coeffs (ca / cb / cc), pool20 / pool32 (mode 1, the max-pool routing), scalar (dh with an odd ld_dh, y with ld = N + 3).
+#            id            rows   K    N    act        x         bias   stats
+FWD_CASES = [("fp32_n48", 300, 40, 48, "bn", "dense", True, True),
+             ("fp32_n100", 1500, 72, 100, "raw", "dense", False, True),
+             ("split_stats", 200, 300, 130, "bn", "dense", True, True),
+             ("split_nostats", 33, 256, 40, "raw", "dense", True, False),
+             ("tc_gate_in", 128, 128, 128, "bn", "dense", True, True),
+             ("rows127", 127, 128, 128, "bn", "dense", True, True),
+             ("k127", 128, 127, 128, "bn", "dense", False, True),
+             ("tc_k512", 256, 512, 256, "bn", "dense", True, True),
+             ("k513", 256, 513, 256, "bn", "dense", True, True),
+             ("n192", 256, 200, 192, "bn", "dense", True, True),
+             ("tc_kpad", 384, 200, 128, "bn", "dense", True, True),
+             ("tc_plain", 1000, 256, 384, "raw", "dense", False, False),
+             ("tc_shape_mask", 256, 128, 128, "bn_mask", "dense", True, True),
+             ("slice", 1100, 128, 128, "bn", "slice", True, True),
+             ("ld_odd", 1100, 64, 72, "bn_mask", "ld_odd", False, True),
+             ("offset", 1100, 64, 48, "bn_mask", "offset", True, True)]
+#                  id                rows  K    N    src                     col_skip ld_dx
+BWD_INPUT_CASES = [("k48", 1100, 48, 72, "plain", 0, None),
+                   ("k100", 1100, 100, 40, "mask+gate+coeffs", 0, None),
+                   ("mask", 1100, 64, 64, "mask", 0, None),
+                   ("gate", 1100, 64, 64, "gate", 0, None),
+                   ("coeffs", 1100, 96, 64, "coeffs", 0, None),
+                   ("split", 200, 72, 300, "gate", 0, None),
+                   ("split_k40", 64, 40, 1024, "mask+coeffs", 0, None),
+                   ("skip_odd", 1100, 70, 64, "mask", 3, 69),
+                   ("skip_odd_split", 200, 70, 256, "plain", 3, 69),
+                   ("pool20", 800, 96, 64, "pool20", 0, None),
+                   ("pool32", 1536, 64, 128, "pool32+coeffs", 0, None),
+                   ("pool20_split", 600, 48, 256, "pool20+coeffs", 0, None),
+                   ("scalar", 1100, 64, 66, "scalar+mask+gate+coeffs", 0, None)]
+#                   id                rows   K    N    act        x         src
+BWD_WEIGHT_CASES = [("t64x64", 200, 40, 48, "bn", "dense", "plain"),
+                    ("t64x128", 3000, 40, 100, "bn_mask", "dense", "mask+gate+coeffs"),
+                    ("t128x64_pool", 1000, 100, 60, "bn", "dense", "pool20+coeffs"),
+                    ("t128x128", 250, 130, 200, "bn_mask", "dense", "coeffs"),
+                    ("t64x128_pool32", 2048, 64, 128, "raw", "dense", "pool32"),
+                    ("scalar", 1500, 66, 70, "bn_mask", "ld_odd", "scalar+mask+gate"),
+                    ("offset", 700, 64, 64, "bn", "offset", "gate"),
+                    ("large", 40009, 72, 136, "bn", "dense", "gate")]
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # metrics
 # ---------------------------------------------------------------------------------------------------------------------
 def rel(got, want):

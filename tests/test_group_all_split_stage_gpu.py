@@ -41,11 +41,22 @@ def _run(p, xyz, pts, mlp):
     return pointnet_sa_module(xyz, pts, None, None, None, mlp, None, True, False, None, "sa", params=p)[1].clone()
 
 
+def _device_kernels(fn):
+    """The names of the device records (kernels, memsets) the profiler took while fn ran.  Now and then a window delivers no
+    device record at all although all its host calls are there, cudaLaunchKernel included: such a window does not show which
+    kernels ran, so fn is profiled again."""
+    for _ in range(3):
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            fn()
+            torch.cuda.synchronize()
+        names = {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+        if names:
+            return names
+    raise AssertionError("three profiler windows without a device record")
+
+
 def _ran_cluster_kernel(fn):
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return any("tc_group_all_kernel" in e.key for e in prof.key_averages())
+    return any("tc_group_all_kernel" in k for k in _device_kernels(fn))
 
 
 def _check(b, mlp, seed):
