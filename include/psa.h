@@ -738,6 +738,64 @@ PSA_API int psa_dense_elu_affine(long long rows, int K, int N, const float* x, l
                                  const float* scale, const float* shift, float* out, long long ldo, void* workspace,
                                  size_t workspace_bytes, psa_stream_t stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * PointCNN, training mode (PointCNN/pointcnn.py:10-52, pointfly.py:298-347 with is_training=True; train.py:138-164).  Every
+ * batch norm takes the statistics of its batch: a layer BN(elu(z)) keeps only a = elu(z) (z itself for X_2, which has no ELU),
+ * and the next layer applies the batch's (s, t) to a.  fp32 FMA in every arithmetic mode, no float atomics: weight gradients
+ * are summed per block over a fixed set of tiles and the block partials added in block order, so a step is bit-reproducible.
+ * Notation of psa_xconv_core; R = b*P queries.
+ * ------------------------------------------------------------------------------------------- */
+
+/* The activations a training forward saves per X-Conv layer, every one contiguous:
+ *   local (R*K, 3) = pts[idx] - q;  a_p0, a_p1 (R*K, c_pts) the two lifting layers;  a_x0, a_x1, a_x2 (R, K*K) X_0, X_1, X_2. */
+typedef struct psa_xconv_saved {
+    float* local;
+    float* a_p0;
+    float* a_p1;
+    float* a_x0;
+    float* a_x1;
+    float* a_x2;
+} psa_xconv_saved;
+
+/* One forward stage of an X-Conv layer, each pre-batch-norm value evaluated with psa_xconv_core's own fmaf chain, so that
+ * psa_xconv_core run with the batch (s, t) of the five layers in `layer` computes its output from exactly these activations:
+ *   stage 0: local, a_p0 = elu(local . w_pts0), a_x0 = elu(local (R, 3K) . w_x0)
+ *   stage 1: a_p1 = elu(BN(a_p0) . w_pts1), a_x1 = elu(depthwise(BN(a_x0), w_x1))   BN(a) = a * s + t with layer's s_pts0 / s_x0 ...
+ *   stage 2: a_x2 = depthwise(BN(a_x1), w_x2)
+ * pts (b,n,3), qrs (b,P,3), idx (b,P,K) as psa_xconv_core takes them; the (s, t) a stage does not read may be NULL. */
+PSA_API int psa_xconv_train_stage(int stage, int b, int n, int P, const float* pts, const float* qrs, const int* idx,
+                                  const psa_xconv* layer, const psa_xconv_saved* saved, psa_stream_t stream);
+
+/* Scratch of psa_xconv_train_bwd_top and psa_xconv_depthwise_bwd for one layer (block partials); 0 for dims they do not take. */
+PSA_API size_t psa_xconv_train_bwd_workspace_bytes(int b, int P, int K, int c_pts, int c_prev, int dm);
+
+/* Backward of the core's top from d_dw (R, c_in*dm), the gradient of psa_xconv_core's output: with X2n = BN(a_x2) (K, K),
+ * F = [BN(a_p1) | fts[idx]] (K, c_in) and fts_X = X2n . F recomputed per query,
+ *   dW_dw (K, c_in, dm) = sum_queries fts_X[i][c] d_dw[c*dm + m];  d fts_X[i][c] = sum_m d_dw[c*dm + m] w_dw[i][c][m];
+ *   dX2n (R, K*K) = d fts_X . F^T;  dF = X2n^T . d fts_X, written as dF_lift (R*K, c_pts) and dF_prev (R*K, c_prev).
+ * fts and dF_prev are given exactly when c_prev > 0; psa_group_point_grad(b, n, c_prev, P, K, dF_prev, idx, ...) turns dF_prev
+ * into the gradient of fts.  Reads layer's s_pts1, t_pts1, s_x2, t_x2, w_dw and saved's a_p1, a_x2. */
+PSA_API int psa_xconv_train_bwd_top(int b, int n, int P, const int* idx, const float* fts, const psa_xconv* layer,
+                                    const psa_xconv_saved* saved, const float* d_dw, float* dX2n, float* dF_lift, float* dF_prev,
+                                    float* dW_dw, void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* Backward of a depthwise X layer z[b*K + m] = sum_a x[a*K + b] W[a][b][m] over R rows, x = a_in * s + t (a_in (R, K*K)):
+ *   dz = g evaluated per element (mode 0: the batch-norm backward of the layer's output, g->y its saved activations), times
+ *        TF's EluGrad (g->y < 0 ? g->y + 1 : 1) when elu != 0;
+ *   dW (K, K, K) = sum_r x[a*K + b] dz[b*K + m];  dx (R, K*K) = sum_m dz[b*K + m] W[a][b][m], the gradient of x.
+ * workspace: psa_xconv_train_bwd_workspace_bytes of the layer. */
+PSA_API int psa_xconv_depthwise_bwd(long long rows, int K, const float* x, const float* s, const float* t, const psa_grad_in* g, int elu,
+                                    const float* W, float* dW, float* dx, void* workspace, size_t workspace_bytes, psa_stream_t stream);
+
+/* dz (rows, C) = g (mode 0) evaluated at every element times TF's EluGrad on g->y: the gradient of z for a layer BN(elu(z)),
+ * materialised for the dense products (psa_train_dense_bwd_weight / _bwd_input with a plain psa_grad_in over dz). */
+PSA_API int psa_elu_bn_dy(long long rows, int C, const psa_grad_in* g, float* dz, psa_stream_t stream);
+
+/* out[r * ldo + c] = a[r][c] * s[c] + t[c] (one fmaf): a (rows, C) contiguous, the batch norm of a layer written into its slice of
+ * a wider row. */
+PSA_API int psa_bn_affine_rows(long long rows, int C, const float* a, const float* s, const float* t, float* out, long long ldo,
+                               psa_stream_t stream);
+
 /* Mean sparse softmax cross-entropy (pointnet2_cls_ssg.py:50-57) and its gradient: logits (b, c), labels (b) int32 ->
  * loss (1), dlogits (b, c) = (softmax - onehot) / b. */
 PSA_API int psa_softmax_xent(int b, int c, const float* logits, const int* labels, float* loss, float* dlogits,

@@ -40,6 +40,11 @@ class PsaXconv(C.Structure):
                                   "t_x1", "w_x2", "s_x2", "t_x2", "w_dw")]
 
 
+class PsaXconvSaved(C.Structure):
+    """psa_xconv_saved (include/psa.h): the activations a training forward keeps per X-Conv layer."""
+    _fields_ = [(f, C.c_void_p) for f in ("local", "a_p0", "a_p1", "a_x0", "a_x1", "a_x2")]
+
+
 class PsaActIn(C.Structure):
     """psa_act_in (include/psa.h): forward input of a training-mode layer."""
     _fields_ = [("x", C.c_void_p), ("ld", C.c_longlong), ("scale", C.c_void_p), ("shift", C.c_void_p), ("mask", C.c_void_p),
@@ -138,6 +143,12 @@ SIGNATURES = {
     "psa_dense_elu_affine": [_ll, _i, _i, _p, _ll, _p, _p, _p, _p, _p, _ll, _p, _sz, _p],
     "psa_softmax_xent": [_i, _i, _p, _p, _p, _p, _p],
     "psa_pool_rows": [_ll, _i, _i, _i, _p, _p, _p, _p],
+    # PointCNN (training)
+    "psa_xconv_train_stage": [_i, _i, _i, _i, _p, _p, _p, C.POINTER(PsaXconv), C.POINTER(PsaXconvSaved), _p],
+    "psa_xconv_train_bwd_top": [_i, _i, _i, _p, _p, C.POINTER(PsaXconv), C.POINTER(PsaXconvSaved)] + [_p] * 6 + [_sz, _p],
+    "psa_xconv_depthwise_bwd": [_ll, _i, _p, _p, _p, _gin, _i, _p, _p, _p, _p, _sz, _p],
+    "psa_elu_bn_dy": [_ll, _i, _gin, _p, _p],
+    "psa_bn_affine_rows": [_ll, _i, _p, _p, _p, _p, _ll, _p],
     "psa_adam_step": [_ll, _p, _p, _p, _p, _f, _f, _f, _f, _i, _f, _p],
 }
 INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_workspace_bytes",
@@ -146,7 +157,7 @@ INFO_SYMBOLS = ("psa_version", "psa_last_error", "psa_sm_arch", "psa_shared_mlp_
                 "psa_scatter_workspace_bytes", "psa_edgeconv_train_workspace_bytes",
                 "psa_edgeconv2_train_workspace_bytes", "psa_sa_conv1_bwd_xyz_workspace_bytes", "psa_spider_conv_workspace_bytes",
                 "psa_spider_conv_bwd_workspace_bytes", "psa_conv3d_workspace_bytes", "psa_dense_elu_affine_workspace_bytes",
-                "psa_conv3d_bwd_workspace_bytes")
+                "psa_conv3d_bwd_workspace_bytes", "psa_xconv_train_bwd_workspace_bytes")
 
 _lib = None
 
@@ -201,6 +212,8 @@ def load() -> C.CDLL:
     lib.psa_conv3d_bwd_workspace_bytes.argtypes = [_i, _i, _i, _i, _i]
     lib.psa_conv3d_bwd_workspace_bytes.restype = C.c_size_t
     lib.psa_dense_elu_affine_workspace_bytes.restype = C.c_size_t
+    lib.psa_xconv_train_bwd_workspace_bytes.argtypes = [_i] * 6
+    lib.psa_xconv_train_bwd_workspace_bytes.restype = C.c_size_t
     lib.psa_version.restype = C.c_int
     lib.psa_sm_arch.restype = C.c_int
     lib.psa_last_error.restype = C.c_char_p

@@ -24,6 +24,7 @@ __all__ = [
     "edgeconv_infer", "sa_conv1_prebn", "pool_rows", "sa_group_all_infer", "set_mlp_mode", "get_mlp_mode",
     "spider_conv", "group_norm_affine", "topk_pool", "fisher_vector", "conv3d", "pool3d", "knn_dilated", "xconv_core",
     "dense_elu_affine", "conv3d_bwd_weight", "conv3d_bwd_data", "conv3d_bwd_macs", "pool3d_max_train", "pool3d_bwd",
+    "elu_bn_dy", "bn_affine_rows", "xconv_depthwise_bwd",
 ]
 
 
@@ -1090,3 +1091,71 @@ def get_mlp_mode() -> int:
     return int(_lib.load().psa_get_mlp_mode())
 
 
+
+
+def elu_bn_dy(a, dh, ca, cb, cc, mask=None) -> torch.Tensor:
+    """The gradient of z for a PointCNN layer BN(elu(z)) in training mode (psa_elu_bn_dy): a (R, C) = elu(z), the batch norm's input;
+    dh (R, C) the gradient of its output (times mask, a dropout mask, when given); ca, cb, cc (C) the coefficients of
+    psa_bn_bwd_coeffs -> (ca dh + cb a + cc) * (a < 0 ? a + 1 : 1), TF's EluGrad on the output."""
+    a = _dev(a, torch.float32, "a", 2)
+    dh = _dev(dh, torch.float32, "dh", 2)
+    rows, c = a.shape
+    if tuple(dh.shape) != (rows, c) or (mask is not None and tuple(mask.shape) != (rows, c)):
+        raise ValueError(f"elu_bn_dy: dh {tuple(dh.shape)} and mask must match a {tuple(a.shape)}")
+    ca, cb, cc = (_dev(t, torch.float32, n, 1) for t, n in ((ca, "ca"), (cb, "cb"), (cc, "cc")))
+    if any(t.shape[0] != c for t in (ca, cb, cc)):
+        raise ValueError(f"elu_bn_dy: ca, cb, cc must have {c} entries")
+    mask = None if mask is None else _dev(mask, torch.float32, "mask", 2)
+    g = _lib.PsaGradIn(y=_ptr(a), ld=c, ca=_ptr(ca), cb=_ptr(cb), cc=_ptr(cc), dh=_ptr(dh), ld_dh=c, mask=_ptr(mask), pool_k=1, C=c)
+    dz = torch.empty_like(a)
+    check(_lib.load().psa_elu_bn_dy(rows, c, C.byref(g), _ptr(dz), _stream()), "elu_bn_dy")
+    return dz
+
+
+def bn_affine_rows(a, scale, shift, out=None, offset: int = 0) -> torch.Tensor:
+    """a * scale + shift per channel (psa_bn_affine_rows): a (R, C) -> (R, C), or written at channels [offset, offset + C) of out
+    (R, C_total) and out returned."""
+    a = _dev(a, torch.float32, "a", 2)
+    rows, c = a.shape
+    scale = _dev(scale, torch.float32, "scale", 1)
+    shift = _dev(shift, torch.float32, "shift", 1)
+    if scale.shape[0] != c or shift.shape[0] != c:
+        raise ValueError(f"bn_affine_rows: scale and shift must have {c} entries")
+    if out is None:
+        out = torch.empty_like(a)
+    elif not (out.is_cuda and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == rows
+              and 0 <= offset and offset + c <= out.shape[1]):
+        raise ValueError(f"bn_affine_rows: out must be a float32 CUDA tensor ({rows}, >= {offset + c}) with unit column stride")
+    check(_lib.load().psa_bn_affine_rows(rows, c, _ptr(a), _ptr(scale), _ptr(shift), C.c_void_p(out.data_ptr() + 4 * offset), out.stride(0),
+                                         _stream()), "bn_affine_rows")
+    return out
+
+
+def xconv_depthwise_bwd(x, scale, shift, a, dh, ca, cb, cc, weights, elu: bool):
+    """Backward of PointCNN's depthwise X layer z = depthwise(x * scale + shift, W) followed by BN(elu(z)) (elu=True, X_1) or BN(z)
+    (X_2) in training mode (psa_xconv_depthwise_bwd): x, a (R, K*K) the saved activations of the input layer and of this one, dh
+    (R, K*K) the gradient of this layer's batch-norm output, ca, cb, cc its psa_bn_bwd_coeffs, weights (..., K, K, K) -> (dW (K, K, K),
+    dx (R, K*K) the gradient of x * scale + shift)."""
+    x = _dev(x, torch.float32, "x", 2)
+    a = _dev(a, torch.float32, "a", 2)
+    dh = _dev(dh, torch.float32, "dh", 2)
+    rows, kk = x.shape
+    k = int(round(kk ** 0.5))
+    if k * k != kk or not 1 <= k <= XCONV_MAX_K or tuple(a.shape) != (rows, kk) or tuple(dh.shape) != (rows, kk):
+        raise ValueError(f"xconv_depthwise_bwd: x {tuple(x.shape)}, a {tuple(a.shape)}, dh {tuple(dh.shape)} must be (R, K*K), K <= {XCONV_MAX_K}")
+    weights = _dev(weights, torch.float32, "weights")
+    if tuple(weights.shape[-3:]) != (k, k, k):
+        raise ValueError(f"xconv_depthwise_bwd: weights {tuple(weights.shape)} are not (..., {k}, {k}, {k})")
+    vec = [_dev(t, torch.float32, n, 1) for t, n in ((scale, "scale"), (shift, "shift"), (ca, "ca"), (cb, "cb"), (cc, "cc"))]
+    if any(t.shape[0] != kk for t in vec):
+        raise ValueError(f"xconv_depthwise_bwd: scale, shift, ca, cb, cc must have {kk} entries")
+    scale, shift, ca, cb, cc = vec
+    lib = _lib.load()
+    g = _lib.PsaGradIn(y=_ptr(a), ld=kk, ca=_ptr(ca), cb=_ptr(cb), cc=_ptr(cc), dh=_ptr(dh), ld_dh=kk, pool_k=1, C=kk)
+    need = int(lib.psa_xconv_train_bwd_workspace_bytes(rows, 1, k, 1, 0, 1))
+    ws = torch.empty(max(need, 4) // 4, dtype=torch.float32, device=x.device)
+    dW = torch.empty((k, k, k), dtype=torch.float32, device=x.device)
+    dx = torch.empty_like(x)
+    check(lib.psa_xconv_depthwise_bwd(rows, k, _ptr(x), _ptr(scale), _ptr(shift), C.byref(g), int(bool(elu)), _ptr(weights), _ptr(dW), _ptr(dx),
+                                      _ptr(ws), C.c_size_t(need), _stream()), "xconv_depthwise_bwd")
+    return dW, dx
